@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- images/sec of the ViT-B/16 224^2 forward path (BASELINE.json metric) on N B200s of one node.
+"""bench.py -- images/sec of the ViT-B/16 224^2 forward path (BASELINE.json metric) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -7,16 +7,16 @@
     python bench.py --impl reference ...      # the reference's own ggml CPU path (oracle/_ref) on the host cores
 
 A "step" is one forward pass (pixels f32 HWC -> probabilities + top-5) over one batch of 256 synthetic images per
-GPU (BASELINE.json configs[1]: vit_base_patch16_224 f16, batch=256, 1xB200).  Images shard across ranks, weights are
+GPU (BASELINE.json configs[1]: vit_base_patch16_224 f16, batch=256, 1xH100).  Images shard across ranks, weights are
 replicated, there is no collective on the data path (SURVEY.md 8e) => "scaling": "weak".
 
 `value`     : whole-job images/s with inputs already resident in HBM (CUDA events on the launching stream, max over ranks),
               exactly K timed steps after W >= 3 warm-up steps.
 `e2e`       : same metric through the reference-facing C-ABI call with HOST (pinned) buffers: H2D of the 154 MB batch and
               D2H of probabilities + top-5 inside the timed region.
-`sustained` : the same step repeated back to back for >= 2 s (the K-step burst runs at boost clocks; under the 1 kW power cap the
+`sustained` : the same step repeated back to back for >= 2 s (the K-step burst runs at boost clocks; under the card's power cap the
               SM clock settles lower), with the clocks sampled over that window.
-`roofline`  : tensor-core roofline of the dominant kernel (an fc1 / fc2 / qkv tcgen05 GEMM), timed live with a CUDA-event pair
+`roofline`  : tensor-core roofline of the dominant kernel (an fc1 / fc2 / qkv wgmma GEMM), timed live with a CUDA-event pair
               around each of its launches in a profiled pass that runs right after the sustained window (hot GPU); the fraction is
               given against BOTH measured cuBLAS peaks of MEASURED_PEAKS.json (sustained = `frac`, burst = `frac_burst`).
 `parity`    : the engine's logits for the 64 seeded fixture images of tests/golden/base_f16_b64.npz (generated from the unmodified
@@ -25,7 +25,11 @@ replicated, there is no collective on the data path (SURVEY.md 8e) => "scaling":
 `configs`   : the other single-GPU configurations of BASELINE.json (ViT-L/16-384 bf16 weights batch 128; ViT-B/16 q8_0 file batch
               256), each with its own images/s, dominant-kernel roofline and parity sample; they run after the headline so `value`
               is not affected.  (N = 1 only.)
-`cpu_baseline`: the reference (oracle/_ref, unmodified ggml CPU path) timed on this box's host cores, bounded sample.
+`cpu_baseline`: the reference (oracle/_ref, unmodified ggml CPU path) timed on this box's host cores, bounded sample (when built).
+
+--dump-outputs DIR writes what the timed path computed in its last timed step -- probabilities [B][classes], top-5 indices and
+top-5 probabilities, as float32 / float64 .npy files -- so two builds can be compared output for output on identical seeded inputs.
+Synthetic model files are cached in $VITB200_CACHE (default: a directory under the system temp dir); nothing is written to the tree.
 """
 import argparse
 import ctypes as C
@@ -41,6 +45,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.abspath(__file__))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+# the tree may be read-only: generated model files go to a per-user temporary cache
+os.environ.setdefault("VITB200_CACHE", os.path.join(__import__("tempfile").gettempdir(), "vitb200-cache-%d" % os.getuid()))
 
 BATCH = 256
 MODEL_CFG = "base"
@@ -49,22 +55,15 @@ FLOPS_PER_IMAGE = {"base": 35.128e9, "large384": 382.133e9, "tiny": 2.507e9}
 KERNEL_NAMES = ["patch", "qkv", "proj", "fc1", "fc2", "head", "attention", "layernorm"]
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of each GEMM of the step, from the committed
-    `ncu --set full` capture (profiles/traffic.json, written by tools/summarize_ncu.py); None when no capture exists."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    return json.load(open(p)) if os.path.exists(p) else {}
-
-
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        burst = float(d.get("bf16_tflops", 1590.0))
-        return {"tflops_sustained": float(d.get("bf16_tflops_sustained", burst)), "tflops_burst": burst, "hbm_gbs": float(d.get("hbm_gbs", 6650.0)),
+        burst = float(d.get("bf16_tflops", 989.0))
+        return {"tflops_sustained": float(d.get("bf16_tflops_sustained", burst)), "tflops_burst": burst, "hbm_gbs": float(d.get("hbm_gbs", 3350.0)),
                 "sustained_clock_mhz": (d.get("clocks_under_load") or {}).get("sm_mhz_median"), "which": "measured (MEASURED_PEAKS.json)"}
-    return {"tflops_sustained": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "sustained_clock_mhz": 1300.0,
-            "which": "fallback (B200_PROFILING.md: 1.59 PFLOP/s burst, ~1.4 sustained, 6.65 TB/s)"}
+    return {"tflops_sustained": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0, "sustained_clock_mhz": None,
+            "which": "data sheet (H100 SXM at 700 W: 989 TFLOP/s dense f16, 3.35 TB/s), not a measured peak"}
 
 
 class ClockSampler(threading.Thread):
@@ -219,10 +218,10 @@ def dominant_roofline(prof, ms_profiled, peaks, clocks, note):
     d = prof[dom]
     avg_s = d["ms_total"] * 1e-3 / d["launches"]
     ach = d["flops_per_launch"] / avg_s / 1e12
-    return {"bound": "tensor", "kernel": f"gemm_tcgen05_kernel ({dom})", "achieved": ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
+    return {"bound": "tensor", "kernel": f"gemm_wgmma_kernel ({dom})", "achieved": ach, "peak": peaks["tflops_sustained"], "unit": "TFLOP/s",
             "frac": ach / peaks["tflops_sustained"], "peak_burst": peaks["tflops_burst"], "frac_burst": ach / peaks["tflops_burst"],
             "sm_mhz_during": clocks.get("sm_mhz"), "peak_sustained_measured_at_mhz": peaks["sustained_clock_mhz"],
-            "traffic": ncu_traffic().get(dom), "traffic_unit": "bytes per launch (ncu dram read+write)", "peak_source": peaks["which"],
+            "peak_source": peaks["which"],
             "avg_launch_ms": avg_s * 1e3, "share_of_step": d["ms_total"] / ms_profiled, "timed_in": note}
 
 
@@ -316,6 +315,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true", help="skip the extra BASELINE.json configurations (ViT-L/16-384, q8_0)")
     ap.add_argument("--sustained-seconds", type=float, default=2.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's outputs as .npy files to DIR")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -349,7 +349,7 @@ def main():
         dist.barrier()
     path = model_path(MODEL_CFG, "f16")
     model = eng.vit_model_load(path, device=local_rank, max_batch=B)
-    # two distinct input batches (2 x 154 MB > 126 MB L2), alternated so no step finds its input in L2
+    # two distinct input batches (2 x 154 MB > 50 MB L2), alternated so no step finds its input in L2
     host_imgs = [torch.from_numpy(gf.synthetic_images(B, 224, seed=1234 + 17 * rank + j)).pin_memory() for j in range(2)]
     dev_imgs = [h.cuda(non_blocking=True) for h in host_imgs]
     d_probs = torch.empty(B, model.num_classes, device="cuda")
@@ -408,6 +408,13 @@ def main():
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
     ms_total = float(t.item())
     value = world * B * args.steps / (ms_total * 1e-3)
+    if args.dump_outputs:
+        # the last timed step's results, before any later region overwrites them (top-5 indices widened exactly to float64)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        sfx = "" if world == 1 else "_rank%d" % rank
+        np.save(os.path.join(args.dump_outputs, "probs%s.npy" % sfx), d_probs.cpu().numpy().astype(np.float32))
+        np.save(os.path.join(args.dump_outputs, "topk_idx%s.npy" % sfx), d_idx.cpu().numpy().astype(np.float64))
+        np.save(os.path.join(args.dump_outputs, "topk_prob%s.npy" % sfx), d_val.cpu().numpy().astype(np.float32))
 
     # ---- region S: the same step back to back for >= sustained_seconds (clock under the power cap settles within ~1 s)
     n_sus = max(args.steps, int(math.ceil(args.sustained_seconds * 1e3 / (ms_local / args.steps))))
@@ -505,7 +512,7 @@ def main():
             "dtype": "f16", "data": "synthetic",
             "config": {"workload": "vit_base_patch16_224 f16 (legacy-ggml model file), batch=%d per GPU, 224x224x3 f32 HWC synthetic images" % B,
                        "global_batch": B * world, "parallelism": "dp%d (images sharded, weights replicated, no collective on the data path)" % world,
-                       "l2": "two alternating 154 MB input batches + >1 GB of activations per step exceed the 126 MB L2; no explicit flush",
+                       "l2": "two alternating 154 MB input batches + >1 GB of activations per step exceed the 50 MB L2; no explicit flush",
                        "attention_operands": "split precision (hi + lo f16 pairs for q, k, v: the reference's f32-operand attention)" if os.environ.get("VITB200_ATTN_HILO", "1") != "0" else "f16 only (VITB200_ATTN_HILO=0)"},
             "e2e": {"value": e2e_value, "unit": "images/s", "h2d_bytes_per_step": B * 3 * 224 * 224 * 4,
                     "d2h_bytes_per_step": B * (model.num_classes * 4 + 5 * 4 + 5 * 4)},
@@ -546,7 +553,8 @@ def main():
                 run_extra_config(eng, L, gf, torch, "vit_base_patch16_224 q8_0 model file (weights dequantised to f16 at upload), batch=256",
                                  "base", "q8_0", 256, 10, 3, os.path.join(gd, "base_q8_0.npz"), peaks, local_rank, stream),
             ]
-        if world == 1 and not args.no_cpu_baseline:
+        from oracle import ref
+        if world == 1 and not args.no_cpu_baseline and ref.available():
             nproc = host_threads()
             rate, nt, dt, tried = cpu_reference_rate(8, thread_candidates())
             line["cpu_baseline"] = {"value": rate, "unit": "images/s", "cores": nt, "kind": "reference",

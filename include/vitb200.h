@@ -1,4 +1,4 @@
-/* vitb200.h -- C ABI of the Blackwell-native ViT forward path (drop-in boundary for staghado/vit.cpp).
+/* vitb200.h -- C ABI of the Hopper-native (sm_90a) ViT forward path (drop-in boundary for staghado/vit.cpp).
  *
  * The reference exposes the forward path as C++ free functions in vit.h:
  *     bool vit_model_load(const std::string&, vit_model&)                       (reference vit.h:120, vit.cpp:308-712)
@@ -170,7 +170,7 @@ typedef struct vitb200_taps
 int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, float *probs, float *logits,
                           const vitb200_taps *taps);
 
-/* Stand-alone run of the tcgen05 GEMM kernel: out[M][N] = epilogue(A[M][K] (f16 bits) x W[N][K]^T (f16 bits)).
+/* Stand-alone run of the wgmma GEMM kernel: out[M][N] = epilogue(A[M][K] (f16 bits) x W[N][K]^T (f16 bits)).
  * epilogue: 0 bias->f16, 1 bias+gelu->f16, 2 bias+resid->f32, 4 bias->f32, 6 bias->split precision (hi = f16(x), lo = f16(x - hi);
  * `out` receives hi + lo).  out is float32[M][N] on the host (f16 results widened).  resid may be NULL unless epilogue == 2. */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
@@ -180,8 +180,8 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
  * ggml.c:8959-9008): x float32 [rows][D] -> y float32 [rows][D] holding the f16 results (the next GEMM's A operand) widened. */
 int vitb200_test_layernorm(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, float *y);
 
-/* Prototype of the reference's q8_0 x q8_0 linear layer on the INTEGER tensor cores (tcgen05.mma kind::i8, one K = 32 MMA per
- * q8_0 block; csrc/gemm_q8_tcgen05.cuh).  Replaces, for one layer, quantize_row_q8_0 (reference ggml-quants.c:702-790: the f32
+/* Prototype of the reference's q8_0 x q8_0 linear layer on the INTEGER tensor cores (wgmma s8, one K = 32 MMA per
+ * q8_0 block; csrc/gemm_q8_wgmma.cuh).  Replaces, for one layer, quantize_row_q8_0 (reference ggml-quants.c:702-790: the f32
  * activation rows x [M][K] are quantised on the device, bit for bit as the reference does) + ggml_vec_dot_q8_0_q8_0
  * (ggml-quants.c:3521+) + the bias add.  w_q8_0 is the tensor as stored in a q8_0 model file: [N][K/32] blocks of {f16 d; int8 q[32]}
  * (ggml-quants.h:42-46).  y = float32 [M][N]; xq (int8 [M][K]) and xd (float32 [M][K/32]) optionally receive the quantised
@@ -192,11 +192,11 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
 
 /* Stand-alone run of one attention kernel (head dim 64) over a fused QKV buffer: qkv = f16 bits [B*N][3*H*64] (what the qkv
  * GEMM leaves behind, reference vit.cpp:826-846), out = float32 [B*N][H*64] (the merged heads before proj, vit.cpp:860-866).
- * kernel: 0 = the engine's choice for N, 1 = mma.sync two-pass, 2 = tcgen05 single block (N <= 224), 3 = tcgen05 two sweeps
- * (224 < N <= 640). */
+ * kernel: 0 = the engine's choice for N, 1 = two-pass mma.sync with 8 warps (any N), 2 = wgmma with TMA-staged operands (N <= 224),
+ * 3 = two-pass mma.sync with 16 warps (128 < N <= 640). */
 int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out);
 
-/* The tcgen05 single-block attention kernel (N <= 224) on split-precision operands, the way the engine runs it: every q, k, v value is
+/* The wgmma attention kernel (N <= 224) on split-precision operands, the way the engine runs it: every q, k, v value is
  * the sum of two f16 numbers, qkv_hi + qkv_lo (what the qkv GEMM's hi-lo epilogue leaves behind: hi = f16(x), lo = f16(x - hi)), so
  * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858). */
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);

@@ -1,4 +1,4 @@
-// integration/benchmark_b200.cpp -- the reference's accuracy harness (tests/benchmark.cpp:34-150) on the B200 engine, batched.
+// integration/benchmark_b200.cpp -- the reference's accuracy harness (tests/benchmark.cpp:34-150) on this engine, batched.
 //
 //   usage: benchmark_b200 <model_path> <dataset_dir> <num_images_per_class> [output_file] [batch]
 //

@@ -159,7 +159,7 @@ def test_bf16_weights_in_f32_container_vs_reference_f32_path():
     path on a file of bf16-representable f32 weights (f16 patch kernel).  The engine rounds f32 weights to f16 at upload,
     which is EXACT for bf16 values with |w| >= 2^-14, and multiplies them with f16 activations; the reference keeps f32
     activations, so agreement is at the f16-activation noise level (SURVEY.md 7.4: 5e-4..1e-3), far from the 5e-3 a
-    bf16-activation design would show.  (f16 x bf16 in one tcgen05.mma is an illegal instruction on B200.)"""
+    bf16-activation design would show.  (One wgmma takes a single operand type: f16 x bf16 is not an option.)"""
     path = model_path("tiny", "bf16w")
     rm = ref.RefModel(path)
     m = eng.vit_model_load(path, 0, 4)

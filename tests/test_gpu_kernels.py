@@ -52,7 +52,7 @@ def test_gemm_against_numpy(M, N, K, epi):
 
 @pytest.mark.parametrize("M,N,K", [(300, 576, 192), (197 * 3, 2304, 768), (129, 384, 192)])
 def test_gemm_split_precision_epilogue(M, N, K):
-    """EPI_BIAS_F16_HILO (the qkv GEMM in front of the tcgen05 attention): hi = f16(x), lo = f16(x - hi); hi + lo must carry the
+    """EPI_BIAS_F16_HILO (the qkv GEMM in front of the split-precision attention): hi = f16(x), lo = f16(x - hi); hi + lo must carry the
     f32 result to ~2^-21 relative (2^-24 absolute once lo is subnormal), i.e. only fp32 accumulation-order noise remains."""
     rng = np.random.default_rng(M + N + K)
     A = rng.standard_normal((M, K)).astype(np.float16)
@@ -115,10 +115,10 @@ def _attention_ref_f32(qkv32, B, N, H):
 
 @pytest.mark.parametrize("B,N,H", [(3, 17, 2), (2, 197, 3), (1, 224, 1), (40, 197, 12), (2, 50, 1)])
 def test_attention_split_precision_against_f32_operand_reference(B, N, H):
-    """attention_tc_kernel with hi + lo operands must follow the f32-operand restatement, not the f16-operand one: a score error of
+    """The wgmma attention kernel with hi + lo operands must follow the f32-operand restatement, not the f16-operand one: a score error of
     2^-12 relative (what rounding q or k to f16 costs) moves x - max across f16 rounding boundaries; with split operands the only
-    differences left are f32 accumulation order + the f16 roundings the reference makes too.  The last case keeps every CTA looping
-    over several (image, head) problems (single-buffered operand groups: empty/full barrier parities)."""
+    differences left are f32 accumulation order + the f16 roundings the reference makes too.  The cases cover one to four 64-query
+    tiles per problem and many (image, head) problems per launch."""
     rng = np.random.default_rng(N * 7 + H)
     qkv = rng.normal(0.0, 1.0, (B * N, 3 * H * 64)).astype(np.float32)
     qkv[:, : H * 64] *= 1.5
@@ -136,17 +136,16 @@ def test_attention_split_precision_against_f32_operand_reference(B, N, H):
 
 
 ATTN_CASES = [  # (B, N, H, kernel)
-    (3, 17, 2, eng.ATTN_TC), (2, 197, 3, eng.ATTN_TC), (2, 197, 3, eng.ATTN_MMA),
-    (2, 577, 2, eng.ATTN_TC_LONG), (2, 577, 2, eng.ATTN_MMA), (1, 225, 1, eng.ATTN_TC_LONG), (3, 384, 1, eng.ATTN_TC_LONG),
-    (2, 401, 2, eng.ATTN_TC_LONG), (1, 640, 1, eng.ATTN_TC_LONG), (20, 577, 16, eng.ATTN_TC_LONG),
+    (3, 17, 2, eng.ATTN_WGMMA), (2, 197, 3, eng.ATTN_WGMMA), (2, 197, 3, eng.ATTN_MMA8),
+    (2, 577, 2, eng.ATTN_MMA16), (2, 577, 2, eng.ATTN_MMA8), (1, 225, 1, eng.ATTN_MMA16), (3, 384, 1, eng.ATTN_MMA16),
+    (2, 401, 2, eng.ATTN_MMA16), (1, 640, 1, eng.ATTN_MMA16), (20, 577, 16, eng.ATTN_MMA16),
 ]
 
 
 @pytest.mark.parametrize("B,N,H,kernel", ATTN_CASES)
 def test_attention_kernels_against_numpy(B, N, H, kernel):
     """Every attention kernel, alone, on random QKV (scores spread over several units so the soft-max is not flat): agreement with
-    the float64 restatement to f16 output rounding + f32 accumulation noise; the last case runs every CTA through many
-    (image, head) problems (persistent-loop parities, K/V ring reuse)."""
+    the float64 restatement to f16 output rounding + f32 accumulation noise; the last case launches many (image, head) problems."""
     rng = np.random.default_rng(N * 131 + H)
     qkv = rng.normal(0.0, 1.0, (B * N, 3 * H * 64)).astype(np.float32)
     qkv[:, : H * 64] *= 1.5                       # Q: |s/8| up to ~5
@@ -165,7 +164,7 @@ Q8_CASES = [(128, 128, 128), (1, 128, 128), (300, 576, 768), (197 * 3, 2304, 768
 
 @pytest.mark.parametrize("M,N,K", Q8_CASES)
 def test_q8_0_gemm_matches_the_reference_integer_dot(M, N, K):
-    """tcgen05 kind::i8 GEMM + on-device activation quantisation against the oracle's quantize_row_q8_0 + vec_dot_q8_0_q8_0
+    """wgmma s8 GEMM + on-device activation quantisation against the oracle's quantize_row_q8_0 + vec_dot_q8_0_q8_0
     (bit-exact restatements of the reference, tests/test_oracle.py): the quantised activations (integer work) must be bit-identical,
     the f32 outputs within 1e-5 of the row's largest output (same products, same f32 accumulation, different order of the
     reference's eight partial lanes)."""

@@ -1,4 +1,4 @@
-"""Dev tool (GPU): throughput of the q8_0 integer tensor-core GEMM prototype (csrc/gemm_q8_tcgen05.cuh) at the ViT-B/16 batch-256
+"""Dev tool (GPU): throughput of the q8_0 integer tensor-core GEMM prototype (csrc/gemm_q8_wgmma.cuh) at the ViT-B/16 batch-256
 layer shapes, CUDA-event timed inside vitb200_test_gemm_q8.  usage: python tools/bench_q8.py [iters]"""
 import json
 import os

@@ -1,4 +1,4 @@
-"""vit.cpp_b200 -- Blackwell-native forward path for staghado/vit.cpp.
+"""vit.cpp_b200 -- Hopper-native (sm_90a) forward path for staghado/vit.cpp.
 
 The product is the C-ABI library built from csrc/ (include/vitb200.h); this Python package is the thin
 host-side mirror of the reference's vit.h interface used by tests/ and bench.py.  The directory name

@@ -3,11 +3,10 @@
 // ggml_allocr + ggml_graph_compute thread pool (reference vit.cpp:1004-1075, ggml.c:15774-16039).
 #include "../../include/vitb200.h"
 
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "kernels.cuh"
-#include "attention_tcgen05.cuh"
-#include "attention_tcgen05_long.cuh"
-#include "gemm_q8_tcgen05.cuh"
+#include "gemm_q8_wgmma.cuh"
+#include "attention_wgmma.cuh"
 #include "gguf_file.hpp"
 #include "preprocess.cuh"
 
@@ -68,45 +67,9 @@ PFN_tmapEncodeTiled tmap_encoder()
 }
 
 // 2-D f16 row-major tensor [rows][cols] with row pitch `pitch` elements, box = 64 columns x box_rows rows,
-// SWIZZLE_128B (matches the UMMA K-major SWIZZLE_128B smem descriptor), out-of-bounds elements read as zero.
-// 2-D f32 row-major tensor [rows][cols], box = 32 columns (128 B) x 32 rows, SWIZZLE_128B: the residual stream X as the
-// residual epilogue loads and stores it (one 4-KB box per epilogue warp and 32-column chunk).
-int make_tmap_f32_box32(CUtensorMap *m, const void *ptr, uint64_t rows, uint64_t cols, uint64_t pitch)
-{
-    PFN_tmapEncodeTiled enc = tmap_encoder();
-    if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {pitch * 4};
-    cuuint32_t box[2] = {32, 32};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void *>(ptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(f32) failed (%d)", (int)r);
-    return 0;
-}
-
-// 3-D f16 view [images][tokens][cols] of a [images*tokens][cols] buffer, box = 64 columns x 32 tokens x 1 image, SWIZZLE_128B:
-// the attention epilogue's store target -- token rows past `tokens` are clipped by the TMA unit instead of spilling into the
-// next image.
-int make_tmap_tokens3d(CUtensorMap *m, const void *ptr, uint64_t images, uint64_t tokens, uint64_t cols)
-{
-    PFN_tmapEncodeTiled enc = tmap_encoder();
-    if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t dims[3] = {cols, tokens, images};
-    cuuint64_t strides[2] = {cols * 2, tokens * cols * 2};
-    cuuint32_t box[3] = {64, 32, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void *>(ptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(3d) failed (%d)", (int)r);
-    return 0;
-}
-
-// 3-D f16 view of a HEAD-MAJOR q / k / v buffer [planes][plane_rows][64] (planes = 3 x heads: q heads, then k heads, then v heads;
-// plane_rows = the arena's token rows): dims {64, rows, planes}, box = 64 columns x box_rows rows x 1 plane, SWIZZLE_128B.  `rows` may be
-// smaller than plane_rows (the qkv epilogue's store map of a batch: rows past the batch are clipped).
+// SWIZZLE_128B (matches the wgmma K-major SWIZZLE_128B smem descriptor), out-of-bounds elements read as zero.
+// 3-D f16 view of a HEAD-MAJOR q / k / v buffer [planes][plane_rows][64] (planes = 3 x heads: q heads, then k heads, then v heads):
+// dims {64, rows, planes}, box = 64 columns x box_rows rows x 1 plane, SWIZZLE_128B (the attention's operand tiles)
 int make_tmap_heads3d(CUtensorMap *m, const void *ptr, uint64_t planes, uint64_t rows, uint64_t plane_rows, uint32_t box_rows)
 {
     PFN_tmapEncodeTiled enc = tmap_encoder();
@@ -118,8 +81,7 @@ int make_tmap_heads3d(CUtensorMap *m, const void *ptr, uint64_t planes, uint64_t
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void *>(ptr), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(heads3d) failed (%d) planes=%llu rows=%llu box_rows=%u", (int)r,
-                                       (unsigned long long)planes, (unsigned long long)rows, box_rows);
+    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(heads3d) failed (%d)", (int)r);
     return 0;
 }
 
@@ -160,7 +122,7 @@ struct Linear
     __half *w = nullptr; // [n_out][ld] f16, K contiguous (ggml ne0 = K)
     float *b = nullptr;  // [n_out]
     int n_out = 0, n_in = 0, ld = 0, bn = 256;
-    CUtensorMap tm;  // box = 64 x (bn / cta_group) rows: the share of the W tile one CTA stages
+    CUtensorMap tm;  // box = 64 x bn rows: the W tile of one k-block
 };
 
 struct Layer
@@ -176,7 +138,7 @@ int pick_bn(int n_out) { return n_out >= 256 ? 256 : 128; }
 struct vitb200_engine
 {
     vitb200_hparams hp;
-    int device = 0, max_batch = 0, num_sms = 148;
+    int device = 0, max_batch = 0, num_sms = 132;
     int N = 0, NP = 0, G = 0, KP = 0, KPp = 0;
     int Cp = 0;           // num_classes rounded up to a multiple of 4: pitch of the internal logits rows (128-bit epilogue stores)
     float *d_sm_scratch = nullptr; // soft-max working rows in global memory, only when num_classes floats exceed shared memory
@@ -192,21 +154,14 @@ struct vitb200_engine
     float *d_img = nullptr, *X = nullptr, *d_logits = nullptr, *d_probs = nullptr, *d_topk_val = nullptr;
     int32_t *d_topk_idx = nullptr;
     __half *A16 = nullptr, *QKV16 = nullptr, *H16 = nullptr, *CLS16 = nullptr, *PA = nullptr;
-    __half *QKV16L = nullptr; // lo halves of q, k, v (x - f16(x), as f16): the tcgen05 attention's split-precision operands
-    int *d_ln_count = nullptr; // fused LayerNorm: one completion counter per 32-row group of the residual stream (zero between launches)
+    __half *QKV16L = nullptr; // lo halves of q, k, v (x - f16(x), as f16): the attention's split-precision operands
+    int *d_ln_count = nullptr; // fused LayerNorm: one completion counter per 128-row M tile of the residual stream (zero between launches)
     bool fused_ln = false;     // LayerNorm applied inside the proj / fc2 residual epilogues (VITB200_FUSED_LN=0: separate kernel)
-    bool attn_hilo = false;   // qkv GEMM emits hi + lo and attention_tc_kernel runs the 3 + 2 term products (VITB200_ATTN_HILO=0: hi only)
-    CUtensorMap tmQl, tmKVl;
-    CUtensorMap tmA_D, tmA_H, tmA_P, tmA_C, tmQ, tmKV, tmAO, tmKV64;
-    // maps of the tensors the GEMM epilogues WRITE with TMA, clipped to batch * N rows so that nothing past the batch is ever
-    // stored (and, for the residual stream, loaded): X f32 (32 x 32 boxes), QKV hi / lo and the MLP hidden buffer f16 (64 x 32 boxes)
-    struct BatchMaps { CUtensorMap X, QKVh, QKVl, H; };
-    std::map<int, BatchMaps> batch_maps;
-    bool attn_tc = false;      // tcgen05 single-block attention (N <= 224)
-    bool attn_tc_long = false; // tcgen05 two-sweep attention (224 < N <= 640); anything longer uses the mma.sync two-pass kernel
+    bool attn_hilo = false;   // qkv GEMM emits hi + lo and the attention runs the 3 + 2 term products (VITB200_ATTN_HILO=0: hi only)
+    CUtensorMap tmA_D, tmA_H, tmA_P, tmA_C;
+    CUtensorMap tmQ, tmKV, tmQl, tmKVl; // attention operand maps (N <= 224: attention_wgmma_kernel)
     int max_k = 16;
     int launches = 0;
-    int cta_group = 2; // CTAs per tcgen05.mma in the GEMMs (2 = CTA pairs; VITB200_CTA_GROUP=1 selects the 1-CTA kernels)
     std::map<int, std::string> labels;
     // host-buffer pipeline (vitb200_forward_async): 2 input/output slots, H2D on a copy stream overlapping the previous
     // call's kernels on the compute stream
@@ -389,8 +344,8 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
         {
             // Rounded once to f16.  A bf16 checkpoint widened to f32 (the only way this container can carry bf16,
             // BASELINE.json configs[2]) converts EXACTLY for every weight with |w| >= 2^-14 (8-bit mantissa fits in 11).
-            // Keeping such weights as bf16 is not an option: tcgen05.mma kind::f16 with a_format = f16 and b_format = bf16
-            // raises "illegal instruction" on B200 (tried in round 1), and bf16 activations cost 5e-3 parity (SURVEY.md 7.4).
+            // Keeping such weights as bf16 would need bf16 activations too (one wgmma takes one operand type), and bf16
+            // activations cost 5e-3 parity (SURVEY.md 7.4).
             const float *f = (const float *)w->data;
             for (size_t i = 0; i < conv.size(); ++i) conv[i] = host_f32_to_f16(f[i]);
         }
@@ -422,7 +377,7 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     CUDA_TRY(cudaMemcpy2D(L->w, (size_t)ld * 2, src, (size_t)n_in * 2, (size_t)n_in * 2, (size_t)n_out, cudaMemcpyHostToDevice));
     // conv bias is declared [1, 1, D] (vit.cpp:516), every other bias [n_out]; the tail up to a multiple of 4 stays zero
     if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
-    return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)(L->bn / e->cta_group));
+    return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)L->bn);
 }
 
 // dynamic shared memory the soft-max kernel may use for its working row (227 KB per CTA minus its static arrays)
@@ -454,18 +409,16 @@ struct ProfScope
     }
 };
 
-// L2 eviction hints on the big streamed-once transfers (profiles/microbench_r02.md: fc1 -4 %, LayerNorm -2 %, proj / fc2 -1 % at batch 256 --
-// the 465 MB of q, k, v and the 310 MB MLP hidden buffer no longer push the LayerNorm output, which the next GEMM reads nine to twelve
-// times, out of the 126 MB L2).  VITB200_L2HINT = bit mask, default 7: 1 = qkv / fc1 output stores evict_first, 2 = attention operand
-// loads evict_first, 4 = LayerNorm input loads evict_first (8 = LayerNorm output stores evict_last: measured worse, off).
+// L2 eviction hints of the stand-alone LayerNorm: its input rows are read once, its output is read by the next GEMM nine to twelve
+// times.  VITB200_L2HINT = bit mask, default 4: 4 = LayerNorm input loads evict_first, 8 = LayerNorm output stores evict_last.
 int l2_hint_mask()
 {
-    static const int m = getenv("VITB200_L2HINT") ? atoi(getenv("VITB200_L2HINT")) : 7;
+    static const int m = getenv("VITB200_L2HINT") ? atoi(getenv("VITB200_L2HINT")) : 4;
     return m;
 }
 
 // Programmatic dependent launch for the per-layer kernels (GEMMs, attention, LayerNorm): each of them ends its prologue with
-// griddepcontrol.launch_dependents + griddepcontrol.wait (ptx.cuh), so kernel k+1's barrier init / TMEM allocation / descriptor
+// griddepcontrol.launch_dependents + griddepcontrol.wait (ptx.cuh), so kernel k+1's barrier init / descriptor
 // prefetch runs on the SMs kernel k has already left.  VITB200_PDL=0 launches them fully serialised.
 bool pdl_enabled()
 {
@@ -486,12 +439,11 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int BN, int EPI, int CG, int DEEPK = 0>
-int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmX, const CUtensorMap &tmO2, const GemmParams &p, cudaStream_t s, int num_sms)
+template <int BN, int EPI>
+int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
-    using Cfg = GemmCfg<BN, EPI == EPI_BIAS_RESID_F32, CG, EPI == EPI_PATCH_GATHER_F32, DEEPK != 0,
-                        EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO>;
-    auto kern = gemm_tcgen05_kernel<BN, EPI, DEEPK, CG>;
+    using Cfg = GemmCfg<BN>;
+    auto kern = gemm_wgmma_kernel<BN, EPI>;
     // the opt-in to > 48 KB dynamic shared memory is per device (one engine per device, possibly several per process)
     static bool attr_set[64] = {};
     int dev = 0;
@@ -501,42 +453,18 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         attr_set[dev & 63] = true;
     }
-    const int m_tiles = (p.M + GEMM_BM * CG - 1) / (GEMM_BM * CG), n_tiles = (p.N + BN - 1) / BN;
-    const int tiles = m_tiles * n_tiles;
-    const int max_groups = num_sms / CG;
-    const int groups = tiles < max_groups ? tiles : max_groups;
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3((unsigned)(groups * CG));
-    cfg.blockDim = dim3((unsigned)Cfg::kThreads);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmX, tmO2, p));
+    const int tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + BN - 1) / BN);
+    CUDA_TRY(launch_pdl(kern, dim3((unsigned)tiles), dim3((unsigned)Cfg::kThreads), (size_t)Cfg::SMEM_BYTES, s, tmA, tmB, p));
     if (e) e->launches++;
     return 0;
 }
 
-// tmB: box rows = bn / cg.  tmX: EPI_BIAS_RESID_F32 -- f32 [M][ldo] map of the residual/output; f16 epilogues -- f16 [M][ldo] map of the
-// output (64 x 32 boxes) and tmO2 the lo tensor of EPI_BIAS_F16_HILO; ignored otherwise
-int launch_gemm(vitb200_engine *e, int cg, int bn, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmX, const CUtensorMap &tmO2, const GemmParams &p, cudaStream_t s, int num_sms)
+// tmB: the weight map, box = 64 x bn rows
+int launch_gemm(vitb200_engine *e, int bn, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
-#define VB_CASE(BN, EPI)                                                                                         \
-    if (bn == BN && epi == EPI)                                                                                  \
-        return cg == 2 ? launch_gemm_t<BN, EPI, 2>(e, tmA, tmB, tmX, tmO2, p, s, num_sms) : launch_gemm_t<BN, EPI, 1>(e, tmA, tmB, tmX, tmO2, p, s, num_sms);
-    if (epi == EPI_PATCH_GATHER_F32) // CTA pairs only (the A producers fill three pipeline stages at a time)
-    {
-        if (cg != 2) return fail("gathered patch embedding needs cta_group 2");
-        return bn == 256 ? launch_gemm_t<256, EPI_PATCH_GATHER_F32, 2>(e, tmA, tmB, tmX, tmO2, p, s, num_sms)
-                         : launch_gemm_t<128, EPI_PATCH_GATHER_F32, 2>(e, tmA, tmB, tmX, tmO2, p, s, num_sms);
-    }
-    if (epi == EPI_BIAS_RESID_F32 && bn == 256 && cg == 2 && p.K >= 2048) // fc2: shallower residual ring, one more operand stage
-        return launch_gemm_t<256, EPI_BIAS_RESID_F32, 2, 1>(e, tmA, tmB, tmX, tmO2, p, s, num_sms);
+    if (p.N % 4 != 0) return fail("GEMM: N = %d is not a multiple of 4", p.N);
+#define VB_CASE(BN, EPI) \
+    if (bn == BN && epi == EPI) return launch_gemm_t<BN, EPI>(e, tmA, tmB, p, s);
     VB_CASE(256, EPI_BIAS_F16) VB_CASE(128, EPI_BIAS_F16)
     VB_CASE(256, EPI_BIAS_F16_HILO) VB_CASE(128, EPI_BIAS_F16_HILO)
     VB_CASE(256, EPI_BIAS_GELU_F16) VB_CASE(128, EPI_BIAS_GELU_F16)
@@ -632,12 +560,51 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
     return 0;
 }
 
+// Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
+// token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision when the lo halves exist; ATT_MMA16 = the mma.sync kernel
+// with 16 warps, 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.
+enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3 };
+constexpr int ATT_MAX_KEYS_16 = 640;
+
+// q / k / v tensor maps of the wgmma attention over `rows` token rows per plane
+int make_attention_maps(vitb200_engine *e, uint64_t rows)
+{
+    const uint64_t planes = 3 * (uint64_t)e->hp.num_attention_heads;
+    if (make_tmap_heads3d(&e->tmQ, e->QKV16, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKV, e->QKV16, planes, rows, rows, ATTW_KEYS))
+        return 1;
+    if (e->QKV16L && (make_tmap_heads3d(&e->tmQl, e->QKV16L, planes, rows, rows, 64) ||
+                      make_tmap_heads3d(&e->tmKVl, e->QKV16L, planes, rows, rows, ATTW_KEYS)))
+        return 1;
+    return 0;
+}
+
+template <bool HILO>
+int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
+{
+    const int smem = attention_wgmma_smem_bytes(HILO);
+    auto kern = attention_wgmma_kernel<HILO>;
+    static bool attr_set[64] = {};
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    if (!attr_set[dev & 63])
+    {
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        attr_set[dev & 63] = true;
+    }
+    const int H = e->hp.num_attention_heads;
+    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)smem, s, e->tmQ, e->tmKV, HILO ? e->tmQl : e->tmQ, HILO ? e->tmKVl : e->tmKV,
+                        e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H))));
+    e->launches++;
+    return 0;
+}
+
 template <int NW>
 int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int N = e->N, D = e->hp.hidden_size, H = e->hp.num_attention_heads;
     const int Npad = (N + ATT_KC - 1) / ATT_KC * ATT_KC;
     const int smem = 2 * Npad * 128;
+    if (smem > 232448) return fail("attention: %d tokens do not fit in shared memory", N);
     auto kern = attention_kernel<NW>;
     static int smem_set[64] = {};
     int dev = 0;
@@ -647,130 +614,18 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
         smem_set[dev & 63] = smem;
     }
-    kern<<<B * H, NW * 32, smem, s>>>(e->QKV16, (size_t)e->max_batch * N, e->A16, N, D, H, Npad, 1.0f / sqrtf((float)(D / H)));
-    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(NW * 32), (size_t)smem, s, e->QKV16, (size_t)e->max_batch * N,
+                        e->A16, N, D, H, Npad, 1.0f / sqrtf((float)(D / H))));
     e->launches++;
     return 0;
 }
 
-int launch_attention_tc(vitb200_engine *e, int B, cudaStream_t s)
+int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO)
 {
-    AttnTcParams p{};
-    p.N = e->N; p.D = e->hp.hidden_size; p.H = e->hp.num_attention_heads;
-    p.n_problems = B * p.H;
-    p.NKP = (e->N + 15) / 16 * 16;
-    p.n_mtiles = (e->N + 127) / 128;
-    p.kv_bytes = (p.NKP * 128 + 1023) / 1024 * 1024;
-    p.scale = 1.0f / sqrtf((float)(p.D / p.H));
-    p.hilo = e->attn_hilo ? 1 : 0;
-    p.load_policy = (l2_hint_mask() & 2) ? ptx::L2_EVICT_FIRST : 0;
-    p.reverse = !(getenv("VITB200_ATTN_REVERSE") && atoi(getenv("VITB200_ATTN_REVERSE")) == 0);
-    const int smem = attention_tc_smem_bytes(p.kv_bytes);
-    static int smem_set[64] = {};
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (smem > smem_set[dev & 63])
-    {
-        CUDA_TRY(cudaFuncSetAttribute(attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        smem_set[dev & 63] = smem;
-    }
-    const int grid = p.n_problems < e->num_sms ? p.n_problems : e->num_sms;
-    // dev knob: VITB200_ATTN_TRACE=<file> dumps the clock64 phase stamps of CTA 0 for the first launch of the process
-    static int trace_state = 0; // 0 unknown, 1 armed, 2 done/off
-    const char *trace_path = trace_state == 0 ? getenv("VITB200_ATTN_TRACE") : nullptr;
-    if (trace_state == 0) trace_state = trace_path ? 1 : 2;
-    long long *d_trace = nullptr;
-    if (trace_state == 1)
-    {
-        CUDA_TRY(cudaMalloc(&d_trace, 16 * 32 * sizeof(long long)));
-        CUDA_TRY(cudaMemset(d_trace, 0, 16 * 32 * sizeof(long long)));
-        p.trace = d_trace;
-    }
-    CUDA_TRY(launch_pdl(attention_tc_kernel, dim3(grid), dim3(ATT_TC_THREADS), (size_t)smem, s, e->tmQ, e->tmKV,
-                        e->attn_hilo ? e->tmQl : e->tmQ, e->attn_hilo ? e->tmKVl : e->tmKV, e->tmAO, p));
-    CUDA_TRY(cudaGetLastError());
-    if (d_trace)
-    {
-        std::vector<long long> h(16 * 32);
-        CUDA_TRY(cudaStreamSynchronize(s));
-        CUDA_TRY(cudaMemcpy(h.data(), d_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d_trace);
-        if (FILE *f = fopen(getenv("VITB200_ATTN_TRACE"), "w"))
-        {
-            for (int i = 0; i < 16; ++i) { for (int j = 0; j < 32; ++j) fprintf(f, "%lld ", h[i * 32 + j]); fprintf(f, "\n"); }
-            fclose(f);
-        }
-        trace_state = 2;
-    }
-    e->launches++;
-    return 0;
-}
-
-int launch_attention_tc_long(vitb200_engine *e, int B, cudaStream_t s)
-{
-    AttnLongParams p{};
-    p.N = e->N; p.D = e->hp.hidden_size; p.H = e->hp.num_attention_heads;
-    p.n_problems = B * p.H;
-    p.NKP = (e->N + 15) / 16 * 16;
-    p.kv_rows = (p.NKP + 63) / 64 * 64;
-    p.n_tiles = (e->N + 127) / 128;
-    {
-        const int chunks = (p.NKP + 31) / 32;    // 32-key chunks; a block holds at most 3 (96 TMEM columns)
-        p.nb = (chunks + 2) / 3;
-        if (p.nb < 2) p.nb = 2;                  // the sweep-B pipeline alternates between two buffers
-    }
-    p.scale = 1.0f / sqrtf((float)(p.D / p.H));
-    p.load_policy = (l2_hint_mask() & 2) ? ptx::L2_EVICT_FIRST : 0;
-    if (p.nb > ATT_LONG_MAX_BLOCKS || (p.NKP + 31) / 32 < p.nb)
-        return fail("attention: %d tokens cannot be cut into 2..%d key blocks", e->N, ATT_LONG_MAX_BLOCKS);
-    for (int j = 0; j < p.nb; ++j) p.key0[j] = att_long_block_key0(p.NKP, p.nb, j);
-    p.key0[p.nb] = p.NKP;
-    if (p.n_tiles < 2) return fail("two-sweep attention needs at least two query tiles (N > 128)");
-    const int smem = attention_tc_long_smem_bytes(p.kv_rows);
-    static int smem_set[64] = {};
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (smem > smem_set[dev & 63])
-    {
-        CUDA_TRY(cudaFuncSetAttribute(attention_tc_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        smem_set[dev & 63] = smem;
-    }
-    const int grid = p.n_problems < e->num_sms ? p.n_problems : e->num_sms;
-    // dev knob: VITB200_ATTN_TRACE=<file> dumps the clock64 phase stamps of CTA 0 (first 16 query tiles) of the first launch of the process
-    static int trace_state = 0; // 0 unknown, 1 armed, 2 done/off
-    if (trace_state == 0) trace_state = getenv("VITB200_ATTN_TRACE") ? 1 : 2;
-    long long *d_trace = nullptr;
-    if (trace_state == 1)
-    {
-        CUDA_TRY(cudaMalloc(&d_trace, 16 * 32 * sizeof(long long)));
-        CUDA_TRY(cudaMemset(d_trace, 0, 16 * 32 * sizeof(long long)));
-        p.trace = d_trace;
-    }
-    CUDA_TRY(launch_pdl(attention_tc_long_kernel, dim3(grid), dim3(ATT_LONG_THREADS), (size_t)smem, s, e->tmQ, e->tmKV64, e->tmAO, p));
-    if (d_trace)
-    {
-        std::vector<long long> h(16 * 32);
-        CUDA_TRY(cudaStreamSynchronize(s));
-        CUDA_TRY(cudaMemcpy(h.data(), d_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost));
-        cudaFree(d_trace);
-        if (FILE *f = fopen(getenv("VITB200_ATTN_TRACE"), "w"))
-        {
-            for (int i = 0; i < 16; ++i) { for (int j = 0; j < 32; ++j) fprintf(f, "%lld ", h[i * 32 + j]); fprintf(f, "\n"); }
-            fclose(f);
-        }
-        trace_state = 2;
-    }
-    e->launches++;
-    return 0;
-}
-
-int launch_attention(vitb200_engine *e, int B, cudaStream_t s)
-{
-    if (e->attn_tc) return launch_attention_tc(e, B, s);
-    if (e->attn_tc_long) return launch_attention_tc_long(e, B, s);
-    const int qtiles = (e->N + 15) / 16;
-    if (qtiles <= 4) return launch_attention_t<4>(e, B, s);
-    if (qtiles <= 14) return launch_attention_t<7>(e, B, s);
+    if (kernel == ATT_AUTO) kernel = e->N <= ATTW_KEYS ? ATT_WGMMA : (e->N <= ATT_MAX_KEYS_16 ? ATT_MMA16 : ATT_MMA8);
+    if (kernel == ATT_WGMMA) return e->attn_hilo ? launch_attention_wgmma<true>(e, B, s) : launch_attention_wgmma<false>(e, B, s);
+    if (e->attn_hilo) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
+    if (kernel == ATT_MMA16) return launch_attention_t<16>(e, B, s);
     return launch_attention_t<8>(e, B, s);
 }
 
@@ -821,45 +676,23 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     const int D = e->hp.hidden_size, N = e->N, T = B * N, C = e->hp.num_classes;
     e->launches = 0;
     __half *PA = e->PA;
-    // the epilogues store whole boxes with TMA (and the residual epilogue read-modify-writes 32-row boxes of X): with maps of exactly T
-    // rows the rows of the last M tile that lie past the batch are zero-filled on load and clipped on store
-    auto bm = e->batch_maps.find(B);
-    if (bm == e->batch_maps.end())
-    {
-        vitb200_engine::BatchMaps m;
-        memset(&m, 0, sizeof(m));
-        if (make_tmap_f32_box32(&m.X, e->X, (uint64_t)T, (uint64_t)D, (uint64_t)D) ||
-            make_tmap_heads3d(&m.QKVh, e->QKV16, 3 * (uint64_t)e->hp.num_attention_heads, (uint64_t)T, (uint64_t)e->max_batch * N, 32) ||
-            (e->QKV16L && make_tmap_heads3d(&m.QKVl, e->QKV16L, 3 * (uint64_t)e->hp.num_attention_heads, (uint64_t)T, (uint64_t)e->max_batch * N, 32)) ||
-            make_tmap(&m.H, e->H16, (uint64_t)T, 4 * (uint64_t)D, 4 * (uint64_t)D, 32))
-            return 1;
-        bm = e->batch_maps.emplace(B, m).first;
-    }
-    const CUtensorMap &tmX = bm->second.X, &tmQKVh = bm->second.QKVh, &tmQKVl = bm->second.QKVl, &tmH = bm->second.H;
-
     // patch embedding (vit.cpp:772-797): the f16 patch matrix PA (im2col of a stride == kernel conv is a pure permutation,
     // ggml.c:11528-11608) is either already there (d_images == NULL: the u8 path's preprocess kernel wrote it) or written by
     // patchify (one warp per patch, coalesced); the TMA-fed GEMM adds conv bias + pos_embed and writes token rows.
-    // VITB200_PATCH_GATHER=1 (P = 16, CTA pairs, 3 channels) selects the single-kernel variant whose A producers gather the f32
-    // pixels straight into the operand tiles: no patch matrix, but its dependent 128-bit loads are L2-latency bound on an SM with no
-    // L1 left (0.29 ms against 0.05 + 0.10 ms at batch 256, profiles/), so it is no longer the default.
     const bool patches_ready = d_images == nullptr;
-    const bool fused_patch = !patches_ready && e->hp.patch_size == 16 && e->cta_group == 2 && e->C == 3 &&
-                             getenv("VITB200_PATCH_GATHER") && atoi(getenv("VITB200_PATCH_GATHER")) == 1;
     {
         GemmParams p{};
         p.M = B * e->NP; p.N = D; p.K = e->KPp; p.bias = e->patch.b; p.out = e->X; p.ldo = D;
         p.pos = e->pos; p.np = e->NP; p.ntok = N;
-        p.img = d_images; p.S = e->hp.img_size; p.G = e->G;
         ProfScope ps(e, PK_PATCH, 2.0 * p.M * p.N * e->KP, s);
-        if (!patches_ready && !fused_patch && launch_patchify(e, d_images, PA, B, s)) return 1;
+        if (!patches_ready && launch_patchify(e, d_images, PA, B, s)) return 1;
         {
             const int n = B * D, threads = 256;
             cls_rows_kernel<<<(n + threads - 1) / threads, threads, 0, s>>>(e->X, e->cls, e->pos, B, N, D);
             CUDA_TRY(cudaGetLastError());
             e->launches++;
         }
-        if (launch_gemm(e, e->cta_group, e->patch.bn, fused_patch ? EPI_PATCH_GATHER_F32 : EPI_PATCH_F32, e->tmA_P, e->patch.tm, tmX, tmX, p, s, e->num_sms)) return 1;
+        if (launch_gemm(e, e->patch.bn, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
     if (taps && tap_f32(taps->embed, e->X, (size_t)T * D, s)) return 1;
 
@@ -878,9 +711,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         }
         {
             GemmParams p{};
-            p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.store_policy = (l2_hint_mask() & 1) ? ptx::L2_EVICT_FIRST : 0;
+            p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.plane_rows = (size_t)e->max_batch * N;
             ProfScope ps(e, PK_QKV, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, e->cta_group, L.qkv.bn, e->attn_hilo ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, tmQKVh, tmQKVl, p, s, e->num_sms)) return 1; // vit.cpp:820-821
+            if (launch_gemm(e, L.qkv.bn, e->attn_hilo ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
         }
         if (tap && tap_qkv(e, taps->qkv, T, s)) return 1;
         {
@@ -893,9 +726,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
             // lands, written over the attention output in A16 (every tile that read those rows has finished its MMAs by then)
             GemmParams p{};
             p.M = T; p.N = D; p.K = D; p.bias = L.proj.b; p.out = e->X; p.ldo = D; p.resid = e->X;
-            if (e->fused_ln) { p.ln_out = e->A16; p.ln_w = L.n2w; p.ln_b = L.n2b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps; p.ln_dbg = getenv("VITB200_LN_DBG") ? atoi(getenv("VITB200_LN_DBG")) : 0; }
+            if (e->fused_ln) { p.ln_out = e->A16; p.ln_w = L.n2w; p.ln_b = L.n2b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps; }
             ProfScope ps(e, PK_PROJ, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, e->cta_group, L.proj.bn, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, tmX, tmX, p, s, e->num_sms)) return 1;
+            if (launch_gemm(e, L.proj.bn, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1;
         }
         if (tap && tap_f32(taps->x1, e->X, (size_t)T * D, s)) return 1;
         if (!e->fused_ln)
@@ -906,9 +739,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         if (tap && tap_f16(taps->ln2, e->A16, (size_t)T * D, s)) return 1;
         {
             GemmParams p{};
-            p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D; p.store_policy = (l2_hint_mask() & 1) ? ptx::L2_EVICT_FIRST : 0;
+            p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D;
             ProfScope ps(e, PK_FC1, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, e->cta_group, L.fc1.bn, EPI_BIAS_GELU_F16, e->tmA_D, L.fc1.tm, tmH, tmH, p, s, e->num_sms)) return 1; // vit.cpp:889-893
+            if (launch_gemm(e, L.fc1.bn, EPI_BIAS_GELU_F16, e->tmA_D, L.fc1.tm, p, s)) return 1; // vit.cpp:889-893
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
@@ -920,10 +753,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
             {
                 const Layer &Ln = e->layers[il + 1];
                 p.ln_out = e->A16; p.ln_w = Ln.n1w; p.ln_b = Ln.n1b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps;
-                p.ln_dbg = getenv("VITB200_LN_DBG") ? atoi(getenv("VITB200_LN_DBG")) : 0;
             }
             ProfScope ps(e, PK_FC2, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, e->cta_group, L.fc2.bn, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, tmX, tmX, p, s, e->num_sms)) return 1;
+            if (launch_gemm(e, L.fc2.bn, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1;
         }
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
         if (e->fused_ln && taps && taps->layer == il + 1 && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1; // norm1 of the next block
@@ -943,7 +775,7 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         GemmParams p{};
         p.M = R; p.N = Cp; p.K = D; p.bias = e->head.b; p.out = lg; p.ldo = Cp;
         ProfScope ps(e, PK_HEAD, 2.0 * p.M * C * p.K, s);
-        if (launch_gemm(e, e->cta_group, e->head.bn, EPI_BIAS_F32, e->tmA_C, e->head.tm, tmX, tmX, p, s, e->num_sms)) return 1;
+        if (launch_gemm(e, e->head.bn, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
     }
     if (d_logits && lg != d_logits)
         CUDA_TRY(cudaMemcpy2DAsync(d_logits, (size_t)C * 4, lg, (size_t)Cp * 4, (size_t)C * 4, (size_t)R, cudaMemcpyDeviceToDevice, s));
@@ -1055,7 +887,7 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     if (hp->hidden_size % hp->num_attention_heads != 0 || hp->hidden_size / hp->num_attention_heads != 64)
         return fail("head dim %d not supported (64 only)", hp->num_attention_heads ? hp->hidden_size / hp->num_attention_heads : 0);
     if (hp->hidden_size % 64 != 0) return fail("hidden size %d must be a multiple of 64", hp->hidden_size);
@@ -1090,7 +922,6 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     e->Cp = (hp->num_classes + 3) / 4 * 4;
     e->KP = e->C * P * P;
     e->KPp = (e->KP + 63) / 64 * 64;
-    e->cta_group = (getenv("VITB200_CTA_GROUP") && atoi(getenv("VITB200_CTA_GROUP")) == 1) ? 1 : 2;
     e->use_graph = !(getenv("VITB200_GRAPH") && atoi(getenv("VITB200_GRAPH")) == 0);
     auto bail = [&](int) { vitb200_destroy(e); e = nullptr; return 1; };
     if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
@@ -1151,12 +982,13 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
             cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming) != cudaSuccess)
             return bail(fail("cudaEventCreate failed"));
     {
-        // Fused LayerNorm (residual epilogue + dedicated LayerNorm warps, gemm_tcgen05.cuh): bit-identical to the stand-alone kernel but
-        // SLOWER on B200 at batch 256 (proj + LN 2.78 ms vs 1.15 + 0.60 ms per forward, DESIGN.md section 3), so it is opt-in
-        // (VITB200_FUSED_LN=1).  It needs the whole row in N % 128 == 0 float4-per-lane form and w, b in shared memory.
+        // Fused LayerNorm (the CTA that completes an M tile of the residual epilogue normalises its rows, gemm_wgmma.cuh): bit-identical
+        // to the stand-alone kernel, opt-in (VITB200_FUSED_LN=1): the normalisation then runs on a few CTAs at the tail of the GEMM instead
+        // of on the whole GPU.  It needs the whole row in N % 128 == 0 float4-per-lane form.
         const bool want = getenv("VITB200_FUSED_LN") && atoi(getenv("VITB200_FUSED_LN")) == 1;
         e->fused_ln = want && D % 128 == 0 && D <= 1024;
-        if (e->fused_ln && dev_alloc(e, &e->d_ln_count, (T + 255) / 256 * 8 + 8)) return bail(1);
+        if (e->fused_ln && (dev_alloc(e, &e->d_ln_count, T / GEMM_BM + 1) || cudaMemset(e->d_ln_count, 0, (T / GEMM_BM + 1) * sizeof(int)) != cudaSuccess))
+            return bail(1);
     }
     if (pa_alias) e->PA = e->H16;
     else
@@ -1167,36 +999,11 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_BM) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_BM) ||
         make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_BM) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_BM))
         return bail(1);
-    {
-        const char *force = getenv("VITB200_ATTENTION"); // bring-up knob: "mma" forces the warp-MMA kernel
-        const bool force_mma = force && strcmp(force, "mma") == 0;
-        e->attn_tc = e->N <= 224 && !force_mma;
-        e->attn_tc_long = e->N > 224 && e->N <= ATT_LONG_MAX_KEYS && !force_mma;
-        if (e->attn_tc_long)
-        {
-            if (make_tmap_heads3d(&e->tmQ, e->QKV16, 3 * (uint64_t)hp->num_attention_heads, T, T, 128) ||
-                make_tmap_heads3d(&e->tmKV64, e->QKV16, 3 * (uint64_t)hp->num_attention_heads, T, T, 64) ||
-                make_tmap_tokens3d(&e->tmAO, e->A16, (uint64_t)B, (uint64_t)e->N, (uint64_t)D))
-                return bail(1);
-        }
-        if (e->attn_tc)
-        {
-            const int NKP = (e->N + 15) / 16 * 16;
-            if (make_tmap_heads3d(&e->tmQ, e->QKV16, 3 * (uint64_t)hp->num_attention_heads, T, T, 128) ||
-                make_tmap_heads3d(&e->tmKV, e->QKV16, 3 * (uint64_t)hp->num_attention_heads, T, T, (uint32_t)NKP) ||
-                make_tmap_tokens3d(&e->tmAO, e->A16, (uint64_t)B, (uint64_t)e->N, (uint64_t)D))
-                return bail(1);
-            // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858); VITB200_ATTN_HILO=0 keeps the f16-only operands
-            e->attn_hilo = !(getenv("VITB200_ATTN_HILO") && atoi(getenv("VITB200_ATTN_HILO")) == 0);
-            if (e->attn_hilo)
-            {
-                if (dev_alloc(e, &e->QKV16L, T * 3 * D) ||
-                    make_tmap_heads3d(&e->tmQl, e->QKV16L, 3 * (uint64_t)hp->num_attention_heads, T, T, 128) ||
-                    make_tmap_heads3d(&e->tmKVl, e->QKV16L, 3 * (uint64_t)hp->num_attention_heads, T, T, (uint32_t)NKP))
-                    return bail(1);
-            }
-        }
-    }
+    // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
+    // memory (N <= 224); VITB200_ATTN_HILO=0 keeps the f16-only operands
+    e->attn_hilo = e->N <= ATTW_KEYS && !(getenv("VITB200_ATTN_HILO") && atoi(getenv("VITB200_ATTN_HILO")) == 0);
+    if (e->attn_hilo && dev_alloc(e, &e->QKV16L, T * 3 * D)) return bail(1);
+    if (e->N <= ATTW_KEYS && make_attention_maps(e, T)) return bail(1);
     if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
     *out = e;
     e = nullptr; // ownership passed to the caller
@@ -1292,7 +1099,7 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     vitb200_engine *e = new vitb200_engine();
     e->device = device;
     auto bail = [&](int rc) { vitb200_destroy(e); return rc; };
@@ -1322,24 +1129,12 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
     // cudaMemcpy from pageable memory may return before the DMA has landed, and the kernels below run on a NON-BLOCKING stream (no implicit
     // ordering with the legacy stream the copies used): wait for the device before launching
     if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
-    if (kernel == 0) kernel = N <= 224 ? 2 : (N <= ATT_LONG_MAX_KEYS ? 3 : 1);
-    if (kernel == 2 && N > 224) return bail(fail("tcgen05 single-block attention needs N <= 224"));
-    if (kernel == 3 && (N <= 128 || N > ATT_LONG_MAX_KEYS)) return bail(fail("tcgen05 two-sweep attention needs 128 < N <= %d", ATT_LONG_MAX_KEYS));
-    e->attn_tc = kernel == 2;
-    e->attn_tc_long = kernel == 3;
-    if (kernel >= 2)
-    {
-        const int NKP = (N + 15) / 16 * 16;
-        if (make_tmap_heads3d(&e->tmQ, e->QKV16, 3 * (uint64_t)H, T, T, 128) ||
-            make_tmap_heads3d(&e->tmKV, e->QKV16, 3 * (uint64_t)H, T, T, (uint32_t)(NKP <= 224 ? NKP : 64)) ||
-            make_tmap_heads3d(&e->tmKV64, e->QKV16, 3 * (uint64_t)H, T, T, 64) ||
-            make_tmap_tokens3d(&e->tmAO, e->A16, (uint64_t)B, (uint64_t)N, (uint64_t)D))
-            return bail(1);
-        if (qkv_lo && (make_tmap_heads3d(&e->tmQl, e->QKV16L, 3 * (uint64_t)H, T, T, 128) ||
-                       make_tmap_heads3d(&e->tmKVl, e->QKV16L, 3 * (uint64_t)H, T, T, (uint32_t)NKP)))
-            return bail(1);
-    }
-    if (launch_attention(e, B, e->stream)) return bail(1);
+    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return bail(fail("attention kernel %d unknown", kernel));
+    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return bail(fail("wgmma attention needs N <= %d", ATTW_KEYS));
+    if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return bail(fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16));
+    if (qkv_lo && kernel != ATT_AUTO && kernel != ATT_WGMMA) return bail(fail("split-precision attention runs in the wgmma kernel"));
+    if (N <= ATTW_KEYS && make_attention_maps(e, T)) return bail(1);
+    if (launch_attention(e, B, e->stream, kernel)) return bail(1);
     if (cudaStreamSynchronize(e->stream) != cudaSuccess) return bail(fail("attention kernel failed: %s", cudaGetErrorString(cudaGetLastError())));
     std::vector<__half> tmp((size_t)T * D);
     if (cudaMemcpy(tmp.data(), e->A16, tmp.size() * 2, cudaMemcpyDeviceToHost) != cudaSuccess) return bail(fail("D2H failed"));
@@ -1646,22 +1441,13 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
             cudaMemcpy(dR, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice);
         }
         const int bn = pick_bn(N);
-        const int cg = (getenv("VITB200_CTA_GROUP") && atoi(getenv("VITB200_CTA_GROUP")) == 1) ? 1 : 2;
-        CUtensorMap tA, tB, tX, tO2;
-        if (make_tmap(&tA, dA, M, K, K, GEMM_BM) || make_tmap(&tB, dW, N, K, K, bn / cg)) break;
-        memset(&tX, 0, sizeof(tX));
-        memset(&tO2, 0, sizeof(tO2));
-        if (f16out && make_tmap(&tX, dO, M, N, N, 32)) break;            // the f16 epilogues store through TMA
-        if (dO2 && make_tmap(&tO2, dO2, M, N, N, 32)) break;
-        if (epilogue == EPI_BIAS_RESID_F32)
-        {
-            // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
-            cudaMemcpy(dO, dR, (size_t)M * N * 4, cudaMemcpyDeviceToDevice);
-            if (make_tmap_f32_box32(&tX, dO, M, N, N)) break;
-        }
+        CUtensorMap tA, tB;
+        if (make_tmap(&tA, dA, M, K, K, GEMM_BM) || make_tmap(&tB, dW, N, K, K, bn)) break;
+        // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
+        if (epilogue == EPI_BIAS_RESID_F32) cudaMemcpy(dO, dR, (size_t)M * N * 4, cudaMemcpyDeviceToDevice);
         GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dO; p.out2 = dO2; p.ldo = N; p.resid = (const float *)dO;
-        if (launch_gemm(nullptr, cg, bn, epilogue, tA, tB, tX, tO2, p, 0, prop.multiProcessorCount)) break;
+        if (launch_gemm(nullptr, bn, epilogue, tA, tB, p, 0)) break;
         cudaError_t err = cudaDeviceSynchronize();
         if (err != cudaSuccess) { fail("GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
         if (f16out)
@@ -1721,7 +1507,7 @@ int vitb200_test_layernorm(int device, int rows, int D, const float *x, const fl
     VB_NOEXCEPT_END((void)0)
 }
 
-// q8_0 linear layer on the integer tensor cores (gemm_q8_tcgen05.cuh; prototype for BASELINE.json configs[4]): x [M][K] f32 is
+// q8_0 linear layer on the integer tensor cores (gemm_q8_wgmma.cuh; prototype for BASELINE.json configs[4]): x [M][K] f32 is
 // quantised on the device exactly as the reference quantises activation rows, w is a q8_0 tensor in the model-file layout
 // ([N][K/32] blocks of {f16 d; int8 q[32]}, ggml-quants.h:42-46).  Outputs: y [M][N] f32, and (optional) the quantised activations
 // xq [M][K] int8, xd [M][K/32] f32.  iters > 0 additionally times `iters` back-to-back GEMM launches (CUDA events) into *ms_per_launch.
@@ -1738,7 +1524,7 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail("device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
     const int KB = K / 32;
     // repack the 34-byte blocks: int8 plane [N][K] + transposed scale plane [K/32][N]
     std::vector<int8_t> wq((size_t)N * K);
@@ -1778,12 +1564,12 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
         const long long qgrid = (n_blocks * 8 + qthreads - 1) / qthreads;
         quantize_q8_0_kernel<<<(unsigned)qgrid, qthreads>>>(dX, dAq, dAd, n_blocks);
         if (cudaGetLastError() != cudaSuccess) { fail("quantize launch failed"); break; }
-        if (cudaFuncSetAttribute(gemm_q8_tcgen05_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Q8_SMEM_BYTES) != cudaSuccess) { fail("cudaFuncSetAttribute failed"); break; }
+        if (cudaFuncSetAttribute(gemm_q8_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Q8_SMEM_BYTES) != cudaSuccess) { fail("cudaFuncSetAttribute failed"); break; }
         Q8GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dY; p.ldo = N;
         const int tiles = ((M + Q8_BM - 1) / Q8_BM) * ((N + Q8_BN - 1) / Q8_BN);
-        const int grid = tiles < prop.multiProcessorCount ? tiles : prop.multiProcessorCount;
-        gemm_q8_tcgen05_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
+        const int grid = tiles;
+        gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
         cudaError_t err = cudaDeviceSynchronize();
         if (err != cudaSuccess) { fail("q8_0 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
         cudaMemcpy(y, dY, (size_t)M * N * 4, cudaMemcpyDeviceToHost);
@@ -1793,7 +1579,7 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
         {
             cudaEventCreate(&e0); cudaEventCreate(&e1);
             cudaEventRecord(e0);
-            for (int i = 0; i < iters; ++i) gemm_q8_tcgen05_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
+            for (int i = 0; i < iters; ++i) gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
             cudaEventRecord(e1);
             err = cudaDeviceSynchronize();
             if (err != cudaSuccess) { fail("q8_0 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }

@@ -111,7 +111,7 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
     ptx::grid_dep_launch(); // PDL: blocks may be resident before the producing GEMM has drained
     ptx::grid_dep_wait();
     const int warps_per_block = blockDim.x >> 5;
-    // rows are taken LAST FIRST: the producing GEMM wrote them in ascending order, so the tail of X is what the 126 MB L2 still
+    // rows are taken LAST FIRST: the producing GEMM wrote them in ascending order, so the tail of X is what the 50 MB L2 still
     // holds when this kernel starts (and the GEMM that follows, walking up from row 0, meets this kernel's freshest output)
     const int row = rows - 1 - (blockIdx.x * warps_per_block + (threadIdx.x >> 5));
     if (row < 0) return;
@@ -305,11 +305,17 @@ __device__ __forceinline__ __half exp_f16_semantics(float x)
 }
 
 // ------------------------------------------------------------------------------------------------
-// Attention for head dim 64.  qkv [T][3D] f16 (q | k | v, head h = columns h*64..), out [T][D] f16.
-// One CTA per (image, head); K and V of that head live in shared memory (XOR-swizzled 16-B chunks);
-// each warp owns 16-query tiles.  Two passes over the keys so the soft-max uses the TRUE row maximum
-// (the f16 rounding of x - max makes online rescaling inexact, SURVEY.md H2): pass 1 = row max of QK^T,
-// pass 2 = P = exp(...), l = sum P, O += P V.  Tensor-core work is mma.sync m16n8k16 (f16 in, f32 acc).
+// Attention for head dim 64.  Replaces the reference's reshape/permute/CONT nodes + mul_mat(K,Q) + scale + soft_max_inplace +
+// mul_mat(V,P) + head merge (reference vit.cpp:826-866; CPU kernels ggml.c:1163-1198 (f32 dot), 10498-10567 (soft-max)).
+// qkv: the head-major buffer the qkv GEMM writes, out [T][D] f16.  One CTA per (image, head); K and V of that head live in shared
+// memory (XOR-swizzled 16-B chunks); each warp owns 16-query tiles.  Two passes over the keys so the soft-max uses the TRUE row maximum (the f16 rounding of x - max makes online rescaling inexact,
+// SURVEY.md H2): pass 1 = row max of QK^T, pass 2 = P = exp(...), l = sum P, O += P V.  Tensor-core work is mma.sync m16n8k16
+// (f16 in, f32 acc).  Used beyond 224 tokens; attention_wgmma.cuh covers N <= 224.
+// Precision of the split-precision attention (attention_wgmma.cuh): the reference feeds F32 q, k, v to both attention mat-muls
+// (vit.cpp:848,858).  The qkv GEMM then leaves every value as TWO f16 numbers, hi = f16(x) and lo = f16(x - hi) (hi + lo carries ~22
+// significant bits), and the tensor cores run
+//   S = Ql Kh^T + Qh Kl^T + Qh Kh^T   (the Ql Kl^T term is below 2^-22 relative)        O = P Vl + P Vh   (P is exactly f16)
+// with f32 accumulation: rounding q, k or v to f16 alone costs ~17 % of the logit-parity budget (DESIGN.md section 4).
 constexpr int ATT_KC = 32; // keys per chunk
 
 __device__ __forceinline__ void att_scores(float (&s)[ATT_KC / 8][4], const uint32_t (&qa)[4][4], uint32_t sK, int kc, int lane)
@@ -339,6 +345,9 @@ attention_kernel(const __half *__restrict__ qkv, size_t plane_rows, __half *__re
 // qkv: the head-major buffer the qkv GEMM writes, [3 H planes][plane_rows][64]: q of head h in plane h, k in H + h, v in 2 H + h
 {
     extern __shared__ __align__(16) uint8_t att_smem[];
+    // launched with programmatic dependent launch: q, k, v are read only once the qkv GEMM has completed
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
     const int b = blockIdx.x / H, h = blockIdx.x - b * H;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint4 *sK4 = reinterpret_cast<uint4 *>(att_smem);

@@ -1,5 +1,5 @@
-// ptx.cuh -- thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences), ldmatrix, mma.sync.
+// ptx.cuh -- thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma, ldmatrix, mma.sync.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -15,21 +15,6 @@ __device__ __forceinline__ uint32_t lane_id()
     uint32_t l;
     asm("mov.u32 %0, %%laneid;" : "=r"(l));
     return l;
-}
-
-// One lane of a converged warp (the same lane every time).  Used instead of `if (lane == 0)` around tcgen05 / TMA issue:
-// the surrounding code then stays warp-uniform, so descriptors live in uniform registers and each UTCHMMA costs one
-// instruction instead of an ELECT / R2UR / BRA.U.ANY loop per operand (ncu: the single-thread form issued ~105 SASS
-// instructions per k-block and capped the tensor pipe at ~73 %).
-__device__ __forceinline__ bool elect_one()
-{
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -62,7 +47,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity)
 // Programmatic dependent launch (PDL): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while
 // its predecessor in the stream is still draining.  grid_dep_launch() lets OUR successor be scheduled as soon as SMs free up;
 // grid_dep_wait() blocks until the predecessor grid has completed and its memory is visible -- everything before it (barrier
-// init, TMEM allocation, descriptor prefetch) overlaps the predecessor's tail.  Both are no-ops for a normally launched kernel.
+// init, descriptor prefetch) overlaps the predecessor's tail.  Both are no-ops for a normally launched kernel.
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // Named barrier among `nthreads` threads of the CTA (id 0 is __syncthreads)
@@ -91,45 +76,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
     {
         if (++spins > (1u << 24)) __trap();
     }
-}
-
-// ---------------------------------------------------------------- thread-block clusters (CTA pairs)
-__device__ __forceinline__ uint32_t cluster_ctarank()
-{
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync()
-{
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  Deliberately WITHOUT
-// .release.cluster: that form compiles to MEMBAR.ALL.GPU + ERRBAR in front of the arrive, which drains every outstanding
-// TMA load of the producer and collapsed the CTA-pair pipeline to depth 1 (ncu: 32 % tensor-pipe, profiles/).  The data these
-// arrivals order is tracked elsewhere (TMA transaction bytes; tcgen05.fence::before_thread_sync for TMEM reads).
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t cta)
-{
-    asm volatile(
-        "{\n\t.reg .b32 r;\n\t"
-        "mapa.shared::cluster.u32 r, %0, %1;\n\t"
-        "mbarrier.arrive.shared::cluster.b64 _, [r];\n\t}"
-        ::"r"(bar), "r"(cta)
-        : "memory");
-}
-
-// Same with release semantics at cluster scope: orders this thread's prior shared-memory writes (made visible to the async
-// proxy by fence.proxy.async) before the arrival is observed in the other CTA.  Costs a GPU-scope MEMBAR: use only off the
-// hot loop (the gathered patch-embedding producer).
-__device__ __forceinline__ void mbar_arrive_remote_release(uint32_t bar, uint32_t cta)
-{
-    asm volatile(
-        "{\n\t.reg .b32 r;\n\t"
-        "mapa.shared::cluster.u32 r, %0, %1;\n\t"
-        "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [r];\n\t}"
-        ::"r"(bar), "r"(cta)
-        : "memory");
 }
 
 // ---------------------------------------------------------------- TMA
@@ -167,15 +113,6 @@ __device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap *m, int c0, in
                  ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2)
                  : "memory");
 }
-// CTA-pair variant: executed by both CTAs of a pair; the data lands in the executing CTA's shared memory, the
-// complete_tx goes to the mbarrier of the pair's leader (even) CTA (peer bit 24 of the shared::cluster address cleared)
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t smem_dst, const CUtensorMap *m, uint32_t bar, int c0, int c1)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-        : "memory");
-}
 // 1-D bulk copies (contiguous bytes, 16-B aligned, size a multiple of 16): global -> shared with mbarrier completion, shared -> global in a
 // bulk async group
 __device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar)
@@ -209,11 +146,6 @@ __device__ __forceinline__ void tma_store_3d(const CUtensorMap *m, uint32_t smem
                  : "memory");
 }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-// acc(f32) += h(f16): one FHADD instead of convert + FADD (PTX mixed-precision add, sm_100+)
-__device__ __forceinline__ void add_f32_f16(float &acc, unsigned short h)
-{
-    asm("add.rn.f32.f16 %0, %1, %0;" : "+f"(acc) : "h"(h));
-}
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void tma_store_wait_read()
@@ -230,7 +162,7 @@ __device__ __forceinline__ void tma_store_wait_group()
 
 // ---------------------------------------------------------------- L2 eviction-priority hints on bulk / tensor copies
 // 64-bit cache policies as produced by createpolicy.fractional.L2::evict_*.b64 with fraction 1.0 (the encodings CUTLASS ships as
-// TMA::CacheHintSm90): streamed-once data (evict_first) should not push reused operands out of the 126 MB L2.
+// TMA::CacheHintSm90): streamed-once data (evict_first) should not push reused operands out of the 50 MB L2.
 constexpr uint64_t L2_EVICT_FIRST = 0x12F0000000000000ull, L2_EVICT_LAST = 0x14F0000000000000ull;
 __device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, uint64_t pol)
 {
@@ -264,150 +196,105 @@ __device__ __forceinline__ void bulk_store_1d_hint(void *gdst, uint32_t smem_src
                  : "memory");
 }
 
-// ---------------------------------------------------------------- tcgen05 / TMEM
-__device__ __forceinline__ void tcgen05_alloc(uint32_t smem_dst, uint32_t ncols)
+// ---------------------------------------------------------------- wgmma (Hopper warpgroup MMA)
+// Shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, 128-B rows (64 f16 or 128 int8 per row), as TMA writes it:
+//   bits [0,14) start address >> 4     bits [16,30) leading byte offset >> 4 (unused for swizzled K-major, 1)
+//   bits [32,46) stride byte offset >> 4 (8 rows * 128 B = 1024)     bits [62,64) layout type: 1 = SWIZZLE_128B
+// A K step of 32 B (16 f16 / 32 int8) inside the swizzle row is +2 in the address field.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(uint32_t smem_addr)
 {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
+    return d;
 }
-__device__ __forceinline__ void tcgen05_relinquish()
+// Same for an MN-major operand (MN contiguous in memory, SWIZZLE_128B), exactly one 64-element MN atom: rows of 128 B are consecutive
+// K indices, 8-row groups (1024 B) tile along K (stride byte offset); the leading byte offset (distance between MN atoms) is unused
+// for a single atom.  A K step of 16 is +2048 B.
+__device__ __forceinline__ uint64_t wgmma_desc_mnmajor_sw128(uint32_t smem_addr)
 {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;
+    return d;
 }
-__device__ __forceinline__ void tcgen05_dealloc(uint32_t taddr, uint32_t ncols)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keep the accumulator registers live and ordered around the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R])
 {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tcgen05_alloc_cg2(uint32_t smem_dst, uint32_t ncols)
-{
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tcgen05_relinquish_cg2()
-{
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tcgen05_dealloc_cg2(uint32_t taddr, uint32_t ncols)
-{
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// CTA-pair commit: arrives on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void tcgen05_commit_cg2(uint32_t bar, uint16_t cta_mask)
-{
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"(cta_mask) : "memory");
-}
-// CTA-pair MMA (M = 256: 128 rows per CTA; B is split along N across the two CTAs); issued by the leader CTA only
-__device__ __forceinline__ void tcgen05_mma_f16_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
+// Re-balance the register file between the producer warpgroup and the MMA warpgroups
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// D(64 x 128, f32, registers) (+)= A(64 x 16, smem desc) * B(128 x 16, smem desc)^T, both K-major f16
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// commit all prior async tcgen05 ops of this thread; arrives once on `bar` when they complete
-__device__ __forceinline__ void tcgen05_commit(uint32_t bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (f16/bf16 inputs, f32 accumulate)
-__device__ __forceinline__ void tcgen05_mma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp gets lane (base_lane + i), r[j] = column j
-__device__ __forceinline__ void tcgen05_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tcgen05_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16])
-{
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-// thread i of the warp writes r[j] to lane (base_lane + i), column (base_col + j)
-__device__ __forceinline__ void tcgen05_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16])
-{
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ void tcgen05_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[8])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-                 : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: A is an M x K f16 matrix held in TMEM, row m on lane m, two f16 per 32-bit
-// column (k = 2*col, 2*col+1) -- cute tmem_frg for M = 128.  A must be K-major.
-__device__ __forceinline__ void tcgen05_mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate)
-{
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 
-// UMMA shared-memory matrix descriptor, K-major operand, SWIZZLE_128B, 64 f16 (=128 B) per row:
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4 (unused for swizzled K-major)
-//   bits [32,46) stride byte offset >> 4 (8 rows * 128 B = 1024)     bits [46,48) version = 1 (sm_100)
-//   bits [61,64) layout type: 2 = SWIZZLE_128B        (cute/arch/mma_sm100_desc.hpp SmemDescriptor)
-__device__ __forceinline__ uint64_t umma_desc_kmajor_sw128(uint32_t smem_addr)
+// D(64 x 256, f32, registers) (+)= A(64 x 16, smem desc) * B(256 x 16, smem desc)^T, both K-major f16
+__device__ __forceinline__ void wgmma_m64n256k16_f16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// Same for an MN-major operand (the MN dimension is contiguous in memory), SWIZZLE_128B, exactly one 64-element MN atom:
-// rows of 128 B are consecutive K indices; 8-row groups (1024 B) tile along K (stride byte offset); the leading byte
-// offset (distance between MN atoms) is irrelevant for a single atom and set to the tile size.
-__device__ __forceinline__ uint64_t umma_desc_mnmajor_sw128(uint32_t smem_addr, uint32_t lbo_bytes)
+
+// D(64 x 224, f32, registers) (+)= A(64 x 16, smem desc) * B(224 x 16, smem desc)^T, both K-major f16
+__device__ __forceinline__ void wgmma_m64n224k16_f16(float (&d)[112], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
 {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %114, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n224k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111}, %112, %113, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// UMMA instruction descriptor for kind::f16: c_format F32 (bit 4), a/b format (0 = f16, 1 = bf16) at bits 7 / 10,
-// a_major / b_major (0 = K-major, 1 = MN-major) at bits 15 / 16, N >> 3 at bits [17,23), M >> 4 at bits [24,29).
-__host__ __device__ constexpr inline uint32_t umma_idesc_f16(int M, int N, int a_fmt, int b_fmt, int a_mn_major = 0, int b_mn_major = 0)
+
+// D(64 x 64, f32, registers) (+)= A(64 x 16, f16 registers: the m16n8k16 A fragment of each warp) * B(16 x 64, smem desc, MN-major f16)
+__device__ __forceinline__ void wgmma_m64n64k16_f16_rs_tb(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc, uint32_t accumulate)
 {
-    return (1u << 4) | ((uint32_t)a_fmt << 7) | ((uint32_t)b_fmt << 10) | ((uint32_t)a_mn_major << 15) |
-           ((uint32_t)b_mn_major << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(accumulate));
+}
+
+// D(64 x 128, s32, registers) = A(64 x 32, smem desc) * B(128 x 32, smem desc)^T, both K-major s8 (fresh accumulator)
+__device__ __forceinline__ void wgmma_m64n128k32_s8(uint32_t (&d)[64], uint64_t adesc, uint64_t bdesc)
+{
+    asm volatile(
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, 0;"
+        : "=r"(d[0]), "=r"(d[1]), "=r"(d[2]), "=r"(d[3]), "=r"(d[4]), "=r"(d[5]), "=r"(d[6]), "=r"(d[7]), "=r"(d[8]), "=r"(d[9]), "=r"(d[10]), "=r"(d[11]), "=r"(d[12]), "=r"(d[13]), "=r"(d[14]), "=r"(d[15]), "=r"(d[16]), "=r"(d[17]), "=r"(d[18]), "=r"(d[19]), "=r"(d[20]), "=r"(d[21]), "=r"(d[22]), "=r"(d[23]), "=r"(d[24]), "=r"(d[25]), "=r"(d[26]), "=r"(d[27]), "=r"(d[28]), "=r"(d[29]), "=r"(d[30]), "=r"(d[31]), "=r"(d[32]), "=r"(d[33]), "=r"(d[34]), "=r"(d[35]), "=r"(d[36]), "=r"(d[37]), "=r"(d[38]), "=r"(d[39]), "=r"(d[40]), "=r"(d[41]), "=r"(d[42]), "=r"(d[43]), "=r"(d[44]), "=r"(d[45]), "=r"(d[46]), "=r"(d[47]), "=r"(d[48]), "=r"(d[49]), "=r"(d[50]), "=r"(d[51]), "=r"(d[52]), "=r"(d[53]), "=r"(d[54]), "=r"(d[55]), "=r"(d[56]), "=r"(d[57]), "=r"(d[58]), "=r"(d[59]), "=r"(d[60]), "=r"(d[61]), "=r"(d[62]), "=r"(d[63])
+        : "l"(adesc), "l"(bdesc));
 }
 
 // ---------------------------------------------------------------- fast math
@@ -423,35 +310,6 @@ __device__ __forceinline__ float rcp_approx(float x)
     float y;
     asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
-}
-
-// ---------------------------------------------------------------- packed FP32 (Blackwell FFMA2 / FMUL2 / FADD2)
-// Two independent IEEE-rounded f32 operations per instruction on a 64-bit register pair: same results as two scalar ops, one
-// issue slot (tools/microbench/chain_r02.cu: the packed forms issue every 2 clocks, i.e. they save issue bandwidth, not FLOPs).
-__device__ __forceinline__ uint64_t pack_f32x2(float a, float b)
-{
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-    return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float &a, float &b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c)
-{
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b)
-{
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b)
-{
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
 }
 
 // ---------------------------------------------------------------- warp-level MMA (attention)

@@ -5,7 +5,7 @@ Names and argument meaning follow the reference (vit.h:118-122) so tests read li
     model = vit_model_load(path)                      # reference vit.cpp:308  (here: parse + upload to the GPU)
     probs, idx, val = vit_predict(model, images)      # reference vit.cpp:1004 (here: batched, on the GPU)
 
-There is NO CPU fallback: if libvitb200.so is missing or no B200 is present these functions raise.
+There is NO CPU fallback: if libvitb200.so is missing or no H100 (sm_90) is present these functions raise.
 """
 from __future__ import annotations
 
@@ -283,7 +283,9 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
     return probs, logits, out
 
 
-ATTN_AUTO, ATTN_MMA, ATTN_TC, ATTN_TC_LONG = 0, 1, 2, 3
+# attention kernels of vitb200_test_attention (include/vitb200.h): engine's choice, mma.sync with 8 warps (any N), wgmma (N <= 224,
+# the split-precision kernel), mma.sync with 16 warps (128 < N <= 640)
+ATTN_AUTO, ATTN_MMA8, ATTN_WGMMA, ATTN_MMA16 = 0, 1, 2, 3
 
 
 def test_attention(qkv16: np.ndarray, B: int, N: int, H: int, kernel: int = ATTN_AUTO, device: int = 0) -> np.ndarray:
@@ -303,7 +305,7 @@ def split_hi_lo(x: np.ndarray):
 
 
 def test_attention_hilo(qkv32: np.ndarray, B: int, N: int, H: int, device: int = 0) -> np.ndarray:
-    """The tcgen05 attention kernel (N <= 224) on split-precision operands: qkv32 float32 [B*N, 3*H*64] is passed as hi + lo."""
+    """The wgmma attention kernel (N <= 224) on split-precision operands: qkv32 float32 [B*N, 3*H*64] is passed as hi + lo."""
     hi, lo = split_hi_lo(np.asarray(qkv32, np.float32).reshape(B * N, 3 * H * 64))
     out = np.empty((B * N, H * 64), np.float32)
     _check(lib().vitb200_test_attention_hilo(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
