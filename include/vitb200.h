@@ -133,7 +133,34 @@ int vitb200_forward_u8_async(vitb200_engine *e, const uint8_t *const *images, co
 int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, float *d_probs, float *d_logits,
                            int32_t *d_topk_idx, float *d_topk_prob, int k, void *stream);
 
-/* Number of kernels this library launched during the most recent forward call. */
+/* ---- encoder features (no reference counterpart: the reference only returns classifier outputs) -----------------------------
+ * The encoder's own outputs instead of the classifier's: every token of the residual stream after any block (a multimodal model's
+ * vision tower), and the pooled pre-logits rows the classifier head reads (retrieval, deduplication, linear probes). */
+typedef struct vitb200_features_req
+{
+    int32_t layers; /* encoder blocks to run, 0..num_hidden_layers.  0 = the embeddings (patch GEMM + conv bias + cls + pos_embed,
+                     * reference vit.cpp:772-797); num_hidden_layers = the whole encoder (vit.cpp:802-901).  Blocks past `layers`
+                     * are not launched. */
+    int32_t norm;   /* 1: apply the model's final LayerNorm (norm.weight / norm.bias, vit.cpp:915-919) to every emitted row;
+                     * 0: the residual stream as it stands after `layers` blocks */
+    int32_t dtype;  /* 0 f32, 1 f16, 2 bf16 -- the 16-bit forms are the f32 result rounded to nearest even */
+} vitb200_features_req;
+
+/* tokens:    [batch][N][D], every token, cls first (N = (img/patch)^2 + 1); may be NULL
+ * prelogits: [batch][head_tokens][D], the rows the classifier head reads (token 0, vit.cpp:910; the first 25 for ViTSTR,
+ *            vitstr.cpp:864-883); may be NULL.  At layers == num_hidden_layers with norm == 1 this is the head's input before
+ *            its f16 rounding.  At least one of the two must be non-NULL.
+ * vitb200_features: HOST buffers, blocking, like vitb200_forward (images as there).
+ * vitb200_features_device: DEVICE buffers (16-byte aligned) enqueued on `stream` without synchronising, like vitb200_forward_device.
+ * vitb200_features_u8: u8 RGB images pre-processed on the GPU, like vitb200_forward_u8 (RGB models only); host outputs, blocking.
+ * Small batches replay a cached CUDA graph per argument set, as the classification calls do. */
+int vitb200_features(vitb200_engine *e, const float *images, int batch, const vitb200_features_req *req, void *tokens, void *prelogits);
+int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch, const vitb200_features_req *req, void *d_tokens,
+                            void *d_prelogits, void *stream);
+int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                        const vitb200_features_req *req, void *tokens, void *prelogits);
+
+/* Number of kernels this library launched during the most recent forward or features call. */
 int vitb200_last_launch_count(const vitb200_engine *e);
 
 /* Per-kernel device timing for roofline reporting: while enabled, CUDA-event pairs are recorded around every

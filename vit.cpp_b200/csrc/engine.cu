@@ -133,6 +133,18 @@ struct Layer
 
 int pick_bn(int n_out) { return n_out >= 256 ? 256 : 128; }
 
+// Argument set of one cached CUDA graph: a classification forward (layers = -1) or an encoder-features call
+struct GraphKey
+{
+    const void *img; int batch; void *probs, *logits, *tidx, *tval; int k;
+    int layers, norm, dtype; void *tok, *pre;
+    bool operator==(const GraphKey &o) const
+    {
+        return img == o.img && batch == o.batch && probs == o.probs && logits == o.logits && tidx == o.tidx && tval == o.tval && k == o.k &&
+               layers == o.layers && norm == o.norm && dtype == o.dtype && tok == o.tok && pre == o.pre;
+    }
+};
+
 } // namespace
 
 struct vitb200_engine
@@ -176,7 +188,7 @@ struct vitb200_engine
     uint8_t *h_u8[2] = {nullptr, nullptr}, *d_u8[2] = {nullptr, nullptr};
     size_t u8_cap[2] = {0, 0};
     // CUDA-graph cache for the kernel schedule of one forward, keyed by its arguments (launch-bound inner loop: ~90 kernels)
-    struct GraphEntry { const void *img; int batch; void *probs, *logits, *tidx, *tval; int k; int state; int launches; cudaGraphExec_t exec; };
+    struct GraphEntry { GraphKey key; int state; int launches; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
     bool use_graph = true;
     // optional per-kernel timing (bench.py roofline): CUDA event pairs around tracked launches
@@ -508,6 +520,25 @@ int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaS
     return 0;
 }
 
+// The row-per-warp kernel: the LayerNorms the bulk-copy kernel below does not take (pooled rows, hidden sizes that are not a multiple
+// of 128) and, with an f32 / bf16 output or NORM = false, the encoder features.  rows_per_group <= 0: all rows are one group.
+template <typename OutT, bool NORM>
+int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
+                          cudaStream_t s, int rows_per_group, size_t group_stride)
+{
+    const int D = e->hp.hidden_size;
+    if (rows_per_group <= 0) rows_per_group = rows > 0 ? rows : 1; // one group: plain consecutive rows
+    const int threads = 256, rows_per_block = threads / 32;
+    const int blocks = (rows + rows_per_block - 1) / rows_per_block;
+    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
+    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
+    else if (D <= 16 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<16, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
+    else return fail("hidden size %d not supported (max 2048)", D);
+    CUDA_TRY(cudaGetLastError());
+    e->launches++;
+    return 0;
+}
+
 int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, __half *y, int rows, cudaStream_t s,
                      int rows_per_group = 0, size_t group_stride = 0)
 {
@@ -548,16 +579,7 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
         e->launches++;
         return 0;
     }
-    if (rows_per_group <= 0) rows_per_group = rows > 0 ? rows : 1; // one group: plain consecutive rows
-    const int threads = 256, rows_per_block = threads / 32;
-    const int blocks = (rows + rows_per_block - 1) / rows_per_block;
-    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
-    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
-    else if (D <= 16 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<16>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
-    else return fail("hidden size %d not supported (max 2048)", D);
-    CUDA_TRY(cudaGetLastError());
-    e->launches++;
-    return 0;
+    return launch_layernorm_rows<__half, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride);
 }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
@@ -666,14 +688,11 @@ int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
     return 0;
 }
 
-// The fixed kernel schedule == reference vit_encode_image (vit.cpp:718-941), batched over images.
-int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
-                float *d_topk_val, int k, cudaStream_t s, const vitb200_taps *taps)
+// The encoder part of the fixed kernel schedule: embeddings (vit.cpp:772-797), then blocks 0 .. layers-1 (vit.cpp:802-901); afterwards
+// the residual stream X holds the encoder's output at that depth.  Resets the launch count.
+int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cudaStream_t s, const vitb200_taps *taps)
 {
-    if (B < 1 || B > e->max_batch) return fail("batch %d out of range (1..%d)", B, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
-    if (!d_images && taps) return fail("debug taps need the f32 image path");
-    const int D = e->hp.hidden_size, N = e->N, T = B * N, C = e->hp.num_classes;
+    const int D = e->hp.hidden_size, N = e->N, T = B * N;
     e->launches = 0;
     __half *PA = e->PA;
     // patch embedding (vit.cpp:772-797): the f16 patch matrix PA (im2col of a stride == kernel conv is a pure permutation,
@@ -696,8 +715,7 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     }
     if (taps && tap_f32(taps->embed, e->X, (size_t)T * D, s)) return 1;
 
-    const int n_layers = e->hp.num_hidden_layers;
-    for (int il = 0; il < n_layers; ++il)
+    for (int il = 0; il < layers; ++il)
     {
         const Layer &L = e->layers[il];
         const bool tap = taps && taps->layer == il;
@@ -745,11 +763,11 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
-            // fc2 + residual (vit.cpp:896-900); fused: + LayerNorm 1 of the NEXT block (the last block's output goes to the pooled
-            // final LayerNorm instead)
+            // fc2 + residual (vit.cpp:896-900); fused: + LayerNorm 1 of the NEXT block (the last block run has no next block: its
+            // output goes to the pooled final LayerNorm or to the encoder features instead)
             GemmParams p{};
             p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X;
-            if (e->fused_ln && il + 1 < n_layers)
+            if (e->fused_ln && il + 1 < layers)
             {
                 const Layer &Ln = e->layers[il + 1];
                 p.ln_out = e->A16; p.ln_w = Ln.n1w; p.ln_b = Ln.n1b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps;
@@ -760,6 +778,18 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
         if (e->fused_ln && taps && taps->layer == il + 1 && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1; // norm1 of the next block
     }
+    return 0;
+}
+
+// The fixed kernel schedule == reference vit_encode_image (vit.cpp:718-941), batched over images.
+int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
+                float *d_topk_val, int k, cudaStream_t s, const vitb200_taps *taps)
+{
+    if (B < 1 || B > e->max_batch) return fail("batch %d out of range (1..%d)", B, e->max_batch);
+    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
+    if (!d_images && taps) return fail("debug taps need the f32 image path");
+    const int D = e->hp.hidden_size, N = e->N, T = B * N, C = e->hp.num_classes;
+    if (run_encoder(e, d_images, B, e->hp.num_hidden_layers, s, taps)) return 1;
     if (taps && tap_f32(taps->x_final, e->X, (size_t)T * D, s)) return 1;
 
     // pool (token 0; the first 25 tokens for ViTSTR, vitstr.cpp:864-883) + final LN + head + soft-max + top-k
@@ -790,26 +820,58 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     return 0;
 }
 
-// run_forward through a cached CUDA graph: the first call with a given argument set runs eagerly (also sets the kernels'
-// function attributes), the second captures + instantiates, later ones replay.  Profiling / taps always run eagerly.
-int run_forward_graphed(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
-                        float *d_topk_val, int k, cudaStream_t s)
+// Encoder features (vitb200_features*): the encoder up to block req->layers, then the requested rows of the residual stream -- all T
+// token rows into d_tokens, the head_tokens pooled rows of every image into d_prelogits -- normalised with the final LayerNorm or not,
+// as f32 / f16 / bf16.  Device destinations; either may be NULL.  An un-normalised f32 output is a copy, every other one a kernel.
+int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_features_req *req, void *d_tokens, void *d_prelogits, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size, N = e->N, TH = e->head_tokens;
+    if (run_encoder(e, d_images, B, req->layers, s, nullptr)) return 1;
+    auto emit = [&](void *dst, int rows, int rows_per_group) -> int {
+        if (!dst) return 0;
+        if (!req->norm && req->dtype == 0)
+        {
+            // [B][rows_per_group][D] out of [B][N][D]: one 2-D copy (the token rows are a single plain copy)
+            const size_t w = (size_t)rows_per_group * D * sizeof(float);
+            CUDA_TRY(cudaMemcpy2DAsync(dst, w, e->X, (size_t)N * D * sizeof(float), w, (size_t)rows / rows_per_group, cudaMemcpyDeviceToDevice, s));
+            return 0;
+        }
+        ProfScope ps(e, PK_LN, 0.0, s);
+        const size_t gs = (size_t)N * D;
+        switch (req->dtype * 2 + (req->norm ? 1 : 0))
+        {
+        case 1: return launch_layernorm_rows<float, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (float *)dst, rows, s, rows_per_group, gs);
+        case 2: return launch_layernorm_rows<__half, false>(e, e->X, (size_t)D, nullptr, nullptr, (__half *)dst, rows, s, rows_per_group, gs);
+        case 3: return launch_layernorm_rows<__half, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__half *)dst, rows, s, rows_per_group, gs);
+        case 4: return launch_layernorm_rows<__nv_bfloat16, false>(e, e->X, (size_t)D, nullptr, nullptr, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
+        case 5: return launch_layernorm_rows<__nv_bfloat16, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
+        }
+        return fail("features: dtype %d unknown", req->dtype);
+    };
+    if (emit(d_tokens, B * N, N)) return 1;
+    return emit(d_prelogits, B * TH, TH);
+}
+
+// `run` (one kernel schedule, no taps) through a cached CUDA graph: the first call with a given argument set runs eagerly (also sets
+// the kernels' function attributes), the second captures + instantiates, later ones replay.  Profiling always runs eagerly.
+template <typename Run>
+int run_graphed(vitb200_engine *e, const GraphKey &key, cudaStream_t s, Run run)
 {
     // Graph replay pays off where the ~90 launches are a visible fraction of the step (small batches); at B = 256 every kernel
     // runs >= 80 us and eager launches stay ahead of the GPU (measured: no gain), so large batches launch eagerly.
-    if (!e->use_graph || e->profile || (long long)B * e->N > 8192) return run_forward(e, d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, s, nullptr);
+    if (!e->use_graph || e->profile || (long long)key.batch * e->N > 8192) return run();
     vitb200_engine::GraphEntry *g = nullptr;
     for (auto &x : e->graphs)
-        if (x.img == d_images && x.batch == B && x.probs == d_probs && x.logits == d_logits && x.tidx == d_topk_idx && x.tval == d_topk_val && x.k == k) { g = &x; break; }
+        if (x.key == key) { g = &x; break; }
     if (!g)
     {
         if (e->graphs.size() >= 16) { if (e->graphs.front().exec) cudaGraphExecDestroy(e->graphs.front().exec); e->graphs.erase(e->graphs.begin()); }
-        e->graphs.push_back({d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, 0, 0, nullptr});
+        e->graphs.push_back({key, 0, 0, nullptr});
         g = &e->graphs.back();
     }
     if (g->state == 0)
     {
-        if (run_forward(e, d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, s, nullptr)) return 1;
+        if (run()) return 1;
         g->state = 1;
         g->launches = e->launches;
         return 0;
@@ -818,7 +880,7 @@ int run_forward_graphed(vitb200_engine *e, const float *d_images, int B, float *
     {
         cudaGraph_t graph = nullptr;
         CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
-        const int rc = run_forward(e, d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, s, nullptr);
+        const int rc = run();
         cudaError_t ce = cudaStreamEndCapture(s, &graph);
         if (rc != 0 || ce != cudaSuccess || !graph)
         {
@@ -826,7 +888,7 @@ int run_forward_graphed(vitb200_engine *e, const float *d_images, int B, float *
             (void)cudaGetLastError();
             g->state = 0;
             e->use_graph = false; // fall back to eager launches (same kernels, same results)
-            return run_forward(e, d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, s, nullptr);
+            return run();
         }
         g->launches = e->launches;
         ce = cudaGraphInstantiate(&g->exec, graph, 0);
@@ -838,6 +900,35 @@ int run_forward_graphed(vitb200_engine *e, const float *d_images, int B, float *
     e->launches = g->launches;
     return 0;
 }
+
+int run_forward_graphed(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
+                        float *d_topk_val, int k, cudaStream_t s)
+{
+    const GraphKey key{d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, -1, 0, 0, nullptr, nullptr};
+    return run_graphed(e, key, s, [&] { return run_forward(e, d_images, B, d_probs, d_logits, d_topk_idx, d_topk_val, k, s, nullptr); });
+}
+
+int run_features_graphed(vitb200_engine *e, const float *d_images, int B, const vitb200_features_req *req, void *d_tokens, void *d_prelogits,
+                         cudaStream_t s)
+{
+    const GraphKey key{d_images, B, nullptr, nullptr, nullptr, nullptr, 0, req->layers, req->norm, req->dtype, d_tokens, d_prelogits};
+    return run_graphed(e, key, s, [&] { return run_features(e, d_images, B, req, d_tokens, d_prelogits, s); });
+}
+
+// Argument checks of the three vitb200_features entry points, before anything is enqueued
+int check_features(const vitb200_engine *e, const void *images, int batch, const vitb200_features_req *req, const void *tokens, const void *prelogits)
+{
+    if (!e || !images || !req) return fail("vitb200_features: null argument");
+    if (req->layers < 0 || req->layers > e->hp.num_hidden_layers)
+        return fail("vitb200_features: layers %d out of range (0..%d)", req->layers, e->hp.num_hidden_layers);
+    if (req->norm != 0 && req->norm != 1) return fail("vitb200_features: norm must be 0 or 1 (got %d)", req->norm);
+    if (req->dtype < 0 || req->dtype > 2) return fail("vitb200_features: dtype %d unknown (0 f32, 1 f16, 2 bf16)", req->dtype);
+    if (!tokens && !prelogits) return fail("vitb200_features: both outputs are NULL");
+    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
+    return 0;
+}
+
+size_t features_elem_bytes(const vitb200_features_req *req) { return req->dtype == 0 ? 4 : 2; }
 
 } // namespace
 
@@ -1169,6 +1260,50 @@ int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, 
     return run_forward_graphed(e, d_images, batch, d_probs, d_logits, d_topk_idx, d_topk_prob, k, s);
 }
 
+int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch, const vitb200_features_req *req, void *d_tokens,
+                            void *d_prelogits, void *stream)
+{
+    if (check_features(e, d_images, batch, req, d_tokens, d_prelogits)) return 1;
+    if (((uintptr_t)d_tokens | (uintptr_t)d_prelogits) % 16 != 0) return fail("vitb200_features_device: output buffers must be 16-byte aligned");
+    CUDA_TRY(cudaSetDevice(e->device));
+    return run_features_graphed(e, d_images, batch, req, d_tokens, d_prelogits, stream ? (cudaStream_t)stream : e->stream);
+}
+
+// Host images -> this call's input slot (slot = call parity) on the copy stream, once the slot's previous call has consumed it; the
+// compute stream waits for the copy.  The caller records ev_done[sl] on the compute stream after its last use of the slot.
+static int stage_images(vitb200_engine *e, const float *images, int batch, int &sl)
+{
+    sl = (int)(e->submits & 1);
+    cudaStream_t cs = e->copy_stream;
+    const size_t img_elems = (size_t)e->C * e->hp.img_size * e->hp.img_size;
+    if (e->submits >= 2) CUDA_TRY(cudaStreamWaitEvent(cs, e->ev_done[sl], 0)); // slot's previous forward has consumed its inputs/outputs
+    CUDA_TRY(cudaMemcpyAsync(e->d_img_slot[sl], images, (size_t)batch * img_elems * sizeof(float), cudaMemcpyHostToDevice, cs));
+    CUDA_TRY(cudaEventRecord(e->ev_h2d[sl], cs));
+    CUDA_TRY(cudaStreamWaitEvent(e->stream, e->ev_h2d[sl], 0));
+    return 0;
+}
+
+// Encoder features to HOST buffers, enqueued on the compute stream: kernel outputs are staged in H16 (the MLP hidden buffer, dead
+// after the last block's fc2: T x 4D f16 holds T x D f32 tokens plus the pooled f32 rows), then copied back; an un-normalised f32
+// output is copied straight out of the residual stream.
+static int features_to_host(vitb200_engine *e, const float *d_images, int batch, const vitb200_features_req *req, void *tokens, void *prelogits)
+{
+    const size_t D = e->hp.hidden_size, N = e->N, TH = e->head_tokens, esz = features_elem_bytes(req);
+    const size_t tok_bytes = (size_t)batch * N * D * esz, pre_bytes = (size_t)batch * TH * D * esz;
+    cudaStream_t s = e->stream;
+    const bool copy = !req->norm && req->dtype == 0;
+    uint8_t *stage = reinterpret_cast<uint8_t *>(e->H16);
+    void *d_tok = tokens && !copy ? stage : nullptr;
+    void *d_pre = prelogits && !copy ? stage + tok_bytes : nullptr;
+    if (run_features_graphed(e, d_images, batch, req, d_tok, d_pre, s)) return 1;
+    if (tokens) CUDA_TRY(cudaMemcpyAsync(tokens, copy ? (const void *)e->X : d_tok, tok_bytes, cudaMemcpyDeviceToHost, s));
+    if (prelogits && copy)
+        CUDA_TRY(cudaMemcpy2DAsync(prelogits, TH * D * 4, e->X, N * D * 4, TH * D * 4, (size_t)batch, cudaMemcpyDeviceToHost, s));
+    else if (prelogits)
+        CUDA_TRY(cudaMemcpyAsync(prelogits, d_pre, pre_bytes, cudaMemcpyDeviceToHost, s));
+    return 0;
+}
+
 // Enqueue one batched forward with HOST buffers.  Slot s = call parity: the H2D of this call runs on the copy stream and
 // may overlap the kernels of the previous call (other slot); kernels + D2H run on the compute stream in call order.
 static int forward_enqueue(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
@@ -1178,15 +1313,11 @@ static int forward_enqueue(vitb200_engine *e, const float *images, int batch, fl
     if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
     if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k); // before anything is enqueued
     CUDA_TRY(cudaSetDevice(e->device));
-    const int sl = (int)(e->submits & 1);
-    cudaStream_t s = e->stream, cs = e->copy_stream;
-    const size_t img_elems = (size_t)e->C * e->hp.img_size * e->hp.img_size;
+    int sl = 0;
+    if (stage_images(e, images, batch, sl)) return 1;
+    cudaStream_t s = e->stream;
     const size_t rows = (size_t)batch * e->head_tokens; // classifier rows returned
     const int C = e->hp.num_classes;
-    if (e->submits >= 2) CUDA_TRY(cudaStreamWaitEvent(cs, e->ev_done[sl], 0)); // slot's previous forward has consumed its inputs/outputs
-    CUDA_TRY(cudaMemcpyAsync(e->d_img_slot[sl], images, (size_t)batch * img_elems * sizeof(float), cudaMemcpyHostToDevice, cs));
-    CUDA_TRY(cudaEventRecord(e->ev_h2d[sl], cs));
-    CUDA_TRY(cudaStreamWaitEvent(s, e->ev_h2d[sl], 0));
     const bool want_topk = k > 0 && (topk_idx || topk_prob);
     float *dp = (probs || want_topk) ? e->d_probs_slot[sl] : nullptr;
     int32_t *di = want_topk ? e->d_topk_idx_slot[sl] : nullptr;
@@ -1314,19 +1445,28 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
     return forward_host(e, images, batch, probs, logits, nullptr, nullptr, 0, taps);
 }
 
+int vitb200_features(vitb200_engine *e, const float *images, int batch, const vitb200_features_req *req, void *tokens, void *prelogits)
+{
+    if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
+    CUDA_TRY(cudaSetDevice(e->device));
+    int sl = 0;
+    if (stage_images(e, images, batch, sl) || features_to_host(e, e->d_img_slot[sl], batch, req, tokens, prelogits)) return 1;
+    CUDA_TRY(cudaEventRecord(e->ev_done[sl], e->stream));
+    e->submits++;
+    return vitb200_sync(e);
+}
+
 // vit_image_preprocess (reference vit.cpp:289-305) for a batch of u8 RGB images of arbitrary sizes, on the GPU, followed by the
 // forward pass: the "images" of vitb200_forward never exist on the host, and (unless images_f32_out asks for them) not in HBM
 // either -- the preprocess kernel writes the f16 patch matrix the patch-embedding GEMM reads.  Pipelined like
 // vitb200_forward_async: the caller's images are packed into this slot's pinned staging buffer, ONE host-to-device copy on the copy
 // stream overlaps the previous call's kernels, nothing synchronises on entry and nothing is allocated once the staging buffers
 // have grown to the largest batch seen.
-static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
-                              float *images_f32_out, float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k)
+// preprocess_u8 is the part up to the patch matrix (and the optional f32 read-back); the caller records ev_done[sl] after its last
+// use of the slot.
+static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                         float *images_f32_out, int &sl)
 {
-    if (!e || !images || !nx || !ny) return fail("null argument");
-    if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
     size_t total = 0;
     for (int b = 0; b < batch; ++b)
     {
@@ -1336,7 +1476,7 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
     const size_t table_off = total;
     total += (size_t)batch * sizeof(PreImage);
     CUDA_TRY(cudaSetDevice(e->device));
-    const int sl = (int)(e->submits & 1);
+    sl = (int)(e->submits & 1);
     cudaStream_t s = e->stream, cs = e->copy_stream;
     // this slot's previous call (two submissions ago) must have consumed its staging buffer before the host overwrites it
     if (e->submits >= 2) CUDA_TRY(cudaEventSynchronize(e->ev_done[sl]));
@@ -1370,6 +1510,19 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
     CUDA_TRY(cudaGetLastError());
     const size_t img_elems = (size_t)3 * S * S;
     if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * img_elems * sizeof(float), cudaMemcpyDeviceToHost, s));
+    return 0;
+}
+
+static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                              float *images_f32_out, float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k)
+{
+    if (!e || !images || !nx || !ny) return fail("null argument");
+    if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
+    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
+    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
+    int sl = 0;
+    if (preprocess_u8(e, images, nx, ny, batch, bilinear, images_f32_out, sl)) return 1;
+    cudaStream_t s = e->stream;
     const bool want_topk = k > 0 && (topk_idx || topk_prob);
     const int C = e->hp.num_classes;
     if (probs || logits || want_topk)
@@ -1403,6 +1556,22 @@ int vitb200_forward_u8(vitb200_engine *e, const uint8_t *const *images, const in
 {
     VB_NOEXCEPT_BEGIN
     if (forward_u8_enqueue(e, images, nx, ny, batch, bilinear, images_f32_out, probs, logits, topk_idx, topk_prob, k)) return 1;
+    return vitb200_sync(e);
+    VB_NOEXCEPT_END((void)0)
+}
+
+int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                        const vitb200_features_req *req, void *tokens, void *prelogits)
+{
+    if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
+    if (!nx || !ny) return fail("vitb200_features_u8: null argument");
+    if (e->C != 3) return fail("vitb200_features_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
+    VB_NOEXCEPT_BEGIN
+    int sl = 0;
+    if (preprocess_u8(e, images, nx, ny, batch, bilinear, nullptr, sl) || features_to_host(e, nullptr, batch, req, tokens, prelogits)) return 1;
+    e->launches += 1; // the preprocess kernel
+    CUDA_TRY(cudaEventRecord(e->ev_done[sl], e->stream));
+    e->submits++;
     return vitb200_sync(e);
     VB_NOEXCEPT_END((void)0)
 }

@@ -2,12 +2,16 @@
 //   patchify_f16_kernel      reference im2col for stride==kernel conv (ggml.c:11528-11608) without the buffer
 //                            reshuffle: pixels HWC f32 -> f16 patch rows, K order c*P*P + ky*P + kx
 //   cls_rows_kernel          token 0 = cls_token + pos_embed[0]                      (vit.cpp:794-797)
-//   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand
+//   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
+//                            and un-normalised forms write the encoder features (vitb200_features)
 //   attention_kernel         per (image, head): S = QK^T / sqrt(hd), softmax with the reference's f16-exp
 //                            semantics (ggml.c:10536-10558), O = P V   (vit.cpp:826-866)
 //   softmax_topk_kernel      final soft-max (vit.cpp:931) + top-k (replaces the host std::sort, vit.cpp:1047-1057)
 #pragma once
 #include "ptx.cuh"
+
+#include <cuda_bf16.h>
+#include <type_traits>
 
 namespace vitb200 {
 
@@ -100,12 +104,49 @@ __global__ void cls_rows_kernel(float *__restrict__ x, const float *__restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
+// Four f32 results -> OutT, stored at float4 index i of a row.  16-bit outputs pair up neighbouring lanes (lanes 2k and 2k+1 hold
+// consecutive float4 indices) so that the even lane issues one 16-byte store for both; `vec16` requires an even float4 count per row.
+// Every lane of the warp must call this (shuffles), `live` says whether its own index is inside the row.
+template <typename OutT>
+__device__ __forceinline__ void store4(OutT *__restrict__ yr, int i, bool live, bool vec16, float o0, float o1, float o2, float o3)
+{
+    if constexpr (sizeof(OutT) == 4)
+    {
+        if (live) reinterpret_cast<float4 *>(yr)[i] = make_float4(o0, o1, o2, o3);
+    }
+    else
+    {
+        uint2 u;
+        if constexpr (std::is_same<OutT, __half>::value)
+        {
+            const __half2 h0 = __floats2half2_rn(o0, o1), h1 = __floats2half2_rn(o2, o3);
+            u.x = *reinterpret_cast<const uint32_t *>(&h0);
+            u.y = *reinterpret_cast<const uint32_t *>(&h1);
+        }
+        else
+        {
+            const __nv_bfloat162 h0 = __floats2bfloat162_rn(o0, o1), h1 = __floats2bfloat162_rn(o2, o3);
+            u.x = *reinterpret_cast<const uint32_t *>(&h0);
+            u.y = *reinterpret_cast<const uint32_t *>(&h1);
+        }
+        if (vec16)
+        {
+            const uint32_t nx = __shfl_xor_sync(0xffffffffu, u.x, 1), ny = __shfl_xor_sync(0xffffffffu, u.y, 1);
+            if (live && !(threadIdx.x & 1)) reinterpret_cast<uint4 *>(yr)[i >> 1] = make_uint4(u.x, u.y, nx, ny);
+        }
+        else if (live)
+            reinterpret_cast<uint2 *>(yr)[i] = u;
+    }
+}
+
 // One warp per row.  mean / biased variance in f32 (the reference sums in double; the difference is
 // ~1e-7 relative), then y = ((x-mean)*scale)*w + b as three separately rounded f32 ops like the
 // reference's NORM, MUL, ADD nodes, then RNE to f16 (the GEMM's src1 conversion, ggml.c:9493-9506).
-template <int MAXV>
+// OutT = float stores those f32 values before that rounding, __nv_bfloat16 rounds them to nearest even bf16 instead.
+// NORM = false skips the normalisation: the selected rows of x are converted and stored as they are (w and b are not read).
+template <int MAXV, typename OutT = __half, bool NORM = true>
 __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_stride, int rows_per_group, size_t group_stride,
-                                     const float *__restrict__ w, const float *__restrict__ b, __half *__restrict__ y, int rows,
+                                     const float *__restrict__ w, const float *__restrict__ b, OutT *__restrict__ y, int rows,
                                      int D, float eps)
 {
     ptx::grid_dep_launch(); // PDL: blocks may be resident before the producing GEMM has drained
@@ -133,44 +174,53 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
             sum += (v[j].x + v[j].y) + (v[j].z + v[j].w);
         }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum / (float)D;
-    float sq = 0.f;
-#pragma unroll
-    for (int j = 0; j < MAXV; ++j)
+    float scale = 1.f;
+    if constexpr (NORM)
     {
-        const int i = lane + 32 * j;
-        if (i < nvec)
-        {
-            v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
-            sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
-        }
-    }
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float var = sq / (float)D;
-    const float scale = 1.0f / sqrtf(var + eps);
+        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        const float mean = sum / (float)D;
+        float sq = 0.f;
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            const int i = lane + 32 * j;
+            if (i < nvec)
+            {
+                v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
+                sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
+            }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+        const float var = sq / (float)D;
+        scale = 1.0f / sqrtf(var + eps);
+    }
     const float4 *w4 = reinterpret_cast<const float4 *>(w);
     const float4 *b4 = reinterpret_cast<const float4 *>(b);
-    uint2 *yr = reinterpret_cast<uint2 *>(y + (size_t)row * D);
+    const bool vec16 = (nvec & 1) == 0;
+    OutT *yr = y + (size_t)row * D;
 #pragma unroll
     for (int j = 0; j < MAXV; ++j)
     {
         const int i = lane + 32 * j;
+        float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;
         if (i < nvec)
         {
-            const float4 ww = __ldg(w4 + i), bb = __ldg(b4 + i);
-            const float o0 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww.x), bb.x);
-            const float o1 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww.y), bb.y);
-            const float o2 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww.z), bb.z);
-            const float o3 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww.w), bb.w);
-            const __half2 h0 = __floats2half2_rn(o0, o1), h1 = __floats2half2_rn(o2, o3);
-            uint2 u;
-            u.x = *reinterpret_cast<const uint32_t *>(&h0);
-            u.y = *reinterpret_cast<const uint32_t *>(&h1);
-            yr[i] = u;
+            if constexpr (NORM)
+            {
+                const float4 ww = __ldg(w4 + i), bb = __ldg(b4 + i);
+                o0 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww.x), bb.x);
+                o1 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww.y), bb.y);
+                o2 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww.z), bb.z);
+                o3 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww.w), bb.w);
+            }
+            else
+            {
+                o0 = v[j].x; o1 = v[j].y; o2 = v[j].z; o3 = v[j].w;
+            }
         }
+        store4(yr, i, i < nvec, vec16, o0, o1, o2, o3);
     }
 }
 

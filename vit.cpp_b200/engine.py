@@ -36,6 +36,11 @@ class Taps(C.Structure):
                                          ("embed", "ln1", "qkv", "attn", "x1", "ln2", "h", "x2", "final_ln", "x_final")]
 
 
+class FeaturesReq(C.Structure):
+    """vitb200_features_req (include/vitb200.h)."""
+    _fields_ = [("layers", C.c_int32), ("norm", C.c_int32), ("dtype", C.c_int32)]
+
+
 class Tensor(C.Structure):
     """vitb200_tensor (include/vitb200.h): one host tensor as found in vit_model::tensors (reference vit.h:88)."""
     _fields_ = [("name", C.c_char_p), ("data", C.c_void_p), ("type", C.c_int32), ("n_dims", C.c_int32), ("ne", C.c_int64 * 4)]
@@ -77,6 +82,9 @@ def lib():
         L.vitb200_forward_u8.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32]
         L.vitb200_forward_u8_async.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i32]
         L.vitb200_forward_device.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp]
+        L.vitb200_features.argtypes = [vp, vp, i32, C.POINTER(FeaturesReq), vp, vp]
+        L.vitb200_features_device.argtypes = [vp, vp, i32, C.POINTER(FeaturesReq), vp, vp, vp]
+        L.vitb200_features_u8.argtypes = [vp, vp, vp, vp, i32, i32, C.POINTER(FeaturesReq), vp, vp]
         L.vitb200_last_launch_count.argtypes = [vp]
         L.vitb200_stream.argtypes = [vp]
         L.vitb200_stream.restype = vp
@@ -256,6 +264,48 @@ def vit_image_preprocess_predict(model: VitModel, images_u8, bilinear: bool = Fa
                                     idx.ctypes.data if predict else None, val.ctypes.data if predict else None, topk if predict else 0),
            "vit_image_preprocess")
     return f32, probs, idx, val, logits
+
+
+BFLOAT16 = "bfloat16"  # numpy has no bf16: such features come back as uint16 bit patterns
+_FEATURE_DTYPES = {np.dtype(np.float32): (0, np.float32), np.dtype(np.float16): (1, np.float16), BFLOAT16: (2, np.uint16)}
+
+
+def _features_call(model: VitModel, B: int, layers, norm: bool, tokens: bool, prelogits: bool, dtype, call):
+    key = dtype if isinstance(dtype, str) else np.dtype(dtype)
+    if key not in _FEATURE_DTYPES:
+        raise ValueError(f"dtype must be float32, float16 or {BFLOAT16!r}, not {dtype!r}")
+    code, np_type = _FEATURE_DTYPES[key]
+    req = FeaturesReq(model.hparams.num_hidden_layers if layers is None else int(layers), int(bool(norm)), code)
+    tok = np.empty((B, model.n_tokens, model.hidden_size), np_type) if tokens else None
+    pre = np.empty((B, model.head_tokens, model.hidden_size), np_type) if prelogits else None
+    call(C.byref(req), tok.ctypes.data if tok is not None else None, pre.ctypes.data if pre is not None else None)
+    return tok, pre
+
+
+def vit_features(model: VitModel, images: np.ndarray, layers=None, norm: bool = True, tokens: bool = True, prelogits: bool = False,
+                 dtype=np.float32):
+    """Encoder features of host images (vitb200_features): the residual stream after `layers` blocks (None = all of them; 0 = the
+    embeddings), passed through the final LayerNorm when `norm`.  Returns (tokens [B,N,D], prelogits [B,head_tokens,D]), None for an
+    output not asked for.  dtype float32, float16 or BFLOAT16 (returned as uint16 bit patterns).  Images as vit_predict takes them."""
+    imgs = np.ascontiguousarray(images, dtype=np.float32)
+    if imgs.ndim == (3 if model.in_chans == 3 else 2):
+        imgs = imgs[None]
+    B = imgs.shape[0]
+    assert imgs.size == B * model.img_size * model.img_size * model.in_chans, imgs.shape
+    return _features_call(model, B, layers, norm, tokens, prelogits, dtype, lambda req, t, p: _check(
+        lib().vitb200_features(model.handle, imgs.ctypes.data, B, req, t, p), "vit_features"))
+
+
+def vit_features_u8(model: VitModel, images_u8, bilinear: bool = False, layers=None, norm: bool = True, tokens: bool = True,
+                    prelogits: bool = False, dtype=np.float32):
+    """vit_features of HxWx3 uint8 RGB images of any size, pre-processed on the GPU like vit_image_preprocess_predict."""
+    imgs = [np.ascontiguousarray(a, dtype=np.uint8) for a in images_u8]
+    B = len(imgs)
+    ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in imgs])
+    nx = (C.c_int * B)(*[a.shape[1] for a in imgs])
+    ny = (C.c_int * B)(*[a.shape[0] for a in imgs])
+    return _features_call(model, B, layers, norm, tokens, prelogits, dtype, lambda req, t, p: _check(
+        lib().vitb200_features_u8(model.handle, ptrs, nx, ny, B, int(bilinear), req, t, p), "vit_features_u8"))
 
 
 TAP_SHAPES = {
