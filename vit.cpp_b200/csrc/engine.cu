@@ -465,8 +465,27 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
         attr_set[dev & 63] = true;
     }
+    // the staged epilogues' TMA maps over exactly M rows and N columns of the output (and of the residual), encoded per launch:
+    // a captured graph keeps them by value
+    CUtensorMap tmO{}, tmX{};
+    if constexpr (gemm_epi_staged(EPI))
+    {
+        using St = GemmStage<BN, EPI>;
+        auto out_map = [&](CUtensorMap *m, const void *ptr) -> int {
+            if (!St::kF16) return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, (uint64_t)p.M, (uint64_t)p.N, (uint64_t)p.ldo, 32, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+            if (p.headmajor)
+            {
+                if (p.N % 64 != 0) return fail("GEMM: head-major output needs N %% 64 == 0 (N = %d)", p.N);
+                return make_tmap_heads3d(m, ptr, (uint64_t)(p.N / 64), (uint64_t)p.M, (uint64_t)p.plane_rows, 64);
+            }
+            return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, (uint64_t)p.M, (uint64_t)p.N, (uint64_t)p.ldo, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+        };
+        if (out_map(&tmO, p.out)) return 1;
+        if (EPI == EPI_BIAS_F16_HILO && out_map(&tmX, p.out2)) return 1;
+        if (EPI == EPI_BIAS_RESID_F32 && out_map(&tmX, p.resid)) return 1;
+    }
     const int tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + BN - 1) / BN);
-    CUDA_TRY(launch_pdl(kern, dim3((unsigned)tiles), dim3((unsigned)Cfg::kThreads), (size_t)Cfg::SMEM_BYTES, s, tmA, tmB, p));
+    CUDA_TRY(launch_pdl(kern, dim3((unsigned)tiles), dim3((unsigned)Cfg::kThreads), (size_t)Cfg::SMEM_BYTES, s, tmA, tmB, tmO, tmX, p));
     if (e) e->launches++;
     return 0;
 }

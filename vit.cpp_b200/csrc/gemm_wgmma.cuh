@@ -8,12 +8,18 @@
 //
 // Structure (sm_90a): one CTA per 128 x BN tile of C, three warpgroups:
 //   warpgroup 0     TMA producer: one thread streams the 128 x 64 A tile and the BN x 64 W tile of every k-block (SWIZZLE_128B)
-//                   into a kStages-deep shared-memory ring; its registers are handed to the MMA warpgroups (setmaxnreg)
+//                   into a kStages-deep shared-memory ring; the other warps load the tile's bias into shared memory once and, for
+//                   the residual epilogue, prefetch the tile's residual rows into L2; its registers are handed to the MMA
+//                   warpgroups (setmaxnreg)
 //   warpgroups 1-2  MMA + epilogue: each owns 64 rows of the tile and issues 4 x wgmma.m64nBNk16 per k-block with the f32 accumulator
-//                   in registers, then applies bias / GELU / hi-lo split / residual / position embedding on those registers and
-//                   stores straight to global memory (rows >= M and columns >= N are not written)
+//                   in registers, then applies bias / GELU / hi-lo split / residual / position embedding on those registers
 // Pipeline: per ring slot a full mbarrier (TMA transaction bytes) and an empty mbarrier (one arrival per MMA warpgroup once the
 // wgmma reading the slot has retired).
+// Staged epilogue (qkv, proj, fc1, fc2): once both MMA warpgroups' wgmmas have retired the operand ring is free; each warpgroup
+// writes its 64 result rows into it as 64-row x 128-B boxes (SWIZZLE_128B, so the fragment-layout writes are free of bank
+// conflicts) and one thread stores them with TMA.  The residual epilogue first TMA-loads its residual rows into the same boxes and
+// adds them there.  The store maps cover exactly M rows and N columns, so rows >= M and columns >= N are not written.  The patch
+// and head epilogues store straight from registers.
 #pragma once
 #include "ptx.cuh"
 
@@ -35,7 +41,7 @@ struct GemmParams
 {
     int M, N, K;        // valid extents (rows of A / rows of W / reduction); N % 4 == 0
     const float *bias;  // [N]
-    void *out;          // f16 or f32, row-major, leading dimension ldo
+    void *out;          // f16 or f32, row-major, leading dimension ldo (16-B aligned rows for the staged epilogues)
     void *out2;         // EPI_BIAS_F16_HILO: the lo halves, same shape as out
     int ldo;
     int headmajor;      // f16 epilogues: 1 = the output is HEAD-MAJOR, [N / 64 planes][plane_rows][64]: every head's q / k / v slice is one
@@ -135,38 +141,74 @@ __device__ __forceinline__ void wgmma_k16(float (&acc)[BN / 2], uint64_t adesc, 
     else ptx::wgmma_m64n128k16_f16(acc, adesc, bdesc, accumulate);
 }
 
+// Epilogues whose result goes out through shared memory and TMA stores (the rest store from registers)
+__host__ __device__ constexpr bool gemm_epi_staged(int epi)
+{
+    return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32;
+}
+
+// Staged-epilogue geometry: each MMA warpgroup's 64 x BN result leaves as boxes of 64 rows x 128 B (64 f16 or 32 f32 columns),
+// one box set per output tensor (hi and lo for EPI_BIAS_F16_HILO), in the operand ring it no longer needs
+template <int BN, int EPI>
+struct GemmStage
+{
+    static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO);
+    static constexpr int kBoxCols = kF16 ? 64 : 32;
+    static constexpr int kBoxes = BN / kBoxCols;   // boxes per output tensor and warpgroup
+    static constexpr int kBoxBytes = 64 * 128;
+    static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
+    static constexpr int kWgBytes = kOuts * kBoxes * kBoxBytes;
+    static_assert(2 * kWgBytes <= GemmCfg<BN>::kStages * (GemmCfg<BN>::A_BYTES + GemmCfg<BN>::B_BYTES), "staged tile exceeds the ring");
+};
+
+// tmOut: the store map of out (f16: box 64 columns x 64 rows, 2-D [M][N] or, head-major, 3-D {64, M, N / 64 planes}; f32: box
+// 32 columns x 64 rows over [M][N]), SWIZZLE_128B.  tmAux: the same map over out2 (EPI_BIAS_F16_HILO) or the load map of resid
+// (EPI_BIAS_RESID_F32).  Both unused by the register epilogues.
 template <int BN, int EPI>
 __global__ void __launch_bounds__(384, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
+                  const __grid_constant__ CUtensorMap tmAux, const GemmParams p)
 {
     static_assert(BN == 128 || BN == 256, "BN");
     using Cfg = GemmCfg<BN>;
     constexpr int kStages = Cfg::kStages;
-    constexpr bool kOutF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO);
+    constexpr bool kStaged = gemm_epi_staged(EPI);
 
     extern __shared__ uint8_t smem_raw[];
     __shared__ int s_ln_last;
+    __shared__ __align__(16) float s_bias[BN]; // the tile's bias, zero past N
     const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u; // SWIZZLE_128B wants 1024-B aligned tiles
     const uint32_t sA = smem_base;
     const uint32_t sB = sA + kStages * Cfg::A_BYTES;
     const uint32_t bars = sB + kStages * Cfg::B_BYTES;
     auto full_bar = [&](int s) { return bars + 8u * s; };
     auto empty_bar = [&](int s) { return bars + 8u * (kStages + s); };
+    const uint32_t bias_bar = bars + 8u * (2 * kStages);
+    auto resid_bar = [&](int cw) { return bars + 8u * (2 * kStages + 1 + cw); };
 
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
     const int n_tiles = (p.N + BN - 1) / BN;
     const int m_blk = blockIdx.x / n_tiles, n_blk = blockIdx.x - m_blk * n_tiles;
     const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
+    const int m0 = m_blk * GEMM_BM, n0 = n_blk * BN;
 
     if (threadIdx.x == 0)
     {
         ptx::prefetch_tensormap(&tmA);
         ptx::prefetch_tensormap(&tmB);
+        if constexpr (kStaged)
+        {
+            ptx::prefetch_tensormap(&tmOut);
+            if constexpr (EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_RESID_F32) ptx::prefetch_tensormap(&tmAux);
+        }
         for (int s = 0; s < kStages; ++s)
         {
             ptx::mbar_init(full_bar(s), 1);
             ptx::mbar_init(empty_bar(s), 2); // one arrival per MMA warpgroup
         }
+        ptx::mbar_init(bias_bar, 96); // producer warps 1-3
+        ptx::mbar_init(resid_bar(0), 1);
+        ptx::mbar_init(resid_bar(1), 1);
         ptx::fence_barrier_init();
     }
     __syncthreads();
@@ -180,16 +222,28 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ptx::setmaxnreg_dec<40>();
         if (tid == 0)
         {
-            const int a_row = m_blk * GEMM_BM, b_row = n_blk * BN;
             for (int kb = 0; kb < num_kb; ++kb)
             {
                 const int s = kb % kStages;
                 ptx::mbar_wait(empty_bar(s), ((kb / kStages) & 1) ^ 1);
                 // out-of-range rows / columns are zero-filled and still count their bytes
                 ptx::mbar_arrive_expect_tx(full_bar(s), Cfg::A_BYTES + Cfg::B_BYTES);
-                ptx::tma_load_2d(sA + s * Cfg::A_BYTES, &tmA, full_bar(s), kb * GEMM_BK, a_row);
-                ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * GEMM_BK, b_row);
+                ptx::tma_load_2d(sA + s * Cfg::A_BYTES, &tmA, full_bar(s), kb * GEMM_BK, m0);
+                ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * GEMM_BK, n0);
             }
+        }
+        else if (tid >= 32)
+        {
+            if constexpr (EPI == EPI_BIAS_RESID_F32)
+            {
+                // the residual rows are read once, by the epilogue: start pulling them into L2 while the main loop runs
+                if (tid == 32)
+                    for (int h = 0; h < 2; ++h)
+                        if (m0 + 64 * h < p.M)
+                            for (int c = n0; c < min(n0 + BN, p.N); c += 32) ptx::tma_prefetch_2d(&tmAux, c, m0 + 64 * h);
+            }
+            for (int c = tid - 32; c < BN; c += 96) s_bias[c] = n0 + c < p.N ? __ldg(p.bias + n0 + c) : 0.f;
+            ptx::mbar_arrive(bias_bar);
         }
         return;
     }
@@ -217,57 +271,131 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     ptx::wgmma_wait<0>();
     ptx::fence_regs(acc);
+    ptx::mbar_wait(bias_bar, 0);
 
-    // ===================== epilogue, straight from the accumulator registers =====================
     // wgmma m64nN layout: thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8) and, per 8-column group j, columns 8 j + 2 (l % 4) (+ 1)
     const int warp = tid >> 5, lane = tid & 31;
-    const int row0 = m_blk * GEMM_BM + cw * 64 + warp * 16 + (lane >> 2);
-    const int col0 = n_blk * BN + 2 * (lane & 3);
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j)
+    if constexpr (kStaged)
     {
-        const int col = col0 + 8 * j;
-        if (col >= p.N) continue; // N % 4 == 0: a column pair is all-in or all-out
-        const float2 b = __ldg(reinterpret_cast<const float2 *>(p.bias + col));
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
+        // ===================== staged epilogue: registers -> swizzled boxes in the free ring -> TMA stores =====================
+        using St = GemmStage<BN, EPI>;
+        const int wm0 = m0 + cw * 64;                                                  // first row of this warpgroup
+        const bool live = wm0 < p.M;                                                   // any of its rows inside M
+        const int nbox = min(St::kBoxes, (p.N - n0 + St::kBoxCols - 1) / St::kBoxCols); // boxes that start inside N
+        const uint32_t stage = smem_base + cw * St::kWgBytes;
+        ptx::named_bar_sync(1, 256); // both warpgroups' wgmmas have retired: nothing reads the ring any more
+        if constexpr (EPI == EPI_BIAS_RESID_F32)
         {
-            const int row = row0 + 8 * h;
-            if (row >= p.M) continue;
-            const float x0 = __fadd_rn(acc[4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
-            if constexpr (kOutF16)
+            if (live)
             {
-                const size_t off = p.headmajor ? ((size_t)(col >> 6) * p.plane_rows + (size_t)row) * 64 + (col & 63) : (size_t)row * p.ldo + col;
-                __half2 hv;
-                if constexpr (EPI == EPI_BIAS_GELU_F16)
+                if (tid == 0)
                 {
-                    const float2 r = __half22float2(__floats2half2_rn(x0, x1)); // ggml.c:1434-1441: y = f16(gelu(f32(f16(x))))
-                    hv = __floats2half2_rn(gelu_tanh_f32(r.x), gelu_tanh_f32(r.y));
+                    ptx::mbar_arrive_expect_tx(resid_bar(cw), nbox * St::kBoxBytes); // partial boxes count in full (zero fill)
+                    for (int b = 0; b < nbox; ++b) ptx::tma_load_2d(stage + b * St::kBoxBytes, &tmAux, resid_bar(cw), n0 + 32 * b, wm0);
                 }
-                else hv = __floats2half2_rn(x0, x1);
-                *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(p.out) + off) = hv;
-                if constexpr (EPI == EPI_BIAS_F16_HILO)
+                ptx::mbar_wait(resid_bar(cw), 0);
+            }
+        }
+        // row r of a box lives at r * 128 B with its 16-B chunks permuted by chunk ^ (r % 8); r % 8 == lane / 4 for every row here
+        const int rr = warp * 16 + (lane >> 2), sw = lane >> 2, q = lane & 3;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+        {
+            const float2 b = *reinterpret_cast<const float2 *>(&s_bias[8 * j + 2 * q]);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+            {
+                const uint32_t row = stage + (uint32_t)(rr + 8 * h) * 128u;
+                const float x0 = __fadd_rn(acc[4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
+                if constexpr (St::kF16)
                 {
-                    const float2 hf = __half22float2(hv); // lo = f16(x - hi): exact difference, |lo| <= 2^-11 |x|
-                    *reinterpret_cast<__half2 *>(reinterpret_cast<__half *>(p.out2) + off) = __floats2half2_rn(__fsub_rn(x0, hf.x), __fsub_rn(x1, hf.y));
+                    const uint32_t a = row + (j / 8) * St::kBoxBytes + (((j % 8) ^ sw) << 4) + 4 * q;
+                    __half2 hv;
+                    if constexpr (EPI == EPI_BIAS_GELU_F16)
+                    {
+                        const float2 r = __half22float2(__floats2half2_rn(x0, x1)); // ggml.c:1434-1441: y = f16(gelu(f32(f16(x))))
+                        hv = __floats2half2_rn(gelu_tanh_f32(r.x), gelu_tanh_f32(r.y));
+                    }
+                    else hv = __floats2half2_rn(x0, x1);
+                    ptx::st_shared_b32(a, *reinterpret_cast<const uint32_t *>(&hv));
+                    if constexpr (EPI == EPI_BIAS_F16_HILO)
+                    {
+                        const float2 hf = __half22float2(hv); // lo = f16(x - hi): exact difference, |lo| <= 2^-11 |x|
+                        const __half2 lo = __floats2half2_rn(__fsub_rn(x0, hf.x), __fsub_rn(x1, hf.y));
+                        ptx::st_shared_b32(a + St::kBoxes * St::kBoxBytes, *reinterpret_cast<const uint32_t *>(&lo));
+                    }
+                }
+                else
+                {
+                    const uint32_t a = row + (j / 4) * St::kBoxBytes + (((2 * (j % 4) + (q >> 1)) ^ sw) << 4) + 8 * (q & 1);
+                    if constexpr (EPI == EPI_BIAS_RESID_F32)
+                    {
+                        const float2 r = ptx::ld_shared_v2_f32(a); // (mul_mat + b) + inpL, vit.cpp:869,873
+                        ptx::st_shared_v2_f32(a, __fadd_rn(x0, r.x), __fadd_rn(x1, r.y));
+                    }
+                    else ptx::st_shared_v2_f32(a, x0, x1);
                 }
             }
-            else if constexpr (EPI == EPI_PATCH_F32)
+        }
+        ptx::fence_proxy_async_smem(); // the writes above are seen by the TMA engine
+        ptx::named_bar_sync(2 + cw, 128);
+        if (tid == 0 && live)
+        {
+            for (int b = 0; b < nbox; ++b)
             {
-                const int img = row / p.np, pp = row - img * p.np;
-                const float2 pe = __ldg(reinterpret_cast<const float2 *>(p.pos + (size_t)(1 + pp) * p.N + col));
-                *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + ((size_t)img * p.ntok + 1 + pp) * p.ldo + col) =
-                    make_float2(__fadd_rn(x0, pe.x), __fadd_rn(x1, pe.y));
-            }
-            else
-            {
-                float *o = reinterpret_cast<float *>(p.out) + (size_t)row * p.ldo + col;
-                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                const uint32_t src = stage + b * St::kBoxBytes;
+                if constexpr (St::kF16)
                 {
-                    const float2 r = *reinterpret_cast<const float2 *>(p.resid + (size_t)row * p.ldo + col); // (mul_mat + b) + inpL, vit.cpp:869,873
-                    *reinterpret_cast<float2 *>(o) = make_float2(__fadd_rn(x0, r.x), __fadd_rn(x1, r.y));
+                    if (p.headmajor)
+                    {
+                        const int plane = (n0 >> 6) + b;
+                        ptx::tma_store_3d(&tmOut, src, 0, wm0, plane);
+                        if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_3d(&tmAux, src + St::kBoxes * St::kBoxBytes, 0, wm0, plane);
+                    }
+                    else
+                    {
+                        ptx::tma_store_2d(&tmOut, src, n0 + 64 * b, wm0);
+                        if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_2d(&tmAux, src + St::kBoxes * St::kBoxBytes, n0 + 64 * b, wm0);
+                    }
                 }
-                else *reinterpret_cast<float2 *>(o) = make_float2(x0, x1);
+                else ptx::tma_store_2d(&tmOut, src, n0 + 32 * b, wm0);
+            }
+            ptx::tma_store_commit();
+            if (EPI == EPI_BIAS_RESID_F32 && p.ln_out != nullptr)
+            {
+                // the fused LayerNorm below reads these rows from global memory, possibly in another CTA: the stores must have landed
+                ptx::tma_store_wait_group<0>();
+                ptx::fence_proxy_async_global();
+                __threadfence();
+            }
+            else ptx::tma_store_wait_read<0>(); // the shared memory must outlive the reads of the stores
+        }
+    }
+    else
+    {
+        // ===================== register epilogue (patch embedding, head) =====================
+        const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
+        const int col0 = n0 + 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+        {
+            const int col = col0 + 8 * j;
+            if (col >= p.N) continue; // N % 4 == 0: a column pair is all-in or all-out
+            const float2 b = *reinterpret_cast<const float2 *>(&s_bias[col - n0]);
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+            {
+                const int row = row0 + 8 * h;
+                if (row >= p.M) continue;
+                const float x0 = __fadd_rn(acc[4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
+                if constexpr (EPI == EPI_PATCH_F32)
+                {
+                    const int img = row / p.np, pp = row - img * p.np;
+                    const float2 pe = __ldg(reinterpret_cast<const float2 *>(p.pos + (size_t)(1 + pp) * p.N + col));
+                    *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + ((size_t)img * p.ntok + 1 + pp) * p.ldo + col) =
+                        make_float2(__fadd_rn(x0, pe.x), __fadd_rn(x1, pe.y));
+                }
+                else *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)row * p.ldo + col) = make_float2(x0, x1);
             }
         }
     }
@@ -277,8 +405,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (p.ln_out != nullptr)
         {
             // fused LayerNorm: the CTA that completes the last column tile of this M tile normalises its rows
-            __threadfence(); // this thread's stores are visible GPU-wide before the counter moves
-            ptx::named_bar_sync(1, 256);
+            ptx::named_bar_sync(1, 256); // both warpgroups' stores are complete and fenced before the counter moves
             if (threadIdx.x == 128)
             {
                 const int last = atomicAdd(p.ln_count + m_blk, 1) == n_tiles - 1;

@@ -24,6 +24,8 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// orders this thread's view of global memory written through the async proxy (completed TMA stores) with its generic accesses
+__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -137,6 +139,17 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *m, uint32_t smem
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d)
 {
     asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory"); }
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b)
+{
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+__device__ __forceinline__ float2 ld_shared_v2_f32(uint32_t addr)
+{
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
 }
 // 3-D tiled store shared -> global (bulk async group); elements outside the tensor are not written
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, int c2)
