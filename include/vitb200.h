@@ -220,7 +220,8 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
 /* Stand-alone run of one attention kernel (head dim 64) over a fused QKV buffer: qkv = f16 bits [B*N][3*H*64] (what the qkv
  * GEMM leaves behind, reference vit.cpp:826-846), out = float32 [B*N][H*64] (the merged heads before proj, vit.cpp:860-866).
  * kernel: 0 = the engine's choice for N, 1 = two-pass mma.sync with 8 warps (any N), 2 = wgmma with TMA-staged operands (N <= 224),
- * 3 = two-pass mma.sync with 16 warps (128 < N <= 640). */
+ * 3 = two-pass mma.sync with 16 warps (128 < N <= 640).  The wgmma kernel always runs on split-precision operands; here their lo
+ * halves are zero, so it computes with the f16 values of qkv as given. */
 int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out);
 
 /* The wgmma attention kernel (N <= 224) on split-precision operands, the way the engine runs it: every q, k, v value is

@@ -197,13 +197,10 @@ def test_rejected_requests_leave_the_engine_intact():
     s.close()
 
 
-@pytest.mark.parametrize("fused_ln", ["0", "1"])
-def test_classification_is_undisturbed_by_features_calls(fused_ln, monkeypatch):
-    """vit_predict before and after a sequence of features calls on the same engine is bit-identical, also with the fused LayerNorm
-    (whose fc2 epilogue writes the next block's LayerNorm 1 inside a full forward); features do not depend on that option either."""
-    monkeypatch.setenv("VITB200_FUSED_LN", fused_ln)
+def test_classification_is_undisturbed_by_features_calls():
+    """vit_predict before and after a sequence of features calls on the same engine is bit-identical, and features from an engine
+    that also classifies match those of an engine that only runs features."""
     m = eng.vit_model_load(model_path("micro", "f16"), 0, 5)
-    monkeypatch.delenv("VITB200_FUSED_LN")
     ref = eng.vit_model_load(model_path("micro", "f16"), 0, 5)
     imgs = gf.synthetic_images(5, m.img_size, seed=19)
     want = eng.vit_predict(m, imgs, 5, want_logits=True)

@@ -286,25 +286,18 @@ def test_class_counts_that_are_not_a_multiple_of_four(classes, tmp_path):
     m.close()
 
 
-def test_fused_layernorm_path_is_bit_identical(monkeypatch):
-    """VITB200_FUSED_LN=1 applies the block LayerNorms inside the proj / fc2 residual epilogues (row-group completion counters +
-    dedicated LayerNorm warps behind a shared-memory queue).  It is opt-in because it measured slower than the stand-alone kernel,
-    but it must stay correct: same arithmetic, so logits are bit-identical, including a ragged batch whose last M tile is partial
-    and a geometry with a 128-column N tile (micro: hidden 128)."""
+def test_forward_launch_count():
+    """The fixed kernel schedule of one forward: patchify + cls rows + patch GEMM, 7 kernels per block (LayerNorm 1, qkv, attention,
+    proj, LayerNorm 2, fc1, fc2), pooled LayerNorm + head + soft-max -- on a geometry with a 128-column N tile (micro: hidden 128) and
+    a ragged batch whose last M tile is partial."""
     for cfg, n in (("micro", 5), ("base", 3)):
         imgs = gf.synthetic_images(n, gf.CONFIGS[cfg][4], seed=12)
-        monkeypatch.delenv("VITB200_FUSED_LN", raising=False)
         m = eng.vit_model_load(model_path(cfg, "f16"), 0, 8)
-        want = eng.vit_predict(m, imgs, 5, want_logits=True)
-        m.close()
-        monkeypatch.setenv("VITB200_FUSED_LN", "1")
-        m = eng.vit_model_load(model_path(cfg, "f16"), 0, 8)
-        got = eng.vit_predict(m, imgs, 5, want_logits=True)
+        eng.vit_predict(m, imgs, 5, want_logits=True)
         launches = m.last_launch_count()
         m.close()
-        assert np.array_equal(got[3], want[3]) and np.array_equal(got[1], want[1])
         L = gf.CONFIGS[cfg][1]
-        assert launches == 3 + 1 + 5 * L + 3   # patchify + cls rows + patch GEMM, first LayerNorm, 5 kernels per block, pooled LN + head + soft-max: no other LayerNorm launches except the first block's and the pooled final one
+        assert launches == 3 + 7 * L + 3
 
 
 def test_error_paths():

@@ -38,7 +38,7 @@ re = np.abs(logits - l_ref).max(1) / np.abs(l_ref).max(1)
 l2 = np.linalg.norm(logits - l_ref, axis=1) / np.linalg.norm(l_ref, axis=1)
 order = np.argsort(-l_ref, 1)[:, :5]
 top5 = (order == idx).all(1)
-print(f"{cfg} {ft} n={n} hilo={os.environ.get('VITB200_ATTN_HILO', '1')} vs {src}")
+print(f"{cfg} {ft} n={n} vs {src}")
 print(f"  max-norm rel: median {np.median(re):.3e} p90 {np.quantile(re, 0.9):.3e} max {re.max():.3e} mean {re.mean():.3e}; images > 1e-3: {(re > 1e-3).sum()}")
 print(f"  L2 rel: median {np.median(l2):.3e} max {l2.max():.3e}; top-1 match {(order[:, 0] == idx[:, 0]).mean():.3f}; top-5 lists identical {top5.sum()}/{n}")
 if floor is not None:

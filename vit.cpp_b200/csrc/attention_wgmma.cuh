@@ -5,11 +5,11 @@
 // maximum, e = f16(exp(f16(s * scale - max))), l = sum e in f32, O = (P V) * (1 / l).
 //
 //   TMA       one thread loads the q tiles (64 rows each) and the whole K and V of the head (224 rows, zero-filled / masked past N)
-//             out of the head-major QKV buffers, SWIZZLE_128B, under one mbarrier -- hi and, with HILO, lo halves
+//             out of the head-major QKV buffers, SWIZZLE_128B, under one mbarrier -- hi and lo halves
 //   S = QK^T  wgmma.m64n224k16, A = Q tile and B = K from shared memory, f32 accumulators in registers (one warpgroup per 64-query
-//             tile; two warpgroups, each taking every other tile).  HILO: S = Ql Kh^T + Qh Kl^T + Qh Kh^T (kernels.cuh explains why)
+//             tile; two warpgroups, each taking every other tile): S = Ql Kh^T + Qh Kl^T + Qh Kh^T (kernels.cuh explains why)
 //   softmax   in registers: each row lives in one quad of lanes; P is packed to f16 in place, already in the A-fragment layout
-//   O = P V   wgmma.m64n64k16 with A = P from registers and B = V (MN-major) from shared memory; HILO: O = P Vl + P Vh
+//   O = P V   wgmma.m64n64k16 with A = P from registers and B = V (MN-major) from shared memory: O = P Vl + P Vh
 #pragma once
 #include "kernels.cuh"
 
@@ -20,12 +20,13 @@ constexpr int ATTW_THREADS = 256;                    // two warpgroups
 constexpr int ATTW_QTILE_BYTES = 64 * 128;           // 64 query rows x 64 dims f16
 constexpr int ATTW_KV_BYTES = ATTW_KEYS * 128;       // 224 rows x 64 dims f16 (28 KB, 1024-B multiple)
 
-__host__ __device__ inline int attention_wgmma_smem_bytes(bool hilo)
+constexpr int ATTW_PARTS = 2;                        // hi and lo halves of every operand
+
+__host__ __device__ inline int attention_wgmma_smem_bytes()
 {
-    return 1024 + (hilo ? 2 : 1) * (4 * ATTW_QTILE_BYTES + 2 * ATTW_KV_BYTES) + 64;
+    return 1024 + ATTW_PARTS * (4 * ATTW_QTILE_BYTES + 2 * ATTW_KV_BYTES) + 64;
 }
 
-template <bool HILO>
 __global__ void __launch_bounds__(ATTW_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                        const __grid_constant__ CUtensorMap tmQl, const __grid_constant__ CUtensorMap tmKVl,
@@ -34,7 +35,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 {
     extern __shared__ uint8_t attw_smem_raw[];
     const uint32_t base = (ptx::smem_u32(attw_smem_raw) + 1023u) & ~1023u;
-    constexpr int kParts = HILO ? 2 : 1;
+    constexpr int kParts = ATTW_PARTS;
     // [part][4 q tiles] | [part] K | [part] V | barrier
     auto sQ = [&](int part, int t) { return base + (uint32_t)(part * 4 + t) * ATTW_QTILE_BYTES; };
     auto sK = [&](int part) { return base + kParts * 4 * ATTW_QTILE_BYTES + (uint32_t)part * ATTW_KV_BYTES; };
@@ -82,14 +83,10 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 #pragma unroll
         for (int k = 0; k < 4; ++k) // 64 dims = 4 x K 16 (+32 B each)
         {
-            if constexpr (HILO)
-            {
-                const uint64_t ql = ptx::wgmma_desc_kmajor_sw128(sQ(1, mt)), kl = ptx::wgmma_desc_kmajor_sw128(sK(1));
-                ptx::wgmma_m64n224k16_f16(s, ql + 2 * k, kh + 2 * k, k != 0);
-                ptx::wgmma_m64n224k16_f16(s, qh + 2 * k, kl + 2 * k, 1);
-                ptx::wgmma_m64n224k16_f16(s, qh + 2 * k, kh + 2 * k, 1);
-            }
-            else ptx::wgmma_m64n224k16_f16(s, qh + 2 * k, kh + 2 * k, k != 0);
+            const uint64_t ql = ptx::wgmma_desc_kmajor_sw128(sQ(1, mt)), kl = ptx::wgmma_desc_kmajor_sw128(sK(1));
+            ptx::wgmma_m64n224k16_f16(s, ql + 2 * k, kh + 2 * k, k != 0);
+            ptx::wgmma_m64n224k16_f16(s, qh + 2 * k, kl + 2 * k, 1);
+            ptx::wgmma_m64n224k16_f16(s, qh + 2 * k, kh + 2 * k, 1);
         }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
@@ -144,12 +141,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             const uint32_t a0 = __float_as_uint(s[8 * kk]), a1 = __float_as_uint(s[8 * kk + 2]);
             const uint32_t a2 = __float_as_uint(s[8 * kk + 4]), a3 = __float_as_uint(s[8 * kk + 6]);
             const uint64_t vh = ptx::wgmma_desc_mnmajor_sw128(sV(0) + (uint32_t)kk * 2048u);
-            if constexpr (HILO)
-            {
-                ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, ptx::wgmma_desc_mnmajor_sw128(sV(1) + (uint32_t)kk * 2048u), kk != 0);
-                ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, vh, 1);
-            }
-            else ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, vh, kk != 0);
+            ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, ptx::wgmma_desc_mnmajor_sw128(sV(1) + (uint32_t)kk * 2048u), kk != 0);
+            ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, vh, 1);
         }
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();

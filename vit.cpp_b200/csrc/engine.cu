@@ -166,10 +166,9 @@ struct vitb200_engine
     float *d_img = nullptr, *X = nullptr, *d_logits = nullptr, *d_probs = nullptr, *d_topk_val = nullptr;
     int32_t *d_topk_idx = nullptr;
     __half *A16 = nullptr, *QKV16 = nullptr, *H16 = nullptr, *CLS16 = nullptr, *PA = nullptr;
-    __half *QKV16L = nullptr; // lo halves of q, k, v (x - f16(x), as f16): the attention's split-precision operands
-    int *d_ln_count = nullptr; // fused LayerNorm: one completion counter per 128-row M tile of the residual stream (zero between launches)
-    bool fused_ln = false;     // LayerNorm applied inside the proj / fc2 residual epilogues (VITB200_FUSED_LN=0: separate kernel)
-    bool attn_hilo = false;   // qkv GEMM emits hi + lo and the attention runs the 3 + 2 term products (VITB200_ATTN_HILO=0: hi only)
+    // lo halves of q, k, v (x - f16(x), as f16): the split-precision operands of the wgmma attention.  Allocated exactly when that
+    // kernel runs (N <= 224); then the qkv GEMM emits hi + lo and the attention runs the 3 + 2 term products.
+    __half *QKV16L = nullptr;
     CUtensorMap tmA_D, tmA_H, tmA_P, tmA_C;
     CUtensorMap tmQ, tmKV, tmQl, tmKVl; // attention operand maps (N <= 224: attention_wgmma_kernel)
     int max_k = 16;
@@ -421,23 +420,9 @@ struct ProfScope
     }
 };
 
-// L2 eviction hints of the stand-alone LayerNorm: its input rows are read once, its output is read by the next GEMM nine to twelve
-// times.  VITB200_L2HINT = bit mask, default 4: 4 = LayerNorm input loads evict_first, 8 = LayerNorm output stores evict_last.
-int l2_hint_mask()
-{
-    static const int m = getenv("VITB200_L2HINT") ? atoi(getenv("VITB200_L2HINT")) : 4;
-    return m;
-}
-
 // Programmatic dependent launch for the per-layer kernels (GEMMs, attention, LayerNorm): each of them ends its prologue with
 // griddepcontrol.launch_dependents + griddepcontrol.wait (ptx.cuh), so kernel k+1's barrier init / descriptor
-// prefetch runs on the SMs kernel k has already left.  VITB200_PDL=0 launches them fully serialised.
-bool pdl_enabled()
-{
-    static const bool on = !(getenv("VITB200_PDL") && atoi(getenv("VITB200_PDL")) == 0);
-    return on;
-}
-
+// prefetch runs on the SMs kernel k has already left.
 template <typename... KArgs, typename... Args>
 cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args &&...args)
 {
@@ -447,7 +432,7 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
@@ -562,10 +547,9 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
                      int rows_per_group = 0, size_t group_stride = 0)
 {
     const int D = e->hp.hidden_size;
-    // block LayerNorms (all rows consecutive): the persistent bulk-copy kernel; VITB200_LN_TMA=0 keeps the row-per-warp kernel
-    static const bool ln_tma = !(getenv("VITB200_LN_TMA") && atoi(getenv("VITB200_LN_TMA")) == 0);
+    // block LayerNorms (all rows consecutive): the persistent bulk-copy kernel
     // (two CTAs per SM must fit: with one, as for D = 1024, it is slower than the row-per-warp kernel -- 4.98 against 3.9 ms per ViT-L forward)
-    if (ln_tma && rows_per_group <= 0 && x_row_stride == (size_t)D && D % 128 == 0 && 2 * (layernorm_tma_smem_bytes(D) + 1024) <= 233472 && rows >= 8)
+    if (rows_per_group <= 0 && x_row_stride == (size_t)D && D % 128 == 0 && 2 * (layernorm_tma_smem_bytes(D) + 1024) <= 233472 && rows >= 8)
     {
         const int smem = layernorm_tma_smem_bytes(D);
         const int nblk = (rows + LN_TMA_ROWS - 1) / LN_TMA_ROWS;
@@ -577,8 +561,7 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
             int dev = 0;
             CUDA_TRY(cudaGetDevice(&dev));
             if (!attr_set[D / 128][dev & 63]) { CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr_set[D / 128][dev & 63] = true; }
-            CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps,
-                                (unsigned long long)((l2_hint_mask() & 4) ? ptx::L2_EVICT_FIRST : 0), (unsigned long long)((l2_hint_mask() & 8) ? ptx::L2_EVICT_LAST : 0)));
+            CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps));
             return 0;
         };
         int rc = 1;
@@ -602,28 +585,25 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
 }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
-// token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision when the lo halves exist; ATT_MMA16 = the mma.sync kernel
-// with 16 warps, 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.
+// token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision; ATT_MMA16 = the mma.sync kernel with 16 warps,
+// 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.
 enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3 };
 constexpr int ATT_MAX_KEYS_16 = 640;
 
-// q / k / v tensor maps of the wgmma attention over `rows` token rows per plane
+// q / k / v tensor maps (hi and lo halves) of the wgmma attention over `rows` token rows per plane
 int make_attention_maps(vitb200_engine *e, uint64_t rows)
 {
     const uint64_t planes = 3 * (uint64_t)e->hp.num_attention_heads;
-    if (make_tmap_heads3d(&e->tmQ, e->QKV16, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKV, e->QKV16, planes, rows, rows, ATTW_KEYS))
-        return 1;
-    if (e->QKV16L && (make_tmap_heads3d(&e->tmQl, e->QKV16L, planes, rows, rows, 64) ||
-                      make_tmap_heads3d(&e->tmKVl, e->QKV16L, planes, rows, rows, ATTW_KEYS)))
+    if (make_tmap_heads3d(&e->tmQ, e->QKV16, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKV, e->QKV16, planes, rows, rows, ATTW_KEYS) ||
+        make_tmap_heads3d(&e->tmQl, e->QKV16L, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKVl, e->QKV16L, planes, rows, rows, ATTW_KEYS))
         return 1;
     return 0;
 }
 
-template <bool HILO>
 int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
 {
-    const int smem = attention_wgmma_smem_bytes(HILO);
-    auto kern = attention_wgmma_kernel<HILO>;
+    const int smem = attention_wgmma_smem_bytes();
+    auto kern = attention_wgmma_kernel;
     static bool attr_set[64] = {};
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
@@ -633,7 +613,7 @@ int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
         attr_set[dev & 63] = true;
     }
     const int H = e->hp.num_attention_heads;
-    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)smem, s, e->tmQ, e->tmKV, HILO ? e->tmQl : e->tmQ, HILO ? e->tmKVl : e->tmKV,
+    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)smem, s, e->tmQ, e->tmKV, e->tmQl, e->tmKVl,
                         e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H))));
     e->launches++;
     return 0;
@@ -664,8 +644,8 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
 int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO)
 {
     if (kernel == ATT_AUTO) kernel = e->N <= ATTW_KEYS ? ATT_WGMMA : (e->N <= ATT_MAX_KEYS_16 ? ATT_MMA16 : ATT_MMA8);
-    if (kernel == ATT_WGMMA) return e->attn_hilo ? launch_attention_wgmma<true>(e, B, s) : launch_attention_wgmma<false>(e, B, s);
-    if (e->attn_hilo) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
+    if (kernel == ATT_WGMMA) return launch_attention_wgmma(e, B, s);
+    if (e->QKV16L) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
     if (kernel == ATT_MMA16) return launch_attention_t<16>(e, B, s);
     return launch_attention_t<8>(e, B, s);
 }
@@ -700,7 +680,7 @@ int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
     const int D = e->hp.hidden_size, H = e->hp.num_attention_heads;
     const size_t plane_rows = (size_t)e->max_batch * e->N, n = (size_t)3 * H * plane_rows * 64;
     std::vector<float> tmp(n);
-    if (tap_f16(tmp.data(), e->QKV16, n, s, e->attn_hilo ? e->QKV16L : nullptr)) return 1;
+    if (tap_f16(tmp.data(), e->QKV16, n, s, e->QKV16L)) return 1;
     for (int t = 0; t < T; ++t)
         for (int pl = 0; pl < 3 * H; ++pl)
             memcpy(dst + (size_t)t * 3 * D + (size_t)pl * 64, tmp.data() + ((size_t)pl * plane_rows + t) * 64, 64 * sizeof(float));
@@ -738,19 +718,16 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
     {
         const Layer &L = e->layers[il];
         const bool tap = taps && taps->layer == il;
-        // LayerNorm 1 (vit.cpp:808-812): a kernel of its own only in front of the first block -- with fused_ln the fc2 epilogue of
-        // the previous block has already left norm1(x) of this block in A16
-        if (il == 0 || !e->fused_ln)
         {
             ProfScope ps(e, PK_LN, 0.0, s);
-            if (launch_layernorm(e, e->X, (size_t)D, L.n1w, L.n1b, e->A16, T, s)) return 1;
+            if (launch_layernorm(e, e->X, (size_t)D, L.n1w, L.n1b, e->A16, T, s)) return 1; // vit.cpp:808-812
             if (tap && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1;
         }
         {
             GemmParams p{};
             p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.plane_rows = (size_t)e->max_batch * N;
             ProfScope ps(e, PK_QKV, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.qkv.bn, e->attn_hilo ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
+            if (launch_gemm(e, L.qkv.bn, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
         }
         if (tap && tap_qkv(e, taps->qkv, T, s)) return 1;
         {
@@ -759,16 +736,12 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         }
         if (tap && tap_f16(taps->attn, e->A16, (size_t)T * D, s)) return 1;
         {
-            // proj + residual (vit.cpp:868-873); fused: + LayerNorm 2 (vit.cpp:881-885) of each 32-row group as its last column tile
-            // lands, written over the attention output in A16 (every tile that read those rows has finished its MMAs by then)
             GemmParams p{};
             p.M = T; p.N = D; p.K = D; p.bias = L.proj.b; p.out = e->X; p.ldo = D; p.resid = e->X;
-            if (e->fused_ln) { p.ln_out = e->A16; p.ln_w = L.n2w; p.ln_b = L.n2b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps; }
             ProfScope ps(e, PK_PROJ, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.proj.bn, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1;
+            if (launch_gemm(e, L.proj.bn, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1; // proj + residual, vit.cpp:868-873
         }
         if (tap && tap_f32(taps->x1, e->X, (size_t)T * D, s)) return 1;
-        if (!e->fused_ln)
         {
             ProfScope ps(e, PK_LN, 0.0, s);
             if (launch_layernorm(e, e->X, (size_t)D, L.n2w, L.n2b, e->A16, T, s)) return 1; // vit.cpp:881-885
@@ -782,20 +755,12 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
-            // fc2 + residual (vit.cpp:896-900); fused: + LayerNorm 1 of the NEXT block (the last block run has no next block: its
-            // output goes to the pooled final LayerNorm or to the encoder features instead)
             GemmParams p{};
             p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X;
-            if (e->fused_ln && il + 1 < layers)
-            {
-                const Layer &Ln = e->layers[il + 1];
-                p.ln_out = e->A16; p.ln_w = Ln.n1w; p.ln_b = Ln.n1b; p.ln_count = e->d_ln_count; p.ln_eps = e->hp.eps;
-            }
             ProfScope ps(e, PK_FC2, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.fc2.bn, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1;
+            if (launch_gemm(e, L.fc2.bn, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
         }
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
-        if (e->fused_ln && taps && taps->layer == il + 1 && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1; // norm1 of the next block
     }
     return 0;
 }
@@ -1032,7 +997,6 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     e->Cp = (hp->num_classes + 3) / 4 * 4;
     e->KP = e->C * P * P;
     e->KPp = (e->KP + 63) / 64 * 64;
-    e->use_graph = !(getenv("VITB200_GRAPH") && atoi(getenv("VITB200_GRAPH")) == 0);
     auto bail = [&](int) { vitb200_destroy(e); e = nullptr; return 1; };
     if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
 
@@ -1091,15 +1055,6 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         if (cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming) != cudaSuccess)
             return bail(fail("cudaEventCreate failed"));
-    {
-        // Fused LayerNorm (the CTA that completes an M tile of the residual epilogue normalises its rows, gemm_wgmma.cuh): bit-identical
-        // to the stand-alone kernel, opt-in (VITB200_FUSED_LN=1): the normalisation then runs on a few CTAs at the tail of the GEMM instead
-        // of on the whole GPU.  It needs the whole row in N % 128 == 0 float4-per-lane form.
-        const bool want = getenv("VITB200_FUSED_LN") && atoi(getenv("VITB200_FUSED_LN")) == 1;
-        e->fused_ln = want && D % 128 == 0 && D <= 1024;
-        if (e->fused_ln && (dev_alloc(e, &e->d_ln_count, T / GEMM_BM + 1) || cudaMemset(e->d_ln_count, 0, (T / GEMM_BM + 1) * sizeof(int)) != cudaSuccess))
-            return bail(1);
-    }
     if (pa_alias) e->PA = e->H16;
     else
     {
@@ -1110,10 +1065,8 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_BM) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_BM))
         return bail(1);
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
-    // memory (N <= 224); VITB200_ATTN_HILO=0 keeps the f16-only operands
-    e->attn_hilo = e->N <= ATTW_KEYS && !(getenv("VITB200_ATTN_HILO") && atoi(getenv("VITB200_ATTN_HILO")) == 0);
-    if (e->attn_hilo && dev_alloc(e, &e->QKV16L, T * 3 * D)) return bail(1);
-    if (e->N <= ATTW_KEYS && make_attention_maps(e, T)) return bail(1);
+    // memory (N <= 224), i.e. wherever the wgmma attention runs
+    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return bail(1);
     if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
     *out = e;
     e = nullptr; // ownership passed to the caller
@@ -1228,22 +1181,24 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
     };
     to_head_major(qkv);
     if (cudaMemcpy(e->QKV16, hm.data(), (size_t)T * 3 * D * 2, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail("H2D failed"));
-    if (qkv_lo)
+    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return bail(fail("attention kernel %d unknown", kernel));
+    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return bail(fail("wgmma attention needs N <= %d", ATTW_KEYS));
+    if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return bail(fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16));
+    if (kernel == ATT_WGMMA || (kernel == ATT_AUTO && N <= ATTW_KEYS))
     {
-        if (N > 224) return bail(fail("split-precision attention needs N <= 224"));
+        // the wgmma kernel always runs on split-precision operands: without lo halves it reads zero lo planes (dev_alloc zero-fills
+        // them), whose products add exact zeros
         if (dev_alloc(e, &e->QKV16L, (size_t)T * 3 * D)) return bail(1);
-        to_head_major(qkv_lo);
-        if (cudaMemcpy(e->QKV16L, hm.data(), (size_t)T * 3 * D * 2, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail("H2D failed"));
-        e->attn_hilo = true;
+        if (qkv_lo)
+        {
+            to_head_major(qkv_lo);
+            if (cudaMemcpy(e->QKV16L, hm.data(), (size_t)T * 3 * D * 2, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail("H2D failed"));
+        }
+        if (make_attention_maps(e, T)) return bail(1);
     }
     // cudaMemcpy from pageable memory may return before the DMA has landed, and the kernels below run on a NON-BLOCKING stream (no implicit
     // ordering with the legacy stream the copies used): wait for the device before launching
     if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
-    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return bail(fail("attention kernel %d unknown", kernel));
-    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return bail(fail("wgmma attention needs N <= %d", ATTW_KEYS));
-    if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return bail(fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16));
-    if (qkv_lo && kernel != ATT_AUTO && kernel != ATT_WGMMA) return bail(fail("split-precision attention runs in the wgmma kernel"));
-    if (N <= ATTW_KEYS && make_attention_maps(e, T)) return bail(1);
     if (launch_attention(e, B, e->stream, kernel)) return bail(1);
     if (cudaStreamSynchronize(e->stream) != cudaSuccess) return bail(fail("attention kernel failed: %s", cudaGetErrorString(cudaGetLastError())));
     std::vector<__half> tmp((size_t)T * D);

@@ -50,14 +50,6 @@ struct GemmParams
     const float *resid; // EPI_BIAS_RESID_F32: [M][ldo] (may alias out)
     const float *pos;   // EPI_PATCH_F32: pos_embed [ntok][N]
     int np, ntok;       // EPI_PATCH_F32: patches / tokens per image
-    // EPI_BIAS_RESID_F32 with a fused LayerNorm (N == hidden size, N % 128 == 0, N <= 1024): the LayerNorm that follows the residual add
-    // (vit.cpp:881-885 after proj, vit.cpp:808-812 of the next block after fc2) is applied to a 128-row M tile by the CTA that stores the
-    // last of its column tiles (ln_count: one counter per M tile, zero on entry and left zero), while the rows are still in L2; ln_out
-    // receives the f16 rows [M][N].  NULL = no fusion.
-    __half *ln_out;
-    const float *ln_w, *ln_b;
-    int *ln_count;
-    float ln_eps;
 };
 
 constexpr int GEMM_BM = 128;
@@ -86,52 +78,6 @@ __device__ __forceinline__ float gelu_tanh_f32(float x)
     const float w = fmaf(x * x, -0.10294323958083856f, -2.3022081981625516f);
     const float e = ptx::ex2_approx(x * w);                      // e^{-2u}
     return x * ptx::rcp_approx(1.0f + e);
-}
-
-// One warp normalises one row of X (f32, already complete in L2) into the f16 A operand of the next GEMM: the arithmetic of
-// layernorm_f16_kernel (kernels.cuh) -- f32 two-pass mean / biased variance, then ((x - mean) * scale) * w + b as three separately
-// rounded operations (the reference's NORM, MUL, ADD nodes, ggml.c:8959-9008, vit.cpp:808-812), RNE to f16 -- with w and b read from
-// global memory and the row read past L1 (ld.global.cg: other SMs wrote it).  nv = D / 128 float4 per lane (<= 8).
-__device__ __forceinline__ void ln_row_load(const float *xrow, int nv, int lane, float4 (&v)[8])
-{
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        if (j < nv) v[j] = __ldcg(reinterpret_cast<const float4 *>(xrow) + lane + 32 * j);
-}
-__device__ __forceinline__ void ln_row_finish(float4 (&v)[8], int nv, int D, int lane, const float4 *w4, const float4 *b4, float eps, __half *yrow)
-{
-    float sum = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        if (j < nv) sum += (v[j].x + v[j].y) + (v[j].z + v[j].w);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    const float mean = sum / (float)D;
-    float sq = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        if (j < nv)
-        {
-            v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
-            sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
-        }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-    const float scale = 1.0f / sqrtf(sq / (float)D + eps);
-    uint2 *yr = reinterpret_cast<uint2 *>(yrow);
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        if (j < nv)
-        {
-            const int i = lane + 32 * j;
-            const float4 ww = w4[i], bb = b4[i];
-            const __half2 h0 = __floats2half2_rn(__fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww.x), bb.x), __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww.y), bb.y));
-            const __half2 h1 = __floats2half2_rn(__fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww.z), bb.z), __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww.w), bb.w));
-            uint2 u;
-            u.x = *reinterpret_cast<const uint32_t *>(&h0);
-            u.y = *reinterpret_cast<const uint32_t *>(&h1);
-            yr[i] = u;
-        }
 }
 
 template <int BN>
@@ -175,7 +121,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     constexpr bool kStaged = gemm_epi_staged(EPI);
 
     extern __shared__ uint8_t smem_raw[];
-    __shared__ int s_ln_last;
     __shared__ __align__(16) float s_bias[BN]; // the tile's bias, zero past N
     const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u; // SWIZZLE_128B wants 1024-B aligned tiles
     const uint32_t sA = smem_base;
@@ -361,14 +306,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 else ptx::tma_store_2d(&tmOut, src, n0 + 32 * b, wm0);
             }
             ptx::tma_store_commit();
-            if (EPI == EPI_BIAS_RESID_F32 && p.ln_out != nullptr)
-            {
-                // the fused LayerNorm below reads these rows from global memory, possibly in another CTA: the stores must have landed
-                ptx::tma_store_wait_group<0>();
-                ptx::fence_proxy_async_global();
-                __threadfence();
-            }
-            else ptx::tma_store_wait_read<0>(); // the shared memory must outlive the reads of the stores
+            ptx::tma_store_wait_read<0>(); // the shared memory must outlive the reads of the stores
         }
     }
     else
@@ -396,36 +334,6 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         make_float2(__fadd_rn(x0, pe.x), __fadd_rn(x1, pe.y));
                 }
                 else *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)row * p.ldo + col) = make_float2(x0, x1);
-            }
-        }
-    }
-
-    if constexpr (EPI == EPI_BIAS_RESID_F32)
-    {
-        if (p.ln_out != nullptr)
-        {
-            // fused LayerNorm: the CTA that completes the last column tile of this M tile normalises its rows
-            ptx::named_bar_sync(1, 256); // both warpgroups' stores are complete and fenced before the counter moves
-            if (threadIdx.x == 128)
-            {
-                const int last = atomicAdd(p.ln_count + m_blk, 1) == n_tiles - 1;
-                if (last) p.ln_count[m_blk] = 0;
-                s_ln_last = last;
-            }
-            ptx::named_bar_sync(1, 256);
-            if (s_ln_last)
-            {
-                __threadfence();
-                const float *X = reinterpret_cast<const float *>(p.out);
-                const float4 *w4 = reinterpret_cast<const float4 *>(p.ln_w), *b4 = reinterpret_cast<const float4 *>(p.ln_b);
-                const int rows = min(GEMM_BM, p.M - m_blk * GEMM_BM), nv = p.N >> 7;
-                for (int r = (threadIdx.x - 128) >> 5; r < rows; r += 8)
-                {
-                    const size_t grow = (size_t)m_blk * GEMM_BM + r;
-                    float4 v[8];
-                    ln_row_load(X + grow * p.ldo, nv, lane, v);
-                    ln_row_finish(v, nv, p.N, lane, w4, b4, p.ln_eps, p.ln_out + grow * p.N);
-                }
             }
         }
     }

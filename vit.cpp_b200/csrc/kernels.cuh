@@ -236,8 +236,7 @@ __host__ __device__ inline int layernorm_tma_smem_bytes(int D) { return 128 + LN
 
 template <int NV> // float4 per lane = D / 128
 __global__ void __launch_bounds__(LN_TMA_THREADS, 2)
-layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, const float *__restrict__ b, __half *__restrict__ y, int rows, float eps,
-                     unsigned long long load_policy, unsigned long long store_policy) // L2 eviction hints of the bulk copies (0 = none)
+layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, const float *__restrict__ b, __half *__restrict__ y, int rows, float eps)
 {
     constexpr int D = NV * 128;
     extern __shared__ uint8_t ln_smem_raw[];
@@ -270,8 +269,8 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
                 const int nr = rows - row0 < LN_TMA_ROWS ? rows - row0 : LN_TMA_ROWS;
                 ptx::mbar_wait(empty_bar(st), ph ^ 1);
                 ptx::mbar_arrive_expect_tx(full_bar(st), (uint32_t)(nr * D * 4));
-                if (load_policy) ptx::bulk_load_1d_hint(s_in + st * IN_BYTES, x + (size_t)row0 * D, (uint32_t)(nr * D * 4), full_bar(st), load_policy);
-                else ptx::bulk_load_1d(s_in + st * IN_BYTES, x + (size_t)row0 * D, (uint32_t)(nr * D * 4), full_bar(st));
+                // the input rows are read once (the output is what the next GEMM reads again and again): evict them first
+                ptx::bulk_load_1d_hint(s_in + st * IN_BYTES, x + (size_t)row0 * D, (uint32_t)(nr * D * 4), full_bar(st), ptx::L2_EVICT_FIRST);
                 if (++st == LN_TMA_STAGES) { st = 0; ph ^= 1; }
             }
         }
@@ -337,8 +336,7 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
             ptx::named_bar_sync(1, 32 * LN_TMA_ROWS);
             if (threadIdx.x == 0)
             {
-                if (store_policy) ptx::bulk_store_1d_hint(y + (size_t)row0 * D, ob, (uint32_t)(nr * D * 2), store_policy);
-                else ptx::bulk_store_1d(y + (size_t)row0 * D, ob, (uint32_t)(nr * D * 2));
+                ptx::bulk_store_1d(y + (size_t)row0 * D, ob, (uint32_t)(nr * D * 2));
                 ptx::tma_store_commit();
             }
             if (++st == LN_TMA_STAGES) { st = 0; ph ^= 1; }

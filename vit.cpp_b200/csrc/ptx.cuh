@@ -10,13 +10,6 @@ namespace ptx {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ uint32_t lane_id()
-{
-    uint32_t l;
-    asm("mov.u32 %0, %%laneid;" : "=r"(l));
-    return l;
-}
-
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 {
@@ -24,8 +17,6 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count)
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// orders this thread's view of global memory written through the async proxy (completed TMA stores) with its generic accesses
-__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 __device__ __forceinline__ void mbar_arrive(uint32_t bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
@@ -56,19 +47,6 @@ __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.w
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads)
 {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-// Non-blocking probe (no hardware suspend window): for event loops that poll several barriers
-__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity)
-{
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return ok != 0;
 }
 // Bounded spin: a protocol bug traps (launch fails with an error) instead of hanging the GPU.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity)
@@ -109,20 +87,7 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const CUtensorMap
         ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap *m, int c0, int c1, int c2)
-{
-    asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global.tile [%0, {%1, %2, %3}];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1), "r"(c2)
-                 : "memory");
-}
-// 1-D bulk copies (contiguous bytes, 16-B aligned, size a multiple of 16): global -> shared with mbarrier completion, shared -> global in a
-// bulk async group
-__device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(bar)
-                 : "memory");
-}
+// 1-D bulk store (contiguous bytes, 16-B aligned, size a multiple of 16): shared -> global in a bulk async group
 __device__ __forceinline__ void bulk_store_1d(void *gdst, uint32_t smem_src, uint32_t bytes)
 {
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
@@ -135,10 +100,6 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap *m, uint32_t smem
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1)
                  : "memory");
-}
-__device__ __forceinline__ void st_shared_v4(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d)
-{
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
 }
 __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t a) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(a) : "memory"); }
 __device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b)
@@ -166,46 +127,15 @@ __device__ __forceinline__ void tma_store_wait_read()
     asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 
-// wait until at most N of this thread's most recent bulk groups are still pending (FULL completion: the global writes are done)
-template <int N>
-__device__ __forceinline__ void tma_store_wait_group()
-{
-    asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---------------------------------------------------------------- L2 eviction-priority hints on bulk / tensor copies
-// 64-bit cache policies as produced by createpolicy.fractional.L2::evict_*.b64 with fraction 1.0 (the encodings CUTLASS ships as
-// TMA::CacheHintSm90): streamed-once data (evict_first) should not push reused operands out of the 50 MB L2.
-constexpr uint64_t L2_EVICT_FIRST = 0x12F0000000000000ull, L2_EVICT_LAST = 0x14F0000000000000ull;
-__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, uint64_t pol)
-{
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "l"(pol)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_store_3d_hint(const CUtensorMap *m, uint32_t smem_src, int c0, int c1, int c2, uint64_t pol)
-{
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3, %4}], [%1], %5;"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "l"(pol)
-                 : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_hint(uint32_t smem_dst, const CUtensorMap *m, uint32_t bar, int c0, int c1, int c2, uint64_t pol)
-{
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4, %5}], [%2], %6;"
-        ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(m)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "l"(pol)
-        : "memory");
-}
+// ---------------------------------------------------------------- L2 eviction-priority hint on a bulk copy
+// 64-bit cache policy as produced by createpolicy.fractional.L2::evict_first.b64 with fraction 1.0 (the encoding CUTLASS ships as
+// TMA::CacheHintSm90): streamed-once data should not push reused operands out of the 50 MB L2.
+constexpr uint64_t L2_EVICT_FIRST = 0x12F0000000000000ull;
+// 1-D bulk load global -> shared with mbarrier completion (contiguous bytes, 16-B aligned, size a multiple of 16) and an L2 cache policy
 __device__ __forceinline__ void bulk_load_1d_hint(uint32_t smem_dst, const void *gsrc, uint32_t bytes, uint32_t bar, uint64_t pol)
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
                  ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(bar), "l"(pol)
-                 : "memory");
-}
-__device__ __forceinline__ void bulk_store_1d_hint(void *gdst, uint32_t smem_src, uint32_t bytes, uint64_t pol)
-{
-    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;"
-                 ::"l"(reinterpret_cast<uint64_t>(gdst)), "r"(smem_src), "r"(bytes), "l"(pol)
                  : "memory");
 }
 
