@@ -121,8 +121,8 @@ struct Linear
 {
     __half *w = nullptr; // [n_out][ld] f16, K contiguous (ggml ne0 = K)
     float *b = nullptr;  // [n_out]
-    int n_out = 0, n_in = 0, ld = 0, bn = 256;
-    CUtensorMap tm;  // box = 64 x bn rows: the W tile of one k-block
+    int n_out = 0, n_in = 0, ld = 0;
+    CUtensorMap tm;  // box = 64 x GEMM_BN rows: the W tile of one k-block
 };
 
 struct Layer
@@ -130,8 +130,6 @@ struct Layer
     float *n1w = nullptr, *n1b = nullptr, *n2w = nullptr, *n2b = nullptr;
     Linear qkv, proj, fc1, fc2;
 };
-
-int pick_bn(int n_out) { return n_out >= 256 ? 256 : 128; }
 
 // Argument set of one cached CUDA graph: a classification forward (layers = -1) or an encoder-features call
 struct GraphKey
@@ -343,7 +341,7 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     if (conv_p > 0) { if (check_shape(w, wname, conv_p, conv_p, n_in / (conv_p * conv_p), n_out)) return 1; } // [P, P, C, D], vit.cpp:515
     else if (check_shape(w, wname, n_in, n_out, 1, 1)) return 1;                                             // [in, out], vit.cpp:531-543
     if (quant_block_bytes(w->type) && n_in % 32 != 0) return fail("tensor '%s': quantised rows must be a multiple of 32", wname.c_str());
-    L->n_out = n_out; L->n_in = n_in; L->ld = ld; L->bn = pick_bn(n_out);
+    L->n_out = n_out; L->n_in = n_in; L->ld = ld;
     if (dev_alloc(e, &L->w, (size_t)n_out * ld)) return 1;
     CUDA_TRY(cudaMemset(L->w, 0, (size_t)n_out * ld * sizeof(__half)));
     const void *src = w->data;
@@ -388,7 +386,7 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     CUDA_TRY(cudaMemcpy2D(L->w, (size_t)ld * 2, src, (size_t)n_in * 2, (size_t)n_in * 2, (size_t)n_out, cudaMemcpyHostToDevice));
     // conv bias is declared [1, 1, D] (vit.cpp:516), every other bias [n_out]; the tail up to a multiple of 4 stays zero
     if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
-    return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)L->bn);
+    return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)GEMM_BN);
 }
 
 // dynamic shared memory the soft-max kernel may use for its working row (227 KB per CTA minus its static arrays)
@@ -436,18 +434,31 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int BN, int EPI>
+template <int EPI, int STAGES>
 int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
-    using Cfg = GemmCfg<BN>;
-    auto kern = gemm_wgmma_kernel<BN, EPI>;
+    using Cfg = GemmCfg<STAGES>;
+    auto kern = gemm_wgmma_kernel<EPI, STAGES>;
+    // clusters of two CTAs that share the A tile (multicast), with programmatic dependent launch as in launch_pdl
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(2); cfg.blockDim = dim3((unsigned)Cfg::kThreads); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = s;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[1].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 2;
     // the opt-in to > 48 KB dynamic shared memory is per device (one engine per device, possibly several per process)
     static bool attr_set[64] = {};
+    static int max_clusters[64] = {};
     int dev = 0;
     CUDA_TRY(cudaGetDevice(&dev));
     if (!attr_set[dev & 63])
     {
         CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+        CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_clusters[dev & 63], kern, &cfg));
+        if (max_clusters[dev & 63] < 1) return fail("GEMM: no cluster of two CTAs fits on device %d", dev);
         attr_set[dev & 63] = true;
     }
     // the staged epilogues' TMA maps over exactly M rows and N columns of the output (and of the residual), encoded per launch:
@@ -455,7 +466,7 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     CUtensorMap tmO{}, tmX{};
     if constexpr (gemm_epi_staged(EPI))
     {
-        using St = GemmStage<BN, EPI>;
+        using St = GemmStage<EPI, STAGES>;
         auto out_map = [&](CUtensorMap *m, const void *ptr) -> int {
             if (!St::kF16) return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, (uint64_t)p.M, (uint64_t)p.N, (uint64_t)p.ldo, 32, 64, CU_TENSOR_MAP_SWIZZLE_128B);
             if (p.headmajor)
@@ -469,26 +480,24 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
         if (EPI == EPI_BIAS_F16_HILO && out_map(&tmX, p.out2)) return 1;
         if (EPI == EPI_BIAS_RESID_F32 && out_map(&tmX, p.resid)) return 1;
     }
-    const int tiles = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + BN - 1) / BN);
-    CUDA_TRY(launch_pdl(kern, dim3((unsigned)tiles), dim3((unsigned)Cfg::kThreads), (size_t)Cfg::SMEM_BYTES, s, tmA, tmB, tmO, tmX, p));
+    // persistent: as many clusters as fit at once, each walking the pairs of column tiles cluster, cluster + clusters, ...
+    const int pairs = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN));
+    cfg.gridDim = dim3(2u * (unsigned)std::min(pairs, max_clusters[dev & 63]));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmO, tmX, p));
     if (e) e->launches++;
     return 0;
 }
 
-// tmB: the weight map, box = 64 x bn rows
-int launch_gemm(vitb200_engine *e, int bn, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
+// tmB: the weight map, box = 64 x GEMM_BN rows
+int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
     if (p.N % 4 != 0) return fail("GEMM: N = %d is not a multiple of 4", p.N);
-#define VB_CASE(BN, EPI) \
-    if (bn == BN && epi == EPI) return launch_gemm_t<BN, EPI>(e, tmA, tmB, p, s);
-    VB_CASE(256, EPI_BIAS_F16) VB_CASE(128, EPI_BIAS_F16)
-    VB_CASE(256, EPI_BIAS_F16_HILO) VB_CASE(128, EPI_BIAS_F16_HILO)
-    VB_CASE(256, EPI_BIAS_GELU_F16) VB_CASE(128, EPI_BIAS_GELU_F16)
-    VB_CASE(256, EPI_BIAS_RESID_F32) VB_CASE(128, EPI_BIAS_RESID_F32)
-    VB_CASE(256, EPI_PATCH_F32) VB_CASE(128, EPI_PATCH_F32)
-    VB_CASE(256, EPI_BIAS_F32) VB_CASE(128, EPI_BIAS_F32)
+    const bool deep = p.K >= GEMM_DEEP_K; // ring depth by reduction length (GemmCfg)
+#define VB_CASE(EPI) \
+    if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
+    VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
 #undef VB_CASE
-    return fail("no GEMM instantiation for bn=%d epilogue=%d", bn, epi);
+    return fail("no GEMM instantiation for epilogue=%d", epi);
 }
 
 int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaStream_t s)
@@ -710,7 +719,7 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
             CUDA_TRY(cudaGetLastError());
             e->launches++;
         }
-        if (launch_gemm(e, e->patch.bn, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
+        if (launch_gemm(e, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
     if (taps && tap_f32(taps->embed, e->X, (size_t)T * D, s)) return 1;
 
@@ -727,7 +736,7 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
             GemmParams p{};
             p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.plane_rows = (size_t)e->max_batch * N;
             ProfScope ps(e, PK_QKV, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.qkv.bn, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
+            if (launch_gemm(e, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
         }
         if (tap && tap_qkv(e, taps->qkv, T, s)) return 1;
         {
@@ -739,7 +748,7 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
             GemmParams p{};
             p.M = T; p.N = D; p.K = D; p.bias = L.proj.b; p.out = e->X; p.ldo = D; p.resid = e->X;
             ProfScope ps(e, PK_PROJ, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.proj.bn, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1; // proj + residual, vit.cpp:868-873
+            if (launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1; // proj + residual, vit.cpp:868-873
         }
         if (tap && tap_f32(taps->x1, e->X, (size_t)T * D, s)) return 1;
         {
@@ -751,14 +760,14 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
             GemmParams p{};
             p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D;
             ProfScope ps(e, PK_FC1, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.fc1.bn, EPI_BIAS_GELU_F16, e->tmA_D, L.fc1.tm, p, s)) return 1; // vit.cpp:889-893
+            if (launch_gemm(e, EPI_BIAS_GELU_F16, e->tmA_D, L.fc1.tm, p, s)) return 1; // vit.cpp:889-893
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
             GemmParams p{};
             p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X;
             ProfScope ps(e, PK_FC2, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, L.fc2.bn, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
+            if (launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
         }
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
     }
@@ -789,7 +798,7 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
         GemmParams p{};
         p.M = R; p.N = Cp; p.K = D; p.bias = e->head.b; p.out = lg; p.ldo = Cp;
         ProfScope ps(e, PK_HEAD, 2.0 * p.M * C * p.K, s);
-        if (launch_gemm(e, e->head.bn, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
+        if (launch_gemm(e, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
     }
     if (d_logits && lg != d_logits)
         CUDA_TRY(cudaMemcpy2DAsync(d_logits, (size_t)C * 4, lg, (size_t)Cp * 4, (size_t)C * 4, (size_t)R, cudaMemcpyDeviceToDevice, s));
@@ -1061,8 +1070,8 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         if (dev_alloc(e, &e->PA, pa_elems)) return bail(1);
         if (cudaMemset(e->PA, 0, pa_elems * sizeof(__half)) != cudaSuccess) return bail(fail("cudaMemset failed"));
     }
-    if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_BM) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_BM) ||
-        make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_BM) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_BM))
+    if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_A_BOX_ROWS) ||
+        make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_A_BOX_ROWS))
         return bail(1);
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
     // memory (N <= 224), i.e. wherever the wgmma attention runs
@@ -1583,14 +1592,13 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
             if (cudaMalloc(&dR, (size_t)M * N * 4)) { fail("cudaMalloc failed"); break; }
             cudaMemcpy(dR, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice);
         }
-        const int bn = pick_bn(N);
         CUtensorMap tA, tB;
-        if (make_tmap(&tA, dA, M, K, K, GEMM_BM) || make_tmap(&tB, dW, N, K, K, bn)) break;
+        if (make_tmap(&tA, dA, M, K, K, GEMM_A_BOX_ROWS) || make_tmap(&tB, dW, N, K, K, GEMM_BN)) break;
         // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
         if (epilogue == EPI_BIAS_RESID_F32) cudaMemcpy(dO, dR, (size_t)M * N * 4, cudaMemcpyDeviceToDevice);
         GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dO; p.out2 = dO2; p.ldo = N; p.resid = (const float *)dO;
-        if (launch_gemm(nullptr, bn, epilogue, tA, tB, p, 0)) break;
+        if (launch_gemm(nullptr, epilogue, tA, tB, p, 0)) break;
         cudaError_t err = cudaDeviceSynchronize();
         if (err != cudaSuccess) { fail("GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
         if (f16out)

@@ -6,20 +6,34 @@
 // Numerics follow the reference recipe: A = activations already rounded to f16 (RNE, ggml.c:9493-9506),
 // W = the f16 weights as stored in the model file (ne0 = K contiguous, vit.cpp:531-543), fp32 accumulation.
 //
-// Structure (sm_90a): one CTA per 128 x BN tile of C, three warpgroups:
-//   warpgroup 0     TMA producer: one thread streams the 128 x 64 A tile and the BN x 64 W tile of every k-block (SWIZZLE_128B)
-//                   into a kStages-deep shared-memory ring; the other warps load the tile's bias into shared memory once and, for
-//                   the residual epilogue, prefetch the tile's residual rows into L2; its registers are handed to the MMA
-//                   warpgroups (setmaxnreg)
-//   warpgroups 1-2  MMA + epilogue: each owns 64 rows of the tile and issues 4 x wgmma.m64nBNk16 per k-block with the f32 accumulator
-//                   in registers, then applies bias / GELU / hi-lo split / residual / position embedding on those registers
-// Pipeline: per ring slot a full mbarrier (TMA transaction bytes) and an empty mbarrier (one arrival per MMA warpgroup once the
-// wgmma reading the slot has retired).
-// Staged epilogue (qkv, proj, fc1, fc2): once both MMA warpgroups' wgmmas have retired the operand ring is free; each warpgroup
-// writes its 64 result rows into it as 64-row x 128-B boxes (SWIZZLE_128B, so the fragment-layout writes are free of bank
-// conflicts) and one thread stores them with TMA.  The residual epilogue first TMA-loads its residual rows into the same boxes and
-// adds them there.  The store maps cover exactly M rows and N columns, so rows >= M and columns >= N are not written.  The patch
-// and head epilogues store straight from registers.
+// Structure (sm_90a): a persistent grid of as many two-CTA clusters as fit at once.  C is cut into 128 x 128 tiles; two
+// neighbouring column tiles form a pair, pairs are numbered with N fastest within an M band, and cluster c takes pairs c,
+// c + clusters, ..., CTA r of the cluster the column tile 2 j + r of each (a tile past N when the count is odd is computed and never
+// stored).  The two CTAs share the pair's A tile: each loads half of it into both with a TMA multicast, so a k-block moves 24 KB from
+// L2 per CTA instead of 32 KB (the 128 x 128 tile alone made the main loop L2-bandwidth bound).  Each CTA hands its tiles
+// alternately to its two MMA warpgroups (ping-pong):
+//   warpgroup 0     TMA producer: one thread streams the A half and the 128 x 64 W tile of every k-block of every tile of the CTA, in
+//                   the order the MMA warpgroups consume them, into a ring of 32 KB stages (SWIZZLE_128B); for the residual
+//                   epilogue it also prefetches each tile's residual rows into L2 when it starts the tile; before exiting it waits
+//                   until both CTAs have released every slot; its registers are handed to the MMA warpgroups (setmaxnreg)
+//   warpgroups 1-2  MMA + epilogue: each owns a whole tile at a time and issues 2 x wgmma.m64n128k16 (rows 0-63 and 64-127) per k16
+//                   step with the 128 f32 accumulators per thread in registers, then applies bias / GELU / hi-lo split / residual /
+//                   position embedding to them
+// Pipeline: per ring slot a full mbarrier (TMA transaction bytes, both A halves and the W tile) and an empty mbarrier (two arrivals:
+// the warpgroup that consumed the slot, in this CTA and in the peer, once the wgmma reading it has retired; the peer's multicast
+// writes into the slot too).  Slots and their phases run on across tile boundaries, so the ring does not drain between tiles.  The
+// two warpgroups' main loops take turns on the tensor cores through a pair of named barriers: a warpgroup starts tile i's k-loop
+// once the other one has issued tile i-1's, and runs tile i's epilogue while the other runs tile i+1's k-loop.
+// Ring depth (template STAGES, chosen by K on the host): 6 stages with 16 KB staging buffers for K >= GEMM_DEEP_K, whose main loop
+// dominates and needs the deeper ring to hide its load latency; 5 stages with 32 KB buffers otherwise, where the epilogue's share
+// is larger and fewer, larger passes shorten it.
+// Staged epilogue (qkv, proj, fc1, fc2): each MMA warpgroup has its own staging buffer outside the ring.  The tile leaves in passes
+// of one 64-row half x 64 or 128 columns: the warpgroup writes a pass as 64-row x 128-B boxes (SWIZZLE_128B, so the fragment-layout
+// writes are free of bank conflicts) and one thread stores them with TMA.  A pass reuses buffer space only once the stores of the
+// pass that used it have read it.  The residual epilogue first TMA-loads the pass's residual rows into the same boxes and adds them
+// there; the first pass's residual is loaded at tile start, under the k-loop.  The store maps cover exactly M rows and N columns,
+// so rows >= M and columns >= N are not written; a tile reads and writes only its own rows and columns, so the residual may alias
+// the output.  The patch and head epilogues store straight from registers.
 #pragma once
 #include "ptx.cuh"
 
@@ -52,20 +66,28 @@ struct GemmParams
     int np, ntok;       // EPI_PATCH_F32: patches / tokens per image
 };
 
-constexpr int GEMM_BM = 128;
+constexpr int GEMM_BM = 128; // rows of a tile
+constexpr int GEMM_BN = 128; // columns of a tile (the W map's box rows)
+constexpr int GEMM_A_BOX_ROWS = GEMM_BM / 2; // the A map's box: each CTA of a cluster pair loads half of the A tile they share
 constexpr int GEMM_BK = 64;
 
-template <int BN>
+// Shared memory holds six 32 KB ring stages and two 16 KB staging buffers, or five stages and two 32 KB buffers.  A long reduction
+// (K >= GEMM_DEEP_K) is main-loop bound and wants the deeper ring to hide the L2 latency of its loads; a short one spends a larger
+// share in the epilogue, which wants the larger buffer (fewer store / residual round trips per tile).
+constexpr int GEMM_DEEP_K = 2048;
+
+template <int STAGES>
 struct GemmCfg
 {
+    static_assert(STAGES == 5 || STAGES == 6, "ring depth");
     static constexpr int kThreads = 384;                 // producer warpgroup + two MMA warpgroups
     static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-    static constexpr int B_BYTES = BN * GEMM_BK * 2;
+    static constexpr int B_BYTES = GEMM_BN * GEMM_BK * 2;
+    static constexpr int kStages = STAGES;               // operand ring depth
+    static constexpr int kStageBytes = STAGES == 6 ? 16384 : 32768; // epilogue staging buffer per MMA warpgroup
     static constexpr int kSmemLimit = 232448;            // 227 KB per CTA
-    static constexpr int kStagesFit = (kSmemLimit - 1024 - 256) / (A_BYTES + B_BYTES);
-    static constexpr int kStages = kStagesFit > 6 ? 6 : kStagesFit; // operand ring depth: whatever fits, at most 6
-    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + kStages * (A_BYTES + B_BYTES) + 256 /*barriers*/;
-    static_assert(SMEM_BYTES <= kSmemLimit, "exceeds the 227 KB per-CTA shared memory limit");
+    static constexpr int SMEM_BYTES = 1024 /*align slack*/ + kStages * (A_BYTES + B_BYTES) + 2 * kStageBytes + 256 /*barriers*/;
+    static_assert(SMEM_BYTES + 2 * GEMM_BN * 4 /*s_bias*/ <= kSmemLimit, "exceeds the 227 KB per-CTA shared memory limit");
 };
 
 // GELU, tanh form (the reference's formula, ggml.c:1418-1424) on an f16-valued input, evaluated in f32 as
@@ -80,62 +102,76 @@ __device__ __forceinline__ float gelu_tanh_f32(float x)
     return x * ptx::rcp_approx(1.0f + e);
 }
 
-template <int BN>
-__device__ __forceinline__ void wgmma_k16(float (&acc)[BN / 2], uint64_t adesc, uint64_t bdesc, uint32_t accumulate)
-{
-    if constexpr (BN == 256) ptx::wgmma_m64n256k16_f16(acc, adesc, bdesc, accumulate);
-    else ptx::wgmma_m64n128k16_f16(acc, adesc, bdesc, accumulate);
-}
-
 // Epilogues whose result goes out through shared memory and TMA stores (the rest store from registers)
 __host__ __device__ constexpr bool gemm_epi_staged(int epi)
 {
     return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32;
 }
 
-// Staged-epilogue geometry: each MMA warpgroup's 64 x BN result leaves as boxes of 64 rows x 128 B (64 f16 or 32 f32 columns),
-// one box set per output tensor (hi and lo for EPI_BIAS_F16_HILO), in the operand ring it no longer needs
-template <int BN, int EPI>
+// Staged-epilogue geometry: a warpgroup's 128 x 128 result leaves in passes of one 64-row half x kPassCols columns; a pass is
+// kColBoxes boxes of 64 rows x 128 B (64 f16 or 32 f32 columns) per output tensor (hi and lo for EPI_BIAS_F16_HILO) and fills the
+// staging buffer
+template <int EPI, int STAGES>
 struct GemmStage
 {
+    using Cfg = GemmCfg<STAGES>;
     static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO);
-    static constexpr int kBoxCols = kF16 ? 64 : 32;
-    static constexpr int kBoxes = BN / kBoxCols;   // boxes per output tensor and warpgroup
-    static constexpr int kBoxBytes = 64 * 128;
     static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
-    static constexpr int kWgBytes = kOuts * kBoxes * kBoxBytes;
-    static_assert(2 * kWgBytes <= GemmCfg<BN>::kStages * (GemmCfg<BN>::A_BYTES + GemmCfg<BN>::B_BYTES), "staged tile exceeds the ring");
+    static constexpr int kBoxCols = kF16 ? 64 : 32;
+    static constexpr int kBoxBytes = 64 * 128;
+    static constexpr int kFitCols = Cfg::kStageBytes / (64 * kOuts * (kF16 ? 2 : 4));
+    static constexpr int kPassCols = kFitCols < GEMM_BN ? kFitCols : GEMM_BN; // 16 KB: 128 (f16), 64 (hi + lo, f32); 32 KB: 128
+    static constexpr int kColGroups = GEMM_BN / kPassCols;
+    static constexpr int kPasses = 2 * kColGroups; // row half outer, column group inner
+    static constexpr int kColBoxes = kPassCols / kBoxCols;
+    static constexpr int kPassBytes = kOuts * kColBoxes * kBoxBytes;
+    static constexpr int kSlots = Cfg::kStageBytes / kPassBytes; // passes the buffer holds at once (2: f16 in 32 KB)
+    static_assert(kSlots * kPassBytes == Cfg::kStageBytes, "passes tile the staging buffer");
+    // offset of box (output o, column box c) in the staging buffer
+    __host__ __device__ static constexpr uint32_t box(int o, int c) { return (uint32_t)((o * kColBoxes + c) * kBoxBytes); }
 };
 
 // tmOut: the store map of out (f16: box 64 columns x 64 rows, 2-D [M][N] or, head-major, 3-D {64, M, N / 64 planes}; f32: box
 // 32 columns x 64 rows over [M][N]), SWIZZLE_128B.  tmAux: the same map over out2 (EPI_BIAS_F16_HILO) or the load map of resid
 // (EPI_BIAS_RESID_F32).  Both unused by the register epilogues.
-template <int BN, int EPI>
+template <int EPI, int STAGES>
 __global__ void __launch_bounds__(384, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
                   const __grid_constant__ CUtensorMap tmAux, const GemmParams p)
 {
-    static_assert(BN == 128 || BN == 256, "BN");
-    using Cfg = GemmCfg<BN>;
+    using Cfg = GemmCfg<STAGES>;
     constexpr int kStages = Cfg::kStages;
     constexpr bool kStaged = gemm_epi_staged(EPI);
+    constexpr int kBarTurn = 1; // + warpgroup: named barrier "this warpgroup may start its next k-loop"
+    constexpr int kBarWg = 3;   // + warpgroup: the warpgroup's own epilogue barrier
 
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(16) float s_bias[BN]; // the tile's bias, zero past N
+    __shared__ __align__(16) float s_bias[2][GEMM_BN]; // per MMA warpgroup: its current tile's bias, zero past N
     const uint32_t smem_base = (ptx::smem_u32(smem_raw) + 1023u) & ~1023u; // SWIZZLE_128B wants 1024-B aligned tiles
     const uint32_t sA = smem_base;
     const uint32_t sB = sA + kStages * Cfg::A_BYTES;
-    const uint32_t bars = sB + kStages * Cfg::B_BYTES;
+    const uint32_t sStage = sB + kStages * Cfg::B_BYTES;
+    const uint32_t bars = sStage + 2 * Cfg::kStageBytes;
     auto full_bar = [&](int s) { return bars + 8u * s; };
     auto empty_bar = [&](int s) { return bars + 8u * (kStages + s); };
-    const uint32_t bias_bar = bars + 8u * (2 * kStages);
-    auto resid_bar = [&](int cw) { return bars + 8u * (2 * kStages + 1 + cw); };
+    auto resid_bar = [&](int cw) { return bars + 8u * (2 * kStages + cw); };
+    using St = GemmStage<EPI, STAGES>;
+    // EPI_BIAS_RESID_F32: TMA-load the residual of one pass (64 rows from `row`, the column boxes from c0 that start inside N) into
+    // the staging buffer `dst` of warpgroup cw, completing on resid_bar(cw); partial boxes are zero-filled and count in full
+    auto resid_load = [&](uint32_t dst, int c0, int row, int cw) {
+        const int ncb = min(St::kColBoxes, (p.N - c0 + St::kBoxCols - 1) / St::kBoxCols);
+        ptx::mbar_arrive_expect_tx(resid_bar(cw), ncb * St::kBoxBytes);
+        for (int c = 0; c < ncb; ++c) ptx::tma_load_2d(dst + St::box(0, c), &tmAux, resid_bar(cw), c0 + 32 * c, row);
+    };
 
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-    const int n_tiles = (p.N + BN - 1) / BN;
-    const int m_blk = blockIdx.x / n_tiles, n_blk = blockIdx.x - m_blk * n_tiles;
+    // the two CTAs of a cluster take the two column tiles of a pair (a tile past N when the count is odd: computed, never stored)
+    const unsigned rank = ptx::cluster_ctarank();
+    const unsigned cluster = blockIdx.x >> 1, clusters = gridDim.x >> 1;
+    const unsigned n_pairs = (unsigned)(p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN);
+    // pair u exists (its M band starts inside M); tested against p.M rather than a pair count, which would hold a register
+    auto pair_exists = [&](unsigned u) { return (int)(u / n_pairs) * GEMM_BM < p.M; };
     const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
-    const int m0 = m_blk * GEMM_BM, n0 = n_blk * BN;
 
     if (threadIdx.x == 0)
     {
@@ -149,14 +185,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int s = 0; s < kStages; ++s)
         {
             ptx::mbar_init(full_bar(s), 1);
-            ptx::mbar_init(empty_bar(s), 2); // one arrival per MMA warpgroup
+            ptx::mbar_init(empty_bar(s), 2); // the MMA warpgroup that consumed the slot, in this CTA and in the peer
         }
-        ptx::mbar_init(bias_bar, 96); // producer warps 1-3
         ptx::mbar_init(resid_bar(0), 1);
         ptx::mbar_init(resid_bar(1), 1);
         ptx::fence_barrier_init();
     }
-    __syncthreads();
+    ptx::cluster_sync(); // the peer multicasts into this CTA's ring and arrives on its empty barriers
     // prologue done (it overlapped the previous kernel's tail under PDL); from here on the kernel touches upstream data
     ptx::grid_dep_launch();
     ptx::grid_dep_wait();
@@ -167,176 +202,231 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ptx::setmaxnreg_dec<40>();
         if (tid == 0)
         {
-            for (int kb = 0; kb < num_kb; ++kb)
+            int s = 0;
+            uint32_t ph = 0;
+            for (unsigned u = cluster; pair_exists(u); u += clusters)
             {
-                const int s = kb % kStages;
-                ptx::mbar_wait(empty_bar(s), ((kb / kStages) & 1) ^ 1);
-                // out-of-range rows / columns are zero-filled and still count their bytes
-                ptx::mbar_arrive_expect_tx(full_bar(s), Cfg::A_BYTES + Cfg::B_BYTES);
-                ptx::tma_load_2d(sA + s * Cfg::A_BYTES, &tmA, full_bar(s), kb * GEMM_BK, m0);
-                ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * GEMM_BK, n0);
-            }
-        }
-        else if (tid >= 32)
-        {
-            if constexpr (EPI == EPI_BIAS_RESID_F32)
-            {
-                // the residual rows are read once, by the epilogue: start pulling them into L2 while the main loop runs
-                if (tid == 32)
+                const unsigned m_blk = u / n_pairs;
+                const int m0 = (int)m_blk * GEMM_BM, n0 = (int)(2 * (u - m_blk * n_pairs) + rank) * GEMM_BN;
+                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                {
+                    // the residual rows are read once, by the epilogue: start pulling them into L2 while the tile's main loop runs
                     for (int h = 0; h < 2; ++h)
                         if (m0 + 64 * h < p.M)
-                            for (int c = n0; c < min(n0 + BN, p.N); c += 32) ptx::tma_prefetch_2d(&tmAux, c, m0 + 64 * h);
+                            for (int c = n0; c < min(n0 + GEMM_BN, p.N); c += 32) ptx::tma_prefetch_2d(&tmAux, c, m0 + 64 * h);
+                }
+                for (int kb = 0; kb < num_kb; ++kb)
+                {
+                    ptx::mbar_wait(empty_bar(s), ph ^ 1); // free in both CTAs: the A half below lands in both
+                    // out-of-range rows / columns are zero-filled and still count their bytes; the A tile is shared by the pair,
+                    // each CTA loads 64 of its rows into both CTAs
+                    ptx::mbar_arrive_expect_tx(full_bar(s), Cfg::A_BYTES + Cfg::B_BYTES);
+                    ptx::tma_load_2d_multicast(sA + s * Cfg::A_BYTES + rank * (Cfg::A_BYTES / 2), &tmA, full_bar(s), kb * GEMM_BK,
+                                               m0 + rank * GEMM_A_BOX_ROWS, 0x3);
+                    ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * GEMM_BK, n0);
+                    if (++s == kStages) { s = 0; ph ^= 1; }
+                }
             }
-            for (int c = tid - 32; c < BN; c += 96) s_bias[c] = n0 + c < p.N ? __ldg(p.bias + n0 + c) : 0.f;
-            ptx::mbar_arrive(bias_bar);
+            // every slot released by both CTAs: no arrival from the peer is still on its way when this CTA exits
+            for (int k = 0; k < kStages; ++k)
+            {
+                ptx::mbar_wait(empty_bar(s), ph ^ 1);
+                if (++s == kStages) { s = 0; ph ^= 1; }
+            }
         }
         return;
     }
 
     // ===================== MMA warpgroups =====================
     ptx::setmaxnreg_inc<232>();
-    const int cw = wg - 1; // rows 64 cw .. 64 cw + 63 of the tile
-    float acc[BN / 2];
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < num_kb; ++kb)
-    {
-        const int s = kb % kStages;
-        ptx::mbar_wait(full_bar(s), (kb / kStages) & 1);
-        const uint64_t adesc = ptx::wgmma_desc_kmajor_sw128(sA + s * Cfg::A_BYTES + cw * 64 * 128);
-        const uint64_t bdesc = ptx::wgmma_desc_kmajor_sw128(sB + s * Cfg::B_BYTES);
-        ptx::fence_regs(acc);
-        ptx::wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) wgmma_k16<BN>(acc, adesc + 2 * k, bdesc + 2 * k, (kb | k) != 0); // +32 B along K
-        ptx::wgmma_commit();
-        ptx::wgmma_wait<1>(); // the previous k-block's MMAs have retired: its slot can be refilled
-        ptx::fence_regs(acc);
-        if (kb > 0 && tid == 0) ptx::mbar_arrive(empty_bar((kb - 1) % kStages));
-    }
-    ptx::wgmma_wait<0>();
-    ptx::fence_regs(acc);
-    ptx::mbar_wait(bias_bar, 0);
-
+    const int cw = wg - 1;
     // wgmma m64nN layout: thread (warp w, lane l) holds rows 16 w + l / 4 (+ 8) and, per 8-column group j, columns 8 j + 2 (l % 4) (+ 1)
     const int warp = tid >> 5, lane = tid & 31;
-    if constexpr (kStaged)
+    uint32_t resid_ph = 0;
+    float acc[2][GEMM_BN / 2]; // rows 0-63 and 64-127 of the tile
+    // i: the tile's place in this CTA's sequence; tiles i and i + 1 go to different warpgroups
+    for (unsigned i = cw, u = cluster + cw * clusters; pair_exists(u); i += 2, u += 2 * clusters)
     {
-        // ===================== staged epilogue: registers -> swizzled boxes in the free ring -> TMA stores =====================
-        using St = GemmStage<BN, EPI>;
-        const int wm0 = m0 + cw * 64;                                                  // first row of this warpgroup
-        const bool live = wm0 < p.M;                                                   // any of its rows inside M
-        const int nbox = min(St::kBoxes, (p.N - n0 + St::kBoxCols - 1) / St::kBoxCols); // boxes that start inside N
-        const uint32_t stage = smem_base + cw * St::kWgBytes;
-        ptx::named_bar_sync(1, 256); // both warpgroups' wgmmas have retired: nothing reads the ring any more
-        if constexpr (EPI == EPI_BIAS_RESID_F32)
+        const unsigned m_blk = u / n_pairs;
+        const int m0 = (int)m_blk * GEMM_BM, n0 = (int)(2 * (u - m_blk * n_pairs) + rank) * GEMM_BN;
+        const float bias_v = n0 + tid < p.N ? __ldg(p.bias + n0 + tid) : 0.f; // lands while the other warpgroup's k-loop runs
+        if constexpr (kStaged)
         {
-            if (live)
+            // the staging buffer is free once the previous tile's last stores have read it (that overlaps the wait for this
+            // warpgroup's turn); the residual of the first pass then lands in it while the k-loop runs
+            if (tid == 0)
             {
+                ptx::tma_store_wait_read<0>();
+                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                    if (n0 < p.N) resid_load(sStage + cw * Cfg::kStageBytes, n0, m0, cw);
+            }
+        }
+
+        // the tile's k-blocks sit at positions i * num_kb ... of the ring sequence
+        const int g0 = i * num_kb;
+        int s = g0 % kStages, s_prev = 0;
+        uint32_t ph = (uint32_t)(g0 / kStages) & 1;
+        if (i > 0) ptx::named_bar_sync(kBarTurn + cw, 256); // the other warpgroup has issued tile i-1's k-loop
+        // every earlier reader of s_bias[cw] (tile i-2's epilogue) passed the barrier above before this write
+        s_bias[cw][tid] = bias_v;
+        for (int kb = 0; kb < num_kb; ++kb)
+        {
+            ptx::mbar_wait(full_bar(s), ph);
+            const uint64_t adesc0 = ptx::wgmma_desc_kmajor_sw128(sA + s * Cfg::A_BYTES);
+            const uint64_t adesc1 = ptx::wgmma_desc_kmajor_sw128(sA + s * Cfg::A_BYTES + 64 * 128);
+            const uint64_t bdesc = ptx::wgmma_desc_kmajor_sw128(sB + s * Cfg::B_BYTES);
+            ptx::fence_regs(acc[0]);
+            ptx::fence_regs(acc[1]);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < GEMM_BK / 16; ++k) // +32 B along K per k16 step
+            {
+                ptx::wgmma_m64n128k16_f16(acc[0], adesc0 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                ptx::wgmma_m64n128k16_f16(acc[1], adesc1 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<1>(); // the previous k-block's MMAs have retired: its slot can be refilled
+            ptx::fence_regs(acc[0]);
+            ptx::fence_regs(acc[1]);
+            if (kb > 0 && tid == 0) { ptx::mbar_arrive(empty_bar(s_prev)); ptx::mbar_arrive_cluster(empty_bar(s_prev), rank ^ 1); }
+            s_prev = s;
+            if (++s == kStages) { s = 0; ph ^= 1; }
+        }
+        if (pair_exists(u + clusters)) ptx::named_bar_arrive(kBarTurn + (cw ^ 1), 256); // tile i+1 may start its k-loop
+        ptx::wgmma_wait<0>();
+        ptx::fence_regs(acc[0]);
+        ptx::fence_regs(acc[1]);
+        if (tid == 0) { ptx::mbar_arrive(empty_bar(s_prev)); ptx::mbar_arrive_cluster(empty_bar(s_prev), rank ^ 1); }
+
+        if constexpr (kStaged)
+        {
+            // ===================== staged epilogue: registers -> swizzled boxes -> TMA stores =====================
+            const uint32_t stage = sStage + cw * Cfg::kStageBytes;
+            // row r of a box lives at r * 128 B with its 16-B chunks permuted by chunk ^ (r % 8); r % 8 == lane / 4 for every row here
+            const int rr = warp * 16 + (lane >> 2), sw = lane >> 2, q = lane & 3;
+#pragma unroll
+            for (int ps = 0; ps < St::kPasses; ++ps)
+            {
+                const int hm = ps / St::kColGroups, cg = ps % St::kColGroups; // rows 64 hm .., columns cg * kPassCols ..
+                const int c0 = n0 + cg * St::kPassCols;
+                if (c0 >= p.N || m0 + 64 * hm >= p.M) continue; // nothing of this pass is stored (uniform over the warpgroup)
+                const int ncb = min(St::kColBoxes, (p.N - c0 + St::kBoxCols - 1) / St::kBoxCols); // boxes that start inside N
+                const uint32_t buf = stage + (ps % St::kSlots) * St::kPassBytes;
+                if (ps > 0 && tid == 0)
+                {
+                    if (ps >= St::kSlots) ptx::tma_store_wait_read<St::kSlots - 1>(); // the stores of the pass that used buf have read it
+                    if constexpr (EPI == EPI_BIAS_RESID_F32) resid_load(buf, c0, m0 + 64 * hm, cw);
+                }
+                ptx::named_bar_sync(kBarWg + cw, 128); // pass 0: s_bias[cw] is written
+                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                {
+                    ptx::mbar_wait(resid_bar(cw), resid_ph);
+                    resid_ph ^= 1;
+                }
+#pragma unroll
+                for (int jj = 0; jj < St::kPassCols / 8; ++jj)
+                {
+                    const int j = cg * (St::kPassCols / 8) + jj; // 8-column group of the tile
+                    const float2 b = *reinterpret_cast<const float2 *>(&s_bias[cw][8 * j + 2 * q]);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                    {
+                        const float x0 = __fadd_rn(acc[hm][4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[hm][4 * j + 2 * h + 1], b.y);
+                        const uint32_t row = buf + (uint32_t)(rr + 8 * h) * 128u;
+                        if constexpr (St::kF16)
+                        {
+                            const uint32_t a = row + (((jj % 8) ^ sw) << 4) + 4 * q;
+                            __half2 hv;
+                            if constexpr (EPI == EPI_BIAS_GELU_F16)
+                            {
+                                const float2 r = __half22float2(__floats2half2_rn(x0, x1)); // ggml.c:1434-1441: y = f16(gelu(f32(f16(x))))
+                                hv = __floats2half2_rn(gelu_tanh_f32(r.x), gelu_tanh_f32(r.y));
+                            }
+                            else hv = __floats2half2_rn(x0, x1);
+                            ptx::st_shared_b32(a + St::box(0, jj / 8), *reinterpret_cast<const uint32_t *>(&hv));
+                            if constexpr (EPI == EPI_BIAS_F16_HILO)
+                            {
+                                const float2 hf = __half22float2(hv); // lo = f16(x - hi): exact difference, |lo| <= 2^-11 |x|
+                                const __half2 lo = __floats2half2_rn(__fsub_rn(x0, hf.x), __fsub_rn(x1, hf.y));
+                                ptx::st_shared_b32(a + St::box(1, jj / 8), *reinterpret_cast<const uint32_t *>(&lo));
+                            }
+                        }
+                        else
+                        {
+                            const uint32_t a = row + St::box(0, jj / 4) + (((2 * (jj % 4) + (q >> 1)) ^ sw) << 4) + 8 * (q & 1);
+                            if constexpr (EPI == EPI_BIAS_RESID_F32)
+                            {
+                                const float2 r = ptx::ld_shared_v2_f32(a); // (mul_mat + b) + inpL, vit.cpp:869,873
+                                ptx::st_shared_v2_f32(a, __fadd_rn(x0, r.x), __fadd_rn(x1, r.y));
+                            }
+                            else ptx::st_shared_v2_f32(a, x0, x1);
+                        }
+                    }
+                }
+                ptx::fence_proxy_async_smem(); // the writes above are seen by the TMA engine
+                ptx::named_bar_sync(kBarWg + cw, 128);
                 if (tid == 0)
                 {
-                    ptx::mbar_arrive_expect_tx(resid_bar(cw), nbox * St::kBoxBytes); // partial boxes count in full (zero fill)
-                    for (int b = 0; b < nbox; ++b) ptx::tma_load_2d(stage + b * St::kBoxBytes, &tmAux, resid_bar(cw), n0 + 32 * b, wm0);
-                }
-                ptx::mbar_wait(resid_bar(cw), 0);
-            }
-        }
-        // row r of a box lives at r * 128 B with its 16-B chunks permuted by chunk ^ (r % 8); r % 8 == lane / 4 for every row here
-        const int rr = warp * 16 + (lane >> 2), sw = lane >> 2, q = lane & 3;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j)
-        {
-            const float2 b = *reinterpret_cast<const float2 *>(&s_bias[8 * j + 2 * q]);
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-            {
-                const uint32_t row = stage + (uint32_t)(rr + 8 * h) * 128u;
-                const float x0 = __fadd_rn(acc[4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
-                if constexpr (St::kF16)
-                {
-                    const uint32_t a = row + (j / 8) * St::kBoxBytes + (((j % 8) ^ sw) << 4) + 4 * q;
-                    __half2 hv;
-                    if constexpr (EPI == EPI_BIAS_GELU_F16)
+                    const int row = m0 + 64 * hm;
+                    for (int c = 0; c < ncb; ++c)
                     {
-                        const float2 r = __half22float2(__floats2half2_rn(x0, x1)); // ggml.c:1434-1441: y = f16(gelu(f32(f16(x))))
-                        hv = __floats2half2_rn(gelu_tanh_f32(r.x), gelu_tanh_f32(r.y));
+                        const uint32_t src = buf + St::box(0, c);
+                        if constexpr (St::kF16)
+                        {
+                            if (p.headmajor)
+                            {
+                                const int plane = (c0 >> 6) + c;
+                                ptx::tma_store_3d(&tmOut, src, 0, row, plane);
+                                if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_3d(&tmAux, buf + St::box(1, c), 0, row, plane);
+                            }
+                            else
+                            {
+                                ptx::tma_store_2d(&tmOut, src, c0 + 64 * c, row);
+                                if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_2d(&tmAux, buf + St::box(1, c), c0 + 64 * c, row);
+                            }
+                        }
+                        else ptx::tma_store_2d(&tmOut, src, c0 + 32 * c, row);
                     }
-                    else hv = __floats2half2_rn(x0, x1);
-                    ptx::st_shared_b32(a, *reinterpret_cast<const uint32_t *>(&hv));
-                    if constexpr (EPI == EPI_BIAS_F16_HILO)
-                    {
-                        const float2 hf = __half22float2(hv); // lo = f16(x - hi): exact difference, |lo| <= 2^-11 |x|
-                        const __half2 lo = __floats2half2_rn(__fsub_rn(x0, hf.x), __fsub_rn(x1, hf.y));
-                        ptx::st_shared_b32(a + St::kBoxes * St::kBoxBytes, *reinterpret_cast<const uint32_t *>(&lo));
-                    }
-                }
-                else
-                {
-                    const uint32_t a = row + (j / 4) * St::kBoxBytes + (((2 * (j % 4) + (q >> 1)) ^ sw) << 4) + 8 * (q & 1);
-                    if constexpr (EPI == EPI_BIAS_RESID_F32)
-                    {
-                        const float2 r = ptx::ld_shared_v2_f32(a); // (mul_mat + b) + inpL, vit.cpp:869,873
-                        ptx::st_shared_v2_f32(a, __fadd_rn(x0, r.x), __fadd_rn(x1, r.y));
-                    }
-                    else ptx::st_shared_v2_f32(a, x0, x1);
+                    ptx::tma_store_commit();
                 }
             }
         }
-        ptx::fence_proxy_async_smem(); // the writes above are seen by the TMA engine
-        ptx::named_bar_sync(2 + cw, 128);
-        if (tid == 0 && live)
+        else
         {
-            for (int b = 0; b < nbox; ++b)
+            // ===================== register epilogue (patch embedding, head) =====================
+            ptx::named_bar_sync(kBarWg + cw, 128); // s_bias[cw] is written
+            const int col0 = n0 + 2 * (lane & 3);
+#pragma unroll
+            for (int hm = 0; hm < 2; ++hm)
             {
-                const uint32_t src = stage + b * St::kBoxBytes;
-                if constexpr (St::kF16)
+                const int row0 = m0 + 64 * hm + warp * 16 + (lane >> 2);
+#pragma unroll
+                for (int j = 0; j < GEMM_BN / 8; ++j)
                 {
-                    if (p.headmajor)
+                    const int col = col0 + 8 * j;
+                    if (col >= p.N) continue; // N % 4 == 0: a column pair is all-in or all-out
+                    const float2 b = *reinterpret_cast<const float2 *>(&s_bias[cw][col - n0]);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
                     {
-                        const int plane = (n0 >> 6) + b;
-                        ptx::tma_store_3d(&tmOut, src, 0, wm0, plane);
-                        if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_3d(&tmAux, src + St::kBoxes * St::kBoxBytes, 0, wm0, plane);
-                    }
-                    else
-                    {
-                        ptx::tma_store_2d(&tmOut, src, n0 + 64 * b, wm0);
-                        if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_2d(&tmAux, src + St::kBoxes * St::kBoxBytes, n0 + 64 * b, wm0);
+                        const int row = row0 + 8 * h;
+                        if (row >= p.M) continue;
+                        const float x0 = __fadd_rn(acc[hm][4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[hm][4 * j + 2 * h + 1], b.y);
+                        if constexpr (EPI == EPI_PATCH_F32)
+                        {
+                            const int img = row / p.np, pp = row - img * p.np;
+                            const float2 pe = __ldg(reinterpret_cast<const float2 *>(p.pos + (size_t)(1 + pp) * p.N + col));
+                            *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + ((size_t)img * p.ntok + 1 + pp) * p.ldo + col) =
+                                make_float2(__fadd_rn(x0, pe.x), __fadd_rn(x1, pe.y));
+                        }
+                        else *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)row * p.ldo + col) = make_float2(x0, x1);
                     }
                 }
-                else ptx::tma_store_2d(&tmOut, src, n0 + 32 * b, wm0);
-            }
-            ptx::tma_store_commit();
-            ptx::tma_store_wait_read<0>(); // the shared memory must outlive the reads of the stores
-        }
-    }
-    else
-    {
-        // ===================== register epilogue (patch embedding, head) =====================
-        const int row0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
-        const int col0 = n0 + 2 * (lane & 3);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j)
-        {
-            const int col = col0 + 8 * j;
-            if (col >= p.N) continue; // N % 4 == 0: a column pair is all-in or all-out
-            const float2 b = *reinterpret_cast<const float2 *>(&s_bias[col - n0]);
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-            {
-                const int row = row0 + 8 * h;
-                if (row >= p.M) continue;
-                const float x0 = __fadd_rn(acc[4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[4 * j + 2 * h + 1], b.y);
-                if constexpr (EPI == EPI_PATCH_F32)
-                {
-                    const int img = row / p.np, pp = row - img * p.np;
-                    const float2 pe = __ldg(reinterpret_cast<const float2 *>(p.pos + (size_t)(1 + pp) * p.N + col));
-                    *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + ((size_t)img * p.ntok + 1 + pp) * p.ldo + col) =
-                        make_float2(__fadd_rn(x0, pe.x), __fadd_rn(x1, pe.y));
-                }
-                else *reinterpret_cast<float2 *>(reinterpret_cast<float *>(p.out) + (size_t)row * p.ldo + col) = make_float2(x0, x1);
             }
         }
     }
+    if constexpr (kStaged)
+        if (tid == 0) ptx::tma_store_wait_read<0>(); // the shared memory must outlive the reads of the last stores
 }
 
 } // namespace vitb200
