@@ -128,6 +128,25 @@ int vitb200_forward_u8(vitb200_engine *e, const uint8_t *const *images, const in
 int vitb200_forward_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                              float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k);
 
+/* Text recognition with a ViTSTR model (1-channel, head_tokens >= 2; reference extensions/vitstr.cpp), image to text on the GPU:
+ * the extension's vit_image_preprocess (vitstr.cpp:128-201: grayscale in double, its own bilinear resize to img^2 with no half-pixel
+ * offset, (v / 255 - 0.5) * 2), the forward pass, and its greedy decode (vitstr.cpp:1020-1054: the arg-max of token rows
+ * 1 .. head_tokens-1, lowest class id among equal maxima, stopping at the first row whose arg-max is class 1 = [s]).
+ * `images[b]` is interleaved RGB u8, nx[b] x ny[b] pixels with nx, ny >= 2, as the extension's load_image_from_file produces
+ * (vitstr.cpp:107-125).  Outputs (host, any of them may be NULL; all NULL = preprocess only):
+ *   images_f32_out  float32 [batch][img][img]   the pre-processed images (the extension's image_f32)
+ *   chars           int32   [batch][head_tokens - 1]  decoded class ids, -1 past the end of the string (id2label gives the text)
+ *   lengths         int32   [batch]             characters before [s] (head_tokens - 1 if it never wins)
+ *   scores          double  [batch]             the extension's `conf`: the product of the emitted maxima, in token order; 1 if empty
+ *   probs           float32 [batch][head_tokens][num_classes]  as vitb200_forward returns them for this model
+ * vitb200_recognize_u8_async follows vitb200_forward_u8_async's buffer rules (images are copied inside the call; outputs must stay
+ * valid until vitb200_sync()) and shares its two pipeline slots; vitb200_recognize_u8 == the async form + vitb200_sync, plus the
+ * optional f32 read-back. */
+int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, float *images_f32_out,
+                         int32_t *chars, int32_t *lengths, double *scores, float *probs);
+int vitb200_recognize_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int32_t *chars,
+                               int32_t *lengths, double *scores, float *probs);
+
 /* Same with DEVICE buffers on the engine's device, enqueued on `stream` (a cudaStream_t; NULL = the engine's own
  * stream) without synchronising: the caller owns ordering.  This is the resident-data path bench.py times. */
 int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, float *d_probs, float *d_logits,

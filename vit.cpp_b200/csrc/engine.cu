@@ -184,6 +184,10 @@ struct vitb200_engine
     // followed by the per-image descriptors) and its device twin; grown only when a batch needs more than any batch before it
     uint8_t *h_u8[2] = {nullptr, nullptr}, *d_u8[2] = {nullptr, nullptr};
     size_t u8_cap[2] = {0, 0};
+    // text recognition (vitb200_recognize_u8*, 1-channel models with head_tokens >= 2): per pipeline slot the decoded class ids
+    // [max_batch][head_tokens - 1], lengths [max_batch] and scores [max_batch]
+    int32_t *d_chars_slot[2] = {nullptr, nullptr}, *d_len_slot[2] = {nullptr, nullptr};
+    double *d_score_slot[2] = {nullptr, nullptr};
     // CUDA-graph cache for the kernel schedule of one forward, keyed by its arguments (launch-bound inner loop: ~90 kernels)
     struct GraphEntry { GraphKey key; int state; int launches; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -1059,6 +1063,11 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         dev_alloc(e, &e->d_logits_slot[1], R * hp->num_classes) || dev_alloc(e, &e->d_topk_idx_slot[1], R * e->max_k) ||
         dev_alloc(e, &e->d_topk_val_slot[1], R * e->max_k))
         return bail(1);
+    if (e->C == 1 && e->head_tokens >= 2)
+        for (int i = 0; i < 2; ++i)
+            if (dev_alloc(e, &e->d_chars_slot[i], B * (e->head_tokens - 1)) || dev_alloc(e, &e->d_len_slot[i], B) ||
+                dev_alloc(e, &e->d_score_slot[i], B))
+                return bail(1);
     if (cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
     for (int i = 0; i < 2; ++i)
         if (cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming) != cudaSuccess ||
@@ -1445,10 +1454,10 @@ int vitb200_features(vitb200_engine *e, const float *images, int batch, const vi
 // vitb200_forward_async: the caller's images are packed into this slot's pinned staging buffer, ONE host-to-device copy on the copy
 // stream overlaps the previous call's kernels, nothing synchronises on entry and nothing is allocated once the staging buffers
 // have grown to the largest batch seen.
-// preprocess_u8 is the part up to the patch matrix (and the optional f32 read-back); the caller records ev_done[sl] after its last
-// use of the slot.
-static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
-                         float *images_f32_out, int &sl)
+// stage_u8 packs the images into this call's slot and makes the compute stream wait for their copy (d_u8[sl] holds the pixels,
+// then the PreImage table at table_off); preprocess_u8 adds the RGB kernel up to the patch matrix (and the optional f32 read-back).
+// The caller records ev_done[sl] after its last use of the slot.
+static int stage_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int &sl, size_t &table_off)
 {
     size_t total = 0;
     for (int b = 0; b < batch; ++b)
@@ -1456,7 +1465,7 @@ static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const 
         if (!images[b] || nx[b] < 1 || ny[b] < 1) return fail("image %d: bad pointer or size", b);
         total += ((size_t)nx[b] * ny[b] * 3 + 255) / 256 * 256;
     }
-    const size_t table_off = total;
+    table_off = total;
     total += (size_t)batch * sizeof(PreImage);
     CUDA_TRY(cudaSetDevice(e->device));
     sl = (int)(e->submits & 1);
@@ -1485,6 +1494,15 @@ static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const 
     CUDA_TRY(cudaMemcpyAsync(e->d_u8[sl], e->h_u8[sl], total, cudaMemcpyHostToDevice, cs));
     CUDA_TRY(cudaEventRecord(e->ev_h2d[sl], cs));
     CUDA_TRY(cudaStreamWaitEvent(s, e->ev_h2d[sl], 0));
+    return 0;
+}
+
+static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                         float *images_f32_out, int &sl)
+{
+    size_t table_off = 0;
+    if (stage_u8(e, images, nx, ny, batch, sl, table_off)) return 1;
+    cudaStream_t s = e->stream;
     const int S = e->hp.img_size;
     dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
     float *d_f32 = images_f32_out ? e->d_img_slot[sl] : nullptr;
@@ -1555,6 +1573,75 @@ int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const i
     e->launches += 1; // the preprocess kernel
     CUDA_TRY(cudaEventRecord(e->ev_done[sl], e->stream));
     e->submits++;
+    return vitb200_sync(e);
+    VB_NOEXCEPT_END((void)0)
+}
+
+// Text recognition with the ViTSTR extension (reference extensions/vitstr.cpp): its grayscale preprocess (vitstr.cpp:128-201) writes
+// the 1-channel patch matrix, the forward pass leaves the top-1 class and probability of every head token in the slot, and its greedy
+// decode (vitstr.cpp:1020-1054) turns token rows 1 .. head_tokens-1 into class ids, a length and a score -- all on the device, in the
+// same two-slot pipeline as vitb200_forward_async / vitb200_forward_u8_async.  Every argument is checked before anything is enqueued.
+static int recognize_enqueue(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, float *images_f32_out,
+                             int32_t *chars, int32_t *lengths, double *scores, float *probs)
+{
+    if (!e || !images || !nx || !ny) return fail("vitb200_recognize_u8: null argument");
+    if (e->C != 1)
+        return fail("vitb200_recognize_u8 implements the ViTSTR grayscale preprocess (1-channel, vitstr.cpp:128-201); this model takes "
+                    "%d-channel input", e->C);
+    if (e->head_tokens < 2) return fail("vitb200_recognize_u8: head_tokens is %d; the greedy decode reads token rows 1 .. head_tokens-1", e->head_tokens);
+    if (e->hp.patch_size != 16 && e->hp.patch_size != 8) return fail("1-channel input: patch size %d not supported (8, 16)", e->hp.patch_size);
+    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
+    for (int b = 0; b < batch; ++b)
+    {
+        if (!images[b]) return fail("vitb200_recognize_u8: null argument (image %d)", b);
+        if (nx[b] < 2 || ny[b] < 2) return fail("image %d is %dx%d pixels; the grayscale resize needs at least 2x2", b, nx[b], ny[b]);
+    }
+    int sl = 0;
+    size_t table_off = 0;
+    if (stage_u8(e, images, nx, ny, batch, sl, table_off)) return 1;
+    cudaStream_t s = e->stream;
+    const int S = e->hp.img_size, TH = e->head_tokens, C = e->hp.num_classes;
+    float *d_f32 = images_f32_out ? e->d_img_slot[sl] : nullptr;
+    dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
+    preprocess_gray_kernel<<<grid, 256, 0, s>>>(e->d_u8[sl], reinterpret_cast<const PreImage *>(e->d_u8[sl] + table_off), d_f32, S, e->PA,
+                                                e->hp.patch_size, e->KPp);
+    CUDA_TRY(cudaGetLastError());
+    if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * S * S * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (chars || lengths || scores || probs)
+    {
+        // patches ready (d_images = NULL); top-1 of every head token into the slot; probabilities only when asked for
+        if (run_forward_graphed(e, nullptr, batch, probs ? e->d_probs_slot[sl] : nullptr, nullptr, e->d_topk_idx_slot[sl],
+                                e->d_topk_val_slot[sl], 1, s))
+            return 1;
+        vitstr_decode_kernel<<<(batch + 127) / 128, 128, 0, s>>>(e->d_topk_idx_slot[sl], e->d_topk_val_slot[sl], batch, TH,
+                                                                 e->d_chars_slot[sl], e->d_len_slot[sl], e->d_score_slot[sl]);
+        CUDA_TRY(cudaGetLastError());
+        e->launches += 2; // the preprocess and decode kernels
+        if (chars) CUDA_TRY(cudaMemcpyAsync(chars, e->d_chars_slot[sl], (size_t)batch * (TH - 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        if (lengths) CUDA_TRY(cudaMemcpyAsync(lengths, e->d_len_slot[sl], (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        if (scores) CUDA_TRY(cudaMemcpyAsync(scores, e->d_score_slot[sl], (size_t)batch * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (probs) CUDA_TRY(cudaMemcpyAsync(probs, e->d_probs_slot[sl], (size_t)batch * TH * C * sizeof(float), cudaMemcpyDeviceToHost, s));
+    }
+    else
+        e->launches = 1; // preprocess only
+    CUDA_TRY(cudaEventRecord(e->ev_done[sl], s));
+    e->submits++;
+    return 0;
+}
+
+int vitb200_recognize_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int32_t *chars,
+                               int32_t *lengths, double *scores, float *probs)
+{
+    VB_NOEXCEPT_BEGIN
+    return recognize_enqueue(e, images, nx, ny, batch, nullptr, chars, lengths, scores, probs);
+    VB_NOEXCEPT_END((void)0)
+}
+
+int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, float *images_f32_out,
+                         int32_t *chars, int32_t *lengths, double *scores, float *probs)
+{
+    VB_NOEXCEPT_BEGIN
+    if (recognize_enqueue(e, images, nx, ny, batch, images_f32_out, chars, lengths, scores, probs)) return 1;
     return vitb200_sync(e);
     VB_NOEXCEPT_END((void)0)
 }

@@ -109,4 +109,81 @@ __global__ void preprocess_kernel(const uint8_t *__restrict__ staging, const Pre
     }
 }
 
+// ---- The ViTSTR extension's vit_image_preprocess (reference extensions/vitstr.cpp:128-201): u8 RGB -> grayscale -> bilinear resize
+// to img_size^2 -> (v / 255 - 0.5) * 2, 1 channel, no rounding to u8 in between.  Operation for operation as the extension's build
+// (gcc -O3 -mavx2 -mfma, -std=gnu++11 so contraction is on) computes it, read off its disassembly:
+//  * rgb_to_grayscale (vitstr.cpp:128-132, an out-of-line scalar function) in DOUBLE: fma(0.114, b, fma(0.299, r, 0.587 * g)),
+//    truncated to u8.  Not an identity on gray pixels: 75 of the 256 levels (v, v, v) come out as v - 1 (0.99...9 truncates);
+//  * the resize (vitstr.cpp:150-172) in float, sampling at x * (nx / S) with NO half-pixel offset; u = gx - (int)gx is taken
+//    BEFORE the clamp px0 = max(0, min(gxi, nx - 2)) and not recomputed after it, so the last columns / rows extrapolate towards
+//    px0 + 1 <= nx - 1.  The four products are summed as fma(g11, u*v, fma(g10, (1-u)*v, fma(g00, (1-u)*(1-v), (u*(1-v)) * g01)));
+//  * normalisation (vitstr.cpp:175): val / 255 - 0.5, times 2.  The padding loops (vitstr.cpp:181-198) never run.
+// Images narrower or shorter than 2 pixels are rejected on the host (the extension reads outside such an image).
+__device__ __forceinline__ float gray_level(const uint8_t *rgb)
+{
+    const double y = __fma_rn(0.114, (double)rgb[2], __fma_rn(0.299, (double)rgb[0], __dmul_rn(0.587, (double)rgb[1])));
+    return (float)(uint8_t)(int)y;
+}
+
+// out (float32 [B][S][S], may be NULL) and/or patches (may be NULL): the 1-channel f16 patch matrix of the patch-embedding GEMM,
+// k = ky*P + kx, row pitch ldk.  Same staging layout (PreImage table + interleaved RGB u8) as preprocess_kernel.
+__global__ void preprocess_gray_kernel(const uint8_t *__restrict__ staging, const PreImage *__restrict__ imgs, float *__restrict__ out,
+                                       int S, __half *__restrict__ patches, int P, int ldk)
+{
+    const int b = blockIdx.y;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= S * S) return;
+    const int y = idx / S, x = idx - y * S; // output row, column
+    const PreImage im = imgs[b];
+    const uint8_t *src = staging + im.offset;
+    const int nx = im.nx, ny = im.ny;
+    const float x_scale = __fdiv_rn((float)nx, (float)S), y_scale = __fdiv_rn((float)ny, (float)S);
+    const float gx = __fmul_rn((float)x, x_scale), gy = __fmul_rn((float)y, y_scale);
+    const int gxi = (int)gx, gyi = (int)gy;
+    const float u = __fsub_rn(gx, (float)gxi), v = __fsub_rn(gy, (float)gyi);
+    const int px0 = max(0, min(gxi, nx - 2)), py0 = max(0, min(gyi, ny - 2));
+    const uint8_t *r0 = src + (size_t)py0 * nx * 3, *r1 = r0 + (size_t)nx * 3;
+    const float g00 = gray_level(r0 + px0 * 3), g01 = gray_level(r0 + px0 * 3 + 3);
+    const float g10 = gray_level(r1 + px0 * 3), g11 = gray_level(r1 + px0 * 3 + 3);
+    const float omu = __fsub_rn(1.0f, u), omv = __fsub_rn(1.0f, v);
+    float val = __fmul_rn(__fmul_rn(u, omv), g01);
+    val = __fmaf_rn(__fmul_rn(omu, omv), g00, val);
+    val = __fmaf_rn(__fmul_rn(omu, v), g10, val);
+    val = __fmaf_rn(__fmul_rn(u, v), g11, val);
+    val = __fmul_rn(__fsub_rn(__fdiv_rn(val, 255.0f), 0.5f), 2.0f);
+    if (out) out[(size_t)b * S * S + idx] = val;
+    if (patches)
+    {
+        const int G = S / P, py = y / P, ky = y - py * P, pxi = x / P, kx = x - pxi * P;
+        patches[((size_t)b * G * G + (size_t)py * G + pxi) * ldk + ky * P + kx] = __float2half_rn(val);
+    }
+}
+
+// The extension's greedy decode (vitstr.cpp:1020-1054), one thread per image: the arg-max of token rows 1 .. TH-1 in order (top1_idx /
+// top1_val: softmax_topk_kernel with k = 1, whose tie rule -- lowest index among equal maxima -- is the extension's `>` scan from
+// class 0), stopping at the first row whose arg-max is class 1 ([s], end of sentence).  chars [B][TH-1] (-1 past the end),
+// lengths [B], scores [B] = the product of the emitted maxima in double, multiplied in token order (`conf *= max_value`; 1 if empty).
+__global__ void vitstr_decode_kernel(const int32_t *__restrict__ top1_idx, const float *__restrict__ top1_val, int B, int TH,
+                                     int32_t *__restrict__ chars, int32_t *__restrict__ lengths, double *__restrict__ scores)
+{
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int n = TH - 1;
+    double conf = 1.0;
+    int len = 0;
+    bool eos = false;
+    for (int t = 1; t < TH; ++t)
+    {
+        const size_t row = (size_t)b * TH + t;
+        const int id = top1_idx[row];
+        eos = eos || id == 1;
+        chars[(size_t)b * n + t - 1] = eos ? -1 : id;
+        if (eos) continue;
+        conf = __dmul_rn(conf, (double)top1_val[row]);
+        ++len;
+    }
+    lengths[b] = len;
+    scores[b] = conf;
+}
+
 } // namespace vitb200

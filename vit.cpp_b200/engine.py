@@ -82,6 +82,8 @@ def lib():
         L.vitb200_forward_u8.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, i32]
         L.vitb200_forward_u8_async.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp, vp, vp, i32]
         L.vitb200_forward_device.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp]
+        L.vitb200_recognize_u8.argtypes = [vp, vp, vp, vp, i32, vp, vp, vp, vp, vp]
+        L.vitb200_recognize_u8_async.argtypes = [vp, vp, vp, vp, i32, vp, vp, vp, vp]
         L.vitb200_features.argtypes = [vp, vp, i32, C.POINTER(FeaturesReq), vp, vp]
         L.vitb200_features_device.argtypes = [vp, vp, i32, C.POINTER(FeaturesReq), vp, vp, vp]
         L.vitb200_features_u8.argtypes = [vp, vp, vp, vp, i32, i32, C.POINTER(FeaturesReq), vp, vp]
@@ -118,10 +120,17 @@ class VitModel:
         self.n_tokens = (hp.img_size // hp.patch_size) ** 2 + 1
         self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713)
         self.head_tokens = lib().vitb200_head_tokens(self._h)  # classifier rows per image (1, or 25 for ViTSTR)
+        self._labels = None
 
     def label(self, i: int) -> Optional[str]:
         s = lib().vitb200_label(self._h, i)
         return s.decode() if s else None
+
+    def labels(self) -> Optional[list]:
+        """id2label as a list indexed by class id; None unless the model file names every class."""
+        if self._labels is None:
+            self._labels = [self.label(i) for i in range(self.num_classes)]
+        return None if any(s is None for s in self._labels) else self._labels
 
     @property
     def handle(self):
@@ -248,11 +257,7 @@ def sync_all(models):
 def vit_image_preprocess_predict(model: VitModel, images_u8, bilinear: bool = False, topk: int = 5, predict: bool = True):
     """reference vit_image_preprocess (vit.cpp:289) + vit_predict on the GPU for a list of HxWx3 uint8 RGB arrays of any size.
     Returns (image_f32 batch [B,S,S,3], probs, topk_idx, topk_prob, logits); the last four are None if predict is False."""
-    imgs = [np.ascontiguousarray(a, dtype=np.uint8) for a in images_u8]
-    B = len(imgs)
-    ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in imgs])
-    nx = (C.c_int * B)(*[a.shape[1] for a in imgs])
-    ny = (C.c_int * B)(*[a.shape[0] for a in imgs])
+    _, B, ptrs, nx, ny = _u8_batch(images_u8)
     S = model.img_size
     f32 = np.empty((B, S, S, 3), np.float32)
     probs = np.empty((B, model.num_classes), np.float32) if predict else None
@@ -264,6 +269,43 @@ def vit_image_preprocess_predict(model: VitModel, images_u8, bilinear: bool = Fa
                                     idx.ctypes.data if predict else None, val.ctypes.data if predict else None, topk if predict else 0),
            "vit_image_preprocess")
     return f32, probs, idx, val, logits
+
+
+def _u8_batch(images_u8):
+    """HxWx3 uint8 arrays -> (the contiguous arrays, which the caller keeps alive during the call, B, pointer / width / height arrays)."""
+    imgs =[np.ascontiguousarray(a, dtype=np.uint8) for a in images_u8]
+    B = len(imgs)
+    ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in imgs])
+    nx = (C.c_int * B)(*[a.shape[1] for a in imgs])
+    ny = (C.c_int * B)(*[a.shape[0] for a in imgs])
+    return imgs, B, ptrs, nx, ny
+
+
+def vitstr_recognize_u8(model: VitModel, images_u8, probs: bool = False):
+    """Text recognition with a ViTSTR model (vitb200_recognize_u8): HxWx3 uint8 RGB arrays of any size >= 2x2 go through the extension's
+    grayscale preprocess, the forward pass and its greedy decode (reference extensions/vitstr.cpp:128-201, 1020-1054) on the GPU.
+    Returns (texts, scores float64[B], chars int32[B, n-1], lengths int32[B]) (+ probs float32[B, n, classes] if `probs`), n =
+    head_tokens.  texts[b] joins model.label(id) over the decoded ids, as the extension prints them; None if the model has no id2label."""
+    _, B, ptrs, nx, ny = _u8_batch(images_u8)
+    n = model.head_tokens
+    chars = np.empty((B, max(n - 1, 0)), np.int32)
+    lengths = np.empty(B, np.int32)
+    scores = np.empty(B, np.float64)
+    pr = np.empty((B, n, model.num_classes), np.float32) if probs else None
+    _check(lib().vitb200_recognize_u8(model.handle, ptrs, nx, ny, B, None, chars.ctypes.data, lengths.ctypes.data, scores.ctypes.data,
+                                      pr.ctypes.data if probs else None), "vitstr_recognize_u8")
+    names = model.labels()
+    texts = None if names is None else ["".join(names[i] for i in chars[b, :lengths[b]]) for b in range(B)]
+    return (texts, scores, chars, lengths, pr) if probs else (texts, scores, chars, lengths)
+
+
+def vitstr_preprocess_u8(model: VitModel, images_u8) -> np.ndarray:
+    """The ViTSTR extension's vit_image_preprocess (vitstr.cpp:128-201) on the GPU for HxWx3 uint8 RGB arrays: float32[B, S, S]."""
+    _, B, ptrs, nx, ny = _u8_batch(images_u8)
+    S = model.img_size
+    out = np.empty((B, S, S), np.float32)
+    _check(lib().vitb200_recognize_u8(model.handle, ptrs, nx, ny, B, out.ctypes.data, None, None, None, None), "vitstr_preprocess_u8")
+    return out
 
 
 BFLOAT16 = "bfloat16"  # numpy has no bf16: such features come back as uint16 bit patterns
@@ -299,11 +341,7 @@ def vit_features(model: VitModel, images: np.ndarray, layers=None, norm: bool = 
 def vit_features_u8(model: VitModel, images_u8, bilinear: bool = False, layers=None, norm: bool = True, tokens: bool = True,
                     prelogits: bool = False, dtype=np.float32):
     """vit_features of HxWx3 uint8 RGB images of any size, pre-processed on the GPU like vit_image_preprocess_predict."""
-    imgs = [np.ascontiguousarray(a, dtype=np.uint8) for a in images_u8]
-    B = len(imgs)
-    ptrs = (C.c_void_p * B)(*[a.ctypes.data for a in imgs])
-    nx = (C.c_int * B)(*[a.shape[1] for a in imgs])
-    ny = (C.c_int * B)(*[a.shape[0] for a in imgs])
+    _, B, ptrs, nx, ny = _u8_batch(images_u8)
     return _features_call(model, B, layers, norm, tokens, prelogits, dtype, lambda req, t, p: _check(
         lib().vitb200_features_u8(model.handle, ptrs, nx, ny, B, int(bilinear), req, t, p), "vit_features_u8"))
 
