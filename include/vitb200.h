@@ -73,6 +73,21 @@ int vitb200_create_from_file(const char *path, int device, int max_batch, vitb20
 int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                       int head_tokens, vitb200_engine **out);
 int vitb200_create_from_file_ex(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out);
+/* FP8 engine: the same arguments and the same entry points (forward in every form, u8, features, recognition, sharded), with the
+ * qkv and fc1 linear layers of every block on the e4m3 tensor cores.  Numerics (everything not listed is the f16 engine's):
+ *   weights     attn.qkv.weight and mlp.fc1.weight, taken as the f16 values the f16 engine would store (any file format), get one f32
+ *               scale per tensor, sw = amax / 448 (1 when amax = 0), and are stored only as qw = e4m3_rn_satfinite(w * (448 / amax)).
+ *   activations LayerNorms 1 and 2 quantise each token row of their f32 output y (the values the f16 engine rounds to f16) with its
+ *               own scale: sa = amax / 448 over the row (1 when amax = 0), q = e4m3_rn_satfinite(y * (448 / amax)).
+ *   GEMM        x[m][n] = acc * (sa[m] * sw) + bias[n], acc = sum_k q[m][k] qw[n][k] accumulated by the tensor cores in f32 (on Hopper
+ *               an e4m3 MMA adds its products with fewer than f32's mantissa bits); then the f16 engine's epilogue on x (qkv: hi + lo
+ *               split for the attention; fc1: f16, GELU, f16).
+ * proj, fc2, the patch embedding, attention, the final LayerNorm and the head are unchanged.  The ln1 / ln2 debug taps return q * sa.
+ * The accuracy cost against the reference is stated in README.md. */
+int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
+                       int head_tokens, vitb200_engine **out);
+int vitb200_create_from_file_fp8(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out);
+int vitb200_fp8(const vitb200_engine *e);         /* 1 for an FP8 engine, else 0 */
 int vitb200_in_chans(const vitb200_engine *e);    /* 3, or 1 for a ViTSTR model */
 int vitb200_head_tokens(const vitb200_engine *e); /* classifier rows per image */
 
@@ -225,6 +240,20 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
 /* Stand-alone run of the block LayerNorm kernel the forward schedule uses (reference ggml_norm + ggml_mul + ggml_add, vit.cpp:808-812,
  * ggml.c:8959-9008): x float32 [rows][D] -> y float32 [rows][D] holding the f16 results (the next GEMM's A operand) widened. */
 int vitb200_test_layernorm(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, float *y);
+
+/* Host-only: the FP8 engine's upload-time quantisation of one weight tensor (vitb200_create_fp8): n f16 values (bits) -> n e4m3
+ * bytes q and the tensor's scale *scale.  Needs no GPU. */
+int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, float *scale);
+
+/* Stand-alone run of the e4m3 GEMM the FP8 engine uses for qkv and fc1: A [M][K] and W [N][K] e4m3 bytes, a_scale float32 [M] (one per
+ * A row), w_scale, bias [N]; out float32 [M][N] = the epilogue's f16 result widened (epilogue 0 bias->f16, 1 bias+gelu->f16,
+ * 6 split precision: hi + lo) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
+int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
+                          float w_scale, const float *bias, float *out);
+
+/* The FP8 engine's LayerNorm 1 / 2 alone, the kernel chosen as vitb200_test_layernorm chooses it: x float32 [rows][D] -> q e4m3 bytes
+ * [rows][D] and the row scales sa float32 [rows].  D % 16 == 0. */
+int vitb200_test_layernorm_fp8(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, uint8_t *q, float *sa);
 
 /* Prototype of the reference's q8_0 x q8_0 linear layer on the INTEGER tensor cores (wgmma s8, one K = 32 MMA per
  * q8_0 block; csrc/gemm_q8_wgmma.cuh).  Replaces, for one layer, quantize_row_q8_0 (reference ggml-quants.c:702-790: the f32

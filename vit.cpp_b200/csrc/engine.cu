@@ -11,6 +11,7 @@
 #include "preprocess.cuh"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -117,12 +118,21 @@ int make_tmap_2d(CUtensorMap *m, CUtensorMapDataType dt, size_t elem_bytes, cons
     return 0;
 }
 
+// e4m3 row-major tensor [rows][cols] (pitch = cols bytes, a multiple of 16): box = 128 columns (one 128-B swizzled row, an e4m3
+// k-block) x box_rows rows, SWIZZLE_128B, out-of-bounds elements read as zero
+int make_tmap_e4m3(CUtensorMap *m, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows)
+{
+    return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ptr, rows, cols, cols, 2 * GEMM_BK, box_rows, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 struct Linear
 {
     __half *w = nullptr; // [n_out][ld] f16, K contiguous (ggml ne0 = K)
+    uint8_t *w8 = nullptr; // FP8 engine, qkv and fc1: [n_out][ld] e4m3 instead of w; the weight is w8 * w_scale
+    float w_scale = 1.f;
     float *b = nullptr;  // [n_out]
     int n_out = 0, n_in = 0, ld = 0;
-    CUtensorMap tm;  // box = 64 x GEMM_BN rows: the W tile of one k-block
+    CUtensorMap tm;  // box = one k-block (64 f16 or 128 e4m3 = 128 B) x GEMM_BN rows: the W tile of one k-block
 };
 
 struct Layer
@@ -154,6 +164,12 @@ struct vitb200_engine
     float *d_sm_scratch = nullptr; // soft-max working rows in global memory, only when num_classes floats exceed shared memory
     int C = 3;            // input channels: 3 (vit.cpp) or 1 (ViTSTR extension, vitstr.cpp:713), taken from the patch kernel's shape
     int head_tokens = 1;  // tokens the classifier head reads per image: 1 (token 0, vit.cpp:910) or 25 (vitstr.cpp:864-903)
+    // FP8 engine (vitb200_create_fp8): LayerNorms 1 and 2 write e4m3 rows A8 with per-row scales SA, and the qkv and fc1 GEMMs run
+    // e4m3 x e4m3 against per-tensor-scaled e4m3 weights; everything else is the f16 engine's schedule
+    bool fp8 = false;
+    uint8_t *A8 = nullptr;
+    float *SA = nullptr;
+    CUtensorMap tmA8;
     cudaStream_t stream = nullptr;
     std::vector<void *> allocs;
     // weights
@@ -274,6 +290,17 @@ int upload_f32(vitb200_engine *e, const vitb200_tensor *t, int n, const std::str
 uint16_t host_f32_to_f16(float f) { const __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
 float host_f16_to_f32(uint16_t u) { __half h; memcpy(&h, &u, 2); return __half2float(h); }
 
+// The FP8 engine's weight quantisation: one scale for the whole tensor, sw = amax / 448 (1 when amax = 0), and
+// q = e4m3_rn_satfinite(w (448 / amax)), from the f16 values the f16 engine would store.  Returns sw.
+float quantize_e4m3(const uint16_t *w, size_t n, uint8_t *q)
+{
+    float amax = 0.f;
+    for (size_t i = 0; i < n; ++i) amax = std::max(amax, std::fabs(host_f16_to_f32(w[i])));
+    const float inv = amax > 0.f ? 448.f / amax : 1.f;
+    for (size_t i = 0; i < n; ++i) q[i] = (uint8_t)__nv_cvt_float_to_fp8(host_f16_to_f32(w[i]) * inv, __NV_SATFINITE, __NV_E4M3);
+    return amax > 0.f ? amax / 448.f : 1.f;
+}
+
 // ggml block formats of 32 weights (ggml-quants.h:11-47), keyed by ggml_type / file ftype (vit.cpp:645-672).
 size_t quant_block_bytes(int type)
 {
@@ -334,8 +361,9 @@ void dequant_block(int type, const uint8_t *blk, float *y)
 //          dots them against activations quantised on the fly to q8_0/q8_1 (ggml.c type traits vec_dot_type).
 //   type 0 (F32): rounded once to f16 (the reference keeps f32 weights AND f32 activations, ggml.c:1163-1198).
 //   type 30 (BF16, GGUF containers): widened to f32, then as type 0.
+// e4m3: the f16 values are quantised once more (quantize_e4m3) and only the e4m3 copy goes to the device.
 int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::string &wname, const std::string &bname,
-                  int n_out, int n_in, int ld, Linear *L, int conv_p = 0)
+                  int n_out, int n_in, int ld, Linear *L, int conv_p = 0, bool e4m3 = false)
 {
     const vitb200_tensor *w = find_tensor(t, n, wname);
     if (!w) return fail("missing tensor '%s'", wname.c_str());
@@ -346,8 +374,6 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     else if (check_shape(w, wname, n_in, n_out, 1, 1)) return 1;                                             // [in, out], vit.cpp:531-543
     if (quant_block_bytes(w->type) && n_in % 32 != 0) return fail("tensor '%s': quantised rows must be a multiple of 32", wname.c_str());
     L->n_out = n_out; L->n_in = n_in; L->ld = ld;
-    if (dev_alloc(e, &L->w, (size_t)n_out * ld)) return 1;
-    CUDA_TRY(cudaMemset(L->w, 0, (size_t)n_out * ld * sizeof(__half)));
     const void *src = w->data;
     std::vector<uint16_t> conv;
     if (w->type != 1)
@@ -387,9 +413,22 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
         }
         src = conv.data();
     }
-    CUDA_TRY(cudaMemcpy2D(L->w, (size_t)ld * 2, src, (size_t)n_in * 2, (size_t)n_in * 2, (size_t)n_out, cudaMemcpyHostToDevice));
+    if (e4m3)
+    {
+        std::vector<uint8_t> q((size_t)n_out * n_in);
+        L->w_scale = quantize_e4m3((const uint16_t *)src, q.size(), q.data());
+        if (dev_alloc(e, &L->w8, (size_t)n_out * ld)) return 1;
+        CUDA_TRY(cudaMemcpy2D(L->w8, (size_t)ld, q.data(), (size_t)n_in, (size_t)n_in, (size_t)n_out, cudaMemcpyHostToDevice));
+    }
+    else
+    {
+        if (dev_alloc(e, &L->w, (size_t)n_out * ld)) return 1;
+        CUDA_TRY(cudaMemset(L->w, 0, (size_t)n_out * ld * sizeof(__half)));
+        CUDA_TRY(cudaMemcpy2D(L->w, (size_t)ld * 2, src, (size_t)n_in * 2, (size_t)n_in * 2, (size_t)n_out, cudaMemcpyHostToDevice));
+    }
     // conv bias is declared [1, 1, D] (vit.cpp:516), every other bias [n_out]; the tail up to a multiple of 4 stays zero
     if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
+    if (e4m3) return make_tmap_e4m3(&L->tm, L->w8, (uint64_t)n_out, (uint64_t)ld, (uint32_t)GEMM_BN);
     return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)GEMM_BN);
 }
 
@@ -438,11 +477,11 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-template <int EPI, int STAGES>
+template <int EPI, int STAGES, int OP = GEMM_OP_F16>
 int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
     using Cfg = GemmCfg<STAGES>;
-    auto kern = gemm_wgmma_kernel<EPI, STAGES>;
+    auto kern = gemm_wgmma_kernel<EPI, STAGES, OP>;
     // clusters of two CTAs that share the A tile (multicast), with programmatic dependent launch as in launch_pdl
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3(2); cfg.blockDim = dim3((unsigned)Cfg::kThreads); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = s;
@@ -492,11 +531,21 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     return 0;
 }
 
-// tmB: the weight map, box = 64 x GEMM_BN rows
-int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
+// tmB: the weight map, box = one k-block x GEMM_BN rows.  e4m3: A and W are e4m3 maps (make_tmap_e4m3), p.a_scale / p.w_scale their
+// scales; the f16-output epilogues only (qkv and fc1 of the FP8 engine)
+int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s, bool e4m3 = false)
 {
     if (p.N % 4 != 0) return fail("GEMM: N = %d is not a multiple of 4", p.N);
     const bool deep = p.K >= GEMM_DEEP_K; // ring depth by reduction length (GemmCfg)
+    if (e4m3)
+    {
+        if (!p.a_scale) return fail("e4m3 GEMM: no A scales");
+#define VB_CASE(EPI) \
+    if (epi == EPI) return deep ? launch_gemm_t<EPI, 6, GEMM_OP_E4M3>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, GEMM_OP_E4M3>(e, tmA, tmB, p, s);
+        VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16)
+#undef VB_CASE
+        return fail("no e4m3 GEMM instantiation for epilogue=%d", epi);
+    }
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
     VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
@@ -539,25 +588,28 @@ int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaS
 
 // The row-per-warp kernel: the LayerNorms the bulk-copy kernel below does not take (pooled rows, hidden sizes that are not a multiple
 // of 128) and, with an f32 / bf16 output or NORM = false, the encoder features.  rows_per_group <= 0: all rows are one group.
+// OutT = __nv_fp8_e4m3: y_scale receives the per-row scales.
 template <typename OutT, bool NORM>
 int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
-                          cudaStream_t s, int rows_per_group, size_t group_stride)
+                          cudaStream_t s, int rows_per_group, size_t group_stride, float *y_scale = nullptr)
 {
     const int D = e->hp.hidden_size;
     if (rows_per_group <= 0) rows_per_group = rows > 0 ? rows : 1; // one group: plain consecutive rows
     const int threads = 256, rows_per_block = threads / 32;
     const int blocks = (rows + rows_per_block - 1) / rows_per_block;
-    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
-    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
-    else if (D <= 16 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<16, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps));
+    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
+    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
+    else if (D <= 16 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<16, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
     else return fail("hidden size %d not supported (max 2048)", D);
     CUDA_TRY(cudaGetLastError());
     e->launches++;
     return 0;
 }
 
-int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, __half *y, int rows, cudaStream_t s,
-                     int rows_per_group = 0, size_t group_stride = 0)
+// OutT = __half: the f16 A operand; __nv_fp8_e4m3: the FP8 engine's e4m3 A operand and its row scales y_scale
+template <typename OutT = __half>
+int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows, cudaStream_t s,
+                     int rows_per_group = 0, size_t group_stride = 0, float *y_scale = nullptr)
 {
     const int D = e->hp.hidden_size;
     // block LayerNorms (all rows consecutive): the persistent bulk-copy kernel
@@ -574,27 +626,27 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
             int dev = 0;
             CUDA_TRY(cudaGetDevice(&dev));
             if (!attr_set[D / 128][dev & 63]) { CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr_set[D / 128][dev & 63] = true; }
-            CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps));
+            CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps, y_scale));
             return 0;
         };
         int rc = 1;
         switch (D / 128)
         {
-        case 1: rc = launch(layernorm_tma_kernel<1>); break;
-        case 2: rc = launch(layernorm_tma_kernel<2>); break;
-        case 3: rc = launch(layernorm_tma_kernel<3>); break;
-        case 4: rc = launch(layernorm_tma_kernel<4>); break;
-        case 5: rc = launch(layernorm_tma_kernel<5>); break;
-        case 6: rc = launch(layernorm_tma_kernel<6>); break;
-        case 7: rc = launch(layernorm_tma_kernel<7>); break;
-        case 8: rc = launch(layernorm_tma_kernel<8>); break;
+        case 1: rc = launch(layernorm_tma_kernel<1, OutT>); break;
+        case 2: rc = launch(layernorm_tma_kernel<2, OutT>); break;
+        case 3: rc = launch(layernorm_tma_kernel<3, OutT>); break;
+        case 4: rc = launch(layernorm_tma_kernel<4, OutT>); break;
+        case 5: rc = launch(layernorm_tma_kernel<5, OutT>); break;
+        case 6: rc = launch(layernorm_tma_kernel<6, OutT>); break;
+        case 7: rc = launch(layernorm_tma_kernel<7, OutT>); break;
+        case 8: rc = launch(layernorm_tma_kernel<8, OutT>); break;
         }
         if (rc) return 1;
         CUDA_TRY(cudaGetLastError());
         e->launches++;
         return 0;
     }
-    return launch_layernorm_rows<__half, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride);
+    return launch_layernorm_rows<OutT, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride, y_scale);
 }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
@@ -686,6 +738,24 @@ int tap_f16(float *dst, const __half *src, size_t n, cudaStream_t s, const __hal
     return 0;
 }
 
+// debug tap of e4m3 rows with per-row scales (the FP8 engine's LayerNorm outputs): q * scale in f32
+int tap_e4m3(float *dst, const uint8_t *q, const float *scale, size_t rows, size_t cols, cudaStream_t s)
+{
+    if (!dst) return 0;
+    CUDA_TRY(cudaStreamSynchronize(s));
+    std::vector<uint8_t> tq(rows * cols);
+    std::vector<float> ts(rows);
+    CUDA_TRY(cudaMemcpy(tq.data(), q, tq.size(), cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaMemcpy(ts.data(), scale, rows * sizeof(float), cudaMemcpyDeviceToHost));
+    for (size_t r = 0; r < rows; ++r)
+        for (size_t c = 0; c < cols; ++c)
+        {
+            const __half_raw h = __nv_cvt_fp8_to_halfraw((__nv_fp8_storage_t)tq[r * cols + c], __NV_E4M3);
+            dst[r * cols + c] = host_f16_to_f32(h.x) * ts[r];
+        }
+    return 0;
+}
+
 // debug tap of the q | k | v activations in the reference's [tokens][3 D] order (the device buffers are head-major: [3 H][rows][64])
 int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
 {
@@ -733,14 +803,23 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         const bool tap = taps && taps->layer == il;
         {
             ProfScope ps(e, PK_LN, 0.0, s);
-            if (launch_layernorm(e, e->X, (size_t)D, L.n1w, L.n1b, e->A16, T, s)) return 1; // vit.cpp:808-812
-            if (tap && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1;
+            if (e->fp8)
+            {
+                if (launch_layernorm(e, e->X, (size_t)D, L.n1w, L.n1b, (__nv_fp8_e4m3 *)e->A8, T, s, 0, 0, e->SA)) return 1;
+                if (tap && tap_e4m3(taps->ln1, e->A8, e->SA, (size_t)T, (size_t)D, s)) return 1;
+            }
+            else
+            {
+                if (launch_layernorm(e, e->X, (size_t)D, L.n1w, L.n1b, e->A16, T, s)) return 1; // vit.cpp:808-812
+                if (tap && tap_f16(taps->ln1, e->A16, (size_t)T * D, s)) return 1;
+            }
         }
         {
             GemmParams p{};
             p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.plane_rows = (size_t)e->max_batch * N;
+            p.a_scale = e->SA; p.w_scale = L.qkv.w_scale;
             ProfScope ps(e, PK_QKV, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->tmA_D, L.qkv.tm, p, s)) return 1; // vit.cpp:820-821
+            if (launch_gemm(e, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->fp8 ? e->tmA8 : e->tmA_D, L.qkv.tm, p, s, e->fp8)) return 1; // vit.cpp:820-821
         }
         if (tap && tap_qkv(e, taps->qkv, T, s)) return 1;
         {
@@ -757,14 +836,16 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (tap && tap_f32(taps->x1, e->X, (size_t)T * D, s)) return 1;
         {
             ProfScope ps(e, PK_LN, 0.0, s);
-            if (launch_layernorm(e, e->X, (size_t)D, L.n2w, L.n2b, e->A16, T, s)) return 1; // vit.cpp:881-885
+            if (e->fp8 ? launch_layernorm(e, e->X, (size_t)D, L.n2w, L.n2b, (__nv_fp8_e4m3 *)e->A8, T, s, 0, 0, e->SA)
+                       : launch_layernorm(e, e->X, (size_t)D, L.n2w, L.n2b, e->A16, T, s)) return 1; // vit.cpp:881-885
         }
-        if (tap && tap_f16(taps->ln2, e->A16, (size_t)T * D, s)) return 1;
+        if (tap && (e->fp8 ? tap_e4m3(taps->ln2, e->A8, e->SA, (size_t)T, (size_t)D, s) : tap_f16(taps->ln2, e->A16, (size_t)T * D, s))) return 1;
         {
             GemmParams p{};
             p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D;
+            p.a_scale = e->SA; p.w_scale = L.fc1.w_scale;
             ProfScope ps(e, PK_FC1, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, EPI_BIAS_GELU_F16, e->tmA_D, L.fc1.tm, p, s)) return 1; // vit.cpp:889-893
+            if (launch_gemm(e, EPI_BIAS_GELU_F16, e->fp8 ? e->tmA8 : e->tmA_D, L.fc1.tm, p, s, e->fp8)) return 1; // vit.cpp:889-893
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
@@ -945,21 +1026,33 @@ int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *t, int n, in
     } catch (const std::exception &ex) { cleanup; return fail("%s: %s", __func__, ex.what()); }            \
     catch (...) { cleanup; return fail("%s: unknown exception", __func__); }
 
-static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
                        vitb200_engine *&e, vitb200_engine **out);
 
-int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
-                      vitb200_engine **out)
+static int create_checked(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
+                          vitb200_engine **out)
 {
     if (!hp || !t || !out) return fail("vitb200_create: null argument");
     *out = nullptr;
     vitb200_engine *e = nullptr;
     VB_NOEXCEPT_BEGIN
-    return create_impl(hp, t, n, device, max_batch, head_tokens, e, out);
+    return create_impl(hp, t, n, device, max_batch, head_tokens, fp8, e, out);
     VB_NOEXCEPT_END(if (e) vitb200_destroy(e))
 }
 
-static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+                      vitb200_engine **out)
+{
+    return create_checked(hp, t, n, device, max_batch, head_tokens, false, out);
+}
+
+int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+                       vitb200_engine **out)
+{
+    return create_checked(hp, t, n, device, max_batch, head_tokens, true, out);
+}
+
+static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
                        vitb200_engine *&e, vitb200_engine **out)
 {
     // hyper-parameter sanity first (no division by a field a corrupt file may have zeroed; no device needed to reject them)
@@ -988,6 +1081,7 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     if (e->hp.eps <= 0.f) e->hp.eps = 1e-6f;
     e->device = device;
     e->max_batch = max_batch;
+    e->fp8 = fp8;
     e->num_sms = prop.multiProcessorCount;
     const int D = hp->hidden_size, P = hp->patch_size;
     e->G = hp->img_size / P;
@@ -1025,9 +1119,9 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         if (upload_f32(e, t, n, p + "norm1.weight", D, 1, 1, 1, &L.n1w) || upload_f32(e, t, n, p + "norm1.bias", D, 1, 1, 1, &L.n1b) ||
             upload_f32(e, t, n, p + "norm2.weight", D, 1, 1, 1, &L.n2w) || upload_f32(e, t, n, p + "norm2.bias", D, 1, 1, 1, &L.n2b))
             return bail(1);
-        if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv) ||
+        if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv, 0, fp8) ||
             upload_linear(e, t, n, p + "attn.proj.weight", p + "attn.proj.bias", D, D, D, &L.proj) ||
-            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, D, &L.fc1) ||
+            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, D, &L.fc1, 0, fp8) ||
             upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 4 * D, &L.fc2))
             return bail(1);
     }
@@ -1082,6 +1176,7 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_A_BOX_ROWS) ||
         make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_A_BOX_ROWS))
         return bail(1);
+    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || make_tmap_e4m3(&e->tmA8, e->A8, T, D, GEMM_A_BOX_ROWS))) return bail(1);
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
     // memory (N <= 224), i.e. wherever the wgmma attention runs
     if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return bail(1);
@@ -1123,6 +1218,7 @@ const char *vitb200_label(const vitb200_engine *e, int class_id)
 int vitb200_last_launch_count(const vitb200_engine *e) { return e ? e->launches : 0; }
 int vitb200_in_chans(const vitb200_engine *e) { return e ? e->C : 0; }
 int vitb200_head_tokens(const vitb200_engine *e) { return e ? e->head_tokens : 0; }
+int vitb200_fp8(const vitb200_engine *e) { return e && e->fp8 ? 1 : 0; }
 
 int vitb200_profile_enable(vitb200_engine *e, int on)
 {
@@ -1745,6 +1841,98 @@ int vitb200_test_layernorm(int device, int rows, int D, const float *x, const fl
     VB_NOEXCEPT_END((void)0)
 }
 
+int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, float *scale)
+{
+    if (!w_f16 || !q || !scale || n < 1) return fail("bad argument");
+    *scale = quantize_e4m3(w_f16, (size_t)n, q);
+    return 0;
+}
+
+// Stand-alone run of the e4m3 GEMM as the FP8 engine launches it (qkv and fc1): A [M][K] and W [N][K] e4m3 bytes, a_scale [M], w_scale.
+int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
+                          float w_scale, const float *bias, float *out)
+{
+    if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
+    if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
+    if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO)
+        return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6)", epilogue);
+    VB_NOEXCEPT_BEGIN
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
+    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
+    CUDA_TRY(cudaSetDevice(device));
+    uint8_t *dA = nullptr, *dW = nullptr;
+    float *dS = nullptr, *dB = nullptr;
+    __half *dO = nullptr, *dO2 = nullptr;
+    const size_t osz = (size_t)M * N * 2;
+    int rc = 1;
+    do
+    {
+        if (cudaMalloc(&dA, (size_t)M * K) || cudaMalloc(&dW, (size_t)N * K) || cudaMalloc(&dS, (size_t)M * 4) || cudaMalloc(&dB, (size_t)N * 4) ||
+            cudaMalloc(&dO, osz) || cudaMalloc(&dO2, osz)) { fail("cudaMalloc failed"); break; }
+        cudaMemcpy(dA, A, (size_t)M * K, cudaMemcpyHostToDevice);
+        cudaMemcpy(dW, W, (size_t)N * K, cudaMemcpyHostToDevice);
+        cudaMemcpy(dS, a_scale, (size_t)M * 4, cudaMemcpyHostToDevice);
+        cudaMemcpy(dB, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
+        cudaMemset(dO, 0, osz);
+        cudaMemset(dO2, 0, osz);
+        CUtensorMap tA, tB;
+        if (make_tmap_e4m3(&tA, dA, M, K, GEMM_A_BOX_ROWS) || make_tmap_e4m3(&tB, dW, N, K, GEMM_BN)) break;
+        GemmParams p{};
+        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dO; p.out2 = dO2; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
+        if (launch_gemm(nullptr, epilogue, tA, tB, p, 0, true)) break;
+        cudaError_t err = cudaDeviceSynchronize();
+        if (err != cudaSuccess) { fail("e4m3 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
+        std::vector<__half> hi((size_t)M * N), lo((size_t)M * N);
+        cudaMemcpy(hi.data(), dO, osz, cudaMemcpyDeviceToHost);
+        cudaMemcpy(lo.data(), dO2, osz, cudaMemcpyDeviceToHost);
+        // split-precision result: hi + lo (exact in f32); the other epilogues leave lo zero
+        for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
+        rc = 0;
+    } while (0);
+    cudaFree(dA); cudaFree(dW); cudaFree(dS); cudaFree(dB); cudaFree(dO); cudaFree(dO2);
+    return rc;
+    VB_NOEXCEPT_END((void)0)
+}
+
+// The FP8 engine's LayerNorm 1 / 2 alone, launched as vitb200_test_layernorm launches the f16 one: q [rows][D] e4m3 bytes, sa [rows].
+int vitb200_test_layernorm_fp8(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, uint8_t *q, float *sa)
+{
+    if (!x || !w || !b || !q || !sa || rows < 1 || D < 4 || D % 16 != 0 || D > 2048) return fail("bad argument");
+    VB_NOEXCEPT_BEGIN
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
+    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
+    CUDA_TRY(cudaSetDevice(device));
+    cudaDeviceProp prop;
+    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+    vitb200_engine e{};
+    e.hp.hidden_size = D; e.hp.eps = eps; e.num_sms = prop.multiProcessorCount; e.device = device;
+    float *dx = nullptr, *dw = nullptr, *db = nullptr, *ds = nullptr;
+    uint8_t *dq = nullptr;
+    int rc = 1;
+    do
+    {
+        if (cudaMalloc(&dx, (size_t)rows * D * 4) || cudaMalloc(&dw, (size_t)D * 4) || cudaMalloc(&db, (size_t)D * 4) || cudaMalloc(&dq, (size_t)rows * D) ||
+            cudaMalloc(&ds, (size_t)rows * 4)) { fail("cudaMalloc failed"); break; }
+        cudaMemcpy(dx, x, (size_t)rows * D * 4, cudaMemcpyHostToDevice);
+        cudaMemcpy(dw, w, (size_t)D * 4, cudaMemcpyHostToDevice);
+        cudaMemcpy(db, b, (size_t)D * 4, cudaMemcpyHostToDevice);
+        cudaMemset(dq, 0xFF, (size_t)rows * D);
+        cudaMemset(ds, 0xFF, (size_t)rows * 4);
+        if (cudaDeviceSynchronize() != cudaSuccess) { fail("device sync failed"); break; }
+        if (launch_layernorm(&e, dx, (size_t)D, dw, db, (__nv_fp8_e4m3 *)dq, rows, 0, 0, 0, ds)) break;
+        cudaError_t err = cudaDeviceSynchronize();
+        if (err != cudaSuccess) { fail("LayerNorm kernel failed: %s", cudaGetErrorString(err)); break; }
+        cudaMemcpy(q, dq, (size_t)rows * D, cudaMemcpyDeviceToHost);
+        cudaMemcpy(sa, ds, (size_t)rows * 4, cudaMemcpyDeviceToHost);
+        rc = 0;
+    } while (0);
+    cudaFree(dx); cudaFree(dw); cudaFree(db); cudaFree(dq); cudaFree(ds);
+    return rc;
+    VB_NOEXCEPT_END((void)0)
+}
+
 // q8_0 linear layer on the integer tensor cores (gemm_q8_wgmma.cuh; prototype for BASELINE.json configs[4]): x [M][K] f32 is
 // quantised on the device exactly as the reference quantises activation rows, w is a q8_0 tensor in the model-file layout
 // ([N][K/32] blocks of {f16 d; int8 q[32]}, ggml-quants.h:42-46).  Outputs: y [M][N] f32, and (optional) the quantised activations
@@ -1846,7 +2034,19 @@ extern "C" int vitb200_create_from_file(const char *path, int device, int max_ba
     return vitb200_create_from_file_ex(path, device, max_batch, 1, out);
 }
 
+static int create_from_file(const char *path, int device, int max_batch, int head_tokens, bool fp8, vitb200_engine **out);
+
 extern "C" int vitb200_create_from_file_ex(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
+{
+    return create_from_file(path, device, max_batch, head_tokens, false, out);
+}
+
+extern "C" int vitb200_create_from_file_fp8(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
+{
+    return create_from_file(path, device, max_batch, head_tokens, true, out);
+}
+
+static int create_from_file(const char *path, int device, int max_batch, int head_tokens, bool fp8, vitb200_engine **out)
 {
     if (!path || !out) return fail("null argument");
     *out = nullptr;
@@ -1891,7 +2091,7 @@ extern "C" int vitb200_create_from_file_ex(const char *path, int device, int max
         for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
     }
     const std::map<int, std::string> &labels = g.labels;
-    int rc = vitb200_create_ex(&hp, ts.data(), (int)ts.size(), device, max_batch, head_tokens, out);
+    int rc = create_checked(&hp, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out);
     if (rc == 0) (*out)->labels = labels;
     return rc;
     VB_NOEXCEPT_END(if (*out) { vitb200_destroy(*out); *out = nullptr; })

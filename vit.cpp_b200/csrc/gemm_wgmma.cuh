@@ -27,6 +27,11 @@
 // Ring depth (template STAGES, chosen by K on the host): 6 stages with 16 KB staging buffers for K >= GEMM_DEEP_K, whose main loop
 // dominates and needs the deeper ring to hide its load latency; 5 stages with 32 KB buffers otherwise, where the epilogue's share
 // is larger and fewer, larger passes shorten it.
+// Operand format (template OP): f16 x f16, or e4m3 x e4m3 for the FP8 engine's qkv and fc1.  A 128-B swizzled row holds 64 f16 or
+// 128 e4m3 values, so an e4m3 k-block is 128 elements with the same stage bytes, TMA boxes and multicast; each k-block issues
+// 4 x 2 wgmma.m64n128k32.e4m3 instead of 4 x 2 m64n128k16.f16.  The e4m3 operands carry one scale per A row (token) and one for
+// all of W, so C[m][n] = a_scale[m] w_scale sum_k qa[m][k] qw[n][k]: the main loop is a plain f32-accumulated MMA and the scale is one
+// multiply in the epilogue, x = acc (a_scale[m] w_scale), after which the epilogue runs unchanged on x.
 // Staged epilogue (qkv, proj, fc1, fc2): each MMA warpgroup has its own staging buffer outside the ring.  The tile leaves in passes
 // of one 64-row half x 64 or 128 columns: the warpgroup writes a pass as 64-row x 128-B boxes (SWIZZLE_128B, so the fragment-layout
 // writes are free of bank conflicts) and one thread stores them with TMA.  A pass reuses buffer space only once the stores of the
@@ -38,6 +43,12 @@
 #include "ptx.cuh"
 
 namespace vitb200 {
+
+enum GemmOperand
+{
+    GEMM_OP_F16 = 0,  // A and W f16, k-block of 64
+    GEMM_OP_E4M3 = 1, // A and W e4m3 with a per-row A scale and a per-tensor W scale (GemmParams), k-block of 128
+};
 
 enum GemmEpilogue
 {
@@ -64,12 +75,14 @@ struct GemmParams
     const float *resid; // EPI_BIAS_RESID_F32: [M][ldo] (may alias out)
     const float *pos;   // EPI_PATCH_F32: pos_embed [ntok][N]
     int np, ntok;       // EPI_PATCH_F32: patches / tokens per image
+    const float *a_scale; // GEMM_OP_E4M3: [M] f32, the scale of each A row
+    float w_scale;        // GEMM_OP_E4M3: the scale of W
 };
 
 constexpr int GEMM_BM = 128; // rows of a tile
 constexpr int GEMM_BN = 128; // columns of a tile (the W map's box rows)
 constexpr int GEMM_A_BOX_ROWS = GEMM_BM / 2; // the A map's box: each CTA of a cluster pair loads half of the A tile they share
-constexpr int GEMM_BK = 64;
+constexpr int GEMM_BK = 64; // f16 elements of a k-block (128 B per row); e4m3 k-blocks hold twice as many
 
 // Shared memory holds six 32 KB ring stages and two 16 KB staging buffers, or five stages and two 32 KB buffers.  A long reduction
 // (K >= GEMM_DEEP_K) is main-loop bound and wants the deeper ring to hide the L2 latency of its loads; a short one spends a larger
@@ -134,7 +147,7 @@ struct GemmStage
 // tmOut: the store map of out (f16: box 64 columns x 64 rows, 2-D [M][N] or, head-major, 3-D {64, M, N / 64 planes}; f32: box
 // 32 columns x 64 rows over [M][N]), SWIZZLE_128B.  tmAux: the same map over out2 (EPI_BIAS_F16_HILO) or the load map of resid
 // (EPI_BIAS_RESID_F32).  Both unused by the register epilogues.
-template <int EPI, int STAGES>
+template <int EPI, int STAGES, int OP = GEMM_OP_F16>
 __global__ void __launch_bounds__(384, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
                   const __grid_constant__ CUtensorMap tmAux, const GemmParams p)
@@ -142,6 +155,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     using Cfg = GemmCfg<STAGES>;
     constexpr int kStages = Cfg::kStages;
     constexpr bool kStaged = gemm_epi_staged(EPI);
+    constexpr bool kE4M3 = OP == GEMM_OP_E4M3;
+    static_assert(!kE4M3 || kStaged, "e4m3 operands: staged epilogues only");
+    constexpr int kKb = kE4M3 ? 2 * GEMM_BK : GEMM_BK; // K elements per k-block
     constexpr int kBarTurn = 1; // + warpgroup: named barrier "this warpgroup may start its next k-loop"
     constexpr int kBarWg = 3;   // + warpgroup: the warpgroup's own epilogue barrier
 
@@ -171,7 +187,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const unsigned n_pairs = (unsigned)(p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN);
     // pair u exists (its M band starts inside M); tested against p.M rather than a pair count, which would hold a register
     auto pair_exists = [&](unsigned u) { return (int)(u / n_pairs) * GEMM_BM < p.M; };
-    const int num_kb = (p.K + GEMM_BK - 1) / GEMM_BK;
+    const int num_kb = (p.K + kKb - 1) / kKb;
 
     if (threadIdx.x == 0)
     {
@@ -221,9 +237,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     // out-of-range rows / columns are zero-filled and still count their bytes; the A tile is shared by the pair,
                     // each CTA loads 64 of its rows into both CTAs
                     ptx::mbar_arrive_expect_tx(full_bar(s), Cfg::A_BYTES + Cfg::B_BYTES);
-                    ptx::tma_load_2d_multicast(sA + s * Cfg::A_BYTES + rank * (Cfg::A_BYTES / 2), &tmA, full_bar(s), kb * GEMM_BK,
+                    ptx::tma_load_2d_multicast(sA + s * Cfg::A_BYTES + rank * (Cfg::A_BYTES / 2), &tmA, full_bar(s), kb * kKb,
                                                m0 + rank * GEMM_A_BOX_ROWS, 0x3);
-                    ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * GEMM_BK, n0);
+                    ptx::tma_load_2d(sB + s * Cfg::B_BYTES, &tmB, full_bar(s), kb * kKb, n0);
                     if (++s == kStages) { s = 0; ph ^= 1; }
                 }
             }
@@ -279,10 +295,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             ptx::fence_regs(acc[1]);
             ptx::wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < GEMM_BK / 16; ++k) // +32 B along K per k16 step
+            for (int k = 0; k < 4; ++k) // +32 B along K per step: k16 (f16) or k32 (e4m3)
             {
-                ptx::wgmma_m64n128k16_f16(acc[0], adesc0 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
-                ptx::wgmma_m64n128k16_f16(acc[1], adesc1 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                if constexpr (kE4M3)
+                {
+                    ptx::wgmma_m64n128k32_e4m3(acc[0], adesc0 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                    ptx::wgmma_m64n128k32_e4m3(acc[1], adesc1 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                }
+                else
+                {
+                    ptx::wgmma_m64n128k16_f16(acc[0], adesc0 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                    ptx::wgmma_m64n128k16_f16(acc[1], adesc1 + 2 * k, bdesc + 2 * k, (kb | k) != 0);
+                }
             }
             ptx::wgmma_commit();
             ptx::wgmma_wait<1>(); // the previous k-block's MMAs have retired: its slot can be refilled
@@ -312,6 +336,18 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (c0 >= p.N || m0 + 64 * hm >= p.M) continue; // nothing of this pass is stored (uniform over the warpgroup)
                 const int ncb = min(St::kColBoxes, (p.N - c0 + St::kBoxCols - 1) / St::kBoxCols); // boxes that start inside N
                 const uint32_t buf = stage + (ps % St::kSlots) * St::kPassBytes;
+                // e4m3: the scales of this thread's two rows of the pass (rr and rr + 8 of row half hm) times the W scale, rows past M
+                // not stored; read per pass (four held from the k-loop on cost the split epilogue a spill), under the barrier below
+                float row_scale[2];
+                if constexpr (kE4M3)
+                {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+                    {
+                        const int row = m0 + 64 * hm + rr + 8 * h;
+                        row_scale[h] = row < p.M ? __fmul_rn(__ldg(p.a_scale + row), p.w_scale) : 0.f;
+                    }
+                }
                 if (ps > 0 && tid == 0)
                 {
                     if (ps >= St::kSlots) ptx::tma_store_wait_read<St::kSlots - 1>(); // the stores of the pass that used buf have read it
@@ -331,7 +367,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
                     {
-                        const float x0 = __fadd_rn(acc[hm][4 * j + 2 * h], b.x), x1 = __fadd_rn(acc[hm][4 * j + 2 * h + 1], b.y);
+                        float a0 = acc[hm][4 * j + 2 * h], a1 = acc[hm][4 * j + 2 * h + 1];
+                        if constexpr (kE4M3) { a0 = __fmul_rn(a0, row_scale[h]); a1 = __fmul_rn(a1, row_scale[h]); }
+                        const float x0 = __fadd_rn(a0, b.x), x1 = __fadd_rn(a1, b.y);
                         const uint32_t row = buf + (uint32_t)(rr + 8 * h) * 128u;
                         if constexpr (St::kF16)
                         {

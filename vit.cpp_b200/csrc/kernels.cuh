@@ -3,7 +3,7 @@
 //                            reshuffle: pixels HWC f32 -> f16 patch rows, K order c*P*P + ky*P + kx
 //   cls_rows_kernel          token 0 = cls_token + pos_embed[0]                      (vit.cpp:794-797)
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
-//                            and un-normalised forms write the encoder features (vitb200_features)
+//                            and un-normalised forms write the encoder features (vitb200_features), its e4m3 form the FP8 A operand
 //   attention_kernel         per (image, head): S = QK^T / sqrt(hd), softmax with the reference's f16-exp
 //                            semantics (ggml.c:10536-10558), O = P V   (vit.cpp:826-866)
 //   softmax_topk_kernel      final soft-max (vit.cpp:931) + top-k (replaces the host std::sort, vit.cpp:1047-1057)
@@ -11,6 +11,7 @@
 #include "ptx.cuh"
 
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <type_traits>
 
 namespace vitb200 {
@@ -144,11 +145,15 @@ __device__ __forceinline__ void store4(OutT *__restrict__ yr, int i, bool live, 
 // reference's NORM, MUL, ADD nodes, then RNE to f16 (the GEMM's src1 conversion, ggml.c:9493-9506).
 // OutT = float stores those f32 values before that rounding, __nv_bfloat16 rounds them to nearest even bf16 instead.
 // NORM = false skips the normalisation: the selected rows of x are converted and stored as they are (w and b are not read).
+// OutT = __nv_fp8_e4m3 (FP8 engine, NORM only) quantises each row of those f32 values with its own scale: amax = max |y| over the row,
+// y_scale[row] = amax / 448 and y = e4m3_rn_satfinite(y (448 / amax)); an all-zero row gets scale 1.
 template <int MAXV, typename OutT = __half, bool NORM = true>
 __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_stride, int rows_per_group, size_t group_stride,
                                      const float *__restrict__ w, const float *__restrict__ b, OutT *__restrict__ y, int rows,
-                                     int D, float eps)
+                                     int D, float eps, float *__restrict__ y_scale)
 {
+    constexpr bool kE4M3 = std::is_same<OutT, __nv_fp8_e4m3>::value;
+    static_assert(!kE4M3 || NORM, "e4m3 output: normalised rows only");
     ptx::grid_dep_launch(); // PDL: blocks may be resident before the producing GEMM has drained
     ptx::grid_dep_wait();
     const int warps_per_block = blockDim.x >> 5;
@@ -200,6 +205,7 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
     const float4 *b4 = reinterpret_cast<const float4 *>(b);
     const bool vec16 = (nvec & 1) == 0;
     OutT *yr = y + (size_t)row * D;
+    float amax = 0.f;
 #pragma unroll
     for (int j = 0; j < MAXV; ++j)
     {
@@ -220,7 +226,27 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
                 o0 = v[j].x; o1 = v[j].y; o2 = v[j].z; o3 = v[j].w;
             }
         }
-        store4(yr, i, i < nvec, vec16, o0, o1, o2, o3);
+        if constexpr (kE4M3)
+        {
+            v[j] = make_float4(o0, o1, o2, o3);
+            amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3))));
+        }
+        else store4(yr, i, i < nvec, vec16, o0, o1, o2, o3);
+    }
+    if constexpr (kE4M3)
+    {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        const float inv = amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f;
+        if (lane == 0) y_scale[row] = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            const int i = lane + 32 * j;
+            if (i < nvec)
+                reinterpret_cast<uint32_t *>(yr)[i] =
+                    ptx::cvt_e4m3x4(__fmul_rn(v[j].x, inv), __fmul_rn(v[j].y, inv), __fmul_rn(v[j].z, inv), __fmul_rn(v[j].w, inv));
+        }
     }
 }
 
@@ -230,19 +256,22 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
 // shared-memory ring with cp.async.bulk + mbarrier, warps 0-7 each normalise one row out of shared memory (identical arithmetic to the
 // kernel above, w / b kept in registers for the whole launch) into a double-buffered staging block that leaves as ONE contiguous
 // bulk store of 8 f16 rows.  Purpose: the row-per-warp kernel above reaches 5.9 TB/s alone but 4.8 TB/s inside the step (6 304 short
-// blocks ramping up and draining between two persistent GEMMs).
+// blocks ramping up and draining between two persistent GEMMs).  OutT = __nv_fp8_e4m3: the FP8 engine's per-row quantisation, as
+// layernorm_f16_kernel does it; the row scales go straight to y_scale.
 constexpr int LN_TMA_ROWS = 8, LN_TMA_STAGES = 3, LN_TMA_THREADS = 288;
 __host__ __device__ inline int layernorm_tma_smem_bytes(int D) { return 128 + LN_TMA_STAGES * LN_TMA_ROWS * D * 4 + 2 * LN_TMA_ROWS * D * 2 + 64; }
 
-template <int NV> // float4 per lane = D / 128
+template <int NV, typename OutT = __half> // float4 per lane = D / 128
 __global__ void __launch_bounds__(LN_TMA_THREADS, 2)
-layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, const float *__restrict__ b, __half *__restrict__ y, int rows, float eps)
+layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, const float *__restrict__ b, OutT *__restrict__ y, int rows, float eps,
+                     float *__restrict__ y_scale)
 {
     constexpr int D = NV * 128;
+    constexpr bool kE4M3 = std::is_same<OutT, __nv_fp8_e4m3>::value;
     extern __shared__ uint8_t ln_smem_raw[];
     const uint32_t base = (ptx::smem_u32(ln_smem_raw) + 127u) & ~127u;
     uint8_t *smem = ln_smem_raw + (base - ptx::smem_u32(ln_smem_raw));
-    constexpr uint32_t IN_BYTES = LN_TMA_ROWS * D * 4, OUT_BYTES = LN_TMA_ROWS * D * 2;
+    constexpr uint32_t IN_BYTES = LN_TMA_ROWS * D * 4, OUT_BYTES = LN_TMA_ROWS * D * sizeof(OutT);
     const uint32_t s_in = base, s_out = base + LN_TMA_STAGES * IN_BYTES, bars = s_out + 2 * OUT_BYTES;
     auto full_bar = [&](int st) { return bars + 8u * st; };
     auto empty_bar = [&](int st) { return bars + 8u * (LN_TMA_STAGES + st); };
@@ -318,7 +347,31 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
             const uint32_t ob = s_out + (uint32_t)(it & 1) * OUT_BYTES;
             if (threadIdx.x == 0) ptx::tma_store_wait_read<1>();
             ptx::named_bar_sync(1, 32 * LN_TMA_ROWS);
-            if (warp < nr)
+            if constexpr (kE4M3)
+            {
+                if (warp < nr)
+                {
+                    float amax = 0.f;
+#pragma unroll
+                    for (int j = 0; j < NV; ++j)
+                    {
+                        v[j].x = __fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww[j].x), bb[j].x);
+                        v[j].y = __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww[j].y), bb[j].y);
+                        v[j].z = __fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww[j].z), bb[j].z);
+                        v[j].w = __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww[j].w), bb[j].w);
+                        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
+                    }
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+                    const float inv = amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f;
+                    if (lane == 0) y_scale[row0 + warp] = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+                    uint32_t *yr = reinterpret_cast<uint32_t *>(smem + (ob - base) + (size_t)warp * D);
+#pragma unroll
+                    for (int j = 0; j < NV; ++j)
+                        yr[lane + 32 * j] = ptx::cvt_e4m3x4(__fmul_rn(v[j].x, inv), __fmul_rn(v[j].y, inv), __fmul_rn(v[j].z, inv), __fmul_rn(v[j].w, inv));
+                }
+            }
+            else if (warp < nr)
             {
                 uint2 *yr = reinterpret_cast<uint2 *>(smem + (ob - base) + (size_t)warp * D * 2);
 #pragma unroll
@@ -336,7 +389,7 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
             ptx::named_bar_sync(1, 32 * LN_TMA_ROWS);
             if (threadIdx.x == 0)
             {
-                ptx::bulk_store_1d(y + (size_t)row0 * D, ob, (uint32_t)(nr * D * 2));
+                ptx::bulk_store_1d(y + (size_t)row0 * D, ob, (uint32_t)(nr * D * sizeof(OutT)));
                 ptx::tma_store_commit();
             }
             if (++st == LN_TMA_STAGES) { st = 0; ph ^= 1; }

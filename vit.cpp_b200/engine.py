@@ -68,6 +68,12 @@ def lib():
         L.vitb200_in_chans.argtypes = [vp]
         L.vitb200_head_tokens.argtypes = [vp]
         L.vitb200_create.argtypes = [vp, vp, i32, i32, i32, C.POINTER(vp)]
+        L.vitb200_create_fp8.argtypes = [vp, vp, i32, i32, i32, i32, C.POINTER(vp)]
+        L.vitb200_create_from_file_fp8.argtypes = [C.c_char_p, i32, i32, i32, C.POINTER(vp)]
+        L.vitb200_fp8.argtypes = [vp]
+        L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
+        L.vitb200_test_gemm_fp8.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
+        L.vitb200_test_layernorm_fp8.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
         L.vitb200_destroy.argtypes = [vp]
         L.vitb200_destroy.restype = None
         L.vitb200_get_hparams.argtypes = [vp, C.POINTER(Hparams)]
@@ -120,6 +126,7 @@ class VitModel:
         self.n_tokens = (hp.img_size // hp.patch_size) ** 2 + 1
         self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713)
         self.head_tokens = lib().vitb200_head_tokens(self._h)  # classifier rows per image (1, or 25 for ViTSTR)
+        self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
         self._labels = None
 
     def label(self, i: int) -> Optional[str]:
@@ -151,18 +158,20 @@ class VitModel:
             pass
 
 
-def vit_model_load(fname: str, device: int = 0, max_batch: int = 256, head_tokens: int = 1) -> VitModel:
+def vit_model_load(fname: str, device: int = 0, max_batch: int = 256, head_tokens: int = 1, fp8: bool = False) -> VitModel:
     """reference: bool vit_model_load(const std::string &fname, vit_model &model)  (vit.cpp:308).  head_tokens = 25 loads a
-    ViTSTR model (reference extensions/vitstr.cpp: 1-channel input, classifier over the first 25 tokens)."""
+    ViTSTR model (reference extensions/vitstr.cpp: 1-channel input, classifier over the first 25 tokens).  fp8 = True builds the
+    FP8 engine (vitb200_create_from_file_fp8: qkv and fc1 on the e4m3 tensor cores, numerics in include/vitb200.h)."""
     h = C.c_void_p()
-    _check(lib().vitb200_create_from_file_ex(fname.encode(), device, max_batch, head_tokens, C.byref(h)), "vit_model_load")
+    create = lib().vitb200_create_from_file_fp8 if fp8 else lib().vitb200_create_from_file_ex
+    _check(create(fname.encode(), device, max_batch, head_tokens, C.byref(h)), "vit_model_load")
     return VitModel(h, device, max_batch)
 
 
-def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens: int = 1, edit=None) -> VitModel:
+def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens: int = 1, edit=None, fp8: bool = False) -> VitModel:
     """vitb200_create_ex with a caller-built tensor list -- what the vit.h-side shim does with vit_model::tensors.  `vf` is a parsed
     model file (ggml_file.VitFile: numpy-shaped f32 / f16 arrays); `edit(entries)` may reorder / duplicate / reshape the list of
-    [name, array, ggml_type, ne] entries first (tests of the loader's shape and name checks)."""
+    [name, array, ggml_type, ne] entries first (tests of the loader's shape and name checks).  fp8 = True: vitb200_create_fp8."""
     entries = []
     for name, arr in vf.tensors.items():
         if name.endswith(".q8_0_raw"):
@@ -186,7 +195,8 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
             t.ne[i] = ne[i] if i < len(ne) else 1
     hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, 1e-6)
     h = C.c_void_p()
-    _check(lib().vitb200_create_ex(C.byref(hp), ts, len(entries), device, max_batch, head_tokens, C.byref(h)), "vitb200_create")
+    create = lib().vitb200_create_fp8 if fp8 else lib().vitb200_create_ex
+    _check(create(C.byref(hp), ts, len(entries), device, max_batch, head_tokens, C.byref(h)), "vitb200_create")
     return VitModel(h, device, max_batch)
 
 
@@ -451,3 +461,39 @@ def test_layernorm(x, w, b, eps: float = 1e-6, device: int = 0):
     _check(lib().vitb200_test_layernorm(device, x.shape[0], x.shape[1], x.ctypes.data, w.ctypes.data, b.ctypes.data, eps, y.ctypes.data),
            "vitb200_test_layernorm")
     return y
+
+
+def test_quantize_fp8(w16: np.ndarray):
+    """Host-only: the FP8 engine's weight quantisation (vitb200_test_quantize_fp8): float16 array -> (uint8 e4m3 bytes, same shape;
+    f32 scale)."""
+    w = np.ascontiguousarray(w16, np.float16)
+    q = np.empty(w.shape, np.uint8)
+    sc = C.c_float(0.0)
+    _check(lib().vitb200_test_quantize_fp8(w.ctypes.data, w.size, q.ctypes.data, C.cast(C.pointer(sc), C.c_void_p)),
+           "vitb200_test_quantize_fp8")
+    return q, sc.value
+
+
+def test_gemm_fp8(M: int, N: int, K: int, epilogue: int, A8: np.ndarray, a_scale: np.ndarray, W8: np.ndarray, w_scale: float,
+                  bias: np.ndarray, device: int = 0) -> np.ndarray:
+    """The e4m3 GEMM alone (vitb200_test_gemm_fp8): A8 uint8 [M][K], W8 uint8 [N][K] e4m3 bytes -> float32 [M][N]."""
+    A = np.ascontiguousarray(A8, np.uint8)
+    W = np.ascontiguousarray(W8, np.uint8)
+    sa = np.ascontiguousarray(a_scale, np.float32)
+    b = np.ascontiguousarray(bias, np.float32)
+    out = np.empty((M, N), np.float32)
+    _check(lib().vitb200_test_gemm_fp8(device, M, N, K, epilogue, A.ctypes.data, sa.ctypes.data, W.ctypes.data, float(w_scale),
+                                       b.ctypes.data, out.ctypes.data), "vitb200_test_gemm_fp8")
+    return out
+
+
+def test_layernorm_fp8(x, w, b, eps: float = 1e-6, device: int = 0):
+    """The FP8 engine's block LayerNorm alone (vitb200_test_layernorm_fp8): x float32 [rows][D] -> (uint8 e4m3 [rows][D], float32 [rows])."""
+    x = np.ascontiguousarray(x, np.float32)
+    w = np.ascontiguousarray(w, np.float32)
+    b = np.ascontiguousarray(b, np.float32)
+    q = np.empty(x.shape, np.uint8)
+    sa = np.empty(x.shape[0], np.float32)
+    _check(lib().vitb200_test_layernorm_fp8(device, x.shape[0], x.shape[1], x.ctypes.data, w.ctypes.data, b.ctypes.data, eps,
+                                            q.ctypes.data, sa.ctypes.data), "vitb200_test_layernorm_fp8")
+    return q, sa
