@@ -56,7 +56,11 @@ typedef struct vitb200_tensor
 /* Create an engine from weights that already live in host memory (this is what a vit.h-side shim calls with
  * the contents of vit_model::tensors).  Weights are repacked and uploaded once; the host arena is not retained.
  * max_batch bounds the batch accepted by vitb200_forward*.  Replaces, per model, what the reference re-does per
- * image in vit_predict (graph build x2, ggml_allocr, thread pool; vit.cpp:1009-1036). */
+ * image in vit_predict (graph build x2, ggml_allocr, thread pool; vit.cpp:1009-1036).
+ * Accepted shapes (every create function; anything else fails here, with a message naming the limit, not in the first forward):
+ *   head dim 64 (hidden_size = 64 * num_attention_heads), hidden_size <= 2048 (the widest LayerNorm row a warp holds);
+ *   patch_size 8, 14, 16 or 32 for 3-channel input, 8 or 16 for 1-channel input, dividing img_size;
+ *   at most 896 tokens, (img_size / patch_size)^2 + 1 (K and V of one attention head in 227 KB of shared memory). */
 int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                    vitb200_engine **out);
 

@@ -145,3 +145,21 @@ def test_zeroed_hyper_parameters_are_rejected_not_divided_by(tmp_path):
         with pytest.raises(eng.VitB200Error) as ei:
             eng.vit_model_load(str(f))
         assert "invalid" in str(ei.value) or "expected" in str(ei.value), str(ei.value)
+
+
+@pytest.mark.parametrize("hp,in_chans,limit", [
+    ((64, 1, 1, 12, 24), 3, "patch size 12 not supported for 3-channel input (8, 14, 16, 32)"),
+    ((64, 1, 1, 14, 28), 1, "patch size 14 not supported for 1-channel input (8, 16)"),
+    ((64, 1, 1, 8, 240), 3, "901 tokens not supported (max 896"),
+    ((2112, 1, 33, 16, 32), 3, "hidden size 2112 not supported (max 2048)"),
+], ids=["patch12", "gray_patch14", "tokens901", "hidden2112"])
+def test_shapes_without_a_kernel_are_rejected_at_load(hp, in_chans, limit, tmp_path):
+    """Real checkpoints reach these shapes (a grayscale P 14 model, ViT-S/8 at 240 px, a hidden size past the widest LayerNorm): such a
+    file must fail to load, naming the limit, instead of loading and then failing in every forward call.  Checked ahead of the device
+    probe, so it is testable here; the largest accepted shapes load and run in tests/test_gpu_geometry.py (d2048, p8 at 785 tokens)."""
+    f = str(tmp_path / "m.bin")
+    gf.write_synthetic(f, hp, 1, classes=10, in_chans=in_chans)
+    for fp8 in (False, True):
+        with pytest.raises(eng.VitB200Error) as ei:
+            eng.vit_model_load(f, fp8=fp8)
+        assert limit in str(ei.value), str(ei.value)

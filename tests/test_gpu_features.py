@@ -42,7 +42,7 @@ def final_ln_tap(m, imgs):
     return out
 
 
-@pytest.mark.parametrize("cfg", ["micro", "tiny", "large384x2"])
+@pytest.mark.parametrize("cfg", ["micro", "tiny", "large384x2", "d1536"])   # d1536: the row-per-warp kernel at 12 of 16 float4 per lane
 def test_features_match_restatement(cfg):
     path = model_path(cfg, "f16")
     vf = gf.read(path)
@@ -88,8 +88,8 @@ def test_prelogits_are_the_head_input(cfg, head_tokens):
     m.close()
 
 
-def test_16_bit_outputs_are_the_f32_output_rounded():
-    m = eng.vit_model_load(model_path("tiny", "f16"), 0, 4)
+def _check_16_bit_outputs_are_the_f32_output_rounded(cfg):
+    m = eng.vit_model_load(model_path(cfg, "f16"), 0, 4)
     L = m.hparams.num_hidden_layers
     imgs = gf.synthetic_images(3, m.img_size, seed=15)
     for layers in (0, L - 1, L):
@@ -102,6 +102,15 @@ def test_16_bit_outputs_are_the_f32_output_rounded():
             assert np.array_equal(p16.view(np.uint16), p32.astype(np.float16).view(np.uint16)), (layers, norm)
             assert np.array_equal(tbf, bf16_bits(t32)) and np.array_equal(pbf, bf16_bits(p32)), (layers, norm)
     m.close()
+
+
+def test_16_bit_outputs_are_the_f32_output_rounded():
+    _check_16_bit_outputs_are_the_f32_output_rounded("tiny")
+
+
+def test_16_bit_outputs_of_the_widest_layernorm_are_the_f32_output_rounded():
+    """d1536: the f16 and bf16 forms of the row-per-warp kernel at 16 float4 per lane (1024 < D <= 2048)."""
+    _check_16_bit_outputs_are_the_f32_output_rounded("d1536")
 
 
 def test_batch_invariance_and_graph_replay():

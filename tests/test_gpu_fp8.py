@@ -111,7 +111,8 @@ def test_gemm_random_against_f64(K):
 
 
 # ---- LayerNorm -> e4m3 ---------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("rows,D", [(1, 768), (7, 768), (8, 768), (9, 768), (591, 768), (1154, 1024), (4097, 128), (34, 128), (50, 192), (2, 384)])
+@pytest.mark.parametrize("rows,D", [(1, 768), (7, 768), (8, 768), (9, 768), (591, 768), (1154, 1024), (4097, 128), (34, 128), (50, 192), (2, 384),
+                                    (591, 256), (591, 384), (57, 512), (4097, 640), (300, 896), (9, 1536), (33, 2048)])
 def test_layernorm_e4m3_matches_the_emulation(rows, D):
     """Both kernels (bulk-copy for D % 128 == 0 and >= 8 rows, row-per-warp otherwise), the row counts of
     test_layernorm_matches_the_restatement.  The kernel's f32 LayerNorm and the restatement's differ in the last bits, so a value near an

@@ -139,13 +139,17 @@ ATTN_CASES = [  # (B, N, H, kernel)
     (3, 17, 2, eng.ATTN_WGMMA), (2, 197, 3, eng.ATTN_WGMMA), (2, 197, 3, eng.ATTN_MMA8),
     (2, 577, 2, eng.ATTN_MMA16), (2, 577, 2, eng.ATTN_MMA8), (1, 225, 1, eng.ATTN_MMA16), (3, 384, 1, eng.ATTN_MMA16),
     (2, 401, 2, eng.ATTN_MMA16), (1, 640, 1, eng.ATTN_MMA16), (20, 577, 16, eng.ATTN_MMA16),
+    # 8 warps past the 16-warp kernel's 640 keys, as the engine picks it (ViT-S/8, ViT-B/8: 785 tokens); 896 is the largest token count
+    # whose K and V fit in shared memory, the largest request of any attention launch
+    (2, 785, 2, eng.ATTN_MMA8), (3, 700, 4, eng.ATTN_AUTO), (1, 896, 1, eng.ATTN_MMA8),
 ]
 
 
 @pytest.mark.parametrize("B,N,H,kernel", ATTN_CASES)
 def test_attention_kernels_against_numpy(B, N, H, kernel):
     """Every attention kernel, alone, on random QKV (scores spread over several units so the soft-max is not flat): agreement with
-    the float64 restatement to f16 output rounding + f32 accumulation noise; the last case launches many (image, head) problems."""
+    the float64 restatement to f16 output rounding + f32 accumulation noise; the (20, 577, 16) case launches many (image, head)
+    problems.  At 896 tokens, one more token is refused by the launcher before anything runs."""
     rng = np.random.default_rng(N * 131 + H)
     qkv = rng.normal(0.0, 1.0, (B * N, 3 * H * 64)).astype(np.float32)
     qkv[:, : H * 64] *= 1.5                       # Q: |s/8| up to ~5
@@ -156,6 +160,11 @@ def test_attention_kernels_against_numpy(B, N, H, kernel):
     err = np.abs(out - ref)
     tol = 2.0 ** -10 * np.abs(ref) + 2e-3 * np.abs(ref).max()
     assert (err <= tol).all(), (err.max(), np.abs(ref).max(), np.unravel_index(err.argmax(), err.shape))
+    if N == 896:
+        more = rng.normal(0.0, 1.0, (B * 897, 3 * H * 64)).astype(np.float16)
+        with pytest.raises(eng.VitB200Error) as ei:
+            eng.test_attention(more, B, 897, H, kernel)
+        assert "897 tokens do not fit" in str(ei.value) and "max 896" in str(ei.value)
 
 
 # ---- q8_0 linear layer on the integer tensor cores (prototype, BASELINE.json configs[4]) ---------------------------------------
@@ -186,10 +195,12 @@ def test_q8_0_gemm_matches_the_reference_integer_dot(M, N, K):
 
 
 # ---- LayerNorm: the persistent bulk-copy kernel (D % 128 == 0, >= 8 rows) and the row-per-warp kernel behind the same launcher -----------
-@pytest.mark.parametrize("rows,D", [(1, 768), (7, 768), (8, 768), (9, 768), (591, 768), (1154, 1024), (4097, 128), (34, 128), (50, 192), (2, 384)])
+@pytest.mark.parametrize("rows,D", [(1, 768), (7, 768), (8, 768), (9, 768), (591, 768), (1154, 1024), (4097, 128), (34, 128), (50, 192), (2, 384),
+                                    (591, 256), (591, 384), (57, 512), (4097, 640), (300, 896), (9, 1536), (33, 2048)])
 def test_layernorm_matches_the_restatement(rows, D):
     """Row counts around the 8-row block size (partial last block, fewer rows than one block -> row-per-warp kernel), more blocks than
-    resident CTAs, hidden sizes of every model in the tests; against the oracle's ggml_norm * w + b rounded to f16 (the GEMM's src1
+    resident CTAs; hidden sizes of every bulk-copy instantiation (D / 128 = 1 ... 7 float4 per lane) and of every row-per-warp one up to
+    the largest accepted hidden size (16 float4 per lane at D = 2048); against the oracle's ggml_norm * w + b rounded to f16 (the GEMM's src1
     conversion): at most one f16 ulp apart (the reference sums in double, the kernel in f32), bit-equal on > 99.5 % of the elements."""
     rng = np.random.default_rng(rows * 131 + D)
     x = (rng.standard_normal((rows, D)) * rng.uniform(0.5, 4.0, (rows, 1)) + rng.uniform(-1, 1, (rows, 1))).astype(np.float32)

@@ -432,8 +432,10 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)GEMM_BN);
 }
 
-// dynamic shared memory the soft-max kernel may use for its working row (227 KB per CTA minus its static arrays)
-constexpr size_t kSoftmaxSmemMax = 232448 - 1024;
+// the largest dynamic shared memory one CTA may opt in to on sm_90 (227 KB)
+constexpr int kSmemOptinMax = 232448;
+// dynamic shared memory the soft-max kernel may use for its working row (the per-CTA limit minus its static arrays)
+constexpr size_t kSoftmaxSmemMax = kSmemOptinMax - 1024;
 
 enum ProfKind { PK_PATCH = 0, PK_QKV, PK_PROJ, PK_FC1, PK_FC2, PK_HEAD, PK_ATTN, PK_LN, PK_COUNT };
 
@@ -553,14 +555,19 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
 
+// The patch sizes launch_patchify has a kernel for, by channel count (vitb200_create rejects any other)
+inline bool patchify_supports(int P, int C) { return C == 1 ? (P == 8 || P == 16) : (P == 8 || P == 14 || P == 16 || P == 32); }
+inline const char *patchify_sizes(int C) { return C == 1 ? "8, 16" : "8, 14, 16, 32"; }
+
 int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaStream_t s)
 {
     const long long total = (long long)B * e->G * e->hp.patch_size * e->G;
     const int threads = 256;
     const int blocks = (int)((total + threads - 1) / threads);
+    if (!patchify_supports(e->hp.patch_size, e->C))
+        return fail("%d-channel input: patch size %d not supported (%s)", e->C, e->hp.patch_size, patchify_sizes(e->C));
     if (e->C == 1)
     {
-        if (e->hp.patch_size != 16 && e->hp.patch_size != 8) return fail("1-channel input: patch size %d not supported (8, 16)", e->hp.patch_size);
         if (e->hp.patch_size == 16) patchify_f16_kernel<16, 1><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp);
         else patchify_f16_kernel<8, 1><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp);
         CUDA_TRY(cudaGetLastError());
@@ -579,7 +586,7 @@ int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaS
     case 14: patchify_f16_kernel<14><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
     case 8: patchify_f16_kernel<8><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
     case 32: patchify_f16_kernel<32><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
-    default: return fail("patch size %d not supported (8, 14, 16, 32)", e->hp.patch_size);
+    default: return fail("patch size %d not supported (%s)", e->hp.patch_size, patchify_sizes(e->C));
     }
     CUDA_TRY(cudaGetLastError());
     e->launches++;
@@ -588,7 +595,11 @@ int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaS
 
 // The row-per-warp kernel: the LayerNorms the bulk-copy kernel below does not take (pooled rows, hidden sizes that are not a multiple
 // of 128) and, with an f32 / bf16 output or NORM = false, the encoder features.  rows_per_group <= 0: all rows are one group.
-// OutT = __nv_fp8_e4m3: y_scale receives the per-row scales.
+// OutT = __nv_fp8_e4m3: y_scale receives the per-row scales.  A lane holds up to LN_ROWS_MAX_V float4 of its row, which bounds the
+// hidden size the engine accepts.
+constexpr int LN_ROWS_MAX_V = 16;
+constexpr int LN_MAX_HIDDEN = LN_ROWS_MAX_V * 128;
+
 template <typename OutT, bool NORM>
 int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
                           cudaStream_t s, int rows_per_group, size_t group_stride, float *y_scale = nullptr)
@@ -599,8 +610,8 @@ int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride
     const int blocks = (rows + rows_per_block - 1) / rows_per_block;
     if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
     else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
-    else if (D <= 16 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<16, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
-    else return fail("hidden size %d not supported (max 2048)", D);
+    else if (D <= LN_MAX_HIDDEN) CUDA_TRY(launch_pdl(layernorm_f16_kernel<LN_ROWS_MAX_V, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
+    else return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     CUDA_TRY(cudaGetLastError());
     e->launches++;
     return 0;
@@ -684,13 +695,19 @@ int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
     return 0;
 }
 
+// The mma.sync kernels hold K and V of one (image, head) problem in shared memory: N tokens padded to whole key chunks, 64 f16 each.
+// That bounds the token count the engine accepts.
+constexpr int attention_smem_bytes(int N) { return 2 * ((N + ATT_KC - 1) / ATT_KC * ATT_KC) * 128; }
+constexpr int ATT_MAX_TOKENS = kSmemOptinMax / (2 * 128) / ATT_KC * ATT_KC;
+static_assert(attention_smem_bytes(ATT_MAX_TOKENS) <= kSmemOptinMax && attention_smem_bytes(ATT_MAX_TOKENS + 1) > kSmemOptinMax);
+
 template <int NW>
 int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int N = e->N, D = e->hp.hidden_size, H = e->hp.num_attention_heads;
     const int Npad = (N + ATT_KC - 1) / ATT_KC * ATT_KC;
-    const int smem = 2 * Npad * 128;
-    if (smem > 232448) return fail("attention: %d tokens do not fit in shared memory", N);
+    const int smem = attention_smem_bytes(N);
+    if (smem > kSmemOptinMax) return fail("attention: %d tokens do not fit in shared memory (max %d)", N, ATT_MAX_TOKENS);
     auto kern = attention_kernel<NW>;
     static int smem_set[64] = {};
     int dev = 0;
@@ -1061,6 +1078,22 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         hp->patch_size < 1 || hp->patch_size > 64 || hp->img_size < hp->patch_size || hp->img_size > 4096 || n < 1)
         return fail("invalid hyper-parameters (hidden %d, layers %d, heads %d, classes %d, patch %d, img %d)", hp->hidden_size,
                     hp->num_hidden_layers, hp->num_attention_heads, hp->num_classes, hp->patch_size, hp->img_size);
+    // input channels from the patch kernel [P, P, C, D] (vit.cpp:515; C = 1 in vitstr.cpp:482)
+    const vitb200_tensor *pw = find_tensor(t, n, "patch_embed.proj.weight");
+    const int64_t per_c = (int64_t)hp->hidden_size * hp->patch_size * hp->patch_size;
+    if (!pw || nelem(pw) % per_c != 0 || (nelem(pw) / per_c != 1 && nelem(pw) / per_c != 3))
+        return fail("tensor 'patch_embed.proj.weight' is missing or is not a 1- or 3-channel %dx%d kernel", hp->patch_size, hp->patch_size);
+    const int in_chans = (int)(nelem(pw) / per_c);
+    // shapes no kernel is built for: rejected here, where the caller can act on it, rather than by every forward call
+    if (hp->hidden_size % hp->num_attention_heads != 0 || hp->hidden_size / hp->num_attention_heads != 64)
+        return fail("head dim %d not supported (64 only)", hp->hidden_size / hp->num_attention_heads);
+    if (hp->img_size % hp->patch_size != 0) return fail("img_size %d not a multiple of patch_size %d", hp->img_size, hp->patch_size);
+    if (!patchify_supports(hp->patch_size, in_chans))
+        return fail("patch size %d not supported for %d-channel input (%s)", hp->patch_size, in_chans, patchify_sizes(in_chans));
+    if (hp->hidden_size > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", hp->hidden_size, LN_MAX_HIDDEN);
+    const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + 1;
+    if (n_tokens > ATT_MAX_TOKENS)
+        return fail("%d tokens not supported (max %d: K and V of one attention head must fit in shared memory)", n_tokens, ATT_MAX_TOKENS);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
         return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
@@ -1069,10 +1102,6 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-    if (hp->hidden_size % hp->num_attention_heads != 0 || hp->hidden_size / hp->num_attention_heads != 64)
-        return fail("head dim %d not supported (64 only)", hp->num_attention_heads ? hp->hidden_size / hp->num_attention_heads : 0);
-    if (hp->hidden_size % 64 != 0) return fail("hidden size %d must be a multiple of 64", hp->hidden_size);
-    if (hp->img_size % hp->patch_size != 0) return fail("img_size %d not a multiple of patch_size %d", hp->img_size, hp->patch_size);
     if (max_batch < 1) return fail("max_batch must be >= 1");
     if (check_unique_names(t, n)) return 1;
 
@@ -1087,18 +1116,7 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     e->G = hp->img_size / P;
     e->NP = e->G * e->G;
     e->N = e->NP + 1;
-    {
-        // input channels from the patch kernel [P, P, C, D] (vit.cpp:515; C = 1 in vitstr.cpp:482)
-        const vitb200_tensor *pw = find_tensor(t, n, "patch_embed.proj.weight");
-        const int64_t per_c = (int64_t)D * P * P;
-        if (!pw || nelem(pw) % per_c != 0 || (nelem(pw) / per_c != 1 && nelem(pw) / per_c != 3))
-        {
-            delete e;
-            e = nullptr;
-            return fail("tensor 'patch_embed.proj.weight' is missing or is not a 1- or 3-channel %dx%d kernel", P, P);
-        }
-        e->C = (int)(nelem(pw) / per_c);
-    }
+    e->C = in_chans;
     if (head_tokens < 1 || head_tokens > e->N) { const int ntok = e->N; delete e; e = nullptr; return fail("head_tokens %d out of range (1..%d)", head_tokens, ntok); }
     e->head_tokens = head_tokens;
     e->Cp = (hp->num_classes + 3) / 4 * 4;

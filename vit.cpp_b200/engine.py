@@ -365,16 +365,21 @@ TAP_SHAPES = {
 
 
 def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=tuple(TAP_SHAPES)):
-    """Forward with intermediates copied back (tests only)."""
+    """Forward with intermediates copied back (tests only).  For a ViTSTR model (head_tokens = n) the outputs and the final_ln tap
+    gain a token axis, as in vit_predict."""
     imgs = np.ascontiguousarray(images, dtype=np.float32)
+    if imgs.ndim == (3 if model.in_chans == 3 else 2):
+        imgs = imgs[None]
     B = imgs.shape[0]
-    probs = np.empty((B, model.num_classes), np.float32)
-    logits = np.empty((B, model.num_classes), np.float32)
+    lead = (B,) if model.head_tokens == 1 else (B, model.head_tokens)
+    probs = np.empty(lead + (model.num_classes,), np.float32)
+    logits = np.empty(lead + (model.num_classes,), np.float32)
     tp = Taps()
     tp.layer = tap_layer
     out = {}
     for n in taps:
-        out[n] = np.zeros(TAP_SHAPES[n](B, model.n_tokens, model.hidden_size), np.float32)
+        shape = TAP_SHAPES[n](B, model.n_tokens, model.hidden_size)
+        out[n] = np.zeros(lead + shape[1:] if n == "final_ln" else shape, np.float32)
         setattr(tp, n, out[n].ctypes.data)
     _check(lib().vitb200_forward_debug(model.handle, imgs.ctypes.data, B, probs.ctypes.data, logits.ctypes.data,
                                        C.byref(tp)), "vit_predict_debug")

@@ -35,14 +35,25 @@ CONFIGS = {
     # small shapes for fast unit tests (not reference configs)
     "micro": (128, 2, 2, 16, 64),
     "micro14": (128, 2, 2, 14, 56),
+    # 2-layer models at the geometries the engine selects kernels by (tests/test_gpu_geometry.py): patch sizes 8 (785 tokens, as
+    # DINO ViT-S/8) and 32, 14 with K padding; hidden sizes from one head (64) to the largest accepted (2048)
+    "p8": (384, 2, 6, 8, 224),
+    "p32": (512, 2, 8, 32, 384),
+    "d640": (640, 2, 10, 16, 256),
+    "d896p14": (896, 2, 14, 14, 224),
+    "d320": (320, 2, 5, 16, 160),
+    "d1536": (1536, 2, 24, 16, 64),
+    "d2048": (2048, 1, 32, 16, 32),
+    "d64": (64, 2, 1, 16, 32),
+    "vitstr_p8": (128, 2, 2, 8, 64),
     # ViT-L/16-384 geometry (hidden 1024, 16 heads, 577 tokens) cut to 2 layers so CPU-side checks stay fast
     "large384x2": (1024, 2, 16, 16, 384),
     # ViTSTR extension (reference extensions/vitstr.cpp): 1-channel 224x224 input, 96 classes, classifier over 25 tokens
     "vitstr_micro": (128, 2, 2, 16, 96),
     "vitstr_tiny": (192, 12, 3, 16, 224),
 }
-IN_CHANS = {"vitstr_micro": 1, "vitstr_tiny": 1}      # default 3
-NUM_CLASSES = {"vitstr_micro": 96, "vitstr_tiny": 96}  # default 1000
+IN_CHANS = {"vitstr_micro": 1, "vitstr_tiny": 1, "vitstr_p8": 1}      # default 3
+NUM_CLASSES = {"vitstr_micro": 96, "vitstr_tiny": 96, "vitstr_p8": 96}  # default 1000
 
 
 @dataclass
@@ -134,12 +145,13 @@ def _write_header(f, hp: Tuple[int, ...], ftype: int, classes: int):
         f.write(s)
 
 
-def write_synthetic(path: str, config: str = "tiny", ftype: int = 1, classes: int = 0, seed: int = 0,
-                    round_bf16: bool = False) -> None:
+def write_synthetic(path: str, config="tiny", ftype: int = 1, classes: int = 0, seed: int = 0,
+                    round_bf16: bool = False, in_chans: int = 0) -> None:
     """Write a synthetic model.  ftype 1: 2-D(+4-D) weights f16, rest f32 (convert-pth-to-ggml.py:143-147).
-    ftype 0: everything f32 EXCEPT the patch kernel, which the loader hard-codes as F16 (vit.cpp:515)."""
-    hidden, layers, heads, patch, img = CONFIGS[config]
-    in_chans = IN_CHANS.get(config, 3)
+    ftype 0: everything f32 EXCEPT the patch kernel, which the loader hard-codes as F16 (vit.cpp:515).
+    config: a name in CONFIGS, or a (hidden, layers, heads, patch, img) tuple."""
+    hidden, layers, heads, patch, img = CONFIGS[config] if isinstance(config, str) else config
+    in_chans = in_chans or IN_CHANS.get(config, 3)
     classes = classes or NUM_CLASSES.get(config, 1000)
     assert ftype in (0, 1)
     tens = synth_tensors(hidden, layers, classes, patch, img, seed, round_bf16, in_chans)
