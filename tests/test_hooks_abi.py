@@ -1,0 +1,33 @@
+"""CPU tests of the kernel test hooks' device check: without a GPU every hook that launches a kernel fails with the engine's
+"no CPU fallback" message instead of running on the host or reporting a raw CUDA error."""
+import numpy as np
+import pytest
+
+from tests.util import pkg
+
+eng = pkg.engine
+
+M = N = K = 128
+D, ROWS = 128, 8
+B, NT, H = 1, 16, 1
+
+HOOKS = {
+    "gemm": lambda: eng.test_gemm(M, N, K, 0, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16), np.zeros(N, np.float32)),
+    "gemm_fp8": lambda: eng.test_gemm_fp8(M, N, K, 0, np.zeros((M, K), np.uint8), np.ones(M, np.float32), np.zeros((N, K), np.uint8),
+                                          1.0, np.zeros(N, np.float32)),
+    "gemm_q8": lambda: eng.test_gemm_q8(np.zeros((M, K), np.float32), np.zeros(N * (K // 32) * 34, np.uint8), np.zeros(N, np.float32)),
+    "layernorm": lambda: eng.test_layernorm(np.zeros((ROWS, D), np.float32), np.ones(D, np.float32), np.zeros(D, np.float32)),
+    "layernorm_fp8": lambda: eng.test_layernorm_fp8(np.zeros((ROWS, D), np.float32), np.ones(D, np.float32), np.zeros(D, np.float32)),
+    "attention": lambda: eng.test_attention(np.zeros((B * NT, 3 * H * 64), np.float16), B, NT, H),
+    "attention_hilo": lambda: eng.test_attention_hilo(np.zeros((B * NT, 3 * H * 64), np.float32), B, NT, H),
+}
+
+
+@pytest.mark.parametrize("hook", sorted(HOOKS))
+def test_device_hooks_have_no_cpu_fallback(hook):
+    import torch
+    if torch.cuda.is_available():
+        pytest.skip("GPU present")
+    with pytest.raises(eng.VitB200Error) as ei:
+        HOOKS[hook]()
+    assert "no CPU fallback" in str(ei.value)

@@ -18,6 +18,8 @@
 #include <cstring>
 #include <fstream>
 #include <map>
+#include <memory>
+#include <mutex>
 #include <string>
 #include <vector>
 
@@ -37,6 +39,20 @@ int fail(const char *fmt, ...)
     g_err = buf;
     fprintf(stderr, "vitb200: %s\n", buf); // reference convention: message on stderr + non-zero return
     return 1;
+}
+
+// The C ABI promises "non-zero return, never abort": nothing may unwind through an extern "C" frame.  Host-side allocations
+// (std::vector staging buffers sized from a model file, the graph cache, debug taps) can throw; every exported function that can
+// reach one runs its body through this.
+template <class F>
+int guarded(const char *fn, F &&body) noexcept
+{
+    try
+    {
+        return body();
+    }
+    catch (const std::exception &ex) { return fail("%s: %s", fn, ex.what()); }
+    catch (...) { return fail("%s: unknown exception", fn); }
 }
 
 #define CUDA_TRY(x)                                                                       \
@@ -153,6 +169,22 @@ struct GraphKey
     }
 };
 
+// One of the two host-pipeline slots (vitb200_forward_async, the u8 and recognition entry points): call n uses slot n & 1, so its
+// H2D copy on the copy stream can overlap call n - 1's kernels on the compute stream
+struct Slot
+{
+    float *img = nullptr, *probs = nullptr, *logits = nullptr, *topk_val = nullptr;
+    int32_t *topk_idx = nullptr;
+    // text recognition (1-channel models with head_tokens >= 2): decoded class ids [max_batch][head_tokens - 1], lengths, scores
+    int32_t *chars = nullptr, *len = nullptr;
+    double *score = nullptr;
+    // GPU preprocessing: a PINNED host staging buffer (the caller's images are packed into it, followed by the per-image
+    // descriptors) and its device twin; grown only when a batch needs more than any batch before it
+    uint8_t *h_u8 = nullptr, *d_u8 = nullptr;
+    size_t u8_cap = 0;
+    cudaEvent_t ev_h2d = nullptr, ev_done = nullptr;
+};
+
 } // namespace
 
 struct vitb200_engine
@@ -177,8 +209,7 @@ struct vitb200_engine
     Linear patch, head;
     std::vector<Layer> layers;
     // activations (static arena, sized for max_batch)
-    float *d_img = nullptr, *X = nullptr, *d_logits = nullptr, *d_probs = nullptr, *d_topk_val = nullptr;
-    int32_t *d_topk_idx = nullptr;
+    float *X = nullptr, *d_logits = nullptr;
     __half *A16 = nullptr, *QKV16 = nullptr, *H16 = nullptr, *CLS16 = nullptr, *PA = nullptr;
     // lo halves of q, k, v (x - f16(x), as f16): the split-precision operands of the wgmma attention.  Allocated exactly when that
     // kernel runs (N <= 224); then the qkv GEMM emits hi + lo and the attention runs the 3 + 2 term products.
@@ -191,19 +222,8 @@ struct vitb200_engine
     // host-buffer pipeline (vitb200_forward_async): 2 input/output slots, H2D on a copy stream overlapping the previous
     // call's kernels on the compute stream
     cudaStream_t copy_stream = nullptr;
-    float *d_img_slot[2] = {nullptr, nullptr}, *d_probs_slot[2] = {nullptr, nullptr}, *d_logits_slot[2] = {nullptr, nullptr};
-    float *d_topk_val_slot[2] = {nullptr, nullptr};
-    int32_t *d_topk_idx_slot[2] = {nullptr, nullptr};
-    cudaEvent_t ev_h2d[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+    Slot slot[2];
     unsigned long long submits = 0;
-    // GPU preprocessing (vitb200_forward_u8*): per pipeline slot a PINNED host staging buffer (the caller's images are packed into it,
-    // followed by the per-image descriptors) and its device twin; grown only when a batch needs more than any batch before it
-    uint8_t *h_u8[2] = {nullptr, nullptr}, *d_u8[2] = {nullptr, nullptr};
-    size_t u8_cap[2] = {0, 0};
-    // text recognition (vitb200_recognize_u8*, 1-channel models with head_tokens >= 2): per pipeline slot the decoded class ids
-    // [max_batch][head_tokens - 1], lengths [max_batch] and scores [max_batch]
-    int32_t *d_chars_slot[2] = {nullptr, nullptr}, *d_len_slot[2] = {nullptr, nullptr};
-    double *d_score_slot[2] = {nullptr, nullptr};
     // CUDA-graph cache for the kernel schedule of one forward, keyed by its arguments (launch-bound inner loop: ~90 kernels)
     struct GraphEntry { GraphKey key; int state; int launches; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -479,6 +499,33 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
+// Opts `kern` in to `bytes` of dynamic shared memory on the current device, and raises that limit when a later launch needs more.
+// The attribute belongs to the process and device, not to an engine, so one table serves every engine on every host thread.  It is
+// set on a kernel's first eager run, never inside a graph capture (run_graphed captures an argument set's second call only).
+// cluster_cfg: also counts, once, the clusters of that launch configuration that fit on the device at a time, into *clusters.
+struct KernelAttr
+{
+    int smem = 0, clusters = 0;
+};
+std::mutex g_attr_mutex;
+std::map<std::pair<const void *, int>, KernelAttr> g_attr;
+
+int smem_optin(const void *kern, int bytes, const cudaLaunchConfig_t *cluster_cfg = nullptr, int *clusters = nullptr)
+{
+    int dev = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(g_attr_mutex);
+    KernelAttr &a = g_attr[{kern, dev}];
+    if (bytes > a.smem)
+    {
+        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        if (cluster_cfg) CUDA_TRY(cudaOccupancyMaxActiveClusters(&a.clusters, kern, cluster_cfg));
+        a.smem = bytes;
+    }
+    if (clusters) *clusters = a.clusters;
+    return 0;
+}
+
 template <int EPI, int STAGES, int OP = GEMM_OP_F16>
 int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
@@ -494,17 +541,13 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     attr[1].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 2;
-    // the opt-in to > 48 KB dynamic shared memory is per device (one engine per device, possibly several per process)
-    static bool attr_set[64] = {};
-    static int max_clusters[64] = {};
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63])
+    int max_clusters = 0;
+    if (smem_optin((const void *)kern, Cfg::SMEM_BYTES, &cfg, &max_clusters)) return 1;
+    if (max_clusters < 1)
     {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        CUDA_TRY(cudaOccupancyMaxActiveClusters(&max_clusters[dev & 63], kern, &cfg));
-        if (max_clusters[dev & 63] < 1) return fail("GEMM: no cluster of two CTAs fits on device %d", dev);
-        attr_set[dev & 63] = true;
+        int dev = 0;
+        CUDA_TRY(cudaGetDevice(&dev));
+        return fail("GEMM: no cluster of two CTAs fits on device %d", dev);
     }
     // the staged epilogues' TMA maps over exactly M rows and N columns of the output (and of the residual), encoded per launch:
     // a captured graph keeps them by value
@@ -527,9 +570,9 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     }
     // persistent: as many clusters as fit at once, each walking the pairs of column tiles cluster, cluster + clusters, ...
     const int pairs = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN));
-    cfg.gridDim = dim3(2u * (unsigned)std::min(pairs, max_clusters[dev & 63]));
+    cfg.gridDim = dim3(2u * (unsigned)std::min(pairs, max_clusters));
     CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmO, tmX, p));
-    if (e) e->launches++;
+    e->launches++;
     return 0;
 }
 
@@ -631,12 +674,7 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
         const int nblk = (rows + LN_TMA_ROWS - 1) / LN_TMA_ROWS;
         const int grid = std::min(nblk, 2 * e->num_sms);
         auto launch = [&](auto kern) -> int {
-            // per kernel instantiation (all of them share this lambda's type: index by D / 128) and per device (one engine per device,
-            // possibly several per process)
-            static bool attr_set[9][64] = {};
-            int dev = 0;
-            CUDA_TRY(cudaGetDevice(&dev));
-            if (!attr_set[D / 128][dev & 63]) { CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); attr_set[D / 128][dev & 63] = true; }
+            if (smem_optin((const void *)kern, smem)) return 1;
             CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps, y_scale));
             return 0;
         };
@@ -680,14 +718,7 @@ int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int smem = attention_wgmma_smem_bytes();
     auto kern = attention_wgmma_kernel;
-    static bool attr_set[64] = {};
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (!attr_set[dev & 63])
-    {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        attr_set[dev & 63] = true;
-    }
+    if (smem_optin((const void *)kern, smem)) return 1;
     const int H = e->hp.num_attention_heads;
     CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)smem, s, e->tmQ, e->tmKV, e->tmQl, e->tmKVl,
                         e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H))));
@@ -709,14 +740,7 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
     const int smem = attention_smem_bytes(N);
     if (smem > kSmemOptinMax) return fail("attention: %d tokens do not fit in shared memory (max %d)", N, ATT_MAX_TOKENS);
     auto kern = attention_kernel<NW>;
-    static int smem_set[64] = {};
-    int dev = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    if (smem > smem_set[dev & 63])
-    {
-        CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-        smem_set[dev & 63] = smem;
-    }
+    if (smem_optin((const void *)kern, smem)) return 1;
     CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(NW * 32), (size_t)smem, s, e->QKV16, (size_t)e->max_batch * N,
                         e->A16, N, D, H, Npad, 1.0f / sqrtf((float)(D / H))));
     e->launches++;
@@ -876,12 +900,23 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
     return 0;
 }
 
+int check_batch(const vitb200_engine *e, int batch)
+{
+    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
+    return 0;
+}
+
+int check_k(const vitb200_engine *e, int k)
+{
+    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
+    return 0;
+}
+
 // The fixed kernel schedule == reference vit_encode_image (vit.cpp:718-941), batched over images.
 int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
                 float *d_topk_val, int k, cudaStream_t s, const vitb200_taps *taps)
 {
-    if (B < 1 || B > e->max_batch) return fail("batch %d out of range (1..%d)", B, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
+    if (check_batch(e, B) || check_k(e, k)) return 1;
     if (!d_images && taps) return fail("debug taps need the f32 image path");
     const int D = e->hp.hidden_size, N = e->N, T = B * N, C = e->hp.num_classes;
     if (run_encoder(e, d_images, B, e->hp.num_hidden_layers, s, taps)) return 1;
@@ -1019,59 +1054,37 @@ int check_features(const vitb200_engine *e, const void *images, int batch, const
     if (req->norm != 0 && req->norm != 1) return fail("vitb200_features: norm must be 0 or 1 (got %d)", req->norm);
     if (req->dtype < 0 || req->dtype > 2) return fail("vitb200_features: dtype %d unknown (0 f32, 1 f16, 2 bf16)", req->dtype);
     if (!tokens && !prelogits) return fail("vitb200_features: both outputs are NULL");
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
-    return 0;
+    return check_batch(e, batch);
 }
 
 size_t features_elem_bytes(const vitb200_features_req *req) { return req->dtype == 0 ? 4 : 2; }
 
-} // namespace
-
-extern "C" {
-
-const char *vitb200_last_error(void) { return g_err.c_str(); }
-
-int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, vitb200_engine **out)
+// Selects `device` for the calling thread and requires an sm_90 part: the device check of vitb200_create and of every test hook
+int open_device(int device, cudaDeviceProp &prop)
 {
-    return vitb200_create_ex(hp, t, n, device, max_batch, 1, out);
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
+        return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
+    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
+    CUDA_TRY(cudaSetDevice(device));
+    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
+    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
+    return 0;
 }
 
-// The C ABI promises "non-zero return, never abort": nothing may unwind through an extern "C" frame.  Host-side allocations
-// (std::vector staging buffers sized from a model file) can throw; every entry point that owns such code runs it through this.
-#define VB_NOEXCEPT_BEGIN try {
-#define VB_NOEXCEPT_END(cleanup)                                                                          \
-    } catch (const std::exception &ex) { cleanup; return fail("%s: %s", __func__, ex.what()); }            \
-    catch (...) { cleanup; return fail("%s: unknown exception", __func__); }
+// An engine that vitb200_destroy frees unless it is released: a half-built one, or a test hook's scratch engine
+struct EngineDeleter
+{
+    void operator()(vitb200_engine *e) const { vitb200_destroy(e); }
+};
+using EnginePtr = std::unique_ptr<vitb200_engine, EngineDeleter>;
 
-static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
-                       vitb200_engine *&e, vitb200_engine **out);
-
-static int create_checked(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
-                          vitb200_engine **out)
+// Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
+int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
+                vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
 {
     if (!hp || !t || !out) return fail("vitb200_create: null argument");
     *out = nullptr;
-    vitb200_engine *e = nullptr;
-    VB_NOEXCEPT_BEGIN
-    return create_impl(hp, t, n, device, max_batch, head_tokens, fp8, e, out);
-    VB_NOEXCEPT_END(if (e) vitb200_destroy(e))
-}
-
-int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
-                      vitb200_engine **out)
-{
-    return create_checked(hp, t, n, device, max_batch, head_tokens, false, out);
-}
-
-int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
-                       vitb200_engine **out)
-{
-    return create_checked(hp, t, n, device, max_batch, head_tokens, true, out);
-}
-
-static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
-                       vitb200_engine *&e, vitb200_engine **out)
-{
     // hyper-parameter sanity first (no division by a field a corrupt file may have zeroed; no device needed to reject them)
     if (hp->hidden_size < 64 || hp->hidden_size > 8192 || hp->num_hidden_layers < 1 || hp->num_hidden_layers > 4096 ||
         hp->num_attention_heads < 1 || hp->num_attention_heads > 128 || hp->num_classes < 1 || hp->num_classes > (1 << 20) ||
@@ -1094,18 +1107,14 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + 1;
     if (n_tokens > ATT_MAX_TOKENS)
         return fail("%d tokens not supported (max %d: K and V of one attention head must fit in shared memory)", n_tokens, ATT_MAX_TOKENS);
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
+    if (open_device(device, prop)) return 1;
     if (max_batch < 1) return fail("max_batch must be >= 1");
     if (check_unique_names(t, n)) return 1;
+    if (head_tokens < 1 || head_tokens > n_tokens) return fail("head_tokens %d out of range (1..%d)", head_tokens, n_tokens);
 
-    e = new vitb200_engine();
+    EnginePtr owner(new vitb200_engine());
+    vitb200_engine *e = owner.get();
     e->hp = *hp;
     if (e->hp.eps <= 0.f) e->hp.eps = 1e-6f;
     e->device = device;
@@ -1117,18 +1126,16 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     e->NP = e->G * e->G;
     e->N = e->NP + 1;
     e->C = in_chans;
-    if (head_tokens < 1 || head_tokens > e->N) { const int ntok = e->N; delete e; e = nullptr; return fail("head_tokens %d out of range (1..%d)", head_tokens, ntok); }
     e->head_tokens = head_tokens;
     e->Cp = (hp->num_classes + 3) / 4 * 4;
     e->KP = e->C * P * P;
     e->KPp = (e->KP + 63) / 64 * 64;
-    auto bail = [&](int) { vitb200_destroy(e); e = nullptr; return 1; };
-    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
+    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
 
     // ---- weights (names: reference vit.cpp:518-579)
-    if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls)) return bail(1);
-    if (upload_f32(e, t, n, "pos_embed", D, e->N, 1, 1, &e->pos)) return bail(1);
-    if (upload_linear(e, t, n, "patch_embed.proj.weight", "patch_embed.proj.bias", D, e->KP, e->KPp, &e->patch, P)) return bail(1);
+    if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls)) return 1;
+    if (upload_f32(e, t, n, "pos_embed", D, e->N, 1, 1, &e->pos)) return 1;
+    if (upload_linear(e, t, n, "patch_embed.proj.weight", "patch_embed.proj.bias", D, e->KP, e->KPp, &e->patch, P)) return 1;
     e->layers.resize(hp->num_hidden_layers);
     for (int i = 0; i < hp->num_hidden_layers; ++i)
     {
@@ -1136,15 +1143,15 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
         const std::string p = "blocks." + std::to_string(i) + ".";
         if (upload_f32(e, t, n, p + "norm1.weight", D, 1, 1, 1, &L.n1w) || upload_f32(e, t, n, p + "norm1.bias", D, 1, 1, 1, &L.n1b) ||
             upload_f32(e, t, n, p + "norm2.weight", D, 1, 1, 1, &L.n2w) || upload_f32(e, t, n, p + "norm2.bias", D, 1, 1, 1, &L.n2b))
-            return bail(1);
+            return 1;
         if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv, 0, fp8) ||
             upload_linear(e, t, n, p + "attn.proj.weight", p + "attn.proj.bias", D, D, D, &L.proj) ||
             upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, D, &L.fc1, 0, fp8) ||
             upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 4 * D, &L.fc2))
-            return bail(1);
+            return 1;
     }
-    if (upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b)) return bail(1);
-    if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, D, D, &e->head)) return bail(1);
+    if (upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b)) return 1;
+    if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, D, D, &e->head)) return 1;
 
     // ---- activation arena
     const size_t B = (size_t)max_batch, T = B * e->N;
@@ -1155,53 +1162,164 @@ static int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n
     const bool pa_alias = (e->KPp == e->KP) && pa_elems <= h16;
     const size_t R = B * (size_t)e->head_tokens;                        // classifier rows: pooled tokens of all images
     const size_t img_elems = (size_t)e->C * hp->img_size * hp->img_size; // per image
-    if (dev_alloc(e, &e->d_img, B * img_elems) || dev_alloc(e, &e->X, T * D) ||
-        dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->H16, h16) ||
-        dev_alloc(e, &e->CLS16, R * D) || dev_alloc(e, &e->d_logits, R * e->Cp) || dev_alloc(e, &e->d_logits_slot[0], R * hp->num_classes) ||
-        dev_alloc(e, &e->d_probs, R * hp->num_classes) || dev_alloc(e, &e->d_topk_idx, R * e->max_k) ||
-        dev_alloc(e, &e->d_topk_val, R * e->max_k))
-        return bail(1);
-    e->d_img_slot[0] = e->d_img; e->d_probs_slot[0] = e->d_probs;
+    if (dev_alloc(e, &e->X, T * D) || dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->H16, h16) ||
+        dev_alloc(e, &e->CLS16, R * D) || dev_alloc(e, &e->d_logits, R * e->Cp))
+        return 1;
     {
         // soft-max working row: dynamic shared memory up to the per-CTA limit (opt-in above 48 KB), global scratch beyond it
         const size_t row_bytes = (size_t)hp->num_classes * sizeof(float);
-        if (row_bytes > kSoftmaxSmemMax) { if (dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return bail(1); }
+        if (row_bytes > kSoftmaxSmemMax) { if (dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return 1; }
         else if (row_bytes > 48 * 1024 &&
                  cudaFuncSetAttribute(softmax_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSoftmaxSmemMax) != cudaSuccess)
-            return bail(fail("cudaFuncSetAttribute(softmax_topk_kernel) failed"));
+            return fail("cudaFuncSetAttribute(softmax_topk_kernel) failed");
     }
-    e->d_topk_idx_slot[0] = e->d_topk_idx; e->d_topk_val_slot[0] = e->d_topk_val;
-    if (dev_alloc(e, &e->d_img_slot[1], B * img_elems) || dev_alloc(e, &e->d_probs_slot[1], R * hp->num_classes) ||
-        dev_alloc(e, &e->d_logits_slot[1], R * hp->num_classes) || dev_alloc(e, &e->d_topk_idx_slot[1], R * e->max_k) ||
-        dev_alloc(e, &e->d_topk_val_slot[1], R * e->max_k))
-        return bail(1);
-    if (e->C == 1 && e->head_tokens >= 2)
-        for (int i = 0; i < 2; ++i)
-            if (dev_alloc(e, &e->d_chars_slot[i], B * (e->head_tokens - 1)) || dev_alloc(e, &e->d_len_slot[i], B) ||
-                dev_alloc(e, &e->d_score_slot[i], B))
-                return bail(1);
-    if (cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("cudaStreamCreate failed"));
-    for (int i = 0; i < 2; ++i)
-        if (cudaEventCreateWithFlags(&e->ev_h2d[i], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&e->ev_done[i], cudaEventDisableTiming) != cudaSuccess)
-            return bail(fail("cudaEventCreate failed"));
+    for (Slot &sl : e->slot)
+    {
+        if (dev_alloc(e, &sl.img, B * img_elems) || dev_alloc(e, &sl.probs, R * hp->num_classes) || dev_alloc(e, &sl.logits, R * hp->num_classes) ||
+            dev_alloc(e, &sl.topk_idx, R * e->max_k) || dev_alloc(e, &sl.topk_val, R * e->max_k))
+            return 1;
+        if (e->C == 1 && e->head_tokens >= 2 &&
+            (dev_alloc(e, &sl.chars, B * (e->head_tokens - 1)) || dev_alloc(e, &sl.len, B) || dev_alloc(e, &sl.score, B)))
+            return 1;
+        if (cudaEventCreateWithFlags(&sl.ev_h2d, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess)
+            return fail("cudaEventCreate failed");
+    }
+    if (cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
     if (pa_alias) e->PA = e->H16;
     else
     {
-        if (dev_alloc(e, &e->PA, pa_elems)) return bail(1);
-        if (cudaMemset(e->PA, 0, pa_elems * sizeof(__half)) != cudaSuccess) return bail(fail("cudaMemset failed"));
+        if (dev_alloc(e, &e->PA, pa_elems)) return 1;
+        if (cudaMemset(e->PA, 0, pa_elems * sizeof(__half)) != cudaSuccess) return fail("cudaMemset failed");
     }
     if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_A_BOX_ROWS) ||
         make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_A_BOX_ROWS))
-        return bail(1);
-    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || make_tmap_e4m3(&e->tmA8, e->A8, T, D, GEMM_A_BOX_ROWS))) return bail(1);
+        return 1;
+    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || make_tmap_e4m3(&e->tmA8, e->A8, T, D, GEMM_A_BOX_ROWS))) return 1;
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
     // memory (N <= 224), i.e. wherever the wgmma attention runs
-    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return bail(1);
-    if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
-    *out = e;
-    e = nullptr; // ownership passed to the caller
+    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return 1;
+    if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
+    if (labels) e->labels = *labels;
+    *out = owner.release();
     return 0;
+}
+
+// The test hooks' harness: each hook opens the device into a scratch engine with a non-blocking stream of its own, allocates with
+// dev_alloc (vitb200_destroy frees it with the engine) and checks every copy.
+int scratch_engine(int device, EnginePtr &e)
+{
+    cudaDeviceProp prop;
+    if (open_device(device, prop)) return 1;
+    e.reset(new vitb200_engine());
+    e->device = device;
+    e->num_sms = prop.multiProcessorCount;
+    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail("stream creation failed");
+    return 0;
+}
+
+// host -> a new device buffer of `count` elements
+template <typename T>
+int upload(vitb200_engine *e, T **d, const void *src, size_t count)
+{
+    if (dev_alloc(e, d, count)) return 1;
+    CUDA_TRY(cudaMemcpy(*d, src, count * sizeof(T), cudaMemcpyHostToDevice));
+    return 0;
+}
+
+// Runs a test hook's kernels on the scratch engine's stream and waits for them; `what` names them in the error.  cudaMemcpy from
+// pageable memory may return before the DMA has landed, and the kernels run on a NON-BLOCKING stream (no implicit ordering with the
+// legacy stream the uploads used): the device is synchronised before the launch.
+template <class Launch>
+int run_scratch(vitb200_engine *e, const char *what, Launch launch)
+{
+    if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
+    if (launch()) return 1;
+    const cudaError_t err = cudaStreamSynchronize(e->stream);
+    if (err != cudaSuccess)
+    {
+        (void)cudaGetLastError();
+        return fail("%s failed: %s", what, cudaGetErrorString(err));
+    }
+    return 0;
+}
+
+// Stand-alone run of the block LayerNorm as the engine launches it (persistent bulk-copy kernel for hidden sizes that are a multiple of 128
+// and >= 8 rows, the row-per-warp kernel otherwise): x [rows][D] f32 -> y [rows][D] (f16 results widened to f32).
+// OutT = __nv_fp8_e4m3: the FP8 engine's LayerNorm 1 / 2, y e4m3 and y_scale the row scales.  Both outputs are poisoned with 0xFF
+// first, so an element the kernel never writes reads back as NaN.
+template <typename OutT>
+int test_layernorm_impl(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, OutT **y,
+                        float **y_scale, EnginePtr &owner)
+{
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
+    e->hp.hidden_size = D; e->hp.eps = eps;
+    float *dx = nullptr, *dw = nullptr, *db = nullptr;
+    if (upload(e, &dx, x, (size_t)rows * D) || upload(e, &dw, w, D) || upload(e, &db, b, D) || dev_alloc(e, y, (size_t)rows * D)) return 1;
+    CUDA_TRY(cudaMemset(*y, 0xFF, (size_t)rows * D * sizeof(OutT)));
+    if (y_scale)
+    {
+        if (dev_alloc(e, y_scale, rows)) return 1;
+        CUDA_TRY(cudaMemset(*y_scale, 0xFF, (size_t)rows * sizeof(float)));
+    }
+    return run_scratch(e, "LayerNorm kernel",
+                       [&] { return launch_layernorm(e, dx, (size_t)D, dw, db, *y, rows, e->stream, 0, 0, y_scale ? *y_scale : nullptr); });
+}
+
+// One call of the host pipeline: begin_submit picks its slot; end_submit marks the slot's last use (everything enqueued on the compute
+// stream so far) and counts the call
+Slot &begin_submit(vitb200_engine *e) { return e->slot[e->submits & 1]; }
+
+int end_submit(vitb200_engine *e, Slot &sl)
+{
+    CUDA_TRY(cudaEventRecord(sl.ev_done, e->stream));
+    e->submits++;
+    return 0;
+}
+
+// The classifier forward of one pipelined call into slot sl, then the copies of the requested outputs to the caller's host buffers.
+// d_images: sl.img, or NULL when the u8 preprocess has written the patch matrix.
+int classify_to_host(vitb200_engine *e, const Slot &sl, const float *d_images, int batch, float *probs, float *logits, int32_t *topk_idx,
+                     float *topk_prob, int k, const vitb200_taps *taps)
+{
+    cudaStream_t s = e->stream;
+    const bool want_topk = k > 0 && (topk_idx || topk_prob);
+    float *dp = (probs || want_topk) ? sl.probs : nullptr;
+    int32_t *di = want_topk ? sl.topk_idx : nullptr;
+    float *dv = want_topk ? sl.topk_val : nullptr;
+    const int kk = want_topk ? k : 0;
+    if (taps ? run_forward(e, d_images, batch, dp, sl.logits, di, dv, kk, s, taps) : run_forward_graphed(e, d_images, batch, dp, sl.logits, di, dv, kk, s))
+        return 1;
+    const size_t rows = (size_t)batch * e->head_tokens, C = e->hp.num_classes; // classifier rows returned
+    if (probs) CUDA_TRY(cudaMemcpyAsync(probs, sl.probs, rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (logits) CUDA_TRY(cudaMemcpyAsync(logits, sl.logits, rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
+    if (want_topk && topk_idx) CUDA_TRY(cudaMemcpyAsync(topk_idx, sl.topk_idx, rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+    if (want_topk && topk_prob) CUDA_TRY(cudaMemcpyAsync(topk_prob, sl.topk_val, rows * k * sizeof(float), cudaMemcpyDeviceToHost, s));
+    return 0;
+}
+
+} // namespace
+
+extern "C" {
+
+const char *vitb200_last_error(void) { return g_err.c_str(); }
+
+int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, 1, false, out); });
+}
+
+int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+                      vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, head_tokens, false, out); });
+}
+
+int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+                       vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, head_tokens, true, out); });
 }
 
 void vitb200_destroy(vitb200_engine *e)
@@ -1210,20 +1328,27 @@ void vitb200_destroy(vitb200_engine *e)
     cudaSetDevice(e->device);
     for (void *p : e->allocs) cudaFree(p);
     for (auto &g : e->graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
-    for (int i = 0; i < 2; ++i) { if (e->d_u8[i]) cudaFree(e->d_u8[i]); if (e->h_u8[i]) cudaFreeHost(e->h_u8[i]); }
+    for (Slot &sl : e->slot)
+    {
+        if (sl.d_u8) cudaFree(sl.d_u8);
+        if (sl.h_u8) cudaFreeHost(sl.h_u8);
+        if (sl.ev_h2d) cudaEventDestroy(sl.ev_h2d);
+        if (sl.ev_done) cudaEventDestroy(sl.ev_done);
+    }
     for (auto &r : e->prof) { cudaEventDestroy(r.a); cudaEventDestroy(r.b); }
     for (auto ev : e->event_pool) cudaEventDestroy(ev);
     if (e->stream) cudaStreamDestroy(e->stream);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-    for (int i = 0; i < 2; ++i) { if (e->ev_h2d[i]) cudaEventDestroy(e->ev_h2d[i]); if (e->ev_done[i]) cudaEventDestroy(e->ev_done[i]); }
     delete e;
 }
 
 int vitb200_get_hparams(const vitb200_engine *e, vitb200_hparams *out)
 {
-    if (!e || !out) return fail("null argument");
-    *out = e->hp;
-    return 0;
+    return guarded(__func__, [&] {
+        if (!e || !out) return fail("null argument");
+        *out = e->hp;
+        return 0;
+    });
 }
 
 const char *vitb200_label(const vitb200_engine *e, int class_id)
@@ -1240,70 +1365,47 @@ int vitb200_fp8(const vitb200_engine *e) { return e && e->fp8 ? 1 : 0; }
 
 int vitb200_profile_enable(vitb200_engine *e, int on)
 {
-    if (!e) return fail("null argument");
-    CUDA_TRY(cudaSetDevice(e->device));
-    CUDA_TRY(cudaDeviceSynchronize());
-    for (auto &r : e->prof) { e->event_pool.push_back(r.a); e->event_pool.push_back(r.b); }
-    e->prof.clear();
-    e->profile = on != 0;
-    return 0;
+    return guarded(__func__, [&]() -> int {
+        if (!e) return fail("null argument");
+        CUDA_TRY(cudaSetDevice(e->device));
+        CUDA_TRY(cudaDeviceSynchronize());
+        for (auto &r : e->prof) { e->event_pool.push_back(r.a); e->event_pool.push_back(r.b); }
+        e->prof.clear();
+        e->profile = on != 0;
+        return 0;
+    });
 }
 
 int vitb200_profile_read(vitb200_engine *e, int kind, double *ms_total, int *launches, double *flops_per_launch)
 {
-    if (!e || !ms_total || !launches || !flops_per_launch) return fail("null argument");
-    if (kind < 0 || kind >= PK_COUNT) return fail("profile kind %d out of range", kind);
-    CUDA_TRY(cudaSetDevice(e->device));
-    CUDA_TRY(cudaDeviceSynchronize());
-    double ms = 0.0, fl = 0.0;
-    int n = 0;
-    for (auto &r : e->prof)
-    {
-        if (r.kind != kind) continue;
-        float t = 0.f;
-        CUDA_TRY(cudaEventElapsedTime(&t, r.a, r.b));
-        ms += t; fl = r.flops; ++n;
-    }
-    *ms_total = ms; *launches = n; *flops_per_launch = fl;
-    return 0;
-}
-static int test_attention_impl(int device, int kernel, int B, int N, int H, const uint16_t *qkv, const uint16_t *qkv_lo, float *out);
-
-int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out)
-{
-    VB_NOEXCEPT_BEGIN
-    return test_attention_impl(device, kernel, B, N, H, qkv, nullptr, out);
-    VB_NOEXCEPT_END((void)0)
-}
-
-int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
-{
-    if (!qkv_lo) return fail("bad argument");
-    VB_NOEXCEPT_BEGIN
-    return test_attention_impl(device, 2, B, N, H, qkv_hi, qkv_lo, out);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&]() -> int {
+        if (!e || !ms_total || !launches || !flops_per_launch) return fail("null argument");
+        if (kind < 0 || kind >= PK_COUNT) return fail("profile kind %d out of range", kind);
+        CUDA_TRY(cudaSetDevice(e->device));
+        CUDA_TRY(cudaDeviceSynchronize());
+        double ms = 0.0, fl = 0.0;
+        int n = 0;
+        for (auto &r : e->prof)
+        {
+            if (r.kind != kind) continue;
+            float t = 0.f;
+            CUDA_TRY(cudaEventElapsedTime(&t, r.a, r.b));
+            ms += t; fl = r.flops; ++n;
+        }
+        *ms_total = ms; *launches = n; *flops_per_launch = fl;
+        return 0;
+    });
 }
 
 static int test_attention_impl(int device, int kernel, int B, int N, int H, const uint16_t *qkv, const uint16_t *qkv_lo, float *out)
 {
     if (!qkv || !out || B < 1 || N < 1 || H < 1) return fail("bad argument");
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-        return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-    vitb200_engine *e = new vitb200_engine();
-    e->device = device;
-    auto bail = [&](int rc) { vitb200_destroy(e); return rc; };
-    e->num_sms = prop.multiProcessorCount;
+    EnginePtr owner;
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
     e->N = N; e->hp.hidden_size = H * 64; e->hp.num_attention_heads = H; e->max_batch = B;
     const int D = H * 64;
     const uint64_t T = (uint64_t)B * N;
-    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(fail("stream creation failed"));
-    if (dev_alloc(e, &e->QKV16, (size_t)T * 3 * D) || dev_alloc(e, &e->A16, (size_t)T * D)) return bail(1);
     // the kernels read the HEAD-MAJOR layout the qkv GEMM writes ([3 H][T][64]); the caller hands over the reference's [T][3 D]
     std::vector<uint16_t> hm((size_t)T * 3 * D);
     auto to_head_major = [&](const uint16_t *src) {
@@ -1312,45 +1414,49 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
                 memcpy(&hm[((size_t)pl * T + t) * 64], src + (size_t)t * 3 * D + (size_t)pl * 64, 128);
     };
     to_head_major(qkv);
-    if (cudaMemcpy(e->QKV16, hm.data(), (size_t)T * 3 * D * 2, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail("H2D failed"));
-    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return bail(fail("attention kernel %d unknown", kernel));
-    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return bail(fail("wgmma attention needs N <= %d", ATTW_KEYS));
-    if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return bail(fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16));
+    if (upload(e, &e->QKV16, hm.data(), hm.size()) || dev_alloc(e, &e->A16, (size_t)T * D)) return 1;
+    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return fail("attention kernel %d unknown", kernel);
+    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return fail("wgmma attention needs N <= %d", ATTW_KEYS);
+    if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16);
     if (kernel == ATT_WGMMA || (kernel == ATT_AUTO && N <= ATTW_KEYS))
     {
         // the wgmma kernel always runs on split-precision operands: without lo halves it reads zero lo planes (dev_alloc zero-fills
         // them), whose products add exact zeros
-        if (dev_alloc(e, &e->QKV16L, (size_t)T * 3 * D)) return bail(1);
-        if (qkv_lo)
-        {
-            to_head_major(qkv_lo);
-            if (cudaMemcpy(e->QKV16L, hm.data(), (size_t)T * 3 * D * 2, cudaMemcpyHostToDevice) != cudaSuccess) return bail(fail("H2D failed"));
-        }
-        if (make_attention_maps(e, T)) return bail(1);
+        if (qkv_lo) to_head_major(qkv_lo);
+        if (qkv_lo ? upload(e, &e->QKV16L, hm.data(), hm.size()) : dev_alloc(e, &e->QKV16L, hm.size())) return 1;
+        if (make_attention_maps(e, T)) return 1;
     }
-    // cudaMemcpy from pageable memory may return before the DMA has landed, and the kernels below run on a NON-BLOCKING stream (no implicit
-    // ordering with the legacy stream the copies used): wait for the device before launching
-    if (cudaDeviceSynchronize() != cudaSuccess) return bail(fail("device sync after upload failed"));
-    if (launch_attention(e, B, e->stream, kernel)) return bail(1);
-    if (cudaStreamSynchronize(e->stream) != cudaSuccess) return bail(fail("attention kernel failed: %s", cudaGetErrorString(cudaGetLastError())));
-    std::vector<__half> tmp((size_t)T * D);
-    if (cudaMemcpy(tmp.data(), e->A16, tmp.size() * 2, cudaMemcpyDeviceToHost) != cudaSuccess) return bail(fail("D2H failed"));
-    for (size_t i = 0; i < tmp.size(); ++i) out[i] = __half2float(tmp[i]);
-    return bail(0);
+    if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
+    return tap_f16(out, e->A16, (size_t)T * D, e->stream);
+}
+
+int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out)
+{
+    return guarded(__func__, [&] { return test_attention_impl(device, kernel, B, N, H, qkv, nullptr, out); });
+}
+
+int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
+{
+    return guarded(__func__, [&] {
+        if (!qkv_lo) return fail("bad argument");
+        return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out);
+    });
 }
 
 int vitb200_test_dequant(int type, const void *blocks, int64_t n_blocks, uint16_t *out_f16)
 {
-    const size_t bs = quant_block_bytes(type);
-    if (!bs) return fail("type %d is not a supported block format", type);
-    if (!blocks || !out_f16 || n_blocks < 0) return fail("null argument");
-    float y[32];
-    for (int64_t b = 0; b < n_blocks; ++b)
-    {
-        dequant_block(type, (const uint8_t *)blocks + (size_t)b * bs, y);
-        for (int i = 0; i < 32; ++i) out_f16[b * 32 + i] = host_f32_to_f16(y[i]);
-    }
-    return 0;
+    return guarded(__func__, [&] {
+        const size_t bs = quant_block_bytes(type);
+        if (!bs) return fail("type %d is not a supported block format", type);
+        if (!blocks || !out_f16 || n_blocks < 0) return fail("null argument");
+        float y[32];
+        for (int64_t b = 0; b < n_blocks; ++b)
+        {
+            dequant_block(type, (const uint8_t *)blocks + (size_t)b * bs, y);
+            for (int i = 0; i < 32; ++i) out_f16[b * 32 + i] = host_f32_to_f16(y[i]);
+        }
+        return 0;
+    });
 }
 
 void *vitb200_stream(vitb200_engine *e) { return e ? (void *)e->stream : nullptr; }
@@ -1358,34 +1464,35 @@ void *vitb200_stream(vitb200_engine *e) { return e ? (void *)e->stream : nullptr
 int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, float *d_probs, float *d_logits,
                            int32_t *d_topk_idx, float *d_topk_prob, int k, void *stream)
 {
-    if (!e || !d_images) return fail("null argument");
-    CUDA_TRY(cudaSetDevice(e->device));
-    cudaStream_t s = stream ? (cudaStream_t)stream : e->stream;
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
-    return run_forward_graphed(e, d_images, batch, d_probs, d_logits, d_topk_idx, d_topk_prob, k, s);
+    return guarded(__func__, [&]() -> int {
+        if (!e || !d_images) return fail("null argument");
+        CUDA_TRY(cudaSetDevice(e->device));
+        if (check_batch(e, batch) || check_k(e, k)) return 1;
+        return run_forward_graphed(e, d_images, batch, d_probs, d_logits, d_topk_idx, d_topk_prob, k, stream ? (cudaStream_t)stream : e->stream);
+    });
 }
 
 int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch, const vitb200_features_req *req, void *d_tokens,
                             void *d_prelogits, void *stream)
 {
-    if (check_features(e, d_images, batch, req, d_tokens, d_prelogits)) return 1;
-    if (((uintptr_t)d_tokens | (uintptr_t)d_prelogits) % 16 != 0) return fail("vitb200_features_device: output buffers must be 16-byte aligned");
-    CUDA_TRY(cudaSetDevice(e->device));
-    return run_features_graphed(e, d_images, batch, req, d_tokens, d_prelogits, stream ? (cudaStream_t)stream : e->stream);
+    return guarded(__func__, [&]() -> int {
+        if (check_features(e, d_images, batch, req, d_tokens, d_prelogits)) return 1;
+        if (((uintptr_t)d_tokens | (uintptr_t)d_prelogits) % 16 != 0) return fail("vitb200_features_device: output buffers must be 16-byte aligned");
+        CUDA_TRY(cudaSetDevice(e->device));
+        return run_features_graphed(e, d_images, batch, req, d_tokens, d_prelogits, stream ? (cudaStream_t)stream : e->stream);
+    });
 }
 
-// Host images -> this call's input slot (slot = call parity) on the copy stream, once the slot's previous call has consumed it; the
-// compute stream waits for the copy.  The caller records ev_done[sl] on the compute stream after its last use of the slot.
-static int stage_images(vitb200_engine *e, const float *images, int batch, int &sl)
+// Host images -> this call's input slot on the copy stream, once the slot's previous call has consumed it; the compute stream waits
+// for the copy.  The device is waited on, not the host: only device memory is overwritten.
+static int stage_images(vitb200_engine *e, const Slot &sl, const float *images, int batch)
 {
-    sl = (int)(e->submits & 1);
     cudaStream_t cs = e->copy_stream;
     const size_t img_elems = (size_t)e->C * e->hp.img_size * e->hp.img_size;
-    if (e->submits >= 2) CUDA_TRY(cudaStreamWaitEvent(cs, e->ev_done[sl], 0)); // slot's previous forward has consumed its inputs/outputs
-    CUDA_TRY(cudaMemcpyAsync(e->d_img_slot[sl], images, (size_t)batch * img_elems * sizeof(float), cudaMemcpyHostToDevice, cs));
-    CUDA_TRY(cudaEventRecord(e->ev_h2d[sl], cs));
-    CUDA_TRY(cudaStreamWaitEvent(e->stream, e->ev_h2d[sl], 0));
+    if (e->submits >= 2) CUDA_TRY(cudaStreamWaitEvent(cs, sl.ev_done, 0)); // slot's previous forward has consumed its inputs/outputs
+    CUDA_TRY(cudaMemcpyAsync(sl.img, images, (size_t)batch * img_elems * sizeof(float), cudaMemcpyHostToDevice, cs));
+    CUDA_TRY(cudaEventRecord(sl.ev_h2d, cs));
+    CUDA_TRY(cudaStreamWaitEvent(e->stream, sl.ev_h2d, 0));
     return 0;
 }
 
@@ -1410,50 +1517,34 @@ static int features_to_host(vitb200_engine *e, const float *d_images, int batch,
     return 0;
 }
 
-// Enqueue one batched forward with HOST buffers.  Slot s = call parity: the H2D of this call runs on the copy stream and
-// may overlap the kernels of the previous call (other slot); kernels + D2H run on the compute stream in call order.
+// Enqueue one batched forward with HOST buffers.  The H2D of this call runs on the copy stream and may overlap the kernels of the
+// previous call (other slot); kernels + D2H run on the compute stream in call order.
 static int forward_enqueue(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
                            float *topk_prob, int k, const vitb200_taps *taps)
 {
     if (!e || !images) return fail("null argument");
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k); // before anything is enqueued
+    if (check_batch(e, batch) || check_k(e, k)) return 1; // before anything is enqueued
     CUDA_TRY(cudaSetDevice(e->device));
-    int sl = 0;
-    if (stage_images(e, images, batch, sl)) return 1;
-    cudaStream_t s = e->stream;
-    const size_t rows = (size_t)batch * e->head_tokens; // classifier rows returned
-    const int C = e->hp.num_classes;
-    const bool want_topk = k > 0 && (topk_idx || topk_prob);
-    float *dp = (probs || want_topk) ? e->d_probs_slot[sl] : nullptr;
-    int32_t *di = want_topk ? e->d_topk_idx_slot[sl] : nullptr;
-    float *dv = want_topk ? e->d_topk_val_slot[sl] : nullptr;
-    const int kk = want_topk ? k : 0;
-    if (taps ? run_forward(e, e->d_img_slot[sl], batch, dp, e->d_logits_slot[sl], di, dv, kk, s, taps)
-             : run_forward_graphed(e, e->d_img_slot[sl], batch, dp, e->d_logits_slot[sl], di, dv, kk, s))
-        return 1;
-    if (probs) CUDA_TRY(cudaMemcpyAsync(probs, e->d_probs_slot[sl], rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (logits) CUDA_TRY(cudaMemcpyAsync(logits, e->d_logits_slot[sl], rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
-    if (want_topk && topk_idx) CUDA_TRY(cudaMemcpyAsync(topk_idx, e->d_topk_idx_slot[sl], rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-    if (want_topk && topk_prob) CUDA_TRY(cudaMemcpyAsync(topk_prob, e->d_topk_val_slot[sl], rows * k * sizeof(float), cudaMemcpyDeviceToHost, s));
-    CUDA_TRY(cudaEventRecord(e->ev_done[sl], s));
-    e->submits++;
-    return 0;
+    Slot &sl = begin_submit(e);
+    if (stage_images(e, sl, images, batch) || classify_to_host(e, sl, sl.img, batch, probs, logits, topk_idx, topk_prob, k, taps)) return 1;
+    return end_submit(e, sl);
 }
 
 int vitb200_forward_async(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
                           float *topk_prob, int k)
 {
-    return forward_enqueue(e, images, batch, probs, logits, topk_idx, topk_prob, k, nullptr);
+    return guarded(__func__, [&] { return forward_enqueue(e, images, batch, probs, logits, topk_idx, topk_prob, k, nullptr); });
 }
 
 int vitb200_sync(vitb200_engine *e)
 {
-    if (!e) return fail("null argument");
-    CUDA_TRY(cudaSetDevice(e->device));
-    CUDA_TRY(cudaStreamSynchronize(e->copy_stream));
-    CUDA_TRY(cudaStreamSynchronize(e->stream));
-    return 0;
+    return guarded(__func__, [&]() -> int {
+        if (!e) return fail("null argument");
+        CUDA_TRY(cudaSetDevice(e->device));
+        CUDA_TRY(cudaStreamSynchronize(e->copy_stream));
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+        return 0;
+    });
 }
 
 static int forward_host(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
@@ -1472,7 +1563,7 @@ static int forward_sharded_impl(vitb200_engine *const *engines, int n_engines, c
     if (!engines || n_engines < 1 || !images) return fail("null argument");
     const vitb200_engine *e0 = engines[0];
     if (!e0) return fail("null engine");
-    if (k < 0 || k > e0->max_k) return fail("k %d out of range (0..%d)", k, e0->max_k);
+    if (check_k(e0, k)) return 1;
     {
         // validate every shard before the first one is enqueued
         const int base0 = batch / n_engines, rem0 = batch % n_engines;
@@ -1520,7 +1611,7 @@ static int forward_sharded_impl(vitb200_engine *const *engines, int n_engines, c
 int vitb200_forward_sharded(vitb200_engine *const *engines, int n_engines, const float *images, int batch, float *probs, float *logits,
                             int32_t *topk_idx, float *topk_prob, int k)
 {
-    return forward_sharded_impl(engines, n_engines, images, batch, probs, logits, topk_idx, topk_prob, k, true);
+    return guarded(__func__, [&] { return forward_sharded_impl(engines, n_engines, images, batch, probs, logits, topk_idx, topk_prob, k, true); });
 }
 
 // Pipelined form: every shard goes through its engine's two-slot vitb200_forward_async pipeline and the call returns; the host
@@ -1528,38 +1619,40 @@ int vitb200_forward_sharded(vitb200_engine *const *engines, int n_engines, const
 int vitb200_forward_sharded_async(vitb200_engine *const *engines, int n_engines, const float *images, int batch, float *probs,
                                   float *logits, int32_t *topk_idx, float *topk_prob, int k)
 {
-    return forward_sharded_impl(engines, n_engines, images, batch, probs, logits, topk_idx, topk_prob, k, false);
+    return guarded(__func__, [&] { return forward_sharded_impl(engines, n_engines, images, batch, probs, logits, topk_idx, topk_prob, k, false); });
 }
 
 int vitb200_sync_all(vitb200_engine *const *engines, int n_engines)
 {
-    if (!engines || n_engines < 1) return fail("null argument");
-    int rc = 0;
-    for (int g = 0; g < n_engines; ++g)
-        if (engines[g] && vitb200_sync(engines[g])) rc = 1;
-    return rc;
+    return guarded(__func__, [&] {
+        if (!engines || n_engines < 1) return fail("null argument");
+        int rc = 0;
+        for (int g = 0; g < n_engines; ++g)
+            if (engines[g] && vitb200_sync(engines[g])) rc = 1;
+        return rc;
+    });
 }
 
 int vitb200_forward(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
                     float *topk_prob, int k)
 {
-    return forward_host(e, images, batch, probs, logits, topk_idx, topk_prob, k, nullptr);
+    return guarded(__func__, [&] { return forward_host(e, images, batch, probs, logits, topk_idx, topk_prob, k, nullptr); });
 }
 
 int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, const vitb200_taps *taps)
 {
-    return forward_host(e, images, batch, probs, logits, nullptr, nullptr, 0, taps);
+    return guarded(__func__, [&] { return forward_host(e, images, batch, probs, logits, nullptr, nullptr, 0, taps); });
 }
 
 int vitb200_features(vitb200_engine *e, const float *images, int batch, const vitb200_features_req *req, void *tokens, void *prelogits)
 {
-    if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
-    CUDA_TRY(cudaSetDevice(e->device));
-    int sl = 0;
-    if (stage_images(e, images, batch, sl) || features_to_host(e, e->d_img_slot[sl], batch, req, tokens, prelogits)) return 1;
-    CUDA_TRY(cudaEventRecord(e->ev_done[sl], e->stream));
-    e->submits++;
-    return vitb200_sync(e);
+    return guarded(__func__, [&]() -> int {
+        if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
+        CUDA_TRY(cudaSetDevice(e->device));
+        Slot &sl = begin_submit(e);
+        if (stage_images(e, sl, images, batch) || features_to_host(e, sl.img, batch, req, tokens, prelogits) || end_submit(e, sl)) return 1;
+        return vitb200_sync(e);
+    });
 }
 
 // vit_image_preprocess (reference vit.cpp:289-305) for a batch of u8 RGB images of arbitrary sizes, on the GPU, followed by the
@@ -1568,10 +1661,10 @@ int vitb200_features(vitb200_engine *e, const float *images, int batch, const vi
 // vitb200_forward_async: the caller's images are packed into this slot's pinned staging buffer, ONE host-to-device copy on the copy
 // stream overlaps the previous call's kernels, nothing synchronises on entry and nothing is allocated once the staging buffers
 // have grown to the largest batch seen.
-// stage_u8 packs the images into this call's slot and makes the compute stream wait for their copy (d_u8[sl] holds the pixels,
-// then the PreImage table at table_off); preprocess_u8 adds the RGB kernel up to the patch matrix (and the optional f32 read-back).
-// The caller records ev_done[sl] after its last use of the slot.
-static int stage_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int &sl, size_t &table_off)
+// stage_u8 packs the images into slot sl and makes the compute stream wait for their copy (sl.d_u8 holds the pixels, then the
+// PreImage table at table_off); it waits on the host, because it overwrites pinned host memory the slot's previous copy may still be
+// reading.  preprocess_u8 adds the RGB kernel up to the patch matrix (and the optional f32 read-back).
+static int stage_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, size_t &table_off)
 {
     size_t total = 0;
     for (int b = 0; b < batch; ++b)
@@ -1582,45 +1675,44 @@ static int stage_u8(vitb200_engine *e, const uint8_t *const *images, const int *
     table_off = total;
     total += (size_t)batch * sizeof(PreImage);
     CUDA_TRY(cudaSetDevice(e->device));
-    sl = (int)(e->submits & 1);
     cudaStream_t s = e->stream, cs = e->copy_stream;
     // this slot's previous call (two submissions ago) must have consumed its staging buffer before the host overwrites it
-    if (e->submits >= 2) CUDA_TRY(cudaEventSynchronize(e->ev_done[sl]));
-    if (total > e->u8_cap[sl])
+    if (e->submits >= 2) CUDA_TRY(cudaEventSynchronize(sl.ev_done));
+    if (total > sl.u8_cap)
     {
         const size_t cap = total + total / 4;
-        if (e->h_u8[sl]) cudaFreeHost(e->h_u8[sl]);
-        if (e->d_u8[sl]) cudaFree(e->d_u8[sl]);
-        e->h_u8[sl] = nullptr; e->d_u8[sl] = nullptr; e->u8_cap[sl] = 0;
-        CUDA_TRY(cudaHostAlloc((void **)&e->h_u8[sl], cap, cudaHostAllocDefault));
-        CUDA_TRY(cudaMalloc((void **)&e->d_u8[sl], cap));
-        e->u8_cap[sl] = cap;
+        if (sl.h_u8) cudaFreeHost(sl.h_u8);
+        if (sl.d_u8) cudaFree(sl.d_u8);
+        sl.h_u8 = nullptr; sl.d_u8 = nullptr; sl.u8_cap = 0;
+        CUDA_TRY(cudaHostAlloc((void **)&sl.h_u8, cap, cudaHostAllocDefault));
+        CUDA_TRY(cudaMalloc((void **)&sl.d_u8, cap));
+        sl.u8_cap = cap;
     }
-    PreImage *table = reinterpret_cast<PreImage *>(e->h_u8[sl] + table_off);
+    PreImage *table = reinterpret_cast<PreImage *>(sl.h_u8 + table_off);
     size_t off = 0;
     for (int b = 0; b < batch; ++b)
     {
         const size_t n = (size_t)nx[b] * ny[b] * 3;
-        memcpy(e->h_u8[sl] + off, images[b], n);
+        memcpy(sl.h_u8 + off, images[b], n);
         table[b].offset = off; table[b].nx = nx[b]; table[b].ny = ny[b];
         off += (n + 255) / 256 * 256;
     }
-    CUDA_TRY(cudaMemcpyAsync(e->d_u8[sl], e->h_u8[sl], total, cudaMemcpyHostToDevice, cs));
-    CUDA_TRY(cudaEventRecord(e->ev_h2d[sl], cs));
-    CUDA_TRY(cudaStreamWaitEvent(s, e->ev_h2d[sl], 0));
+    CUDA_TRY(cudaMemcpyAsync(sl.d_u8, sl.h_u8, total, cudaMemcpyHostToDevice, cs));
+    CUDA_TRY(cudaEventRecord(sl.ev_h2d, cs));
+    CUDA_TRY(cudaStreamWaitEvent(s, sl.ev_h2d, 0));
     return 0;
 }
 
-static int preprocess_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
-                         float *images_f32_out, int &sl)
+static int preprocess_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
+                         float *images_f32_out)
 {
     size_t table_off = 0;
-    if (stage_u8(e, images, nx, ny, batch, sl, table_off)) return 1;
+    if (stage_u8(e, sl, images, nx, ny, batch, table_off)) return 1;
     cudaStream_t s = e->stream;
     const int S = e->hp.img_size;
     dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
-    float *d_f32 = images_f32_out ? e->d_img_slot[sl] : nullptr;
-    preprocess_kernel<<<grid, 256, 0, s>>>(e->d_u8[sl], reinterpret_cast<const PreImage *>(e->d_u8[sl] + table_off), d_f32, S, bilinear ? 1 : 0,
+    float *d_f32 = images_f32_out ? sl.img : nullptr;
+    preprocess_kernel<<<grid, 256, 0, s>>>(sl.d_u8, reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, bilinear ? 1 : 0,
                                            e->PA, e->hp.patch_size, e->KPp);
     CUDA_TRY(cudaGetLastError());
     const size_t img_elems = (size_t)3 * S * S;
@@ -1633,62 +1725,45 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
 {
     if (!e || !images || !nx || !ny) return fail("null argument");
     if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
-    if (k < 0 || k > e->max_k) return fail("k %d out of range (0..%d)", k, e->max_k);
-    int sl = 0;
-    if (preprocess_u8(e, images, nx, ny, batch, bilinear, images_f32_out, sl)) return 1;
-    cudaStream_t s = e->stream;
-    const bool want_topk = k > 0 && (topk_idx || topk_prob);
-    const int C = e->hp.num_classes;
-    if (probs || logits || want_topk)
+    if (check_batch(e, batch) || check_k(e, k)) return 1;
+    Slot &sl = begin_submit(e);
+    if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, images_f32_out)) return 1;
+    if (probs || logits || (k > 0 && (topk_idx || topk_prob)))
     {
-        float *dp = (probs || want_topk) ? e->d_probs_slot[sl] : nullptr;
-        if (run_forward_graphed(e, nullptr, batch, dp, e->d_logits_slot[sl], want_topk ? e->d_topk_idx_slot[sl] : nullptr,
-                                want_topk ? e->d_topk_val_slot[sl] : nullptr, want_topk ? k : 0, s))
-            return 1;
+        if (classify_to_host(e, sl, nullptr, batch, probs, logits, topk_idx, topk_prob, k, nullptr)) return 1;
         e->launches += 1; // the preprocess kernel
-        const size_t rows = (size_t)batch * e->head_tokens;
-        if (probs) CUDA_TRY(cudaMemcpyAsync(probs, e->d_probs_slot[sl], rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
-        if (logits) CUDA_TRY(cudaMemcpyAsync(logits, e->d_logits_slot[sl], rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
-        if (want_topk && topk_idx) CUDA_TRY(cudaMemcpyAsync(topk_idx, e->d_topk_idx_slot[sl], rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        if (want_topk && topk_prob) CUDA_TRY(cudaMemcpyAsync(topk_prob, e->d_topk_val_slot[sl], rows * k * sizeof(float), cudaMemcpyDeviceToHost, s));
     }
-    CUDA_TRY(cudaEventRecord(e->ev_done[sl], s));
-    e->submits++;
-    return 0;
+    return end_submit(e, sl);
 }
 
 int vitb200_forward_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                              float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k)
 {
-    VB_NOEXCEPT_BEGIN
-    return forward_u8_enqueue(e, images, nx, ny, batch, bilinear, nullptr, probs, logits, topk_idx, topk_prob, k);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] { return forward_u8_enqueue(e, images, nx, ny, batch, bilinear, nullptr, probs, logits, topk_idx, topk_prob, k); });
 }
 
 int vitb200_forward_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                        float *images_f32_out, float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k)
 {
-    VB_NOEXCEPT_BEGIN
-    if (forward_u8_enqueue(e, images, nx, ny, batch, bilinear, images_f32_out, probs, logits, topk_idx, topk_prob, k)) return 1;
-    return vitb200_sync(e);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] {
+        if (forward_u8_enqueue(e, images, nx, ny, batch, bilinear, images_f32_out, probs, logits, topk_idx, topk_prob, k)) return 1;
+        return vitb200_sync(e);
+    });
 }
 
 int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                         const vitb200_features_req *req, void *tokens, void *prelogits)
 {
-    if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
-    if (!nx || !ny) return fail("vitb200_features_u8: null argument");
-    if (e->C != 3) return fail("vitb200_features_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-    VB_NOEXCEPT_BEGIN
-    int sl = 0;
-    if (preprocess_u8(e, images, nx, ny, batch, bilinear, nullptr, sl) || features_to_host(e, nullptr, batch, req, tokens, prelogits)) return 1;
-    e->launches += 1; // the preprocess kernel
-    CUDA_TRY(cudaEventRecord(e->ev_done[sl], e->stream));
-    e->submits++;
-    return vitb200_sync(e);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] {
+        if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
+        if (!nx || !ny) return fail("vitb200_features_u8: null argument");
+        if (e->C != 3) return fail("vitb200_features_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
+        Slot &sl = begin_submit(e);
+        if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, nullptr) || features_to_host(e, nullptr, batch, req, tokens, prelogits)) return 1;
+        e->launches += 1; // the preprocess kernel
+        if (end_submit(e, sl)) return 1;
+        return vitb200_sync(e);
+    });
 }
 
 // Text recognition with the ViTSTR extension (reference extensions/vitstr.cpp): its grayscale preprocess (vitstr.cpp:128-201) writes
@@ -1704,251 +1779,144 @@ static int recognize_enqueue(vitb200_engine *e, const uint8_t *const *images, co
                     "%d-channel input", e->C);
     if (e->head_tokens < 2) return fail("vitb200_recognize_u8: head_tokens is %d; the greedy decode reads token rows 1 .. head_tokens-1", e->head_tokens);
     if (e->hp.patch_size != 16 && e->hp.patch_size != 8) return fail("1-channel input: patch size %d not supported (8, 16)", e->hp.patch_size);
-    if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
+    if (check_batch(e, batch)) return 1;
     for (int b = 0; b < batch; ++b)
     {
         if (!images[b]) return fail("vitb200_recognize_u8: null argument (image %d)", b);
         if (nx[b] < 2 || ny[b] < 2) return fail("image %d is %dx%d pixels; the grayscale resize needs at least 2x2", b, nx[b], ny[b]);
     }
-    int sl = 0;
+    Slot &sl = begin_submit(e);
     size_t table_off = 0;
-    if (stage_u8(e, images, nx, ny, batch, sl, table_off)) return 1;
+    if (stage_u8(e, sl, images, nx, ny, batch, table_off)) return 1;
     cudaStream_t s = e->stream;
     const int S = e->hp.img_size, TH = e->head_tokens, C = e->hp.num_classes;
-    float *d_f32 = images_f32_out ? e->d_img_slot[sl] : nullptr;
+    float *d_f32 = images_f32_out ? sl.img : nullptr;
     dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
-    preprocess_gray_kernel<<<grid, 256, 0, s>>>(e->d_u8[sl], reinterpret_cast<const PreImage *>(e->d_u8[sl] + table_off), d_f32, S, e->PA,
+    preprocess_gray_kernel<<<grid, 256, 0, s>>>(sl.d_u8, reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, e->PA,
                                                 e->hp.patch_size, e->KPp);
     CUDA_TRY(cudaGetLastError());
     if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * S * S * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (chars || lengths || scores || probs)
     {
         // patches ready (d_images = NULL); top-1 of every head token into the slot; probabilities only when asked for
-        if (run_forward_graphed(e, nullptr, batch, probs ? e->d_probs_slot[sl] : nullptr, nullptr, e->d_topk_idx_slot[sl],
-                                e->d_topk_val_slot[sl], 1, s))
-            return 1;
-        vitstr_decode_kernel<<<(batch + 127) / 128, 128, 0, s>>>(e->d_topk_idx_slot[sl], e->d_topk_val_slot[sl], batch, TH,
-                                                                 e->d_chars_slot[sl], e->d_len_slot[sl], e->d_score_slot[sl]);
+        if (run_forward_graphed(e, nullptr, batch, probs ? sl.probs : nullptr, nullptr, sl.topk_idx, sl.topk_val, 1, s)) return 1;
+        vitstr_decode_kernel<<<(batch + 127) / 128, 128, 0, s>>>(sl.topk_idx, sl.topk_val, batch, TH, sl.chars, sl.len, sl.score);
         CUDA_TRY(cudaGetLastError());
         e->launches += 2; // the preprocess and decode kernels
-        if (chars) CUDA_TRY(cudaMemcpyAsync(chars, e->d_chars_slot[sl], (size_t)batch * (TH - 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        if (lengths) CUDA_TRY(cudaMemcpyAsync(lengths, e->d_len_slot[sl], (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
-        if (scores) CUDA_TRY(cudaMemcpyAsync(scores, e->d_score_slot[sl], (size_t)batch * sizeof(double), cudaMemcpyDeviceToHost, s));
-        if (probs) CUDA_TRY(cudaMemcpyAsync(probs, e->d_probs_slot[sl], (size_t)batch * TH * C * sizeof(float), cudaMemcpyDeviceToHost, s));
+        if (chars) CUDA_TRY(cudaMemcpyAsync(chars, sl.chars, (size_t)batch * (TH - 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        if (lengths) CUDA_TRY(cudaMemcpyAsync(lengths, sl.len, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
+        if (scores) CUDA_TRY(cudaMemcpyAsync(scores, sl.score, (size_t)batch * sizeof(double), cudaMemcpyDeviceToHost, s));
+        if (probs) CUDA_TRY(cudaMemcpyAsync(probs, sl.probs, (size_t)batch * TH * C * sizeof(float), cudaMemcpyDeviceToHost, s));
     }
     else
         e->launches = 1; // preprocess only
-    CUDA_TRY(cudaEventRecord(e->ev_done[sl], s));
-    e->submits++;
-    return 0;
+    return end_submit(e, sl);
 }
 
 int vitb200_recognize_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int32_t *chars,
                                int32_t *lengths, double *scores, float *probs)
 {
-    VB_NOEXCEPT_BEGIN
-    return recognize_enqueue(e, images, nx, ny, batch, nullptr, chars, lengths, scores, probs);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] { return recognize_enqueue(e, images, nx, ny, batch, nullptr, chars, lengths, scores, probs); });
 }
 
 int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, float *images_f32_out,
                          int32_t *chars, int32_t *lengths, double *scores, float *probs)
 {
-    VB_NOEXCEPT_BEGIN
-    if (recognize_enqueue(e, images, nx, ny, batch, images_f32_out, chars, lengths, scores, probs)) return 1;
-    return vitb200_sync(e);
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] {
+        if (recognize_enqueue(e, images, nx, ny, batch, images_f32_out, chars, lengths, scores, probs)) return 1;
+        return vitb200_sync(e);
+    });
 }
 
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
                       const float *resid, float *out)
 {
-    if (!A || !W || !bias || !out) return fail("null argument");
-    if (K % 8 != 0) return fail("K must be a multiple of 8");
-    CUDA_TRY(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    __half *dA = nullptr, *dW = nullptr;
-    float *dB = nullptr, *dR = nullptr;
-    void *dO = nullptr;
-    const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO;
-    const size_t osz = (size_t)M * N * (f16out ? 2 : 4);
-    void *dO2 = nullptr;
-    int rc = 1;
-    do
-    {
-        if (cudaMalloc(&dA, (size_t)M * K * 2) || cudaMalloc(&dW, (size_t)N * K * 2) || cudaMalloc(&dB, (size_t)N * 4) || cudaMalloc(&dO, osz)) { fail("cudaMalloc failed"); break; }
-        cudaMemcpy(dA, A, (size_t)M * K * 2, cudaMemcpyHostToDevice);
-        cudaMemcpy(dW, W, (size_t)N * K * 2, cudaMemcpyHostToDevice);
-        cudaMemcpy(dB, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
-        cudaMemset(dO, 0, osz);
-        if (epilogue == EPI_BIAS_F16_HILO)
-        {
-            if (cudaMalloc(&dO2, osz)) { fail("cudaMalloc failed"); break; }
-            cudaMemset(dO2, 0, osz);
-        }
-        if (epilogue == EPI_BIAS_RESID_F32)
-        {
-            if (!resid) { fail("resid required"); break; }
-            if (cudaMalloc(&dR, (size_t)M * N * 4)) { fail("cudaMalloc failed"); break; }
-            cudaMemcpy(dR, resid, (size_t)M * N * 4, cudaMemcpyHostToDevice);
-        }
-        CUtensorMap tA, tB;
-        if (make_tmap(&tA, dA, M, K, K, GEMM_A_BOX_ROWS) || make_tmap(&tB, dW, N, K, K, GEMM_BN)) break;
+    return guarded(__func__, [&]() -> int {
+        if (!A || !W || !bias || !out) return fail("null argument");
+        if (K % 8 != 0) return fail("K must be a multiple of 8");
+        if (epilogue == EPI_BIAS_RESID_F32 && !resid) return fail("resid required");
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO;
+        const size_t MN = (size_t)M * N;
+        __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
+        float *dB = nullptr, *o32 = nullptr;
+        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dB, bias, N)) return 1;
+        if (f16out && (dev_alloc(e, &hi, MN) || (epilogue == EPI_BIAS_F16_HILO && dev_alloc(e, &lo, MN)))) return 1;
         // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
-        if (epilogue == EPI_BIAS_RESID_F32) cudaMemcpy(dO, dR, (size_t)M * N * 4, cudaMemcpyDeviceToDevice);
+        if (!f16out && (epilogue == EPI_BIAS_RESID_F32 ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
+        CUtensorMap tA, tB;
+        if (make_tmap(&tA, dA, M, K, K, GEMM_A_BOX_ROWS) || make_tmap(&tB, dW, N, K, K, GEMM_BN)) return 1;
         GemmParams p{};
-        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dO; p.out2 = dO2; p.ldo = N; p.resid = (const float *)dO;
-        if (launch_gemm(nullptr, epilogue, tA, tB, p, 0)) break;
-        cudaError_t err = cudaDeviceSynchronize();
-        if (err != cudaSuccess) { fail("GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
-        if (f16out)
-        {
-            std::vector<__half> tmp((size_t)M * N);
-            cudaMemcpy(tmp.data(), dO, osz, cudaMemcpyDeviceToHost);
-            for (size_t i = 0; i < tmp.size(); ++i) out[i] = __half2float(tmp[i]);
-            if (dO2) // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
-            {
-                cudaMemcpy(tmp.data(), dO2, osz, cudaMemcpyDeviceToHost);
-                for (size_t i = 0; i < tmp.size(); ++i) out[i] += __half2float(tmp[i]);
-            }
-        }
-        else
-            cudaMemcpy(out, dO, osz, cudaMemcpyDeviceToHost);
-        rc = 0;
-    } while (0);
-    cudaFree(dA); cudaFree(dW); cudaFree(dB); cudaFree(dO); cudaFree(dR); cudaFree(dO2);
-    return rc;
+        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = N; p.resid = o32;
+        if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
+        // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
+        return f16out ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
+    });
 }
 
-// Stand-alone run of the block LayerNorm as the engine launches it (persistent bulk-copy kernel for hidden sizes that are a multiple of 128
-// and >= 8 rows, the row-per-warp kernel otherwise): x [rows][D] f32 -> y [rows][D] (f16 results widened to f32).
 int vitb200_test_layernorm(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, float *y)
 {
-    if (!x || !w || !b || !y || rows < 1 || D < 4 || D % 4 != 0 || D > 2048) return fail("bad argument");
-    VB_NOEXCEPT_BEGIN
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    vitb200_engine e{};
-    e.hp.hidden_size = D; e.hp.eps = eps; e.num_sms = prop.multiProcessorCount; e.device = device;
-    float *dx = nullptr, *dw = nullptr, *db = nullptr;
-    __half *dy = nullptr;
-    int rc = 1;
-    do
-    {
-        if (cudaMalloc(&dx, (size_t)rows * D * 4) || cudaMalloc(&dw, (size_t)D * 4) || cudaMalloc(&db, (size_t)D * 4) || cudaMalloc(&dy, (size_t)rows * D * 2)) { fail("cudaMalloc failed"); break; }
-        cudaMemcpy(dx, x, (size_t)rows * D * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(dw, w, (size_t)D * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(db, b, (size_t)D * 4, cudaMemcpyHostToDevice);
-        cudaMemset(dy, 0xFF, (size_t)rows * D * 2);
-        if (cudaDeviceSynchronize() != cudaSuccess) { fail("device sync failed"); break; }
-        if (launch_layernorm(&e, dx, (size_t)D, dw, db, dy, rows, 0)) break;
-        cudaError_t err = cudaDeviceSynchronize();
-        if (err != cudaSuccess) { fail("LayerNorm kernel failed: %s", cudaGetErrorString(err)); break; }
-        std::vector<__half> tmp((size_t)rows * D);
-        cudaMemcpy(tmp.data(), dy, tmp.size() * 2, cudaMemcpyDeviceToHost);
-        for (size_t i = 0; i < tmp.size(); ++i) y[i] = __half2float(tmp[i]);
-        rc = 0;
-    } while (0);
-    cudaFree(dx); cudaFree(dw); cudaFree(db); cudaFree(dy);
-    return rc;
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&] {
+        if (!x || !w || !b || !y || rows < 1 || D < 4 || D % 4 != 0 || D > 2048) return fail("bad argument");
+        EnginePtr owner;
+        __half *dy = nullptr;
+        if (test_layernorm_impl(device, rows, D, x, w, b, eps, &dy, nullptr, owner)) return 1;
+        return tap_f16(y, dy, (size_t)rows * D, owner->stream);
+    });
 }
 
 int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, float *scale)
 {
-    if (!w_f16 || !q || !scale || n < 1) return fail("bad argument");
-    *scale = quantize_e4m3(w_f16, (size_t)n, q);
-    return 0;
+    return guarded(__func__, [&] {
+        if (!w_f16 || !q || !scale || n < 1) return fail("bad argument");
+        *scale = quantize_e4m3(w_f16, (size_t)n, q);
+        return 0;
+    });
 }
 
 // Stand-alone run of the e4m3 GEMM as the FP8 engine launches it (qkv and fc1): A [M][K] and W [N][K] e4m3 bytes, a_scale [M], w_scale.
 int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
                           float w_scale, const float *bias, float *out)
 {
-    if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
-    if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
-    if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO)
-        return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6)", epilogue);
-    VB_NOEXCEPT_BEGIN
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
-    uint8_t *dA = nullptr, *dW = nullptr;
-    float *dS = nullptr, *dB = nullptr;
-    __half *dO = nullptr, *dO2 = nullptr;
-    const size_t osz = (size_t)M * N * 2;
-    int rc = 1;
-    do
-    {
-        if (cudaMalloc(&dA, (size_t)M * K) || cudaMalloc(&dW, (size_t)N * K) || cudaMalloc(&dS, (size_t)M * 4) || cudaMalloc(&dB, (size_t)N * 4) ||
-            cudaMalloc(&dO, osz) || cudaMalloc(&dO2, osz)) { fail("cudaMalloc failed"); break; }
-        cudaMemcpy(dA, A, (size_t)M * K, cudaMemcpyHostToDevice);
-        cudaMemcpy(dW, W, (size_t)N * K, cudaMemcpyHostToDevice);
-        cudaMemcpy(dS, a_scale, (size_t)M * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(dB, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
-        cudaMemset(dO, 0, osz);
-        cudaMemset(dO2, 0, osz);
+    return guarded(__func__, [&]() -> int {
+        if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
+        if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
+        if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO)
+            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6)", epilogue);
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        const size_t MN = (size_t)M * N;
+        uint8_t *dA = nullptr, *dW = nullptr;
+        float *dS = nullptr, *dB = nullptr;
+        __half *hi = nullptr, *lo = nullptr;
+        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dS, a_scale, M) || upload(e, &dB, bias, N) ||
+            dev_alloc(e, &hi, MN) || dev_alloc(e, &lo, MN))
+            return 1;
         CUtensorMap tA, tB;
-        if (make_tmap_e4m3(&tA, dA, M, K, GEMM_A_BOX_ROWS) || make_tmap_e4m3(&tB, dW, N, K, GEMM_BN)) break;
+        if (make_tmap_e4m3(&tA, dA, M, K, GEMM_A_BOX_ROWS) || make_tmap_e4m3(&tB, dW, N, K, GEMM_BN)) return 1;
         GemmParams p{};
-        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dO; p.out2 = dO2; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
-        if (launch_gemm(nullptr, epilogue, tA, tB, p, 0, true)) break;
-        cudaError_t err = cudaDeviceSynchronize();
-        if (err != cudaSuccess) { fail("e4m3 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
-        std::vector<__half> hi((size_t)M * N), lo((size_t)M * N);
-        cudaMemcpy(hi.data(), dO, osz, cudaMemcpyDeviceToHost);
-        cudaMemcpy(lo.data(), dO2, osz, cudaMemcpyDeviceToHost);
+        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
+        if (run_scratch(e, "e4m3 GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, true); })) return 1;
         // split-precision result: hi + lo (exact in f32); the other epilogues leave lo zero
-        for (size_t i = 0; i < hi.size(); ++i) out[i] = __half2float(hi[i]) + __half2float(lo[i]);
-        rc = 0;
-    } while (0);
-    cudaFree(dA); cudaFree(dW); cudaFree(dS); cudaFree(dB); cudaFree(dO); cudaFree(dO2);
-    return rc;
-    VB_NOEXCEPT_END((void)0)
+        return tap_f16(out, hi, MN, e->stream, lo);
+    });
 }
 
 // The FP8 engine's LayerNorm 1 / 2 alone, launched as vitb200_test_layernorm launches the f16 one: q [rows][D] e4m3 bytes, sa [rows].
 int vitb200_test_layernorm_fp8(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, uint8_t *q, float *sa)
 {
-    if (!x || !w || !b || !q || !sa || rows < 1 || D < 4 || D % 16 != 0 || D > 2048) return fail("bad argument");
-    VB_NOEXCEPT_BEGIN
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    vitb200_engine e{};
-    e.hp.hidden_size = D; e.hp.eps = eps; e.num_sms = prop.multiProcessorCount; e.device = device;
-    float *dx = nullptr, *dw = nullptr, *db = nullptr, *ds = nullptr;
-    uint8_t *dq = nullptr;
-    int rc = 1;
-    do
-    {
-        if (cudaMalloc(&dx, (size_t)rows * D * 4) || cudaMalloc(&dw, (size_t)D * 4) || cudaMalloc(&db, (size_t)D * 4) || cudaMalloc(&dq, (size_t)rows * D) ||
-            cudaMalloc(&ds, (size_t)rows * 4)) { fail("cudaMalloc failed"); break; }
-        cudaMemcpy(dx, x, (size_t)rows * D * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(dw, w, (size_t)D * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(db, b, (size_t)D * 4, cudaMemcpyHostToDevice);
-        cudaMemset(dq, 0xFF, (size_t)rows * D);
-        cudaMemset(ds, 0xFF, (size_t)rows * 4);
-        if (cudaDeviceSynchronize() != cudaSuccess) { fail("device sync failed"); break; }
-        if (launch_layernorm(&e, dx, (size_t)D, dw, db, (__nv_fp8_e4m3 *)dq, rows, 0, 0, 0, ds)) break;
-        cudaError_t err = cudaDeviceSynchronize();
-        if (err != cudaSuccess) { fail("LayerNorm kernel failed: %s", cudaGetErrorString(err)); break; }
-        cudaMemcpy(q, dq, (size_t)rows * D, cudaMemcpyDeviceToHost);
-        cudaMemcpy(sa, ds, (size_t)rows * 4, cudaMemcpyDeviceToHost);
-        rc = 0;
-    } while (0);
-    cudaFree(dx); cudaFree(dw); cudaFree(db); cudaFree(dq); cudaFree(ds);
-    return rc;
-    VB_NOEXCEPT_END((void)0)
+    return guarded(__func__, [&]() -> int {
+        if (!x || !w || !b || !q || !sa || rows < 1 || D < 4 || D % 16 != 0 || D > 2048) return fail("bad argument");
+        EnginePtr owner;
+        __nv_fp8_e4m3 *dq = nullptr;
+        float *ds = nullptr;
+        if (test_layernorm_impl(device, rows, D, x, w, b, eps, &dq, &ds, owner)) return 1;
+        CUDA_TRY(cudaMemcpy(q, dq, (size_t)rows * D, cudaMemcpyDeviceToHost));
+        return tap_f32(sa, ds, rows, owner->stream);
+    });
 }
 
 // q8_0 linear layer on the integer tensor cores (gemm_q8_wgmma.cuh; prototype for BASELINE.json configs[4]): x [M][K] f32 is
@@ -1958,86 +1926,77 @@ int vitb200_test_layernorm_fp8(int device, int rows, int D, const float *x, cons
 int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const void *w_q8_0, const float *bias, float *y,
                          int8_t *xq, float *xd, int iters, float *ms_per_launch)
 {
-    if (!x || !w_q8_0 || !bias || !y || M < 1 || N < 1 || K < 1) return fail("bad argument");
-    if (K % Q8_BK != 0) return fail("K must be a multiple of %d", Q8_BK);
-    if (N % 4 != 0) return fail("N must be a multiple of 4");
-    VB_NOEXCEPT_BEGIN
-    int ndev = 0;
-    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail("no CUDA device: the vit.cpp_b200 forward path has no CPU fallback");
-    if (device < 0 || device >= ndev) return fail("device %d out of range (%d devices)", device, ndev);
-    CUDA_TRY(cudaSetDevice(device));
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) return fail("device %d is sm_%d%d; this library is built for sm_90a (H100) only", device, prop.major, prop.minor);
-    const int KB = K / 32;
-    // repack the 34-byte blocks: int8 plane [N][K] + transposed scale plane [K/32][N]
-    std::vector<int8_t> wq((size_t)N * K);
-    std::vector<float> wdT((size_t)KB * N);
-    const uint8_t *blk = (const uint8_t *)w_q8_0;
-    for (int n = 0; n < N; ++n)
-        for (int b = 0; b < KB; ++b)
-        {
-            const uint8_t *src = blk + ((size_t)n * KB + b) * 34;
-            uint16_t du;
-            memcpy(&du, src, 2);
-            wdT[(size_t)b * N + n] = host_f16_to_f32(du);
-            memcpy(&wq[(size_t)n * K + (size_t)b * 32], src + 2, 32);
-        }
-    float *dX = nullptr, *dAd = nullptr, *dWd = nullptr, *dB = nullptr, *dY = nullptr;
-    int8_t *dAq = nullptr, *dWq = nullptr;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    int rc = 1;
-    do
-    {
-        if (cudaMalloc(&dX, (size_t)M * K * 4) || cudaMalloc(&dAq, (size_t)M * K) || cudaMalloc(&dAd, (size_t)M * KB * 4) ||
-            cudaMalloc(&dWq, (size_t)N * K) || cudaMalloc(&dWd, (size_t)KB * N * 4) || cudaMalloc(&dB, (size_t)N * 4) ||
-            cudaMalloc(&dY, (size_t)M * N * 4)) { fail("cudaMalloc failed"); break; }
-        cudaMemcpy(dX, x, (size_t)M * K * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(dWq, wq.data(), wq.size(), cudaMemcpyHostToDevice);
-        cudaMemcpy(dWd, wdT.data(), wdT.size() * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(dB, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
-        cudaMemset(dY, 0, (size_t)M * N * 4);
+    return guarded(__func__, [&]() -> int {
+        if (!x || !w_q8_0 || !bias || !y || M < 1 || N < 1 || K < 1) return fail("bad argument");
+        if (K % Q8_BK != 0) return fail("K must be a multiple of %d", Q8_BK);
+        if (N % 4 != 0) return fail("N must be a multiple of 4");
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        cudaStream_t s = e->stream;
+        const int KB = K / 32;
+        // repack the 34-byte blocks: int8 plane [N][K] + transposed scale plane [K/32][N]
+        std::vector<int8_t> wq((size_t)N * K);
+        std::vector<float> wdT((size_t)KB * N);
+        const uint8_t *blk = (const uint8_t *)w_q8_0;
+        for (int n = 0; n < N; ++n)
+            for (int b = 0; b < KB; ++b)
+            {
+                const uint8_t *src = blk + ((size_t)n * KB + b) * 34;
+                uint16_t du;
+                memcpy(&du, src, 2);
+                wdT[(size_t)b * N + n] = host_f16_to_f32(du);
+                memcpy(&wq[(size_t)n * K + (size_t)b * 32], src + 2, 32);
+            }
+        float *dX = nullptr, *dAd = nullptr, *dWd = nullptr, *dB = nullptr, *dY = nullptr;
+        int8_t *dAq = nullptr, *dWq = nullptr;
+        if (upload(e, &dX, x, (size_t)M * K) || dev_alloc(e, &dAq, (size_t)M * K) || dev_alloc(e, &dAd, (size_t)M * KB) ||
+            upload(e, &dWq, wq.data(), wq.size()) || upload(e, &dWd, wdT.data(), wdT.size()) || upload(e, &dB, bias, N) ||
+            dev_alloc(e, &dY, (size_t)M * N))
+            return 1;
         CUtensorMap tA, tW, tAd, tWd;
         if (make_tmap_2d(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dAq, (uint64_t)M, (uint64_t)K, (uint64_t)K, Q8_BK, Q8_BM, CU_TENSOR_MAP_SWIZZLE_128B) ||
             make_tmap_2d(&tW, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dWq, (uint64_t)N, (uint64_t)K, (uint64_t)K, Q8_BK, Q8_BN, CU_TENSOR_MAP_SWIZZLE_128B) ||
             make_tmap_2d(&tAd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dAd, (uint64_t)M, (uint64_t)KB, (uint64_t)KB, 4, Q8_BM, CU_TENSOR_MAP_SWIZZLE_NONE) ||
             make_tmap_2d(&tWd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dWd, (uint64_t)KB, (uint64_t)N, (uint64_t)N, Q8_BN, 4, CU_TENSOR_MAP_SWIZZLE_NONE))
-            break;
-        const long long n_blocks = (long long)M * KB;
-        const int qthreads = 256;
-        const long long qgrid = (n_blocks * 8 + qthreads - 1) / qthreads;
-        quantize_q8_0_kernel<<<(unsigned)qgrid, qthreads>>>(dX, dAq, dAd, n_blocks);
-        if (cudaGetLastError() != cudaSuccess) { fail("quantize launch failed"); break; }
-        if (cudaFuncSetAttribute(gemm_q8_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Q8_SMEM_BYTES) != cudaSuccess) { fail("cudaFuncSetAttribute failed"); break; }
+            return 1;
+        if (cudaFuncSetAttribute(gemm_q8_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Q8_SMEM_BYTES) != cudaSuccess) return fail("cudaFuncSetAttribute failed");
         Q8GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dY; p.ldo = N;
-        const int tiles = ((M + Q8_BM - 1) / Q8_BM) * ((N + Q8_BN - 1) / Q8_BN);
-        const int grid = tiles;
-        gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
-        cudaError_t err = cudaDeviceSynchronize();
-        if (err != cudaSuccess) { fail("q8_0 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
-        cudaMemcpy(y, dY, (size_t)M * N * 4, cudaMemcpyDeviceToHost);
-        if (xq) cudaMemcpy(xq, dAq, (size_t)M * K, cudaMemcpyDeviceToHost);
-        if (xd) cudaMemcpy(xd, dAd, (size_t)M * KB * 4, cudaMemcpyDeviceToHost);
+        const int grid = ((M + Q8_BM - 1) / Q8_BM) * ((N + Q8_BN - 1) / Q8_BN); // one CTA per tile
+        auto run = [&] {
+            const long long n_blocks = (long long)M * KB;
+            const int qthreads = 256;
+            const long long qgrid = (n_blocks * 8 + qthreads - 1) / qthreads;
+            quantize_q8_0_kernel<<<(unsigned)qgrid, qthreads, 0, s>>>(dX, dAq, dAd, n_blocks);
+            if (cudaGetLastError() != cudaSuccess) return fail("quantize launch failed");
+            gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES, s>>>(tA, tW, tAd, tWd, p);
+            return 0;
+        };
+        if (run_scratch(e, "q8_0 GEMM kernel", run) || tap_f32(y, dY, (size_t)M * N, s)) return 1;
+        if (xq) CUDA_TRY(cudaMemcpy(xq, dAq, (size_t)M * K, cudaMemcpyDeviceToHost));
+        if (xd) CUDA_TRY(cudaMemcpy(xd, dAd, (size_t)M * KB * 4, cudaMemcpyDeviceToHost));
         if (iters > 0 && ms_per_launch)
         {
-            cudaEventCreate(&e0); cudaEventCreate(&e1);
-            cudaEventRecord(e0);
-            for (int i = 0; i < iters; ++i) gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES>>>(tA, tW, tAd, tWd, p);
-            cudaEventRecord(e1);
-            err = cudaDeviceSynchronize();
-            if (err != cudaSuccess) { fail("q8_0 GEMM kernel failed: %s", cudaGetErrorString(err)); break; }
+            // the engine's event pool is destroyed with it
+            cudaEvent_t t0 = nullptr, t1 = nullptr;
+            CUDA_TRY(cudaEventCreate(&t0));
+            e->event_pool.push_back(t0);
+            CUDA_TRY(cudaEventCreate(&t1));
+            e->event_pool.push_back(t1);
+            auto timed = [&]() -> int {
+                CUDA_TRY(cudaEventRecord(t0, s));
+                for (int i = 0; i < iters; ++i) gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES, s>>>(tA, tW, tAd, tWd, p);
+                CUDA_TRY(cudaEventRecord(t1, s));
+                return 0;
+            };
+            if (run_scratch(e, "q8_0 GEMM kernel", timed)) return 1;
             float ms = 0.f;
-            cudaEventElapsedTime(&ms, e0, e1);
+            CUDA_TRY(cudaEventElapsedTime(&ms, t0, t1));
             *ms_per_launch = ms / (float)iters;
         }
-        rc = 0;
-    } while (0);
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-    cudaFree(dX); cudaFree(dAq); cudaFree(dAd); cudaFree(dWq); cudaFree(dWd); cudaFree(dB); cudaFree(dY);
-    return rc;
-    VB_NOEXCEPT_END((void)0)
+        return 0;
+    });
 }
 
 } // extern "C"
@@ -2047,28 +2006,10 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
 // convert-pth-to-ggml.py:105-158).  Validation mirrors the reference: magic, known tensor names, element
 // counts; failures return non-zero with a message, never abort.
 
-extern "C" int vitb200_create_from_file(const char *path, int device, int max_batch, vitb200_engine **out)
-{
-    return vitb200_create_from_file_ex(path, device, max_batch, 1, out);
-}
-
-static int create_from_file(const char *path, int device, int max_batch, int head_tokens, bool fp8, vitb200_engine **out);
-
-extern "C" int vitb200_create_from_file_ex(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
-{
-    return create_from_file(path, device, max_batch, head_tokens, false, out);
-}
-
-extern "C" int vitb200_create_from_file_fp8(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
-{
-    return create_from_file(path, device, max_batch, head_tokens, true, out);
-}
-
 static int create_from_file(const char *path, int device, int max_batch, int head_tokens, bool fp8, vitb200_engine **out)
 {
     if (!path || !out) return fail("null argument");
     *out = nullptr;
-    VB_NOEXCEPT_BEGIN
     std::ifstream fin(path, std::ios::binary);
     if (!fin) return fail("failed to open '%s'", path);
     fin.seekg(0, std::ios::end);
@@ -2108,9 +2049,20 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
         ts[i].n_dims = g.tensors[i].n_dims;
         for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
     }
-    const std::map<int, std::string> &labels = g.labels;
-    int rc = create_checked(&hp, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out);
-    if (rc == 0) (*out)->labels = labels;
-    return rc;
-    VB_NOEXCEPT_END(if (*out) { vitb200_destroy(*out); *out = nullptr; })
+    return create_impl(&hp, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out, &g.labels);
+}
+
+extern "C" int vitb200_create_from_file(const char *path, int device, int max_batch, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_from_file(path, device, max_batch, 1, false, out); });
+}
+
+extern "C" int vitb200_create_from_file_ex(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_from_file(path, device, max_batch, head_tokens, false, out); });
+}
+
+extern "C" int vitb200_create_from_file_fp8(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_from_file(path, device, max_batch, head_tokens, true, out); });
 }
