@@ -91,6 +91,27 @@ int vitb200_create_from_file_ex(const char *path, int device, int max_batch, int
 int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                        int head_tokens, vitb200_engine **out);
 int vitb200_create_from_file_fp8(const char *path, int device, int max_batch, int head_tokens, vitb200_engine **out);
+/* ---- architecture variants: CLIP image towers (no reference counterpart) ------------------------------------------------------
+ * The reference's ViT is timm's VisionTransformer with tanh GELU and no pre-norm.  CLIP towers (OpenAI and LAION CLIP, LLaVA's vision
+ * encoder, timm's vit_*_clip_* models) add a LayerNorm on the embeddings and use another MLP activation. */
+typedef struct vitb200_arch
+{
+    int32_t pre_norm;   /* 0: none (the reference).  1: LayerNorm 'norm_pre.weight' / 'norm_pre.bias' [D] (HF CLIP's pre_layrnorm, timm's
+                         *    norm_pre) on every token row of the embeddings (cls included), written back to the f32 residual stream, before
+                         *    block 0.  Same arithmetic and eps as the block LayerNorms, f32 out. */
+    int32_t activation; /* MLP activation after fc1: 0 GELU, tanh form, through ggml's f16 table (the reference, unchanged); 1 GELU, erf form,
+                         * 0.5 x (1 + erf(x / sqrt 2)); 2 QuickGELU, x / (1 + exp(-1.702 x)).  Forms 1 and 2 take x = acc + bias (FP8 engine:
+                         * acc (sa sw) + bias) in f32, without rounding it to f16 first, and store f16(act(x)). */
+} vitb200_arch;
+/* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = {0, 0}, the reference).
+ * Fields out of range, and pre_norm = 1 without both norm_pre tensors, fail here before the device is touched.  Every entry point
+ * works on such an engine; the u8 entry points keep vit.cpp's preprocessing (a CLIP caller normalises its own images and uses the f32
+ * or device entry points).  The launch count of one forward is 3 + 7 L + 3, plus 1 with the pre-norm.
+ * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer) and vit.activation ("gelu_tanh", "gelu_erf",
+ * "quick_gelu"; any other string fails the load) and then holds 2 more tensors; legacy-ggml files are always the reference's. */
+int vitb200_create_arch(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *tensors, int n_tensors, int device,
+                        int max_batch, int head_tokens, int fp8, vitb200_engine **out);
+int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out);
 int vitb200_fp8(const vitb200_engine *e);         /* 1 for an FP8 engine, else 0 */
 int vitb200_in_chans(const vitb200_engine *e);    /* 3, or 1 for a ViTSTR model */
 int vitb200_head_tokens(const vitb200_engine *e); /* classifier rows per image */
@@ -177,8 +198,9 @@ int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, 
 typedef struct vitb200_features_req
 {
     int32_t layers; /* encoder blocks to run, 0..num_hidden_layers.  0 = the embeddings (patch GEMM + conv bias + cls + pos_embed,
-                     * reference vit.cpp:772-797); num_hidden_layers = the whole encoder (vit.cpp:802-901).  Blocks past `layers`
-                     * are not launched. */
+                     * reference vit.cpp:772-797), after the pre-norm when the model has one (vitb200_arch): the input of block 0, which
+                     * is Hugging Face CLIP's hidden_states[0]; num_hidden_layers = the whole encoder (vit.cpp:802-901).  Blocks past
+                     * `layers` are not launched.  LLaVA's image features: layers = num_hidden_layers - 1, norm = 0, tokens 1..N-1. */
     int32_t norm;   /* 1: apply the model's final LayerNorm (norm.weight / norm.bias, vit.cpp:915-919) to every emitted row;
                      * 0: the residual stream as it stands after `layers` blocks */
     int32_t dtype;  /* 0 f32, 1 f16, 2 bf16 -- the 16-bit forms are the f32 result rounded to nearest even */
@@ -220,7 +242,7 @@ const char *vitb200_last_error(void);
 typedef struct vitb200_taps
 {
     int32_t layer;
-    float *embed;    /* [batch][N][D]  */
+    float *embed;    /* [batch][N][D]  the input of block 0 (after the pre-norm, if any) */
     float *ln1;      /* [batch][N][D]  */
     float *qkv;      /* [batch][N][3D] */
     float *attn;     /* [batch][N][D]  */
@@ -237,7 +259,8 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
 
 /* Stand-alone run of the wgmma GEMM kernel: out[M][N] = epilogue(A[M][K] (f16 bits) x W[N][K]^T (f16 bits)).
  * epilogue: 0 bias->f16, 1 bias+gelu->f16, 2 bias+resid->f32, 4 bias->f32, 6 bias->split precision (hi = f16(x), lo = f16(x - hi);
- * `out` receives hi + lo).  out is float32[M][N] on the host (f16 results widened).  resid may be NULL unless epilogue == 2. */
+ * `out` receives hi + lo), 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16 (vitb200_arch.activation 1 and 2).  out is float32[M][N] on the
+ * host (f16 results widened).  resid may be NULL unless epilogue == 2. */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
                       const float *bias, const float *resid, float *out);
 
@@ -251,7 +274,7 @@ int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, floa
 
 /* Stand-alone run of the e4m3 GEMM the FP8 engine uses for qkv and fc1: A [M][K] and W [N][K] e4m3 bytes, a_scale float32 [M] (one per
  * A row), w_scale, bias [N]; out float32 [M][N] = the epilogue's f16 result widened (epilogue 0 bias->f16, 1 bias+gelu->f16,
- * 6 split precision: hi + lo) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
+ * 6 split precision: hi + lo, 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
 int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
                           float w_scale, const float *bias, float *out);
 

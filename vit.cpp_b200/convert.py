@@ -1,6 +1,8 @@
 """Offline converters for ViT checkpoints -- the timm-free counterpart of the reference's convert-pth-to-ggml.py and quantize.cpp.
 
     python -m convert <checkpoint.pth|.safetensors> <out.gguf> [--ftype 0|1] [--heads H] [--labels labels.json] [--container legacy|gguf]
+                      [--keep-norm-pre] [--activation gelu_tanh|gelu_erf|quick_gelu] [--eps E]     (timm; these three need GGUF)
+    python -m convert <CLIP model.safetensors|.pth> <out.gguf> --hf-config config.json             (Hugging Face CLIP vision tower)
     python -m convert --quantize <in.gguf> <out.gguf> q8_0
 
 * `state_dict_to_model_file` follows reference convert-pth-to-ggml.py:105-158 step by step (header, id2label table, tensors in
@@ -9,6 +11,8 @@
   here with numpy only) -- instead of instantiating the model through timm.  Hyper-parameters are inferred from the tensor shapes
   (timm `VisionTransformer` names, reference vit.cpp:518-579); the head count is not recoverable from shapes and defaults to
   hidden / 64 (true for every timm ViT the reference lists).
+* `clip_to_model_file` converts a Hugging Face CLIP vision tower (`vision_model.*` of CLIPVisionModel, CLIPVisionModelWithProjection
+  or CLIPModel) to a GGUF file with the pre-norm, QuickGELU or erf GELU and eps 1e-5 (`clip_to_timm` holds the name mapping).
 * `quantize_model_file` restates reference quantize.cpp for q8_0 (every 2-D `*weight` tensor, quantize_row_q8_0_reference,
   ggml-quants.c): byte-identical to the reference binary's output (pinned by the CPU test-suite).
 
@@ -102,13 +106,24 @@ def infer_hparams(sd: Dict[str, np.ndarray], heads: Optional[int] = None):
 
 
 def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: int = 1, heads: Optional[int] = None,
-                             id2label: Optional[Dict[int, str]] = None, container: str = "legacy") -> None:
+                             id2label: Optional[Dict[int, str]] = None, container: str = "legacy", keep_norm_pre: bool = False,
+                             activation: str = "gelu_tanh", eps: float = 1e-6) -> None:
+    """keep_norm_pre, activation, eps: the architecture of a CLIP-pretrained timm ViT (norm_pre, QuickGELU or erf GELU, eps 1e-5);
+    GGUF only.  Without them the file is the reference converter's, which drops norm_pre."""
     assert ftype in (0, 1)
+    if activation not in gf.ACTIVATIONS:
+        raise ValueError(f"activation {activation!r} unknown ({', '.join(gf.ACTIVATIONS)})")
+    if container != "gguf" and (keep_norm_pre or activation != "gelu_tanh" or eps != 1e-6):
+        raise ValueError("a pre-norm, another activation or another eps needs --container gguf: a legacy ggml file carries the "
+                         "reference's architecture only")
+    if keep_norm_pre and not ("norm_pre.weight" in sd and "norm_pre.bias" in sd):
+        raise ValueError("keep_norm_pre: the state_dict has no norm_pre.weight / norm_pre.bias")
     hidden, layers, heads, classes, patch, img, in_chans = infer_hparams(sd, heads)
     id2label = id2label or {i: f"LABEL_{i}" for i in range(classes)}   # convert-pth-to-ggml.py:95-96 fallback names
-    vf = gf.VitFile(hidden, layers, heads, classes, patch, img, ftype, dict(id2label))
+    vf = gf.VitFile(hidden, layers, heads, classes, patch, img, ftype, dict(id2label), eps=eps, pre_norm=int(keep_norm_pre),
+                    activation=activation)
     for k, v in sd.items():
-        if k.startswith("norm_pre"):                                     # convert-pth-to-ggml.py:127-130
+        if k.startswith("norm_pre") and not keep_norm_pre:               # convert-pth-to-ggml.py:127-130
             continue
         a = np.asarray(v)
         if k == "patch_embed.proj.bias":
@@ -118,13 +133,73 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
         f16 = (ftype == 1 and np.asarray(v).ndim != 1 and k not in ("pos_embed", "cls_token")) or k == "patch_embed.proj.weight"
         vf.tensors[k] = a.astype(np.float16 if f16 else np.float32)
         vf.tensor_ftype[k] = 1 if f16 else 0
-    expect = 4 + 12 * layers + 4                                         # vit.cpp:697
+    expect = 4 + 12 * layers + 4 + 2 * vf.pre_norm                      # vit.cpp:697, plus norm_pre.weight / .bias
     if len(vf.tensors) != expect:
         raise ValueError(f"state_dict has {len(vf.tensors)} tensors after filtering, a {layers}-layer ViT needs {expect}")
     if container == "gguf":
         gf.write_gguf(out_path, vf, "keep")
     else:
         write_legacy(out_path, vf)
+
+
+# Hugging Face CLIP activations -> the file's (vitb200_arch.activation); HF's "gelu" is the erf form
+_HF_ACTIVATIONS = {"quick_gelu": "quick_gelu", "gelu": "gelu_erf"}
+
+
+def is_hf_clip(sd: Dict[str, np.ndarray]) -> bool:
+    """A CLIPVisionModel, CLIPVisionModelWithProjection or CLIPModel state dict (the vision tower under `vision_model.`)."""
+    return any(k.startswith("vision_model.") for k in sd)
+
+
+def clip_to_timm(sd: Dict[str, np.ndarray], config: dict):
+    """Hugging Face CLIP vision tower -> (timm VisionTransformer state dict in timm's key order, heads, activation, eps).
+    config: the model's config.json (a CLIPConfig's `vision_config` is used when present).  The projection becomes the classifier
+    head (bias 0), so the logits are HF's image_embeds; without one the head is the identity and the logits are the pooler_output.
+    text_model.*, text_projection, logit_scale and position_ids are ignored."""
+    vc = config.get("vision_config", config)
+    act = vc.get("hidden_act", "quick_gelu")
+    if act not in _HF_ACTIVATIONS:
+        raise ValueError(f"hidden_act {act!r} is not supported (quick_gelu or gelu)")
+    v = {k[len("vision_model."):]: np.asarray(a, np.float32) for k, a in sd.items() if k.startswith("vision_model.")}
+    pw = v["embeddings.patch_embedding.weight"]                          # (D, C, P, P), no bias
+    D = int(pw.shape[0])
+    heads = int(vc.get("num_attention_heads", D // 64))
+    if D % heads or D // heads != 64:
+        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    layers = 1 + max(int(m.group(1)) for k in v for m in [re.match(r"encoder\.layers\.(\d+)\.", k)] if m)
+    out = {
+        "cls_token": v["embeddings.class_embedding"].reshape(1, 1, D),
+        "pos_embed": v["embeddings.position_embedding.weight"].reshape(1, -1, D),
+        "patch_embed.proj.weight": pw,
+        "patch_embed.proj.bias": np.zeros(D, np.float32),
+        "norm_pre.weight": v["pre_layrnorm.weight"],                     # HF's spelling
+        "norm_pre.bias": v["pre_layrnorm.bias"],
+    }
+    hf_name = {"norm1": "layer_norm1", "attn.proj": "self_attn.out_proj", "norm2": "layer_norm2", "mlp.fc1": "mlp.fc1", "mlp.fc2": "mlp.fc2"}
+    for i in range(layers):
+        h, t = f"encoder.layers.{i}.", f"blocks.{i}."
+        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        for dst in ("norm1", "attn.qkv", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"):  # timm's state_dict order
+            for p in ("weight", "bias"):
+                if dst == "attn.qkv":  # rows [q; k; v]
+                    out[f"{t}{dst}.{p}"] = np.concatenate([v[f"{h}self_attn.{x}_proj.{p}"] for x in "qkv"], axis=0)
+                else:
+                    out[f"{t}{dst}.{p}"] = v[f"{h}{hf_name[dst]}.{p}"]
+    out["norm.weight"], out["norm.bias"] = v["post_layernorm.weight"], v["post_layernorm.bias"]
+    proj = sd.get("visual_projection.weight")
+    out["head.weight"] = np.asarray(proj, np.float32) if proj is not None else np.eye(D, dtype=np.float32)
+    out["head.bias"] = np.zeros(out["head.weight"].shape[0], np.float32)
+    return out, heads, _HF_ACTIVATIONS[act], float(vc.get("layer_norm_eps", 1e-5))
+
+
+def clip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
+                       container: str = "gguf") -> None:
+    """A Hugging Face CLIP vision tower -> GGUF model file (pre-norm, the config's activation and eps)."""
+    if container != "gguf":
+        raise ValueError("a CLIP tower needs --container gguf: a legacy ggml file carries the reference's architecture only")
+    tsd, heads, activation, eps = clip_to_timm(sd, config)
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", keep_norm_pre=True, activation=activation, eps=eps)
 
 
 def write_legacy(path: str, vf) -> None:
@@ -202,13 +277,26 @@ def main(argv):
     ap.add_argument("--ftype", type=int, choices=[0, 1], default=1)
     ap.add_argument("--heads", type=int, default=None)
     ap.add_argument("--labels", default=None, help="JSON file {class id: label}")
-    ap.add_argument("--container", choices=["legacy", "gguf"], default="legacy")
+    ap.add_argument("--container", choices=["legacy", "gguf"], default=None,
+                    help="default: legacy for the reference's architecture, gguf for a CLIP tower or the options below")
+    ap.add_argument("--hf-config", default=None, help="config.json of a Hugging Face CLIP checkpoint (required for one)")
+    ap.add_argument("--keep-norm-pre", action="store_true", help="timm: keep norm_pre as the model's pre-norm (GGUF only)")
+    ap.add_argument("--activation", choices=list(gf.ACTIVATIONS), default="gelu_tanh", help="timm: the MLP activation (GGUF only)")
+    ap.add_argument("--eps", type=float, default=1e-6, help="timm: the LayerNorm epsilon (GGUF only)")
     a = ap.parse_args(argv)
     if a.quantize:
         quantize_model_file(a.src, a.dst, a.fmt)
         return
     labels = {int(k): v for k, v in json.load(open(a.labels)).items()} if a.labels else None
-    state_dict_to_model_file(load_state_dict(a.src), a.dst, a.ftype, a.heads, labels, a.container)
+    sd = load_state_dict(a.src)
+    if is_hf_clip(sd):
+        if not a.hf_config:
+            raise SystemExit("a Hugging Face CLIP state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
+        clip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf")
+        return
+    new_arch = a.keep_norm_pre or a.activation != "gelu_tanh" or a.eps != 1e-6
+    state_dict_to_model_file(sd, a.dst, a.ftype, a.heads, labels, a.container or ("gguf" if new_arch else "legacy"),
+                             a.keep_norm_pre, a.activation, a.eps)
 
 
 if __name__ == "__main__":

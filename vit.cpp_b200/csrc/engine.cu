@@ -190,6 +190,8 @@ struct Slot
 struct vitb200_engine
 {
     vitb200_hparams hp;
+    vitb200_arch arch{0, 0}; // pre-norm and MLP activation; {0, 0} is the reference's architecture
+    float *npre_w = nullptr, *npre_b = nullptr; // arch.pre_norm: norm_pre.weight / norm_pre.bias
     int device = 0, max_batch = 0, num_sms = 132;
     int N = 0, NP = 0, G = 0, KP = 0, KPp = 0;
     int Cp = 0;           // num_classes rounded up to a multiple of 4: pitch of the internal logits rows (128-bit epilogue stores)
@@ -587,13 +589,14 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
         if (!p.a_scale) return fail("e4m3 GEMM: no A scales");
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6, GEMM_OP_E4M3>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, GEMM_OP_E4M3>(e, tmA, tmB, p, s);
-        VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16)
+        VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
 #undef VB_CASE
         return fail("no e4m3 GEMM instantiation for epilogue=%d", epi);
     }
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
     VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
+    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
 #undef VB_CASE
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
@@ -696,6 +699,26 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
         return 0;
     }
     return launch_layernorm_rows<OutT, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride, y_scale);
+}
+
+// The pre-norm: the row-per-warp LayerNorm in place on `rows` consecutive f32 rows of x
+int launch_layernorm_inplace(vitb200_engine *e, float *x, const float *w, const float *b, int rows, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size;
+    const int threads = 256, blocks = (rows + threads / 32 - 1) / (threads / 32);
+    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<4>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
+    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<8>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
+    else if (D <= LN_MAX_HIDDEN) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<LN_ROWS_MAX_V>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
+    else return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
+    CUDA_TRY(cudaGetLastError());
+    e->launches++;
+    return 0;
+}
+
+// The fc1 epilogue of the model's MLP activation (vitb200_arch.activation)
+int fc1_epilogue(const vitb200_engine *e)
+{
+    return e->arch.activation == 1 ? EPI_BIAS_GELU_ERF_F16 : e->arch.activation == 2 ? EPI_BIAS_QUICK_GELU_F16 : EPI_BIAS_GELU_F16;
 }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
@@ -836,6 +859,12 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         }
         if (launch_gemm(e, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
+    if (e->arch.pre_norm)
+    {
+        // CLIP's ln_pre (timm norm_pre) on every token row, back into the stream every TMA map points at
+        ProfScope ps(e, PK_LN, 0.0, s);
+        if (launch_layernorm_inplace(e, e->X, e->npre_w, e->npre_b, T, s)) return 1;
+    }
     if (taps && tap_f32(taps->embed, e->X, (size_t)T * D, s)) return 1;
 
     for (int il = 0; il < layers; ++il)
@@ -886,7 +915,7 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
             p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D;
             p.a_scale = e->SA; p.w_scale = L.fc1.w_scale;
             ProfScope ps(e, PK_FC1, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, EPI_BIAS_GELU_F16, e->fp8 ? e->tmA8 : e->tmA_D, L.fc1.tm, p, s, e->fp8)) return 1; // vit.cpp:889-893
+            if (launch_gemm(e, fc1_epilogue(e), e->fp8 ? e->tmA8 : e->tmA_D, L.fc1.tm, p, s, e->fp8)) return 1; // vit.cpp:889-893
         }
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
@@ -1080,8 +1109,8 @@ struct EngineDeleter
 using EnginePtr = std::unique_ptr<vitb200_engine, EngineDeleter>;
 
 // Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
-int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens, bool fp8,
-                vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
+int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
+                bool fp8, vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
 {
     if (!hp || !t || !out) return fail("vitb200_create: null argument");
     *out = nullptr;
@@ -1091,6 +1120,12 @@ int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int d
         hp->patch_size < 1 || hp->patch_size > 64 || hp->img_size < hp->patch_size || hp->img_size > 4096 || n < 1)
         return fail("invalid hyper-parameters (hidden %d, layers %d, heads %d, classes %d, patch %d, img %d)", hp->hidden_size,
                     hp->num_hidden_layers, hp->num_attention_heads, hp->num_classes, hp->patch_size, hp->img_size);
+    const vitb200_arch ar = arch ? *arch : vitb200_arch{0, 0};
+    if (ar.pre_norm != 0 && ar.pre_norm != 1) return fail("vitb200_arch.pre_norm = %d out of range (0 none, 1 LayerNorm 'norm_pre')", ar.pre_norm);
+    if (ar.activation < 0 || ar.activation > 2)
+        return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu)", ar.activation);
+    if (ar.pre_norm && (!find_tensor(t, n, "norm_pre.weight") || !find_tensor(t, n, "norm_pre.bias")))
+        return fail("vitb200_arch.pre_norm = 1 needs the tensors 'norm_pre.weight' and 'norm_pre.bias'");
     // input channels from the patch kernel [P, P, C, D] (vit.cpp:515; C = 1 in vitstr.cpp:482)
     const vitb200_tensor *pw = find_tensor(t, n, "patch_embed.proj.weight");
     const int64_t per_c = (int64_t)hp->hidden_size * hp->patch_size * hp->patch_size;
@@ -1116,6 +1151,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int d
     EnginePtr owner(new vitb200_engine());
     vitb200_engine *e = owner.get();
     e->hp = *hp;
+    e->arch = ar;
     if (e->hp.eps <= 0.f) e->hp.eps = 1e-6f;
     e->device = device;
     e->max_batch = max_batch;
@@ -1136,6 +1172,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int d
     if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls)) return 1;
     if (upload_f32(e, t, n, "pos_embed", D, e->N, 1, 1, &e->pos)) return 1;
     if (upload_linear(e, t, n, "patch_embed.proj.weight", "patch_embed.proj.bias", D, e->KP, e->KPp, &e->patch, P)) return 1;
+    if (ar.pre_norm && (upload_f32(e, t, n, "norm_pre.weight", D, 1, 1, 1, &e->npre_w) || upload_f32(e, t, n, "norm_pre.bias", D, 1, 1, 1, &e->npre_b)))
+        return 1;
     e->layers.resize(hp->num_hidden_layers);
     for (int i = 0; i < hp->num_hidden_layers; ++i)
     {
@@ -1307,19 +1345,34 @@ const char *vitb200_last_error(void) { return g_err.c_str(); }
 
 int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, vitb200_engine **out)
 {
-    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, 1, false, out); });
+    return guarded(__func__, [&] { return create_impl(hp, nullptr, t, n, device, max_batch, 1, false, out); });
 }
 
 int vitb200_create_ex(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
                       vitb200_engine **out)
 {
-    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, head_tokens, false, out); });
+    return guarded(__func__, [&] { return create_impl(hp, nullptr, t, n, device, max_batch, head_tokens, false, out); });
 }
 
 int vitb200_create_fp8(const vitb200_hparams *hp, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
                        vitb200_engine **out)
 {
-    return guarded(__func__, [&] { return create_impl(hp, t, n, device, max_batch, head_tokens, true, out); });
+    return guarded(__func__, [&] { return create_impl(hp, nullptr, t, n, device, max_batch, head_tokens, true, out); });
+}
+
+int vitb200_create_arch(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *t, int n, int device, int max_batch,
+                        int head_tokens, int fp8, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_impl(hp, arch, t, n, device, max_batch, head_tokens, fp8 != 0, out); });
+}
+
+int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out)
+{
+    return guarded(__func__, [&] {
+        if (!e || !out) return fail("null argument");
+        *out = e->arch;
+        return 0;
+    });
 }
 
 void vitb200_destroy(vitb200_engine *e)
@@ -1838,7 +1891,8 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
         EnginePtr owner;
         if (scratch_engine(device, owner)) return 1;
         vitb200_engine *e = owner.get();
-        const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO;
+        const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
+                            epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16;
         const size_t MN = (size_t)M * N;
         __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
         float *dB = nullptr, *o32 = nullptr;
@@ -1883,8 +1937,9 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
     return guarded(__func__, [&]() -> int {
         if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
         if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
-        if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO)
-            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6)", epilogue);
+        if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 &&
+            epilogue != EPI_BIAS_QUICK_GELU_F16)
+            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8)", epilogue);
         EnginePtr owner;
         if (scratch_engine(device, owner)) return 1;
         vitb200_engine *e = owner.get();
@@ -2038,7 +2093,9 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
     hp.num_attention_heads = i32(g.num_attention_heads); hp.num_classes = i32(g.num_classes);
     hp.patch_size = i32(g.patch_size); hp.img_size = i32(g.img_size); hp.ftype = i32(g.ftype); hp.eps = g.eps;
     if (hp.num_hidden_layers < 1 || hp.num_hidden_layers > 4096) return fail("invalid model file '%s' (num_hidden_layers %d)", path, hp.num_hidden_layers);
-    const int expected = 4 + 12 * hp.num_hidden_layers + 4; // vit.cpp:697
+    if (g.pre_norm != 0 && g.pre_norm != 1) return fail("invalid model file '%s' (vit.pre_norm %lld)", path, (long long)g.pre_norm);
+    const vitb200_arch arch{(int32_t)g.pre_norm, g.activation};
+    const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm; // vit.cpp:697, plus norm_pre.weight / .bias
     if ((int)g.tensors.size() != expected) return fail("model file has %d tensors, but %d tensors were expected", (int)g.tensors.size(), expected);
     std::vector<vitb200_tensor> ts(g.tensors.size());
     for (size_t i = 0; i < g.tensors.size(); ++i)
@@ -2049,7 +2106,7 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
         ts[i].n_dims = g.tensors[i].n_dims;
         for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
     }
-    return create_impl(&hp, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out, &g.labels);
+    return create_impl(&hp, &arch, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out, &g.labels);
 }
 
 extern "C" int vitb200_create_from_file(const char *path, int device, int max_batch, vitb200_engine **out)

@@ -60,6 +60,8 @@ enum GemmEpilogue
     EPI_BIAS_F16_HILO = 6,  // x = acc + bias kept to ~22 significant bits as TWO f16 tensors: out = hi = f16(x), out2 = lo = f16(x - hi)
                             // (qkv in front of the split-precision attention: the reference feeds f32 q, k, v to both attention mat-muls,
                             // vit.cpp:848,858; hi + lo lets the f16 tensor cores reproduce that with split-precision MMAs)
+    EPI_BIAS_GELU_ERF_F16 = 7,   // out f16 = f16(gelu_erf(acc + bias)), x in f32 without rounding to f16 first   (fc1 of LAION CLIP)
+    EPI_BIAS_QUICK_GELU_F16 = 8, // out f16 = f16(quick_gelu(acc + bias)), likewise                               (fc1 of OpenAI CLIP)
 };
 
 struct GemmParams
@@ -115,10 +117,23 @@ __device__ __forceinline__ float gelu_tanh_f32(float x)
     return x * ptx::rcp_approx(1.0f + e);
 }
 
+// GELU, erf form: 0.5 x (1 + erf(x / sqrt 2)) = x Phi(x), evaluated as x * normcdff(x).  normcdff is erfc-based, so the left tail keeps
+// its relative accuracy where 1 + erf(x / sqrt 2) would cancel; for x << 0 it underflows to 0 and the result is -0.
+__device__ __forceinline__ float gelu_erf_f32(float x) { return x * normcdff(x); }
+
+// QuickGELU (OpenAI CLIP): x sigma(1.702 x) = x / (1 + e^{-1.702 x}).  For x << 0, e^{-1.702 x} is +inf, its reciprocal 0 and the
+// result -0; never NaN for a finite x.
+__device__ __forceinline__ float quick_gelu_f32(float x)
+{
+    const float e = ptx::ex2_approx(x * -2.4554670f); // -1.702 log2(e)
+    return x * ptx::rcp_approx(1.0f + e);
+}
+
 // Epilogues whose result goes out through shared memory and TMA stores (the rest store from registers)
 __host__ __device__ constexpr bool gemm_epi_staged(int epi)
 {
-    return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32;
+    return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32 ||
+           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16;
 }
 
 // Staged-epilogue geometry: a warpgroup's 128 x 128 result leaves in passes of one 64-row half x kPassCols columns; a pass is
@@ -128,7 +143,8 @@ template <int EPI, int STAGES>
 struct GemmStage
 {
     using Cfg = GemmCfg<STAGES>;
-    static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO);
+    static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_GELU_ERF_F16 ||
+                                  EPI == EPI_BIAS_QUICK_GELU_F16);
     static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
     static constexpr int kBoxCols = kF16 ? 64 : 32;
     static constexpr int kBoxBytes = 64 * 128;
@@ -380,6 +396,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                 const float2 r = __half22float2(__floats2half2_rn(x0, x1)); // ggml.c:1434-1441: y = f16(gelu(f32(f16(x))))
                                 hv = __floats2half2_rn(gelu_tanh_f32(r.x), gelu_tanh_f32(r.y));
                             }
+                            else if constexpr (EPI == EPI_BIAS_GELU_ERF_F16) hv = __floats2half2_rn(gelu_erf_f32(x0), gelu_erf_f32(x1));
+                            else if constexpr (EPI == EPI_BIAS_QUICK_GELU_F16) hv = __floats2half2_rn(quick_gelu_f32(x0), quick_gelu_f32(x1));
                             else hv = __floats2half2_rn(x0, x1);
                             ptx::st_shared_b32(a + St::box(0, jj / 8), *reinterpret_cast<const uint32_t *>(&hv));
                             if constexpr (EPI == EPI_BIAS_F16_HILO)

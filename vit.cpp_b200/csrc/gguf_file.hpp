@@ -7,6 +7,8 @@
 //     general.architecture = "vit"                         general.alignment (default 32)          general.file_type (optional)
 //     vit.hidden_size, vit.num_hidden_layers, vit.num_attention_heads, vit.num_classes, vit.patch_size, vit.image_size  (integers)
 //     vit.layer_norm_eps (float32, default 1e-6)           vit.id2label (array of strings, index = class id; optional)
+//     vit.pre_norm (bool or integer, default 0: 1 = a LayerNorm 'norm_pre' before block 0, as in CLIP towers)
+//     vit.activation (string, default "gelu_tanh"; "gelu_erf" or "quick_gelu": the MLP activation)
 // Layout (gguf.md): header {magic "GGUF", u32 version, u64 n_tensors, u64 n_kv}, n_kv x {string key, u32 type, value},
 // n_tensors x {string name, u32 n_dims, u64 ne[n_dims], u32 type, u64 offset}, padding to the alignment, tensor data (offsets
 // relative to the start of the data section).  Strings are {u64 length, bytes}.
@@ -31,6 +33,8 @@ struct GgufModel
 {
     int64_t hidden_size = 0, num_hidden_layers = 0, num_attention_heads = 0, num_classes = 0, patch_size = 0, img_size = 0, ftype = 1;
     float eps = 1e-6f;
+    int64_t pre_norm = 0; // vit.pre_norm (vitb200_arch.pre_norm; the loader checks the range)
+    int32_t activation = 0; // vit.activation: 0 gelu_tanh, 1 gelu_erf, 2 quick_gelu (vitb200_arch.activation)
     std::map<int, std::string> labels;
     std::vector<GgufTensor> tensors;
     std::string error;
@@ -86,6 +90,13 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             std::string v;
             if (!rd_str(v)) return fail("truncated GGUF string value");
             if (key == "general.architecture") arch = v;
+            else if (key == "vit.activation")
+            {
+                if (v == "gelu_tanh") m.activation = 0;
+                else if (v == "gelu_erf") m.activation = 1;
+                else if (v == "quick_gelu") m.activation = 2;
+                else return fail("unknown vit.activation '" + v + "' (gelu_tanh, gelu_erf or quick_gelu)");
+            }
         }
         else if (vt == 9) // array
         {
@@ -137,6 +148,7 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             else if (key == "vit.patch_size") m.patch_size = iv;
             else if (key == "vit.image_size" || key == "vit.img_size") m.img_size = iv;
             else if (key == "vit.layer_norm_eps") m.eps = (float)fv;
+            else if (key == "vit.pre_norm") m.pre_norm = iv;
         }
     }
     if (!arch.empty() && arch != "vit") return fail("GGUF architecture is '" + arch + "', expected 'vit'");

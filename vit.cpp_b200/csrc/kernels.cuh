@@ -4,6 +4,7 @@
 //   cls_rows_kernel          token 0 = cls_token + pos_embed[0]                      (vit.cpp:794-797)
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
 //                            and un-normalised forms write the encoder features (vitb200_features), its e4m3 form the FP8 A operand
+//   layernorm_inplace_kernel the same arithmetic in place on f32 rows (the pre-norm of CLIP towers)
 //   attention_kernel         per (image, head): S = QK^T / sqrt(hd), softmax with the reference's f16-exp
 //                            semantics (ggml.c:10536-10558), O = P V   (vit.cpp:826-866)
 //   softmax_topk_kernel      final soft-max (vit.cpp:931) + top-k (replaces the host std::sort, vit.cpp:1047-1057)
@@ -147,15 +148,14 @@ __device__ __forceinline__ void store4(OutT *__restrict__ yr, int i, bool live, 
 // NORM = false skips the normalisation: the selected rows of x are converted and stored as they are (w and b are not read).
 // OutT = __nv_fp8_e4m3 (FP8 engine, NORM only) quantises each row of those f32 values with its own scale: amax = max |y| over the row,
 // y_scale[row] = amax / 448 and y = e4m3_rn_satfinite(y (448 / amax)); an all-zero row gets scale 1.
-template <int MAXV, typename OutT = __half, bool NORM = true>
-__global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_stride, int rows_per_group, size_t group_stride,
-                                     const float *__restrict__ w, const float *__restrict__ b, OutT *__restrict__ y, int rows,
-                                     int D, float eps, float *__restrict__ y_scale)
+// The body is a device function so that the in-place form below can run it with y == x: a warp holds its whole row in registers
+// before it writes any of it, and no two warps share a row.
+template <int MAXV, typename OutT, bool NORM>
+__device__ __forceinline__ void layernorm_row_warp(const float *x, size_t x_row_stride, int rows_per_group, size_t group_stride, const float *w,
+                                                   const float *b, OutT *y, int rows, int D, float eps, float *y_scale)
 {
     constexpr bool kE4M3 = std::is_same<OutT, __nv_fp8_e4m3>::value;
     static_assert(!kE4M3 || NORM, "e4m3 output: normalised rows only");
-    ptx::grid_dep_launch(); // PDL: blocks may be resident before the producing GEMM has drained
-    ptx::grid_dep_wait();
     const int warps_per_block = blockDim.x >> 5;
     // rows are taken LAST FIRST: the producing GEMM wrote them in ascending order, so the tail of X is what the 50 MB L2 still
     // holds when this kernel starts (and the GEMM that follows, walking up from row 0, meets this kernel's freshest output)
@@ -248,6 +248,26 @@ __global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_s
                     ptx::cvt_e4m3x4(__fmul_rn(v[j].x, inv), __fmul_rn(v[j].y, inv), __fmul_rn(v[j].z, inv), __fmul_rn(v[j].w, inv));
         }
     }
+}
+
+template <int MAXV, typename OutT = __half, bool NORM = true>
+__global__ void layernorm_f16_kernel(const float *__restrict__ x, size_t x_row_stride, int rows_per_group, size_t group_stride,
+                                     const float *__restrict__ w, const float *__restrict__ b, OutT *__restrict__ y, int rows,
+                                     int D, float eps, float *__restrict__ y_scale)
+{
+    ptx::grid_dep_launch(); // PDL: blocks may be resident before the producing GEMM has drained
+    ptx::grid_dep_wait();
+    layernorm_row_warp<MAXV, OutT, NORM>(x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, eps, y_scale);
+}
+
+// The same LayerNorm in place on `rows` consecutive f32 rows of x (the pre-norm of CLIP towers, on the residual stream before block 0):
+// f32 in, f32 out, no rounding to f16
+template <int MAXV>
+__global__ void layernorm_inplace_kernel(float *x, const float *__restrict__ w, const float *__restrict__ b, int rows, int D, float eps)
+{
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
+    layernorm_row_warp<MAXV, float, true>(x, (size_t)D, rows, 0, w, b, x, rows, D, eps, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -16,6 +16,8 @@ from typing import Optional
 
 import numpy as np
 
+from .ggml_file import ACTIVATIONS  # vitb200_arch.activation -> name (the GGUF key vit.activation)
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
 HEADER_PATH = os.path.join(os.path.dirname(_HERE), "include", "vitb200.h")
@@ -29,6 +31,11 @@ class VitB200Error(RuntimeError):
 class Hparams(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("hidden_size", "num_hidden_layers", "num_attention_heads", "num_classes",
                                           "patch_size", "img_size", "ftype")] + [("eps", C.c_float)]
+
+
+class Arch(C.Structure):
+    """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ACTIVATIONS."""
+    _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32)]
 
 
 class Taps(C.Structure):
@@ -71,6 +78,8 @@ def lib():
         L.vitb200_create_fp8.argtypes = [vp, vp, i32, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_create_from_file_fp8.argtypes = [C.c_char_p, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_fp8.argtypes = [vp]
+        L.vitb200_create_arch.argtypes = [vp, C.POINTER(Arch), vp, i32, i32, i32, i32, i32, C.POINTER(vp)]
+        L.vitb200_get_arch.argtypes = [vp, C.POINTER(Arch)]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
         L.vitb200_test_gemm_fp8.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
         L.vitb200_test_layernorm_fp8.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
@@ -127,6 +136,10 @@ class VitModel:
         self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713)
         self.head_tokens = lib().vitb200_head_tokens(self._h)  # classifier rows per image (1, or 25 for ViTSTR)
         self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
+        a = Arch()
+        _check(lib().vitb200_get_arch(self._h, C.byref(a)), "vitb200_get_arch")
+        # the architecture (vitb200_arch): {"pre_norm": bool, "activation": one of ACTIVATIONS}; the reference's is (False, "gelu_tanh")
+        self.arch = {"pre_norm": bool(a.pre_norm), "activation": ACTIVATIONS[a.activation]}
         self._labels = None
 
     def label(self, i: int) -> Optional[str]:
@@ -169,9 +182,10 @@ def vit_model_load(fname: str, device: int = 0, max_batch: int = 256, head_token
 
 
 def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens: int = 1, edit=None, fp8: bool = False) -> VitModel:
-    """vitb200_create_ex with a caller-built tensor list -- what the vit.h-side shim does with vit_model::tensors.  `vf` is a parsed
-    model file (ggml_file.VitFile: numpy-shaped f32 / f16 arrays); `edit(entries)` may reorder / duplicate / reshape the list of
-    [name, array, ggml_type, ne] entries first (tests of the loader's shape and name checks).  fp8 = True: vitb200_create_fp8."""
+    """vitb200_create_arch with a caller-built tensor list -- what the vit.h-side shim does with vit_model::tensors.  `vf` is a parsed
+    model file (ggml_file.VitFile: numpy-shaped f32 / f16 arrays, its eps, pre_norm and activation); `edit(entries)` may reorder /
+    duplicate / reshape the list of [name, array, ggml_type, ne] entries first (tests of the loader's shape and name checks).
+    fp8 = True: the FP8 engine (vitb200_create_fp8).  A reference-architecture file gives what vitb200_create_ex gives."""
     entries = []
     for name, arr in vf.tensors.items():
         if name.endswith(".q8_0_raw"):
@@ -193,10 +207,12 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
         t.name, t.data, t.type, t.n_dims = nm, a.ctypes.data, ft, len(ne)
         for i in range(4):
             t.ne[i] = ne[i] if i < len(ne) else 1
-    hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, 1e-6)
+    hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, vf.eps)
+    act = ACTIVATIONS.index(vf.activation) if vf.activation in ACTIVATIONS else -1  # an unknown name is refused by the engine
+    arch = Arch(int(vf.pre_norm), act)
     h = C.c_void_p()
-    create = lib().vitb200_create_fp8 if fp8 else lib().vitb200_create_ex
-    _check(create(C.byref(hp), ts, len(entries), device, max_batch, head_tokens, C.byref(h)), "vitb200_create")
+    _check(lib().vitb200_create_arch(C.byref(hp), C.byref(arch), ts, len(entries), device, max_batch, head_tokens, int(fp8), C.byref(h)),
+           "vitb200_create")
     return VitModel(h, device, max_batch)
 
 

@@ -25,6 +25,8 @@ import numpy as np
 
 GGML_FILE_MAGIC = 0x67676D6C
 QK8_0 = 32  # ggml-quants.h:42-46 block_q8_0 { f16 d; int8 qs[32]; }
+# MLP activations, in the order of vitb200_arch.activation: the reference's tanh GELU (ggml's f16 table), erf GELU, QuickGELU
+ACTIVATIONS = ("gelu_tanh", "gelu_erf", "quick_gelu")
 
 CONFIGS = {
     # name: (hidden, layers, heads, patch, img)
@@ -68,6 +70,11 @@ class VitFile:
     id2label: Dict[int, str] = field(default_factory=dict)
     tensors: Dict[str, np.ndarray] = field(default_factory=dict)  # numpy-shaped (timm order)
     tensor_ftype: Dict[str, int] = field(default_factory=dict)
+    # architecture (vitb200_arch in include/vitb200.h; GGUF keys vit.layer_norm_eps, vit.pre_norm, vit.activation): the defaults are the
+    # reference's, the only values a legacy-ggml file can carry
+    eps: float = 1e-6
+    pre_norm: int = 0            # 1: LayerNorm 'norm_pre.*' on the embeddings before block 0 (CLIP towers)
+    activation: str = "gelu_tanh"  # MLP activation: one of ACTIVATIONS
 
     @property
     def n_tokens(self) -> int:
@@ -313,7 +320,14 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
                  ("vit.num_attention_heads", vf.num_attention_heads), ("vit.num_classes", vf.num_classes),
                  ("vit.patch_size", vf.patch_size), ("vit.image_size", vf.img_size)):
         kv_u32(k, v)
-    kv.append(gstr(b"vit.layer_norm_eps") + struct.pack("<If", _GGUF_F32, 1e-6))
+    kv.append(gstr(b"vit.layer_norm_eps") + struct.pack("<If", _GGUF_F32, vf.eps))
+    # the architecture keys only when they differ from the reference's values, so that a reference-architecture file is unchanged
+    if vf.pre_norm:
+        kv_u32("vit.pre_norm", int(vf.pre_norm))
+    if vf.activation != "gelu_tanh":
+        if vf.activation not in ACTIVATIONS:
+            raise ValueError(f"write_gguf: unknown activation {vf.activation!r} ({', '.join(ACTIVATIONS)})")
+        kv.append(gstr(b"vit.activation") + struct.pack("<I", _GGUF_STR) + gstr(vf.activation.encode()))
     if vf.id2label:
         labels = [vf.id2label.get(i, "").encode() for i in range(max(vf.id2label) + 1)]
         kv.append(gstr(b"vit.id2label") + struct.pack("<IIQ", _GGUF_ARR, _GGUF_STR, len(labels)) + b"".join(gstr(x) for x in labels))
@@ -385,6 +399,9 @@ def read_gguf(path: str) -> VitFile:
     vf = VitFile(kv["vit.hidden_size"], kv["vit.num_hidden_layers"], kv["vit.num_attention_heads"], kv["vit.num_classes"],
                  kv["vit.patch_size"], kv.get("vit.image_size", kv.get("vit.img_size")), kv.get("general.file_type", 1))
     vf.id2label = dict(enumerate(kv.get("vit.id2label", [])))
+    vf.eps = kv.get("vit.layer_norm_eps", 1e-6)
+    vf.pre_norm = int(kv.get("vit.pre_norm", 0))
+    vf.activation = kv.get("vit.activation", "gelu_tanh")
     align = kv.get("general.alignment", 32)
     infos = []
     for _ in range(n_tensors):
