@@ -220,7 +220,9 @@ int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch,
 int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                         const vitb200_features_req *req, void *tokens, void *prelogits);
 
-/* Number of kernels this library launched during the most recent forward or features call. */
+/* Number of kernels launched by the most recent call on this engine that enqueued work: a forward, features or recognition call,
+ * including one that only pre-processes images (vitb200_forward_u8 without outputs: 1).  A call rejected by its argument checks
+ * leaves the count as it was. */
 int vitb200_last_launch_count(const vitb200_engine *e);
 
 /* Per-kernel device timing for roofline reporting: while enabled, CUDA-event pairs are recorded around every

@@ -300,6 +300,40 @@ def test_forward_launch_count():
         assert launches == 3 + 7 * L + 3
 
 
+def test_launch_count_is_the_last_call_that_enqueued_work():
+    """Every entry point reports its own kernels: the u8 preprocess alone is 1 launch, whatever ran before it; the u8 paths count the
+    preprocess kernel in place of patchify, through eager, captured and replayed schedules; a rejected call leaves the count alone."""
+    m = eng.vit_model_load(model_path("micro", "f16"), 0, 4)
+    L = m.hparams.num_hidden_layers
+    forward = 3 + 7 * L + 3
+    imgs = gf.synthetic_images(3, m.img_size, seed=12)
+    rng = np.random.default_rng(5)
+    u8 = [rng.integers(0, 256, size=s + (3,), dtype=np.uint8) for s in ((300, 280), (224, 224), (97, 131))]
+    eng.vit_predict(m, imgs, 5)
+    assert m.last_launch_count() == forward
+    eng.vit_image_preprocess_predict(m, u8, predict=False)
+    assert m.last_launch_count() == 1
+    for rep in range(6):  # two pipeline slots, each run eagerly, captured and replayed
+        eng.vit_image_preprocess_predict(m, u8)
+        assert m.last_launch_count() == forward, rep
+    for layers in (0, L):
+        eng.vit_features(m, imgs, layers, prelogits=True)
+        want = m.last_launch_count()
+        for rep in range(6):
+            eng.vit_features_u8(m, u8, layers=layers, prelogits=True)
+            assert m.last_launch_count() == want, (layers, rep)
+    # rejected before anything is enqueued: batch > max_batch, an empty image
+    eng.vit_image_preprocess_predict(m, u8, predict=False)
+    with pytest.raises(eng.VitB200Error):
+        eng.vit_predict(m, gf.synthetic_images(5, m.img_size, seed=1), 5)
+    with pytest.raises(eng.VitB200Error):
+        eng.vit_features(m, gf.synthetic_images(5, m.img_size, seed=1))
+    with pytest.raises(eng.VitB200Error):
+        eng.vit_image_preprocess_predict(m, [u8[0], np.zeros((0, 8, 3), np.uint8)])
+    assert m.last_launch_count() == 1
+    m.close()
+
+
 def test_error_paths():
     m = eng.vit_model_load(model_path("micro", "f16"), 0, 2)
     imgs = gf.synthetic_images(3, m.img_size, seed=1)

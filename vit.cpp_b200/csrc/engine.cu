@@ -83,62 +83,24 @@ PFN_tmapEncodeTiled tmap_encoder()
     return fn;
 }
 
-// 2-D f16 row-major tensor [rows][cols] with row pitch `pitch` elements, box = 64 columns x box_rows rows,
-// SWIZZLE_128B (matches the wgmma K-major SWIZZLE_128B smem descriptor), out-of-bounds elements read as zero.
-// 3-D f16 view of a HEAD-MAJOR q / k / v buffer [planes][plane_rows][64] (planes = 3 x heads: q heads, then k heads, then v heads):
-// dims {64, rows, planes}, box = 64 columns x box_rows rows x 1 plane, SWIZZLE_128B (the attention's operand tiles)
-int make_tmap_heads3d(CUtensorMap *m, const void *ptr, uint64_t planes, uint64_t rows, uint64_t plane_rows, uint32_t box_rows)
+// A 2-D or 3-D tensor map over ptr: dims and box in elements, innermost first; strides in bytes, of dimensions 1 .. rank-1.  Dense
+// elements, L2 promotion of 256 B, out-of-bounds elements read as zero.  The GEMM operands and the attention's q / k / v tiles use
+// SWIZZLE_128B with a box one 128-byte row wide: the layout the wgmma K-major SWIZZLE_128B shared-memory descriptor reads.
+template <int R>
+int make_tmap(CUtensorMap *m, CUtensorMapDataType dt, const void *ptr, const cuuint64_t (&dims)[R], const cuuint64_t (&strides)[R - 1],
+              const cuuint32_t (&box)[R], CUtensorMapSwizzle sw = CU_TENSOR_MAP_SWIZZLE_128B)
 {
+    static_assert(R == 2 || R == 3, "2-D and 3-D maps only");
     PFN_tmapEncodeTiled enc = tmap_encoder();
     if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t dims[3] = {64, rows, planes};
-    cuuint64_t strides[2] = {128, plane_rows * 128};
-    cuuint32_t box[3] = {64, box_rows, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void *>(ptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(heads3d) failed (%d)", (int)r);
+    const cuuint32_t estr[3] = {1, 1, 1};
+    const CUresult r = enc(m, dt, R, const_cast<void *>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+        return fail("cuTensorMapEncodeTiled failed (%d): dims {%llu, %llu, %llu}, row stride %llu B, box {%u, %u, %u}", (int)r,
+                    (unsigned long long)dims[0], (unsigned long long)dims[1], R > 2 ? (unsigned long long)dims[R - 1] : 1ull,
+                    (unsigned long long)strides[0], box[0], box[1], R > 2 ? box[R - 1] : 1u);
     return 0;
-}
-
-int make_tmap(CUtensorMap *m, const void *ptr, uint64_t rows, uint64_t cols, uint64_t pitch, uint32_t box_rows)
-{
-    PFN_tmapEncodeTiled enc = tmap_encoder();
-    if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {pitch * 2};
-    cuuint32_t box[2] = {64, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void *>(ptr), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled failed (%d) rows=%llu cols=%llu pitch=%llu box_rows=%u", (int)r,
-                                       (unsigned long long)rows, (unsigned long long)cols, (unsigned long long)pitch, box_rows);
-    return 0;
-}
-
-// generic 2-D row-major tensor map (the q8_0 prototype's int8 planes and f32 scale planes)
-int make_tmap_2d(CUtensorMap *m, CUtensorMapDataType dt, size_t elem_bytes, const void *ptr, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
-                 uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle sw)
-{
-    PFN_tmapEncodeTiled enc = tmap_encoder();
-    if (!enc) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {pitch_elems * elem_bytes};
-    cuuint32_t box[2] = {box_cols, box_rows};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(m, dt, 2, const_cast<void *>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
-                     CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled(2d) failed (%d) rows=%llu cols=%llu", (int)r, (unsigned long long)rows, (unsigned long long)cols);
-    return 0;
-}
-
-// e4m3 row-major tensor [rows][cols] (pitch = cols bytes, a multiple of 16): box = 128 columns (one 128-B swizzled row, an e4m3
-// k-block) x box_rows rows, SWIZZLE_128B, out-of-bounds elements read as zero
-int make_tmap_e4m3(CUtensorMap *m, const void *ptr, uint64_t rows, uint64_t cols, uint32_t box_rows)
-{
-    return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, ptr, rows, cols, cols, 2 * GEMM_BK, box_rows, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 struct Linear
@@ -450,8 +412,9 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     }
     // conv bias is declared [1, 1, D] (vit.cpp:516), every other bias [n_out]; the tail up to a multiple of 4 stays zero
     if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
-    if (e4m3) return make_tmap_e4m3(&L->tm, L->w8, (uint64_t)n_out, (uint64_t)ld, (uint32_t)GEMM_BN);
-    return make_tmap(&L->tm, L->w, (uint64_t)n_out, (uint64_t)ld, (uint64_t)ld, (uint32_t)GEMM_BN);
+    const cuuint64_t cols = (cuuint64_t)ld, rows = (cuuint64_t)n_out;
+    if (e4m3) return make_tmap(&L->tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, L->w8, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_BN});
+    return make_tmap(&L->tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, L->w, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_BN});
 }
 
 // the largest dynamic shared memory one CTA may opt in to on sm_90 (227 KB)
@@ -485,21 +448,31 @@ struct ProfScope
     }
 };
 
-// Programmatic dependent launch for the per-layer kernels (GEMMs, attention, LayerNorm): each of them ends its prologue with
-// griddepcontrol.launch_dependents + griddepcontrol.wait (ptx.cuh), so kernel k+1's barrier init / descriptor
-// prefetch runs on the SMs kernel k has already left.
-template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args &&...args)
+// Launch attributes of `launch`, or-ed together: programmatic dependent launch, and clusters of two CTAs
+enum : unsigned { LAUNCH_PLAIN = 0, LAUNCH_PDL = 1, LAUNCH_CLUSTER2 = 2 };
+
+struct LaunchConfig
 {
     cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
+    cudaLaunchAttribute attr[2];
+    LaunchConfig(dim3 grid, dim3 block, size_t smem, cudaStream_t s, unsigned attrs)
+    {
+        cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = s; cfg.attrs = attr;
+        if (attrs & LAUNCH_CLUSTER2)
+        {
+            cudaLaunchAttribute &a = attr[cfg.numAttrs++];
+            a.id = cudaLaunchAttributeClusterDimension;
+            a.val.clusterDim.x = 2; a.val.clusterDim.y = 1; a.val.clusterDim.z = 1;
+        }
+        if (attrs & LAUNCH_PDL)
+        {
+            cudaLaunchAttribute &a = attr[cfg.numAttrs++];
+            a.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+            a.val.programmaticStreamSerializationAllowed = 1;
+        }
+    }
+    LaunchConfig(const LaunchConfig &) = delete; // cfg.attrs points into this object
+};
 
 // Opts `kern` in to `bytes` of dynamic shared memory on the current device, and raises that limit when a later launch needs more.
 // The attribute belongs to the process and device, not to an engine, so one table serves every engine on every host thread.  It is
@@ -528,23 +501,38 @@ int smem_optin(const void *kern, int bytes, const cudaLaunchConfig_t *cluster_cf
     return 0;
 }
 
+// Every kernel of the engine and of the test hooks is launched here: with the attributes `attrs` selects, opted in through smem_optin
+// when it needs more than the default 48 KB of dynamic shared memory, checked, and counted in e->launches.
+// LAUNCH_PDL lets the kernel start while the kernel before it on the stream is still running.  Only a kernel that calls
+// griddepcontrol.wait (ptx.cuh) before it touches memory its predecessor writes is correct under it: the GEMM, the attention kernels
+// and the LayerNorms, whose barrier init and descriptor prefetch then run on the SMs the previous kernel has already left.
+template <typename... KArgs, typename... Args>
+int launch(vitb200_engine *e, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, unsigned attrs, Args &&...args)
+{
+    if (smem > 48 * 1024 && smem_optin((const void *)kern, (int)smem)) return 1;
+    LaunchConfig c(grid, block, smem, s, attrs);
+    const cudaError_t err = cudaLaunchKernelEx(&c.cfg, kern, std::forward<Args>(args)...);
+    if (err != cudaSuccess)
+    {
+        (void)cudaGetLastError();
+        return fail("kernel launch (grid %u x %u, block %u, %zu B shared memory) failed: %s", grid.x, grid.y, block.x, smem, cudaGetErrorString(err));
+    }
+    e->launches++;
+    return 0;
+}
+
 template <int EPI, int STAGES, int OP = GEMM_OP_F16>
 int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
 {
     using Cfg = GemmCfg<STAGES>;
     auto kern = gemm_wgmma_kernel<EPI, STAGES, OP>;
-    // clusters of two CTAs that share the A tile (multicast), with programmatic dependent launch as in launch_pdl
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2); cfg.blockDim = dim3((unsigned)Cfg::kThreads); cfg.dynamicSmemBytes = Cfg::SMEM_BYTES; cfg.stream = s;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 2;
+    // clusters of two CTAs that share the A tile (multicast)
+    constexpr unsigned attrs = LAUNCH_CLUSTER2 | LAUNCH_PDL;
     int max_clusters = 0;
-    if (smem_optin((const void *)kern, Cfg::SMEM_BYTES, &cfg, &max_clusters)) return 1;
+    {
+        const LaunchConfig c(dim3(2), dim3((unsigned)Cfg::kThreads), Cfg::SMEM_BYTES, s, attrs);
+        if (smem_optin((const void *)kern, Cfg::SMEM_BYTES, &c.cfg, &max_clusters)) return 1;
+    }
     if (max_clusters < 1)
     {
         int dev = 0;
@@ -557,14 +545,16 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     if constexpr (gemm_epi_staged(EPI))
     {
         using St = GemmStage<EPI, STAGES>;
+        const cuuint64_t M = (cuuint64_t)p.M, N = (cuuint64_t)p.N, ldo = (cuuint64_t)p.ldo;
         auto out_map = [&](CUtensorMap *m, const void *ptr) -> int {
-            if (!St::kF16) return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, (uint64_t)p.M, (uint64_t)p.N, (uint64_t)p.ldo, 32, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+            if (!St::kF16) return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, ptr, {N, M}, {4 * ldo}, {32, 64});
             if (p.headmajor)
             {
+                // [N / 64 head planes][plane_rows][64], as the attention reads it
                 if (p.N % 64 != 0) return fail("GEMM: head-major output needs N %% 64 == 0 (N = %d)", p.N);
-                return make_tmap_heads3d(m, ptr, (uint64_t)(p.N / 64), (uint64_t)p.M, (uint64_t)p.plane_rows, 64);
+                return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {64, M, N / 64}, {128, 128 * (cuuint64_t)p.plane_rows}, {64, 64, 1});
             }
-            return make_tmap_2d(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, (uint64_t)p.M, (uint64_t)p.N, (uint64_t)p.ldo, 64, 64, CU_TENSOR_MAP_SWIZZLE_128B);
+            return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {N, M}, {2 * ldo}, {64, 64});
         };
         if (out_map(&tmO, p.out)) return 1;
         if (EPI == EPI_BIAS_F16_HILO && out_map(&tmX, p.out2)) return 1;
@@ -572,13 +562,11 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     }
     // persistent: as many clusters as fit at once, each walking the pairs of column tiles cluster, cluster + clusters, ...
     const int pairs = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN));
-    cfg.gridDim = dim3(2u * (unsigned)std::min(pairs, max_clusters));
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, tmA, tmB, tmO, tmX, p));
-    e->launches++;
-    return 0;
+    return launch(e, kern, dim3(2u * (unsigned)std::min(pairs, max_clusters)), dim3((unsigned)Cfg::kThreads), Cfg::SMEM_BYTES, s, attrs, tmA, tmB,
+                  tmO, tmX, p);
 }
 
-// tmB: the weight map, box = one k-block x GEMM_BN rows.  e4m3: A and W are e4m3 maps (make_tmap_e4m3), p.a_scale / p.w_scale their
+// tmB: the weight map, box = one k-block x GEMM_BN rows.  e4m3: A and W are e4m3 maps, p.a_scale / p.w_scale their
 // scales; the f16-output epilogues only (qkv and fc1 of the FP8 engine)
 int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s, bool e4m3 = false)
 {
@@ -601,42 +589,35 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
 
-// The patch sizes launch_patchify has a kernel for, by channel count (vitb200_create rejects any other)
-inline bool patchify_supports(int P, int C) { return C == 1 ? (P == 8 || P == 16) : (P == 8 || P == 14 || P == 16 || P == 32); }
+// The patchify kernel for patch size P and C input channels, NULL for a size it has none for (vitb200_create rejects those)
+using PatchifyKernel = void (*)(const float *, __half *, int, int, int, int);
+PatchifyKernel patchify_kernel(int P, int C)
+{
+    if (C == 1) return P == 8 ? patchify_f16_kernel<8, 1> : P == 16 ? patchify_f16_kernel<16, 1> : nullptr;
+    switch (P)
+    {
+    case 8: return patchify_f16_kernel<8>;
+    case 14: return patchify_f16_kernel<14>;
+    case 16: return patchify16_warp_kernel;
+    case 32: return patchify_f16_kernel<32>;
+    }
+    return nullptr;
+}
+inline bool patchify_supports(int P, int C) { return patchify_kernel(P, C) != nullptr; }
 inline const char *patchify_sizes(int C) { return C == 1 ? "8, 16" : "8, 14, 16, 32"; }
 
 int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaStream_t s)
 {
-    const long long total = (long long)B * e->G * e->hp.patch_size * e->G;
-    const int threads = 256;
-    const int blocks = (int)((total + threads - 1) / threads);
-    if (!patchify_supports(e->hp.patch_size, e->C))
-        return fail("%d-channel input: patch size %d not supported (%s)", e->C, e->hp.patch_size, patchify_sizes(e->C));
-    if (e->C == 1)
-    {
-        if (e->hp.patch_size == 16) patchify_f16_kernel<16, 1><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp);
-        else patchify_f16_kernel<8, 1><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp);
-        CUDA_TRY(cudaGetLastError());
-        e->launches++;
-        return 0;
-    }
-    switch (e->hp.patch_size)
-    {
-    case 16:
+    const PatchifyKernel kern = patchify_kernel(e->hp.patch_size, e->C);
+    if (!kern) return fail("%d-channel input: patch size %d not supported (%s)", e->C, e->hp.patch_size, patchify_sizes(e->C));
+    if (kern == patchify16_warp_kernel)
     {
         const int n_patches = B * e->G * e->G; // one warp per patch, grid-stride over a few waves
-        const int wblocks = std::min((n_patches + 7) / 8, e->num_sms * 16);
-        patchify16_warp_kernel<<<wblocks, 256, 0, s>>>(img, A, n_patches, e->hp.img_size, e->G, e->KPp);
-        break;
+        return launch(e, kern, dim3(std::min((n_patches + 7) / 8, e->num_sms * 16)), dim3(256), 0, s, LAUNCH_PLAIN, img, A, n_patches,
+                      e->hp.img_size, e->G, e->KPp);
     }
-    case 14: patchify_f16_kernel<14><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
-    case 8: patchify_f16_kernel<8><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
-    case 32: patchify_f16_kernel<32><<<blocks, threads, 0, s>>>(img, A, B, e->hp.img_size, e->G, e->KPp); break;
-    default: return fail("patch size %d not supported (%s)", e->hp.patch_size, patchify_sizes(e->C));
-    }
-    CUDA_TRY(cudaGetLastError());
-    e->launches++;
-    return 0;
+    const long long total = (long long)B * e->G * e->hp.patch_size * e->G;
+    return launch(e, kern, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s, LAUNCH_PLAIN, img, A, B, e->hp.img_size, e->G, e->KPp);
 }
 
 // The row-per-warp kernel: the LayerNorms the bulk-copy kernel below does not take (pooled rows, hidden sizes that are not a multiple
@@ -651,16 +632,14 @@ int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride
                           cudaStream_t s, int rows_per_group, size_t group_stride, float *y_scale = nullptr)
 {
     const int D = e->hp.hidden_size;
+    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     if (rows_per_group <= 0) rows_per_group = rows > 0 ? rows : 1; // one group: plain consecutive rows
     const int threads = 256, rows_per_block = threads / 32;
     const int blocks = (rows + rows_per_block - 1) / rows_per_block;
-    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<4, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
-    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_f16_kernel<8, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
-    else if (D <= LN_MAX_HIDDEN) CUDA_TRY(launch_pdl(layernorm_f16_kernel<LN_ROWS_MAX_V, OutT, NORM>, dim3(blocks), dim3(threads), 0, s, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D, e->hp.eps, y_scale));
-    else return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
-    CUDA_TRY(cudaGetLastError());
-    e->launches++;
-    return 0;
+    const auto kern = D <= 4 * 128 ? layernorm_f16_kernel<4, OutT, NORM>
+                    : D <= 8 * 128 ? layernorm_f16_kernel<8, OutT, NORM> : layernorm_f16_kernel<LN_ROWS_MAX_V, OutT, NORM>;
+    return launch(e, kern, dim3(blocks), dim3(threads), 0, s, LAUNCH_PDL, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D,
+                  e->hp.eps, y_scale);
 }
 
 // OutT = __half: the f16 A operand; __nv_fp8_e4m3: the FP8 engine's e4m3 A operand and its row scales y_scale
@@ -676,27 +655,11 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
         const int smem = layernorm_tma_smem_bytes(D);
         const int nblk = (rows + LN_TMA_ROWS - 1) / LN_TMA_ROWS;
         const int grid = std::min(nblk, 2 * e->num_sms);
-        auto launch = [&](auto kern) -> int {
-            if (smem_optin((const void *)kern, smem)) return 1;
-            CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, x, w, b, y, rows, e->hp.eps, y_scale));
-            return 0;
-        };
-        int rc = 1;
-        switch (D / 128)
-        {
-        case 1: rc = launch(layernorm_tma_kernel<1, OutT>); break;
-        case 2: rc = launch(layernorm_tma_kernel<2, OutT>); break;
-        case 3: rc = launch(layernorm_tma_kernel<3, OutT>); break;
-        case 4: rc = launch(layernorm_tma_kernel<4, OutT>); break;
-        case 5: rc = launch(layernorm_tma_kernel<5, OutT>); break;
-        case 6: rc = launch(layernorm_tma_kernel<6, OutT>); break;
-        case 7: rc = launch(layernorm_tma_kernel<7, OutT>); break;
-        case 8: rc = launch(layernorm_tma_kernel<8, OutT>); break;
-        }
-        if (rc) return 1;
-        CUDA_TRY(cudaGetLastError());
-        e->launches++;
-        return 0;
+        // by float4 per lane, D / 128 (at most 7 here: two CTAs per SM hold rows of up to 896 floats)
+        using Kern = decltype(&layernorm_tma_kernel<1, OutT>);
+        const Kern kernels[8] = {layernorm_tma_kernel<1, OutT>, layernorm_tma_kernel<2, OutT>, layernorm_tma_kernel<3, OutT>, layernorm_tma_kernel<4, OutT>,
+                                 layernorm_tma_kernel<5, OutT>, layernorm_tma_kernel<6, OutT>, layernorm_tma_kernel<7, OutT>, layernorm_tma_kernel<8, OutT>};
+        return launch(e, kernels[D / 128 - 1], dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, LAUNCH_PDL, x, w, b, y, rows, e->hp.eps, y_scale);
     }
     return launch_layernorm_rows<OutT, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride, y_scale);
 }
@@ -705,14 +668,10 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
 int launch_layernorm_inplace(vitb200_engine *e, float *x, const float *w, const float *b, int rows, cudaStream_t s)
 {
     const int D = e->hp.hidden_size;
+    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     const int threads = 256, blocks = (rows + threads / 32 - 1) / (threads / 32);
-    if (D <= 4 * 128) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<4>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
-    else if (D <= 8 * 128) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<8>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
-    else if (D <= LN_MAX_HIDDEN) CUDA_TRY(launch_pdl(layernorm_inplace_kernel<LN_ROWS_MAX_V>, dim3(blocks), dim3(threads), 0, s, x, w, b, rows, D, e->hp.eps));
-    else return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
-    CUDA_TRY(cudaGetLastError());
-    e->launches++;
-    return 0;
+    const auto kern = D <= 4 * 128 ? layernorm_inplace_kernel<4> : D <= 8 * 128 ? layernorm_inplace_kernel<8> : layernorm_inplace_kernel<LN_ROWS_MAX_V>;
+    return launch(e, kern, dim3(blocks), dim3(threads), 0, s, LAUNCH_PDL, x, w, b, rows, D, e->hp.eps);
 }
 
 // The fc1 epilogue of the model's MLP activation (vitb200_arch.activation)
@@ -730,23 +689,21 @@ constexpr int ATT_MAX_KEYS_16 = 640;
 // q / k / v tensor maps (hi and lo halves) of the wgmma attention over `rows` token rows per plane
 int make_attention_maps(vitb200_engine *e, uint64_t rows)
 {
-    const uint64_t planes = 3 * (uint64_t)e->hp.num_attention_heads;
-    if (make_tmap_heads3d(&e->tmQ, e->QKV16, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKV, e->QKV16, planes, rows, rows, ATTW_KEYS) ||
-        make_tmap_heads3d(&e->tmQl, e->QKV16L, planes, rows, rows, 64) || make_tmap_heads3d(&e->tmKVl, e->QKV16L, planes, rows, rows, ATTW_KEYS))
+    // the head-major buffer [3 H planes][rows][64]; a box is 64 query rows or ATTW_KEYS key rows of one plane
+    const cuuint64_t planes = 3 * (cuuint64_t)e->hp.num_attention_heads;
+    auto map = [&](CUtensorMap *m, const __half *ptr, cuuint32_t box_rows) {
+        return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {64, rows, planes}, {128, 128 * rows}, {64, box_rows, 1});
+    };
+    if (map(&e->tmQ, e->QKV16, 64) || map(&e->tmKV, e->QKV16, ATTW_KEYS) || map(&e->tmQl, e->QKV16L, 64) || map(&e->tmKVl, e->QKV16L, ATTW_KEYS))
         return 1;
     return 0;
 }
 
 int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
 {
-    const int smem = attention_wgmma_smem_bytes();
-    auto kern = attention_wgmma_kernel;
-    if (smem_optin((const void *)kern, smem)) return 1;
     const int H = e->hp.num_attention_heads;
-    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)smem, s, e->tmQ, e->tmKV, e->tmQl, e->tmKVl,
-                        e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H))));
-    e->launches++;
-    return 0;
+    return launch(e, attention_wgmma_kernel, dim3(B * H), dim3(ATTW_THREADS), (size_t)attention_wgmma_smem_bytes(), s, LAUNCH_PDL, e->tmQ, e->tmKV,
+                  e->tmQl, e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
 }
 
 // The mma.sync kernels hold K and V of one (image, head) problem in shared memory: N tokens padded to whole key chunks, 64 f16 each.
@@ -762,12 +719,8 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
     const int Npad = (N + ATT_KC - 1) / ATT_KC * ATT_KC;
     const int smem = attention_smem_bytes(N);
     if (smem > kSmemOptinMax) return fail("attention: %d tokens do not fit in shared memory (max %d)", N, ATT_MAX_TOKENS);
-    auto kern = attention_kernel<NW>;
-    if (smem_optin((const void *)kern, smem)) return 1;
-    CUDA_TRY(launch_pdl(kern, dim3(B * H), dim3(NW * 32), (size_t)smem, s, e->QKV16, (size_t)e->max_batch * N,
-                        e->A16, N, D, H, Npad, 1.0f / sqrtf((float)(D / H))));
-    e->launches++;
-    return 0;
+    return launch(e, attention_kernel<NW>, dim3(B * H), dim3(NW * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16, (size_t)e->max_batch * N, e->A16,
+                  N, D, H, Npad, 1.0f / sqrtf((float)(D / H)));
 }
 
 int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO)
@@ -835,11 +788,10 @@ int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
 }
 
 // The encoder part of the fixed kernel schedule: embeddings (vit.cpp:772-797), then blocks 0 .. layers-1 (vit.cpp:802-901); afterwards
-// the residual stream X holds the encoder's output at that depth.  Resets the launch count.
+// the residual stream X holds the encoder's output at that depth.
 int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cudaStream_t s, const vitb200_taps *taps)
 {
     const int D = e->hp.hidden_size, N = e->N, T = B * N;
-    e->launches = 0;
     __half *PA = e->PA;
     // patch embedding (vit.cpp:772-797): the f16 patch matrix PA (im2col of a stride == kernel conv is a pure permutation,
     // ggml.c:11528-11608) is either already there (d_images == NULL: the u8 path's preprocess kernel wrote it) or written by
@@ -851,12 +803,7 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         p.pos = e->pos; p.np = e->NP; p.ntok = N;
         ProfScope ps(e, PK_PATCH, 2.0 * p.M * p.N * e->KP, s);
         if (!patches_ready && launch_patchify(e, d_images, PA, B, s)) return 1;
-        {
-            const int n = B * D, threads = 256;
-            cls_rows_kernel<<<(n + threads - 1) / threads, threads, 0, s>>>(e->X, e->cls, e->pos, B, N, D);
-            CUDA_TRY(cudaGetLastError());
-            e->launches++;
-        }
+        if (launch(e, cls_rows_kernel, dim3((B * D + 255) / 256), dim3(256), 0, s, LAUNCH_PLAIN, e->X, e->cls, e->pos, B, N, D)) return 1;
         if (launch_gemm(e, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
     if (e->arch.pre_norm)
@@ -972,9 +919,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     {
         const size_t row_bytes = (size_t)C * sizeof(float);
         float *scratch = row_bytes > kSoftmaxSmemMax ? e->d_sm_scratch : nullptr;
-        softmax_topk_kernel<<<R, 256, scratch ? 0 : row_bytes, s>>>(lg, Cp, d_probs, d_topk_idx, d_topk_val, C, k, scratch);
-        CUDA_TRY(cudaGetLastError());
-        e->launches++;
+        if (launch(e, softmax_topk_kernel, dim3(R), dim3(256), scratch ? 0 : row_bytes, s, LAUNCH_PLAIN, lg, Cp, d_probs, d_topk_idx, d_topk_val, C, k,
+                   scratch))
+            return 1;
     }
     return 0;
 }
@@ -1032,15 +979,18 @@ int run_graphed(vitb200_engine *e, const GraphKey &key, cudaStream_t s, Run run)
     {
         if (run()) return 1;
         g->state = 1;
-        g->launches = e->launches;
         return 0;
     }
     if (g->state == 1)
     {
         cudaGraph_t graph = nullptr;
+        const int before = e->launches;
         CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
         const int rc = run();
         cudaError_t ce = cudaStreamEndCapture(s, &graph);
+        // the captured kernels did not run: the graph launch below, or the eager fallback, counts them
+        g->launches = e->launches - before;
+        e->launches = before;
         if (rc != 0 || ce != cudaSuccess || !graph)
         {
             if (graph) cudaGraphDestroy(graph);
@@ -1049,14 +999,13 @@ int run_graphed(vitb200_engine *e, const GraphKey &key, cudaStream_t s, Run run)
             e->use_graph = false; // fall back to eager launches (same kernels, same results)
             return run();
         }
-        g->launches = e->launches;
         ce = cudaGraphInstantiate(&g->exec, graph, 0);
         cudaGraphDestroy(graph);
         if (ce != cudaSuccess) { g->exec = nullptr; g->state = 0; e->use_graph = false; return fail("cudaGraphInstantiate failed: %s", cudaGetErrorString(ce)); }
         g->state = 2;
     }
     CUDA_TRY(cudaGraphLaunch(g->exec, s));
-    e->launches = g->launches;
+    e->launches += g->launches;
     return 0;
 }
 
@@ -1203,14 +1152,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (dev_alloc(e, &e->X, T * D) || dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->H16, h16) ||
         dev_alloc(e, &e->CLS16, R * D) || dev_alloc(e, &e->d_logits, R * e->Cp))
         return 1;
-    {
-        // soft-max working row: dynamic shared memory up to the per-CTA limit (opt-in above 48 KB), global scratch beyond it
-        const size_t row_bytes = (size_t)hp->num_classes * sizeof(float);
-        if (row_bytes > kSoftmaxSmemMax) { if (dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return 1; }
-        else if (row_bytes > 48 * 1024 &&
-                 cudaFuncSetAttribute(softmax_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSoftmaxSmemMax) != cudaSuccess)
-            return fail("cudaFuncSetAttribute(softmax_topk_kernel) failed");
-    }
+    // soft-max working row: dynamic shared memory up to the per-CTA limit, global scratch beyond it
+    if ((size_t)hp->num_classes * sizeof(float) > kSoftmaxSmemMax && dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return 1;
     for (Slot &sl : e->slot)
     {
         if (dev_alloc(e, &sl.img, B * img_elems) || dev_alloc(e, &sl.probs, R * hp->num_classes) || dev_alloc(e, &sl.logits, R * hp->num_classes) ||
@@ -1230,10 +1173,15 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         if (dev_alloc(e, &e->PA, pa_elems)) return 1;
         if (cudaMemset(e->PA, 0, pa_elems * sizeof(__half)) != cudaSuccess) return fail("cudaMemset failed");
     }
-    if (make_tmap(&e->tmA_D, e->A16, T, D, D, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_H, e->H16, T, 4 * (uint64_t)D, 4 * (uint64_t)D, GEMM_A_BOX_ROWS) ||
-        make_tmap(&e->tmA_P, e->PA, B * e->NP, e->KPp, e->KPp, GEMM_A_BOX_ROWS) || make_tmap(&e->tmA_C, e->CLS16, R, D, D, GEMM_A_BOX_ROWS))
+    // the GEMMs' A operands [rows][cols], dense rows: box = one k-block (128 B) x GEMM_A_BOX_ROWS rows
+    auto a_map = [&](CUtensorMap *m, const void *ptr, cuuint64_t rows, cuuint64_t cols, bool e4m3 = false) {
+        return e4m3 ? make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, ptr, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_A_BOX_ROWS})
+                    : make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_A_BOX_ROWS});
+    };
+    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, 4 * (cuuint64_t)D) || a_map(&e->tmA_P, e->PA, B * e->NP, e->KPp) ||
+        a_map(&e->tmA_C, e->CLS16, R, D))
         return 1;
-    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || make_tmap_e4m3(&e->tmA8, e->A8, T, D, GEMM_A_BOX_ROWS))) return 1;
+    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
     // memory (N <= 224), i.e. wherever the wgmma attention runs
     if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return 1;
@@ -1305,9 +1253,13 @@ int test_layernorm_impl(int device, int rows, int D, const float *x, const float
                        [&] { return launch_layernorm(e, dx, (size_t)D, dw, db, *y, rows, e->stream, 0, 0, y_scale ? *y_scale : nullptr); });
 }
 
-// One call of the host pipeline: begin_submit picks its slot; end_submit marks the slot's last use (everything enqueued on the compute
-// stream so far) and counts the call
-Slot &begin_submit(vitb200_engine *e) { return e->slot[e->submits & 1]; }
+// One call of the host pipeline, once its arguments are checked: begin_submit picks its slot and starts the call's launch count; end_submit
+// marks the slot's last use (everything enqueued on the compute stream so far) and counts the call
+Slot &begin_submit(vitb200_engine *e)
+{
+    e->launches = 0;
+    return e->slot[e->submits & 1];
+}
 
 int end_submit(vitb200_engine *e, Slot &sl)
 {
@@ -1521,6 +1473,7 @@ int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, 
         if (!e || !d_images) return fail("null argument");
         CUDA_TRY(cudaSetDevice(e->device));
         if (check_batch(e, batch) || check_k(e, k)) return 1;
+        e->launches = 0;
         return run_forward_graphed(e, d_images, batch, d_probs, d_logits, d_topk_idx, d_topk_prob, k, stream ? (cudaStream_t)stream : e->stream);
     });
 }
@@ -1532,6 +1485,7 @@ int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch,
         if (check_features(e, d_images, batch, req, d_tokens, d_prelogits)) return 1;
         if (((uintptr_t)d_tokens | (uintptr_t)d_prelogits) % 16 != 0) return fail("vitb200_features_device: output buffers must be 16-byte aligned");
         CUDA_TRY(cudaSetDevice(e->device));
+        e->launches = 0;
         return run_features_graphed(e, d_images, batch, req, d_tokens, d_prelogits, stream ? (cudaStream_t)stream : e->stream);
     });
 }
@@ -1716,15 +1670,19 @@ int vitb200_features(vitb200_engine *e, const float *images, int batch, const vi
 // have grown to the largest batch seen.
 // stage_u8 packs the images into slot sl and makes the compute stream wait for their copy (sl.d_u8 holds the pixels, then the
 // PreImage table at table_off); it waits on the host, because it overwrites pinned host memory the slot's previous copy may still be
-// reading.  preprocess_u8 adds the RGB kernel up to the patch matrix (and the optional f32 read-back).
+// reading.  preprocess_u8 adds the RGB kernel up to the patch matrix (and the optional f32 read-back).  The caller has checked the
+// images (check_u8_images, or the recognition's own check).
+static int check_u8_images(const uint8_t *const *images, const int *nx, const int *ny, int batch)
+{
+    for (int b = 0; b < batch; ++b)
+        if (!images[b] || nx[b] < 1 || ny[b] < 1) return fail("image %d: bad pointer or size", b);
+    return 0;
+}
+
 static int stage_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, size_t &table_off)
 {
     size_t total = 0;
-    for (int b = 0; b < batch; ++b)
-    {
-        if (!images[b] || nx[b] < 1 || ny[b] < 1) return fail("image %d: bad pointer or size", b);
-        total += ((size_t)nx[b] * ny[b] * 3 + 255) / 256 * 256;
-    }
+    for (int b = 0; b < batch; ++b) total += ((size_t)nx[b] * ny[b] * 3 + 255) / 256 * 256;
     table_off = total;
     total += (size_t)batch * sizeof(PreImage);
     CUDA_TRY(cudaSetDevice(e->device));
@@ -1763,11 +1721,10 @@ static int preprocess_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *imag
     if (stage_u8(e, sl, images, nx, ny, batch, table_off)) return 1;
     cudaStream_t s = e->stream;
     const int S = e->hp.img_size;
-    dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
     float *d_f32 = images_f32_out ? sl.img : nullptr;
-    preprocess_kernel<<<grid, 256, 0, s>>>(sl.d_u8, reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, bilinear ? 1 : 0,
-                                           e->PA, e->hp.patch_size, e->KPp);
-    CUDA_TRY(cudaGetLastError());
+    if (launch(e, preprocess_kernel, dim3((unsigned)((S * S + 255) / 256), (unsigned)batch), dim3(256), 0, s, LAUNCH_PLAIN, sl.d_u8,
+               reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, bilinear ? 1 : 0, e->PA, e->hp.patch_size, e->KPp))
+        return 1;
     const size_t img_elems = (size_t)3 * S * S;
     if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * img_elems * sizeof(float), cudaMemcpyDeviceToHost, s));
     return 0;
@@ -1778,14 +1735,11 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
 {
     if (!e || !images || !nx || !ny) return fail("null argument");
     if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-    if (check_batch(e, batch) || check_k(e, k)) return 1;
+    if (check_batch(e, batch) || check_k(e, k) || check_u8_images(images, nx, ny, batch)) return 1;
     Slot &sl = begin_submit(e);
     if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, images_f32_out)) return 1;
-    if (probs || logits || (k > 0 && (topk_idx || topk_prob)))
-    {
-        if (classify_to_host(e, sl, nullptr, batch, probs, logits, topk_idx, topk_prob, k, nullptr)) return 1;
-        e->launches += 1; // the preprocess kernel
-    }
+    if ((probs || logits || (k > 0 && (topk_idx || topk_prob))) && classify_to_host(e, sl, nullptr, batch, probs, logits, topk_idx, topk_prob, k, nullptr))
+        return 1;
     return end_submit(e, sl);
 }
 
@@ -1811,10 +1765,11 @@ int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const i
         if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
         if (!nx || !ny) return fail("vitb200_features_u8: null argument");
         if (e->C != 3) return fail("vitb200_features_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
+        if (check_u8_images(images, nx, ny, batch)) return 1;
         Slot &sl = begin_submit(e);
-        if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, nullptr) || features_to_host(e, nullptr, batch, req, tokens, prelogits)) return 1;
-        e->launches += 1; // the preprocess kernel
-        if (end_submit(e, sl)) return 1;
+        if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, nullptr) || features_to_host(e, nullptr, batch, req, tokens, prelogits) ||
+            end_submit(e, sl))
+            return 1;
         return vitb200_sync(e);
     });
 }
@@ -1844,25 +1799,22 @@ static int recognize_enqueue(vitb200_engine *e, const uint8_t *const *images, co
     cudaStream_t s = e->stream;
     const int S = e->hp.img_size, TH = e->head_tokens, C = e->hp.num_classes;
     float *d_f32 = images_f32_out ? sl.img : nullptr;
-    dim3 grid((unsigned)((S * S + 255) / 256), (unsigned)batch);
-    preprocess_gray_kernel<<<grid, 256, 0, s>>>(sl.d_u8, reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, e->PA,
-                                                e->hp.patch_size, e->KPp);
-    CUDA_TRY(cudaGetLastError());
+    if (launch(e, preprocess_gray_kernel, dim3((unsigned)((S * S + 255) / 256), (unsigned)batch), dim3(256), 0, s, LAUNCH_PLAIN, sl.d_u8,
+               reinterpret_cast<const PreImage *>(sl.d_u8 + table_off), d_f32, S, e->PA, e->hp.patch_size, e->KPp))
+        return 1;
     if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * S * S * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (chars || lengths || scores || probs)
     {
         // patches ready (d_images = NULL); top-1 of every head token into the slot; probabilities only when asked for
-        if (run_forward_graphed(e, nullptr, batch, probs ? sl.probs : nullptr, nullptr, sl.topk_idx, sl.topk_val, 1, s)) return 1;
-        vitstr_decode_kernel<<<(batch + 127) / 128, 128, 0, s>>>(sl.topk_idx, sl.topk_val, batch, TH, sl.chars, sl.len, sl.score);
-        CUDA_TRY(cudaGetLastError());
-        e->launches += 2; // the preprocess and decode kernels
+        if (run_forward_graphed(e, nullptr, batch, probs ? sl.probs : nullptr, nullptr, sl.topk_idx, sl.topk_val, 1, s) ||
+            launch(e, vitstr_decode_kernel, dim3((batch + 127) / 128), dim3(128), 0, s, LAUNCH_PLAIN, sl.topk_idx, sl.topk_val, batch, TH, sl.chars,
+                   sl.len, sl.score))
+            return 1;
         if (chars) CUDA_TRY(cudaMemcpyAsync(chars, sl.chars, (size_t)batch * (TH - 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
         if (lengths) CUDA_TRY(cudaMemcpyAsync(lengths, sl.len, (size_t)batch * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
         if (scores) CUDA_TRY(cudaMemcpyAsync(scores, sl.score, (size_t)batch * sizeof(double), cudaMemcpyDeviceToHost, s));
         if (probs) CUDA_TRY(cudaMemcpyAsync(probs, sl.probs, (size_t)batch * TH * C * sizeof(float), cudaMemcpyDeviceToHost, s));
     }
-    else
-        e->launches = 1; // preprocess only
     return end_submit(e, sl);
 }
 
@@ -1901,7 +1853,10 @@ int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint1
         // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
         if (!f16out && (epilogue == EPI_BIAS_RESID_F32 ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
         CUtensorMap tA, tB;
-        if (make_tmap(&tA, dA, M, K, K, GEMM_A_BOX_ROWS) || make_tmap(&tB, dW, N, K, K, GEMM_BN)) return 1;
+        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
+        if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dA, {Ku, Mu}, {2 * Ku}, {GEMM_BK, GEMM_A_BOX_ROWS}) ||
+            make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dW, {Ku, Nu}, {2 * Ku}, {GEMM_BK, GEMM_BN}))
+            return 1;
         GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = N; p.resid = o32;
         if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
@@ -1951,7 +1906,10 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
             dev_alloc(e, &hi, MN) || dev_alloc(e, &lo, MN))
             return 1;
         CUtensorMap tA, tB;
-        if (make_tmap_e4m3(&tA, dA, M, K, GEMM_A_BOX_ROWS) || make_tmap_e4m3(&tB, dW, N, K, GEMM_BN)) return 1;
+        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
+        if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, dA, {Ku, Mu}, {Ku}, {2 * GEMM_BK, GEMM_A_BOX_ROWS}) ||
+            make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_UINT8, dW, {Ku, Nu}, {Ku}, {2 * GEMM_BK, GEMM_BN}))
+            return 1;
         GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
         if (run_scratch(e, "e4m3 GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, true); })) return 1;
@@ -2010,23 +1968,22 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
             dev_alloc(e, &dY, (size_t)M * N))
             return 1;
         CUtensorMap tA, tW, tAd, tWd;
-        if (make_tmap_2d(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dAq, (uint64_t)M, (uint64_t)K, (uint64_t)K, Q8_BK, Q8_BM, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            make_tmap_2d(&tW, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, dWq, (uint64_t)N, (uint64_t)K, (uint64_t)K, Q8_BK, Q8_BN, CU_TENSOR_MAP_SWIZZLE_128B) ||
-            make_tmap_2d(&tAd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dAd, (uint64_t)M, (uint64_t)KB, (uint64_t)KB, 4, Q8_BM, CU_TENSOR_MAP_SWIZZLE_NONE) ||
-            make_tmap_2d(&tWd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, dWd, (uint64_t)KB, (uint64_t)N, (uint64_t)N, Q8_BN, 4, CU_TENSOR_MAP_SWIZZLE_NONE))
+        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K, KBu = (cuuint64_t)KB;
+        if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, dAq, {Ku, Mu}, {Ku}, {Q8_BK, Q8_BM}) ||
+            make_tmap(&tW, CU_TENSOR_MAP_DATA_TYPE_UINT8, dWq, {Ku, Nu}, {Ku}, {Q8_BK, Q8_BN}) ||
+            make_tmap(&tAd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dAd, {KBu, Mu}, {4 * KBu}, {4, Q8_BM}, CU_TENSOR_MAP_SWIZZLE_NONE) ||
+            make_tmap(&tWd, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, dWd, {Nu, KBu}, {4 * Nu}, {Q8_BN, 4}, CU_TENSOR_MAP_SWIZZLE_NONE))
             return 1;
-        if (cudaFuncSetAttribute(gemm_q8_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Q8_SMEM_BYTES) != cudaSuccess) return fail("cudaFuncSetAttribute failed");
         Q8GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = dY; p.ldo = N;
         const int grid = ((M + Q8_BM - 1) / Q8_BM) * ((N + Q8_BN - 1) / Q8_BN); // one CTA per tile
+        auto gemm = [&] { return launch(e, gemm_q8_wgmma_kernel, dim3(grid), dim3(Q8_THREADS), Q8_SMEM_BYTES, s, LAUNCH_PLAIN, tA, tW, tAd, tWd, p); };
         auto run = [&] {
             const long long n_blocks = (long long)M * KB;
             const int qthreads = 256;
             const long long qgrid = (n_blocks * 8 + qthreads - 1) / qthreads;
-            quantize_q8_0_kernel<<<(unsigned)qgrid, qthreads, 0, s>>>(dX, dAq, dAd, n_blocks);
-            if (cudaGetLastError() != cudaSuccess) return fail("quantize launch failed");
-            gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES, s>>>(tA, tW, tAd, tWd, p);
-            return 0;
+            if (launch(e, quantize_q8_0_kernel, dim3((unsigned)qgrid), dim3(qthreads), 0, s, LAUNCH_PLAIN, dX, dAq, dAd, n_blocks)) return 1;
+            return gemm();
         };
         if (run_scratch(e, "q8_0 GEMM kernel", run) || tap_f32(y, dY, (size_t)M * N, s)) return 1;
         if (xq) CUDA_TRY(cudaMemcpy(xq, dAq, (size_t)M * K, cudaMemcpyDeviceToHost));
@@ -2041,7 +1998,8 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
             e->event_pool.push_back(t1);
             auto timed = [&]() -> int {
                 CUDA_TRY(cudaEventRecord(t0, s));
-                for (int i = 0; i < iters; ++i) gemm_q8_wgmma_kernel<<<grid, Q8_THREADS, Q8_SMEM_BYTES, s>>>(tA, tW, tAd, tWd, p);
+                for (int i = 0; i < iters; ++i)
+                    if (gemm()) return 1;
                 CUDA_TRY(cudaEventRecord(t1, s));
                 return 0;
             };
