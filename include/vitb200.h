@@ -102,13 +102,25 @@ typedef struct vitb200_arch
     int32_t activation; /* MLP activation after fc1: 0 GELU, tanh form, through ggml's f16 table (the reference, unchanged); 1 GELU, erf form,
                          * 0.5 x (1 + erf(x / sqrt 2)); 2 QuickGELU, x / (1 + exp(-1.702 x)).  Forms 1 and 2 take x = acc + bias (FP8 engine:
                          * acc (sa sw) + bias) in f32, without rounding it to f16 first, and store f16(act(x)). */
+    /* DINOv2 (HF Dinov2Model / Dinov2WithRegistersModel and their ForImageClassification heads).  Zero is the behaviour above. */
+    int32_t layer_scale; /* 0 or 1.  1: x = x + f32(f32(acc + bias) * gamma[n]) after proj ('blocks.{i}.ls1.gamma' [D]) and fc2
+                          * ('blocks.{i}.ls2.gamma' [D]), gamma kept in f32 (HF's LayerScale order; not folded into the f16 weights). */
+    int32_t reg_tokens;  /* R = 0..16 register tokens ('reg_token' [1, R, D]).  Token rows per image are [cls, reg_1..R, patch_1..P],
+                          * N = P + 1 + R; 'pos_embed' is [1, N, D] with the R register rows after the class row (zero for DINOv2). */
+    int32_t pool;        /* 0: the head reads the first head_tokens rows (the reference).  1: the head reads one row of 2 D per image,
+                          * LN(token 0) || mean over the P patch rows of LN(patch) (registers excluded, LN = the final LayerNorm):
+                          * DINOv2's classifier input.  'head.weight' is then [C][2 D] and head_tokens must be 1. */
 } vitb200_arch;
-/* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = {0, 0}, the reference).
- * Fields out of range, and pre_norm = 1 without both norm_pre tensors, fail here before the device is touched.  Every entry point
- * works on such an engine; the u8 entry points keep vit.cpp's preprocessing (a CLIP caller normalises its own images and uses the f32
- * or device entry points).  The launch count of one forward is 3 + 7 L + 3, plus 1 with the pre-norm.
- * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer) and vit.activation ("gelu_tanh", "gelu_erf",
- * "quick_gelu"; any other string fails the load) and then holds 2 more tensors; legacy-ggml files are always the reference's. */
+/* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = all zero, the reference).
+ * Fields out of range, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every ls1 / ls2 gamma, reg_tokens > 0 without
+ * 'reg_token', pool = 1 with head_tokens > 1, and a head whose K is not D (pool 0) or 2 D (pool 1) fail here before the device is
+ * touched; so does N > 896 tokens, registers included.  Every entry point works on such an engine; the u8 entry points keep vit.cpp's
+ * preprocessing (a CLIP or DINOv2 caller normalises its own images and uses the f32 or device entry points).  The launch count of one
+ * forward is 3 + 7 L + 3, plus 1 with the pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm).
+ * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer), vit.activation ("gelu_tanh", "gelu_erf",
+ * "quick_gelu"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and vit.pool ("token" or
+ * "cls_patch_mean"; any other string fails the load), and then holds 2 more tensors with the pre-norm, 2 L more with LayerScale and
+ * 1 more with registers; a file without these keys is the reference's architecture, and legacy-ggml files never carry them. */
 int vitb200_create_arch(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *tensors, int n_tensors, int device,
                         int max_batch, int head_tokens, int fp8, vitb200_engine **out);
 int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out);
@@ -206,10 +218,12 @@ typedef struct vitb200_features_req
     int32_t dtype;  /* 0 f32, 1 f16, 2 bf16 -- the 16-bit forms are the f32 result rounded to nearest even */
 } vitb200_features_req;
 
-/* tokens:    [batch][N][D], every token, cls first (N = (img/patch)^2 + 1); may be NULL
+/* tokens:    [batch][N][D], every token, cls first, then the R register tokens, then the patches (N = (img/patch)^2 + 1 + R,
+ *            Hugging Face's last_hidden_state / hidden_states[i] order); may be NULL
  * prelogits: [batch][head_tokens][D], the rows the classifier head reads (token 0, vit.cpp:910; the first 25 for ViTSTR,
- *            vitstr.cpp:864-883); may be NULL.  At layers == num_hidden_layers with norm == 1 this is the head's input before
- *            its f16 rounding.  At least one of the two must be non-NULL.
+ *            vitstr.cpp:864-883); with vitb200_arch.pool = 1, [batch][1][2 D]: token 0 || the mean of the patch rows, each row
+ *            through the final LayerNorm first when norm == 1.  May be NULL.  At layers == num_hidden_layers with norm == 1 this is
+ *            the head's input before its f16 rounding.  At least one of the two must be non-NULL.
  * vitb200_features: HOST buffers, blocking, like vitb200_forward (images as there).
  * vitb200_features_device: DEVICE buffers (16-byte aligned) enqueued on `stream` without synchronising, like vitb200_forward_device.
  * vitb200_features_u8: u8 RGB images pre-processed on the GPU, like vitb200_forward_u8 (RGB models only); host outputs, blocking.
@@ -252,7 +266,7 @@ typedef struct vitb200_taps
     float *ln2;      /* [batch][N][D]  */
     float *h;        /* [batch][N][4D] */
     float *x2;       /* [batch][N][D]  */
-    float *final_ln; /* [batch][D]     */
+    float *final_ln; /* [batch][D]     the head's f16 input ([batch][2 D] with vitb200_arch.pool = 1) */
     float *x_final;  /* [batch][N][D]  */
 } vitb200_taps;
 
@@ -265,6 +279,11 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
  * host (f16 results widened).  resid may be NULL unless epilogue == 2. */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
                       const float *bias, const float *resid, float *out);
+
+/* The same with the LayerScale residual epilogue (vitb200_arch.layer_scale, proj and fc2): out float32 [M][N] =
+ * f32(f32(acc + bias[n]) * gamma[n]) + resid[m][n], computed in place on a copy of resid as the engine does.  K % 8 == 0, N % 4 == 0. */
+int vitb200_test_gemm_layer_scale(int device, int M, int N, int K, const uint16_t *A, const uint16_t *W, const float *bias,
+                                  const float *gamma, const float *resid, float *out);
 
 /* Stand-alone run of the block LayerNorm kernel the forward schedule uses (reference ggml_norm + ggml_mul + ggml_add, vit.cpp:808-812,
  * ggml.c:8959-9008): x float32 [rows][D] -> y float32 [rows][D] holding the f16 results (the next GEMM's A operand) widened. */

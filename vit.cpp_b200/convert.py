@@ -3,6 +3,7 @@
     python -m convert <checkpoint.pth|.safetensors> <out.gguf> [--ftype 0|1] [--heads H] [--labels labels.json] [--container legacy|gguf]
                       [--keep-norm-pre] [--activation gelu_tanh|gelu_erf|quick_gelu] [--eps E]     (timm; these three need GGUF)
     python -m convert <CLIP model.safetensors|.pth> <out.gguf> --hf-config config.json             (Hugging Face CLIP vision tower)
+    python -m convert <DINOv2 model.safetensors> <out.gguf> --hf-config config.json [--img-size S]  (Hugging Face DINOv2)
     python -m convert --quantize <in.gguf> <out.gguf> q8_0
 
 * `state_dict_to_model_file` follows reference convert-pth-to-ggml.py:105-158 step by step (header, id2label table, tensors in
@@ -13,6 +14,9 @@
   hidden / 64 (true for every timm ViT the reference lists).
 * `clip_to_model_file` converts a Hugging Face CLIP vision tower (`vision_model.*` of CLIPVisionModel, CLIPVisionModelWithProjection
   or CLIPModel) to a GGUF file with the pre-norm, QuickGELU or erf GELU and eps 1e-5 (`clip_to_timm` holds the name mapping).
+* `dinov2_to_model_file` converts a Hugging Face DINOv2 (Dinov2Model, Dinov2WithRegistersModel and their ForImageClassification
+  heads) to a GGUF file with LayerScale, register tokens and, with a classifier, the class-plus-patch-mean head (`dinov2_to_timm`).
+  `--img-size S` resamples the patch position grid of any converted model to S / patch, as Hugging Face does at run time.
 * `quantize_model_file` restates reference quantize.cpp for q8_0 (every 2-D `*weight` tensor, quantize_row_q8_0_reference,
   ggml-quants.c): byte-identical to the reference binary's output (pinned by the CPU test-suite).
 
@@ -89,14 +93,20 @@ def load_state_dict(path: str) -> Dict[str, np.ndarray]:
     return {k: v.detach().to(torch.float32).numpy() for k, v in sd.items() if hasattr(v, "detach")}
 
 
+def reg_token_count(sd: Dict[str, np.ndarray]) -> int:
+    """R, the register tokens of a state dict ('reg_token' [1, R, D]; 0 without one)."""
+    return int(sd["reg_token"].shape[1]) if "reg_token" in sd else 0
+
+
 def infer_hparams(sd: Dict[str, np.ndarray], heads: Optional[int] = None):
     """(hidden, layers, heads, classes, patch, img, in_chans) from timm VisionTransformer tensor shapes."""
     pw = sd["patch_embed.proj.weight"]                       # (D, C, P, P)
     hidden, in_chans, patch = int(pw.shape[0]), int(pw.shape[1]), int(pw.shape[2])
-    n_tok = int(sd["pos_embed"].shape[1])                    # (1, N, D), N = (img / patch)^2 + 1
-    grid = int(round((n_tok - 1) ** 0.5))
-    if grid * grid + 1 != n_tok:
-        raise ValueError(f"pos_embed has {n_tok} tokens: not a square patch grid plus one class token")
+    n_tok = int(sd["pos_embed"].shape[1])                    # (1, N, D), N = (img / patch)^2 + 1 + R
+    R = reg_token_count(sd)
+    grid = int(round(max(n_tok - 1 - R, 0) ** 0.5))
+    if grid * grid + 1 + R != n_tok:
+        raise ValueError(f"pos_embed has {n_tok} tokens: not a square patch grid plus one class token" + (f" and {R} registers" if R else ""))
     layers = 1 + max(int(m.group(1)) for k in sd for m in [re.match(r"blocks\.(\d+)\.", k)] if m)
     classes = int(sd["head.weight"].shape[0])
     heads = heads or hidden // 64
@@ -105,12 +115,47 @@ def infer_hparams(sd: Dict[str, np.ndarray], heads: Optional[int] = None):
     return hidden, layers, heads, classes, patch, grid * patch, in_chans
 
 
+def resample_pos_embed(pos: np.ndarray, prefix: int, grid: int, antialias: bool = False) -> np.ndarray:
+    """pos_embed [1, prefix + G^2, D] -> [1, prefix + grid^2, D]: the patch rows resampled on their square grid exactly as Hugging
+    Face's interpolate_pos_encoding does it at run time (torch bicubic, align_corners False, in float32; Dinov2WithRegisters also
+    antialiases), the `prefix` rows (class token, registers) kept."""
+    import torch
+    pos = np.asarray(pos, np.float32)
+    D = pos.shape[-1]
+    patches = pos.reshape(-1, D)[prefix:]
+    G = int(round(len(patches) ** 0.5))
+    if G * G != len(patches):
+        raise ValueError(f"pos_embed has {len(patches)} patch rows: not a square grid")
+    if G == grid:
+        return pos
+    t = torch.from_numpy(np.ascontiguousarray(patches.reshape(1, G, G, D).transpose(0, 3, 1, 2)))
+    r = torch.nn.functional.interpolate(t, size=(grid, grid), mode="bicubic", align_corners=False, antialias=antialias)
+    out = r.permute(0, 2, 3, 1).reshape(grid * grid, D).numpy()
+    return np.concatenate([pos.reshape(-1, D)[:prefix], out]).reshape(1, -1, D).astype(np.float32)
+
+
 def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: int = 1, heads: Optional[int] = None,
                              id2label: Optional[Dict[int, str]] = None, container: str = "legacy", keep_norm_pre: bool = False,
-                             activation: str = "gelu_tanh", eps: float = 1e-6) -> None:
+                             activation: str = "gelu_tanh", eps: float = 1e-6, pool: str = "token", img_size: Optional[int] = None,
+                             antialias: bool = False) -> None:
     """keep_norm_pre, activation, eps: the architecture of a CLIP-pretrained timm ViT (norm_pre, QuickGELU or erf GELU, eps 1e-5);
-    GGUF only.  Without them the file is the reference converter's, which drops norm_pre."""
+    GGUF only.  Without them the file is the reference converter's, which drops norm_pre.  LayerScale ('blocks.{i}.ls1.gamma' /
+    'ls2.gamma') and register tokens ('reg_token', with their R rows after the class row of pos_embed) are taken when the state dict has
+    them; pool 'cls_patch_mean' makes the head read [class token || patch mean] (DINOv2's classifier).  img_size: resample the patch
+    position grid to img_size / patch (resample_pos_embed)."""
     assert ftype in (0, 1)
+    layer_scale = int(any(k.endswith(".ls1.gamma") for k in sd))
+    R = reg_token_count(sd)
+    if pool not in gf.POOLS:
+        raise ValueError(f"pool {pool!r} unknown ({', '.join(gf.POOLS)})")
+    if container != "gguf" and (layer_scale or R or pool != "token"):
+        raise ValueError("LayerScale, register tokens or another pool need --container gguf: a legacy ggml file carries the reference's "
+                         "architecture only")
+    if img_size is not None:
+        P = int(sd["patch_embed.proj.weight"].shape[2])
+        if img_size % P:
+            raise ValueError(f"img_size {img_size} is not a multiple of the patch size {P}")
+        sd = dict(sd, pos_embed=resample_pos_embed(sd["pos_embed"], 1 + R, img_size // P, antialias))
     if activation not in gf.ACTIVATIONS:
         raise ValueError(f"activation {activation!r} unknown ({', '.join(gf.ACTIVATIONS)})")
     if container != "gguf" and (keep_norm_pre or activation != "gelu_tanh" or eps != 1e-6):
@@ -121,7 +166,7 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
     hidden, layers, heads, classes, patch, img, in_chans = infer_hparams(sd, heads)
     id2label = id2label or {i: f"LABEL_{i}" for i in range(classes)}   # convert-pth-to-ggml.py:95-96 fallback names
     vf = gf.VitFile(hidden, layers, heads, classes, patch, img, ftype, dict(id2label), eps=eps, pre_norm=int(keep_norm_pre),
-                    activation=activation)
+                    activation=activation, layer_scale=layer_scale, reg_tokens=R, pool=pool)
     for k, v in sd.items():
         if k.startswith("norm_pre") and not keep_norm_pre:               # convert-pth-to-ggml.py:127-130
             continue
@@ -130,10 +175,11 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
             a = a.reshape(1, a.shape[0], 1, 1)                           # convert-pth-to-ggml.py:150-151
         # convert-pth-to-ggml.py:143-147; the loader additionally hard-codes the patch kernel as F16 (vit.cpp:515), so an f32
         # file must still carry it as f16 (SURVEY.md 8c: the reference's own --ftype 0 output does not load)
-        f16 = (ftype == 1 and np.asarray(v).ndim != 1 and k not in ("pos_embed", "cls_token")) or k == "patch_embed.proj.weight"
+        f16 = (ftype == 1 and np.asarray(v).ndim != 1 and k not in ("pos_embed", "cls_token", "reg_token")) or k == "patch_embed.proj.weight"
         vf.tensors[k] = a.astype(np.float16 if f16 else np.float32)
         vf.tensor_ftype[k] = 1 if f16 else 0
-    expect = 4 + 12 * layers + 4 + 2 * vf.pre_norm                      # vit.cpp:697, plus norm_pre.weight / .bias
+    # vit.cpp:697, plus norm_pre.weight / .bias, the two LayerScale gammas of every block and reg_token
+    expect = 4 + 12 * layers + 4 + 2 * vf.pre_norm + 2 * layers * layer_scale + (R > 0)
     if len(vf.tensors) != expect:
         raise ValueError(f"state_dict has {len(vf.tensors)} tensors after filtering, a {layers}-layer ViT needs {expect}")
     if container == "gguf":
@@ -200,6 +246,83 @@ def clip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, f
         raise ValueError("a CLIP tower needs --container gguf: a legacy ggml file carries the reference's architecture only")
     tsd, heads, activation, eps = clip_to_timm(sd, config)
     state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", keep_norm_pre=True, activation=activation, eps=eps)
+
+
+_DINOV2_PREFIXES = ("dinov2.", "dinov2_with_registers.")
+
+
+def is_hf_dinov2(sd: Dict[str, np.ndarray]) -> bool:
+    """A Dinov2Model, Dinov2WithRegistersModel or their ForImageClassification state dict (keys unprefixed or under `dinov2.` /
+    `dinov2_with_registers.`)."""
+    return any(k.endswith("embeddings.patch_embeddings.projection.weight") for k in sd) and any(".layer_scale1.lambda1" in k for k in sd)
+
+
+def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
+    """Hugging Face DINOv2 -> (timm-named state dict, heads, activation, eps, pool, antialias).  query / key / value become attn.qkv,
+    attention.output.dense attn.proj, layer_scale{1,2}.lambda1 ls{1,2}.gamma, embeddings.register_tokens reg_token (with R zero rows
+    inserted into pos_embed after the class row: registers get no position embedding), layernorm norm; mask_token is dropped.  A
+    classifier becomes the head with pool 'cls_patch_mean' (its logits are HF's); without one the head is the identity with pool 'token',
+    so the logits are HF's pooler_output.  antialias: how HF resamples this class's position grid (Dinov2WithRegisters antialiases)."""
+    act = config.get("hidden_act", "gelu")
+    if act != "gelu":
+        raise ValueError(f"hidden_act {act!r} is not supported (gelu only)")
+    if config.get("use_swiglu_ffn", False):
+        raise ValueError("use_swiglu_ffn: SwiGLU MLPs (DINOv2 ViT-g) are not supported")
+    if not config.get("qkv_bias", True):
+        raise ValueError("qkv_bias false is not supported (the engine's qkv has a bias)")
+    if config.get("mlp_ratio", 4) != 4:
+        raise ValueError(f"mlp_ratio {config.get('mlp_ratio')} is not supported (4 only)")
+    pre = next((p for p in _DINOV2_PREFIXES if any(k.startswith(p) for k in sd)), "")
+    v = {k[len(pre):]: np.asarray(a, np.float32) for k, a in sd.items() if k.startswith(pre)}
+    pw = v["embeddings.patch_embeddings.projection.weight"]            # (D, C, P, P)
+    D = int(pw.shape[0])
+    heads = int(config.get("num_attention_heads", D // 64))
+    if D % heads or D // heads != 64:
+        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    layers = 1 + max(int(m.group(1)) for k in v for m in [re.match(r"encoder\.layer\.(\d+)\.", k)] if m)
+    reg = v.get("embeddings.register_tokens")
+    R = 0 if reg is None else int(reg.shape[1])
+    pos = v["embeddings.position_embeddings"].reshape(1, -1, D)
+    out = {"cls_token": v["embeddings.cls_token"].reshape(1, 1, D),
+           "pos_embed": np.concatenate([pos[:, :1], np.zeros((1, R, D), np.float32), pos[:, 1:]], axis=1),
+           "patch_embed.proj.weight": pw, "patch_embed.proj.bias": v["embeddings.patch_embeddings.projection.bias"]}
+    if R:
+        out["reg_token"] = reg.reshape(1, R, D)
+    for i in range(layers):
+        h, t = f"encoder.layer.{i}.", f"blocks.{i}."
+        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        for p in ("weight", "bias"):
+            out[f"{t}norm1.{p}"] = v[f"{h}norm1.{p}"]
+        for p in ("weight", "bias"):                                     # rows [q; k; v]
+            out[f"{t}attn.qkv.{p}"] = np.concatenate([v[f"{h}attention.attention.{x}.{p}"] for x in ("query", "key", "value")], axis=0)
+        for p in ("weight", "bias"):
+            out[f"{t}attn.proj.{p}"] = v[f"{h}attention.output.dense.{p}"]
+        out[f"{t}ls1.gamma"] = v[h + "layer_scale1.lambda1"]
+        for dst, src in (("norm2", "norm2"), ("mlp.fc1", "mlp.fc1"), ("mlp.fc2", "mlp.fc2")):
+            for p in ("weight", "bias"):
+                out[f"{t}{dst}.{p}"] = v[f"{h}{src}.{p}"]
+        out[f"{t}ls2.gamma"] = v[h + "layer_scale2.lambda1"]
+    out["norm.weight"], out["norm.bias"] = v["layernorm.weight"], v["layernorm.bias"]
+    cls_w = sd.get("classifier.weight")
+    if cls_w is not None:
+        out["head.weight"], out["head.bias"] = np.asarray(cls_w, np.float32), np.asarray(sd["classifier.bias"], np.float32)
+    else:
+        out["head.weight"], out["head.bias"] = np.eye(D, dtype=np.float32), np.zeros(D, np.float32)
+    pool = "cls_patch_mean" if cls_w is not None else "token"
+    return out, heads, "gelu_erf", float(config.get("layer_norm_eps", 1e-6)), pool, R > 0
+
+
+def dinov2_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
+                         container: str = "gguf", img_size: Optional[int] = None) -> None:
+    """A Hugging Face DINOv2 -> GGUF model file (LayerScale, registers, erf GELU, the config's eps; the classifier's pool)."""
+    if container != "gguf":
+        raise ValueError("a DINOv2 model needs --container gguf: a legacy ggml file carries the reference's architecture only")
+    tsd, heads, activation, eps, pool, antialias = dinov2_to_timm(sd, config)
+    if id2label is None and "id2label" in config and "classifier.weight" in sd:
+        id2label = {int(k): str(x) for k, x in config["id2label"].items()}
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool, img_size=img_size,
+                             antialias=antialias)
 
 
 def write_legacy(path: str, vf) -> None:
@@ -279,16 +402,23 @@ def main(argv):
     ap.add_argument("--labels", default=None, help="JSON file {class id: label}")
     ap.add_argument("--container", choices=["legacy", "gguf"], default=None,
                     help="default: legacy for the reference's architecture, gguf for a CLIP tower or the options below")
-    ap.add_argument("--hf-config", default=None, help="config.json of a Hugging Face CLIP checkpoint (required for one)")
+    ap.add_argument("--hf-config", default=None, help="config.json of a Hugging Face CLIP or DINOv2 checkpoint (required for one)")
     ap.add_argument("--keep-norm-pre", action="store_true", help="timm: keep norm_pre as the model's pre-norm (GGUF only)")
     ap.add_argument("--activation", choices=list(gf.ACTIVATIONS), default="gelu_tanh", help="timm: the MLP activation (GGUF only)")
     ap.add_argument("--eps", type=float, default=1e-6, help="timm: the LayerNorm epsilon (GGUF only)")
+    ap.add_argument("--img-size", type=int, default=None,
+                    help="resample the patch position embeddings to this input size (default: the checkpoint's grid)")
     a = ap.parse_args(argv)
     if a.quantize:
         quantize_model_file(a.src, a.dst, a.fmt)
         return
     labels = {int(k): v for k, v in json.load(open(a.labels)).items()} if a.labels else None
     sd = load_state_dict(a.src)
+    if is_hf_dinov2(sd):
+        if not a.hf_config:
+            raise SystemExit("a Hugging Face DINOv2 state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
+        dinov2_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", a.img_size)
+        return
     if is_hf_clip(sd):
         if not a.hf_config:
             raise SystemExit("a Hugging Face CLIP state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
@@ -296,7 +426,7 @@ def main(argv):
         return
     new_arch = a.keep_norm_pre or a.activation != "gelu_tanh" or a.eps != 1e-6
     state_dict_to_model_file(sd, a.dst, a.ftype, a.heads, labels, a.container or ("gguf" if new_arch else "legacy"),
-                             a.keep_norm_pre, a.activation, a.eps)
+                             a.keep_norm_pre, a.activation, a.eps, img_size=a.img_size)
 
 
 if __name__ == "__main__":

@@ -116,6 +116,7 @@ struct Linear
 struct Layer
 {
     float *n1w = nullptr, *n1b = nullptr, *n2w = nullptr, *n2b = nullptr;
+    float *ls1 = nullptr, *ls2 = nullptr; // vitb200_arch.layer_scale: the LayerScale gamma [D] of proj and of fc2
     Linear qkv, proj, fc1, fc2;
 };
 
@@ -152,14 +153,15 @@ struct Slot
 struct vitb200_engine
 {
     vitb200_hparams hp;
-    vitb200_arch arch{0, 0}; // pre-norm and MLP activation; {0, 0} is the reference's architecture
+    vitb200_arch arch{}; // pre-norm, MLP activation, LayerScale, register tokens, head pooling; all zero is the reference's architecture
     float *npre_w = nullptr, *npre_b = nullptr; // arch.pre_norm: norm_pre.weight / norm_pre.bias
     int device = 0, max_batch = 0, num_sms = 132;
-    int N = 0, NP = 0, G = 0, KP = 0, KPp = 0;
+    int N = 0, NP = 0, G = 0, KP = 0, KPp = 0; // N = NP + 1 + arch.reg_tokens token rows per image
     int Cp = 0;           // num_classes rounded up to a multiple of 4: pitch of the internal logits rows (128-bit epilogue stores)
     float *d_sm_scratch = nullptr; // soft-max working rows in global memory, only when num_classes floats exceed shared memory
     int C = 3;            // input channels: 3 (vit.cpp) or 1 (ViTSTR extension, vitstr.cpp:713), taken from the patch kernel's shape
     int head_tokens = 1;  // tokens the classifier head reads per image: 1 (token 0, vit.cpp:910) or 25 (vitstr.cpp:864-903)
+    int KH = 0;           // the head's K: D, or 2 D with arch.pool = 1 (CLS16 rows are [LN(cls) || mean of LN(patches)])
     // FP8 engine (vitb200_create_fp8): LayerNorms 1 and 2 write e4m3 rows A8 with per-row scales SA, and the qkv and fc1 GEMMs run
     // e4m3 x e4m3 against per-tensor-scaled e4m3 weights; everything else is the f16 engine's schedule
     bool fp8 = false;
@@ -169,7 +171,7 @@ struct vitb200_engine
     cudaStream_t stream = nullptr;
     std::vector<void *> allocs;
     // weights
-    float *cls = nullptr, *pos = nullptr, *norm_w = nullptr, *norm_b = nullptr;
+    float *cls = nullptr, *pos = nullptr, *norm_w = nullptr, *norm_b = nullptr; // cls: [1 + reg_tokens][D], cls_token then reg_token
     Linear patch, head;
     std::vector<Layer> layers;
     // activations (static arena, sized for max_batch)
@@ -558,7 +560,7 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
         };
         if (out_map(&tmO, p.out)) return 1;
         if (EPI == EPI_BIAS_F16_HILO && out_map(&tmX, p.out2)) return 1;
-        if (EPI == EPI_BIAS_RESID_F32 && out_map(&tmX, p.resid)) return 1;
+        if (gemm_epi_resid(EPI) && out_map(&tmX, p.resid)) return 1;
     }
     // persistent: as many clusters as fit at once, each walking the pairs of column tiles cluster, cluster + clusters, ...
     const int pairs = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN));
@@ -584,7 +586,7 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
     VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
-    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
+    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16) VB_CASE(EPI_BIAS_SCALE_RESID_F32)
 #undef VB_CASE
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
@@ -626,6 +628,8 @@ int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaS
 // hidden size the engine accepts.
 constexpr int LN_ROWS_MAX_V = 16;
 constexpr int LN_MAX_HIDDEN = LN_ROWS_MAX_V * 128;
+// register tokens a model may have (vitb200_arch.reg_tokens; DINOv2 with registers has 4)
+constexpr int VB_MAX_REG_TOKENS = 16;
 
 template <typename OutT, bool NORM>
 int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
@@ -674,11 +678,27 @@ int launch_layernorm_inplace(vitb200_engine *e, float *x, const float *w, const 
     return launch(e, kern, dim3(blocks), dim3(threads), 0, s, LAUNCH_PDL, x, w, b, rows, D, e->hp.eps);
 }
 
+// DINOv2's classifier input (vitb200_arch.pool = 1): per image, [LN(token 0) || mean of LN(patch rows)] into y [B][2 D] (NORM = false:
+// the rows as they are), rows 1 .. reg_tokens left out
+template <typename OutT, bool NORM>
+int launch_pool(vitb200_engine *e, OutT *y, int B, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size;
+    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
+    const auto kern = D <= 4 * 128 ? cls_patch_mean_kernel<4, OutT, NORM>
+                    : D <= 8 * 128 ? cls_patch_mean_kernel<8, OutT, NORM> : cls_patch_mean_kernel<LN_ROWS_MAX_V, OutT, NORM>;
+    return launch(e, kern, dim3(B), dim3(POOL_WARPS * 32), (size_t)POOL_WARPS * D * sizeof(float), s, LAUNCH_PDL, e->X, e->N,
+                  1 + e->arch.reg_tokens, e->norm_w, e->norm_b, y, D, e->hp.eps);
+}
+
 // The fc1 epilogue of the model's MLP activation (vitb200_arch.activation)
 int fc1_epilogue(const vitb200_engine *e)
 {
     return e->arch.activation == 1 ? EPI_BIAS_GELU_ERF_F16 : e->arch.activation == 2 ? EPI_BIAS_QUICK_GELU_F16 : EPI_BIAS_GELU_F16;
 }
+
+// The residual epilogue of proj and fc2: with LayerScale (vitb200_arch.layer_scale) the branch is scaled by gamma before the add
+int resid_epilogue(const vitb200_engine *e) { return e->arch.layer_scale ? EPI_BIAS_SCALE_RESID_F32 : EPI_BIAS_RESID_F32; }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
 // token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision; ATT_MMA16 = the mma.sync kernel with 16 warps,
@@ -798,12 +818,16 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
     // patchify (one warp per patch, coalesced); the TMA-fed GEMM adds conv bias + pos_embed and writes token rows.
     const bool patches_ready = d_images == nullptr;
     {
+        // the epilogue writes patch p of an image to row 1 + p and adds position row 1 + p: with R register tokens both bases move
+        // down by R rows, so patch p lands in row 1 + R + p with position row 1 + R + p
+        const int R = e->arch.reg_tokens;
         GemmParams p{};
-        p.M = B * e->NP; p.N = D; p.K = e->KPp; p.bias = e->patch.b; p.out = e->X; p.ldo = D;
-        p.pos = e->pos; p.np = e->NP; p.ntok = N;
+        p.M = B * e->NP; p.N = D; p.K = e->KPp; p.bias = e->patch.b; p.out = e->X + (size_t)R * D; p.ldo = D;
+        p.pos = e->pos + (size_t)R * D; p.np = e->NP; p.ntok = N;
         ProfScope ps(e, PK_PATCH, 2.0 * p.M * p.N * e->KP, s);
         if (!patches_ready && launch_patchify(e, d_images, PA, B, s)) return 1;
-        if (launch(e, cls_rows_kernel, dim3((B * D + 255) / 256), dim3(256), 0, s, LAUNCH_PLAIN, e->X, e->cls, e->pos, B, N, D)) return 1;
+        if (launch(e, cls_rows_kernel, dim3((B * (1 + R) * D + 255) / 256), dim3(256), 0, s, LAUNCH_PLAIN, e->X, e->cls, e->pos, B, 1 + R, N, D))
+            return 1;
         if (launch_gemm(e, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
     if (e->arch.pre_norm)
@@ -846,9 +870,9 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (tap && tap_f16(taps->attn, e->A16, (size_t)T * D, s)) return 1;
         {
             GemmParams p{};
-            p.M = T; p.N = D; p.K = D; p.bias = L.proj.b; p.out = e->X; p.ldo = D; p.resid = e->X;
+            p.M = T; p.N = D; p.K = D; p.bias = L.proj.b; p.out = e->X; p.ldo = D; p.resid = e->X; p.gamma = L.ls1;
             ProfScope ps(e, PK_PROJ, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_D, L.proj.tm, p, s)) return 1; // proj + residual, vit.cpp:868-873
+            if (launch_gemm(e, resid_epilogue(e), e->tmA_D, L.proj.tm, p, s)) return 1; // proj + residual, vit.cpp:868-873
         }
         if (tap && tap_f32(taps->x1, e->X, (size_t)T * D, s)) return 1;
         {
@@ -867,9 +891,9 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
         {
             GemmParams p{};
-            p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X;
+            p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X; p.gamma = L.ls2;
             ProfScope ps(e, PK_FC2, 2.0 * p.M * p.N * p.K, s);
-            if (launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
+            if (launch_gemm(e, resid_epilogue(e), e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
         }
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
     }
@@ -899,17 +923,20 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     if (taps && tap_f32(taps->x_final, e->X, (size_t)T * D, s)) return 1;
 
     // pool (token 0; the first 25 tokens for ViTSTR, vitstr.cpp:864-883) + final LN + head + soft-max + top-k
-    // (vit.cpp:910-933, 1047-1057); one row of the head GEMM / one soft-max per pooled token
+    // (vit.cpp:910-933, 1047-1057); one row of the head GEMM / one soft-max per pooled token.  DINOv2 (arch.pool = 1): one row of
+    // [LN(token 0) || mean of LN(patches)] per image
     const int TH = e->head_tokens, R = B * TH;
-    if (launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->CLS16, R, s, TH, (size_t)N * D)) return 1;
-    if (taps && tap_f16(taps->final_ln, e->CLS16, (size_t)R * D, s)) return 1;
+    if (e->arch.pool ? launch_pool<__half, true>(e, e->CLS16, B, s)
+                     : launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->CLS16, R, s, TH, (size_t)N * D))
+        return 1;
+    if (taps && tap_f16(taps->final_ln, e->CLS16, (size_t)R * e->KH, s)) return 1;
     // internal logits rows have pitch Cp (num_classes padded to 4; the padded W rows are TMA zero fill, the padded bias is 0);
     // a caller's dense [rows][num_classes] buffer is written directly when the two coincide, else through a 2-D copy
     const int Cp = e->Cp;
     float *lg = (d_logits && Cp == C) ? d_logits : e->d_logits;
     {
         GemmParams p{};
-        p.M = R; p.N = Cp; p.K = D; p.bias = e->head.b; p.out = lg; p.ldo = Cp;
+        p.M = R; p.N = Cp; p.K = e->KH; p.bias = e->head.b; p.out = lg; p.ldo = Cp;
         ProfScope ps(e, PK_HEAD, 2.0 * p.M * C * p.K, s);
         if (launch_gemm(e, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
     }
@@ -955,6 +982,21 @@ int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_
         return fail("features: dtype %d unknown", req->dtype);
     };
     if (emit(d_tokens, B * N, N)) return 1;
+    if (d_prelogits && e->arch.pool)
+    {
+        // DINOv2: [token 0 || mean of the patch rows] per image, through the final LayerNorm or not
+        ProfScope ps(e, PK_LN, 0.0, s);
+        switch (req->dtype * 2 + (req->norm ? 1 : 0))
+        {
+        case 0: return launch_pool<float, false>(e, (float *)d_prelogits, B, s);
+        case 1: return launch_pool<float, true>(e, (float *)d_prelogits, B, s);
+        case 2: return launch_pool<__half, false>(e, (__half *)d_prelogits, B, s);
+        case 3: return launch_pool<__half, true>(e, (__half *)d_prelogits, B, s);
+        case 4: return launch_pool<__nv_bfloat16, false>(e, (__nv_bfloat16 *)d_prelogits, B, s);
+        case 5: return launch_pool<__nv_bfloat16, true>(e, (__nv_bfloat16 *)d_prelogits, B, s);
+        }
+        return fail("features: dtype %d unknown", req->dtype);
+    }
     return emit(d_prelogits, B * TH, TH);
 }
 
@@ -1069,12 +1111,34 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         hp->patch_size < 1 || hp->patch_size > 64 || hp->img_size < hp->patch_size || hp->img_size > 4096 || n < 1)
         return fail("invalid hyper-parameters (hidden %d, layers %d, heads %d, classes %d, patch %d, img %d)", hp->hidden_size,
                     hp->num_hidden_layers, hp->num_attention_heads, hp->num_classes, hp->patch_size, hp->img_size);
-    const vitb200_arch ar = arch ? *arch : vitb200_arch{0, 0};
+    const vitb200_arch ar = arch ? *arch : vitb200_arch{};
     if (ar.pre_norm != 0 && ar.pre_norm != 1) return fail("vitb200_arch.pre_norm = %d out of range (0 none, 1 LayerNorm 'norm_pre')", ar.pre_norm);
     if (ar.activation < 0 || ar.activation > 2)
         return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu)", ar.activation);
+    if (ar.layer_scale != 0 && ar.layer_scale != 1)
+        return fail("vitb200_arch.layer_scale = %d out of range (0 none, 1 LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma')", ar.layer_scale);
+    if (ar.reg_tokens < 0 || ar.reg_tokens > VB_MAX_REG_TOKENS)
+        return fail("vitb200_arch.reg_tokens = %d out of range (0..%d register tokens)", ar.reg_tokens, VB_MAX_REG_TOKENS);
+    if (ar.pool != 0 && ar.pool != 1) return fail("vitb200_arch.pool = %d out of range (0 token, 1 cls_patch_mean)", ar.pool);
     if (ar.pre_norm && (!find_tensor(t, n, "norm_pre.weight") || !find_tensor(t, n, "norm_pre.bias")))
         return fail("vitb200_arch.pre_norm = 1 needs the tensors 'norm_pre.weight' and 'norm_pre.bias'");
+    for (int i = 0; ar.layer_scale && i < hp->num_hidden_layers; ++i)
+        for (const char *g : {"ls1", "ls2"})
+        {
+            const std::string name = "blocks." + std::to_string(i) + "." + g + ".gamma";
+            if (!find_tensor(t, n, name)) return fail("vitb200_arch.layer_scale = 1 needs the tensor '%s'", name.c_str());
+        }
+    if (ar.reg_tokens > 0 && !find_tensor(t, n, "reg_token"))
+        return fail("vitb200_arch.reg_tokens = %d needs the tensor 'reg_token'", ar.reg_tokens);
+    if (ar.pool && head_tokens != 1) return fail("vitb200_arch.pool = 1 needs head_tokens = 1 (got %d)", head_tokens);
+    {
+        // the head's K: the pooled row it reads is D wide, or 2 D with the class-plus-patch-mean pool
+        const vitb200_tensor *hw = find_tensor(t, n, "head.weight");
+        const int64_t k = (ar.pool ? 2 : 1) * (int64_t)hp->hidden_size;
+        if (hw && dim_of(hw, 0) != k)
+            return fail("vitb200_arch.pool = %d needs 'head.weight' with K = %lld (%s), got [%lld, %lld]", ar.pool, (long long)k,
+                        ar.pool ? "2 D: class token || patch mean" : "D", (long long)dim_of(hw, 0), (long long)dim_of(hw, 1));
+    }
     // input channels from the patch kernel [P, P, C, D] (vit.cpp:515; C = 1 in vitstr.cpp:482)
     const vitb200_tensor *pw = find_tensor(t, n, "patch_embed.proj.weight");
     const int64_t per_c = (int64_t)hp->hidden_size * hp->patch_size * hp->patch_size;
@@ -1088,7 +1152,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (!patchify_supports(hp->patch_size, in_chans))
         return fail("patch size %d not supported for %d-channel input (%s)", hp->patch_size, in_chans, patchify_sizes(in_chans));
     if (hp->hidden_size > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", hp->hidden_size, LN_MAX_HIDDEN);
-    const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + 1;
+    const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + 1 + ar.reg_tokens;
     if (n_tokens > ATT_MAX_TOKENS)
         return fail("%d tokens not supported (max %d: K and V of one attention head must fit in shared memory)", n_tokens, ATT_MAX_TOKENS);
     cudaDeviceProp prop;
@@ -1109,16 +1173,24 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     const int D = hp->hidden_size, P = hp->patch_size;
     e->G = hp->img_size / P;
     e->NP = e->G * e->G;
-    e->N = e->NP + 1;
+    e->N = e->NP + 1 + ar.reg_tokens;
     e->C = in_chans;
     e->head_tokens = head_tokens;
+    e->KH = (ar.pool ? 2 : 1) * hp->hidden_size;
     e->Cp = (hp->num_classes + 3) / 4 * 4;
     e->KP = e->C * P * P;
     e->KPp = (e->KP + 63) / 64 * 64;
     if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
 
     // ---- weights (names: reference vit.cpp:518-579)
-    if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls)) return 1;
+    // the prefix rows [cls_token; reg_token] as one array, the cls_rows_kernel's source
+    if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls, (int64_t)(1 + ar.reg_tokens) * D)) return 1;
+    if (ar.reg_tokens > 0)
+    {
+        float *reg = nullptr;
+        if (upload_f32(e, t, n, "reg_token", D, ar.reg_tokens, 1, 1, &reg)) return 1;
+        CUDA_TRY(cudaMemcpy(e->cls + D, reg, (size_t)ar.reg_tokens * D * sizeof(float), cudaMemcpyDeviceToDevice));
+    }
     if (upload_f32(e, t, n, "pos_embed", D, e->N, 1, 1, &e->pos)) return 1;
     if (upload_linear(e, t, n, "patch_embed.proj.weight", "patch_embed.proj.bias", D, e->KP, e->KPp, &e->patch, P)) return 1;
     if (ar.pre_norm && (upload_f32(e, t, n, "norm_pre.weight", D, 1, 1, 1, &e->npre_w) || upload_f32(e, t, n, "norm_pre.bias", D, 1, 1, 1, &e->npre_b)))
@@ -1136,9 +1208,11 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
             upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, D, &L.fc1, 0, fp8) ||
             upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 4 * D, &L.fc2))
             return 1;
+        if (ar.layer_scale && (upload_f32(e, t, n, p + "ls1.gamma", D, 1, 1, 1, &L.ls1) || upload_f32(e, t, n, p + "ls2.gamma", D, 1, 1, 1, &L.ls2)))
+            return 1;
     }
     if (upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b)) return 1;
-    if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, D, D, &e->head)) return 1;
+    if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, e->KH, e->KH, &e->head)) return 1;
 
     // ---- activation arena
     const size_t B = (size_t)max_batch, T = B * e->N;
@@ -1150,7 +1224,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     const size_t R = B * (size_t)e->head_tokens;                        // classifier rows: pooled tokens of all images
     const size_t img_elems = (size_t)e->C * hp->img_size * hp->img_size; // per image
     if (dev_alloc(e, &e->X, T * D) || dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->H16, h16) ||
-        dev_alloc(e, &e->CLS16, R * D) || dev_alloc(e, &e->d_logits, R * e->Cp))
+        dev_alloc(e, &e->CLS16, R * e->KH) || dev_alloc(e, &e->d_logits, R * e->Cp))
         return 1;
     // soft-max working row: dynamic shared memory up to the per-CTA limit, global scratch beyond it
     if ((size_t)hp->num_classes * sizeof(float) > kSoftmaxSmemMax && dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return 1;
@@ -1179,7 +1253,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
                     : make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_A_BOX_ROWS});
     };
     if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, 4 * (cuuint64_t)D) || a_map(&e->tmA_P, e->PA, B * e->NP, e->KPp) ||
-        a_map(&e->tmA_C, e->CLS16, R, D))
+        a_map(&e->tmA_C, e->CLS16, R, e->KH))
         return 1;
     if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
@@ -1509,15 +1583,16 @@ static int stage_images(vitb200_engine *e, const Slot &sl, const float *images, 
 static int features_to_host(vitb200_engine *e, const float *d_images, int batch, const vitb200_features_req *req, void *tokens, void *prelogits)
 {
     const size_t D = e->hp.hidden_size, N = e->N, TH = e->head_tokens, esz = features_elem_bytes(req);
-    const size_t tok_bytes = (size_t)batch * N * D * esz, pre_bytes = (size_t)batch * TH * D * esz;
+    // pooled rows per image: head_tokens rows of D, or one row of 2 D with arch.pool = 1 (always a kernel's output)
+    const size_t tok_bytes = (size_t)batch * N * D * esz, pre_bytes = (size_t)batch * TH * e->KH * esz;
     cudaStream_t s = e->stream;
-    const bool copy = !req->norm && req->dtype == 0;
+    const bool copy = !req->norm && req->dtype == 0, pre_copy = copy && !e->arch.pool;
     uint8_t *stage = reinterpret_cast<uint8_t *>(e->H16);
     void *d_tok = tokens && !copy ? stage : nullptr;
-    void *d_pre = prelogits && !copy ? stage + tok_bytes : nullptr;
+    void *d_pre = prelogits && !pre_copy ? stage + tok_bytes : nullptr;
     if (run_features_graphed(e, d_images, batch, req, d_tok, d_pre, s)) return 1;
     if (tokens) CUDA_TRY(cudaMemcpyAsync(tokens, copy ? (const void *)e->X : d_tok, tok_bytes, cudaMemcpyDeviceToHost, s));
-    if (prelogits && copy)
+    if (prelogits && pre_copy)
         CUDA_TRY(cudaMemcpy2DAsync(prelogits, TH * D * 4, e->X, N * D * 4, TH * D * 4, (size_t)batch, cudaMemcpyDeviceToHost, s));
     else if (prelogits)
         CUDA_TRY(cudaMemcpyAsync(prelogits, d_pre, pre_bytes, cudaMemcpyDeviceToHost, s));
@@ -1833,35 +1908,53 @@ int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const 
     });
 }
 
+// vitb200_test_gemm and vitb200_test_gemm_layer_scale: gamma is the LayerScale epilogue's [N] (NULL for every other epilogue)
+static int test_gemm_impl(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
+                          const float *gamma, const float *resid, float *out)
+{
+    if (!A || !W || !bias || !out) return fail("null argument");
+    if (K % 8 != 0) return fail("K must be a multiple of 8");
+    if (gemm_epi_resid(epilogue) && !resid) return fail("resid required");
+    if ((epilogue == EPI_BIAS_SCALE_RESID_F32) != (gamma != nullptr))
+        return fail("gamma goes with the LayerScale epilogue %d only (vitb200_test_gemm_layer_scale)", EPI_BIAS_SCALE_RESID_F32);
+    EnginePtr owner;
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
+    const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
+                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16;
+    const size_t MN = (size_t)M * N;
+    __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
+    float *dB = nullptr, *o32 = nullptr;
+    if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dB, bias, N)) return 1;
+    if (f16out && (dev_alloc(e, &hi, MN) || (epilogue == EPI_BIAS_F16_HILO && dev_alloc(e, &lo, MN)))) return 1;
+    // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
+    if (!f16out && (gemm_epi_resid(epilogue) ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
+    float *dG = nullptr;
+    if (gamma && upload(e, &dG, gamma, N)) return 1;
+    CUtensorMap tA, tB;
+    const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
+    if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dA, {Ku, Mu}, {2 * Ku}, {GEMM_BK, GEMM_A_BOX_ROWS}) ||
+        make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dW, {Ku, Nu}, {2 * Ku}, {GEMM_BK, GEMM_BN}))
+        return 1;
+    GemmParams p{};
+    p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = N; p.resid = o32; p.gamma = dG;
+    if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
+    // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
+    return f16out ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
+}
+
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
                       const float *resid, float *out)
 {
+    return guarded(__func__, [&] { return test_gemm_impl(device, M, N, K, epilogue, A, W, bias, nullptr, resid, out); });
+}
+
+int vitb200_test_gemm_layer_scale(int device, int M, int N, int K, const uint16_t *A, const uint16_t *W, const float *bias,
+                                  const float *gamma, const float *resid, float *out)
+{
     return guarded(__func__, [&]() -> int {
-        if (!A || !W || !bias || !out) return fail("null argument");
-        if (K % 8 != 0) return fail("K must be a multiple of 8");
-        if (epilogue == EPI_BIAS_RESID_F32 && !resid) return fail("resid required");
-        EnginePtr owner;
-        if (scratch_engine(device, owner)) return 1;
-        vitb200_engine *e = owner.get();
-        const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
-                            epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16;
-        const size_t MN = (size_t)M * N;
-        __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
-        float *dB = nullptr, *o32 = nullptr;
-        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dB, bias, N)) return 1;
-        if (f16out && (dev_alloc(e, &hi, MN) || (epilogue == EPI_BIAS_F16_HILO && dev_alloc(e, &lo, MN)))) return 1;
-        // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
-        if (!f16out && (epilogue == EPI_BIAS_RESID_F32 ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
-        CUtensorMap tA, tB;
-        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
-        if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dA, {Ku, Mu}, {2 * Ku}, {GEMM_BK, GEMM_A_BOX_ROWS}) ||
-            make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dW, {Ku, Nu}, {2 * Ku}, {GEMM_BK, GEMM_BN}))
-            return 1;
-        GemmParams p{};
-        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = N; p.resid = o32;
-        if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
-        // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
-        return f16out ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
+        if (!gamma || !resid) return fail("null argument");
+        return test_gemm_impl(device, M, N, K, EPI_BIAS_SCALE_RESID_F32, A, W, bias, gamma, resid, out);
     });
 }
 
@@ -2052,8 +2145,12 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
     hp.patch_size = i32(g.patch_size); hp.img_size = i32(g.img_size); hp.ftype = i32(g.ftype); hp.eps = g.eps;
     if (hp.num_hidden_layers < 1 || hp.num_hidden_layers > 4096) return fail("invalid model file '%s' (num_hidden_layers %d)", path, hp.num_hidden_layers);
     if (g.pre_norm != 0 && g.pre_norm != 1) return fail("invalid model file '%s' (vit.pre_norm %lld)", path, (long long)g.pre_norm);
-    const vitb200_arch arch{(int32_t)g.pre_norm, g.activation};
-    const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm; // vit.cpp:697, plus norm_pre.weight / .bias
+    if (g.layer_scale != 0 && g.layer_scale != 1) return fail("invalid model file '%s' (vit.layer_scale %lld)", path, (long long)g.layer_scale);
+    if (g.reg_tokens < 0 || g.reg_tokens > VB_MAX_REG_TOKENS)
+        return fail("invalid model file '%s' (vit.reg_tokens %lld, 0..%d)", path, (long long)g.reg_tokens, VB_MAX_REG_TOKENS);
+    const vitb200_arch arch{(int32_t)g.pre_norm, g.activation, (int32_t)g.layer_scale, (int32_t)g.reg_tokens, g.pool};
+    // vit.cpp:697, plus norm_pre.weight / .bias, the ls1 / ls2 gammas of every block and reg_token
+    const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm + 2 * hp.num_hidden_layers * arch.layer_scale + (arch.reg_tokens > 0);
     if ((int)g.tensors.size() != expected) return fail("model file has %d tensors, but %d tensors were expected", (int)g.tensors.size(), expected);
     std::vector<vitb200_tensor> ts(g.tensors.size());
     for (size_t i = 0; i < g.tensors.size(); ++i)

@@ -62,6 +62,7 @@ enum GemmEpilogue
                             // vit.cpp:848,858; hi + lo lets the f16 tensor cores reproduce that with split-precision MMAs)
     EPI_BIAS_GELU_ERF_F16 = 7,   // out f16 = f16(gelu_erf(acc + bias)), x in f32 without rounding to f16 first   (fc1 of LAION CLIP)
     EPI_BIAS_QUICK_GELU_F16 = 8, // out f16 = f16(quick_gelu(acc + bias)), likewise                               (fc1 of OpenAI CLIP)
+    EPI_BIAS_SCALE_RESID_F32 = 9, // out f32 = f32((acc + bias) * gamma[n]) + resid: LayerScale, HF's order    (proj, fc2 of DINOv2)
 };
 
 struct GemmParams
@@ -79,6 +80,7 @@ struct GemmParams
     int np, ntok;       // EPI_PATCH_F32: patches / tokens per image
     const float *a_scale; // GEMM_OP_E4M3: [M] f32, the scale of each A row
     float w_scale;        // GEMM_OP_E4M3: the scale of W
+    const float *gamma;   // EPI_BIAS_SCALE_RESID_F32: [N] f32, the LayerScale of each output column
 };
 
 constexpr int GEMM_BM = 128; // rows of a tile
@@ -103,6 +105,7 @@ struct GemmCfg
     static constexpr int kSmemLimit = 232448;            // 227 KB per CTA
     static constexpr int SMEM_BYTES = 1024 /*align slack*/ + kStages * (A_BYTES + B_BYTES) + 2 * kStageBytes + 256 /*barriers*/;
     static_assert(SMEM_BYTES + 2 * GEMM_BN * 4 /*s_bias*/ <= kSmemLimit, "exceeds the 227 KB per-CTA shared memory limit");
+    static_assert(STAGES != 6 || SMEM_BYTES + 2 * GEMM_BN * 4 + 2 * 64 * 4 /*s_bias, s_gamma*/ <= kSmemLimit, "LayerScale: exceeds 227 KB");
 };
 
 // GELU, tanh form (the reference's formula, ggml.c:1418-1424) on an f16-valued input, evaluated in f32 as
@@ -133,8 +136,11 @@ __device__ __forceinline__ float quick_gelu_f32(float x)
 __host__ __device__ constexpr bool gemm_epi_staged(int epi)
 {
     return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32 ||
-           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16;
+           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32;
 }
+
+// Epilogues that add the residual stream (loaded into the staging buffer with TMA)
+__host__ __device__ constexpr bool gemm_epi_resid(int epi) { return epi == EPI_BIAS_RESID_F32 || epi == EPI_BIAS_SCALE_RESID_F32; }
 
 // Staged-epilogue geometry: a warpgroup's 128 x 128 result leaves in passes of one 64-row half x kPassCols columns; a pass is
 // kColBoxes boxes of 64 rows x 128 B (64 f16 or 32 f32 columns) per output tensor (hi and lo for EPI_BIAS_F16_HILO) and fills the
@@ -162,7 +168,7 @@ struct GemmStage
 
 // tmOut: the store map of out (f16: box 64 columns x 64 rows, 2-D [M][N] or, head-major, 3-D {64, M, N / 64 planes}; f32: box
 // 32 columns x 64 rows over [M][N]), SWIZZLE_128B.  tmAux: the same map over out2 (EPI_BIAS_F16_HILO) or the load map of resid
-// (EPI_BIAS_RESID_F32).  Both unused by the register epilogues.
+// (EPI_BIAS_RESID_F32, EPI_BIAS_SCALE_RESID_F32).  Both unused by the register epilogues.
 template <int EPI, int STAGES, int OP = GEMM_OP_F16>
 __global__ void __launch_bounds__(384, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmOut,
@@ -188,7 +194,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     auto empty_bar = [&](int s) { return bars + 8u * (kStages + s); };
     auto resid_bar = [&](int cw) { return bars + 8u * (2 * kStages + cw); };
     using St = GemmStage<EPI, STAGES>;
-    // EPI_BIAS_RESID_F32: TMA-load the residual of one pass (64 rows from `row`, the column boxes from c0 that start inside N) into
+    // residual epilogues: TMA-load the residual of one pass (64 rows from `row`, the column boxes from c0 that start inside N) into
     // the staging buffer `dst` of warpgroup cw, completing on resid_bar(cw); partial boxes are zero-filled and count in full
     auto resid_load = [&](uint32_t dst, int c0, int row, int cw) {
         const int ncb = min(St::kColBoxes, (p.N - c0 + St::kBoxCols - 1) / St::kBoxCols);
@@ -212,7 +218,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if constexpr (kStaged)
         {
             ptx::prefetch_tensormap(&tmOut);
-            if constexpr (EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_RESID_F32) ptx::prefetch_tensormap(&tmAux);
+            if constexpr (EPI == EPI_BIAS_F16_HILO || gemm_epi_resid(EPI)) ptx::prefetch_tensormap(&tmAux);
         }
         for (int s = 0; s < kStages; ++s)
         {
@@ -240,7 +246,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             {
                 const unsigned m_blk = u / n_pairs;
                 const int m0 = (int)m_blk * GEMM_BM, n0 = (int)(2 * (u - m_blk * n_pairs) + rank) * GEMM_BN;
-                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                if constexpr (gemm_epi_resid(EPI))
                 {
                     // the residual rows are read once, by the epilogue: start pulling them into L2 while the tile's main loop runs
                     for (int h = 0; h < 2; ++h)
@@ -289,7 +295,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (tid == 0)
             {
                 ptx::tma_store_wait_read<0>();
-                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                if constexpr (gemm_epi_resid(EPI))
                     if (n0 < p.N) resid_load(sStage + cw * Cfg::kStageBytes, n0, m0, cw);
             }
         }
@@ -364,13 +370,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                         row_scale[h] = row < p.M ? __fmul_rn(__ldg(p.a_scale + row), p.w_scale) : 0.f;
                     }
                 }
+                // LayerScale gamma of the pass's columns (zero past N): staged in shared memory per pass where a pass is at most 64
+                // columns (6-stage ring; a 1 KB whole-tile array beside s_bias would take the CTA past the 227 KB of shared memory by
+                // 256 bytes, and loads held in registers across the pass spill there), read through L1 at its use otherwise (5-stage
+                // ring, 128-column passes).  The end-of-pass barrier below orders these writes after the previous pass's reads.
+                constexpr bool kGammaSmem = EPI == EPI_BIAS_SCALE_RESID_F32 && St::kPassCols <= 64;
+                __shared__ __align__(16) float s_gamma[2][kGammaSmem ? St::kPassCols : 1];
+                if constexpr (kGammaSmem)
+                    if (tid < St::kPassCols) s_gamma[cw][tid] = c0 + tid < p.N ? __ldg(p.gamma + c0 + tid) : 0.f;
                 if (ps > 0 && tid == 0)
                 {
                     if (ps >= St::kSlots) ptx::tma_store_wait_read<St::kSlots - 1>(); // the stores of the pass that used buf have read it
-                    if constexpr (EPI == EPI_BIAS_RESID_F32) resid_load(buf, c0, m0 + 64 * hm, cw);
+                    if constexpr (gemm_epi_resid(EPI)) resid_load(buf, c0, m0 + 64 * hm, cw);
                 }
                 ptx::named_bar_sync(kBarWg + cw, 128); // pass 0: s_bias[cw] is written
-                if constexpr (EPI == EPI_BIAS_RESID_F32)
+                if constexpr (gemm_epi_resid(EPI))
                 {
                     ptx::mbar_wait(resid_bar(cw), resid_ph);
                     resid_ph ^= 1;
@@ -380,6 +394,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 {
                     const int j = cg * (St::kPassCols / 8) + jj; // 8-column group of the tile
                     const float2 b = *reinterpret_cast<const float2 *>(&s_bias[cw][8 * j + 2 * q]);
+                    float2 g = make_float2(0.f, 0.f); // LayerScale: the column pair's gamma (columns past N are never stored)
+                    if constexpr (kGammaSmem) g = *reinterpret_cast<const float2 *>(&s_gamma[cw][8 * jj + 2 * q]);
+                    else if constexpr (EPI == EPI_BIAS_SCALE_RESID_F32)
+                        if (n0 + 8 * j + 2 * q < p.N) g = __ldg(reinterpret_cast<const float2 *>(p.gamma + n0 + 8 * j + 2 * q));
 #pragma unroll
                     for (int h = 0; h < 2; ++h)
                     {
@@ -414,6 +432,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             {
                                 const float2 r = ptx::ld_shared_v2_f32(a); // (mul_mat + b) + inpL, vit.cpp:869,873
                                 ptx::st_shared_v2_f32(a, __fadd_rn(x0, r.x), __fadd_rn(x1, r.y));
+                            }
+                            else if constexpr (EPI == EPI_BIAS_SCALE_RESID_F32)
+                            {
+                                const float2 r = ptx::ld_shared_v2_f32(a); // x + gamma * (mul_mat + b), HF Dinov2Layer's order
+                                ptx::st_shared_v2_f32(a, __fadd_rn(__fmul_rn(x0, g.x), r.x), __fadd_rn(__fmul_rn(x1, g.y), r.y));
                             }
                             else ptx::st_shared_v2_f32(a, x0, x1);
                         }

@@ -9,6 +9,9 @@
 //     vit.layer_norm_eps (float32, default 1e-6)           vit.id2label (array of strings, index = class id; optional)
 //     vit.pre_norm (bool or integer, default 0: 1 = a LayerNorm 'norm_pre' before block 0, as in CLIP towers)
 //     vit.activation (string, default "gelu_tanh"; "gelu_erf" or "quick_gelu": the MLP activation)
+//     vit.layer_scale (bool or integer, default 0: 1 = LayerScale gammas 'blocks.{i}.ls1.gamma' / 'ls2.gamma', as in DINOv2)
+//     vit.reg_tokens (integer, default 0: register tokens 'reg_token' after the class token)
+//     vit.pool (string, default "token"; "cls_patch_mean": the head reads the class token || the mean of the patch tokens)
 // Layout (gguf.md): header {magic "GGUF", u32 version, u64 n_tensors, u64 n_kv}, n_kv x {string key, u32 type, value},
 // n_tensors x {string name, u32 n_dims, u64 ne[n_dims], u32 type, u64 offset}, padding to the alignment, tensor data (offsets
 // relative to the start of the data section).  Strings are {u64 length, bytes}.
@@ -35,6 +38,8 @@ struct GgufModel
     float eps = 1e-6f;
     int64_t pre_norm = 0; // vit.pre_norm (vitb200_arch.pre_norm; the loader checks the range)
     int32_t activation = 0; // vit.activation: 0 gelu_tanh, 1 gelu_erf, 2 quick_gelu (vitb200_arch.activation)
+    int64_t layer_scale = 0, reg_tokens = 0; // vit.layer_scale, vit.reg_tokens (vitb200_arch; the loader checks the ranges)
+    int32_t pool = 0;       // vit.pool: 0 token, 1 cls_patch_mean (vitb200_arch.pool)
     std::map<int, std::string> labels;
     std::vector<GgufTensor> tensors;
     std::string error;
@@ -97,6 +102,12 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
                 else if (v == "quick_gelu") m.activation = 2;
                 else return fail("unknown vit.activation '" + v + "' (gelu_tanh, gelu_erf or quick_gelu)");
             }
+            else if (key == "vit.pool")
+            {
+                if (v == "token") m.pool = 0;
+                else if (v == "cls_patch_mean") m.pool = 1;
+                else return fail("unknown vit.pool '" + v + "' (token or cls_patch_mean)");
+            }
         }
         else if (vt == 9) // array
         {
@@ -149,6 +160,8 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             else if (key == "vit.image_size" || key == "vit.img_size") m.img_size = iv;
             else if (key == "vit.layer_norm_eps") m.eps = (float)fv;
             else if (key == "vit.pre_norm") m.pre_norm = iv;
+            else if (key == "vit.layer_scale") m.layer_scale = iv;
+            else if (key == "vit.reg_tokens") m.reg_tokens = iv;
         }
     }
     if (!arch.empty() && arch != "vit") return fail("GGUF architecture is '" + arch + "', expected 'vit'");

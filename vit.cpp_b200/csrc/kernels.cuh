@@ -1,7 +1,8 @@
 // kernels.cuh -- the non-GEMM kernels of the forward path (all HBM-bound except attention):
 //   patchify_f16_kernel      reference im2col for stride==kernel conv (ggml.c:11528-11608) without the buffer
 //                            reshuffle: pixels HWC f32 -> f16 patch rows, K order c*P*P + ky*P + kx
-//   cls_rows_kernel          token 0 = cls_token + pos_embed[0]                      (vit.cpp:794-797)
+//   cls_rows_kernel          token 0 = cls_token + pos_embed[0] (vit.cpp:794-797), and the register tokens after it
+//   cls_patch_mean_kernel    DINOv2's classifier input: LN(token 0) || the mean of LN(patch rows), one CTA per image
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
 //                            and un-normalised forms write the encoder features (vitb200_features), its e4m3 form the FP8 A operand
 //   layernorm_inplace_kernel the same arithmetic in place on f32 rows (the pre-norm of CLIP towers)
@@ -96,13 +97,15 @@ __global__ void patchify16_warp_kernel(const float *__restrict__ img, __half *__
     }
 }
 
-// x[b*ntok + 0][:] = cls[:] + pos[0][:]
-__global__ void cls_rows_kernel(float *__restrict__ x, const float *__restrict__ cls, const float *__restrict__ pos, int B, int ntok, int D)
+// The prefix rows r = 0 .. rows-1 of every image: x[b*ntok + r][:] = prefix[r][:] + pos[r][:], prefix = [cls_token; reg_token]
+// (rows = 1 + vitb200_arch.reg_tokens; the patch GEMM writes the rows after them)
+__global__ void cls_rows_kernel(float *__restrict__ x, const float *__restrict__ prefix, const float *__restrict__ pos, int B, int rows, int ntok,
+                                int D)
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * D) return;
-    const int b = i / D, o = i - b * D;
-    x[(size_t)b * ntok * D + o] = __fadd_rn(cls[o], pos[o]);
+    if (i >= B * rows * D) return;
+    const int b = i / (rows * D), o = i - b * rows * D; // o = r D + column
+    x[(size_t)b * ntok * D + o] = __fadd_rn(prefix[o], pos[o]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -268,6 +271,134 @@ __global__ void layernorm_inplace_kernel(float *x, const float *__restrict__ w, 
     ptx::grid_dep_launch();
     ptx::grid_dep_wait();
     layernorm_row_warp<MAXV, float, true>(x, (size_t)D, rows, 0, w, b, x, rows, D, eps, nullptr);
+}
+
+// ------------------------------------------------------------------------------------------------
+// DINOv2's classifier input (vitb200_arch.pool = 1): per image, y[0 .. D) = LN(token 0) and y[D .. 2 D) = the mean over the patch rows
+// first_patch .. ntok-1 of LN(row) (the register rows between them are left out), LN = the row-per-warp LayerNorm's arithmetic above
+// (NORM = false: the rows as they are).  One CTA of 8 warps per image: warp w normalises patch rows w, w + 8, ... and keeps its column
+// sums in registers in that order; the eight partial sums then meet in shared memory and are added warp 0 first, 7 last, and divided
+// by the patch count.  No atomics and nothing shared between images: an image gives the same bits alone as in any batch.
+// OutT: __half (the head GEMM's A operand [B][2 D]), float or __nv_bfloat16 (the features' prelogits).  Dynamic shared memory 8 D floats.
+constexpr int POOL_WARPS = 8;
+
+template <typename OutT>
+__device__ __forceinline__ OutT to_out(float v)
+{
+    if constexpr (std::is_same<OutT, __half>::value) return __float2half_rn(v);
+    else if constexpr (std::is_same<OutT, __nv_bfloat16>::value) return __float2bfloat16_rn(v);
+    else return v;
+}
+
+// One row of D floats into a warp's registers, normalised as layernorm_row_warp normalises it (NORM = false: as it is): lane l holds
+// float4 l + 32 j of the row in o[j]
+template <int MAXV, bool NORM>
+__device__ __forceinline__ void layernorm_row_regs(const float *__restrict__ xrow, const float *__restrict__ w, const float *__restrict__ b,
+                                                   int D, float eps, int lane, float4 (&o)[MAXV])
+{
+    const int nvec = D >> 2;
+    const float4 *xr = reinterpret_cast<const float4 *>(xrow);
+    float sum = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j)
+    {
+        const int i = lane + 32 * j;
+        o[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (i < nvec)
+        {
+            o[j] = xr[i];
+            sum += (o[j].x + o[j].y) + (o[j].z + o[j].w);
+        }
+    }
+    if constexpr (NORM)
+    {
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, s);
+        const float mean = sum / (float)D;
+        float sq = 0.f;
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            const int i = lane + 32 * j;
+            if (i < nvec)
+            {
+                o[j].x -= mean; o[j].y -= mean; o[j].z -= mean; o[j].w -= mean;
+                sq += (o[j].x * o[j].x + o[j].y * o[j].y) + (o[j].z * o[j].z + o[j].w * o[j].w);
+            }
+        }
+#pragma unroll
+        for (int s = 16; s > 0; s >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, s);
+        const float scale = 1.0f / sqrtf(sq / (float)D + eps);
+        const float4 *w4 = reinterpret_cast<const float4 *>(w);
+        const float4 *b4 = reinterpret_cast<const float4 *>(b);
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            const int i = lane + 32 * j;
+            if (i < nvec)
+            {
+                const float4 ww = __ldg(w4 + i), bb = __ldg(b4 + i);
+                o[j].x = __fadd_rn(__fmul_rn(__fmul_rn(o[j].x, scale), ww.x), bb.x);
+                o[j].y = __fadd_rn(__fmul_rn(__fmul_rn(o[j].y, scale), ww.y), bb.y);
+                o[j].z = __fadd_rn(__fmul_rn(__fmul_rn(o[j].z, scale), ww.z), bb.z);
+                o[j].w = __fadd_rn(__fmul_rn(__fmul_rn(o[j].w, scale), ww.w), bb.w);
+            }
+        }
+    }
+}
+
+template <int MAXV, typename OutT = __half, bool NORM = true>
+__global__ void __launch_bounds__(POOL_WARPS * 32)
+cls_patch_mean_kernel(const float *__restrict__ x, int ntok, int first_patch, const float *__restrict__ w, const float *__restrict__ b,
+                      OutT *__restrict__ y, int D, float eps)
+{
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
+    extern __shared__ float4 s_part[]; // [POOL_WARPS][D / 4]
+    const int img = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nvec = D >> 2;
+    const float *xi = x + (size_t)img * ntok * D;
+    OutT *yi = y + (size_t)img * 2 * D;
+    float4 o[MAXV], acc[MAXV];
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int r = first_patch + warp; r < ntok; r += POOL_WARPS)
+    {
+        layernorm_row_regs<MAXV, NORM>(xi + (size_t)r * D, w, b, D, eps, lane, o);
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            acc[j].x = __fadd_rn(acc[j].x, o[j].x); acc[j].y = __fadd_rn(acc[j].y, o[j].y);
+            acc[j].z = __fadd_rn(acc[j].z, o[j].z); acc[j].w = __fadd_rn(acc[j].w, o[j].w);
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j)
+        if (lane + 32 * j < nvec) s_part[warp * nvec + lane + 32 * j] = acc[j];
+    if (warp == 0)
+    {
+        // the class row, under the other warps' wait at the barrier
+        layernorm_row_regs<MAXV, NORM>(xi, w, b, D, eps, lane, o);
+#pragma unroll
+        for (int j = 0; j < MAXV; ++j)
+        {
+            const int i = lane + 32 * j;
+            if (i < nvec)
+            {
+                yi[4 * i] = to_out<OutT>(o[j].x); yi[4 * i + 1] = to_out<OutT>(o[j].y);
+                yi[4 * i + 2] = to_out<OutT>(o[j].z); yi[4 * i + 3] = to_out<OutT>(o[j].w);
+            }
+        }
+    }
+    __syncthreads();
+    const float count = (float)(ntok - first_patch);
+    const float *part = reinterpret_cast<const float *>(s_part);
+    for (int c = threadIdx.x; c < D; c += POOL_WARPS * 32)
+    {
+        float s = part[c];
+#pragma unroll
+        for (int k = 1; k < POOL_WARPS; ++k) s = __fadd_rn(s, part[k * D + c]);
+        yi[D + c] = to_out<OutT>(__fdiv_rn(s, count));
+    }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -16,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from .ggml_file import ACTIVATIONS  # vitb200_arch.activation -> name (the GGUF key vit.activation)
+from .ggml_file import ACTIVATIONS, POOLS  # vitb200_arch.activation / .pool -> name (the GGUF keys vit.activation / vit.pool)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
@@ -34,8 +34,10 @@ class Hparams(C.Structure):
 
 
 class Arch(C.Structure):
-    """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ACTIVATIONS."""
-    _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32)]
+    """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ACTIVATIONS, layer_scale 0 / 1,
+    reg_tokens 0..16, pool an index into ggml_file.POOLS.  Fields not given are 0: Arch(pre_norm, activation) is a CLIP tower."""
+    _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32), ("layer_scale", C.c_int32), ("reg_tokens", C.c_int32),
+                ("pool", C.c_int32)]
 
 
 class Taps(C.Structure):
@@ -107,6 +109,7 @@ def lib():
         L.vitb200_stream.restype = vp
         L.vitb200_forward_debug.argtypes = [vp, f32p, i32, f32p, f32p, C.POINTER(Taps)]
         L.vitb200_test_gemm.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+        L.vitb200_test_gemm_layer_scale.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
         L.vitb200_test_dequant.argtypes = [i32, vp, C.c_int64, vp]
         L.vitb200_test_gemm_q8.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, i32, vp]
         L.vitb200_test_layernorm.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp]
@@ -140,6 +143,9 @@ class VitModel:
         _check(lib().vitb200_get_arch(self._h, C.byref(a)), "vitb200_get_arch")
         # the architecture (vitb200_arch): {"pre_norm": bool, "activation": one of ACTIVATIONS}; the reference's is (False, "gelu_tanh")
         self.arch = {"pre_norm": bool(a.pre_norm), "activation": ACTIVATIONS[a.activation]}
+        # DINOv2 (vitb200_arch): LayerScale on, register tokens (rows 1 .. reg_tokens of every image), the head's input (one of POOLS)
+        self.layer_scale, self.reg_tokens, self.pool = bool(a.layer_scale), int(a.reg_tokens), POOLS[a.pool]
+        self.n_tokens += self.reg_tokens
         self._labels = None
 
     def label(self, i: int) -> Optional[str]:
@@ -209,7 +215,8 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
             t.ne[i] = ne[i] if i < len(ne) else 1
     hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, vf.eps)
     act = ACTIVATIONS.index(vf.activation) if vf.activation in ACTIVATIONS else -1  # an unknown name is refused by the engine
-    arch = Arch(int(vf.pre_norm), act)
+    pool = POOLS.index(vf.pool) if vf.pool in POOLS else -1  # likewise
+    arch = Arch(int(vf.pre_norm), act, int(vf.layer_scale), int(vf.reg_tokens), pool)
     h = C.c_void_p()
     _check(lib().vitb200_create_arch(C.byref(hp), C.byref(arch), ts, len(entries), device, max_batch, head_tokens, int(fp8), C.byref(h)),
            "vitb200_create")
@@ -345,7 +352,9 @@ def _features_call(model: VitModel, B: int, layers, norm: bool, tokens: bool, pr
     code, np_type = _FEATURE_DTYPES[key]
     req = FeaturesReq(model.hparams.num_hidden_layers if layers is None else int(layers), int(bool(norm)), code)
     tok = np.empty((B, model.n_tokens, model.hidden_size), np_type) if tokens else None
-    pre = np.empty((B, model.head_tokens, model.hidden_size), np_type) if prelogits else None
+    # DINOv2's pool (model.pool == "cls_patch_mean"): one row of 2 D per image, class token || patch mean
+    pre_shape = (B, 1, 2 * model.hidden_size) if model.pool == "cls_patch_mean" else (B, model.head_tokens, model.hidden_size)
+    pre = np.empty(pre_shape, np_type) if prelogits else None
     call(C.byref(req), tok.ctypes.data if tok is not None else None, pre.ctypes.data if pre is not None else None)
     return tok, pre
 
@@ -354,7 +363,7 @@ def vit_features(model: VitModel, images: np.ndarray, layers=None, norm: bool = 
                  dtype=np.float32):
     """Encoder features of host images (vitb200_features): the residual stream after `layers` blocks (None = all of them; 0 = the
     embeddings), passed through the final LayerNorm when `norm`.  Returns (tokens [B,N,D], prelogits [B,head_tokens,D]), None for an
-    output not asked for.  dtype float32, float16 or BFLOAT16 (returned as uint16 bit patterns).  Images as vit_predict takes them."""
+    output not asked for; with model.pool == "cls_patch_mean" (DINOv2) prelogits is [B,1,2D], the class token || the patch mean.  dtype float32, float16 or BFLOAT16 (returned as uint16 bit patterns).  Images as vit_predict takes them."""
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     if imgs.ndim == (3 if model.in_chans == 3 else 2):
         imgs = imgs[None]
@@ -395,6 +404,8 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
     out = {}
     for n in taps:
         shape = TAP_SHAPES[n](B, model.n_tokens, model.hidden_size)
+        if n == "final_ln" and model.pool == "cls_patch_mean":
+            shape = (B, 2 * model.hidden_size)
         out[n] = np.zeros(lead + shape[1:] if n == "final_ln" else shape, np.float32)
         setattr(tp, n, out[n].ctypes.data)
     _check(lib().vitb200_forward_debug(model.handle, imgs.ctypes.data, B, probs.ctypes.data, logits.ctypes.data,
@@ -451,6 +462,18 @@ def test_gemm(M: int, N: int, K: int, epilogue: int, A16: np.ndarray, W16: np.nd
     out = np.empty((M, N), np.float32)
     _check(lib().vitb200_test_gemm(device, M, N, K, epilogue, A.ctypes.data, W.ctypes.data, b.ctypes.data,
                                    r.ctypes.data if r is not None else None, out.ctypes.data), "vitb200_test_gemm")
+    return out
+
+
+def test_gemm_layer_scale(M: int, N: int, K: int, A16: np.ndarray, W16: np.ndarray, bias: np.ndarray, gamma: np.ndarray,
+                          resid: np.ndarray, device: int = 0) -> np.ndarray:
+    """The LayerScale residual epilogue alone (vitb200_test_gemm_layer_scale): f32(f32(A W^T + bias) * gamma) + resid, [M][N] f32."""
+    A = np.ascontiguousarray(A16, np.float16)
+    W = np.ascontiguousarray(W16, np.float16)
+    b, g, r = (np.ascontiguousarray(x, np.float32) for x in (bias, gamma, resid))
+    out = np.empty((M, N), np.float32)
+    _check(lib().vitb200_test_gemm_layer_scale(device, M, N, K, A.ctypes.data, W.ctypes.data, b.ctypes.data, g.ctypes.data, r.ctypes.data,
+                                               out.ctypes.data), "vitb200_test_gemm_layer_scale")
     return out
 
 

@@ -27,6 +27,8 @@ GGML_FILE_MAGIC = 0x67676D6C
 QK8_0 = 32  # ggml-quants.h:42-46 block_q8_0 { f16 d; int8 qs[32]; }
 # MLP activations, in the order of vitb200_arch.activation: the reference's tanh GELU (ggml's f16 table), erf GELU, QuickGELU
 ACTIVATIONS = ("gelu_tanh", "gelu_erf", "quick_gelu")
+# head inputs, in the order of vitb200_arch.pool: the first head_tokens rows, or DINOv2's LN(class token) || mean of LN(patch tokens)
+POOLS = ("token", "cls_patch_mean")
 
 CONFIGS = {
     # name: (hidden, layers, heads, patch, img)
@@ -75,11 +77,15 @@ class VitFile:
     eps: float = 1e-6
     pre_norm: int = 0            # 1: LayerNorm 'norm_pre.*' on the embeddings before block 0 (CLIP towers)
     activation: str = "gelu_tanh"  # MLP activation: one of ACTIVATIONS
+    # DINOv2 (GGUF keys vit.layer_scale, vit.reg_tokens, vit.pool)
+    layer_scale: int = 0         # 1: LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma' on the attention and MLP branches
+    reg_tokens: int = 0          # register tokens 'reg_token' [1, R, D], rows 1 .. R of every image
+    pool: str = "token"          # head input: one of POOLS
 
     @property
     def n_tokens(self) -> int:
         g = self.img_size // self.patch_size
-        return g * g + 1
+        return g * g + 1 + self.reg_tokens
 
 
 def tensor_specs(hidden: int, layers: int, classes: int, patch: int, img: int, in_chans: int = 3):
@@ -328,6 +334,14 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
         if vf.activation not in ACTIVATIONS:
             raise ValueError(f"write_gguf: unknown activation {vf.activation!r} ({', '.join(ACTIVATIONS)})")
         kv.append(gstr(b"vit.activation") + struct.pack("<I", _GGUF_STR) + gstr(vf.activation.encode()))
+    if vf.layer_scale:
+        kv_u32("vit.layer_scale", int(vf.layer_scale))
+    if vf.reg_tokens:
+        kv_u32("vit.reg_tokens", int(vf.reg_tokens))
+    if vf.pool != "token":
+        if vf.pool not in POOLS:
+            raise ValueError(f"write_gguf: unknown pool {vf.pool!r} ({', '.join(POOLS)})")
+        kv.append(gstr(b"vit.pool") + struct.pack("<I", _GGUF_STR) + gstr(vf.pool.encode()))
     if vf.id2label:
         labels = [vf.id2label.get(i, "").encode() for i in range(max(vf.id2label) + 1)]
         kv.append(gstr(b"vit.id2label") + struct.pack("<IIQ", _GGUF_ARR, _GGUF_STR, len(labels)) + b"".join(gstr(x) for x in labels))
@@ -402,6 +416,9 @@ def read_gguf(path: str) -> VitFile:
     vf.eps = kv.get("vit.layer_norm_eps", 1e-6)
     vf.pre_norm = int(kv.get("vit.pre_norm", 0))
     vf.activation = kv.get("vit.activation", "gelu_tanh")
+    vf.layer_scale = int(kv.get("vit.layer_scale", 0))
+    vf.reg_tokens = int(kv.get("vit.reg_tokens", 0))
+    vf.pool = kv.get("vit.pool", "token")
     align = kv.get("general.alignment", 32)
     infos = []
     for _ in range(n_tensors):
