@@ -140,7 +140,11 @@ const char *vitb200_label(const vitb200_engine *e, int class_id);
  * Any output pointer may be NULL.  probs/logits: float32[batch][num_classes]; probs are the reference's
  * soft-maxed `state.prediction` (vit.cpp:931-933), logits the pre-softmax node (vit.cpp:928).
  * topk_idx/topk_prob: [batch][k], probabilities descending (the head of the reference's sorted
- * `predictions`, vit.cpp:1047-1057). */
+ * `predictions`, vit.cpp:1047-1057), the lowest class id first among equal probabilities.  Entries r >= num_classes (k > num_classes)
+ * are (-1, 0); so is every entry of a row whose probabilities are NaN (a NaN or +Inf logit), so an id is always -1 or in
+ * [0, num_classes).
+ * Images are independent: an image's outputs (here, and in every forward, features and recognition call) depend only on that image,
+ * whatever its batch mates or the images of earlier calls held -- NaN and Inf pixels, or pixels that overflow f16, included. */
 int vitb200_forward(vitb200_engine *e, const float *images, int batch, float *probs, float *logits, int32_t *topk_idx,
                     float *topk_prob, int k);
 
@@ -324,6 +328,12 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
  * the sum of two f16 numbers, qkv_hi + qkv_lo (what the qkv GEMM's hi-lo epilogue leaves behind: hi = f16(x), lo = f16(x - hi)), so
  * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858). */
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+
+/* Stand-alone run of the classifier's soft-max + top-k kernel, launched as the forward launches it (the working row in shared memory
+ * up to 227 KB of classes, in global scratch beyond): logits float32 [rows][C] (dense) are copied into rows of pitch round_up(C, 4),
+ * as the head GEMM leaves them, with NaN in the padding columns; probs float32 [rows][C], topk_idx int32 / topk_val float32 [rows][k]
+ * on the host (may be NULL when k == 0).  0 <= k <= 16; top-k entries as vitb200_forward returns them. */
+int vitb200_test_softmax_topk(int device, int rows, int C, int k, const float *logits, float *probs, int32_t *topk_idx, float *topk_val);
 
 /* Host-only: the upload-time weight conversion of one quantised tensor, `n_blocks` ggml blocks of 32 weights
  * (type = ggml_type / file ftype: 2 q4_0, 3 q4_1, 6 q5_0, 7 q5_1, 8 q8_0; ggml-quants.h:11-47) -> f16 bits, exactly what

@@ -214,3 +214,230 @@ def test_layernorm_matches_the_restatement(rows, D):
     # un-cancelled terms (|terms| < 10 here)
     assert (np.abs(y - ref) <= np.maximum(ulp, 4e-6)).all(), float((np.abs(y - ref) / np.maximum(ulp, 4e-6)).max())
     assert (y == ref).mean() > 0.995
+
+
+# ---- attention kernels at their edges ------------------------------------------------------------------------------------------------
+# Token counts on both sides of every tile boundary of each kernel: the wgmma kernel's 64-query tiles and 224-key box, the mma.sync
+# kernels' 16-query warp tiles, 32-key chunks and the 16-warp kernel's 640-key limit.  "hilo" is the wgmma kernel on split-precision
+# operands (vitb200_test_attention_hilo), the way the engine runs it.
+EDGE_N = {eng.ATTN_WGMMA: [1, 63, 64, 65, 128, 129, 197, 223, 224], "hilo": [1, 63, 64, 65, 128, 129, 197, 223, 224],
+          eng.ATTN_MMA16: [129, 160, 640], eng.ATTN_MMA8: [1, 31, 32, 33, 641, 896]}
+EDGE_CASES = [(kern, n) for kern, ns in EDGE_N.items() for n in ns]
+EDGE_IDS = [f"{'hilo' if kern == 'hilo' else {1: 'mma8', 2: 'wgmma', 3: 'mma16'}[kern]}-N{n}" for kern, n in EDGE_CASES]
+EDGE_B, EDGE_H = 3, 2
+
+
+def _pack(q, k, v):
+    """q, k, v [B][N][H][64] -> the fused [B*N][3*H*64] buffer the qkv GEMM leaves behind (q heads, then k heads, then v heads)."""
+    B, N, H, _ = q.shape
+    return np.stack([q, k, v], axis=2).reshape(B * N, 3 * H * 64)
+
+
+def _run_attention(kern, qkv32, B, N, H):
+    """f16 kernels get f16(qkv); the hi + lo hook gets qkv as f32 and reads hi = f16(x), lo = f16(x - hi)."""
+    if kern == "hilo":
+        return eng.test_attention_hilo(qkv32, B, N, H)
+    return eng.test_attention(qkv32.astype(np.float16), B, N, H, kern)
+
+
+def _operand(kern, x32):
+    """The value the kernel sees for an f32 operand: f16(x), or hi + lo for the split-precision hook."""
+    if kern == "hilo":
+        hi, lo = eng.split_hi_lo(x32)
+        return hi.astype(np.float64) + lo.astype(np.float64)
+    return x32.astype(np.float16).astype(np.float64)
+
+
+@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_routes_every_row_exactly(kern, N):
+    """Keys are random +-1 rows and q_i = 8 k_pi(i) for a random permutation pi of each (image, head): the chosen score (64 after the 1/8
+    scale) beats every other by >= 20, and f16(exp(x)) is exactly 0 below -17.33, so every probability row is exactly one-hot and the
+    output row i must be v_pi(i) bit for bit.  Every K and V row of every image, head, key chunk and query tile must land where it belongs."""
+    B, H = EDGE_B, EDGE_H
+    rng = np.random.default_rng(1000 + N)
+    k = rng.choice(np.array([-1.0, 1.0], np.float32), size=(B, N, H, 64))
+    perm = np.stack([np.stack([rng.permutation(N) for _ in range(H)], 1) for _ in range(B)])  # [B][N][H]
+    q = np.take_along_axis(k, perm[..., None], axis=1) * 8.0
+    v = rng.standard_normal((B, N, H, 64)).astype(np.float32)
+    s = np.einsum("bihd,bjhd->bhij", q.astype(np.float64), k.astype(np.float64)) / 8.0
+    chosen = np.take_along_axis(s, perm.transpose(0, 2, 1)[..., None], axis=-1)[..., 0]
+    assert (chosen == 64.0).all()
+    if N > 1:
+        runner_up = np.sort(s, axis=-1)[..., -2]
+        assert (chosen - runner_up >= 20.0).all(), float((chosen - runner_up).min())
+    out = _run_attention(kern, _pack(q, k, v), B, N, H)
+    want = np.take_along_axis(_operand(kern, v), perm[..., None], axis=1).astype(np.float16).astype(np.float32)
+    got = out.reshape(B, N, H, 64)
+    bad = np.argwhere(got != want)
+    assert bad.size == 0, (len(bad), bad[:5].tolist())
+
+
+@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_uniform_rows_average_exactly_the_real_keys(kern, N):
+    """q = 0: every score is 0, every e is 1 and the output is the mean of the N real V rows.  Against float64 within one f16 output
+    ulp plus the f32 summation error; a padded or foreign key counted in the sum l scales the output by N / N_padded and fails."""
+    B, H = EDGE_B, EDGE_H
+    rng = np.random.default_rng(2000 + N)
+    q = np.zeros((B, N, H, 64), np.float32)
+    k = rng.standard_normal((B, N, H, 64)).astype(np.float32)
+    v = (1.0 + 0.5 * rng.standard_normal((B, N, H, 64))).astype(np.float32)
+    out = _run_attention(kern, _pack(q, k, v), B, N, H).reshape(B, N, H, 64)
+    vs = _operand(kern, v)
+    ref = vs.mean(axis=1, keepdims=True)
+    tol = np.spacing(np.abs(ref).astype(np.float16)).astype(np.float64) + 2 * (N + 2) * 2.0 ** -24 * np.abs(vs).mean(axis=1, keepdims=True)
+    err = np.abs(out - ref)
+    assert (err <= tol).all(), float((err / tol).max())
+
+
+@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_all_negative_scores(kern, N):
+    """Every scaled score in [-6, -2] (asserted in float64): against the float64 restatement at the usual tolerance.  A zero-filled
+    padding key (score 0) that escaped the masking would become the row maximum and add e = 1 per padded key to l."""
+    B, H = EDGE_B, EDGE_H
+    rng = np.random.default_rng(3000 + N)
+    k = rng.standard_normal((B, N, H, 64)).astype(np.float32)
+    q = (0.3 * rng.standard_normal((B, N, H, 64))).astype(np.float32)
+    k[..., 0], q[..., 0] = 1.0, -32.0                    # -4 after the 1/8 scale, the rest within +-2
+    v = rng.standard_normal((B, N, H, 64)).astype(np.float32)
+    qkv = _pack(q, k, v)
+    x = _operand(kern, qkv)
+    s = np.einsum("bihd,bjhd->bhij", x.reshape(B, N, 3, H, 64)[:, :, 0], x.reshape(B, N, 3, H, 64)[:, :, 1]) / 8.0
+    assert s.min() >= -6.0 and s.max() <= -2.0, (s.min(), s.max())
+    out = _run_attention(kern, qkv, B, N, H)
+    ref = _attention_ref_f32(x.astype(np.float32), B, N, H)[0] if kern == "hilo" else _attention_ref(qkv.astype(np.float16), B, N, H)
+    err = np.abs(out - ref)
+    tol = 2.0 ** -10 * np.abs(ref) + 2e-3 * np.abs(ref).max()
+    assert (err <= tol).all(), (err.max(), np.abs(ref).max())
+
+
+@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_non_finite_values_stay_in_their_image(kern, N):
+    """NaN, then +Inf, in the Q rows, then the K rows, then the V rows of one image (first, middle, last of three): every other image's
+    output is bit-identical to the same launch with that image clean."""
+    B, H = EDGE_B, EDGE_H
+    rng = np.random.default_rng(4000 + N)
+    qkv = rng.normal(0.0, 1.0, (B, N, 3, H, 64)).astype(np.float32)
+    clean = _run_attention(kern, qkv.reshape(B * N, -1), B, N, H).reshape(B, N, -1)
+    assert np.isfinite(clean).all()
+    for val in (np.nan, np.inf):
+        for part in range(3):
+            for img in range(B):
+                x = qkv.copy()
+                x[img, :, part] = val
+                out = _run_attention(kern, x.reshape(B * N, -1), B, N, H).reshape(B, N, -1)
+                others = [b for b in range(B) if b != img]
+                assert np.array_equal(out[others], clean[others]), (val, "qkv"[part], img)
+
+
+# ---- the classifier's soft-max + top-k kernel -------------------------------------------------------------------------------------------
+# Inputs x (exact f16 values) where the kernel's f16(exp(x)) differs from the reference's f16 exp table: ex2.approx may land one f16 ulp
+# from expf.  {f16 bits of x: f16 bits of the kernel's exp(x)}, as measured on an H100 (NVIDIA H100 80GB HBM3).  Both inputs have
+# exp(x) within 2^-3 f16 ulp of a rounding midpoint: exp(-2.615234375) = 0.0731506..., table 0.07318115, kernel 0.07312012;
+# exp(-2.966796875) = 0.0514679..., table 0.05148315, kernel 0.05145264.
+EXP_ULP_OFF = {0xC13B: 0x2CAE, 0xC1EF: 0x2A96}
+
+
+def _kernel_exp(x):
+    """f16(exp(f16(x))) as the kernel computes it: the reference's table, except at the inputs of EXP_ULP_OFF."""
+    e = rs.exp_table(np.asarray(x, np.float32))
+    if EXP_ULP_OFF:
+        bits = np.asarray(x, np.float32).astype(np.float16).view(np.uint16)
+        for xb, eb in EXP_ULP_OFF.items():
+            e[bits == xb] = np.array([eb], np.uint16).view(np.float16)[0]
+    return e
+
+
+def test_softmax_exp_of_every_f16_input():
+    """One row [0, x_1 .. x_n], the x every f16 value in [-18, 0) (19.6 k classes).  p_0 = 1/sum e exactly, so round_f16(p_i / p_0)
+    recovers the kernel's e_i exactly: each must be within one f16 ulp of the reference's exp table, and off by one ulp only at the
+    inputs listed in EXP_ULP_OFF.  The probabilities are e * (1/sum e) within the f32 summation error of a float64 computation."""
+    bits = np.arange(0x8001, 0xCC81, dtype=np.uint16)       # -2^-24 .. -18
+    xs = bits.view(np.float16).astype(np.float32)
+    assert xs.min() == -18.0 and xs.max() < 0
+    row = np.concatenate([[0.0], xs]).astype(np.float32)[None]
+    probs, _, _ = eng.test_softmax_topk(row, 0)
+    p0 = np.float64(probs[0, 0])
+    e = (probs[0, 1:].astype(np.float64) / p0).astype(np.float16)
+    table = rs.exp_table(xs).astype(np.float16)
+    off = np.abs(e.view(np.uint16).astype(np.int32) - table.view(np.uint16).astype(np.int32))
+    found = {int(b): int(eb) for b, eb in zip(bits[off != 0], e.view(np.uint16)[off != 0])}
+    assert off.max() <= 1, int(off.max())
+    assert found == EXP_ULP_OFF, f"EXP_ULP_OFF = {found!r}"
+    ef = np.concatenate([[1.0], e.astype(np.float64)])
+    ref = ef / ef.sum()
+    n = row.shape[1]
+    assert (np.abs(probs[0] - ref) <= (n / 256 + 32) * 2.0 ** -23 * ref + 1e-45).all()
+
+
+def _softmax_ref(x):
+    """float64 soft-max with the kernel's f16 exp of the f32 difference x - max."""
+    z = (x - x.max(axis=1, keepdims=True)).astype(np.float32)
+    e = _kernel_exp(z).astype(np.float64)
+    return e / e.sum(axis=1, keepdims=True)
+
+
+def _topk_ref(probs, k):
+    """Top-k of the kernel's own probabilities: descending, lowest index first among equals, (-1, 0) past the class count."""
+    rows, C = probs.shape
+    idx = np.full((rows, k), -1, np.int32)
+    val = np.zeros((rows, k), np.float32)
+    order = np.lexsort((np.broadcast_to(np.arange(C), probs.shape), -probs.astype(np.float64)), axis=1)[:, :min(k, C)]
+    idx[:, :order.shape[1]] = order
+    val[:, :order.shape[1]] = np.take_along_axis(probs, order, axis=1)
+    return idx, val
+
+
+SOFTMAX_CASES = [(3, 1, 0), (3, 1, 1), (2, 1, 16), (5, 2, 2), (5, 2, 3), (7, 255, 5), (7, 256, 16), (300, 257, 5), (4, 1000, 16),
+                 (300, 1001, 1), (3, 21843, 5), (2, 60000, 16), (2, 60000, 0)]
+
+
+@pytest.mark.parametrize("rows,C,k", SOFTMAX_CASES)
+def test_softmax_topk_class_counts(rows, C, k):
+    """Class counts around the 256-thread stride and the pitch padding (NaN in the padding columns must not be read), ImageNet heads,
+    21843 classes in shared memory and 60000 on the global scratch path; k from 0 to 16 with k = C and k > C."""
+    rng = np.random.default_rng(rows * 7 + C + k)
+    x = (3.0 * rng.standard_normal((rows, C))).astype(np.float32)
+    probs, idx, val = eng.test_softmax_topk(x, k)
+    ref = _softmax_ref(x)
+    assert (np.abs(probs - ref) <= (C / 256 + 32) * 2.0 ** -23 * ref + 1e-45).all()
+    want_i, want_v = _topk_ref(probs, k)
+    assert np.array_equal(idx, want_i) and np.array_equal(val, want_v)
+
+
+def test_softmax_topk_ties():
+    """Equal maxima at indices held by different threads and warps (and by one thread in two strides): lowest index first.  An all-equal
+    row: indices 0 .. k-1, equal probabilities."""
+    C, k = 1000, 8
+    rng = np.random.default_rng(5)
+    x = rng.standard_normal((2, C)).astype(np.float32)
+    tied = [999, 300, 259, 37, 3]
+    x[0, tied] = 6.0
+    x[1] = 0.25
+    probs, idx, val = eng.test_softmax_topk(x, k)
+    assert idx[0, :5].tolist() == sorted(tied) and (val[0, :5] == val[0, 0]).all() and val[0, 5] < val[0, 0]
+    assert idx[1].tolist() == list(range(k)) and (val[1] == probs[1, 0]).all() and (probs[1] == probs[1, 0]).all()
+    want_i, want_v = _topk_ref(probs, k)
+    assert np.array_equal(idx, want_i) and np.array_equal(val, want_v)
+
+
+def test_softmax_topk_non_finite_rows():
+    """A NaN row, a row with a +Inf logit (Inf - Inf is NaN) and a row with -Inf logits among finite ones, each next to finite rows:
+    the finite rows are bit-identical to a launch without the others, the -Inf classes get probability 0, and a NaN row gets k entries
+    (-1, 0) -- never an index outside [0, C)."""
+    C, k = 1001, 5
+    rng = np.random.default_rng(6)
+    x = (3.0 * rng.standard_normal((7, C))).astype(np.float32)
+    x[1, 17] = np.nan
+    x[3, 500] = np.inf
+    x[5, [0, 255, 256, 1000]] = -np.inf
+    probs, idx, val = eng.test_softmax_topk(x, k)
+    finite = [0, 2, 4, 6]
+    p_f, i_f, v_f = eng.test_softmax_topk(x[finite], k)
+    assert np.array_equal(probs[finite], p_f) and np.array_equal(idx[finite], i_f) and np.array_equal(val[finite], v_f)
+    for r in (1, 3):
+        assert (idx[r] == -1).all() and (val[r] == 0).all(), (r, idx[r].tolist())
+    assert (probs[5, [0, 255, 256, 1000]] == 0).all() and np.isfinite(probs[5]).all() and abs(float(probs[5].sum()) - 1) < 1e-3
+    ok = [0, 2, 4, 5, 6]
+    want_i, want_v = _topk_ref(probs[ok], k)
+    assert np.array_equal(idx[ok], want_i) and np.array_equal(val[ok], want_v)
+    assert ((idx == -1) | ((idx >= 0) & (idx < C))).all()

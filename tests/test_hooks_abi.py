@@ -20,6 +20,7 @@ HOOKS = {
     "layernorm_fp8": lambda: eng.test_layernorm_fp8(np.zeros((ROWS, D), np.float32), np.ones(D, np.float32), np.zeros(D, np.float32)),
     "attention": lambda: eng.test_attention(np.zeros((B * NT, 3 * H * 64), np.float16), B, NT, H),
     "attention_hilo": lambda: eng.test_attention_hilo(np.zeros((B * NT, 3 * H * 64), np.float32), B, NT, H),
+    "softmax_topk": lambda: eng.test_softmax_topk(np.zeros((ROWS, 10), np.float32), 5),
 }
 
 

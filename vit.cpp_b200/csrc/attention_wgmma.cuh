@@ -4,8 +4,10 @@
 // (reference vit.cpp:826-866) for the 197-token geometries.  Same soft-max semantics as attention_kernel (kernels.cuh): the TRUE row
 // maximum, e = f16(exp(f16(s * scale - max))), l = sum e in f32, O = (P V) * (1 / l).
 //
-//   TMA       one thread loads the q tiles (64 rows each) and the whole K and V of the head (224 rows, zero-filled / masked past N)
-//             out of the head-major QKV buffers, SWIZZLE_128B, under one mbarrier -- hi and lo halves
+//   TMA       one thread loads the q tiles (64 rows each) and the whole K and V of the head (224 rows) out of the head-major QKV
+//             buffers, SWIZZLE_128B, under one mbarrier -- hi and lo halves.  The maps see each (plane, image) as a slice of exactly N
+//             rows, so every row past the image's own N is TMA zero fill: no other image's q, k or v (nor a stale row of an earlier
+//             call) reaches shared memory, and a NaN or Inf there cannot turn the P V product of this image into NaN
 //   S = QK^T  wgmma.m64n224k16, A = Q tile and B = K from shared memory, f32 accumulators in registers (one warpgroup per 64-query
 //             tile; two warpgroups, each taking every other tile): S = Ql Kh^T + Qh Kl^T + Qh Kh^T (kernels.cuh explains why)
 //   softmax   in registers: each row lives in one quad of lanes; P is packed to f16 in place, already in the A-fragment layout
@@ -30,8 +32,9 @@ __host__ __device__ inline int attention_wgmma_smem_bytes()
 __global__ void __launch_bounds__(ATTW_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                        const __grid_constant__ CUtensorMap tmQl, const __grid_constant__ CUtensorMap tmKVl,
-                       __half *__restrict__ out, int N, int D, int H, float scale)
-// tmQ / tmQl: 3-D maps {64, rows, 3 H planes} of the hi / lo QKV buffers with 64-row boxes; tmKV / tmKVl: the same with 224-row boxes
+                       __half *__restrict__ out, int N, int D, int H, int nb, float scale)
+// tmQ / tmQl: 3-D maps {64, N, 3 H nb} of the hi / lo QKV buffers with 64-row boxes, nb = images per plane (the buffers' max_batch):
+// slice p nb + b holds the N rows of image b in plane p; tmKV / tmKVl: the same with 224-row boxes
 {
     extern __shared__ uint8_t attw_smem_raw[];
     const uint32_t base = (ptx::smem_u32(attw_smem_raw) + 1023u) & ~1023u;
@@ -44,7 +47,6 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
 
     const int b = blockIdx.x / H, h = blockIdx.x - b * H;
     const int n_mt = (N + 63) >> 6;
-    const int row0 = b * N; // this image's first token row in every plane
     if (threadIdx.x == 0)
     {
         ptx::prefetch_tensormap(&tmQ);
@@ -62,9 +64,10 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         for (int part = 0; part < kParts; ++part)
         {
             const CUtensorMap *mq = part ? &tmQl : &tmQ, *mkv = part ? &tmKVl : &tmKV;
-            for (int t = 0; t < n_mt; ++t) ptx::tma_load_3d(sQ(part, t), mq, bar, 0, row0 + 64 * t, h);
-            ptx::tma_load_3d(sK(part), mkv, bar, 0, row0, H + h);
-            ptx::tma_load_3d(sV(part), mkv, bar, 0, row0, 2 * H + h);
+            const int q_slice = h * nb + b, plane_slices = H * nb; // image b of q plane h; k and v planes lie H and 2 H planes further
+            for (int t = 0; t < n_mt; ++t) ptx::tma_load_3d(sQ(part, t), mq, bar, 0, 64 * t, q_slice);
+            ptx::tma_load_3d(sK(part), mkv, bar, 0, 0, q_slice + plane_slices);
+            ptx::tma_load_3d(sV(part), mkv, bar, 0, 0, q_slice + 2 * plane_slices);
         }
     }
     ptx::mbar_wait(bar, 0);

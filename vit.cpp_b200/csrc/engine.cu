@@ -209,7 +209,8 @@ int dev_alloc(vitb200_engine *e, T **p, size_t count)
     void *q = nullptr;
     CUDA_TRY(cudaMalloc(&q, count * sizeof(T) + 256));
     e->allocs.push_back(q);
-    // activation rows past the current batch are read (and masked) by the attention tiles: they must never hold NaN bit patterns
+    // zeroed once, so that no buffer starts out holding NaN bit patterns; no kernel relies on it afterwards (the attention kernels read
+    // only the current image's rows: TMA zero fill past N in the wgmma kernel, explicit zeros in the mma.sync kernels)
     CUDA_TRY(cudaMemset(q, 0, count * sizeof(T) + 256));
     *p = reinterpret_cast<T *>(q);
     return 0;
@@ -706,13 +707,15 @@ int resid_epilogue(const vitb200_engine *e) { return e->arch.layer_scale ? EPI_B
 enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3 };
 constexpr int ATT_MAX_KEYS_16 = 640;
 
-// q / k / v tensor maps (hi and lo halves) of the wgmma attention over `rows` token rows per plane
-int make_attention_maps(vitb200_engine *e, uint64_t rows)
+// q / k / v tensor maps (hi and lo halves) of the wgmma attention over planes of max_batch * N token rows
+int make_attention_maps(vitb200_engine *e)
 {
-    // the head-major buffer [3 H planes][rows][64]; a box is 64 query rows or ATTW_KEYS key rows of one plane
-    const cuuint64_t planes = 3 * (cuuint64_t)e->hp.num_attention_heads;
+    // the head-major buffer [3 H planes][max_batch][N][64], seen as 3 H max_batch slices of N rows: slice p max_batch + b is image b of
+    // plane p.  A box is 64 query rows or ATTW_KEYS key rows of one slice; rows past N are out of bounds and read as zero, never as
+    // the next image's rows.
+    const cuuint64_t N = (cuuint64_t)e->N, slices = 3 * (cuuint64_t)e->hp.num_attention_heads * (cuuint64_t)e->max_batch;
     auto map = [&](CUtensorMap *m, const __half *ptr, cuuint32_t box_rows) {
-        return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {64, rows, planes}, {128, 128 * rows}, {64, box_rows, 1});
+        return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {64, N, slices}, {128, 128 * N}, {64, box_rows, 1});
     };
     if (map(&e->tmQ, e->QKV16, 64) || map(&e->tmKV, e->QKV16, ATTW_KEYS) || map(&e->tmQl, e->QKV16L, 64) || map(&e->tmKVl, e->QKV16L, ATTW_KEYS))
         return 1;
@@ -723,7 +726,7 @@ int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int H = e->hp.num_attention_heads;
     return launch(e, attention_wgmma_kernel, dim3(B * H), dim3(ATTW_THREADS), (size_t)attention_wgmma_smem_bytes(), s, LAUNCH_PDL, e->tmQ, e->tmKV,
-                  e->tmQl, e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
+                  e->tmQl, e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, e->max_batch, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
 }
 
 // The mma.sync kernels hold K and V of one (image, head) problem in shared memory: N tokens padded to whole key chunks, 64 f16 each.
@@ -912,6 +915,18 @@ int check_k(const vitb200_engine *e, int k)
     return 0;
 }
 
+// Soft-max + top-k of `rows` logits rows of pitch ldl >= C: the working row in dynamic shared memory up to kSoftmaxSmemMax, beyond it
+// in e->d_sm_scratch ([rows][C] floats)
+int launch_softmax_topk(vitb200_engine *e, const float *lg, int ldl, int rows, int C, float *d_probs, int32_t *d_topk_idx, float *d_topk_val,
+                        int k, cudaStream_t s)
+{
+    const size_t row_bytes = (size_t)C * sizeof(float);
+    float *scratch = row_bytes > kSoftmaxSmemMax ? e->d_sm_scratch : nullptr;
+    if (row_bytes > kSoftmaxSmemMax && !scratch) return fail("soft-max: %d classes need a global working row and none is allocated", C);
+    return launch(e, softmax_topk_kernel, dim3(rows), dim3(256), scratch ? 0 : row_bytes, s, LAUNCH_PLAIN, lg, ldl, d_probs, d_topk_idx,
+                  d_topk_val, C, k, scratch);
+}
+
 // The fixed kernel schedule == reference vit_encode_image (vit.cpp:718-941), batched over images.
 int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
                 float *d_topk_val, int k, cudaStream_t s, const vitb200_taps *taps)
@@ -942,14 +957,7 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     }
     if (d_logits && lg != d_logits)
         CUDA_TRY(cudaMemcpy2DAsync(d_logits, (size_t)C * 4, lg, (size_t)Cp * 4, (size_t)C * 4, (size_t)R, cudaMemcpyDeviceToDevice, s));
-    if (d_probs || (k > 0 && (d_topk_idx || d_topk_val)))
-    {
-        const size_t row_bytes = (size_t)C * sizeof(float);
-        float *scratch = row_bytes > kSoftmaxSmemMax ? e->d_sm_scratch : nullptr;
-        if (launch(e, softmax_topk_kernel, dim3(R), dim3(256), scratch ? 0 : row_bytes, s, LAUNCH_PLAIN, lg, Cp, d_probs, d_topk_idx, d_topk_val, C, k,
-                   scratch))
-            return 1;
-    }
+    if ((d_probs || (k > 0 && (d_topk_idx || d_topk_val))) && launch_softmax_topk(e, lg, Cp, R, C, d_probs, d_topk_idx, d_topk_val, k, s)) return 1;
     return 0;
 }
 
@@ -1258,7 +1266,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
     // memory (N <= 224), i.e. wherever the wgmma attention runs
-    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e, T))) return 1;
+    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e))) return 1;
     if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
     if (labels) e->labels = *labels;
     *out = owner.release();
@@ -1503,7 +1511,7 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
         // them), whose products add exact zeros
         if (qkv_lo) to_head_major(qkv_lo);
         if (qkv_lo ? upload(e, &e->QKV16L, hm.data(), hm.size()) : dev_alloc(e, &e->QKV16L, hm.size())) return 1;
-        if (make_attention_maps(e, T)) return 1;
+        if (make_attention_maps(e)) return 1;
     }
     if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
     return tap_f16(out, e->A16, (size_t)T * D, e->stream);
@@ -1519,6 +1527,42 @@ int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t 
     return guarded(__func__, [&] {
         if (!qkv_lo) return fail("bad argument");
         return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out);
+    });
+}
+
+int vitb200_test_softmax_topk(int device, int rows, int C, int k, const float *logits, float *probs, int32_t *topk_idx, float *topk_val)
+{
+    return guarded(__func__, [&]() -> int {
+        if (!logits || !probs || rows < 1 || C < 1 || C > (1 << 20)) return fail("bad argument");
+        if (k > 0 && (!topk_idx || !topk_val)) return fail("null argument");
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        e->max_k = 16;
+        if (check_k(e, k)) return 1;
+        // rows of pitch Cp, as the head GEMM leaves them; the padding columns hold NaN, which the kernel must never read
+        const int Cp = (C + 3) / 4 * 4;
+        std::vector<float> padded((size_t)rows * Cp, std::nanf(""));
+        for (int r = 0; r < rows; ++r) memcpy(&padded[(size_t)r * Cp], logits + (size_t)r * C, (size_t)C * sizeof(float));
+        float *dl = nullptr, *dp = nullptr, *dv = nullptr;
+        int32_t *di = nullptr;
+        if (upload(e, &dl, padded.data(), padded.size()) || dev_alloc(e, &dp, (size_t)rows * C) || dev_alloc(e, &di, (size_t)rows * k + 1) ||
+            dev_alloc(e, &dv, (size_t)rows * k + 1))
+            return 1;
+        // outputs poisoned with 0x7f bytes (3.4e38, index 2139062143): an entry the kernel never writes cannot pass for a result
+        CUDA_TRY(cudaMemset(dp, 0x7f, (size_t)rows * C * sizeof(float)));
+        CUDA_TRY(cudaMemset(di, 0x7f, ((size_t)rows * k + 1) * sizeof(int32_t)));
+        CUDA_TRY(cudaMemset(dv, 0x7f, ((size_t)rows * k + 1) * sizeof(float)));
+        if ((size_t)C * sizeof(float) > kSoftmaxSmemMax && dev_alloc(e, &e->d_sm_scratch, (size_t)rows * C)) return 1;
+        if (run_scratch(e, "soft-max kernel", [&] { return launch_softmax_topk(e, dl, Cp, rows, C, dp, k ? di : nullptr, k ? dv : nullptr, k, e->stream); }))
+            return 1;
+        CUDA_TRY(cudaMemcpy(probs, dp, (size_t)rows * C * sizeof(float), cudaMemcpyDeviceToHost));
+        if (k > 0)
+        {
+            CUDA_TRY(cudaMemcpy(topk_idx, di, (size_t)rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost));
+            CUDA_TRY(cudaMemcpy(topk_val, dv, (size_t)rows * k * sizeof(float), cudaMemcpyDeviceToHost));
+        }
+        return 0;
     });
 }
 

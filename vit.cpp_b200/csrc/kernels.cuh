@@ -718,7 +718,7 @@ attention_kernel(const __half *__restrict__ qkv, size_t plane_rows, __half *__re
 // ascending on ties) by k rounds of block arg-max.  logits rows have pitch ldl (>= C: the head GEMM pads the class count to a
 // multiple of 4), probs rows are dense.  The working copy of the row lives in dynamic shared memory when C floats fit (the
 // launcher opts in up to the 227 KB limit), otherwise in `scratch` (global, [rows][C]); entries r >= C of a top-k list (k > C)
-// are (-1, 0).
+// are (-1, 0), and so is every entry of a row whose probabilities are NaN (a NaN logit, or +Inf: Inf - Inf).
 __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, float *__restrict__ probs, int32_t *__restrict__ topk_idx,
                                     float *__restrict__ topk_val, int C, int k, float *__restrict__ scratch)
 {
@@ -787,6 +787,7 @@ __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, f
         {
             for (int w = 1; w < nw; ++w)
                 if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi)) { bv = red_v[w]; bi = red_i[w]; }
+            if (bi == 0x7fffffff) { bi = -1; bv = 0.f; } // no probability compares >= 0: a NaN row
             if (topk_idx) topk_idx[(size_t)img * k + r] = bi;
             if (topk_val) topk_val[(size_t)img * k + r] = bv;
             if (bi >= 0 && bi < C) sp[bi] = -2.f;

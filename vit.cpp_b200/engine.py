@@ -115,6 +115,7 @@ def lib():
         L.vitb200_test_layernorm.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp]
         L.vitb200_test_attention.argtypes = [i32, i32, i32, i32, i32, vp, vp]
         L.vitb200_test_attention_hilo.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+        L.vitb200_test_softmax_topk.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -441,6 +442,19 @@ def test_attention_hilo(qkv32: np.ndarray, B: int, N: int, H: int, device: int =
     _check(lib().vitb200_test_attention_hilo(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
            "vitb200_test_attention_hilo")
     return out
+
+
+def test_softmax_topk(logits: np.ndarray, k: int, device: int = 0):
+    """The classifier's soft-max + top-k kernel alone (vitb200_test_softmax_topk): logits float32 [rows][C] -> (probs float32
+    [rows][C], topk_idx int32 [rows][k], topk_val float32 [rows][k])."""
+    x = np.ascontiguousarray(logits, np.float32)
+    rows, C = x.shape
+    probs = np.empty((rows, C), np.float32)
+    idx = np.empty((rows, k), np.int32)
+    val = np.empty((rows, k), np.float32)
+    _check(lib().vitb200_test_softmax_topk(device, rows, C, k, x.ctypes.data, probs.ctypes.data, idx.ctypes.data if k else None,
+                                           val.ctypes.data if k else None), "vitb200_test_softmax_topk")
+    return probs, idx, val
 
 
 def test_dequant(ggml_type: int, blocks: np.ndarray) -> np.ndarray:
