@@ -100,8 +100,10 @@ typedef struct vitb200_arch
                          *    norm_pre) on every token row of the embeddings (cls included), written back to the f32 residual stream, before
                          *    block 0.  Same arithmetic and eps as the block LayerNorms, f32 out. */
     int32_t activation; /* MLP activation after fc1: 0 GELU, tanh form, through ggml's f16 table (the reference, unchanged); 1 GELU, erf form,
-                         * 0.5 x (1 + erf(x / sqrt 2)); 2 QuickGELU, x / (1 + exp(-1.702 x)).  Forms 1 and 2 take x = acc + bias (FP8 engine:
-                         * acc (sa sw) + bias) in f32, without rounding it to f16 first, and store f16(act(x)). */
+                         * 0.5 x (1 + erf(x / sqrt 2)); 2 QuickGELU, x / (1 + exp(-1.702 x)); 3 GELU, tanh form as PyTorch's
+                         * gelu(approximate='tanh') ('gelu_pytorch_tanh'), 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))), with pools 2 and 3
+                         * only (SigLIP).  Forms 1, 2 and 3 take x = acc + bias (FP8 engine: acc (sa sw) + bias) in f32, without rounding it to
+                         * f16 first, and store f16(act(x)). */
     /* DINOv2 (HF Dinov2Model / Dinov2WithRegistersModel and their ForImageClassification heads).  Zero is the behaviour above. */
     int32_t layer_scale; /* 0 or 1.  1: x = x + f32(f32(acc + bias) * gamma[n]) after proj ('blocks.{i}.ls1.gamma' [D]) and fc2
                           * ('blocks.{i}.ls2.gamma' [D]), gamma kept in f32 (HF's LayerScale order; not folded into the f16 weights). */
@@ -109,18 +111,31 @@ typedef struct vitb200_arch
                           * N = P + 1 + R; 'pos_embed' is [1, N, D] with the R register rows after the class row (zero for DINOv2). */
     int32_t pool;        /* 0: the head reads the first head_tokens rows (the reference).  1: the head reads one row of 2 D per image,
                           * LN(token 0) || mean over the P patch rows of LN(patch) (registers excluded, LN = the final LayerNorm):
-                          * DINOv2's classifier input.  'head.weight' is then [C][2 D] and head_tokens must be 1. */
+                          * DINOv2's classifier input.  'head.weight' is then [C][2 D] and head_tokens must be 1.
+                          * SigLIP (HF SiglipVisionModel, SiglipForImageClassification): pools 2 and 3 have NO class token -- the token rows
+                          * are [patch_1..P], N = P, 'pos_embed' is [1, P, D], there is no 'cls_token', reg_tokens = 0, head_tokens = 1.
+                          * 2 'map': the attention-pooling head (HF SiglipMultiheadAttentionPoolingHead, timm AttentionPoolLatent): one learned
+                          *   probe 'attn_pool.latent' [1, 1, D], q = latent Wq^T + bq ('attn_pool.q.*', computed once at load in f64, kept
+                          *   in f32), attends per head over k | v = LN(rows) Wkv^T + bkv ('attn_pool.kv.*' [2 D, D], rows k then v; LN = the
+                          *   final LayerNorm) with softmax(q k / 8) in f32; h = out_proj ('attn_pool.proj.*'); pooled = h + fc2(act(fc1(
+                          *   LN_head(h)))) ('attn_pool.norm.*', 'attn_pool.mlp.fc1.*' [4 D, D], 'attn_pool.mlp.fc2.*'), f32.  The head reads
+                          *   f16(pooled): HF's pooler_output.  f16 operands and f32 accumulation in the f16 and FP8 engines alike.
+                          * 3 'mean': the head reads the mean over all P rows of LN(row): SiglipForImageClassification's classifier input. */
 } vitb200_arch;
 /* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = all zero, the reference).
- * Fields out of range, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every ls1 / ls2 gamma, reg_tokens > 0 without
- * 'reg_token', pool = 1 with head_tokens > 1, and a head whose K is not D (pool 0) or 2 D (pool 1) fail here before the device is
- * touched; so does N > 896 tokens, registers included.  Every entry point works on such an engine; the u8 entry points keep vit.cpp's
- * preprocessing (a CLIP or DINOv2 caller normalises its own images and uses the f32 or device entry points).  The launch count of one
- * forward is 3 + 7 L + 3, plus 1 with the pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm).
+ * Fields out of range, activation = 3 with pool 0 or 1, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every
+ * ls1 / ls2 gamma, reg_tokens > 0 without 'reg_token', pool > 0 with head_tokens > 1, pool 2 or 3 with a 'cls_token' tensor, with
+ * reg_tokens > 0 or with a 'pos_embed' of other than P rows, pool 2 without one of its 13 'attn_pool.*' tensors, and a head whose K is
+ * not D (pools 0, 2, 3) or 2 D (pool 1) fail here before the device is touched; so does N > 896 tokens, registers included.  Every entry
+ * point works on such an engine; the u8 entry points keep vit.cpp's preprocessing (a CLIP, DINOv2 or SigLIP caller normalises its own
+ * images and uses the f32 or device entry points).  The launch count of one forward is 3 + 7 L + 3 for pools 0 and 1, plus 1 with the
+ * pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm); 2 + 7 L + 3 for pool 3 (no class-row kernel); 2 + 7 L + 10 for
+ * pool 2 (the head adds LN, k | v GEMM, attention, out_proj, LN, fc1, fc2 and the f16 rounding of its row).
  * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer), vit.activation ("gelu_tanh", "gelu_erf",
- * "quick_gelu"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and vit.pool ("token" or
- * "cls_patch_mean"; any other string fails the load), and then holds 2 more tensors with the pre-norm, 2 L more with LayerScale and
- * 1 more with registers; a file without these keys is the reference's architecture, and legacy-ggml files never carry them. */
+ * "quick_gelu", "gelu_pytorch_tanh"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and
+ * vit.pool ("token", "cls_patch_mean", "map" or "mean"; any other string fails the load), and then holds 2 more tensors with the
+ * pre-norm, 2 L more with LayerScale and 1 more with registers, 1 fewer (no 'cls_token') with pools 2 and 3 and 13 more with pool 2;
+ * a file without these keys is the reference's architecture, and legacy-ggml files never carry them. */
 int vitb200_create_arch(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *tensors, int n_tensors, int device,
                         int max_batch, int head_tokens, int fp8, vitb200_engine **out);
 int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out);
@@ -223,11 +238,15 @@ typedef struct vitb200_features_req
 } vitb200_features_req;
 
 /* tokens:    [batch][N][D], every token, cls first, then the R register tokens, then the patches (N = (img/patch)^2 + 1 + R,
- *            Hugging Face's last_hidden_state / hidden_states[i] order); may be NULL
+ *            Hugging Face's last_hidden_state / hidden_states[i] order); with vitb200_arch.pool 2 or 3 (SigLIP), [batch][P][D], the
+ *            patch rows only (P = (img/patch)^2, HF's last_hidden_state / hidden_states[i]).  May be NULL
  * prelogits: [batch][head_tokens][D], the rows the classifier head reads (token 0, vit.cpp:910; the first 25 for ViTSTR,
  *            vitstr.cpp:864-883); with vitb200_arch.pool = 1, [batch][1][2 D]: token 0 || the mean of the patch rows, each row
- *            through the final LayerNorm first when norm == 1.  May be NULL.  At layers == num_hidden_layers with norm == 1 this is
- *            the head's input before its f16 rounding.  At least one of the two must be non-NULL.
+ *            through the final LayerNorm first when norm == 1; with pool = 2, [batch][1][D]: the attention-pooling head run on the
+ *            final LayerNorm of the rows at depth `layers` (HF's pooler_output at layers == num_hidden_layers; needs norm == 1); with
+ *            pool = 3, [batch][1][D]: the mean of the rows, through the final LayerNorm first when norm == 1.  May be NULL.  At
+ *            layers == num_hidden_layers with norm == 1 this is the head's input before its f16 rounding.  At least one of the two must be
+ *            non-NULL.
  * vitb200_features: HOST buffers, blocking, like vitb200_forward (images as there).
  * vitb200_features_device: DEVICE buffers (16-byte aligned) enqueued on `stream` without synchronising, like vitb200_forward_device.
  * vitb200_features_u8: u8 RGB images pre-processed on the GPU, like vitb200_forward_u8 (RGB models only); host outputs, blocking.
@@ -245,7 +264,8 @@ int vitb200_last_launch_count(const vitb200_engine *e);
 
 /* Per-kernel device timing for roofline reporting: while enabled, CUDA-event pairs are recorded around every
  * launch of the tracked kernels on the stream the forward runs on.  kind: 0 patch GEMM, 1 qkv GEMM, 2 proj GEMM,
- * 3 fc1 GEMM, 4 fc2 GEMM, 5 head GEMM, 6 attention, 7 layernorm.  profile_read synchronises the device and returns
+ * 3 fc1 GEMM, 4 fc2 GEMM, 5 head GEMM, 6 attention, 7 layernorm, 8 the attention-pooling head of vitb200_arch.pool = 2 (every
+ * launch it makes but its two LayerNorms, which are kind 7).  profile_read synchronises the device and returns
  * the summed duration, the launch count and the algorithmic FLOPs of one launch (0 for HBM-bound kernels). */
 int vitb200_profile_enable(vitb200_engine *e, int on);
 int vitb200_profile_read(vitb200_engine *e, int kind, double *ms_total, int *launches, double *flops_per_launch);
@@ -270,7 +290,7 @@ typedef struct vitb200_taps
     float *ln2;      /* [batch][N][D]  */
     float *h;        /* [batch][N][4D] */
     float *x2;       /* [batch][N][D]  */
-    float *final_ln; /* [batch][D]     the head's f16 input ([batch][2 D] with vitb200_arch.pool = 1) */
+    float *final_ln; /* [batch][D]     the head's f16 input ([batch][2 D] with vitb200_arch.pool = 1; the pooled row with pool 2, 3) */
     float *x_final;  /* [batch][N][D]  */
 } vitb200_taps;
 
@@ -279,7 +299,8 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
 
 /* Stand-alone run of the wgmma GEMM kernel: out[M][N] = epilogue(A[M][K] (f16 bits) x W[N][K]^T (f16 bits)).
  * epilogue: 0 bias->f16, 1 bias+gelu->f16, 2 bias+resid->f32, 4 bias->f32, 6 bias->split precision (hi = f16(x), lo = f16(x - hi);
- * `out` receives hi + lo), 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16 (vitb200_arch.activation 1 and 2).  out is float32[M][N] on the
+ * `out` receives hi + lo), 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16 (vitb200_arch.activation 1, 2
+ * and 3).  out is float32[M][N] on the
  * host (f16 results widened).  resid may be NULL unless epilogue == 2. */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
                       const float *bias, const float *resid, float *out);
@@ -299,7 +320,8 @@ int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, floa
 
 /* Stand-alone run of the e4m3 GEMM the FP8 engine uses for qkv and fc1: A [M][K] and W [N][K] e4m3 bytes, a_scale float32 [M] (one per
  * A row), w_scale, bias [N]; out float32 [M][N] = the epilogue's f16 result widened (epilogue 0 bias->f16, 1 bias+gelu->f16,
- * 6 split precision: hi + lo, 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
+ * 6 split precision: hi + lo, 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16) of
+ * x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
 int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
                           float w_scale, const float *bias, float *out);
 
@@ -328,6 +350,12 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
  * the sum of two f16 numbers, qkv_hi + qkv_lo (what the qkv GEMM's hi-lo epilogue leaves behind: hi = f16(x), lo = f16(x - hi)), so
  * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858). */
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+
+/* Stand-alone run of the attention-pooling head's attention kernel (vitb200_arch.pool = 2) through the engine's launcher: one query
+ * q float32 [H*64] (the probe's, scaled by 1/8 inside) per head against the P key rows of each image; kv = f16 bits [B*P][2*H*64], every
+ * row k then v (what the k | v GEMM computes), out = float32 [B][H*64] = the f16 result sum_j softmax_j(q_h k_j / 8) v_j, widened.
+ * 1 <= P <= 896. */
+int vitb200_test_attention_pool(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out);
 
 /* Stand-alone run of the classifier's soft-max + top-k kernel, launched as the forward launches it (the working row in shared memory
  * up to 227 KB of classes, in global scratch beyond): logits float32 [rows][C] (dense) are copied into rows of pitch round_up(C, 4),

@@ -4,6 +4,7 @@
                       [--keep-norm-pre] [--activation gelu_tanh|gelu_erf|quick_gelu] [--eps E]     (timm; these three need GGUF)
     python -m convert <CLIP model.safetensors|.pth> <out.gguf> --hf-config config.json             (Hugging Face CLIP vision tower)
     python -m convert <DINOv2 model.safetensors> <out.gguf> --hf-config config.json [--img-size S]  (Hugging Face DINOv2)
+    python -m convert <SigLIP model.safetensors> <out.gguf> --hf-config config.json               (Hugging Face SigLIP vision tower)
     python -m convert --quantize <in.gguf> <out.gguf> q8_0
 
 * `state_dict_to_model_file` follows reference convert-pth-to-ggml.py:105-158 step by step (header, id2label table, tensors in
@@ -17,6 +18,9 @@
 * `dinov2_to_model_file` converts a Hugging Face DINOv2 (Dinov2Model, Dinov2WithRegistersModel and their ForImageClassification
   heads) to a GGUF file with LayerScale, register tokens and, with a classifier, the class-plus-patch-mean head (`dinov2_to_timm`).
   `--img-size S` resamples the patch position grid of any converted model to S / patch, as Hugging Face does at run time.
+* `siglip_to_model_file` converts a Hugging Face SigLIP vision tower (SiglipVisionModel, the vision tower of SiglipModel, or
+  SiglipForImageClassification) to a GGUF file without a class token, with PyTorch's tanh GELU and the attention-pooling head (pool 'map')
+  or, with a classifier, the token mean (pool 'mean') (`siglip_to_timm`).
 * `quantize_model_file` restates reference quantize.cpp for q8_0 (every 2-D `*weight` tensor, quantize_row_q8_0_reference,
   ggml-quants.c): byte-identical to the reference binary's output (pinned by the CPU test-suite).
 
@@ -102,11 +106,13 @@ def infer_hparams(sd: Dict[str, np.ndarray], heads: Optional[int] = None):
     """(hidden, layers, heads, classes, patch, img, in_chans) from timm VisionTransformer tensor shapes."""
     pw = sd["patch_embed.proj.weight"]                       # (D, C, P, P)
     hidden, in_chans, patch = int(pw.shape[0]), int(pw.shape[1]), int(pw.shape[2])
-    n_tok = int(sd["pos_embed"].shape[1])                    # (1, N, D), N = (img / patch)^2 + 1 + R
+    n_tok = int(sd["pos_embed"].shape[1])                    # (1, N, D), N = (img / patch)^2 + 1 + R, or (img / patch)^2 without cls_token
     R = reg_token_count(sd)
-    grid = int(round(max(n_tok - 1 - R, 0) ** 0.5))
-    if grid * grid + 1 + R != n_tok:
-        raise ValueError(f"pos_embed has {n_tok} tokens: not a square patch grid plus one class token" + (f" and {R} registers" if R else ""))
+    prefix = 1 + R if "cls_token" in sd else 0
+    grid = int(round(max(n_tok - prefix, 0) ** 0.5))
+    if grid * grid + prefix != n_tok:
+        raise ValueError(f"pos_embed has {n_tok} tokens: not a square patch grid" + (" plus one class token" if prefix else "") +
+                         (f" and {R} registers" if R else ""))
     layers = 1 + max(int(m.group(1)) for k in sd for m in [re.match(r"blocks\.(\d+)\.", k)] if m)
     classes = int(sd["head.weight"].shape[0])
     heads = heads or hidden // 64
@@ -141,8 +147,9 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
     """keep_norm_pre, activation, eps: the architecture of a CLIP-pretrained timm ViT (norm_pre, QuickGELU or erf GELU, eps 1e-5);
     GGUF only.  Without them the file is the reference converter's, which drops norm_pre.  LayerScale ('blocks.{i}.ls1.gamma' /
     'ls2.gamma') and register tokens ('reg_token', with their R rows after the class row of pos_embed) are taken when the state dict has
-    them; pool 'cls_patch_mean' makes the head read [class token || patch mean] (DINOv2's classifier).  img_size: resample the patch
-    position grid to img_size / patch (resample_pos_embed)."""
+    them; pool 'cls_patch_mean' makes the head read [class token || patch mean] (DINOv2's classifier); pools 'map' and 'mean' (SigLIP) are
+    for a state dict without 'cls_token', 'map' with the 13 'attn_pool.*' tensors.  img_size: resample the patch position grid to
+    img_size / patch (resample_pos_embed)."""
     assert ftype in (0, 1)
     layer_scale = int(any(k.endswith(".ls1.gamma") for k in sd))
     R = reg_token_count(sd)
@@ -175,11 +182,12 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
             a = a.reshape(1, a.shape[0], 1, 1)                           # convert-pth-to-ggml.py:150-151
         # convert-pth-to-ggml.py:143-147; the loader additionally hard-codes the patch kernel as F16 (vit.cpp:515), so an f32
         # file must still carry it as f16 (SURVEY.md 8c: the reference's own --ftype 0 output does not load)
-        f16 = (ftype == 1 and np.asarray(v).ndim != 1 and k not in ("pos_embed", "cls_token", "reg_token")) or k == "patch_embed.proj.weight"
+        f16 = (ftype == 1 and np.asarray(v).ndim != 1 and k not in _F32_TOKENS) or k == "patch_embed.proj.weight"
         vf.tensors[k] = a.astype(np.float16 if f16 else np.float32)
         vf.tensor_ftype[k] = 1 if f16 else 0
-    # vit.cpp:697, plus norm_pre.weight / .bias, the two LayerScale gammas of every block and reg_token
-    expect = 4 + 12 * layers + 4 + 2 * vf.pre_norm + 2 * layers * layer_scale + (R > 0)
+    # vit.cpp:697, plus norm_pre.weight / .bias, the two LayerScale gammas of every block and reg_token; SigLIP's pools have no cls_token,
+    # and the attention-pooling head 13 tensors
+    expect = 4 + 12 * layers + 4 + 2 * vf.pre_norm + 2 * layers * layer_scale + (R > 0) - (pool in gf.PATCH_ONLY_POOLS) + 13 * (pool == "map")
     if len(vf.tensors) != expect:
         raise ValueError(f"state_dict has {len(vf.tensors)} tensors after filtering, a {layers}-layer ViT needs {expect}")
     if container == "gguf":
@@ -187,6 +195,9 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
     else:
         write_legacy(out_path, vf)
 
+
+# token rows and the pooling head's probe: kept f32 like every 1-D tensor
+_F32_TOKENS = ("pos_embed", "cls_token", "reg_token", "attn_pool.latent")
 
 # Hugging Face CLIP activations -> the file's (vitb200_arch.activation); HF's "gelu" is the erf form
 _HF_ACTIVATIONS = {"quick_gelu": "quick_gelu", "gelu": "gelu_erf"}
@@ -325,6 +336,78 @@ def dinov2_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str,
                              antialias=antialias)
 
 
+def is_hf_siglip(sd: Dict[str, np.ndarray]) -> bool:
+    """A SiglipVisionModel, SiglipModel or SiglipForImageClassification state dict: a CLIP-like vision tower (`vision_model.`) with a
+    post_layernorm and position embeddings but no class embedding."""
+    return ("vision_model.post_layernorm.weight" in sd and "vision_model.embeddings.position_embedding.weight" in sd and
+            "vision_model.embeddings.class_embedding" not in sd)
+
+
+def siglip_to_timm(sd: Dict[str, np.ndarray], config: dict):
+    """Hugging Face SigLIP vision tower -> (timm-named state dict, heads, activation, eps, pool).  config: the model's config.json (a
+    SiglipConfig's `vision_config` is used when present).  The token rows are the patches only (no cls_token).  Without a classifier the
+    attention-pooling head becomes timm's AttentionPoolLatent tensors (head.probe -> attn_pool.latent, in_proj rows q -> attn_pool.q, k and
+    v -> attn_pool.kv, out_proj -> attn_pool.proj, layernorm -> attn_pool.norm, mlp -> attn_pool.mlp) with pool 'map' and an identity
+    head, so the logits are HF's pooler_output; SiglipForImageClassification's classifier becomes the head with pool 'mean' (its unused
+    head.* is dropped).  text_model.*, logit_scale and logit_bias are ignored."""
+    vc = config.get("vision_config", config)
+    act = vc.get("hidden_act", "gelu_pytorch_tanh")
+    if act != "gelu_pytorch_tanh":
+        raise ValueError(f"hidden_act {act!r} is not supported (gelu_pytorch_tanh only)")
+    v = {k[len("vision_model."):]: np.asarray(a, np.float32) for k, a in sd.items() if k.startswith("vision_model.")}
+    pw = v["embeddings.patch_embedding.weight"]                          # (D, C, P, P)
+    D = int(pw.shape[0])
+    heads = int(vc.get("num_attention_heads", D // 64))
+    if D % heads or D // heads != 64:
+        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    inter = int(vc.get("intermediate_size", 4 * D))
+    if inter != 4 * D:
+        raise ValueError(f"intermediate_size {inter} is not supported (4 x hidden = {4 * D} only)")
+    classifier = "classifier.weight" in sd
+    if not classifier and not vc.get("vision_use_head", True):
+        raise ValueError("vision_use_head = false is not supported without a classifier: the tower's pooled output is its attention-pooling "
+                         "head")
+    layers = 1 + max(int(m.group(1)) for k in v for m in [re.match(r"encoder\.layers\.(\d+)\.", k)] if m)
+    out = {"pos_embed": v["embeddings.position_embedding.weight"].reshape(1, -1, D), "patch_embed.proj.weight": pw,
+           "patch_embed.proj.bias": v["embeddings.patch_embedding.bias"]}
+    hf_name = {"norm1": "layer_norm1", "attn.proj": "self_attn.out_proj", "norm2": "layer_norm2", "mlp.fc1": "mlp.fc1", "mlp.fc2": "mlp.fc2"}
+    for i in range(layers):
+        h, t = f"encoder.layers.{i}.", f"blocks.{i}."
+        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        for dst in ("norm1", "attn.qkv", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"):  # timm's state_dict order
+            for p in ("weight", "bias"):
+                if dst == "attn.qkv":  # rows [q; k; v]
+                    out[f"{t}{dst}.{p}"] = np.concatenate([v[f"{h}self_attn.{x}_proj.{p}"] for x in "qkv"], axis=0)
+                else:
+                    out[f"{t}{dst}.{p}"] = v[f"{h}{hf_name[dst]}.{p}"]
+    out["norm.weight"], out["norm.bias"] = v["post_layernorm.weight"], v["post_layernorm.bias"]
+    if classifier:
+        out["head.weight"], out["head.bias"] = np.asarray(sd["classifier.weight"], np.float32), np.asarray(sd["classifier.bias"], np.float32)
+        return out, heads, act, float(vc.get("layer_norm_eps", 1e-6)), "mean"
+    w, b = v["head.attention.in_proj_weight"], v["head.attention.in_proj_bias"]     # rows [q; k; v]
+    out["attn_pool.latent"] = v["head.probe"].reshape(1, 1, D)
+    out["attn_pool.q.weight"], out["attn_pool.q.bias"] = w[:D], b[:D]
+    out["attn_pool.kv.weight"], out["attn_pool.kv.bias"] = w[D:], b[D:]
+    for dst, src in (("proj", "attention.out_proj"), ("norm", "layernorm"), ("mlp.fc1", "mlp.fc1"), ("mlp.fc2", "mlp.fc2")):
+        for p in ("weight", "bias"):
+            out[f"attn_pool.{dst}.{p}"] = v[f"head.{src}.{p}"]
+    out["head.weight"], out["head.bias"] = np.eye(D, dtype=np.float32), np.zeros(D, np.float32)
+    return out, heads, act, float(vc.get("layer_norm_eps", 1e-6)), "map"
+
+
+def siglip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
+                         container: str = "gguf") -> None:
+    """A Hugging Face SigLIP vision tower -> GGUF model file (no class token, gelu_pytorch_tanh, the config's eps; pool 'map' or, with a
+    classifier, 'mean')."""
+    if container != "gguf":
+        raise ValueError("a SigLIP tower needs --container gguf: a legacy ggml file carries the reference's architecture only")
+    tsd, heads, activation, eps, pool = siglip_to_timm(sd, config)
+    if id2label is None and "id2label" in config and "classifier.weight" in sd:
+        id2label = {int(k): str(x) for k, x in config["id2label"].items()}
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool)
+
+
 def write_legacy(path: str, vf) -> None:
     """A VitFile (f32 / f16 / raw q8_0 tensors) -> legacy-ggml container, tensor order as stored."""
     with open(path, "wb") as f:
@@ -402,7 +485,7 @@ def main(argv):
     ap.add_argument("--labels", default=None, help="JSON file {class id: label}")
     ap.add_argument("--container", choices=["legacy", "gguf"], default=None,
                     help="default: legacy for the reference's architecture, gguf for a CLIP tower or the options below")
-    ap.add_argument("--hf-config", default=None, help="config.json of a Hugging Face CLIP or DINOv2 checkpoint (required for one)")
+    ap.add_argument("--hf-config", default=None, help="config.json of a Hugging Face CLIP, DINOv2 or SigLIP checkpoint (required for one)")
     ap.add_argument("--keep-norm-pre", action="store_true", help="timm: keep norm_pre as the model's pre-norm (GGUF only)")
     ap.add_argument("--activation", choices=list(gf.ACTIVATIONS), default="gelu_tanh", help="timm: the MLP activation (GGUF only)")
     ap.add_argument("--eps", type=float, default=1e-6, help="timm: the LayerNorm epsilon (GGUF only)")
@@ -418,6 +501,13 @@ def main(argv):
         if not a.hf_config:
             raise SystemExit("a Hugging Face DINOv2 state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
         dinov2_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", a.img_size)
+        return
+    if is_hf_siglip(sd):
+        if not a.hf_config:
+            raise SystemExit("a Hugging Face SigLIP state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
+        if a.img_size:
+            raise SystemExit("--img-size: resampling a SigLIP tower's position embeddings is not supported")
+        siglip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf")
         return
     if is_hf_clip(sd):
         if not a.hf_config:

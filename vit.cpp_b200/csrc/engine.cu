@@ -156,12 +156,16 @@ struct vitb200_engine
     vitb200_arch arch{}; // pre-norm, MLP activation, LayerScale, register tokens, head pooling; all zero is the reference's architecture
     float *npre_w = nullptr, *npre_b = nullptr; // arch.pre_norm: norm_pre.weight / norm_pre.bias
     int device = 0, max_batch = 0, num_sms = 132;
-    int N = 0, NP = 0, G = 0, KP = 0, KPp = 0; // N = NP + 1 + arch.reg_tokens token rows per image
+    int N = 0, NP = 0, G = 0, KP = 0, KPp = 0; // N = prefix_rows(arch) + NP token rows per image
     int Cp = 0;           // num_classes rounded up to a multiple of 4: pitch of the internal logits rows (128-bit epilogue stores)
     float *d_sm_scratch = nullptr; // soft-max working rows in global memory, only when num_classes floats exceed shared memory
     int C = 3;            // input channels: 3 (vit.cpp) or 1 (ViTSTR extension, vitstr.cpp:713), taken from the patch kernel's shape
     int head_tokens = 1;  // tokens the classifier head reads per image: 1 (token 0, vit.cpp:910) or 25 (vitstr.cpp:864-903)
     int KH = 0;           // the head's K: D, or 2 D with arch.pool = 1 (CLS16 rows are [LN(cls) || mean of LN(patches)])
+    // SigLIP's attention-pooling head (arch.pool = 2): the probe's query pool_q [D] (latent Wq^T + bq, f32), k | v, out_proj, the
+    // head's LayerNorm and MLP; POOL32 [max_batch][D] f32 holds the pooled rows (out_proj's output, then + the MLP's)
+    float *pool_q = nullptr, *pool_nw = nullptr, *pool_nb = nullptr, *POOL32 = nullptr;
+    Linear pool_kv, pool_proj, pool_fc1, pool_fc2;
     // FP8 engine (vitb200_create_fp8): LayerNorms 1 and 2 write e4m3 rows A8 with per-row scales SA, and the qkv and fc1 GEMMs run
     // e4m3 x e4m3 against per-tensor-scaled e4m3 weights; everything else is the f16 engine's schedule
     bool fp8 = false;
@@ -425,7 +429,7 @@ constexpr int kSmemOptinMax = 232448;
 // dynamic shared memory the soft-max kernel may use for its working row (the per-CTA limit minus its static arrays)
 constexpr size_t kSoftmaxSmemMax = kSmemOptinMax - 1024;
 
-enum ProfKind { PK_PATCH = 0, PK_QKV, PK_PROJ, PK_FC1, PK_FC2, PK_HEAD, PK_ATTN, PK_LN, PK_COUNT };
+enum ProfKind { PK_PATCH = 0, PK_QKV, PK_PROJ, PK_FC1, PK_FC2, PK_HEAD, PK_ATTN, PK_LN, PK_POOL, PK_COUNT };
 
 struct ProfScope
 {
@@ -581,13 +585,14 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6, GEMM_OP_E4M3>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, GEMM_OP_E4M3>(e, tmA, tmB, p, s);
         VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
+        VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16)
 #undef VB_CASE
         return fail("no e4m3 GEMM instantiation for epilogue=%d", epi);
     }
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
     VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
-    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16) VB_CASE(EPI_BIAS_SCALE_RESID_F32)
+    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16) VB_CASE(EPI_BIAS_SCALE_RESID_F32) VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16)
 #undef VB_CASE
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
@@ -631,6 +636,9 @@ constexpr int LN_ROWS_MAX_V = 16;
 constexpr int LN_MAX_HIDDEN = LN_ROWS_MAX_V * 128;
 // register tokens a model may have (vitb200_arch.reg_tokens; DINOv2 with registers has 4)
 constexpr int VB_MAX_REG_TOKENS = 16;
+
+// Token rows in front of an image's patch rows: the class token and the registers, or none with SigLIP's pools (vitb200_arch.pool 2, 3)
+int prefix_rows(const vitb200_arch &a) { return a.pool >= 2 ? 0 : 1 + a.reg_tokens; }
 
 template <typename OutT, bool NORM>
 int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
@@ -680,7 +688,7 @@ int launch_layernorm_inplace(vitb200_engine *e, float *x, const float *w, const 
 }
 
 // DINOv2's classifier input (vitb200_arch.pool = 1): per image, [LN(token 0) || mean of LN(patch rows)] into y [B][2 D] (NORM = false:
-// the rows as they are), rows 1 .. reg_tokens left out
+// the rows as they are), rows 1 .. reg_tokens left out.  SigLIP's (pool = 3, no class token): the mean of LN(every row) into y [B][D]
 template <typename OutT, bool NORM>
 int launch_pool(vitb200_engine *e, OutT *y, int B, cudaStream_t s)
 {
@@ -689,13 +697,19 @@ int launch_pool(vitb200_engine *e, OutT *y, int B, cudaStream_t s)
     const auto kern = D <= 4 * 128 ? cls_patch_mean_kernel<4, OutT, NORM>
                     : D <= 8 * 128 ? cls_patch_mean_kernel<8, OutT, NORM> : cls_patch_mean_kernel<LN_ROWS_MAX_V, OutT, NORM>;
     return launch(e, kern, dim3(B), dim3(POOL_WARPS * 32), (size_t)POOL_WARPS * D * sizeof(float), s, LAUNCH_PDL, e->X, e->N,
-                  1 + e->arch.reg_tokens, e->norm_w, e->norm_b, y, D, e->hp.eps);
+                  prefix_rows(e->arch), e->norm_w, e->norm_b, y, D, e->hp.eps);
 }
 
 // The fc1 epilogue of the model's MLP activation (vitb200_arch.activation)
 int fc1_epilogue(const vitb200_engine *e)
 {
-    return e->arch.activation == 1 ? EPI_BIAS_GELU_ERF_F16 : e->arch.activation == 2 ? EPI_BIAS_QUICK_GELU_F16 : EPI_BIAS_GELU_F16;
+    switch (e->arch.activation)
+    {
+    case 1: return EPI_BIAS_GELU_ERF_F16;
+    case 2: return EPI_BIAS_QUICK_GELU_F16;
+    case 3: return EPI_BIAS_GELU_PYTORCH_TANH_F16;
+    }
+    return EPI_BIAS_GELU_F16;
 }
 
 // The residual epilogue of proj and fc2: with LayerScale (vitb200_arch.layer_scale) the branch is scaled by gamma before the add
@@ -753,6 +767,15 @@ int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_
     if (e->QKV16L) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
     if (kernel == ATT_MMA16) return launch_attention_t<16>(e, B, s);
     return launch_attention_t<8>(e, B, s);
+}
+
+// The attention-pooling head's attention (attention_pool_kernel): the probe query q [D] f32 against the k | v head-major planes kv
+// ([2 H][max_batch * N][64] f16) of B images, N = P key rows each -> out [B][D] f16
+int launch_attention_pool(vitb200_engine *e, const float *q, const __half *kv, __half *out, int B, cudaStream_t s)
+{
+    const int P = e->N, H = e->hp.num_attention_heads;
+    return launch(e, attention_pool_kernel, dim3(B * H), dim3(APOOL_THREADS), (size_t)P * sizeof(float), s, LAUNCH_PLAIN, kv,
+                  (size_t)e->max_batch * P, q, out, P, H);
 }
 
 // D2H helpers for the debug taps
@@ -821,15 +844,16 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
     // patchify (one warp per patch, coalesced); the TMA-fed GEMM adds conv bias + pos_embed and writes token rows.
     const bool patches_ready = d_images == nullptr;
     {
-        // the epilogue writes patch p of an image to row 1 + p and adds position row 1 + p: with R register tokens both bases move
-        // down by R rows, so patch p lands in row 1 + R + p with position row 1 + R + p
-        const int R = e->arch.reg_tokens;
+        // the epilogue writes patch p of an image to row 1 + p and adds position row 1 + p: with R prefix rows (class token and
+        // registers) both bases move by R - 1 rows, so patch p lands in row R + p with position row R + p -- one row up without a
+        // class token (SigLIP), R = 1 + reg_tokens rows down otherwise
+        const int R = prefix_rows(e->arch);
         GemmParams p{};
-        p.M = B * e->NP; p.N = D; p.K = e->KPp; p.bias = e->patch.b; p.out = e->X + (size_t)R * D; p.ldo = D;
-        p.pos = e->pos + (size_t)R * D; p.np = e->NP; p.ntok = N;
+        p.M = B * e->NP; p.N = D; p.K = e->KPp; p.bias = e->patch.b; p.out = e->X + (ptrdiff_t)(R - 1) * D; p.ldo = D;
+        p.pos = e->pos + (ptrdiff_t)(R - 1) * D; p.np = e->NP; p.ntok = N;
         ProfScope ps(e, PK_PATCH, 2.0 * p.M * p.N * e->KP, s);
         if (!patches_ready && launch_patchify(e, d_images, PA, B, s)) return 1;
-        if (launch(e, cls_rows_kernel, dim3((B * (1 + R) * D + 255) / 256), dim3(256), 0, s, LAUNCH_PLAIN, e->X, e->cls, e->pos, B, 1 + R, N, D))
+        if (R > 0 && launch(e, cls_rows_kernel, dim3((B * R * D + 255) / 256), dim3(256), 0, s, LAUNCH_PLAIN, e->X, e->cls, e->pos, B, R, N, D))
             return 1;
         if (launch_gemm(e, EPI_PATCH_F32, e->tmA_P, e->patch.tm, p, s)) return 1;
     }
@@ -927,6 +951,40 @@ int launch_softmax_topk(vitb200_engine *e, const float *lg, int ldl, int rows, i
                   d_topk_val, C, k, scratch);
 }
 
+// SigLIP's attention-pooling head (vitb200_arch.pool = 2, HF SiglipMultiheadAttentionPoolingHead) on the residual stream X of B images
+// at its current depth: POOL32 [B][D] f32 = h + fc2(act(fc1(LN_head(h)))), h = out_proj(the probe's attention over post_layernorm(X)).
+// f16 operands and f32 accumulation in both engines.  Launches: LN, k | v GEMM, attention, out_proj, LN, fc1, fc2.
+int run_map_head(vitb200_engine *e, int B, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size, T = B * e->N;
+    {
+        ProfScope ps(e, PK_LN, 0.0, s);
+        if (launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->A16, T, s)) return 1; // post_layernorm, every token row
+    }
+    {
+        // k | v of every row into the head-major planes 0 .. 2 H - 1 of QKV16, as the qkv GEMM lays out k and v
+        GemmParams kv{};
+        kv.M = T; kv.N = 2 * D; kv.K = D; kv.bias = e->pool_kv.b; kv.out = e->QKV16; kv.ldo = 2 * D; kv.headmajor = 1;
+        kv.plane_rows = (size_t)e->max_batch * e->N;
+        GemmParams o{};
+        o.M = B; o.N = D; o.K = D; o.bias = e->pool_proj.b; o.out = e->POOL32; o.ldo = D;
+        ProfScope ps(e, PK_POOL, 2.0 * kv.M * kv.N * kv.K + 4.0 * T * D + 2.0 * B * D * D, s);
+        if (launch_gemm(e, EPI_BIAS_F16, e->tmA_D, e->pool_kv.tm, kv, s) || launch_attention_pool(e, e->pool_q, e->QKV16, e->CLS16, B, s) ||
+            launch_gemm(e, EPI_BIAS_F32, e->tmA_C, e->pool_proj.tm, o, s))
+            return 1;
+    }
+    {
+        ProfScope ps(e, PK_LN, 0.0, s);
+        if (launch_layernorm_rows<__half, true>(e, e->POOL32, (size_t)D, e->pool_nw, e->pool_nb, e->A16, B, s, 0, 0)) return 1;
+    }
+    GemmParams f1{};
+    f1.M = B; f1.N = 4 * D; f1.K = D; f1.bias = e->pool_fc1.b; f1.out = e->H16; f1.ldo = 4 * D;
+    GemmParams f2{};
+    f2.M = B; f2.N = D; f2.K = 4 * D; f2.bias = e->pool_fc2.b; f2.out = e->POOL32; f2.ldo = D; f2.resid = e->POOL32;
+    ProfScope ps(e, PK_POOL, 2.0 * B * 8.0 * D * D, s);
+    return launch_gemm(e, fc1_epilogue(e), e->tmA_D, e->pool_fc1.tm, f1, s) || launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_H, e->pool_fc2.tm, f2, s);
+}
+
 // The fixed kernel schedule == reference vit_encode_image (vit.cpp:718-941), batched over images.
 int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs, float *d_logits, int32_t *d_topk_idx,
                 float *d_topk_val, int k, cudaStream_t s, const vitb200_taps *taps)
@@ -939,10 +997,17 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
 
     // pool (token 0; the first 25 tokens for ViTSTR, vitstr.cpp:864-883) + final LN + head + soft-max + top-k
     // (vit.cpp:910-933, 1047-1057); one row of the head GEMM / one soft-max per pooled token.  DINOv2 (arch.pool = 1): one row of
-    // [LN(token 0) || mean of LN(patches)] per image
+    // [LN(token 0) || mean of LN(patches)] per image; SigLIP: the attention-pooling head's row rounded to f16 (pool = 2) or the mean of
+    // LN(rows) (pool = 3)
     const int TH = e->head_tokens, R = B * TH;
-    if (e->arch.pool ? launch_pool<__half, true>(e, e->CLS16, B, s)
-                     : launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->CLS16, R, s, TH, (size_t)N * D))
+    if (e->arch.pool == 2)
+    {
+        if (run_map_head(e, B, s)) return 1;
+        ProfScope ps(e, PK_POOL, 0.0, s);
+        if (launch_layernorm_rows<__half, false>(e, e->POOL32, (size_t)D, nullptr, nullptr, e->CLS16, B, s, 0, 0)) return 1;
+    }
+    else if (e->arch.pool ? launch_pool<__half, true>(e, e->CLS16, B, s)
+                          : launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->CLS16, R, s, TH, (size_t)N * D))
         return 1;
     if (taps && tap_f16(taps->final_ln, e->CLS16, (size_t)R * e->KH, s)) return 1;
     // internal logits rows have pitch Cp (num_classes padded to 4; the padded W rows are TMA zero fill, the padded bias is 0);
@@ -989,10 +1054,25 @@ int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_
         }
         return fail("features: dtype %d unknown", req->dtype);
     };
+    if (d_prelogits && e->arch.pool == 2)
+    {
+        // SigLIP's attention-pooling head on the final LayerNorm of the rows at this depth (norm = 1, check_features), before the
+        // token rows are emitted: the host path stages those in H16, where the head's fc1 writes
+        if (run_map_head(e, B, s)) return 1;
+        {
+            ProfScope ps(e, PK_POOL, 0.0, s);
+            const size_t D_ = (size_t)D;
+            if (req->dtype == 0) CUDA_TRY(cudaMemcpyAsync(d_prelogits, e->POOL32, (size_t)B * D_ * sizeof(float), cudaMemcpyDeviceToDevice, s));
+            else if (req->dtype == 1 ? launch_layernorm_rows<__half, false>(e, e->POOL32, D_, nullptr, nullptr, (__half *)d_prelogits, B, s, 0, 0)
+                                     : launch_layernorm_rows<__nv_bfloat16, false>(e, e->POOL32, D_, nullptr, nullptr, (__nv_bfloat16 *)d_prelogits, B, s, 0, 0))
+                return 1;
+        }
+        return emit(d_tokens, B * N, N);
+    }
     if (emit(d_tokens, B * N, N)) return 1;
     if (d_prelogits && e->arch.pool)
     {
-        // DINOv2: [token 0 || mean of the patch rows] per image, through the final LayerNorm or not
+        // DINOv2: [token 0 || mean of the patch rows] per image, through the final LayerNorm or not; SigLIP (pool = 3): the mean alone
         ProfScope ps(e, PK_LN, 0.0, s);
         switch (req->dtype * 2 + (req->norm ? 1 : 0))
         {
@@ -1082,6 +1162,8 @@ int check_features(const vitb200_engine *e, const void *images, int batch, const
     if (req->norm != 0 && req->norm != 1) return fail("vitb200_features: norm must be 0 or 1 (got %d)", req->norm);
     if (req->dtype < 0 || req->dtype > 2) return fail("vitb200_features: dtype %d unknown (0 f32, 1 f16, 2 bf16)", req->dtype);
     if (!tokens && !prelogits) return fail("vitb200_features: both outputs are NULL");
+    if (prelogits && e->arch.pool == 2 && !req->norm)
+        return fail("vitb200_features: the attention-pooling head (vitb200_arch.pool = 2) reads the final LayerNorm's rows: prelogits need norm = 1");
     return check_batch(e, batch);
 }
 
@@ -1107,6 +1189,66 @@ struct EngineDeleter
 };
 using EnginePtr = std::unique_ptr<vitb200_engine, EngineDeleter>;
 
+// SigLIP's attention-pooling head (vitb200_arch.pool = 2), timm AttentionPoolLatent names; 'kv' rows are k then v
+constexpr int kPoolTensorCount = 13;
+const char *const kPoolTensors[kPoolTensorCount] = {
+    "attn_pool.latent", "attn_pool.q.weight", "attn_pool.q.bias", "attn_pool.kv.weight", "attn_pool.kv.bias", "attn_pool.proj.weight",
+    "attn_pool.proj.bias", "attn_pool.norm.weight", "attn_pool.norm.bias", "attn_pool.mlp.fc1.weight", "attn_pool.mlp.fc1.bias",
+    "attn_pool.mlp.fc2.weight", "attn_pool.mlp.fc2.bias"};
+
+// The values of a weight tensor as stored (f32, f16, bf16 or a ggml block format), widened to f64
+int host_values(const vitb200_tensor *x, const std::string &name, std::vector<double> &out)
+{
+    const size_t cnt = (size_t)nelem(x);
+    out.resize(cnt);
+    if (x->type == 0) for (size_t i = 0; i < cnt; ++i) out[i] = ((const float *)x->data)[i];
+    else if (x->type == 1) for (size_t i = 0; i < cnt; ++i) out[i] = host_f16_to_f32(((const uint16_t *)x->data)[i]);
+    else if (x->type == 30)
+        for (size_t i = 0; i < cnt; ++i)
+        {
+            const uint32_t u = (uint32_t)((const uint16_t *)x->data)[i] << 16;
+            float f;
+            memcpy(&f, &u, 4);
+            out[i] = f;
+        }
+    else if (quant_block_bytes(x->type) && cnt % 32 == 0)
+    {
+        float y[32];
+        for (size_t b = 0; b < cnt / 32; ++b)
+        {
+            dequant_block(x->type, (const uint8_t *)x->data + b * quant_block_bytes(x->type), y);
+            for (int i = 0; i < 32; ++i) out[b * 32 + i] = y[i];
+        }
+    }
+    else return fail("tensor '%s': weight type %d is not supported", name.c_str(), x->type);
+    return 0;
+}
+
+// The attention-pooling head's query is the same for every image: latent Wq^T + bq, computed once here in f64 from the stored values
+// ('attn_pool.latent' [1, 1, D] and 'attn_pool.q.bias' [D] f32, 'attn_pool.q.weight' [D][D]) and kept in f32
+int upload_probe_query(vitb200_engine *e, const vitb200_tensor *t, int n, int D)
+{
+    const vitb200_tensor *lat = find_tensor(t, n, "attn_pool.latent"), *w = find_tensor(t, n, "attn_pool.q.weight"), *b = find_tensor(t, n, "attn_pool.q.bias");
+    if (!lat || !w || !b) return fail("missing tensor 'attn_pool.latent', 'attn_pool.q.weight' or 'attn_pool.q.bias'");
+    if (lat->type != 0 || b->type != 0) return fail("tensors 'attn_pool.latent' and 'attn_pool.q.bias' must be f32");
+    if (check_shape(lat, "attn_pool.latent", D, 1, 1, 1) || check_shape(b, "attn_pool.q.bias", D, 1, 1, 1) ||
+        check_shape(w, "attn_pool.q.weight", D, D, 1, 1))
+        return 1;
+    std::vector<double> wv;
+    if (host_values(w, "attn_pool.q.weight", wv)) return 1;
+    const float *l = (const float *)lat->data, *bq = (const float *)b->data;
+    std::vector<float> q(D);
+    for (int i = 0; i < D; ++i)
+    {
+        double acc = 0.0;
+        for (int k = 0; k < D; ++k) acc += (double)l[k] * wv[(size_t)i * D + k];
+        q[i] = (float)(acc + (double)bq[i]);
+    }
+    if (dev_alloc(e, &e->pool_q, (size_t)D)) return 1;
+    CUDA_TRY(cudaMemcpy(e->pool_q, q.data(), (size_t)D * sizeof(float), cudaMemcpyHostToDevice));
+    return 0;
+}
+
 // Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
 int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
                 bool fp8, vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
@@ -1121,13 +1263,31 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
                     hp->num_hidden_layers, hp->num_attention_heads, hp->num_classes, hp->patch_size, hp->img_size);
     const vitb200_arch ar = arch ? *arch : vitb200_arch{};
     if (ar.pre_norm != 0 && ar.pre_norm != 1) return fail("vitb200_arch.pre_norm = %d out of range (0 none, 1 LayerNorm 'norm_pre')", ar.pre_norm);
-    if (ar.activation < 0 || ar.activation > 2)
-        return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu)", ar.activation);
+    if (ar.activation < 0 || ar.activation > 3)
+        return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh)", ar.activation);
     if (ar.layer_scale != 0 && ar.layer_scale != 1)
         return fail("vitb200_arch.layer_scale = %d out of range (0 none, 1 LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma')", ar.layer_scale);
     if (ar.reg_tokens < 0 || ar.reg_tokens > VB_MAX_REG_TOKENS)
         return fail("vitb200_arch.reg_tokens = %d out of range (0..%d register tokens)", ar.reg_tokens, VB_MAX_REG_TOKENS);
-    if (ar.pool != 0 && ar.pool != 1) return fail("vitb200_arch.pool = %d out of range (0 token, 1 cls_patch_mean)", ar.pool);
+    if (ar.pool < 0 || ar.pool > 3) return fail("vitb200_arch.pool = %d out of range (0 token, 1 cls_patch_mean, 2 map, 3 mean)", ar.pool);
+    if (ar.activation == 3 && ar.pool < 2)
+        return fail("vitb200_arch.activation = 3 out of range for pool %d: gelu_pytorch_tanh is the SigLIP towers' activation (pools 2 map and "
+                    "3 mean)", ar.pool);
+    if (ar.pool >= 2)
+    {
+        // SigLIP: the token rows are the patch rows alone
+        if (find_tensor(t, n, "cls_token"))
+            return fail("vitb200_arch.pool = %d out of range for a model with a class token: pools 2 (map) and 3 (mean) read patch rows only, "
+                        "and the tensor 'cls_token' is present", ar.pool);
+        if (ar.reg_tokens > 0) return fail("vitb200_arch.pool = %d needs reg_tokens = 0 (got %d): its token rows are the patch rows only", ar.pool, ar.reg_tokens);
+        const int64_t np = (int64_t)(hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size);
+        const vitb200_tensor *pe = find_tensor(t, n, "pos_embed");
+        if (pe && dim_of(pe, 1) != np)
+            return fail("vitb200_arch.pool = %d needs 'pos_embed' with the %lld patch rows only (no class token), got %lld rows", ar.pool,
+                        (long long)np, (long long)dim_of(pe, 1));
+    }
+    for (int i = 0; ar.pool == 2 && i < kPoolTensorCount; ++i)
+        if (!find_tensor(t, n, kPoolTensors[i])) return fail("vitb200_arch.pool = 2 needs the attention-pooling head's tensor '%s'", kPoolTensors[i]);
     if (ar.pre_norm && (!find_tensor(t, n, "norm_pre.weight") || !find_tensor(t, n, "norm_pre.bias")))
         return fail("vitb200_arch.pre_norm = 1 needs the tensors 'norm_pre.weight' and 'norm_pre.bias'");
     for (int i = 0; ar.layer_scale && i < hp->num_hidden_layers; ++i)
@@ -1138,14 +1298,14 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         }
     if (ar.reg_tokens > 0 && !find_tensor(t, n, "reg_token"))
         return fail("vitb200_arch.reg_tokens = %d needs the tensor 'reg_token'", ar.reg_tokens);
-    if (ar.pool && head_tokens != 1) return fail("vitb200_arch.pool = 1 needs head_tokens = 1 (got %d)", head_tokens);
+    if (ar.pool && head_tokens != 1) return fail("vitb200_arch.pool = %d needs head_tokens = 1 (got %d)", ar.pool, head_tokens);
     {
         // the head's K: the pooled row it reads is D wide, or 2 D with the class-plus-patch-mean pool
         const vitb200_tensor *hw = find_tensor(t, n, "head.weight");
-        const int64_t k = (ar.pool ? 2 : 1) * (int64_t)hp->hidden_size;
+        const int64_t k = (ar.pool == 1 ? 2 : 1) * (int64_t)hp->hidden_size;
         if (hw && dim_of(hw, 0) != k)
             return fail("vitb200_arch.pool = %d needs 'head.weight' with K = %lld (%s), got [%lld, %lld]", ar.pool, (long long)k,
-                        ar.pool ? "2 D: class token || patch mean" : "D", (long long)dim_of(hw, 0), (long long)dim_of(hw, 1));
+                        ar.pool == 1 ? "2 D: class token || patch mean" : "D", (long long)dim_of(hw, 0), (long long)dim_of(hw, 1));
     }
     // input channels from the patch kernel [P, P, C, D] (vit.cpp:515; C = 1 in vitstr.cpp:482)
     const vitb200_tensor *pw = find_tensor(t, n, "patch_embed.proj.weight");
@@ -1160,7 +1320,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (!patchify_supports(hp->patch_size, in_chans))
         return fail("patch size %d not supported for %d-channel input (%s)", hp->patch_size, in_chans, patchify_sizes(in_chans));
     if (hp->hidden_size > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", hp->hidden_size, LN_MAX_HIDDEN);
-    const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + 1 + ar.reg_tokens;
+    const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + prefix_rows(ar);
     if (n_tokens > ATT_MAX_TOKENS)
         return fail("%d tokens not supported (max %d: K and V of one attention head must fit in shared memory)", n_tokens, ATT_MAX_TOKENS);
     cudaDeviceProp prop;
@@ -1181,18 +1341,18 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     const int D = hp->hidden_size, P = hp->patch_size;
     e->G = hp->img_size / P;
     e->NP = e->G * e->G;
-    e->N = e->NP + 1 + ar.reg_tokens;
+    e->N = e->NP + prefix_rows(ar);
     e->C = in_chans;
     e->head_tokens = head_tokens;
-    e->KH = (ar.pool ? 2 : 1) * hp->hidden_size;
+    e->KH = (ar.pool == 1 ? 2 : 1) * hp->hidden_size;
     e->Cp = (hp->num_classes + 3) / 4 * 4;
     e->KP = e->C * P * P;
     e->KPp = (e->KP + 63) / 64 * 64;
     if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
 
     // ---- weights (names: reference vit.cpp:518-579)
-    // the prefix rows [cls_token; reg_token] as one array, the cls_rows_kernel's source
-    if (upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls, (int64_t)(1 + ar.reg_tokens) * D)) return 1;
+    // the prefix rows [cls_token; reg_token] as one array, the cls_rows_kernel's source (none with SigLIP's pools)
+    if (prefix_rows(ar) > 0 && upload_f32(e, t, n, "cls_token", D, 1, 1, 1, &e->cls, (int64_t)(1 + ar.reg_tokens) * D)) return 1;
     if (ar.reg_tokens > 0)
     {
         float *reg = nullptr;
@@ -1221,6 +1381,14 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     }
     if (upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b)) return 1;
     if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, e->KH, e->KH, &e->head)) return 1;
+    if (ar.pool == 2 &&
+        (upload_linear(e, t, n, "attn_pool.kv.weight", "attn_pool.kv.bias", 2 * D, D, D, &e->pool_kv) ||
+         upload_linear(e, t, n, "attn_pool.proj.weight", "attn_pool.proj.bias", D, D, D, &e->pool_proj) ||
+         upload_f32(e, t, n, "attn_pool.norm.weight", D, 1, 1, 1, &e->pool_nw) || upload_f32(e, t, n, "attn_pool.norm.bias", D, 1, 1, 1, &e->pool_nb) ||
+         upload_linear(e, t, n, "attn_pool.mlp.fc1.weight", "attn_pool.mlp.fc1.bias", 4 * D, D, D, &e->pool_fc1) ||
+         upload_linear(e, t, n, "attn_pool.mlp.fc2.weight", "attn_pool.mlp.fc2.bias", D, 4 * D, 4 * D, &e->pool_fc2) ||
+         upload_probe_query(e, t, n, D) || dev_alloc(e, &e->POOL32, (size_t)max_batch * D)))
+        return 1;
 
     // ---- activation arena
     const size_t B = (size_t)max_batch, T = B * e->N;
@@ -1527,6 +1695,28 @@ int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t 
     return guarded(__func__, [&] {
         if (!qkv_lo) return fail("bad argument");
         return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out);
+    });
+}
+
+int vitb200_test_attention_pool(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out)
+{
+    return guarded(__func__, [&]() -> int {
+        if (!q || !kv || !out || B < 1 || P < 1 || P > ATT_MAX_TOKENS || H < 1 || H > 128) return fail("bad argument");
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        e->N = P; e->max_batch = B; e->hp.num_attention_heads = H; e->hp.hidden_size = H * 64;
+        const size_t T = (size_t)B * P, D = (size_t)H * 64;
+        // the head-major planes the k | v GEMM writes ([2 H][T][64]) from the caller's [T][2 D] rows
+        std::vector<uint16_t> hm(T * 2 * D);
+        for (size_t r = 0; r < T; ++r)
+            for (int pl = 0; pl < 2 * H; ++pl) memcpy(&hm[((size_t)pl * T + r) * 64], kv + r * 2 * D + (size_t)pl * 64, 128);
+        float *dq = nullptr;
+        __half *dkv = nullptr, *dout = nullptr;
+        if (upload(e, &dq, q, D) || upload(e, &dkv, hm.data(), hm.size()) || dev_alloc(e, &dout, (size_t)B * D)) return 1;
+        CUDA_TRY(cudaMemset(dout, 0xFF, (size_t)B * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
+        if (run_scratch(e, "attention-pool kernel", [&] { return launch_attention_pool(e, dq, dkv, dout, B, e->stream); })) return 1;
+        return tap_f16(out, dout, (size_t)B * D, e->stream);
     });
 }
 
@@ -1965,7 +2155,7 @@ static int test_gemm_impl(int device, int M, int N, int K, int epilogue, const u
     if (scratch_engine(device, owner)) return 1;
     vitb200_engine *e = owner.get();
     const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
-                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16;
+                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16 || epilogue == EPI_BIAS_GELU_PYTORCH_TANH_F16;
     const size_t MN = (size_t)M * N;
     __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
     float *dB = nullptr, *o32 = nullptr;
@@ -2030,8 +2220,8 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
         if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
         if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
         if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 &&
-            epilogue != EPI_BIAS_QUICK_GELU_F16)
-            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8)", epilogue);
+            epilogue != EPI_BIAS_QUICK_GELU_F16 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16)
+            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8, 10)", epilogue);
         EnginePtr owner;
         if (scratch_engine(device, owner)) return 1;
         vitb200_engine *e = owner.get();
@@ -2050,8 +2240,8 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
         GemmParams p{};
         p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
         if (run_scratch(e, "e4m3 GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, true); })) return 1;
-        // split-precision result: hi + lo (exact in f32); the other epilogues leave lo zero
-        return tap_f16(out, hi, MN, e->stream, lo);
+        // split-precision result: hi + lo (exact in f32); the other epilogues' hi alone, so that a -0 stays -0
+        return tap_f16(out, hi, MN, e->stream, epilogue == EPI_BIAS_F16_HILO ? lo : nullptr);
     });
 }
 
@@ -2193,8 +2383,10 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
     if (g.reg_tokens < 0 || g.reg_tokens > VB_MAX_REG_TOKENS)
         return fail("invalid model file '%s' (vit.reg_tokens %lld, 0..%d)", path, (long long)g.reg_tokens, VB_MAX_REG_TOKENS);
     const vitb200_arch arch{(int32_t)g.pre_norm, g.activation, (int32_t)g.layer_scale, (int32_t)g.reg_tokens, g.pool};
-    // vit.cpp:697, plus norm_pre.weight / .bias, the ls1 / ls2 gammas of every block and reg_token
-    const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm + 2 * hp.num_hidden_layers * arch.layer_scale + (arch.reg_tokens > 0);
+    // vit.cpp:697, plus norm_pre.weight / .bias, the ls1 / ls2 gammas of every block and reg_token; SigLIP's pools have no cls_token,
+    // and the attention-pooling head has 13 tensors of its own
+    const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm + 2 * hp.num_hidden_layers * arch.layer_scale + (arch.reg_tokens > 0) -
+                         (arch.pool >= 2) + (arch.pool == 2 ? kPoolTensorCount : 0);
     if ((int)g.tensors.size() != expected) return fail("model file has %d tensors, but %d tensors were expected", (int)g.tensors.size(), expected);
     std::vector<vitb200_tensor> ts(g.tensors.size());
     for (size_t i = 0; i < g.tensors.size(); ++i)

@@ -63,6 +63,7 @@ enum GemmEpilogue
     EPI_BIAS_GELU_ERF_F16 = 7,   // out f16 = f16(gelu_erf(acc + bias)), x in f32 without rounding to f16 first   (fc1 of LAION CLIP)
     EPI_BIAS_QUICK_GELU_F16 = 8, // out f16 = f16(quick_gelu(acc + bias)), likewise                               (fc1 of OpenAI CLIP)
     EPI_BIAS_SCALE_RESID_F32 = 9, // out f32 = f32((acc + bias) * gamma[n]) + resid: LayerScale, HF's order    (proj, fc2 of DINOv2)
+    EPI_BIAS_GELU_PYTORCH_TANH_F16 = 10, // out f16 = f16(gelu_tanh(acc + bias)), x in f32 without rounding to f16 first (fc1 of SigLIP)
 };
 
 struct GemmParams
@@ -136,7 +137,7 @@ __device__ __forceinline__ float quick_gelu_f32(float x)
 __host__ __device__ constexpr bool gemm_epi_staged(int epi)
 {
     return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32 ||
-           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32;
+           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32 || epi == EPI_BIAS_GELU_PYTORCH_TANH_F16;
 }
 
 // Epilogues that add the residual stream (loaded into the staging buffer with TMA)
@@ -150,7 +151,7 @@ struct GemmStage
 {
     using Cfg = GemmCfg<STAGES>;
     static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_GELU_ERF_F16 ||
-                                  EPI == EPI_BIAS_QUICK_GELU_F16);
+                                  EPI == EPI_BIAS_QUICK_GELU_F16 || EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16);
     static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
     static constexpr int kBoxCols = kF16 ? 64 : 32;
     static constexpr int kBoxBytes = 64 * 128;
@@ -416,6 +417,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             }
                             else if constexpr (EPI == EPI_BIAS_GELU_ERF_F16) hv = __floats2half2_rn(gelu_erf_f32(x0), gelu_erf_f32(x1));
                             else if constexpr (EPI == EPI_BIAS_QUICK_GELU_F16) hv = __floats2half2_rn(quick_gelu_f32(x0), quick_gelu_f32(x1));
+                            else if constexpr (EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16) // PyTorch's tanh GELU: x itself, no f16 table
+                                hv = __floats2half2_rn(gelu_tanh_f32(x0), gelu_tanh_f32(x1));
                             else hv = __floats2half2_rn(x0, x1);
                             ptx::st_shared_b32(a + St::box(0, jj / 8), *reinterpret_cast<const uint32_t *>(&hv));
                             if constexpr (EPI == EPI_BIAS_F16_HILO)

@@ -2,7 +2,9 @@
 //   patchify_f16_kernel      reference im2col for stride==kernel conv (ggml.c:11528-11608) without the buffer
 //                            reshuffle: pixels HWC f32 -> f16 patch rows, K order c*P*P + ky*P + kx
 //   cls_rows_kernel          token 0 = cls_token + pos_embed[0] (vit.cpp:794-797), and the register tokens after it
-//   cls_patch_mean_kernel    DINOv2's classifier input: LN(token 0) || the mean of LN(patch rows), one CTA per image
+//   cls_patch_mean_kernel    DINOv2's classifier input: LN(token 0) || the mean of LN(patch rows), one CTA per image; without a class
+//                            token (SigLIP) the mean alone
+//   attention_pool_kernel    SigLIP's attention-pooling head: one learned query attending over an image's token rows, per head
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
 //                            and un-normalised forms write the encoder features (vitb200_features), its e4m3 form the FP8 A operand
 //   layernorm_inplace_kernel the same arithmetic in place on f32 rows (the pre-norm of CLIP towers)
@@ -276,10 +278,12 @@ __global__ void layernorm_inplace_kernel(float *x, const float *__restrict__ w, 
 // ------------------------------------------------------------------------------------------------
 // DINOv2's classifier input (vitb200_arch.pool = 1): per image, y[0 .. D) = LN(token 0) and y[D .. 2 D) = the mean over the patch rows
 // first_patch .. ntok-1 of LN(row) (the register rows between them are left out), LN = the row-per-warp LayerNorm's arithmetic above
-// (NORM = false: the rows as they are).  One CTA of 8 warps per image: warp w normalises patch rows w, w + 8, ... and keeps its column
+// (NORM = false: the rows as they are).  first_patch = 0 (no class token, vitb200_arch.pool = 3): y[0 .. D) = the mean over all ntok rows,
+// rows of D.  One CTA of 8 warps per image: warp w normalises patch rows w, w + 8, ... and keeps its column
 // sums in registers in that order; the eight partial sums then meet in shared memory and are added warp 0 first, 7 last, and divided
 // by the patch count.  No atomics and nothing shared between images: an image gives the same bits alone as in any batch.
-// OutT: __half (the head GEMM's A operand [B][2 D]), float or __nv_bfloat16 (the features' prelogits).  Dynamic shared memory 8 D floats.
+// OutT: __half (the head GEMM's A operand [B][2 D] or [B][D]), float or __nv_bfloat16 (the features' prelogits).  Dynamic shared memory
+// 8 D floats.
 constexpr int POOL_WARPS = 8;
 
 template <typename OutT>
@@ -357,7 +361,8 @@ cls_patch_mean_kernel(const float *__restrict__ x, int ntok, int first_patch, co
     extern __shared__ float4 s_part[]; // [POOL_WARPS][D / 4]
     const int img = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nvec = D >> 2;
     const float *xi = x + (size_t)img * ntok * D;
-    OutT *yi = y + (size_t)img * 2 * D;
+    const int cls = first_patch > 0 ? 1 : 0; // 1: the row starts with LN(token 0)
+    OutT *yi = y + (size_t)img * (1 + cls) * D;
     float4 o[MAXV], acc[MAXV];
 #pragma unroll
     for (int j = 0; j < MAXV; ++j) acc[j] = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -374,7 +379,7 @@ cls_patch_mean_kernel(const float *__restrict__ x, int ntok, int first_patch, co
 #pragma unroll
     for (int j = 0; j < MAXV; ++j)
         if (lane + 32 * j < nvec) s_part[warp * nvec + lane + 32 * j] = acc[j];
-    if (warp == 0)
+    if (cls && warp == 0)
     {
         // the class row, under the other warps' wait at the barrier
         layernorm_row_regs<MAXV, NORM>(xi, w, b, D, eps, lane, o);
@@ -397,7 +402,100 @@ cls_patch_mean_kernel(const float *__restrict__ x, int ntok, int first_patch, co
         float s = part[c];
 #pragma unroll
         for (int k = 1; k < POOL_WARPS; ++k) s = __fadd_rn(s, part[k * D + c]);
-        yi[D + c] = to_out<OutT>(__fdiv_rn(s, count));
+        yi[cls * D + c] = to_out<OutT>(__fdiv_rn(s, count));
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// SigLIP's attention-pooling head (vitb200_arch.pool = 2), its attention: per (image, head), one query q_h (f32 [64], the learned probe
+// projected once at load) against the image's P key rows, o = sum_j softmax_j(q_h . k_j / 8) v_j, f32 throughout, max subtracted.  k and
+// v are the head-major planes the k | v GEMM writes ([2 H planes][plane_rows][64] f16: planes 0 .. H-1 keys, H .. 2H-1 values); only
+// rows 0 .. P-1 of the image are read, so nothing of another image reaches a sum.  o -> f16 at column 64 h of out [B][D] (merged heads).
+// HBM-bound (2 x 128 B per key, no reuse): 16-byte loads, eight lanes per key row, APOOL_CHUNK keys per CTA pass.  The score of key j is
+// its lanes' products summed in a fixed butterfly, the output column sums are added chunk row by chunk row in a fixed order, so an image
+// gives the same bits alone as in any batch.  Dynamic shared memory: P scores.
+constexpr int APOOL_THREADS = 256;
+constexpr int APOOL_CHUNK = APOOL_THREADS / 8; // key rows per pass
+
+__global__ void __launch_bounds__(APOOL_THREADS)
+attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const float *__restrict__ q, __half *__restrict__ out, int P, int H)
+{
+    extern __shared__ float s_score[]; // [P]
+    __shared__ float s_red[APOOL_THREADS / 32];
+    __shared__ float s_part[APOOL_CHUNK][64 + 1];
+    const int img = blockIdx.x / H, h = blockIdx.x - img * H, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int seg = tid & 7, r0 = tid >> 3; // 16-byte segment (8 columns) of a row; first key row of this thread
+    const uint4 *kp = reinterpret_cast<const uint4 *>(kv + ((size_t)h * plane_rows + (size_t)img * P) * 64);
+    const uint4 *vp = reinterpret_cast<const uint4 *>(kv + ((size_t)(H + h) * plane_rows + (size_t)img * P) * 64);
+    float qr[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) qr[i] = __ldg(q + 64 * h + 8 * seg + i) * 0.125f; // 1 / sqrt(64), exact
+    // scores, and the running maximum of the keys this thread saw
+    // (the whole warp takes every pass, so that its shuffles see all 32 lanes; rows past P are neither read nor scored)
+    float mx = -INFINITY;
+    for (int j0 = 0; j0 < P; j0 += APOOL_CHUNK)
+    {
+        const int j = j0 + r0;
+        const bool live = j < P;
+        const uint4 u = live ? __ldg(kp + (size_t)j * 8 + seg) : make_uint4(0u, 0u, 0u, 0u);
+        const __half2 *k2 = reinterpret_cast<const __half2 *>(&u);
+        float d = 0.f;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+        {
+            const float2 f = __half22float2(k2[i]);
+            d = fmaf(qr[2 * i], f.x, d);
+            d = fmaf(qr[2 * i + 1], f.y, d);
+        }
+        d += __shfl_xor_sync(0xffffffffu, d, 1);
+        d += __shfl_xor_sync(0xffffffffu, d, 2);
+        d += __shfl_xor_sync(0xffffffffu, d, 4);
+        if (live)
+        {
+            if (seg == 0) s_score[j] = d;
+            mx = fmaxf(mx, d);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane == 0) s_red[warp] = mx;
+    __syncthreads(); // also orders the s_score writes before their reads
+    mx = s_red[0];
+#pragma unroll
+    for (int w = 1; w < APOOL_THREADS / 32; ++w) mx = fmaxf(mx, s_red[w]);
+    // o = sum_j e_j v_j / sum_j e_j, e_j = exp(s_j - max): this thread's 8 columns over key rows r0, r0 + CHUNK, ...
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, esum = 0.f;
+    for (int j = r0; j < P; j += APOOL_CHUNK)
+    {
+        const float e = expf(s_score[j] - mx);
+        const uint4 u = __ldg(vp + (size_t)j * 8 + seg);
+        const __half2 *v2 = reinterpret_cast<const __half2 *>(&u);
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+        {
+            const float2 f = __half22float2(v2[i]);
+            acc[2 * i] = fmaf(e, f.x, acc[2 * i]);
+            acc[2 * i + 1] = fmaf(e, f.y, acc[2 * i + 1]);
+        }
+        esum += e;
+    }
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s_part[r0][8 * seg + i] = acc[i];
+    __syncthreads(); // every s_red[w] has been read: it takes the exp sums next
+    // the exp sum: each key row's e was added by its 8 segment lanes alike, so lanes with seg == 0 hold the sums
+    float es = seg == 0 ? esum : 0.f;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) es += __shfl_xor_sync(0xffffffffu, es, o);
+    if (lane == 0) s_red[warp] = es;
+    __syncthreads();
+    if (tid < 64)
+    {
+        float den = s_red[0];
+#pragma unroll
+        for (int w = 1; w < APOOL_THREADS / 32; ++w) den += s_red[w];
+        float o = s_part[0][tid];
+        for (int r = 1; r < APOOL_CHUNK; ++r) o += s_part[r][tid];
+        out[(size_t)img * H * 64 + 64 * h + tid] = __float2half_rn(__fdiv_rn(o, den));
     }
 }
 

@@ -16,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from .ggml_file import ACTIVATIONS, POOLS  # vitb200_arch.activation / .pool -> name (the GGUF keys vit.activation / vit.pool)
+from .ggml_file import ACTIVATIONS, PATCH_ONLY_POOLS, POOLS  # vitb200_arch.activation / .pool -> name (GGUF vit.activation / vit.pool)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
@@ -35,7 +35,8 @@ class Hparams(C.Structure):
 
 class Arch(C.Structure):
     """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ACTIVATIONS, layer_scale 0 / 1,
-    reg_tokens 0..16, pool an index into ggml_file.POOLS.  Fields not given are 0: Arch(pre_norm, activation) is a CLIP tower."""
+    reg_tokens 0..16, pool an index into ggml_file.POOLS (2 and 3: SigLIP, no class token).  Fields not given are 0: Arch(pre_norm,
+    activation) is a CLIP tower."""
     _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32), ("layer_scale", C.c_int32), ("reg_tokens", C.c_int32),
                 ("pool", C.c_int32)]
 
@@ -116,6 +117,7 @@ def lib():
         L.vitb200_test_attention.argtypes = [i32, i32, i32, i32, i32, vp, vp]
         L.vitb200_test_attention_hilo.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_test_softmax_topk.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
+        L.vitb200_test_attention_pool.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -147,6 +149,8 @@ class VitModel:
         # DINOv2 (vitb200_arch): LayerScale on, register tokens (rows 1 .. reg_tokens of every image), the head's input (one of POOLS)
         self.layer_scale, self.reg_tokens, self.pool = bool(a.layer_scale), int(a.reg_tokens), POOLS[a.pool]
         self.n_tokens += self.reg_tokens
+        if self.pool in PATCH_ONLY_POOLS:  # SigLIP: the token rows are the patch rows only
+            self.n_tokens -= 1
         self._labels = None
 
     def label(self, i: int) -> Optional[str]:
@@ -364,7 +368,10 @@ def vit_features(model: VitModel, images: np.ndarray, layers=None, norm: bool = 
                  dtype=np.float32):
     """Encoder features of host images (vitb200_features): the residual stream after `layers` blocks (None = all of them; 0 = the
     embeddings), passed through the final LayerNorm when `norm`.  Returns (tokens [B,N,D], prelogits [B,head_tokens,D]), None for an
-    output not asked for; with model.pool == "cls_patch_mean" (DINOv2) prelogits is [B,1,2D], the class token || the patch mean.  dtype float32, float16 or BFLOAT16 (returned as uint16 bit patterns).  Images as vit_predict takes them."""
+    output not asked for; with model.pool == "cls_patch_mean" (DINOv2) prelogits is [B,1,2D], the class token || the patch mean.  SigLIP
+    (model.pool "map" or "mean"): tokens are the P patch rows (HF's last_hidden_state with norm, hidden_states[layers] without), prelogits
+    [B,1,D] the attention-pooling head's output (HF's pooler_output; norm must be True) or the mean of the rows.  dtype float32, float16 or
+    BFLOAT16 (returned as uint16 bit patterns).  Images as vit_predict takes them."""
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     if imgs.ndim == (3 if model.in_chans == 3 else 2):
         imgs = imgs[None]
@@ -441,6 +448,16 @@ def test_attention_hilo(qkv32: np.ndarray, B: int, N: int, H: int, device: int =
     out = np.empty((B * N, H * 64), np.float32)
     _check(lib().vitb200_test_attention_hilo(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
            "vitb200_test_attention_hilo")
+    return out
+
+
+def test_attention_pool(q: np.ndarray, kv16: np.ndarray, B: int, P: int, H: int, device: int = 0) -> np.ndarray:
+    """The attention-pooling head's attention kernel alone (vitb200_test_attention_pool): q float32 [H*64] (one query per head), kv16
+    float16 [B*P, 2*H*64] (every row k then v) -> float32 [B, H*64], the f16 results of sum_j softmax_j(q_h k_j / 8) v_j."""
+    qq = np.ascontiguousarray(q, np.float32).reshape(H * 64)
+    kv = np.ascontiguousarray(kv16, np.float16).reshape(B * P, 2 * H * 64)
+    out = np.empty((B, H * 64), np.float32)
+    _check(lib().vitb200_test_attention_pool(device, B, P, H, qq.ctypes.data, kv.ctypes.data, out.ctypes.data), "vitb200_test_attention_pool")
     return out
 
 

@@ -25,10 +25,14 @@ import numpy as np
 
 GGML_FILE_MAGIC = 0x67676D6C
 QK8_0 = 32  # ggml-quants.h:42-46 block_q8_0 { f16 d; int8 qs[32]; }
-# MLP activations, in the order of vitb200_arch.activation: the reference's tanh GELU (ggml's f16 table), erf GELU, QuickGELU
-ACTIVATIONS = ("gelu_tanh", "gelu_erf", "quick_gelu")
-# head inputs, in the order of vitb200_arch.pool: the first head_tokens rows, or DINOv2's LN(class token) || mean of LN(patch tokens)
-POOLS = ("token", "cls_patch_mean")
+# MLP activations, in the order of vitb200_arch.activation: the reference's tanh GELU (ggml's f16 table), erf GELU, QuickGELU, PyTorch's
+# tanh GELU on the f32 pre-activation (SigLIP)
+ACTIVATIONS = ("gelu_tanh", "gelu_erf", "quick_gelu", "gelu_pytorch_tanh")
+# head inputs, in the order of vitb200_arch.pool: the first head_tokens rows, DINOv2's LN(class token) || mean of LN(patch tokens), and
+# SigLIP's (no class token) attention-pooling head or mean of LN(tokens)
+POOLS = ("token", "cls_patch_mean", "map", "mean")
+# pools whose token rows are the patch rows only
+PATCH_ONLY_POOLS = ("map", "mean")
 
 CONFIGS = {
     # name: (hidden, layers, heads, patch, img)
@@ -85,7 +89,7 @@ class VitFile:
     @property
     def n_tokens(self) -> int:
         g = self.img_size // self.patch_size
-        return g * g + 1 + self.reg_tokens
+        return g * g if self.pool in PATCH_ONLY_POOLS else g * g + 1 + self.reg_tokens
 
 
 def tensor_specs(hidden: int, layers: int, classes: int, patch: int, img: int, in_chans: int = 3):
@@ -353,7 +357,7 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
         ft = vf.tensor_ftype[name]
         if ft not in (0, 1):
             raise ValueError("write_gguf: quantised tensors are not supported")
-        is_mat = arr.ndim >= 2 and name not in ("cls_token", "pos_embed", "patch_embed.proj.bias")
+        is_mat = arr.ndim >= 2 and name not in ("cls_token", "pos_embed", "patch_embed.proj.bias", "attn_pool.latent")
         if is_mat and name != "patch_embed.proj.weight" and weight_type != "keep":
             ft = {"f32": 0, "f16": 1, "bf16": GGML_TYPE_BF16}[weight_type]
         if ft == 0:
