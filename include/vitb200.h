@@ -102,8 +102,11 @@ typedef struct vitb200_arch
     int32_t activation; /* MLP activation after fc1: 0 GELU, tanh form, through ggml's f16 table (the reference, unchanged); 1 GELU, erf form,
                          * 0.5 x (1 + erf(x / sqrt 2)); 2 QuickGELU, x / (1 + exp(-1.702 x)); 3 GELU, tanh form as PyTorch's
                          * gelu(approximate='tanh') ('gelu_pytorch_tanh'), 0.5 x (1 + tanh(sqrt(2/pi) (x + 0.044715 x^3))), with pools 2 and 3
-                         * only (SigLIP).  Forms 1, 2 and 3 take x = acc + bias (FP8 engine: acc (sa sw) + bias) in f32, without rounding it to
-                         * f16 first, and store f16(act(x)). */
+                         * only (SigLIP); 4 SwiGLU ('swiglu', DINOv2 ViT-g, pools 0 and 1 only): 'mlp.fc1.weight' is [2 F][D] and
+                         * 'mlp.fc1.bias' [2 F] in HF's order (x1 rows 0 .. F-1, then the x2 rows), 'mlp.fc2.weight' [D][F], and
+                         * h = f16(silu(x1) * x2), silu(x) = x / (1 + exp(-x)); F is read from block 0's fc1, every block must agree,
+                         * F % 8 == 0 and 8 <= F <= 8 D.  Forms 1 to 4 take x = acc + bias (FP8 engine: acc (sa sw) + bias) in f32, without
+                         * rounding it to f16 first, and store f16(act(x)). */
     /* DINOv2 (HF Dinov2Model / Dinov2WithRegistersModel and their ForImageClassification heads).  Zero is the behaviour above. */
     int32_t layer_scale; /* 0 or 1.  1: x = x + f32(f32(acc + bias) * gamma[n]) after proj ('blocks.{i}.ls1.gamma' [D]) and fc2
                           * ('blocks.{i}.ls2.gamma' [D]), gamma kept in f32 (HF's LayerScale order; not folded into the f16 weights). */
@@ -123,7 +126,8 @@ typedef struct vitb200_arch
                           * 3 'mean': the head reads the mean over all P rows of LN(row): SiglipForImageClassification's classifier input. */
 } vitb200_arch;
 /* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = all zero, the reference).
- * Fields out of range, activation = 3 with pool 0 or 1, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every
+ * Fields out of range, activation = 3 with pool 0 or 1, activation = 4 with pool 2 or 3, activation = 4 with an odd fc1 row count, an
+ * F that is not a multiple of 8 or outside 8..8 D, or a block whose fc1 or fc2 disagrees with F, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every
  * ls1 / ls2 gamma, reg_tokens > 0 without 'reg_token', pool > 0 with head_tokens > 1, pool 2 or 3 with a 'cls_token' tensor, with
  * reg_tokens > 0 or with a 'pos_embed' of other than P rows, pool 2 without one of its 13 'attn_pool.*' tensors, and a head whose K is
  * not D (pools 0, 2, 3) or 2 D (pool 1) fail here before the device is touched; so does N > 896 tokens, registers included.  Every entry
@@ -132,7 +136,7 @@ typedef struct vitb200_arch
  * pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm); 2 + 7 L + 3 for pool 3 (no class-row kernel); 2 + 7 L + 10 for
  * pool 2 (the head adds LN, k | v GEMM, attention, out_proj, LN, fc1, fc2 and the f16 rounding of its row).
  * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer), vit.activation ("gelu_tanh", "gelu_erf",
- * "quick_gelu", "gelu_pytorch_tanh"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and
+ * "quick_gelu", "gelu_pytorch_tanh", "swiglu"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and
  * vit.pool ("token", "cls_patch_mean", "map" or "mean"; any other string fails the load), and then holds 2 more tensors with the
  * pre-norm, 2 L more with LayerScale and 1 more with registers, 1 fewer (no 'cls_token') with pools 2 and 3 and 13 more with pool 2;
  * a file without these keys is the reference's architecture, and legacy-ggml files never carry them. */
@@ -142,6 +146,7 @@ int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out);
 int vitb200_fp8(const vitb200_engine *e);         /* 1 for an FP8 engine, else 0 */
 int vitb200_in_chans(const vitb200_engine *e);    /* 3, or 1 for a ViTSTR model */
 int vitb200_head_tokens(const vitb200_engine *e); /* classifier rows per image */
+int vitb200_mlp_dim(const vitb200_engine *e);     /* the MLP's hidden width: F with activation 4 (SwiGLU), else 4 D */
 
 void vitb200_destroy(vitb200_engine *e);
 
@@ -288,7 +293,7 @@ typedef struct vitb200_taps
     float *attn;     /* [batch][N][D]  */
     float *x1;       /* [batch][N][D]  */
     float *ln2;      /* [batch][N][D]  */
-    float *h;        /* [batch][N][4D] */
+    float *h;        /* [batch][N][F]  the MLP's hidden activations, F = vitb200_mlp_dim (4 D but with SwiGLU) */
     float *x2;       /* [batch][N][D]  */
     float *final_ln; /* [batch][D]     the head's f16 input ([batch][2 D] with vitb200_arch.pool = 1; the pooled row with pool 2, 3) */
     float *x_final;  /* [batch][N][D]  */
@@ -300,8 +305,8 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
 /* Stand-alone run of the wgmma GEMM kernel: out[M][N] = epilogue(A[M][K] (f16 bits) x W[N][K]^T (f16 bits)).
  * epilogue: 0 bias->f16, 1 bias+gelu->f16, 2 bias+resid->f32, 4 bias->f32, 6 bias->split precision (hi = f16(x), lo = f16(x - hi);
  * `out` receives hi + lo), 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16 (vitb200_arch.activation 1, 2
- * and 3).  out is float32[M][N] on the
- * host (f16 results widened).  resid may be NULL unless epilogue == 2. */
+ * and 3), 11 SwiGLU->f16 (activation 4: W [N][K] and bias [N] in HF's order, N = 2 F, F % 8 == 0; out [M][N / 2] = f16(silu(x1) x2)).
+ * out is float32[M][N] on the host (f16 results widened).  resid may be NULL unless epilogue == 2. */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
                       const float *bias, const float *resid, float *out);
 
@@ -320,8 +325,8 @@ int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, floa
 
 /* Stand-alone run of the e4m3 GEMM the FP8 engine uses for qkv and fc1: A [M][K] and W [N][K] e4m3 bytes, a_scale float32 [M] (one per
  * A row), w_scale, bias [N]; out float32 [M][N] = the epilogue's f16 result widened (epilogue 0 bias->f16, 1 bias+gelu->f16,
- * 6 split precision: hi + lo, 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16) of
- * x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
+ * 6 split precision: hi + lo, 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16, 11 SwiGLU
+ * as vitb200_test_gemm takes it, out [M][N / 2]) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
 int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
                           float w_scale, const float *bias, float *out);
 

@@ -163,8 +163,8 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
         if img_size % P:
             raise ValueError(f"img_size {img_size} is not a multiple of the patch size {P}")
         sd = dict(sd, pos_embed=resample_pos_embed(sd["pos_embed"], 1 + R, img_size // P, antialias))
-    if activation not in gf.ACTIVATIONS:
-        raise ValueError(f"activation {activation!r} unknown ({', '.join(gf.ACTIVATIONS)})")
+    if activation not in gf.ARCH_ACTIVATIONS:
+        raise ValueError(f"activation {activation!r} unknown ({', '.join(gf.ARCH_ACTIVATIONS)})")
     if container != "gguf" and (keep_norm_pre or activation != "gelu_tanh" or eps != 1e-6):
         raise ValueError("a pre-norm, another activation or another eps needs --container gguf: a legacy ggml file carries the "
                          "reference's architecture only")
@@ -273,15 +273,16 @@ def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
     attention.output.dense attn.proj, layer_scale{1,2}.lambda1 ls{1,2}.gamma, embeddings.register_tokens reg_token (with R zero rows
     inserted into pos_embed after the class row: registers get no position embedding), layernorm norm; mask_token is dropped.  A
     classifier becomes the head with pool 'cls_patch_mean' (its logits are HF's); without one the head is the identity with pool 'token',
-    so the logits are HF's pooler_output.  antialias: how HF resamples this class's position grid (Dinov2WithRegisters antialiases)."""
+    so the logits are HF's pooler_output.  antialias: how HF resamples this class's position grid (Dinov2WithRegisters antialiases).
+    use_swiglu_ffn (ViT-g): mlp.weights_in [2 F][D] becomes mlp.fc1 and mlp.weights_out [D][F] mlp.fc2, as they are, with activation
+    'swiglu'; hidden_act and mlp_ratio are ignored, as HF ignores them, and F comes from the tensors."""
+    swiglu = bool(config.get("use_swiglu_ffn", False))
     act = config.get("hidden_act", "gelu")
-    if act != "gelu":
+    if act != "gelu" and not swiglu:
         raise ValueError(f"hidden_act {act!r} is not supported (gelu only)")
-    if config.get("use_swiglu_ffn", False):
-        raise ValueError("use_swiglu_ffn: SwiGLU MLPs (DINOv2 ViT-g) are not supported")
     if not config.get("qkv_bias", True):
         raise ValueError("qkv_bias false is not supported (the engine's qkv has a bias)")
-    if config.get("mlp_ratio", 4) != 4:
+    if config.get("mlp_ratio", 4) != 4 and not swiglu:
         raise ValueError(f"mlp_ratio {config.get('mlp_ratio')} is not supported (4 only)")
     pre = next((p for p in _DINOV2_PREFIXES if any(k.startswith(p) for k in sd)), "")
     v = {k[len(pre):]: np.asarray(a, np.float32) for k, a in sd.items() if k.startswith(pre)}
@@ -301,7 +302,10 @@ def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
         out["reg_token"] = reg.reshape(1, R, D)
     for i in range(layers):
         h, t = f"encoder.layer.{i}.", f"blocks.{i}."
-        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
+        if swiglu:
+            if h + "mlp.weights_in.weight" not in v:
+                raise ValueError(f"use_swiglu_ffn: the config asks for SwiGLU MLPs but block {i} has no mlp.weights_in")
+        elif v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
             raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
         for p in ("weight", "bias"):
             out[f"{t}norm1.{p}"] = v[f"{h}norm1.{p}"]
@@ -310,7 +314,8 @@ def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
         for p in ("weight", "bias"):
             out[f"{t}attn.proj.{p}"] = v[f"{h}attention.output.dense.{p}"]
         out[f"{t}ls1.gamma"] = v[h + "layer_scale1.lambda1"]
-        for dst, src in (("norm2", "norm2"), ("mlp.fc1", "mlp.fc1"), ("mlp.fc2", "mlp.fc2")):
+        mlp = (("mlp.fc1", "mlp.weights_in"), ("mlp.fc2", "mlp.weights_out")) if swiglu else (("mlp.fc1", "mlp.fc1"), ("mlp.fc2", "mlp.fc2"))
+        for dst, src in (("norm2", "norm2"),) + mlp:
             for p in ("weight", "bias"):
                 out[f"{t}{dst}.{p}"] = v[f"{h}{src}.{p}"]
         out[f"{t}ls2.gamma"] = v[h + "layer_scale2.lambda1"]
@@ -321,12 +326,12 @@ def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
     else:
         out["head.weight"], out["head.bias"] = np.eye(D, dtype=np.float32), np.zeros(D, np.float32)
     pool = "cls_patch_mean" if cls_w is not None else "token"
-    return out, heads, "gelu_erf", float(config.get("layer_norm_eps", 1e-6)), pool, R > 0
+    return out, heads, "swiglu" if swiglu else "gelu_erf", float(config.get("layer_norm_eps", 1e-6)), pool, R > 0
 
 
 def dinov2_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
                          container: str = "gguf", img_size: Optional[int] = None) -> None:
-    """A Hugging Face DINOv2 -> GGUF model file (LayerScale, registers, erf GELU, the config's eps; the classifier's pool)."""
+    """A Hugging Face DINOv2 -> GGUF model file (LayerScale, registers, erf GELU or SwiGLU, the config's eps; the classifier's pool)."""
     if container != "gguf":
         raise ValueError("a DINOv2 model needs --container gguf: a legacy ggml file carries the reference's architecture only")
     tsd, heads, activation, eps, pool, antialias = dinov2_to_timm(sd, config)

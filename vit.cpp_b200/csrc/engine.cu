@@ -157,6 +157,7 @@ struct vitb200_engine
     float *npre_w = nullptr, *npre_b = nullptr; // arch.pre_norm: norm_pre.weight / norm_pre.bias
     int device = 0, max_batch = 0, num_sms = 132;
     int N = 0, NP = 0, G = 0, KP = 0, KPp = 0; // N = prefix_rows(arch) + NP token rows per image
+    int F = 0;            // the MLP's hidden width: 4 D, or SwiGLU's F (arch.activation = 4, read from block 0's fc1)
     int Cp = 0;           // num_classes rounded up to a multiple of 4: pitch of the internal logits rows (128-bit epilogue stores)
     float *d_sm_scratch = nullptr; // soft-max working rows in global memory, only when num_classes floats exceed shared memory
     int C = 3;            // input channels: 3 (vit.cpp) or 1 (ViTSTR extension, vitstr.cpp:713), taken from the patch kernel's shape
@@ -261,17 +262,28 @@ int64_t nelem(const vitb200_tensor *t)
     return n;
 }
 
-// f32 tensor with the reference's declared extents {e0, e1, e2, e3} (vit.cpp:510-574); `padded` >= the element count allocates a
-// zero-filled tail (the classifier bias when num_classes is not a multiple of 4)
+// f32 tensor with the reference's declared extents {e0, e1, e2, e3} (vit.cpp:510-574), NULL (with the error set) when it is missing or
+// does not match
+const vitb200_tensor *f32_tensor(const vitb200_tensor *t, int n, const std::string &name, int64_t e0, int64_t e1, int64_t e2, int64_t e3)
+{
+    const vitb200_tensor *x = find_tensor(t, n, name);
+    if (!x) return fail("missing tensor '%s'", name.c_str()), nullptr;
+    if (x->type != 0) return fail("tensor '%s' must be f32 (type %d)", name.c_str(), x->type), nullptr;
+    const int64_t expect = e0 * e1 * e2 * e3;
+    if (nelem(x) != expect)
+        return fail("tensor '%s' has wrong size in model file: got %lld, expected %lld", name.c_str(), (long long)nelem(x), (long long)expect), nullptr;
+    if (check_shape(x, name, e0, e1, e2, e3)) return nullptr;
+    return x;
+}
+
+// f32 tensor uploaded as it is stored; `padded` >= the element count allocates a zero-filled tail (the classifier bias when
+// num_classes is not a multiple of 4)
 int upload_f32(vitb200_engine *e, const vitb200_tensor *t, int n, const std::string &name, int64_t e0, int64_t e1, int64_t e2, int64_t e3,
                float **dst, int64_t padded = 0)
 {
-    const vitb200_tensor *x = find_tensor(t, n, name);
-    if (!x) return fail("missing tensor '%s'", name.c_str());
-    if (x->type != 0) return fail("tensor '%s' must be f32 (type %d)", name.c_str(), x->type);
+    const vitb200_tensor *x = f32_tensor(t, n, name, e0, e1, e2, e3);
+    if (!x) return 1;
     const int64_t expect = e0 * e1 * e2 * e3;
-    if (nelem(x) != expect) return fail("tensor '%s' has wrong size in model file: got %lld, expected %lld", name.c_str(), (long long)nelem(x), (long long)expect);
-    if (check_shape(x, name, e0, e1, e2, e3)) return 1;
     if (dev_alloc(e, dst, (size_t)(padded > expect ? padded : expect))) return 1;
     CUDA_TRY(cudaMemcpy(*dst, x->data, (size_t)expect * sizeof(float), cudaMemcpyHostToDevice));
     return 0;
@@ -342,6 +354,25 @@ void dequant_block(int type, const uint8_t *blk, float *y)
     }
 }
 
+// SwiGLU's fc1 (vitb200_arch.activation = 4) in the layout the EPI_BIAS_SWIGLU_F16 epilogue reads (gemm_wgmma.cuh): HF's [2 F] rows
+// of row_elems values, x1 rows 0 .. F-1 then x2 rows, become [2 Fp] rows, Fp = round_up(F, 64): group g of 64 hidden units holds x1
+// rows 64 g .. 64 g + 63 at 128 g and their x2 rows at 128 g + 64, rows past F zero.  Besides the epilogue this is the only code that
+// knows the layout: the f16 and e4m3 weights, the bias and both GEMM test hooks go through it.
+int swiglu_rows(int F) { return 2 * ((F + SWIGLU_GROUP - 1) / SWIGLU_GROUP * SWIGLU_GROUP); }
+
+template <typename T>
+std::vector<T> swiglu_interleave(const T *src, int F, size_t row_elems)
+{
+    std::vector<T> out((size_t)swiglu_rows(F) * row_elems, T(0));
+    for (int f = 0; f < F; ++f)
+        for (int half = 0; half < 2; ++half)
+        {
+            const size_t dst = (size_t)(2 * SWIGLU_GROUP * (f / SWIGLU_GROUP) + SWIGLU_GROUP * half + f % SWIGLU_GROUP);
+            memcpy(&out[dst * row_elems], src + ((size_t)half * F + f) * row_elems, row_elems * sizeof(T));
+        }
+    return out;
+}
+
 // Weight matrix [n_out][n_in] -> device f16, row pitch padded to ld (zero filled), + its TMA descriptor.
 //   type 1 (F16): used as stored -- the reference's own operand (ggml.c:1200-1236).
 //   type 8 (Q8_0, blocks of {f16 d; int8 q[32]}, ggml-quants.h:42-46): dequantised once to f16(d * q).  The reference
@@ -353,8 +384,10 @@ void dequant_block(int type, const uint8_t *blk, float *y)
 //   type 0 (F32): rounded once to f16 (the reference keeps f32 weights AND f32 activations, ggml.c:1163-1198).
 //   type 30 (BF16, GGUF containers): widened to f32, then as type 0.
 // e4m3: the f16 values are quantised once more (quantize_e4m3) and only the e4m3 copy goes to the device.
+// swiglu: SwiGLU's fc1, n_out = 2 F rows in HF's order; the f16 rows and the bias are interleaved (swiglu_interleave) before the e4m3
+// quantisation, so the device holds swiglu_rows(F) rows.
 int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::string &wname, const std::string &bname,
-                  int n_out, int n_in, int ld, Linear *L, int conv_p = 0, bool e4m3 = false)
+                  int n_out, int n_in, int ld, Linear *L, int conv_p = 0, bool e4m3 = false, bool swiglu = false)
 {
     const vitb200_tensor *w = find_tensor(t, n, wname);
     if (!w) return fail("missing tensor '%s'", wname.c_str());
@@ -364,7 +397,9 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
     if (conv_p > 0) { if (check_shape(w, wname, conv_p, conv_p, n_in / (conv_p * conv_p), n_out)) return 1; } // [P, P, C, D], vit.cpp:515
     else if (check_shape(w, wname, n_in, n_out, 1, 1)) return 1;                                             // [in, out], vit.cpp:531-543
     if (quant_block_bytes(w->type) && n_in % 32 != 0) return fail("tensor '%s': quantised rows must be a multiple of 32", wname.c_str());
-    L->n_out = n_out; L->n_in = n_in; L->ld = ld;
+    const vitb200_tensor *swiglu_b = swiglu ? f32_tensor(t, n, bname, n_out, 1, 1, 1) : nullptr;
+    if (swiglu && !swiglu_b) return 1;
+    const int F = n_out / 2;
     const void *src = w->data;
     std::vector<uint16_t> conv;
     if (w->type != 1)
@@ -404,6 +439,14 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
         }
         src = conv.data();
     }
+    std::vector<uint16_t> inter;
+    if (swiglu)
+    {
+        inter = swiglu_interleave((const uint16_t *)src, F, (size_t)n_in);
+        src = inter.data();
+        n_out = swiglu_rows(F);
+    }
+    L->n_out = n_out; L->n_in = n_in; L->ld = ld;
     if (e4m3)
     {
         std::vector<uint8_t> q((size_t)n_out * n_in);
@@ -417,8 +460,14 @@ int upload_linear(vitb200_engine *e, const vitb200_tensor *t, int n, const std::
         CUDA_TRY(cudaMemset(L->w, 0, (size_t)n_out * ld * sizeof(__half)));
         CUDA_TRY(cudaMemcpy2D(L->w, (size_t)ld * 2, src, (size_t)n_in * 2, (size_t)n_in * 2, (size_t)n_out, cudaMemcpyHostToDevice));
     }
+    if (swiglu)
+    {
+        const std::vector<float> b = swiglu_interleave((const float *)swiglu_b->data, F, 1);
+        if (dev_alloc(e, &L->b, b.size())) return 1;
+        CUDA_TRY(cudaMemcpy(L->b, b.data(), b.size() * sizeof(float), cudaMemcpyHostToDevice));
+    }
     // conv bias is declared [1, 1, D] (vit.cpp:516), every other bias [n_out]; the tail up to a multiple of 4 stays zero
-    if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
+    else if (conv_p > 0 ? upload_f32(e, t, n, bname, 1, 1, n_out, 1, &L->b) : upload_f32(e, t, n, bname, n_out, 1, 1, 1, &L->b, (n_out + 3) / 4 * 4)) return 1;
     const cuuint64_t cols = (cuuint64_t)ld, rows = (cuuint64_t)n_out;
     if (e4m3) return make_tmap(&L->tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, L->w8, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_BN});
     return make_tmap(&L->tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, L->w, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_BN});
@@ -552,7 +601,8 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     if constexpr (gemm_epi_staged(EPI))
     {
         using St = GemmStage<EPI, STAGES>;
-        const cuuint64_t M = (cuuint64_t)p.M, N = (cuuint64_t)p.N, ldo = (cuuint64_t)p.ldo;
+        // SwiGLU stores F columns of the N / 2 it computes
+        const cuuint64_t M = (cuuint64_t)p.M, N = (cuuint64_t)(St::kSwiglu ? p.F : p.N), ldo = (cuuint64_t)p.ldo;
         auto out_map = [&](CUtensorMap *m, const void *ptr) -> int {
             if (!St::kF16) return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, ptr, {N, M}, {4 * ldo}, {32, 64});
             if (p.headmajor)
@@ -578,6 +628,8 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
 int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s, bool e4m3 = false)
 {
     if (p.N % 4 != 0) return fail("GEMM: N = %d is not a multiple of 4", p.N);
+    if (epi == EPI_BIAS_SWIGLU_F16 && (p.F < 1 || p.N != swiglu_rows(p.F)))
+        return fail("SwiGLU GEMM: N = %d is not the interleaved width %d of F = %d", p.N, p.F < 1 ? 0 : swiglu_rows(p.F), p.F);
     const bool deep = p.K >= GEMM_DEEP_K; // ring depth by reduction length (GemmCfg)
     if (e4m3)
     {
@@ -585,7 +637,7 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
 #define VB_CASE(EPI) \
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6, GEMM_OP_E4M3>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, GEMM_OP_E4M3>(e, tmA, tmB, p, s);
         VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
-        VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16)
+        VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16) VB_CASE(EPI_BIAS_SWIGLU_F16)
 #undef VB_CASE
         return fail("no e4m3 GEMM instantiation for epilogue=%d", epi);
     }
@@ -593,6 +645,7 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
     if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
     VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
     VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16) VB_CASE(EPI_BIAS_SCALE_RESID_F32) VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16)
+    VB_CASE(EPI_BIAS_SWIGLU_F16)
 #undef VB_CASE
     return fail("no GEMM instantiation for epilogue=%d", epi);
 }
@@ -708,6 +761,7 @@ int fc1_epilogue(const vitb200_engine *e)
     case 1: return EPI_BIAS_GELU_ERF_F16;
     case 2: return EPI_BIAS_QUICK_GELU_F16;
     case 3: return EPI_BIAS_GELU_PYTORCH_TANH_F16;
+    case 4: return EPI_BIAS_SWIGLU_F16;
     }
     return EPI_BIAS_GELU_F16;
 }
@@ -910,15 +964,16 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (tap && (e->fp8 ? tap_e4m3(taps->ln2, e->A8, e->SA, (size_t)T, (size_t)D, s) : tap_f16(taps->ln2, e->A16, (size_t)T * D, s))) return 1;
         {
             GemmParams p{};
-            p.M = T; p.N = 4 * D; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = 4 * D;
+            // SwiGLU: N = the interleaved 2 round_up(F, 64) rows of fc1, F columns stored
+            p.M = T; p.N = L.fc1.n_out; p.K = D; p.bias = L.fc1.b; p.out = e->H16; p.ldo = e->F; p.F = e->F;
             p.a_scale = e->SA; p.w_scale = L.fc1.w_scale;
-            ProfScope ps(e, PK_FC1, 2.0 * p.M * p.N * p.K, s);
+            ProfScope ps(e, PK_FC1, 2.0 * p.M * (e->arch.activation == 4 ? 2 * e->F : e->F) * p.K, s);
             if (launch_gemm(e, fc1_epilogue(e), e->fp8 ? e->tmA8 : e->tmA_D, L.fc1.tm, p, s, e->fp8)) return 1; // vit.cpp:889-893
         }
-        if (tap && tap_f16(taps->h, e->H16, (size_t)T * 4 * D, s)) return 1;
+        if (tap && tap_f16(taps->h, e->H16, (size_t)T * e->F, s)) return 1;
         {
             GemmParams p{};
-            p.M = T; p.N = D; p.K = 4 * D; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X; p.gamma = L.ls2;
+            p.M = T; p.N = D; p.K = e->F; p.bias = L.fc2.b; p.out = e->X; p.ldo = D; p.resid = e->X; p.gamma = L.ls2;
             ProfScope ps(e, PK_FC2, 2.0 * p.M * p.N * p.K, s);
             if (launch_gemm(e, resid_epilogue(e), e->tmA_H, L.fc2.tm, p, s)) return 1; // fc2 + residual, vit.cpp:896-900
         }
@@ -1263,8 +1318,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
                     hp->num_hidden_layers, hp->num_attention_heads, hp->num_classes, hp->patch_size, hp->img_size);
     const vitb200_arch ar = arch ? *arch : vitb200_arch{};
     if (ar.pre_norm != 0 && ar.pre_norm != 1) return fail("vitb200_arch.pre_norm = %d out of range (0 none, 1 LayerNorm 'norm_pre')", ar.pre_norm);
-    if (ar.activation < 0 || ar.activation > 3)
-        return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh)", ar.activation);
+    if (ar.activation < 0 || ar.activation > 4)
+        return fail("vitb200_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh, 4 swiglu)", ar.activation);
     if (ar.layer_scale != 0 && ar.layer_scale != 1)
         return fail("vitb200_arch.layer_scale = %d out of range (0 none, 1 LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma')", ar.layer_scale);
     if (ar.reg_tokens < 0 || ar.reg_tokens > VB_MAX_REG_TOKENS)
@@ -1273,6 +1328,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (ar.activation == 3 && ar.pool < 2)
         return fail("vitb200_arch.activation = 3 out of range for pool %d: gelu_pytorch_tanh is the SigLIP towers' activation (pools 2 map and "
                     "3 mean)", ar.pool);
+    if (ar.activation == 4 && ar.pool >= 2)
+        return fail("vitb200_arch.activation = 4 out of range for pool %d: swiglu is DINOv2's MLP (pools 0 token and 1 cls_patch_mean)", ar.pool);
     if (ar.pool >= 2)
     {
         // SigLIP: the token rows are the patch rows alone
@@ -1298,6 +1355,28 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         }
     if (ar.reg_tokens > 0 && !find_tensor(t, n, "reg_token"))
         return fail("vitb200_arch.reg_tokens = %d needs the tensor 'reg_token'", ar.reg_tokens);
+    // the MLP's hidden width: 4 D, or SwiGLU's F, from block 0's fc1 [2 F][D]; every block's fc1 and fc2 [D][F] must agree with it
+    int F = 4 * hp->hidden_size;
+    if (ar.activation == 4)
+    {
+        const vitb200_tensor *w1 = find_tensor(t, n, "blocks.0.mlp.fc1.weight");
+        if (!w1) return fail("missing tensor 'blocks.0.mlp.fc1.weight'");
+        const int64_t rows = dim_of(w1, 1), f = rows / 2;
+        if (rows % 2) return fail("vitb200_arch.activation = 4 (swiglu) needs an even row count 2 F in 'blocks.0.mlp.fc1.weight', got %lld", (long long)rows);
+        if (f % 8) return fail("vitb200_arch.activation = 4 (swiglu): F = %lld is not a multiple of 8", (long long)f);
+        if (f < 8 || f > 8 * (int64_t)hp->hidden_size)
+            return fail("vitb200_arch.activation = 4 (swiglu): F = %lld out of range (8..%d = 8 D)", (long long)f, 8 * hp->hidden_size);
+        F = (int)f;
+        for (int i = 0; i < hp->num_hidden_layers; ++i)
+        {
+            const std::string p = "blocks." + std::to_string(i) + ".mlp.";
+            const vitb200_tensor *a = find_tensor(t, n, p + "fc1.weight"), *b = find_tensor(t, n, p + "fc2.weight");
+            if ((a && dim_of(a, 1) != 2 * f) || (b && dim_of(b, 0) != f))
+                return fail("vitb200_arch.activation = 4 (swiglu): block %d's mlp.fc1 [%lld][%lld] or mlp.fc2 [%lld][%lld] disagrees with F = %d "
+                            "(fc1 [2 F][D], fc2 [D][F])", i, a ? (long long)dim_of(a, 1) : 0ll, a ? (long long)dim_of(a, 0) : 0ll,
+                            b ? (long long)dim_of(b, 1) : 0ll, b ? (long long)dim_of(b, 0) : 0ll, F);
+        }
+    }
     if (ar.pool && head_tokens != 1) return fail("vitb200_arch.pool = %d needs head_tokens = 1 (got %d)", ar.pool, head_tokens);
     {
         // the head's K: the pooled row it reads is D wide, or 2 D with the class-plus-patch-mean pool
@@ -1342,6 +1421,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     e->G = hp->img_size / P;
     e->NP = e->G * e->G;
     e->N = e->NP + prefix_rows(ar);
+    e->F = F;
     e->C = in_chans;
     e->head_tokens = head_tokens;
     e->KH = (ar.pool == 1 ? 2 : 1) * hp->hidden_size;
@@ -1373,8 +1453,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
             return 1;
         if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv, 0, fp8) ||
             upload_linear(e, t, n, p + "attn.proj.weight", p + "attn.proj.bias", D, D, D, &L.proj) ||
-            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", 4 * D, D, D, &L.fc1, 0, fp8) ||
-            upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, 4 * D, 4 * D, &L.fc2))
+            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", ar.activation == 4 ? 2 * F : F, D, D, &L.fc1, 0, fp8, ar.activation == 4) ||
+            upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, F, F, &L.fc2))
             return 1;
         if (ar.layer_scale && (upload_f32(e, t, n, p + "ls1.gamma", D, 1, 1, 1, &L.ls1) || upload_f32(e, t, n, p + "ls2.gamma", D, 1, 1, 1, &L.ls2)))
             return 1;
@@ -1392,12 +1472,13 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
 
     // ---- activation arena
     const size_t B = (size_t)max_batch, T = B * e->N;
-    const size_t h16 = T * 4 * D;
+    const size_t R = B * (size_t)e->head_tokens;                        // classifier rows: pooled tokens of all images
+    // the MLP hidden buffer, which the features calls also use to stage T x D f32 tokens and R pooled f32 rows (features_to_host)
+    const size_t h16 = std::max(T * F, 2 * T * D + 2 * R * e->KH);
     // The patch matrix [B*NP][KPp] aliases the MLP hidden buffer (dead while the patch GEMM runs) when it fits and
     // has no K padding; otherwise it gets its own buffer whose zeroed padding columns are never written again.
     const size_t pa_elems = B * e->NP * e->KPp;
     const bool pa_alias = (e->KPp == e->KP) && pa_elems <= h16;
-    const size_t R = B * (size_t)e->head_tokens;                        // classifier rows: pooled tokens of all images
     const size_t img_elems = (size_t)e->C * hp->img_size * hp->img_size; // per image
     if (dev_alloc(e, &e->X, T * D) || dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->H16, h16) ||
         dev_alloc(e, &e->CLS16, R * e->KH) || dev_alloc(e, &e->d_logits, R * e->Cp))
@@ -1428,7 +1509,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         return e4m3 ? make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, ptr, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_A_BOX_ROWS})
                     : make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_A_BOX_ROWS});
     };
-    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, 4 * (cuuint64_t)D) || a_map(&e->tmA_P, e->PA, B * e->NP, e->KPp) ||
+    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, (cuuint64_t)F) || a_map(&e->tmA_P, e->PA, B * e->NP, e->KPp) ||
         a_map(&e->tmA_C, e->CLS16, R, e->KH))
         return 1;
     if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
@@ -1617,6 +1698,7 @@ int vitb200_last_launch_count(const vitb200_engine *e) { return e ? e->launches 
 int vitb200_in_chans(const vitb200_engine *e) { return e ? e->C : 0; }
 int vitb200_head_tokens(const vitb200_engine *e) { return e ? e->head_tokens : 0; }
 int vitb200_fp8(const vitb200_engine *e) { return e && e->fp8 ? 1 : 0; }
+int vitb200_mlp_dim(const vitb200_engine *e) { return e ? e->F : 0; }
 
 int vitb200_profile_enable(vitb200_engine *e, int on)
 {
@@ -2151,27 +2233,35 @@ static int test_gemm_impl(int device, int M, int N, int K, int epilogue, const u
     if (gemm_epi_resid(epilogue) && !resid) return fail("resid required");
     if ((epilogue == EPI_BIAS_SCALE_RESID_F32) != (gamma != nullptr))
         return fail("gamma goes with the LayerScale epilogue %d only (vitb200_test_gemm_layer_scale)", EPI_BIAS_SCALE_RESID_F32);
+    const bool swiglu = epilogue == EPI_BIAS_SWIGLU_F16;
+    if (swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
     EnginePtr owner;
     if (scratch_engine(device, owner)) return 1;
     vitb200_engine *e = owner.get();
     const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
-                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16 || epilogue == EPI_BIAS_GELU_PYTORCH_TANH_F16;
-    const size_t MN = (size_t)M * N;
+                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16 || epilogue == EPI_BIAS_GELU_PYTORCH_TANH_F16 || swiglu;
+    // SwiGLU: W and bias interleaved as the engine uploads them, Nw rows computed, out [M][N / 2]
+    const int F = N / 2, Nw = swiglu ? swiglu_rows(F) : N, No = swiglu ? F : N;
+    std::vector<uint16_t> wi;
+    std::vector<float> bi;
+    if (swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
+    const size_t MN = (size_t)M * No;
     __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
     float *dB = nullptr, *o32 = nullptr;
-    if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dB, bias, N)) return 1;
+    if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dB, bias, Nw)) return 1;
     if (f16out && (dev_alloc(e, &hi, MN) || (epilogue == EPI_BIAS_F16_HILO && dev_alloc(e, &lo, MN)))) return 1;
     // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
     if (!f16out && (gemm_epi_resid(epilogue) ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
     float *dG = nullptr;
     if (gamma && upload(e, &dG, gamma, N)) return 1;
     CUtensorMap tA, tB;
-    const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
+    const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)Nw, Ku = (cuuint64_t)K;
     if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dA, {Ku, Mu}, {2 * Ku}, {GEMM_BK, GEMM_A_BOX_ROWS}) ||
         make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dW, {Ku, Nu}, {2 * Ku}, {GEMM_BK, GEMM_BN}))
         return 1;
     GemmParams p{};
-    p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = N; p.resid = o32; p.gamma = dG;
+    p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = No; p.resid = o32; p.gamma = dG;
+    p.F = F;
     if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
     // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
     return f16out ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
@@ -2219,26 +2309,33 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
     return guarded(__func__, [&]() -> int {
         if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
         if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
+        const bool swiglu = epilogue == EPI_BIAS_SWIGLU_F16;
         if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 &&
-            epilogue != EPI_BIAS_QUICK_GELU_F16 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16)
-            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8, 10)", epilogue);
+            epilogue != EPI_BIAS_QUICK_GELU_F16 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16 && !swiglu)
+            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8, 10, 11)", epilogue);
+        if (swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
         EnginePtr owner;
         if (scratch_engine(device, owner)) return 1;
         vitb200_engine *e = owner.get();
-        const size_t MN = (size_t)M * N;
+        // SwiGLU: W and bias interleaved as the engine uploads them, Nw rows computed, out [M][N / 2]
+        const int F = N / 2, Nw = swiglu ? swiglu_rows(F) : N, No = swiglu ? F : N;
+        std::vector<uint8_t> wi;
+        std::vector<float> bi;
+        if (swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
+        const size_t MN = (size_t)M * No;
         uint8_t *dA = nullptr, *dW = nullptr;
         float *dS = nullptr, *dB = nullptr;
         __half *hi = nullptr, *lo = nullptr;
-        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)N * K) || upload(e, &dS, a_scale, M) || upload(e, &dB, bias, N) ||
+        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dS, a_scale, M) || upload(e, &dB, bias, Nw) ||
             dev_alloc(e, &hi, MN) || dev_alloc(e, &lo, MN))
             return 1;
         CUtensorMap tA, tB;
-        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)N, Ku = (cuuint64_t)K;
+        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)Nw, Ku = (cuuint64_t)K;
         if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, dA, {Ku, Mu}, {Ku}, {2 * GEMM_BK, GEMM_A_BOX_ROWS}) ||
             make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_UINT8, dW, {Ku, Nu}, {Ku}, {2 * GEMM_BK, GEMM_BN}))
             return 1;
         GemmParams p{};
-        p.M = M; p.N = N; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = N; p.a_scale = dS; p.w_scale = w_scale;
+        p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = No; p.a_scale = dS; p.w_scale = w_scale; p.F = F;
         if (run_scratch(e, "e4m3 GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, true); })) return 1;
         // split-precision result: hi + lo (exact in f32); the other epilogues' hi alone, so that a -0 stays -0
         return tap_f16(out, hi, MN, e->stream, epilogue == EPI_BIAS_F16_HILO ? lo : nullptr);

@@ -64,6 +64,7 @@ enum GemmEpilogue
     EPI_BIAS_QUICK_GELU_F16 = 8, // out f16 = f16(quick_gelu(acc + bias)), likewise                               (fc1 of OpenAI CLIP)
     EPI_BIAS_SCALE_RESID_F32 = 9, // out f32 = f32((acc + bias) * gamma[n]) + resid: LayerScale, HF's order    (proj, fc2 of DINOv2)
     EPI_BIAS_GELU_PYTORCH_TANH_F16 = 10, // out f16 = f16(gelu_tanh(acc + bias)), x in f32 without rounding to f16 first (fc1 of SigLIP)
+    EPI_BIAS_SWIGLU_F16 = 11, // out f16 [M][F] = f16(silu(x1) * x2), x = acc + bias in f32, W interleaved by 64 (fc1 of DINOv2 ViT-g; below)
 };
 
 struct GemmParams
@@ -82,6 +83,7 @@ struct GemmParams
     const float *a_scale; // GEMM_OP_E4M3: [M] f32, the scale of each A row
     float w_scale;        // GEMM_OP_E4M3: the scale of W
     const float *gamma;   // EPI_BIAS_SCALE_RESID_F32: [N] f32, the LayerScale of each output column
+    int F;                // EPI_BIAS_SWIGLU_F16: the columns of out; N = 2 round_up(F, 64)
 };
 
 constexpr int GEMM_BM = 128; // rows of a tile
@@ -133,11 +135,27 @@ __device__ __forceinline__ float quick_gelu_f32(float x)
     return x * ptx::rcp_approx(1.0f + e);
 }
 
+// SiLU, SwiGLU's gate: x sigma(x) = x / (1 + e^{-x}), in the form of quick_gelu_f32.  For x << 0, e^{-x} is +inf, its reciprocal 0 and
+// the result -0; never NaN for a finite x.
+__device__ __forceinline__ float silu_f32(float x)
+{
+    const float e = ptx::ex2_approx(x * -1.4426950408889634f); // -log2(e)
+    return x * ptx::rcp_approx(1.0f + e);
+}
+
+// SwiGLU (EPI_BIAS_SWIGLU_F16).  HF's fc1 is [2 F][K]: rows 0 .. F-1 give x1, rows F .. 2F-1 its partners x2, h = silu(x1) x2.  The
+// weights and the bias are interleaved at upload in groups of 64 hidden units (swiglu_interleave in engine.cu): rows 128 g .. 128 g + 63
+// are x1 rows 64 g .., rows 128 g + 64 .. 128 g + 127 the matching x2 rows, rows past F zero, so the GEMM runs with N = 2 round_up(F, 64).
+// Each 128-column tile then holds, in the same thread, x1 in its 8-column groups j < 8 and the partner x2 in group j + 8; a pass (one
+// 64-row half) stores one 64-column f16 box at column n0 / 2 of out [M][F], and the store map covers F columns, so padding is never stored.
+constexpr int SWIGLU_GROUP = 64;
+
 // Epilogues whose result goes out through shared memory and TMA stores (the rest store from registers)
 __host__ __device__ constexpr bool gemm_epi_staged(int epi)
 {
     return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32 ||
-           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32 || epi == EPI_BIAS_GELU_PYTORCH_TANH_F16;
+           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32 || epi == EPI_BIAS_GELU_PYTORCH_TANH_F16 ||
+           epi == EPI_BIAS_SWIGLU_F16;
 }
 
 // Epilogues that add the residual stream (loaded into the staging buffer with TMA)
@@ -151,15 +169,18 @@ struct GemmStage
 {
     using Cfg = GemmCfg<STAGES>;
     static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_GELU_ERF_F16 ||
-                                  EPI == EPI_BIAS_QUICK_GELU_F16 || EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16);
+                                  EPI == EPI_BIAS_QUICK_GELU_F16 || EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16 || EPI == EPI_BIAS_SWIGLU_F16);
+    static constexpr bool kSwiglu = EPI == EPI_BIAS_SWIGLU_F16;
     static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
     static constexpr int kBoxCols = kF16 ? 64 : 32;
     static constexpr int kBoxBytes = 64 * 128;
     static constexpr int kFitCols = Cfg::kStageBytes / (64 * kOuts * (kF16 ? 2 : 4));
     static constexpr int kPassCols = kFitCols < GEMM_BN ? kFitCols : GEMM_BN; // 16 KB: 128 (f16), 64 (hi + lo, f32); 32 KB: 128
+    static_assert(!kSwiglu || kPassCols == GEMM_BN, "SwiGLU: a pass holds both halves of its 64 outputs");
+    static constexpr int kStoreCols = kSwiglu ? kPassCols / 2 : kPassCols; // output columns a pass stores
     static constexpr int kColGroups = GEMM_BN / kPassCols;
     static constexpr int kPasses = 2 * kColGroups; // row half outer, column group inner
-    static constexpr int kColBoxes = kPassCols / kBoxCols;
+    static constexpr int kColBoxes = kStoreCols / kBoxCols;
     static constexpr int kPassBytes = kOuts * kColBoxes * kBoxBytes;
     static constexpr int kSlots = Cfg::kStageBytes / kPassBytes; // passes the buffer holds at once (2: f16 in 32 KB)
     static_assert(kSlots * kPassBytes == Cfg::kStageBytes, "passes tile the staging buffer");
@@ -391,10 +412,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                     resid_ph ^= 1;
                 }
 #pragma unroll
-                for (int jj = 0; jj < St::kPassCols / 8; ++jj)
+                for (int jj = 0; jj < St::kStoreCols / 8; ++jj)
                 {
                     const int j = cg * (St::kPassCols / 8) + jj; // 8-column group of the tile
                     const float2 b = *reinterpret_cast<const float2 *>(&s_bias[cw][8 * j + 2 * q]);
+                    float2 b2 = make_float2(0.f, 0.f); // SwiGLU: the bias of the x2 partners (group j + 8)
+                    if constexpr (St::kSwiglu) b2 = *reinterpret_cast<const float2 *>(&s_bias[cw][8 * (j + 8) + 2 * q]);
                     float2 g = make_float2(0.f, 0.f); // LayerScale: the column pair's gamma (columns past N are never stored)
                     if constexpr (kGammaSmem) g = *reinterpret_cast<const float2 *>(&s_gamma[cw][8 * jj + 2 * q]);
                     else if constexpr (EPI == EPI_BIAS_SCALE_RESID_F32)
@@ -419,6 +442,12 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                             else if constexpr (EPI == EPI_BIAS_QUICK_GELU_F16) hv = __floats2half2_rn(quick_gelu_f32(x0), quick_gelu_f32(x1));
                             else if constexpr (EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16) // PyTorch's tanh GELU: x itself, no f16 table
                                 hv = __floats2half2_rn(gelu_tanh_f32(x0), gelu_tanh_f32(x1));
+                            else if constexpr (St::kSwiglu) // x0, x1 are x1 of two columns; their x2 partners sit 64 columns on
+                            {
+                                float g0 = acc[hm][4 * (j + 8) + 2 * h], g1 = acc[hm][4 * (j + 8) + 2 * h + 1];
+                                if constexpr (kE4M3) { g0 = __fmul_rn(g0, row_scale[h]); g1 = __fmul_rn(g1, row_scale[h]); }
+                                hv = __floats2half2_rn(__fmul_rn(silu_f32(x0), __fadd_rn(g0, b2.x)), __fmul_rn(silu_f32(x1), __fadd_rn(g1, b2.y)));
+                            }
                             else hv = __floats2half2_rn(x0, x1);
                             ptx::st_shared_b32(a + St::box(0, jj / 8), *reinterpret_cast<const uint32_t *>(&hv));
                             if constexpr (EPI == EPI_BIAS_F16_HILO)
@@ -461,6 +490,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                 ptx::tma_store_3d(&tmOut, src, 0, row, plane);
                                 if constexpr (EPI == EPI_BIAS_F16_HILO) ptx::tma_store_3d(&tmAux, buf + St::box(1, c), 0, row, plane);
                             }
+                            else if constexpr (St::kSwiglu) ptx::tma_store_2d(&tmOut, src, c0 / 2, row);
                             else
                             {
                                 ptx::tma_store_2d(&tmOut, src, c0 + 64 * c, row);

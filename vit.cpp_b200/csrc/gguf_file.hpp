@@ -8,7 +8,7 @@
 //     vit.hidden_size, vit.num_hidden_layers, vit.num_attention_heads, vit.num_classes, vit.patch_size, vit.image_size  (integers)
 //     vit.layer_norm_eps (float32, default 1e-6)           vit.id2label (array of strings, index = class id; optional)
 //     vit.pre_norm (bool or integer, default 0: 1 = a LayerNorm 'norm_pre' before block 0, as in CLIP towers)
-//     vit.activation (string, default "gelu_tanh"; "gelu_erf", "quick_gelu" or "gelu_pytorch_tanh": the MLP activation)
+//     vit.activation (string, default "gelu_tanh"; "gelu_erf", "quick_gelu", "gelu_pytorch_tanh" or "swiglu": the MLP activation)
 //     vit.layer_scale (bool or integer, default 0: 1 = LayerScale gammas 'blocks.{i}.ls1.gamma' / 'ls2.gamma', as in DINOv2)
 //     vit.reg_tokens (integer, default 0: register tokens 'reg_token' after the class token)
 //     vit.pool (string, default "token"; "cls_patch_mean": the head reads the class token || the mean of the patch tokens; "map" or
@@ -38,7 +38,7 @@ struct GgufModel
     int64_t hidden_size = 0, num_hidden_layers = 0, num_attention_heads = 0, num_classes = 0, patch_size = 0, img_size = 0, ftype = 1;
     float eps = 1e-6f;
     int64_t pre_norm = 0; // vit.pre_norm (vitb200_arch.pre_norm; the loader checks the range)
-    int32_t activation = 0; // vit.activation: 0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh (vitb200_arch.activation)
+    int32_t activation = 0; // vit.activation: 0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh, 4 swiglu (vitb200_arch.activation)
     int64_t layer_scale = 0, reg_tokens = 0; // vit.layer_scale, vit.reg_tokens (vitb200_arch; the loader checks the ranges)
     int32_t pool = 0;       // vit.pool: 0 token, 1 cls_patch_mean, 2 map, 3 mean (vitb200_arch.pool)
     std::map<int, std::string> labels;
@@ -102,7 +102,8 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
                 else if (v == "gelu_erf") m.activation = 1;
                 else if (v == "quick_gelu") m.activation = 2;
                 else if (v == "gelu_pytorch_tanh") m.activation = 3;
-                else return fail("unknown vit.activation '" + v + "' (gelu_tanh, gelu_erf, quick_gelu or gelu_pytorch_tanh)");
+                else if (v == "swiglu") m.activation = 4;
+                else return fail("unknown vit.activation '" + v + "' (gelu_tanh, gelu_erf, quick_gelu, gelu_pytorch_tanh or swiglu)");
             }
             else if (key == "vit.pool")
             {

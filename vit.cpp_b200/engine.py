@@ -16,7 +16,7 @@ from typing import Optional
 
 import numpy as np
 
-from .ggml_file import ACTIVATIONS, PATCH_ONLY_POOLS, POOLS  # vitb200_arch.activation / .pool -> name (GGUF vit.activation / vit.pool)
+from .ggml_file import ARCH_ACTIVATIONS, PATCH_ONLY_POOLS, POOLS  # vitb200_arch.activation / .pool -> name (GGUF vit.activation / vit.pool)
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
@@ -34,7 +34,7 @@ class Hparams(C.Structure):
 
 
 class Arch(C.Structure):
-    """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ACTIVATIONS, layer_scale 0 / 1,
+    """vitb200_arch (include/vitb200.h): pre_norm 0 / 1, activation an index into ggml_file.ARCH_ACTIVATIONS, layer_scale 0 / 1,
     reg_tokens 0..16, pool an index into ggml_file.POOLS (2 and 3: SigLIP, no class token).  Fields not given are 0: Arch(pre_norm,
     activation) is a CLIP tower."""
     _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32), ("layer_scale", C.c_int32), ("reg_tokens", C.c_int32),
@@ -81,6 +81,7 @@ def lib():
         L.vitb200_create_fp8.argtypes = [vp, vp, i32, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_create_from_file_fp8.argtypes = [C.c_char_p, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_fp8.argtypes = [vp]
+        L.vitb200_mlp_dim.argtypes = [vp]
         L.vitb200_create_arch.argtypes = [vp, C.POINTER(Arch), vp, i32, i32, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_get_arch.argtypes = [vp, C.POINTER(Arch)]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
@@ -144,8 +145,9 @@ class VitModel:
         self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
         a = Arch()
         _check(lib().vitb200_get_arch(self._h, C.byref(a)), "vitb200_get_arch")
-        # the architecture (vitb200_arch): {"pre_norm": bool, "activation": one of ACTIVATIONS}; the reference's is (False, "gelu_tanh")
-        self.arch = {"pre_norm": bool(a.pre_norm), "activation": ACTIVATIONS[a.activation]}
+        # the architecture (vitb200_arch): {"pre_norm": bool, "activation": one of ARCH_ACTIVATIONS}; the reference's is (False, "gelu_tanh")
+        self.arch = {"pre_norm": bool(a.pre_norm), "activation": ARCH_ACTIVATIONS[a.activation]}
+        self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or SwiGLU's F
         # DINOv2 (vitb200_arch): LayerScale on, register tokens (rows 1 .. reg_tokens of every image), the head's input (one of POOLS)
         self.layer_scale, self.reg_tokens, self.pool = bool(a.layer_scale), int(a.reg_tokens), POOLS[a.pool]
         self.n_tokens += self.reg_tokens
@@ -219,7 +221,7 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
         for i in range(4):
             t.ne[i] = ne[i] if i < len(ne) else 1
     hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, vf.eps)
-    act = ACTIVATIONS.index(vf.activation) if vf.activation in ACTIVATIONS else -1  # an unknown name is refused by the engine
+    act = ARCH_ACTIVATIONS.index(vf.activation) if vf.activation in ARCH_ACTIVATIONS else -1  # an unknown name is refused by the engine
     pool = POOLS.index(vf.pool) if vf.pool in POOLS else -1  # likewise
     arch = Arch(int(vf.pre_norm), act, int(vf.layer_scale), int(vf.reg_tokens), pool)
     h = C.c_void_p()
@@ -414,6 +416,8 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
         shape = TAP_SHAPES[n](B, model.n_tokens, model.hidden_size)
         if n == "final_ln" and model.pool == "cls_patch_mean":
             shape = (B, 2 * model.hidden_size)
+        if n == "h":
+            shape = (B, model.n_tokens, model.mlp_dim)
         out[n] = np.zeros(lead + shape[1:] if n == "final_ln" else shape, np.float32)
         setattr(tp, n, out[n].ctypes.data)
     _check(lib().vitb200_forward_debug(model.handle, imgs.ctypes.data, B, probs.ctypes.data, logits.ctypes.data,
@@ -484,13 +488,17 @@ def test_dequant(ggml_type: int, blocks: np.ndarray) -> np.ndarray:
     return out.view(np.float16)
 
 
+# the SwiGLU epilogue of vitb200_test_gemm / vitb200_test_gemm_fp8: W [N][K] in HF's order (N = 2 F), out [M][N / 2]
+EPI_SWIGLU = 11
+
+
 def test_gemm(M: int, N: int, K: int, epilogue: int, A16: np.ndarray, W16: np.ndarray, bias: np.ndarray,
               resid: Optional[np.ndarray] = None, device: int = 0) -> np.ndarray:
     A = np.ascontiguousarray(A16, np.float16)
     W = np.ascontiguousarray(W16, np.float16)
     b = np.ascontiguousarray(bias, np.float32)
     r = np.ascontiguousarray(resid, np.float32) if resid is not None else None
-    out = np.empty((M, N), np.float32)
+    out = np.empty((M, N // 2 if epilogue == EPI_SWIGLU else N), np.float32)
     _check(lib().vitb200_test_gemm(device, M, N, K, epilogue, A.ctypes.data, W.ctypes.data, b.ctypes.data,
                                    r.ctypes.data if r is not None else None, out.ctypes.data), "vitb200_test_gemm")
     return out
@@ -551,12 +559,13 @@ def test_quantize_fp8(w16: np.ndarray):
 
 def test_gemm_fp8(M: int, N: int, K: int, epilogue: int, A8: np.ndarray, a_scale: np.ndarray, W8: np.ndarray, w_scale: float,
                   bias: np.ndarray, device: int = 0) -> np.ndarray:
-    """The e4m3 GEMM alone (vitb200_test_gemm_fp8): A8 uint8 [M][K], W8 uint8 [N][K] e4m3 bytes -> float32 [M][N]."""
+    """The e4m3 GEMM alone (vitb200_test_gemm_fp8): A8 uint8 [M][K], W8 uint8 [N][K] e4m3 bytes -> float32 [M][N] ([M][N / 2] for
+    EPI_SWIGLU)."""
     A = np.ascontiguousarray(A8, np.uint8)
     W = np.ascontiguousarray(W8, np.uint8)
     sa = np.ascontiguousarray(a_scale, np.float32)
     b = np.ascontiguousarray(bias, np.float32)
-    out = np.empty((M, N), np.float32)
+    out = np.empty((M, N // 2 if epilogue == EPI_SWIGLU else N), np.float32)
     _check(lib().vitb200_test_gemm_fp8(device, M, N, K, epilogue, A.ctypes.data, sa.ctypes.data, W.ctypes.data, float(w_scale),
                                        b.ctypes.data, out.ctypes.data), "vitb200_test_gemm_fp8")
     return out

@@ -26,8 +26,11 @@ import numpy as np
 GGML_FILE_MAGIC = 0x67676D6C
 QK8_0 = 32  # ggml-quants.h:42-46 block_q8_0 { f16 d; int8 qs[32]; }
 # MLP activations, in the order of vitb200_arch.activation: the reference's tanh GELU (ggml's f16 table), erf GELU, QuickGELU, PyTorch's
-# tanh GELU on the f32 pre-activation (SigLIP)
+# tanh GELU on the f32 pre-activation (SigLIP); these are the element-wise ones, which a timm state dict may ask for
 ACTIVATIONS = ("gelu_tanh", "gelu_erf", "quick_gelu", "gelu_pytorch_tanh")
+# every vitb200_arch.activation: the above and 4, SwiGLU (DINOv2 ViT-g's gated MLP: fc1 [2 F][D] in HF's x1 | x2 order, h = silu(x1) x2,
+# fc2 [D][F])
+ARCH_ACTIVATIONS = ACTIVATIONS + ("swiglu",)
 # head inputs, in the order of vitb200_arch.pool: the first head_tokens rows, DINOv2's LN(class token) || mean of LN(patch tokens), and
 # SigLIP's (no class token) attention-pooling head or mean of LN(tokens)
 POOLS = ("token", "cls_patch_mean", "map", "mean")
@@ -80,7 +83,7 @@ class VitFile:
     # reference's, the only values a legacy-ggml file can carry
     eps: float = 1e-6
     pre_norm: int = 0            # 1: LayerNorm 'norm_pre.*' on the embeddings before block 0 (CLIP towers)
-    activation: str = "gelu_tanh"  # MLP activation: one of ACTIVATIONS
+    activation: str = "gelu_tanh"  # MLP activation: one of ARCH_ACTIVATIONS
     # DINOv2 (GGUF keys vit.layer_scale, vit.reg_tokens, vit.pool)
     layer_scale: int = 0         # 1: LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma' on the attention and MLP branches
     reg_tokens: int = 0          # register tokens 'reg_token' [1, R, D], rows 1 .. R of every image
@@ -335,8 +338,8 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
     if vf.pre_norm:
         kv_u32("vit.pre_norm", int(vf.pre_norm))
     if vf.activation != "gelu_tanh":
-        if vf.activation not in ACTIVATIONS:
-            raise ValueError(f"write_gguf: unknown activation {vf.activation!r} ({', '.join(ACTIVATIONS)})")
+        if vf.activation not in ARCH_ACTIVATIONS:
+            raise ValueError(f"write_gguf: unknown activation {vf.activation!r} ({', '.join(ARCH_ACTIVATIONS)})")
         kv.append(gstr(b"vit.activation") + struct.pack("<I", _GGUF_STR) + gstr(vf.activation.encode()))
     if vf.layer_scale:
         kv_u32("vit.layer_scale", int(vf.layer_scale))
