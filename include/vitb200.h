@@ -306,7 +306,8 @@ int vitb200_forward_debug(vitb200_engine *e, const float *images, int batch, flo
  * epilogue: 0 bias->f16, 1 bias+gelu->f16, 2 bias+resid->f32, 4 bias->f32, 6 bias->split precision (hi = f16(x), lo = f16(x - hi);
  * `out` receives hi + lo), 7 bias+gelu_erf->f16, 8 bias+quick_gelu->f16, 10 bias+gelu_pytorch_tanh->f16 (vitb200_arch.activation 1, 2
  * and 3), 11 SwiGLU->f16 (activation 4: W [N][K] and bias [N] in HF's order, N = 2 F, F % 8 == 0; out [M][N / 2] = f16(silu(x1) x2)).
- * out is float32[M][N] on the host (f16 results widened).  resid may be NULL unless epilogue == 2. */
+ * out is float32[M][N] on the host (f16 results widened).  resid may be NULL unless epilogue == 2.  Any other epilogue is refused
+ * before the device is touched (3, the patch embedding, needs the position table; 9 runs through vitb200_test_gemm_layer_scale). */
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W,
                       const float *bias, const float *resid, float *out);
 

@@ -1,5 +1,6 @@
 """The FP8 engine on the GPU: the e4m3 GEMM element by element, the e4m3 LayerNorm against the emulation, end-to-end logits against
 the emulation of the recipe (tests/fp8_reference.py), and every entry point on an FP8 engine."""
+import math
 import os
 
 import numpy as np
@@ -8,6 +9,7 @@ import pytest
 from tests.util import pkg, gf, model_path
 from tests import fp8_reference as fr
 from tests.test_fp8_abi import FP8_FLOOR_MAX
+from tests import test_gpu_gemm_schedule as gs
 from oracle import restatement as rs
 
 eng = pkg.engine
@@ -29,7 +31,9 @@ def _sms():
 # ---- GEMM, exact ---------------------------------------------------------------------------------------------------------------
 def _check_exact(M, N, K, epi, seed):
     """Small-integer e4m3 operands (|v| <= 4, exact in e4m3) with power-of-two scales: A is sparse enough that sum_k |a| |w| < 2^11 on
-    every row, so every partial sum is an integer below 2^11 and the result does not depend on the accumulator's width or order."""
+    every row, so every partial sum is an integer below 2^11 and the result does not depend on the accumulator's width or order.
+    Epilogues 7, 8, 10 and 11 also get -1e4 in every TAIL_EVERY-th bias column (of x1 for SwiGLU), and are checked as functions of x
+    (of the pair x1, x2), as in test_gpu_gemm_schedule.py: x is a multiple of 1/8 (scales 1/8 .. 1/2)."""
     rng = np.random.default_rng(seed)
     keep = min(1.0, 96.0 / K)
     A = rng.integers(-2, 3, size=(M, K)) * (rng.random((M, K)) < keep)
@@ -38,22 +42,31 @@ def _check_exact(M, N, K, epi, seed):
     sa = (2.0 ** rng.integers(-1, 2, size=M)).astype(np.float32)
     sw = np.float32(0.25)
     bias = rng.integers(-8, 9, size=N).astype(np.float32)
+    if epi in gs.NEW:
+        bias[:N // 2 if epi == gs.EPI_SWIGLU else N:gs.TAIL_EVERY] = -1e4
     out = eng.test_gemm_fp8(M, N, K, epi, fr.e4m3_bits(A), sa, fr.e4m3_bits(W), sw, bias)
     acc = A.astype(np.float64) @ W.astype(np.float64).T  # BLAS in f64 on integers below 2^11: exact
-    x = (acc * (sa[:, None].astype(np.float64) * sw) + bias).astype(np.float32)  # exact: at most 11 + 4 significant bits
+    x = (acc * (sa[:, None].astype(np.float64) * sw) + bias).astype(np.float32)  # exact: at most 11 + 4 significant bits (17 with -1e4)
+    if epi in gs.NEW:
+        q = (x.astype(np.float64) * 8).astype(np.int64)
+        assert np.array_equal(q / 8, x)
+        if epi == gs.EPI_SWIGLU:
+            assert out.shape == (M, N // 2)
+            want = gs.check_swiglu(out, q[:, :N // 2], q[:, N // 2:], 0.125)
+        else:
+            want = gs.check_activation(out, q, 0.125, epi)
+        return gs.assert_same_bits(out, want)
     if epi == 6:
         want = x  # hi + lo carries 22 bits
     elif epi == 0:
         want = x.astype(np.float16).astype(np.float32)
     elif epi == 1:
         # as in test_gpu_gemm_schedule.py: each output a function of its f16 pre-activation, within one f16 ulp of the table
-        x16 = x.astype(np.float16)
-        vals, inv = np.unique(x16, return_inverse=True)
-        inv = inv.reshape(-1)
-        per_value = np.zeros(vals.size, np.float32)
-        per_value[inv] = out.reshape(-1)
-        want = per_value[inv].reshape(out.shape)
-        table = rs.gelu_table(vals.astype(np.float32))
+        x16 = x.astype(np.float16).astype(np.float32)
+        q = (x16 * 8).astype(np.int64)  # f16 rounds a multiple of 1/8 below 2^11 to another one
+        assert np.array_equal(q / 8, x16)
+        want, seen, per_value = gs.function_of(out, q - q.min())
+        table = rs.gelu_table(((seen + q.min()) / 8).astype(np.float32))
         ulp = np.maximum(np.abs(table), 2.0 ** -14) * 2.0 ** -10
         assert (np.abs(per_value - table) <= ulp).all()
     else:
@@ -66,24 +79,36 @@ def _check_exact(M, N, K, epi, seed):
                              f"tiles (m, n) {tiles[:8]}")
 
 
-@pytest.mark.parametrize("epi", [0, 1, 6])
+@pytest.mark.parametrize("epi", [0, 1, 6, 7, 8, 10, 11])
 @pytest.mark.parametrize("K", [64, 192, 768, 1024, 3072])
 def test_gemm_exact_ragged_m(epi, K):
-    """M ends inside a tile's second 64-row half; K = 64 is a partial k-block (zero-filled), 3072 runs the 6-slot ring."""
+    """M ends inside a tile's second 64-row half; K = 64 is a partial k-block (zero-filled), 3072 runs the 6-slot ring.  SwiGLU: F = 192,
+    3 column tiles, the last pair's second tile past N."""
     _check_exact(197 * 7, 384, K, epi, seed=K + epi)
 
 
 @pytest.mark.parametrize("per_cluster,extra", [(3, 0), (3, 1), (4, -1)])
-@pytest.mark.parametrize("K,epi", [(192, 0), (768, 6), (3072, 1)])
+@pytest.mark.parametrize("K,epi", [(192, 0), (768, 6), (3072, 1), (192, 7), (3072, 7), (320, 8), (2048, 8), (192, 10), (3072, 10),
+                                   (192, 11), (3072, 11)])
 def test_gemm_exact_tile_counts_around_the_grid(per_cluster, extra, K, epi):
+    """As in test_gpu_gemm_schedule.py; SwiGLU with F = 128, one pair per row band."""
     pairs = per_cluster * (_sms() // 2) + extra
     _check_exact(pairs * BM, 2 * BN, K, epi, seed=pairs + K)
 
 
-@pytest.mark.parametrize("N,K,epi", [(2304, 768, 6), (3072, 768, 1)])
+@pytest.mark.parametrize("epi", [7, 8, 10, 11])
+def test_gemm_exact_warpgroups_take_different_column_tiles(epi):
+    """As test_gpu_gemm_schedule.py::test_warpgroups_take_different_column_tiles: a pair count coprime to the cluster count, so the two
+    warpgroups of a CTA run different column tiles (and read their own bias and row scales)."""
+    n_pairs = next(n for n in (5, 7, 11, 13) if math.gcd(n, _sms() // 2) == 1)
+    _check_exact(197 * 63, 2 * BN * n_pairs, 3072, epi, seed=n_pairs + epi)
+
+
+@pytest.mark.parametrize("N,K,epi", [(2304, 768, 6), (3072, 768, 1), (3072, 768, 7), (3072, 768, 8), (3072, 768, 10), (2 * 4096, 1536, 11)])
 def test_gemm_exact_vit_b_shapes(N, K, epi):
-    """qkv and fc1 of ViT-B/16 at batch 256."""
-    _check_exact(256 * 197, N, K, epi, seed=N + K)
+    """qkv and fc1 of ViT-B/16 at batch 256 (tanh GELU with the f16 table, erf, QuickGELU, PyTorch's tanh GELU); ViT-g's SwiGLU fc1
+    (F = 4096) at batch 64 with 4 registers (261 tokens)."""
+    _check_exact(64 * 261 if epi == 11 else 256 * 197, N, K, epi, seed=N + K)
 
 
 # ---- GEMM, random operands -----------------------------------------------------------------------------------------------------

@@ -2229,6 +2229,11 @@ static int test_gemm_impl(int device, int M, int N, int K, int epilogue, const u
                           const float *gamma, const float *resid, float *out)
 {
     if (!A || !W || !bias || !out) return fail("null argument");
+    // the patch-embedding epilogue needs the position table and token geometry, which this hook does not take: only these run here
+    if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_RESID_F32 && epilogue != EPI_BIAS_F32 &&
+        epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 && epilogue != EPI_BIAS_QUICK_GELU_F16 &&
+        epilogue != EPI_BIAS_SCALE_RESID_F32 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16 && epilogue != EPI_BIAS_SWIGLU_F16)
+        return fail("GEMM epilogue %d not supported (0, 1, 2, 4, 6, 7, 8, 10, 11; 9 through vitb200_test_gemm_layer_scale)", epilogue);
     if (K % 8 != 0) return fail("K must be a multiple of 8");
     if (gemm_epi_resid(epilogue) && !resid) return fail("resid required");
     if ((epilogue == EPI_BIAS_SCALE_RESID_F32) != (gamma != nullptr))
