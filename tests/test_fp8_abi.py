@@ -50,7 +50,7 @@ def test_null_and_bad_arguments_are_rejected():
     f = np.zeros(64 * 64, np.float32)
     assert L.vitb200_test_gemm_fp8(0, 64, 64, 64, 0, None, f.ctypes.data, a.ctypes.data, 1.0, f.ctypes.data, f.ctypes.data) != 0
     assert L.vitb200_test_gemm_fp8(0, 64, 64, 64, 0, a.ctypes.data, None, a.ctypes.data, 1.0, f.ctypes.data, f.ctypes.data) != 0
-    for epi in (2, 3, 4, 5):  # f32-output epilogues have no e4m3 form
+    for epi in (eng.EPI_BIAS_RESID_F32, eng.EPI_PATCH_F32, eng.EPI_BIAS_F32, 5):  # f32-output epilogues have no e4m3 form; 5 is none
         assert L.vitb200_test_gemm_fp8(0, 64, 64, 64, epi, a.ctypes.data, f.ctypes.data, a.ctypes.data, 1.0, f.ctypes.data,
                                        f.ctypes.data) != 0 and "epilogue" in _last_error()
     assert L.vitb200_test_gemm_fp8(0, 64, 64, 40, 0, a.ctypes.data, f.ctypes.data, a.ctypes.data, 1.0, f.ctypes.data, f.ctypes.data) != 0

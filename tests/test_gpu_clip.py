@@ -17,13 +17,12 @@ from tests.test_gpu_fp8 import E2E_TOL
 eng = pkg.engine
 pytestmark = pytest.mark.gpu
 
-EPI_GELU_ERF, EPI_QUICK_GELU = 7, 8
 CASES = [("micro", "quick_gelu"), ("micro", "gelu_erf"), ("b32", "quick_gelu"), ("l14_336", "quick_gelu")]
 
 
 def _act64(x, epi):
     x = np.asarray(x, np.float64)
-    if epi == EPI_GELU_ERF:
+    if epi == eng.EPI_BIAS_GELU_ERF_F16:
         from scipy.special import ndtr
         return x * ndtr(x)
     with np.errstate(over="ignore"):
@@ -54,7 +53,7 @@ def _check_epilogue(out, x64, acc_scale, epi):
 
 
 @pytest.mark.parametrize("K", [768, 2048])
-@pytest.mark.parametrize("epi", [EPI_GELU_ERF, EPI_QUICK_GELU])
+@pytest.mark.parametrize("epi", [eng.EPI_BIAS_GELU_ERF_F16, eng.EPI_BIAS_QUICK_GELU_F16])
 def test_activation_epilogue_f16(epi, K):
     """K = 768 runs the 5-stage ring, 2048 the 6-stage one (fc1 of D = 2048)."""
     M, N = 300, 512
@@ -69,7 +68,7 @@ def test_activation_epilogue_f16(epi, K):
 
 
 @pytest.mark.parametrize("K", [768, 2048])
-@pytest.mark.parametrize("epi", [EPI_GELU_ERF, EPI_QUICK_GELU])
+@pytest.mark.parametrize("epi", [eng.EPI_BIAS_GELU_ERF_F16, eng.EPI_BIAS_QUICK_GELU_F16])
 def test_activation_epilogue_e4m3(epi, K):
     """x = acc (sa sw) + bias on e4m3 operands.  Hopper's e4m3 MMA adds with fewer than f32's mantissa bits (2^-11 of sum |a w| measured in
     test_gpu_fp8.py), so the noise term is that of the sum of |a w|."""

@@ -43,24 +43,24 @@ def _check_exact(M, N, K, epi, seed):
     sw = np.float32(0.25)
     bias = rng.integers(-8, 9, size=N).astype(np.float32)
     if epi in gs.NEW:
-        bias[:N // 2 if epi == gs.EPI_SWIGLU else N:gs.TAIL_EVERY] = -1e4
+        bias[:N // 2 if epi == eng.EPI_SWIGLU else N:gs.TAIL_EVERY] = -1e4
     out = eng.test_gemm_fp8(M, N, K, epi, fr.e4m3_bits(A), sa, fr.e4m3_bits(W), sw, bias)
     acc = A.astype(np.float64) @ W.astype(np.float64).T  # BLAS in f64 on integers below 2^11: exact
     x = (acc * (sa[:, None].astype(np.float64) * sw) + bias).astype(np.float32)  # exact: at most 11 + 4 significant bits (17 with -1e4)
     if epi in gs.NEW:
         q = (x.astype(np.float64) * 8).astype(np.int64)
         assert np.array_equal(q / 8, x)
-        if epi == gs.EPI_SWIGLU:
+        if epi == eng.EPI_SWIGLU:
             assert out.shape == (M, N // 2)
             want = gs.check_swiglu(out, q[:, :N // 2], q[:, N // 2:], 0.125)
         else:
             want = gs.check_activation(out, q, 0.125, epi)
         return gs.assert_same_bits(out, want)
-    if epi == 6:
+    if epi == eng.EPI_BIAS_F16_HILO:
         want = x  # hi + lo carries 22 bits
-    elif epi == 0:
+    elif epi == eng.EPI_BIAS_F16:
         want = x.astype(np.float16).astype(np.float32)
-    elif epi == 1:
+    elif epi == eng.EPI_BIAS_GELU_F16:
         # as in test_gpu_gemm_schedule.py: each output a function of its f16 pre-activation, within one f16 ulp of the table
         x16 = x.astype(np.float16).astype(np.float32)
         q = (x16 * 8).astype(np.int64)  # f16 rounds a multiple of 1/8 below 2^11 to another one
@@ -79,7 +79,8 @@ def _check_exact(M, N, K, epi, seed):
                              f"tiles (m, n) {tiles[:8]}")
 
 
-@pytest.mark.parametrize("epi", [0, 1, 6, 7, 8, 10, 11])
+@pytest.mark.parametrize("epi", [eng.EPI_BIAS_F16, eng.EPI_BIAS_GELU_F16, eng.EPI_BIAS_F16_HILO, eng.EPI_BIAS_GELU_ERF_F16,
+                                 eng.EPI_BIAS_QUICK_GELU_F16, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16, eng.EPI_SWIGLU])
 @pytest.mark.parametrize("K", [64, 192, 768, 1024, 3072])
 def test_gemm_exact_ragged_m(epi, K):
     """M ends inside a tile's second 64-row half; K = 64 is a partial k-block (zero-filled), 3072 runs the 6-slot ring.  SwiGLU: F = 192,
@@ -88,15 +89,17 @@ def test_gemm_exact_ragged_m(epi, K):
 
 
 @pytest.mark.parametrize("per_cluster,extra", [(3, 0), (3, 1), (4, -1)])
-@pytest.mark.parametrize("K,epi", [(192, 0), (768, 6), (3072, 1), (192, 7), (3072, 7), (320, 8), (2048, 8), (192, 10), (3072, 10),
-                                   (192, 11), (3072, 11)])
+@pytest.mark.parametrize("K,epi", [(192, eng.EPI_BIAS_F16), (768, eng.EPI_BIAS_F16_HILO), (3072, eng.EPI_BIAS_GELU_F16),
+                                   (192, eng.EPI_BIAS_GELU_ERF_F16), (3072, eng.EPI_BIAS_GELU_ERF_F16), (320, eng.EPI_BIAS_QUICK_GELU_F16),
+                                   (2048, eng.EPI_BIAS_QUICK_GELU_F16), (192, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16),
+                                   (3072, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (192, eng.EPI_SWIGLU), (3072, eng.EPI_SWIGLU)])
 def test_gemm_exact_tile_counts_around_the_grid(per_cluster, extra, K, epi):
     """As in test_gpu_gemm_schedule.py; SwiGLU with F = 128, one pair per row band."""
     pairs = per_cluster * (_sms() // 2) + extra
     _check_exact(pairs * BM, 2 * BN, K, epi, seed=pairs + K)
 
 
-@pytest.mark.parametrize("epi", [7, 8, 10, 11])
+@pytest.mark.parametrize("epi", [eng.EPI_BIAS_GELU_ERF_F16, eng.EPI_BIAS_QUICK_GELU_F16, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16, eng.EPI_SWIGLU])
 def test_gemm_exact_warpgroups_take_different_column_tiles(epi):
     """As test_gpu_gemm_schedule.py::test_warpgroups_take_different_column_tiles: a pair count coprime to the cluster count, so the two
     warpgroups of a CTA run different column tiles (and read their own bias and row scales)."""
@@ -104,11 +107,13 @@ def test_gemm_exact_warpgroups_take_different_column_tiles(epi):
     _check_exact(197 * 63, 2 * BN * n_pairs, 3072, epi, seed=n_pairs + epi)
 
 
-@pytest.mark.parametrize("N,K,epi", [(2304, 768, 6), (3072, 768, 1), (3072, 768, 7), (3072, 768, 8), (3072, 768, 10), (2 * 4096, 1536, 11)])
+@pytest.mark.parametrize("N,K,epi", [(2304, 768, eng.EPI_BIAS_F16_HILO), (3072, 768, eng.EPI_BIAS_GELU_F16),
+                                     (3072, 768, eng.EPI_BIAS_GELU_ERF_F16), (3072, 768, eng.EPI_BIAS_QUICK_GELU_F16),
+                                     (3072, 768, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (2 * 4096, 1536, eng.EPI_SWIGLU)])
 def test_gemm_exact_vit_b_shapes(N, K, epi):
     """qkv and fc1 of ViT-B/16 at batch 256 (tanh GELU with the f16 table, erf, QuickGELU, PyTorch's tanh GELU); ViT-g's SwiGLU fc1
     (F = 4096) at batch 64 with 4 registers (261 tokens)."""
-    _check_exact(64 * 261 if epi == 11 else 256 * 197, N, K, epi, seed=N + K)
+    _check_exact(64 * 261 if epi == eng.EPI_SWIGLU else 256 * 197, N, K, epi, seed=N + K)
 
 
 # ---- GEMM, random operands -----------------------------------------------------------------------------------------------------
@@ -125,7 +130,7 @@ def test_gemm_random_against_f64(K):
     sa = rng.uniform(0.01, 0.02, M).astype(np.float32)
     sw = np.float32(0.003)
     bias = np.zeros(N, np.float32)
-    out = eng.test_gemm_fp8(M, N, K, 6, A, sa, W, sw, bias)
+    out = eng.test_gemm_fp8(M, N, K, eng.EPI_BIAS_F16_HILO, A, sa, W, sw, bias)
     a, w = fr.e4m3_value(A).astype(np.float64), fr.e4m3_value(W).astype(np.float64)
     s = (sa.astype(np.float32) * sw).astype(np.float64)[:, None]  # the kernel rounds sa * sw to f32
     ref = (a @ w.T) * s

@@ -24,9 +24,8 @@ eng = pkg.engine
 pytestmark = pytest.mark.gpu
 
 BM = BN = 128  # the GEMM's tile
-EPI_GELU_ERF, EPI_QUICK_GELU, EPI_LAYER_SCALE, EPI_GELU_PYTORCH_TANH, EPI_SWIGLU = 7, 8, 9, 10, 11
-ACTIVATIONS = (EPI_GELU_ERF, EPI_QUICK_GELU, EPI_GELU_PYTORCH_TANH)
-NEW = ACTIVATIONS + (EPI_LAYER_SCALE, EPI_SWIGLU)
+ACTIVATIONS = (eng.EPI_BIAS_GELU_ERF_F16, eng.EPI_BIAS_QUICK_GELU_F16, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16)
+NEW = ACTIVATIONS + (eng.EPI_BIAS_SCALE_RESID_F32, eng.EPI_SWIGLU)
 TAIL_EVERY = 61  # every 61st bias column (of x1 for SwiGLU) is -1e4: the far left tail, in a different place in every tile
 
 
@@ -38,12 +37,12 @@ def _sms():
 def act64(x, epi):
     """The activation of epilogue 7, 8 or 10 in float64."""
     x = np.asarray(x, np.float64)
-    if epi == EPI_GELU_ERF:
+    if epi == eng.EPI_BIAS_GELU_ERF_F16:
         return x * ndtr(x)
-    if epi == EPI_QUICK_GELU:
+    if epi == eng.EPI_BIAS_QUICK_GELU_F16:
         with np.errstate(over="ignore"):
             return x / (1.0 + np.exp(-1.702 * x))
-    if epi == EPI_GELU_PYTORCH_TANH:
+    if epi == eng.EPI_BIAS_GELU_PYTORCH_TANH_F16:
         return gelu_pytorch_tanh(x)
     raise ValueError(epi)
 
@@ -113,13 +112,13 @@ def _check_new(M, N, K, epi, rng):
     HF's order and returns [M][F]."""
     F = N // 2
     A = rng.integers(-2, 3, size=(M, K), dtype=np.int8)
-    if epi == EPI_SWIGLU:
+    if epi == eng.EPI_SWIGLU:
         A *= (rng.random((M, K)) < min(1.0, 64.0 / K)).astype(np.int8)
     W4 = rng.integers(-8, 9, size=(N, K), dtype=np.int8)
     bias = rng.integers(-8, 9, size=N).astype(np.float32)
-    bias[:F if epi == EPI_SWIGLU else N:TAIL_EVERY] = -1e4
+    bias[:F if epi == eng.EPI_SWIGLU else N:TAIL_EVERY] = -1e4
     A16, W16 = A.astype(np.float16), (W4.astype(np.float32) / 4).astype(np.float16)
-    if epi == EPI_LAYER_SCALE:
+    if epi == eng.EPI_BIAS_SCALE_RESID_F32:
         gamma = np.exp(rng.uniform(np.log(1e-6), np.log(10.0), N)).astype(np.float32)
         resid = (rng.standard_normal((M, N)) * 16).astype(np.float32)
         out = eng.test_gemm_layer_scale(M, N, K, A16, W16, bias, gamma, resid)
@@ -130,10 +129,10 @@ def _check_new(M, N, K, epi, rng):
     for r in (0, M // 2, M - 1):
         assert np.array_equal(q[r], A[r].astype(np.int64) @ W4.astype(np.int64).T)
     q += (4 * bias).astype(np.int64)
-    if epi == EPI_LAYER_SCALE:
+    if epi == eng.EPI_BIAS_SCALE_RESID_F32:
         # the kernel rounds x * gamma, then the sum (__fmul_rn, __fadd_rn): numpy's f32 arithmetic is the same two IEEE roundings
         want = (q.astype(np.float32) * np.float32(0.25)) * gamma + resid
-    elif epi == EPI_SWIGLU:
+    elif epi == eng.EPI_SWIGLU:
         assert out.shape == (M, F)
         want = check_swiglu(out, q[:, :F], q[:, F:], 0.25)
     else:
@@ -148,24 +147,24 @@ def _check(M, N, K, epi, seed):
     A = rng.integers(-2, 3, size=(M, K)).astype(np.float16)
     W = rng.integers(-2, 3, size=(N, K)).astype(np.float16)
     bias = rng.integers(-8, 9, size=N).astype(np.float32)
-    resid = rng.integers(-64, 65, size=(M, N)).astype(np.float32) if epi == 2 else None
+    resid = rng.integers(-64, 65, size=(M, N)).astype(np.float32) if epi == eng.EPI_BIAS_RESID_F32 else None
     out = eng.test_gemm(M, N, K, epi, A, W, bias, resid)  # the residual epilogue runs in place: resid aliases out
     # |partial sums| <= 4 K < 2^24: the f32 product is exact integer arithmetic, whatever order the BLAS sums in
     acc = (A.astype(np.float32) @ W.astype(np.float32).T).astype(np.int64)
     for r in (0, M // 2, M - 1):
         assert np.array_equal(acc[r], A[r].astype(np.int64) @ W.astype(np.int64).T)
     x = (acc + bias.astype(np.int64)).astype(np.float32)
-    if epi == 2:
+    if epi == eng.EPI_BIAS_RESID_F32:
         want = x + resid
-    elif epi == 4:
+    elif epi == eng.EPI_BIAS_F32:
         want = x
-    elif epi == 6:
+    elif epi == eng.EPI_BIAS_F16_HILO:
         # |x| < 2048 is exact in f16: hi = x and lo = 0, and test_gemm returns hi + lo
         assert np.abs(x).max() < 2048
         want = x
-    elif epi == 0:
+    elif epi == eng.EPI_BIAS_F16:
         want = x.astype(np.float16).astype(np.float32)
-    elif epi == 1:
+    elif epi == eng.EPI_BIAS_GELU_F16:
         # The kernel evaluates GELU in f32 (gemm_wgmma.cuh) and rounds to f16 one ulp away from the reference table on a few
         # inputs, so each output must be a function of its pre-activation -- the same at every position -- that is the table's
         # value to within one f16 ulp.  A misplaced tile breaks the first condition.
@@ -189,18 +188,19 @@ def _check(M, N, K, epi, seed):
                              f"tiles (m, n) {tiles[:8]}{' ...' if len(tiles) > 8 else ''}")
 
 
-@pytest.mark.parametrize("epi", [4, 0] + list(NEW))
+@pytest.mark.parametrize("epi", [eng.EPI_BIAS_F32, eng.EPI_BIAS_F16] + list(NEW))
 def test_fewer_tiles_than_sms(epi):
     """The head shape: 2 x 8 tiles, each CTA has one tile and its second warpgroup none; the last column tile is partial.  SwiGLU with
     F = 344: 2 x 6 tiles, the last group of 64 hidden units partial."""
-    _check(256, 2 * 344 if epi == EPI_SWIGLU else 1000, 768, epi, seed=1)
+    _check(256, 2 * 344 if epi == eng.EPI_SWIGLU else 1000, 768, epi, seed=1)
 
 
 _GRID_NEW = [(K, e) for e in NEW for K in (192, 320, 2048, 3072)]
 
 
 @pytest.mark.parametrize("per_cluster,extra", [(4, 0), (4, 1), (4, -1), (3, 0), (3, 1)])
-@pytest.mark.parametrize("K,epi", [(192, 0), (64, 2), (320, 6), (2048, 6)] + _GRID_NEW)
+@pytest.mark.parametrize("K,epi", [(192, eng.EPI_BIAS_F16), (64, eng.EPI_BIAS_RESID_F32), (320, eng.EPI_BIAS_F16_HILO),
+                                   (2048, eng.EPI_BIAS_F16_HILO)] + _GRID_NEW)
 def test_tile_counts_around_the_grid(per_cluster, extra, K, epi):
     """per_cluster x SMs / 2 tile pairs (+ extra).  The engine launches as many clusters as fit at once, which is SMs / 2 on an H100
     SXM; where fewer fit, these counts are still uneven shares of the grid, only not the exact boundaries named here.  With SMs / 2
@@ -212,16 +212,22 @@ def test_tile_counts_around_the_grid(per_cluster, extra, K, epi):
     _check(pairs * BM, 2 * BN, K, epi, seed=pairs + K)
 
 
-@pytest.mark.parametrize("N,K,epi", [(128, 448, 0), (128, 448, 2), (384, 448, 6), (384, 448, 4), (384, 448, 1), (384, 2048, 2),
-                                     (384, 448, 7), (384, 2048, 8), (384, 448, 10), (128, 448, 9), (384, 3072, 9), (2 * 2736, 448, 11),
-                                     (2 * 2736, 2048, 11)])
+@pytest.mark.parametrize("N,K,epi", [(128, 448, eng.EPI_BIAS_F16), (128, 448, eng.EPI_BIAS_RESID_F32), (384, 448, eng.EPI_BIAS_F16_HILO),
+                                     (384, 448, eng.EPI_BIAS_F32), (384, 448, eng.EPI_BIAS_GELU_F16), (384, 2048, eng.EPI_BIAS_RESID_F32),
+                                     (384, 448, eng.EPI_BIAS_GELU_ERF_F16), (384, 2048, eng.EPI_BIAS_QUICK_GELU_F16),
+                                     (384, 448, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (128, 448, eng.EPI_BIAS_SCALE_RESID_F32),
+                                     (384, 3072, eng.EPI_BIAS_SCALE_RESID_F32), (2 * 2736, 448, eng.EPI_SWIGLU),
+                                     (2 * 2736, 2048, eng.EPI_SWIGLU)])
 def test_odd_column_tile_count(N, K, epi):
     """An odd number of column tiles: the second CTA of the last pair computes a tile past N, stores nothing, and still releases its
     share of the ring it shares with the first.  SwiGLU with F = 2736: 43 column tiles."""
     _check(197 * 7, N, K, epi, seed=N + K + epi)
 
 
-@pytest.mark.parametrize("N,epi", [(768, 2), (3072, 1), (2304, 6), (3072, 7), (3072, 8), (3072, 10), (768, 9), (2 * 344, 11)])
+@pytest.mark.parametrize("N,epi", [(768, eng.EPI_BIAS_RESID_F32), (3072, eng.EPI_BIAS_GELU_F16), (2304, eng.EPI_BIAS_F16_HILO),
+                                   (3072, eng.EPI_BIAS_GELU_ERF_F16), (3072, eng.EPI_BIAS_QUICK_GELU_F16),
+                                   (3072, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (768, eng.EPI_BIAS_SCALE_RESID_F32),
+                                   (2 * 344, eng.EPI_SWIGLU)])
 def test_m_tail(N, epi):
     """M = 197 x 255 ends inside a tile's second 64-row half: those rows are computed from zero fill and never stored."""
     _check(197 * 255, N, 768, epi, seed=N + epi)
@@ -241,11 +247,14 @@ def test_warpgroups_take_different_column_tiles(epi, K):
     _check(197 * 63, N, K, epi, seed=N + K + epi)
 
 
-@pytest.mark.parametrize("N,K,epi", [(768, 768, 2), (2304, 768, 6), (2304, 768, 0), (3072, 768, 1), (768, 3072, 2), (3072, 768, 7),
-                                     (3072, 768, 8), (3072, 768, 10), (768, 768, 9), (768, 3072, 9), (2 * 4096, 1536, 11)])
+@pytest.mark.parametrize("N,K,epi", [(768, 768, eng.EPI_BIAS_RESID_F32), (2304, 768, eng.EPI_BIAS_F16_HILO), (2304, 768, eng.EPI_BIAS_F16),
+                                     (3072, 768, eng.EPI_BIAS_GELU_F16), (768, 3072, eng.EPI_BIAS_RESID_F32),
+                                     (3072, 768, eng.EPI_BIAS_GELU_ERF_F16), (3072, 768, eng.EPI_BIAS_QUICK_GELU_F16),
+                                     (3072, 768, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (768, 768, eng.EPI_BIAS_SCALE_RESID_F32),
+                                     (768, 3072, eng.EPI_BIAS_SCALE_RESID_F32), (2 * 4096, 1536, eng.EPI_SWIGLU)])
 def test_full_size(N, K, epi):
     """The ViT-B/16 block GEMMs at batch 256 (M = 256 x 197): proj, qkv (split and plain), fc1 (tanh GELU with the f16 table, erf,
     QuickGELU and PyTorch's tanh GELU) and fc2, the residual ones in place; DINOv2 B/14 with 4 registers (261 tokens) at batch 256: the
     LayerScale proj and fc2; ViT-g's SwiGLU fc1 (F = 4096) at batch 64."""
-    M = {EPI_LAYER_SCALE: 256 * 261, EPI_SWIGLU: 64 * 261}.get(epi, 256 * 197)
+    M = {eng.EPI_BIAS_SCALE_RESID_F32: 256 * 261, eng.EPI_SWIGLU: 64 * 261}.get(epi, 256 * 197)
     _check(M, N, K, epi, seed=N * 7 + K + epi)

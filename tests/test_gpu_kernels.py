@@ -11,21 +11,23 @@ pytestmark = pytest.mark.gpu
 
 def _ref(A, W, bias, epi, resid=None):
     ref = A.astype(np.float64) @ W.astype(np.float64).T + bias
-    if epi == 2:
+    if epi == eng.EPI_BIAS_RESID_F32:
         ref = ref + resid
     ref = ref.astype(np.float32)
-    if epi == 0:
+    if epi == eng.EPI_BIAS_F16:
         ref = ref.astype(np.float16).astype(np.float32)
-    if epi == 1:
+    if epi == eng.EPI_BIAS_GELU_F16:
         ref = rs.gelu_table(ref)  # f16(gelu(f32(f16(x)))) -- ggml.c:1434-1441 table semantics
     return ref
 
 
 # shapes: single tile; M/N/K tails (TMA zero fill + predicated stores); ViT-tiny/base layer shapes; head N=1000
 CASES = [
-    (128, 256, 64, 4), (128, 128, 64, 4), (128, 256, 64, 0), (1, 128, 64, 4), (129, 384, 192, 4),
-    (300, 576, 192, 0), (300, 576, 192, 1), (300, 576, 192, 2), (197 * 3, 768, 768, 2), (197 * 3, 3072, 768, 1),
-    (197 * 2, 768, 3072, 2), (197 * 2, 2304, 768, 0), (256, 1000, 768, 4), (7, 1000, 192, 4), (640, 128, 640, 2),
+    (128, 256, 64, eng.EPI_BIAS_F32), (128, 128, 64, eng.EPI_BIAS_F32), (128, 256, 64, eng.EPI_BIAS_F16), (1, 128, 64, eng.EPI_BIAS_F32),
+    (129, 384, 192, eng.EPI_BIAS_F32), (300, 576, 192, eng.EPI_BIAS_F16), (300, 576, 192, eng.EPI_BIAS_GELU_F16),
+    (300, 576, 192, eng.EPI_BIAS_RESID_F32), (197 * 3, 768, 768, eng.EPI_BIAS_RESID_F32), (197 * 3, 3072, 768, eng.EPI_BIAS_GELU_F16),
+    (197 * 2, 768, 3072, eng.EPI_BIAS_RESID_F32), (197 * 2, 2304, 768, eng.EPI_BIAS_F16), (256, 1000, 768, eng.EPI_BIAS_F32),
+    (7, 1000, 192, eng.EPI_BIAS_F32), (640, 128, 640, eng.EPI_BIAS_RESID_F32),
 ]
 
 
@@ -35,16 +37,16 @@ def test_gemm_against_numpy(M, N, K, epi):
     A = rng.standard_normal((M, K)).astype(np.float16)
     W = (rng.standard_normal((N, K)) * 0.05).astype(np.float16)
     bias = rng.standard_normal(N).astype(np.float32)
-    resid = rng.standard_normal((M, N)).astype(np.float32) if epi == 2 else None
+    resid = rng.standard_normal((M, N)).astype(np.float32) if epi == eng.EPI_BIAS_RESID_F32 else None
     out = eng.test_gemm(M, N, K, epi, A, W, bias, resid)
     ref = _ref(A, W, bias, epi, resid)
     pre = (A.astype(np.float64) @ W.astype(np.float64).T + bias).astype(np.float32)
-    if epi in (2, 4):  # f32 outputs: only fp32 accumulation-order noise
+    if epi in (eng.EPI_BIAS_RESID_F32, eng.EPI_BIAS_F32):  # f32 outputs: only fp32 accumulation-order noise
         np.testing.assert_allclose(out, ref, rtol=0, atol=2e-5 * max(1.0, np.abs(ref).max()))
     else:  # f16 outputs: identical except where fp32 noise flips an f16 rounding (<= 1 ulp, rare)
         # bias epilogue: at most one f16 ulp.  GELU: a flipped rounding of the f16 INPUT moves the output by up to
         # |slope| (<= 1.13) input ulps, plus half an output ulp for the final rounding -> 2.5 * 2^-10 * max(|x|, |y|)
-        ulp = np.maximum(np.maximum(np.abs(ref), np.abs(pre) * (2.5 if epi == 1 else 0.0)), 2.0 ** -14) * 2.0 ** -10
+        ulp = np.maximum(np.maximum(np.abs(ref), np.abs(pre) * (2.5 if epi == eng.EPI_BIAS_GELU_F16 else 0.0)), 2.0 ** -14) * 2.0 ** -10
         noise = 2e-5 * max(1.0, np.abs(ref).max())  # fp32 accumulation noise dominates near zero
         assert (np.abs(out - ref) <= ulp * 1.001 + noise).all()
         assert (out != ref).mean() < 0.02
@@ -58,14 +60,14 @@ def test_gemm_split_precision_epilogue(M, N, K):
     A = rng.standard_normal((M, K)).astype(np.float16)
     W = (rng.standard_normal((N, K)) * 0.05).astype(np.float16)
     bias = rng.standard_normal(N).astype(np.float32)
-    out = eng.test_gemm(M, N, K, 6, A, W, bias)
+    out = eng.test_gemm(M, N, K, eng.EPI_BIAS_F16_HILO, A, W, bias)
     ref = (A.astype(np.float64) @ W.astype(np.float64).T + bias).astype(np.float32)
     hi, lo = eng.split_hi_lo(ref)
     want = hi.astype(np.float32) + lo.astype(np.float32)
     assert np.abs(want - ref).max() <= 2.0 ** -21 * np.abs(ref).max()      # the representation itself
     np.testing.assert_allclose(out, ref, rtol=0, atol=2e-5 * max(1.0, np.abs(ref).max()) * 0.1 + 2.0 ** -20 * np.abs(ref).max())
     # and the hi part alone is exactly what the plain f16 epilogue writes
-    plain = eng.test_gemm(M, N, K, 0, A, W, bias)
+    plain = eng.test_gemm(M, N, K, eng.EPI_BIAS_F16, A, W, bias)
     assert (np.abs(out - plain) <= 2.0 ** -11 * np.abs(plain) + 2.0 ** -24).all()
 
 
@@ -78,9 +80,9 @@ def test_gemm_linearity_at_full_size():
     W1 = rng.integers(-3, 4, size=(N, K)).astype(np.float16)
     W2 = rng.integers(-3, 4, size=(N, K)).astype(np.float16)
     z = np.zeros(N, np.float32)
-    o1 = eng.test_gemm(M, N, K, 4, A, W1, z)
-    o2 = eng.test_gemm(M, N, K, 4, A, W2, z)
-    o12 = eng.test_gemm(M, N, K, 4, A, (W1 + W2), z)
+    o1 = eng.test_gemm(M, N, K, eng.EPI_BIAS_F32, A, W1, z)
+    o2 = eng.test_gemm(M, N, K, eng.EPI_BIAS_F32, A, W2, z)
+    o12 = eng.test_gemm(M, N, K, eng.EPI_BIAS_F32, A, (W1 + W2), z)
     assert np.array_equal(o1 + o2, o12)  # all partial sums are small integers: exact in fp32
     # spot-check rows from the first, a middle and the last M tile against int64 arithmetic
     for r in (0, 127, 128, 25000, M - 1):

@@ -15,7 +15,6 @@ from tests.test_gpu_fp8 import E2E_TOL
 eng = pkg.engine
 pytestmark = pytest.mark.gpu
 
-EPI_GELU_TANH_TABLE, EPI_GELU_PYTORCH_TANH = 1, 10
 
 
 def _sparse(rng, rows, K, nnz=16):
@@ -55,10 +54,10 @@ def test_gelu_pytorch_tanh_epilogue_f16(K):
     """Epilogue 10 on f16 operands, K = 768 (the 5-stage ring) and 3072 (the 6-stage one), against float64; activation 0's f16
     pre-rounding gives other results on the same inputs."""
     M, N, A, W, bias = _epilogue_inputs(K, K)
-    out = eng.test_gemm(M, N, K, EPI_GELU_PYTORCH_TANH, A.astype(np.float16), W.astype(np.float16), bias)
+    out = eng.test_gemm(M, N, K, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16, A.astype(np.float16), W.astype(np.float16), bias)
     x32 = (A.astype(np.float64) @ W.astype(np.float64).T).astype(np.float32) + bias
     _check_gelu(out, x32)
-    table = eng.test_gemm(M, N, K, EPI_GELU_TANH_TABLE, A.astype(np.float16), W.astype(np.float16), bias)
+    table = eng.test_gemm(M, N, K, eng.EPI_BIAS_GELU_F16, A.astype(np.float16), W.astype(np.float16), bias)
     differ = int((table != out).sum())
     print(f"K {K}: {differ} of {out.size} outputs differ from activation 0's (f16-rounded x)")
     assert differ > 0
@@ -72,11 +71,11 @@ def test_gelu_pytorch_tanh_epilogue_e4m3(K):
     sw = 0.5
     A8, W8 = fr.e4m3_bits(A), fr.e4m3_bits(W)
     assert np.array_equal(fr.e4m3_value(A8), A) and np.array_equal(fr.e4m3_value(W8), W)
-    out = eng.test_gemm_fp8(M, N, K, EPI_GELU_PYTORCH_TANH, A8, sa, W8, sw, bias)
+    out = eng.test_gemm_fp8(M, N, K, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16, A8, sa, W8, sw, bias)
     acc = A.astype(np.float64) @ W.astype(np.float64).T
     x32 = (acc * (0.25 * sw)).astype(np.float32) + bias
     _check_gelu(out, x32)
-    table = eng.test_gemm_fp8(M, N, K, EPI_GELU_TANH_TABLE, A8, sa, W8, sw, bias)
+    table = eng.test_gemm_fp8(M, N, K, eng.EPI_BIAS_GELU_F16, A8, sa, W8, sw, bias)
     assert int((table != out).sum()) > 0
 
 

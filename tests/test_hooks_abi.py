@@ -1,6 +1,9 @@
 """CPU tests of the kernel test hooks' device check: without a GPU every hook that launches a kernel fails with the engine's
 "no CPU fallback" message instead of running on the host or reporting a raw CUDA error.  And the GEMM hook's epilogue check, which
 comes before the device is touched, so it holds on any machine."""
+import os
+import re
+
 import numpy as np
 import pytest
 
@@ -13,10 +16,10 @@ D, ROWS = 128, 8
 B, NT, H = 1, 16, 1
 
 HOOKS = {
-    "gemm": lambda: eng.test_gemm(M, N, K, 0, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16), np.zeros(N, np.float32)),
+    "gemm": lambda: eng.test_gemm(M, N, K, eng.EPI_BIAS_F16, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16), np.zeros(N, np.float32)),
     "gemm_layer_scale": lambda: eng.test_gemm_layer_scale(M, N, K, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16),
                                                           np.zeros(N, np.float32), np.ones(N, np.float32), np.zeros((M, N), np.float32)),
-    "gemm_fp8": lambda: eng.test_gemm_fp8(M, N, K, 0, np.zeros((M, K), np.uint8), np.ones(M, np.float32), np.zeros((N, K), np.uint8),
+    "gemm_fp8": lambda: eng.test_gemm_fp8(M, N, K, eng.EPI_BIAS_F16, np.zeros((M, K), np.uint8), np.ones(M, np.float32), np.zeros((N, K), np.uint8),
                                           1.0, np.zeros(N, np.float32)),
     "gemm_q8": lambda: eng.test_gemm_q8(np.zeros((M, K), np.float32), np.zeros(N * (K // 32) * 34, np.uint8), np.zeros(N, np.float32)),
     "layernorm": lambda: eng.test_layernorm(np.zeros((ROWS, D), np.float32), np.ones(D, np.float32), np.zeros(D, np.float32)),
@@ -43,7 +46,7 @@ def _gemm(epi):
                          np.zeros((M, N), np.float32))
 
 
-@pytest.mark.parametrize("epi", [3, 5, 12, -1, 1 << 20])
+@pytest.mark.parametrize("epi", [eng.EPI_PATCH_F32, 5, 12, -1, 1 << 20])
 def test_gemm_hook_refuses_unlisted_epilogues(epi):
     """Epilogue 3 (the patch embedding) would read a position table the hook does not take, and the rest are no epilogue at all: all
     refused on the host, before the device check, so the message is the same with and without a GPU."""
@@ -51,6 +54,17 @@ def test_gemm_hook_refuses_unlisted_epilogues(epi):
         _gemm(epi)
 
 
+def test_epilogue_ids_match_the_kernel():
+    """engine.py's EPI_* names and values are those of enum GemmEpilogue in csrc/gemm_wgmma.cuh, parsed as declared_symbols() parses
+    the header."""
+    src = open(os.path.join(os.path.dirname(eng.LIB_PATH), "csrc", "gemm_wgmma.cuh")).read()
+    body = re.search(r"enum GemmEpilogue\s*\{(.*?)\};", src, re.S).group(1)
+    declared = {name: int(value) for name, value in re.findall(r"^\s*(EPI_\w+)\s*=\s*(\d+)\s*,", re.sub(r"//[^\n]*", "", body), re.M)}
+    exported = {name: getattr(eng, name) for name in dir(eng) if name.startswith("EPI_") and name != "EPI_SWIGLU"}
+    assert exported == declared
+    assert eng.EPI_SWIGLU == eng.EPI_BIAS_SWIGLU_F16
+
+
 def test_gemm_hook_sends_layer_scale_to_its_own_hook():
     with pytest.raises(eng.VitB200Error, match="vitb200_test_gemm_layer_scale"):
-        _gemm(9)
+        _gemm(eng.EPI_BIAS_SCALE_RESID_F32)

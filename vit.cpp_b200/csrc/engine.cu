@@ -598,7 +598,7 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
     // the staged epilogues' TMA maps over exactly M rows and N columns of the output (and of the residual), encoded per launch:
     // a captured graph keeps them by value
     CUtensorMap tmO{}, tmX{};
-    if constexpr (gemm_epi_staged(EPI))
+    if constexpr (gemm_epi(EPI).staged)
     {
         using St = GemmStage<EPI, STAGES>;
         // SwiGLU stores F columns of the N / 2 it computes
@@ -614,13 +614,27 @@ int launch_gemm_t(vitb200_engine *e, const CUtensorMap &tmA, const CUtensorMap &
             return make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {N, M}, {2 * ldo}, {64, 64});
         };
         if (out_map(&tmO, p.out)) return 1;
-        if (EPI == EPI_BIAS_F16_HILO && out_map(&tmX, p.out2)) return 1;
-        if (gemm_epi_resid(EPI) && out_map(&tmX, p.resid)) return 1;
+        if (gemm_epi(EPI).hilo && out_map(&tmX, p.out2)) return 1;
+        if (gemm_epi(EPI).resid && out_map(&tmX, p.resid)) return 1;
     }
     // persistent: as many clusters as fit at once, each walking the pairs of column tiles cluster, cluster + clusters, ...
     const int pairs = ((p.M + GEMM_BM - 1) / GEMM_BM) * ((p.N + 2 * GEMM_BN - 1) / (2 * GEMM_BN));
     return launch(e, kern, dim3(2u * (unsigned)std::min(pairs, max_clusters)), dim3((unsigned)Cfg::kThreads), Cfg::SMEM_BYTES, s, attrs, tmA, tmB,
                   tmO, tmX, p);
+}
+
+// The instantiation for epilogue epi, found by walking the ids from EPI at compile time (e4m3: the ones gemm_epi gives an e4m3 form)
+template <int OP, int EPI = 0>
+int launch_gemm_dispatch(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtensorMap &tmB, const GemmParams &p, cudaStream_t s)
+{
+    if constexpr (EPI == GEMM_EPI_END)
+        return fail(OP == GEMM_OP_E4M3 ? "no e4m3 GEMM instantiation for epilogue=%d" : "no GEMM instantiation for epilogue=%d", epi);
+    else
+    {
+        if constexpr (gemm_epi(EPI).valid && (OP == GEMM_OP_F16 || gemm_epi(EPI).e4m3))
+            if (epi == EPI) return p.K >= GEMM_DEEP_K ? launch_gemm_t<EPI, 6, OP>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, OP>(e, tmA, tmB, p, s);
+        return launch_gemm_dispatch<OP, EPI + 1>(e, epi, tmA, tmB, p, s);
+    }
 }
 
 // tmB: the weight map, box = one k-block x GEMM_BN rows.  e4m3: A and W are e4m3 maps, p.a_scale / p.w_scale their
@@ -630,24 +644,8 @@ int launch_gemm(vitb200_engine *e, int epi, const CUtensorMap &tmA, const CUtens
     if (p.N % 4 != 0) return fail("GEMM: N = %d is not a multiple of 4", p.N);
     if (epi == EPI_BIAS_SWIGLU_F16 && (p.F < 1 || p.N != swiglu_rows(p.F)))
         return fail("SwiGLU GEMM: N = %d is not the interleaved width %d of F = %d", p.N, p.F < 1 ? 0 : swiglu_rows(p.F), p.F);
-    const bool deep = p.K >= GEMM_DEEP_K; // ring depth by reduction length (GemmCfg)
-    if (e4m3)
-    {
-        if (!p.a_scale) return fail("e4m3 GEMM: no A scales");
-#define VB_CASE(EPI) \
-    if (epi == EPI) return deep ? launch_gemm_t<EPI, 6, GEMM_OP_E4M3>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5, GEMM_OP_E4M3>(e, tmA, tmB, p, s);
-        VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16)
-        VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16) VB_CASE(EPI_BIAS_SWIGLU_F16)
-#undef VB_CASE
-        return fail("no e4m3 GEMM instantiation for epilogue=%d", epi);
-    }
-#define VB_CASE(EPI) \
-    if (epi == EPI) return deep ? launch_gemm_t<EPI, 6>(e, tmA, tmB, p, s) : launch_gemm_t<EPI, 5>(e, tmA, tmB, p, s);
-    VB_CASE(EPI_BIAS_F16) VB_CASE(EPI_BIAS_F16_HILO) VB_CASE(EPI_BIAS_GELU_F16) VB_CASE(EPI_BIAS_RESID_F32) VB_CASE(EPI_PATCH_F32) VB_CASE(EPI_BIAS_F32)
-    VB_CASE(EPI_BIAS_GELU_ERF_F16) VB_CASE(EPI_BIAS_QUICK_GELU_F16) VB_CASE(EPI_BIAS_SCALE_RESID_F32) VB_CASE(EPI_BIAS_GELU_PYTORCH_TANH_F16)
-    VB_CASE(EPI_BIAS_SWIGLU_F16)
-#undef VB_CASE
-    return fail("no GEMM instantiation for epilogue=%d", epi);
+    if (e4m3 && !p.a_scale) return fail("e4m3 GEMM: no A scales");
+    return e4m3 ? launch_gemm_dispatch<GEMM_OP_E4M3>(e, epi, tmA, tmB, p, s) : launch_gemm_dispatch<GEMM_OP_F16>(e, epi, tmA, tmB, p, s);
 }
 
 // The patchify kernel for patch size P and C input channels, NULL for a size it has none for (vitb200_create rejects those)
@@ -1584,6 +1582,54 @@ int test_layernorm_impl(int device, int rows, int D, const float *x, const float
                        [&] { return launch_layernorm(e, dx, (size_t)D, dw, db, *y, rows, e->stream, 0, 0, y_scale ? *y_scale : nullptr); });
 }
 
+// The GEMM test hooks' one body: the GEMM alone on a scratch engine, as the engine launches it, with A [M][K] and W [N][K] f16 bits or
+// (GEMM_OP_E4M3) e4m3 bytes.  SwiGLU takes W and bias in HF's order, interleaves them as the engine uploads them and stores [M][N / 2].
+template <int OP, typename T>
+int test_gemm_run(int device, int M, int N, int K, int epilogue, const T *A, const T *W, const float *bias, const float *a_scale,
+                  float w_scale, const float *gamma, const float *resid, float *out)
+{
+    const GemmEpiDesc d = gemm_epi(epilogue);
+    if (d.swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
+    EnginePtr owner;
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
+    const int F = N / 2, Nw = d.swiglu ? swiglu_rows(F) : N, No = d.swiglu ? F : N; // SwiGLU: Nw rows computed, No stored
+    std::vector<T> wi;
+    std::vector<float> bi;
+    if (d.swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
+    const size_t MN = (size_t)M * No;
+    T *dA = nullptr, *dW = nullptr;
+    __half *hi = nullptr, *lo = nullptr;
+    float *dB = nullptr, *dS = nullptr, *dG = nullptr, *o32 = nullptr;
+    if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dB, bias, Nw)) return 1;
+    if ((a_scale && upload(e, &dS, a_scale, M)) || (gamma && upload(e, &dG, gamma, N))) return 1;
+    if (d.f16 && (dev_alloc(e, &hi, MN) || (d.hilo && dev_alloc(e, &lo, MN)))) return 1;
+    // the residual epilogues work in place on the f32 stream, like the engine uses them (X += ...)
+    if (!d.f16 && (d.resid ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
+    constexpr bool e4m3 = OP == GEMM_OP_E4M3;
+    constexpr CUtensorMapDataType type = e4m3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+    constexpr cuuint32_t kb = e4m3 ? 2 * GEMM_BK : GEMM_BK; // one k-block of 128 B
+    const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)Nw, Ku = (cuuint64_t)K;
+    CUtensorMap tA, tB;
+    if (make_tmap(&tA, type, dA, {Ku, Mu}, {sizeof(T) * Ku}, {kb, GEMM_A_BOX_ROWS}) || make_tmap(&tB, type, dW, {Ku, Nu}, {sizeof(T) * Ku}, {kb, GEMM_BN}))
+        return 1;
+    GemmParams p{};
+    p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = d.f16 ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = No; p.resid = o32; p.gamma = dG;
+    p.a_scale = dS; p.w_scale = w_scale; p.F = F;
+    if (run_scratch(e, e4m3 ? "e4m3 GEMM kernel" : "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, e4m3); })) return 1;
+    // split-precision result: hi + lo (exact in f32: the two parts do not overlap); the other f16 epilogues' hi alone, so that a -0 stays -0
+    return d.f16 ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
+}
+
+// "0, 1, ...": the epilogue ids that `accepts`, for a hook's refusal
+std::string gemm_epi_list(bool (*accepts)(int))
+{
+    std::string s;
+    for (int epi = 0; epi < GEMM_EPI_END; ++epi)
+        if (gemm_epi(epi).valid && accepts(epi)) s += (s.empty() ? "" : ", ") + std::to_string(epi);
+    return s;
+}
+
 // One call of the host pipeline, once its arguments are checked: begin_submit picks its slot and starts the call's launch count; end_submit
 // marks the slot's last use (everything enqueued on the compute stream so far) and counts the call
 Slot &begin_submit(vitb200_engine *e)
@@ -2225,57 +2271,25 @@ int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const 
 }
 
 // vitb200_test_gemm and vitb200_test_gemm_layer_scale: gamma is the LayerScale epilogue's [N] (NULL for every other epilogue)
-static int test_gemm_impl(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
-                          const float *gamma, const float *resid, float *out)
+static int test_gemm_f16(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
+                         const float *gamma, const float *resid, float *out)
 {
     if (!A || !W || !bias || !out) return fail("null argument");
-    // the patch-embedding epilogue needs the position table and token geometry, which this hook does not take: only these run here
-    if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_RESID_F32 && epilogue != EPI_BIAS_F32 &&
-        epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 && epilogue != EPI_BIAS_QUICK_GELU_F16 &&
-        epilogue != EPI_BIAS_SCALE_RESID_F32 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16 && epilogue != EPI_BIAS_SWIGLU_F16)
-        return fail("GEMM epilogue %d not supported (0, 1, 2, 4, 6, 7, 8, 10, 11; 9 through vitb200_test_gemm_layer_scale)", epilogue);
+    // the patch-embedding epilogue needs the position table and token geometry, which this hook does not take: every other runs here
+    if (!gemm_epi(epilogue).valid || epilogue == EPI_PATCH_F32)
+        return fail("GEMM epilogue %d not supported (%s; %d through vitb200_test_gemm_layer_scale)", epilogue,
+                    gemm_epi_list([](int epi) { return epi != EPI_PATCH_F32 && epi != EPI_BIAS_SCALE_RESID_F32; }).c_str(), EPI_BIAS_SCALE_RESID_F32);
     if (K % 8 != 0) return fail("K must be a multiple of 8");
-    if (gemm_epi_resid(epilogue) && !resid) return fail("resid required");
+    if (gemm_epi(epilogue).resid && !resid) return fail("resid required");
     if ((epilogue == EPI_BIAS_SCALE_RESID_F32) != (gamma != nullptr))
         return fail("gamma goes with the LayerScale epilogue %d only (vitb200_test_gemm_layer_scale)", EPI_BIAS_SCALE_RESID_F32);
-    const bool swiglu = epilogue == EPI_BIAS_SWIGLU_F16;
-    if (swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
-    EnginePtr owner;
-    if (scratch_engine(device, owner)) return 1;
-    vitb200_engine *e = owner.get();
-    const bool f16out = epilogue == EPI_BIAS_F16 || epilogue == EPI_BIAS_GELU_F16 || epilogue == EPI_BIAS_F16_HILO ||
-                        epilogue == EPI_BIAS_GELU_ERF_F16 || epilogue == EPI_BIAS_QUICK_GELU_F16 || epilogue == EPI_BIAS_GELU_PYTORCH_TANH_F16 || swiglu;
-    // SwiGLU: W and bias interleaved as the engine uploads them, Nw rows computed, out [M][N / 2]
-    const int F = N / 2, Nw = swiglu ? swiglu_rows(F) : N, No = swiglu ? F : N;
-    std::vector<uint16_t> wi;
-    std::vector<float> bi;
-    if (swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
-    const size_t MN = (size_t)M * No;
-    __half *dA = nullptr, *dW = nullptr, *hi = nullptr, *lo = nullptr;
-    float *dB = nullptr, *o32 = nullptr;
-    if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dB, bias, Nw)) return 1;
-    if (f16out && (dev_alloc(e, &hi, MN) || (epilogue == EPI_BIAS_F16_HILO && dev_alloc(e, &lo, MN)))) return 1;
-    // the residual epilogue works in place on the f32 stream, like the engine uses it (X += ...)
-    if (!f16out && (gemm_epi_resid(epilogue) ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
-    float *dG = nullptr;
-    if (gamma && upload(e, &dG, gamma, N)) return 1;
-    CUtensorMap tA, tB;
-    const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)Nw, Ku = (cuuint64_t)K;
-    if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dA, {Ku, Mu}, {2 * Ku}, {GEMM_BK, GEMM_A_BOX_ROWS}) ||
-        make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, dW, {Ku, Nu}, {2 * Ku}, {GEMM_BK, GEMM_BN}))
-        return 1;
-    GemmParams p{};
-    p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = f16out ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = No; p.resid = o32; p.gamma = dG;
-    p.F = F;
-    if (run_scratch(e, "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream); })) return 1;
-    // split-precision result: hi + lo (exact in f32: the two parts do not overlap)
-    return f16out ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
+    return test_gemm_run<GEMM_OP_F16>(device, M, N, K, epilogue, A, W, bias, nullptr, 0.f, gamma, resid, out);
 }
 
 int vitb200_test_gemm(int device, int M, int N, int K, int epilogue, const uint16_t *A, const uint16_t *W, const float *bias,
                       const float *resid, float *out)
 {
-    return guarded(__func__, [&] { return test_gemm_impl(device, M, N, K, epilogue, A, W, bias, nullptr, resid, out); });
+    return guarded(__func__, [&] { return test_gemm_f16(device, M, N, K, epilogue, A, W, bias, nullptr, resid, out); });
 }
 
 int vitb200_test_gemm_layer_scale(int device, int M, int N, int K, const uint16_t *A, const uint16_t *W, const float *bias,
@@ -2283,7 +2297,7 @@ int vitb200_test_gemm_layer_scale(int device, int M, int N, int K, const uint16_
 {
     return guarded(__func__, [&]() -> int {
         if (!gamma || !resid) return fail("null argument");
-        return test_gemm_impl(device, M, N, K, EPI_BIAS_SCALE_RESID_F32, A, W, bias, gamma, resid, out);
+        return test_gemm_f16(device, M, N, K, EPI_BIAS_SCALE_RESID_F32, A, W, bias, gamma, resid, out);
     });
 }
 
@@ -2314,36 +2328,9 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
     return guarded(__func__, [&]() -> int {
         if (!A || !a_scale || !W || !bias || !out) return fail("null argument");
         if (M < 1 || N < 4 || K < 16 || K % 16 != 0) return fail("bad shape (M >= 1, N >= 4, K >= 16 and K %% 16 == 0)");
-        const bool swiglu = epilogue == EPI_BIAS_SWIGLU_F16;
-        if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_GELU_F16 && epilogue != EPI_BIAS_F16_HILO && epilogue != EPI_BIAS_GELU_ERF_F16 &&
-            epilogue != EPI_BIAS_QUICK_GELU_F16 && epilogue != EPI_BIAS_GELU_PYTORCH_TANH_F16 && !swiglu)
-            return fail("e4m3 GEMM epilogue %d not supported (0, 1, 6, 7, 8, 10, 11)", epilogue);
-        if (swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
-        EnginePtr owner;
-        if (scratch_engine(device, owner)) return 1;
-        vitb200_engine *e = owner.get();
-        // SwiGLU: W and bias interleaved as the engine uploads them, Nw rows computed, out [M][N / 2]
-        const int F = N / 2, Nw = swiglu ? swiglu_rows(F) : N, No = swiglu ? F : N;
-        std::vector<uint8_t> wi;
-        std::vector<float> bi;
-        if (swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
-        const size_t MN = (size_t)M * No;
-        uint8_t *dA = nullptr, *dW = nullptr;
-        float *dS = nullptr, *dB = nullptr;
-        __half *hi = nullptr, *lo = nullptr;
-        if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dS, a_scale, M) || upload(e, &dB, bias, Nw) ||
-            dev_alloc(e, &hi, MN) || dev_alloc(e, &lo, MN))
-            return 1;
-        CUtensorMap tA, tB;
-        const cuuint64_t Mu = (cuuint64_t)M, Nu = (cuuint64_t)Nw, Ku = (cuuint64_t)K;
-        if (make_tmap(&tA, CU_TENSOR_MAP_DATA_TYPE_UINT8, dA, {Ku, Mu}, {Ku}, {2 * GEMM_BK, GEMM_A_BOX_ROWS}) ||
-            make_tmap(&tB, CU_TENSOR_MAP_DATA_TYPE_UINT8, dW, {Ku, Nu}, {Ku}, {2 * GEMM_BK, GEMM_BN}))
-            return 1;
-        GemmParams p{};
-        p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = hi; p.out2 = lo; p.ldo = No; p.a_scale = dS; p.w_scale = w_scale; p.F = F;
-        if (run_scratch(e, "e4m3 GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, true); })) return 1;
-        // split-precision result: hi + lo (exact in f32); the other epilogues' hi alone, so that a -0 stays -0
-        return tap_f16(out, hi, MN, e->stream, epilogue == EPI_BIAS_F16_HILO ? lo : nullptr);
+        if (!gemm_epi(epilogue).e4m3)
+            return fail("e4m3 GEMM epilogue %d not supported (%s)", epilogue, gemm_epi_list([](int epi) { return gemm_epi(epi).e4m3; }).c_str());
+        return test_gemm_run<GEMM_OP_E4M3>(device, M, N, K, epilogue, A, W, bias, a_scale, w_scale, nullptr, nullptr, out);
     });
 }
 

@@ -66,6 +66,30 @@ enum GemmEpilogue
     EPI_BIAS_GELU_PYTORCH_TANH_F16 = 10, // out f16 = f16(gelu_tanh(acc + bias)), x in f32 without rounding to f16 first (fc1 of SigLIP)
     EPI_BIAS_SWIGLU_F16 = 11, // out f16 [M][F] = f16(silu(x1) * x2), x = acc + bias in f32, W interleaved by 64 (fc1 of DINOv2 ViT-g; below)
 };
+constexpr int GEMM_EPI_END = EPI_BIAS_SWIGLU_F16 + 1; // one past the largest id: a new epilogue takes this id and moves it on
+
+// What each epilogue is: the kernel, its launch and dispatch and the test hooks derive every per-epilogue choice from this.  staged:
+// stored through shared memory with TMA (else from registers); f16 output (else f32); resid: adds the TMA-loaded residual stream; hilo:
+// outputs hi and lo; swiglu: W interleaved by SWIGLU_GROUP, F of the N columns stored; e4m3: has an e4m3-operand form.  5: valid = false.
+struct GemmEpiDesc { bool valid, staged, f16, resid, hilo, swiglu, e4m3; };
+__host__ __device__ constexpr GemmEpiDesc gemm_epi(int epi)
+{
+    switch (epi) //                                valid  staged f16    resid  hilo   swiglu e4m3
+    {
+    case EPI_BIAS_F16:                   return {true, true,  true,  false, false, false, true};
+    case EPI_BIAS_GELU_F16:              return {true, true,  true,  false, false, false, true};
+    case EPI_BIAS_RESID_F32:             return {true, true,  false, true,  false, false, false};
+    case EPI_PATCH_F32:                  return {true, false, false, false, false, false, false};
+    case EPI_BIAS_F32:                   return {true, false, false, false, false, false, false};
+    case EPI_BIAS_F16_HILO:              return {true, true,  true,  false, true,  false, true};
+    case EPI_BIAS_GELU_ERF_F16:          return {true, true,  true,  false, false, false, true};
+    case EPI_BIAS_QUICK_GELU_F16:        return {true, true,  true,  false, false, false, true};
+    case EPI_BIAS_SCALE_RESID_F32:       return {true, true,  false, true,  false, false, false};
+    case EPI_BIAS_GELU_PYTORCH_TANH_F16: return {true, true,  true,  false, false, false, true};
+    case EPI_BIAS_SWIGLU_F16:            return {true, true,  true,  false, false, true,  true};
+    default:                             return {};
+    }
+}
 
 struct GemmParams
 {
@@ -150,17 +174,6 @@ __device__ __forceinline__ float silu_f32(float x)
 // 64-row half) stores one 64-column f16 box at column n0 / 2 of out [M][F], and the store map covers F columns, so padding is never stored.
 constexpr int SWIGLU_GROUP = 64;
 
-// Epilogues whose result goes out through shared memory and TMA stores (the rest store from registers)
-__host__ __device__ constexpr bool gemm_epi_staged(int epi)
-{
-    return epi == EPI_BIAS_F16 || epi == EPI_BIAS_GELU_F16 || epi == EPI_BIAS_F16_HILO || epi == EPI_BIAS_RESID_F32 ||
-           epi == EPI_BIAS_GELU_ERF_F16 || epi == EPI_BIAS_QUICK_GELU_F16 || epi == EPI_BIAS_SCALE_RESID_F32 || epi == EPI_BIAS_GELU_PYTORCH_TANH_F16 ||
-           epi == EPI_BIAS_SWIGLU_F16;
-}
-
-// Epilogues that add the residual stream (loaded into the staging buffer with TMA)
-__host__ __device__ constexpr bool gemm_epi_resid(int epi) { return epi == EPI_BIAS_RESID_F32 || epi == EPI_BIAS_SCALE_RESID_F32; }
-
 // Staged-epilogue geometry: a warpgroup's 128 x 128 result leaves in passes of one 64-row half x kPassCols columns; a pass is
 // kColBoxes boxes of 64 rows x 128 B (64 f16 or 32 f32 columns) per output tensor (hi and lo for EPI_BIAS_F16_HILO) and fills the
 // staging buffer
@@ -168,10 +181,9 @@ template <int EPI, int STAGES>
 struct GemmStage
 {
     using Cfg = GemmCfg<STAGES>;
-    static constexpr bool kF16 = (EPI == EPI_BIAS_F16 || EPI == EPI_BIAS_GELU_F16 || EPI == EPI_BIAS_F16_HILO || EPI == EPI_BIAS_GELU_ERF_F16 ||
-                                  EPI == EPI_BIAS_QUICK_GELU_F16 || EPI == EPI_BIAS_GELU_PYTORCH_TANH_F16 || EPI == EPI_BIAS_SWIGLU_F16);
-    static constexpr bool kSwiglu = EPI == EPI_BIAS_SWIGLU_F16;
-    static constexpr int kOuts = EPI == EPI_BIAS_F16_HILO ? 2 : 1;
+    static constexpr bool kF16 = gemm_epi(EPI).f16;
+    static constexpr bool kSwiglu = gemm_epi(EPI).swiglu;
+    static constexpr int kOuts = gemm_epi(EPI).hilo ? 2 : 1;
     static constexpr int kBoxCols = kF16 ? 64 : 32;
     static constexpr int kBoxBytes = 64 * 128;
     static constexpr int kFitCols = Cfg::kStageBytes / (64 * kOuts * (kF16 ? 2 : 4));
@@ -198,9 +210,9 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 {
     using Cfg = GemmCfg<STAGES>;
     constexpr int kStages = Cfg::kStages;
-    constexpr bool kStaged = gemm_epi_staged(EPI);
+    constexpr bool kStaged = gemm_epi(EPI).staged;
     constexpr bool kE4M3 = OP == GEMM_OP_E4M3;
-    static_assert(!kE4M3 || kStaged, "e4m3 operands: staged epilogues only");
+    static_assert(gemm_epi(EPI).valid && (!kE4M3 || (kStaged && gemm_epi(EPI).e4m3)), "an epilogue; e4m3: a staged one with an e4m3 form");
     constexpr int kKb = kE4M3 ? 2 * GEMM_BK : GEMM_BK; // K elements per k-block
     constexpr int kBarTurn = 1; // + warpgroup: named barrier "this warpgroup may start its next k-loop"
     constexpr int kBarWg = 3;   // + warpgroup: the warpgroup's own epilogue barrier
@@ -240,7 +252,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if constexpr (kStaged)
         {
             ptx::prefetch_tensormap(&tmOut);
-            if constexpr (EPI == EPI_BIAS_F16_HILO || gemm_epi_resid(EPI)) ptx::prefetch_tensormap(&tmAux);
+            if constexpr (gemm_epi(EPI).hilo || gemm_epi(EPI).resid) ptx::prefetch_tensormap(&tmAux);
         }
         for (int s = 0; s < kStages; ++s)
         {
@@ -268,7 +280,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             {
                 const unsigned m_blk = u / n_pairs;
                 const int m0 = (int)m_blk * GEMM_BM, n0 = (int)(2 * (u - m_blk * n_pairs) + rank) * GEMM_BN;
-                if constexpr (gemm_epi_resid(EPI))
+                if constexpr (gemm_epi(EPI).resid)
                 {
                     // the residual rows are read once, by the epilogue: start pulling them into L2 while the tile's main loop runs
                     for (int h = 0; h < 2; ++h)
@@ -317,7 +329,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if (tid == 0)
             {
                 ptx::tma_store_wait_read<0>();
-                if constexpr (gemm_epi_resid(EPI))
+                if constexpr (gemm_epi(EPI).resid)
                     if (n0 < p.N) resid_load(sStage + cw * Cfg::kStageBytes, n0, m0, cw);
             }
         }
@@ -403,10 +415,10 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                 if (ps > 0 && tid == 0)
                 {
                     if (ps >= St::kSlots) ptx::tma_store_wait_read<St::kSlots - 1>(); // the stores of the pass that used buf have read it
-                    if constexpr (gemm_epi_resid(EPI)) resid_load(buf, c0, m0 + 64 * hm, cw);
+                    if constexpr (gemm_epi(EPI).resid) resid_load(buf, c0, m0 + 64 * hm, cw);
                 }
                 ptx::named_bar_sync(kBarWg + cw, 128); // pass 0: s_bias[cw] is written
-                if constexpr (gemm_epi_resid(EPI))
+                if constexpr (gemm_epi(EPI).resid)
                 {
                     ptx::mbar_wait(resid_bar(cw), resid_ph);
                     resid_ph ^= 1;

@@ -488,8 +488,19 @@ def test_dequant(ggml_type: int, blocks: np.ndarray) -> np.ndarray:
     return out.view(np.float16)
 
 
-# the SwiGLU epilogue of vitb200_test_gemm / vitb200_test_gemm_fp8: W [N][K] in HF's order (N = 2 F), out [M][N / 2]
-EPI_SWIGLU = 11
+# The GEMM epilogue ids of vitb200_test_gemm / vitb200_test_gemm_fp8, named as in enum GemmEpilogue (csrc/gemm_wgmma.cuh)
+EPI_BIAS_F16 = 0
+EPI_BIAS_GELU_F16 = 1
+EPI_BIAS_RESID_F32 = 2
+EPI_PATCH_F32 = 3
+EPI_BIAS_F32 = 4
+EPI_BIAS_F16_HILO = 6
+EPI_BIAS_GELU_ERF_F16 = 7
+EPI_BIAS_QUICK_GELU_F16 = 8
+EPI_BIAS_SCALE_RESID_F32 = 9
+EPI_BIAS_GELU_PYTORCH_TANH_F16 = 10
+EPI_BIAS_SWIGLU_F16 = 11  # W [N][K] in HF's order (N = 2 F), out [M][N / 2]
+EPI_SWIGLU = EPI_BIAS_SWIGLU_F16
 
 
 def test_gemm(M: int, N: int, K: int, epilogue: int, A16: np.ndarray, W16: np.ndarray, bias: np.ndarray,
