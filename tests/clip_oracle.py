@@ -9,7 +9,7 @@ import os
 
 import numpy as np
 
-from tests.util import pkg
+from tests.hf_oracle import init_model
 
 # name: (hidden, heads, layers, patch, image, projection dim)
 GEOMETRIES = {
@@ -22,33 +22,12 @@ HF_ACT = {"quick_gelu": "quick_gelu", "gelu_erf": "gelu"}
 
 def build_hf(geometry: str, activation: str = "quick_gelu", seed: int = 0):
     """The float32 HF model (matrix weights f16-valued) for a geometry of GEOMETRIES; activation 'quick_gelu' or 'gelu_erf'."""
-    import torch
     from transformers import CLIPVisionConfig, CLIPVisionModelWithProjection
     D, H, L, P, S, proj = GEOMETRIES[geometry]
     cfg = CLIPVisionConfig(hidden_size=D, intermediate_size=4 * D, num_attention_heads=H, num_hidden_layers=L, patch_size=P, image_size=S,
                            projection_dim=proj, hidden_act=HF_ACT[activation], layer_norm_eps=1e-5)
-    torch.manual_seed(seed)
-    m = CLIPVisionModelWithProjection(cfg).float().eval()
-    with torch.no_grad():
-        for name, p in m.named_parameters():
-            if "layer_norm" in name or "layrnorm" in name:
-                p.copy_((1.0 if name.endswith("weight") else 0.0) + 0.2 * torch.randn_like(p))
-            elif name.endswith("bias"):
-                p.copy_(0.05 * torch.randn_like(p))
-            elif p.ndim >= 2 and "position_embedding" not in name:
-                fan_in = p[0].numel()
-                p.copy_((torch.randn_like(p) / fan_in ** 0.5).half().float())   # f16-valued, as the engine stores them
-            else:
-                p.copy_(0.5 * torch.randn_like(p))                               # class and position embeddings (f32 in the engine)
-    return m
-
-
-def save_and_convert(model, directory: str) -> str:
-    """save_pretrained + convert.py (the CLI's code path) -> the GGUF path."""
-    model.save_pretrained(directory)
-    out = os.path.join(directory, "clip.gguf")
-    pkg.convert.main([os.path.join(directory, "model.safetensors"), out, "--hf-config", os.path.join(directory, "config.json")])
-    return out
+    # post_layernorm matches neither norm name: its weight and bias keep the 0.5 and 0.05 randn draws the bounds were measured with
+    return init_model(CLIPVisionModelWithProjection, cfg, seed, norms=("layer_norm", "layrnorm"), f32=("position_embedding",))
 
 
 def hf_outputs(model, imgs) -> dict:

@@ -5,11 +5,9 @@ SiglipVisionModel and SiglipForImageClassification are built from a config under
 the attention-pooling head's in_proj / out_proj, patch kernel, classifier) are rounded to f16, as the engine stores them; LayerNorms are
 kept away from the identity.  The model is saved as model.safetensors + config.json and converted with vit.cpp_b200/convert.py; the
 oracle runs the same weights in float64."""
-import os
-
 import numpy as np
 
-from tests.util import pkg
+from tests.hf_oracle import init_model
 
 # name: (hidden, heads, layers, patch, image size)
 GEOMETRIES = {
@@ -30,7 +28,6 @@ def vision_config(geometry: str):
 
 def build_hf(geometry: str, classifier: bool = False, seed: int = 0):
     """The float32 HF model (matrix weights f16-valued): SiglipForImageClassification or SiglipVisionModel."""
-    import torch
     import transformers as tr
     vc = vision_config(geometry)
     if classifier:
@@ -40,32 +37,11 @@ def build_hf(geometry: str, classifier: bool = False, seed: int = 0):
         cls = tr.SiglipForImageClassification
     else:
         cfg, cls = vc, tr.SiglipVisionModel
-    torch.manual_seed(seed)
-    m = cls(cfg).float().eval()
-    with torch.no_grad():
-        for name, p in m.named_parameters():
-            if "norm" in name:
-                p.copy_((1.0 if name.endswith("weight") else 0.0) + 0.2 * torch.randn_like(p))
-            elif name.endswith("bias"):
-                p.copy_(0.05 * torch.randn_like(p))
-            elif p.ndim >= 2 and "position_embedding" not in name and "probe" not in name:
-                fan_in = p[0].numel()
-                p.copy_((torch.randn_like(p) / fan_in ** 0.5).half().float())   # f16-valued, as the engine stores them
-            else:
-                p.copy_(0.5 * torch.randn_like(p))                               # positions, the probe (f32)
-    return m
+    return init_model(cls, cfg, seed, norms=("norm",), f32=("position_embedding", "probe"))
 
 
 def image_size(geometry: str) -> int:
     return GEOMETRIES[geometry][4]
-
-
-def save_and_convert(model, directory: str) -> str:
-    """save_pretrained + convert.py (the CLI's code path) -> the GGUF path."""
-    model.save_pretrained(directory)
-    out = os.path.join(directory, "siglip.gguf")
-    pkg.convert.main([os.path.join(directory, "model.safetensors"), out, "--hf-config", os.path.join(directory, "config.json")])
-    return out
 
 
 def hf_outputs(model, imgs) -> dict:

@@ -1,4 +1,4 @@
-"""CLIP image towers on the CPU: the Hugging Face converter, the GGUF architecture keys, the extended emulation against an independent
+"""CLIP image towers on the CPU: the Hugging Face converter, the GGUF architecture keys, the emulation against an independent
 float64 oracle (transformers' CLIPVisionModelWithProjection), and the refusals that need no GPU."""
 import copy
 import os
@@ -11,7 +11,8 @@ import pytest
 from tests.util import pkg, gf, model_path
 from tests import clip_oracle as co
 from tests import fp8_reference as fr
-from tests.clip_emulation import ArchEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 
 eng = pkg.engine
 cv = pkg.convert
@@ -27,13 +28,13 @@ EMU_BOUND = 1e-3
 def clip(request, tmp_path_factory):
     d = str(tmp_path_factory.mktemp(f"clip_{request.param}"))
     m = co.build_hf("micro", request.param)
-    path = co.save_and_convert(m, d)
+    path = save_and_convert(m, d, "clip")
     imgs = gf.synthetic_images(3, 64, seed=3)
     return request.param, m, d, path, gf.read_gguf(path), imgs, co.hf_outputs(m, imgs)
 
 
 def _distances(vf, imgs, o):
-    emu = ArchEmulation(vf, acc=np.float64, fp8=False)
+    emu = Emulation(vf, acc=np.float64, fp8=False)
     L = vf.num_hidden_layers
     x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
     d = {"image_embeds": fr.rel_dist(emu.forward(imgs), o["image_embeds"]).max(),
@@ -71,7 +72,7 @@ def test_a_broken_mapping_fails_the_oracle_check(clip):
     image embeddings against <= 3.4e-4 for the right mapping.  The two activations differ by a few hundredths at most, so that bug shows
     by one order of magnitude rather than three."""
     act, _, _, _, vf, imgs, o = clip
-    good = fr.rel_dist(ArchEmulation(vf, acc=np.float64, fp8=False).forward(imgs), o["image_embeds"]).max()
+    good = fr.rel_dist(Emulation(vf, acc=np.float64, fp8=False).forward(imgs), o["image_embeds"]).max()
     D = vf.hidden_size
     qk = copy.deepcopy(vf)
     for i in range(vf.num_hidden_layers):
@@ -83,7 +84,7 @@ def test_a_broken_mapping_fails_the_oracle_check(clip):
     no_pre.pre_norm = 0
     other = copy.deepcopy(vf)
     other.activation = "gelu_erf" if act == "quick_gelu" else "quick_gelu"
-    bad = {n: fr.rel_dist(ArchEmulation(b, acc=np.float64, fp8=False).forward(imgs), o["image_embeds"]).max()
+    bad = {n: fr.rel_dist(Emulation(b, acc=np.float64, fp8=False).forward(imgs), o["image_embeds"]).max()
            for n, b in (("qk", qk), ("no_pre", no_pre), ("activation", other))}
     print(act, f"right {good:.2e}", {k: f"{v:.2e}" for k, v in bad.items()})
     assert bad["qk"] > 300 * EMU_BOUND and bad["no_pre"] > 300 * EMU_BOUND
@@ -212,11 +213,3 @@ def test_gguf_parser_fuzzed_with_the_architecture_keys(clip, tmp_path):
     r = subprocess.run([exe, path, model_path("micro", "f16")], capture_output=True, text=True, timeout=300)
     assert r.returncode == 0, (r.stdout[-500:], r.stderr[-3000:])
     assert r.stdout.count("rejected") == 2   # both parsers ran
-
-
-def test_extended_emulation_is_the_fp8_emulation_on_the_reference_architecture():
-    """On a reference-architecture file the extension runs Fp8Emulation's schedule unchanged, in both forms, bit for bit."""
-    vf = gf.read(model_path("micro", "f16"))
-    imgs = gf.synthetic_images(2, vf.img_size, seed=5)
-    for fp8 in (False, True):
-        assert np.array_equal(ArchEmulation(vf, fp8=fp8).forward(imgs), fr.Fp8Emulation(vf, fp8=fp8).forward(imgs)), fp8

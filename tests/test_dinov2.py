@@ -1,5 +1,5 @@
 """DINOv2 on the CPU: the Hugging Face converter for all four classes, the position-grid resampling, the GGUF keys vit.layer_scale /
-vit.reg_tokens / vit.pool, the extended emulation against an independent float64 oracle (transformers' DINOv2 classes), and the
+vit.reg_tokens / vit.pool, the emulation against an independent float64 oracle (transformers' DINOv2 classes), and the
 refusals that need no GPU."""
 import copy
 import ctypes as C
@@ -13,8 +13,8 @@ import pytest
 from tests.util import pkg, gf, model_path
 from tests import dinov2_oracle as do
 from tests import fp8_reference as fr
-from tests.clip_emulation import ArchEmulation
-from tests.dinov2_emulation import DinoEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 
 eng = pkg.engine
 cv = pkg.convert
@@ -32,13 +32,13 @@ def dino(request, tmp_path_factory):
     geo, classifier = request.param
     d = str(tmp_path_factory.mktemp(f"dino_{geo}_{classifier}"))
     m = do.build_hf(geo, classifier)
-    path = do.save_and_convert(m, d, geo)
+    path = save_and_convert(m, d, "dinov2", do.convert_size(geo))
     imgs = gf.synthetic_images(3, do.image_size(geo), seed=3)
     return geo, classifier, m, d, path, gf.read_gguf(path), imgs, do.hf_outputs(m, imgs)
 
 
 def _distances(vf, imgs, o, emu=None):
-    emu = emu or DinoEmulation(vf, acc=np.float64, fp8=False)
+    emu = emu or Emulation(vf, acc=np.float64, fp8=False)
     L = vf.num_hidden_layers
     x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
     d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]).max(), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"]).max()}
@@ -112,12 +112,12 @@ def test_a_broken_mapping_fails_the_oracle_check(dino):
         shifted.tensors["pos_embed"] = pos.reshape(1, -1, vf.hidden_size)
         bad["register position rows"] = _distances(shifted, imgs, o)
     if classifier:
-        class RegsInMean(DinoEmulation):
+        class RegsInMean(Emulation):
             def prelogits(self, x, norm=True):
                 y = rs_ln(self, x)
                 return np.concatenate([y[:, 0], y[:, 1:].mean(axis=1)], axis=1)
 
-        class ClsInMean(DinoEmulation):
+        class ClsInMean(Emulation):
             def prelogits(self, x, norm=True):
                 y = rs_ln(self, x)
                 return np.concatenate([y[:, 0], np.concatenate([y[:, :1], y[:, 1 + self.R:]], axis=1).mean(axis=1)], axis=1)
@@ -138,22 +138,12 @@ def rs_ln(emu, x):
     return rs.layernorm(x.reshape(-1, D), emu.norm_w, emu.norm_b, emu.eps).reshape(B, N, D)
 
 
-def test_extended_emulation_is_arch_emulation_without_the_new_keys():
-    vf = gf.read(model_path("micro", "f16"))
-    imgs = gf.synthetic_images(2, vf.img_size, seed=5)
-    for fp8 in (False, True):
-        a, b = DinoEmulation(vf, fp8=fp8), ArchEmulation(vf, fp8=fp8)
-        assert np.array_equal(a.forward(imgs), b.forward(imgs)), fp8
-        x = a.encode(imgs, 1)
-        assert np.array_equal(x, b.encode(imgs, 1)) and np.array_equal(a.prelogits(x), b.prelogits(x))
-
-
 def test_reference_and_clip_files_carry_no_new_keys(tmp_path):
     from tests import clip_oracle as co
     vf = gf.read(model_path("micro", "f16"))
     p = str(tmp_path / "m.gguf")
     gf.write_gguf(p, vf)
-    clip = co.save_and_convert(co.build_hf("micro"), str(tmp_path / "clip"))
+    clip = save_and_convert(co.build_hf("micro"), str(tmp_path / "clip"), "clip")
     for f in (p, clip):
         raw = open(f, "rb").read()
         assert b"vit.layer_scale" not in raw and b"vit.reg_tokens" not in raw and b"vit.pool" not in raw

@@ -1,5 +1,5 @@
 """The FP8 engine's host side, without a GPU: argument checks of the new entry points, the upload-time weight quantisation against
-torch's e4m3, and the accuracy cost of the FP8 recipe measured on its numpy emulation (tests/fp8_reference.py) against the
+torch's e4m3, and the accuracy cost of the FP8 recipe measured on its numpy emulation (tests/emulation.py) against the
 reference's golden logits."""
 import ctypes as C
 import os
@@ -10,6 +10,7 @@ import torch
 
 from tests.util import pkg, gf, model_path
 from tests import fp8_reference as fr
+from tests.emulation import Emulation
 
 eng = pkg.engine
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -113,9 +114,9 @@ def test_emulated_accuracy_cost_and_floor(cfg, ftype):
     g = np.load(os.path.join(GOLD, f"{cfg}_{ftype}.npz"))
     vf = gf.read(model_path(cfg, ftype))
     imgs = gf.synthetic_images(int(g["n_images"]), vf.img_size, seed=int(g["image_seed"]))
-    f16 = fr.Fp8Emulation(vf, fp8=False).forward(imgs)
-    e32 = fr.Fp8Emulation(vf).forward(imgs)
-    e64 = fr.Fp8Emulation(vf, acc=np.float64).forward(imgs)
+    f16 = Emulation(vf, fp8=False).forward(imgs)
+    e32 = Emulation(vf).forward(imgs)
+    e64 = Emulation(vf, acc=np.float64).forward(imgs)
     # the emulation's f16 form reproduces the golden logits as closely as the f16 engine does: the shared pieces are right
     assert fr.rel_dist(f16, g["logits"]).max() <= (2e-2 if ftype == "q8_0" else 1.5e-3)
     cost = fr.rel_dist(e32, g["logits"])

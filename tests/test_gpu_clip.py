@@ -1,6 +1,5 @@
 """CLIP image towers on the GPU (vitb200_arch: the pre-norm and the QuickGELU / erf-GELU fc1 epilogues), against the float64 Hugging
-Face oracle of tests/clip_oracle.py and the emulation of tests/fp8_reference.py extended to the
-architecture (tests/clip_emulation.py).
+Face oracle of tests/clip_oracle.py and the emulation of tests/emulation.py.
 
 End to end, every output is held to twice the emulation's own distance from the oracle, measured here on the CPU on the same images:
 the emulation has the engine's roundings (f16 GEMM operands, the reference's f16 soft-max table) and the oracle has none, so an engine
@@ -11,7 +10,8 @@ import pytest
 from tests.util import pkg, gf
 from tests import clip_oracle as co
 from tests import fp8_reference as fr
-from tests.clip_emulation import ArchEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 from tests.test_gpu_fp8 import E2E_TOL
 
 eng = pkg.engine
@@ -100,11 +100,11 @@ def _case(geo, act, tmp_path_factory):
     if key not in _built:
         d = str(tmp_path_factory.mktemp(f"{geo}_{act}"))
         m = co.build_hf(geo, act)
-        path = co.save_and_convert(m, d)
+        path = save_and_convert(m, d, "clip")
         vf = gf.read_gguf(path)
         imgs = gf.synthetic_images(3, vf.img_size, seed=3)
         o = co.hf_outputs(m, imgs)
-        emu = ArchEmulation(vf, acc=np.float64, fp8=False)
+        emu = Emulation(vf, acc=np.float64, fp8=False)
         L = vf.num_hidden_layers
         x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
         emu_d = {"logits": fr.rel_dist(emu.forward(imgs), o["image_embeds"]),
@@ -137,7 +137,7 @@ def test_end_to_end_against_the_hf_oracle(geo, act, tmp_path_factory):
     bad = {k: (got[k].max(), emu_d[k].max()) for k in got if got[k].max() > 2 * emu_d[k].max()}
     assert not bad, bad
     # and against the f16 emulation in f32, as test_gpu_geometry.py holds the logits to the restatement
-    emu32 = ArchEmulation(vf, fp8=False).forward(imgs)
+    emu32 = Emulation(vf, fp8=False).forward(imgs)
     d32 = fr.rel_dist(logits, emu32)
     print(f"{geo} {act}: GPU vs f16 emulation {np.array2string(d32, precision=6)}")
     assert d32.max() <= (1.5e-3 if vf.n_tokens <= 224 else 2e-3), d32
@@ -194,6 +194,6 @@ def test_fp8_engine_against_the_fp8_emulation(geo, act, tmp_path_factory):
     assert m.fp8 and m.arch["pre_norm"]
     logits = eng.vit_predict(m, imgs, 5, want_logits=True)[3]
     m.close()
-    d = fr.rel_dist(logits, ArchEmulation(vf).forward(imgs))
+    d = fr.rel_dist(logits, Emulation(vf).forward(imgs))
     print(f"{geo} {act} FP8: GPU vs emulation {np.array2string(d, precision=4)} (bound {E2E_TOL:.4f})")
     assert d.max() <= E2E_TOL, d

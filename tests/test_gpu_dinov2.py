@@ -1,5 +1,5 @@
 """DINOv2 on the GPU (vitb200_arch: the LayerScale residual epilogue, register tokens and the class-plus-patch-mean pool), against the
-float64 Hugging Face oracle of tests/dinov2_oracle.py and the emulation of tests/dinov2_emulation.py.
+float64 Hugging Face oracle of tests/dinov2_oracle.py and the emulation of tests/emulation.py.
 
 End to end, every output is held to twice the emulation's own distance from the oracle, measured here on the CPU on the same images
 (as tests/test_gpu_clip.py does): the emulation has the engine's roundings and the oracle has none."""
@@ -9,7 +9,8 @@ import pytest
 from tests.util import pkg, gf
 from tests import dinov2_oracle as do
 from tests import fp8_reference as fr
-from tests.dinov2_emulation import DinoEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 from tests.test_gpu_fp8 import E2E_TOL
 
 eng = pkg.engine
@@ -51,11 +52,11 @@ def _case(geo, classifier, tmp_path_factory):
     if key not in _built:
         d = str(tmp_path_factory.mktemp(f"{geo}_{classifier}"))
         m = do.build_hf(geo, classifier)
-        path = do.save_and_convert(m, d, geo)
+        path = save_and_convert(m, d, "dinov2", do.convert_size(geo))
         vf = gf.read_gguf(path)
         imgs = gf.synthetic_images(3, vf.img_size, seed=3)
         o = do.hf_outputs(m, imgs)
-        emu = DinoEmulation(vf, acc=np.float64, fp8=False)
+        emu = Emulation(vf, acc=np.float64, fp8=False)
         L = vf.num_hidden_layers
         x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
         emu_d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"])}
@@ -96,13 +97,13 @@ def test_prelogits_forms_agree():
     import tempfile
     geo = "micro_reg"
     d = tempfile.mkdtemp()
-    path = do.save_and_convert(do.build_hf(geo, True), d, geo)
+    path = save_and_convert(do.build_hf(geo, True), d, "dinov2", do.convert_size(geo))
     vf = gf.read_gguf(path)
     imgs = gf.synthetic_images(3, vf.img_size, seed=4)
     m = eng.vit_model_load(path, 0, 3)
     L = vf.num_hidden_layers
     tok, pre = eng.vit_features(m, imgs, layers=L, norm=False, prelogits=True)
-    emu = DinoEmulation(vf, fp8=False)
+    emu = Emulation(vf, fp8=False)
     for norm in (False, True):
         want = emu.prelogits(tok, norm=norm)
         f32 = eng.vit_features(m, imgs, layers=L, norm=norm, tokens=False, prelogits=True)[1].reshape(3, -1)
@@ -168,6 +169,6 @@ def test_fp8_engine_against_the_fp8_emulation(geo, classifier, tmp_path_factory)
     assert m.fp8 and m.layer_scale
     logits = eng.vit_predict(m, imgs, 5, want_logits=True)[3]
     m.close()
-    d = fr.rel_dist(logits, DinoEmulation(vf).forward(imgs))
+    d = fr.rel_dist(logits, Emulation(vf).forward(imgs))
     print(f"{geo} FP8: GPU vs emulation {np.array2string(d, precision=4)} (bound {E2E_TOL:.4f})")
     assert d.max() <= E2E_TOL, d

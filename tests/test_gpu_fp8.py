@@ -1,5 +1,5 @@
 """The FP8 engine on the GPU: the e4m3 GEMM element by element, the e4m3 LayerNorm against the emulation, end-to-end logits against
-the emulation of the recipe (tests/fp8_reference.py), and every entry point on an FP8 engine."""
+the emulation of the recipe (tests/emulation.py), and every entry point on an FP8 engine."""
 import math
 import os
 
@@ -8,6 +8,7 @@ import pytest
 
 from tests.util import pkg, gf, model_path
 from tests import fp8_reference as fr
+from tests.emulation import Emulation
 from tests.test_fp8_abi import FP8_FLOOR_MAX
 from tests import test_gpu_gemm_schedule as gs
 from oracle import restatement as rs
@@ -179,7 +180,7 @@ def test_logits_match_the_emulation(cfg, ftype):
     assert m.fp8
     probs, idx, val, logits = eng.vit_predict(m, imgs, 5, want_logits=True)
     m.close()
-    emu = fr.Fp8Emulation(vf).forward(imgs)
+    emu = Emulation(vf).forward(imgs)
     d = fr.rel_dist(logits, emu)
     print(f"{cfg} {ftype}: GPU vs emulation {np.round(d, 4)}, GPU vs golden {np.round(fr.rel_dist(logits, g['logits']), 4)}")
     assert d.max() <= E2E_TOL
@@ -305,7 +306,7 @@ def test_vitstr_recognition_on_an_fp8_engine():
     assert m.fp8 and m.head_tokens == 25
     imgs = gf.synthetic_gray_images(int(g["n_images"]), vf.img_size, seed=int(g["image_seed"]))
     probs, idx, val, logits = eng.vit_predict(m, imgs, 1, want_logits=True)
-    emu = fr.Fp8Emulation(vf, head_tokens=25).forward(imgs)
+    emu = Emulation(vf, head_tokens=25).forward(imgs)
     assert fr.rel_dist(logits, emu).max() <= E2E_TOL
     rng = np.random.default_rng(2)
     u8 = [rng.integers(0, 256, size=(32, 100, 3), dtype=np.uint8) for _ in range(4)]

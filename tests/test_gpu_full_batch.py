@@ -15,7 +15,7 @@ from tests.util import pkg, gf
 from tests import clip_oracle as co
 from tests import dinov2_oracle as do
 from tests import siglip_oracle as so
-from tests import swiglu_oracle as swo
+from tests.hf_oracle import save_and_convert
 
 eng = pkg.engine
 pytestmark = pytest.mark.gpu
@@ -37,13 +37,13 @@ def _model(family, geo, variant, tmp_path_factory):
         t0 = time.perf_counter()
         d = str(tmp_path_factory.mktemp(f"full_{family}_{geo}_{variant}"))
         if family == "clip":
-            path = co.save_and_convert(co.build_hf(geo, variant), d)
+            path = save_and_convert(co.build_hf(geo, variant), d, "clip")
         elif family == "dinov2":
-            path = do.save_and_convert(do.build_hf(geo, variant), d, geo)
+            path = save_and_convert(do.build_hf(geo, variant), d, "dinov2", do.convert_size(geo))
         elif family == "siglip":
-            path = so.save_and_convert(so.build_hf(geo, variant), d)
+            path = save_and_convert(so.build_hf(geo, variant), d, "siglip")
         else:
-            path = swo.save_and_convert(swo.build_hf(geo, variant), d, geo)
+            path = save_and_convert(do.build_hf(geo, variant, swiglu=True), d, "dinov2", do.convert_size(geo))
         print(f"{family} {geo} {variant}: HF model built and converted in {time.perf_counter() - t0:.1f} s (CPU)")
         _built[key] = path
     return _built[key]

@@ -17,7 +17,7 @@ import pytest
 from scipy.special import ndtr
 
 from tests.util import pkg
-from tests.siglip_emulation import gelu_pytorch_tanh
+from tests.emulation import gelu_pytorch_tanh
 from oracle import restatement as rs
 
 eng = pkg.engine

@@ -20,6 +20,7 @@ from tests.util import pkg, gf, model_path
 from tests.test_gpu_forward import check_parity, rel_err
 from tests.test_gpu_fp8 import E2E_TOL
 from tests import fp8_reference as fr
+from tests.emulation import Emulation
 from oracle import restatement as rs
 
 eng = pkg.engine
@@ -153,7 +154,7 @@ def test_fp8_engine(cfg):
             assert np.abs(got - want).max() <= np.abs(want).max() / 8, (layer, name)
     logits = eng.vit_predict(m, imgs, 5, want_logits=True)[3]
     m.close()
-    emu = fr.Fp8Emulation(vf, head_tokens=ht).forward(imgs)
+    emu = Emulation(vf, head_tokens=ht).forward(imgs)
     d = fr.rel_dist(logits, emu)
     print(f"{cfg} FP8: GPU vs emulation {np.array2string(d, precision=4)} (bound {E2E_TOL:.4f})")
     assert d.max() <= E2E_TOL, d

@@ -10,6 +10,7 @@ import pytest
 
 from tests import clip_oracle as co
 from tests import dinov2_oracle as do
+from tests.hf_oracle import save_and_convert
 from tests.util import pkg, gf, model_path
 
 eng = pkg.engine
@@ -27,10 +28,10 @@ def _path(geo, tmp_path_factory):
     if geo not in _paths:
         if geo == "clip_micro":
             d = str(tmp_path_factory.mktemp("clip_micro"))
-            _paths[geo] = co.save_and_convert(co.build_hf("micro", "quick_gelu"), d)
+            _paths[geo] = save_and_convert(co.build_hf("micro", "quick_gelu"), d, "clip")
         elif geo == "dinov2_micro_reg":
             d = str(tmp_path_factory.mktemp("dinov2_micro_reg"))
-            _paths[geo] = do.save_and_convert(do.build_hf("micro_reg", True), d, "micro_reg")
+            _paths[geo] = save_and_convert(do.build_hf("micro_reg", True), d, "dinov2", do.convert_size("micro_reg"))
         else:
             _paths[geo] = model_path(geo, "f16")
     return _paths[geo]

@@ -1,5 +1,5 @@
 """SigLIP on the GPU (vitb200_arch pools 2 and 3, activation 3): the gelu_pytorch_tanh epilogue and the probe-attention kernel alone, and
-end to end against the float64 Hugging Face oracle of tests/siglip_oracle.py and the emulation of tests/siglip_emulation.py.
+end to end against the float64 Hugging Face oracle of tests/siglip_oracle.py and the emulation of tests/emulation.py.
 
 End to end, every output is held to twice the emulation's own distance from the oracle, measured here on the CPU on the same images
 (as tests/test_gpu_dinov2.py does): the emulation has the engine's roundings and the oracle has none."""
@@ -9,7 +9,8 @@ import pytest
 from tests.util import pkg, gf
 from tests import siglip_oracle as so
 from tests import fp8_reference as fr
-from tests.siglip_emulation import SiglipEmulation, gelu_pytorch_tanh
+from tests.emulation import Emulation, gelu_pytorch_tanh
+from tests.hf_oracle import save_and_convert
 from tests.test_gpu_fp8 import E2E_TOL
 
 eng = pkg.engine
@@ -137,11 +138,11 @@ def _case(geo, classifier, tmp_path_factory):
     if key not in _built:
         d = str(tmp_path_factory.mktemp(f"{geo}_{classifier}"))
         m = so.build_hf(geo, classifier)
-        path = so.save_and_convert(m, d)
+        path = save_and_convert(m, d, "siglip")
         vf = gf.read_gguf(path)
         imgs = gf.synthetic_images(3, vf.img_size, seed=3)
         o = so.hf_outputs(m, imgs)
-        emu = SiglipEmulation(vf, acc=np.float64, fp8=False)
+        emu = Emulation(vf, acc=np.float64, fp8=False)
         L = vf.num_hidden_layers
         x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
         emu_d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"]),
@@ -197,7 +198,7 @@ def test_prelogits_forms_and_the_norm_requirement(tmp_path_factory):
             assert np.array_equal(bf, torch.from_numpy(f32).to(torch.bfloat16).view(torch.int16).numpy().view(np.uint16))
             if classifier:
                 tok = eng.vit_features(m, imgs, layers=L, norm=False)[0]
-                assert fr.rel_dist(f32, SiglipEmulation(vf, fp8=False).prelogits(tok, norm=norm)).max() <= 2e-6
+                assert fr.rel_dist(f32, Emulation(vf, fp8=False).prelogits(tok, norm=norm)).max() <= 2e-6
         if not classifier:
             launches = m.last_launch_count()
             with pytest.raises(eng.VitB200Error, match="prelogits need norm = 1"):
@@ -205,7 +206,7 @@ def test_prelogits_forms_and_the_norm_requirement(tmp_path_factory):
             assert m.last_launch_count() == launches
             # the head at another depth, and the tokens staged next to it on the host path
             tok, pre = eng.vit_features(m, imgs, layers=1, norm=True, prelogits=True)
-            emu = SiglipEmulation(vf, fp8=False)
+            emu = Emulation(vf, fp8=False)
             x1 = emu.encode(imgs, 1)
             assert fr.rel_dist(pre.reshape(3, -1), emu.prelogits(x1)).max() <= 1e-2
             assert fr.rel_dist(tok, emu.final_ln(x1)).max() <= 1e-2
@@ -318,6 +319,6 @@ def test_fp8_engine_against_the_fp8_emulation(geo, classifier, tmp_path_factory)
     assert m.fp8 and m.pool == ("mean" if classifier else "map")
     logits = eng.vit_predict(m, imgs, 5, want_logits=True)[3]
     m.close()
-    d = fr.rel_dist(logits, SiglipEmulation(vf).forward(imgs))
+    d = fr.rel_dist(logits, Emulation(vf).forward(imgs))
     print(f"{geo} FP8: GPU vs emulation {np.array2string(d, precision=4)} (bound {E2E_TOL:.4f})")
     assert d.max() <= E2E_TOL, d

@@ -1,5 +1,5 @@
 """SwiGLU MLPs on the GPU (vitb200_arch.activation = 4, DINOv2 ViT-g): the fc1 epilogue alone in its f16 and e4m3 forms, and whole
-models against the float64 Hugging Face oracle of tests/swiglu_oracle.py and the emulation of tests/swiglu_emulation.py.
+models against the float64 Hugging Face oracle of tests/dinov2_oracle.py and the emulation of tests/emulation.py.
 
 End to end, every output is held to twice the emulation's own distance from the oracle, measured here on the CPU on the same images
 (the rule of tests/test_gpu_dinov2.py): the emulation has the engine's roundings and the oracle has none."""
@@ -7,9 +7,10 @@ import numpy as np
 import pytest
 
 from tests.util import pkg, gf
-from tests import swiglu_oracle as so
+from tests import dinov2_oracle as do
 from tests import fp8_reference as fr
-from tests.swiglu_emulation import SwigluEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 from tests.test_gpu_fp8 import E2E_TOL
 
 eng = pkg.engine
@@ -82,12 +83,12 @@ def _case(geo, classifier, tmp_path_factory):
     key = (geo, classifier)
     if key not in _built:
         d = str(tmp_path_factory.mktemp(f"swiglu_{geo}_{classifier}"))
-        m = so.build_hf(geo, classifier)
-        path = so.save_and_convert(m, d, geo)
+        m = do.build_hf(geo, classifier, swiglu=True)
+        path = save_and_convert(m, d, "dinov2", do.convert_size(geo))
         vf = gf.read_gguf(path)
         imgs = gf.synthetic_images(3, vf.img_size, seed=3)
-        o = so.hf_outputs(m, imgs)
-        emu = SwigluEmulation(vf, acc=np.float64, fp8=False)
+        o = do.hf_outputs(m, imgs)
+        emu = Emulation(vf, acc=np.float64, fp8=False)
         L = vf.num_hidden_layers
         x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
         emu_d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"])}
@@ -199,6 +200,6 @@ def test_fp8_engine_against_the_fp8_emulation(geo, classifier, tmp_path_factory)
     assert m.fp8 and m.arch["activation"] == "swiglu"
     logits = eng.vit_predict(m, imgs, 5, want_logits=True)[3]
     m.close()
-    d = fr.rel_dist(logits, SwigluEmulation(vf).forward(imgs))
+    d = fr.rel_dist(logits, Emulation(vf).forward(imgs))
     print(f"{geo} FP8: GPU vs emulation {np.array2string(d, precision=4)} (bound {E2E_TOL:.4f})")
     assert d.max() <= E2E_TOL, d

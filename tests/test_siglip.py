@@ -1,5 +1,5 @@
 """SigLIP on the CPU: the Hugging Face converter for SiglipVisionModel, the vision tower of SiglipModel and SiglipForImageClassification,
-the GGUF values vit.pool "map" / "mean" and vit.activation "gelu_pytorch_tanh", the extended emulation against an independent float64
+the GGUF values vit.pool "map" / "mean" and vit.activation "gelu_pytorch_tanh", the emulation against an independent float64
 oracle (transformers' SigLIP classes), and the refusals that need no GPU."""
 import copy
 import ctypes as C
@@ -14,8 +14,8 @@ import pytest
 from tests.util import pkg, gf, model_path
 from tests import siglip_oracle as so
 from tests import fp8_reference as fr
-from tests.dinov2_emulation import DinoEmulation
-from tests.siglip_emulation import SiglipEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 
 eng = pkg.engine
 cv = pkg.convert
@@ -33,13 +33,13 @@ def sig(request, tmp_path_factory):
     classifier = request.param
     d = str(tmp_path_factory.mktemp(f"siglip_{classifier}"))
     m = so.build_hf("micro", classifier)
-    path = so.save_and_convert(m, d)
+    path = save_and_convert(m, d, "siglip")
     imgs = gf.synthetic_images(3, so.image_size("micro"), seed=3)
     return classifier, m, d, path, gf.read_gguf(path), imgs, so.hf_outputs(m, imgs)
 
 
 def _distances(vf, imgs, o, emu=None):
-    emu = emu or SiglipEmulation(vf, acc=np.float64, fp8=False)
+    emu = emu or Emulation(vf, acc=np.float64, fp8=False)
     L = vf.num_hidden_layers
     x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
     d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]).max(), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"]).max()}
@@ -106,7 +106,7 @@ def test_emulation_matches_the_hf_oracle(sig):
     assert max(d.values()) <= EMU_BOUND, d
 
 
-class _PreLnPool(SiglipEmulation):
+class _PreLnPool(Emulation):
     """Pools the residual stream without the final LayerNorm."""
 
     def prelogits(self, x, norm=True):
@@ -114,7 +114,7 @@ class _PreLnPool(SiglipEmulation):
         return self.map_head(y) if self.pool == "map" else y.astype(np.float64).mean(axis=1).astype(np.float32)
 
 
-class _NoMlpResidual(SiglipEmulation):
+class _NoMlpResidual(Emulation):
     """The head's MLP output without the residual h."""
 
     def map_head(self, y):
@@ -145,16 +145,6 @@ def test_a_broken_mapping_fails_the_oracle_check(sig):
         assert v > 10 * EMU_BOUND, (k, v)
 
 
-def test_extended_emulation_is_the_dinov2_emulation_without_the_new_keys():
-    vf = gf.read(model_path("micro", "f16"))
-    imgs = gf.synthetic_images(2, vf.img_size, seed=5)
-    for fp8 in (False, True):
-        a, b = SiglipEmulation(vf, fp8=fp8), DinoEmulation(vf, fp8=fp8)
-        assert np.array_equal(a.forward(imgs), b.forward(imgs)), fp8
-        x = a.encode(imgs, 1)
-        assert np.array_equal(x, b.encode(imgs, 1)) and np.array_equal(a.prelogits(x), b.prelogits(x))
-
-
 def test_reference_clip_and_dinov2_files_carry_no_new_keys(tmp_path):
     """No new value or tensor in a reference, CLIP or DINOv2 file, and the writer reproduces each of them byte for byte."""
     from tests import clip_oracle as co
@@ -162,8 +152,8 @@ def test_reference_clip_and_dinov2_files_carry_no_new_keys(tmp_path):
     vf = gf.read(model_path("micro", "f16"))
     p = str(tmp_path / "m.gguf")
     gf.write_gguf(p, vf)
-    clip = co.save_and_convert(co.build_hf("micro"), str(tmp_path / "clip"))
-    dino = do.save_and_convert(do.build_hf("micro_reg", True), str(tmp_path / "dino"), "micro_reg")
+    clip = save_and_convert(co.build_hf("micro"), str(tmp_path / "clip"), "clip")
+    dino = save_and_convert(do.build_hf("micro_reg", True), str(tmp_path / "dino"), "dinov2", do.convert_size("micro_reg"))
     for f in (p, clip, dino):
         raw = open(f, "rb").read()
         assert b"gelu_pytorch_tanh" not in raw and b"attn_pool" not in raw

@@ -11,9 +11,9 @@ import pytest
 
 from tests.util import pkg, gf, model_path
 from tests import dinov2_oracle as do
-from tests import swiglu_oracle as so
 from tests import fp8_reference as fr
-from tests.swiglu_emulation import SwigluEmulation
+from tests.emulation import Emulation
+from tests.hf_oracle import save_and_convert
 
 eng = pkg.engine
 cv = pkg.convert
@@ -31,14 +31,14 @@ D, F = 128, 344
 def dino(request, tmp_path_factory):
     geo, classifier = request.param
     d = str(tmp_path_factory.mktemp(f"swiglu_{geo}_{classifier}"))
-    m = so.build_hf(geo, classifier)
-    path = so.save_and_convert(m, d, geo)
-    imgs = gf.synthetic_images(3, so.image_size(geo), seed=3)
-    return geo, classifier, m, d, path, gf.read_gguf(path), imgs, so.hf_outputs(m, imgs)
+    m = do.build_hf(geo, classifier, swiglu=True)
+    path = save_and_convert(m, d, "dinov2", do.convert_size(geo))
+    imgs = gf.synthetic_images(3, do.image_size(geo), seed=3)
+    return geo, classifier, m, d, path, gf.read_gguf(path), imgs, do.hf_outputs(m, imgs)
 
 
 def _distances(vf, imgs, o):
-    emu = SwigluEmulation(vf, acc=np.float64, fp8=False)
+    emu = Emulation(vf, acc=np.float64, fp8=False)
     L = vf.num_hidden_layers
     x = {i: emu.encode(imgs, i) for i in (0, L - 1, L)}
     d = {"logits": fr.rel_dist(emu.forward(imgs), o["logits"]).max(), "prelogits": fr.rel_dist(emu.prelogits(x[L]), o["prelogits"]).max()}
@@ -49,7 +49,7 @@ def _distances(vf, imgs, o):
 def test_conversion_round_trip(dino):
     """weights_in and weights_out land as fc1 [2 F][D] and fc2 [D][F] unchanged, in HF's x1 | x2 order; the file says "swiglu"."""
     geo, classifier, m, _, path, vf, _, _ = dino
-    R, L = so.GEOMETRIES[geo][5], 2
+    R, L = do.GEOMETRIES[geo][5], 2
     assert m.config.use_swiglu_ffn
     assert (vf.layer_scale, vf.reg_tokens, vf.pool, vf.activation) == (1, R, "cls_patch_mean" if classifier else "token", "swiglu")
     assert b"swiglu" in open(path, "rb").read()
@@ -101,7 +101,7 @@ def test_swiglu_config_ignores_hidden_act_and_mlp_ratio(dino, tmp_path):
     sd = {k: v.detach().numpy() for k, v in m.state_dict().items()}
     out = str(tmp_path / "x.gguf")
     cv.dinov2_to_model_file(sd, {"num_attention_heads": 2, "use_swiglu_ffn": True, "hidden_act": "relu", "mlp_ratio": 3}, out,
-                            img_size=so.image_size(geo))
+                            img_size=do.image_size(geo))
     back = gf.read_gguf(out)
     assert back.activation == "swiglu"
     for k, a in vf.tensors.items():
