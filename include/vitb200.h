@@ -131,8 +131,8 @@ typedef struct vitb200_arch
  * ls1 / ls2 gamma, reg_tokens > 0 without 'reg_token', pool > 0 with head_tokens > 1, pool 2 or 3 with a 'cls_token' tensor, with
  * reg_tokens > 0 or with a 'pos_embed' of other than P rows, pool 2 without one of its 13 'attn_pool.*' tensors, and a head whose K is
  * not D (pools 0, 2, 3) or 2 D (pool 1) fail here before the device is touched; so does N > 896 tokens, registers included.  Every entry
- * point works on such an engine; the u8 entry points keep vit.cpp's preprocessing (a CLIP, DINOv2 or SigLIP caller normalises its own
- * images and uses the f32 or device entry points).  The launch count of one forward is 3 + 7 L + 3 for pools 0 and 1, plus 1 with the
+ * point works on such an engine; the u8 entry points keep vit.cpp's preprocessing unless an image processor is set
+ * (vitb200_set_image_proc: Hugging Face's CLIP, SigLIP and DINOv2 preprocessing).  The launch count of one forward is 3 + 7 L + 3 for pools 0 and 1, plus 1 with the
  * pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm); 2 + 7 L + 3 for pool 3 (no class-row kernel); 2 + 7 L + 10 for
  * pool 2 (the head adds LN, k | v GEMM, attention, out_proj, LN, fc1, fc2 and the f16 rounding of its row).
  * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer), vit.activation ("gelu_tanh", "gelu_erf",
@@ -204,6 +204,38 @@ int vitb200_forward_u8(vitb200_engine *e, const uint8_t *const *images, const in
 int vitb200_forward_u8_async(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                              float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k);
 
+/* ---- Hugging Face image processors (no reference counterpart) ------------------------------------------------------------------
+ * CLIP, SigLIP and DINOv2 towers were trained on pixels prepared by Hugging Face's image processors (CLIPImageProcessor,
+ * SiglipImageProcessor, BitImageProcessor), not by vit_image_preprocess.  With an image processor set, every RGB u8 entry point
+ * (vitb200_forward_u8, vitb200_forward_u8_async, vitb200_features_u8, images_f32_out included) prepares its images as the PIL backend
+ * of those processors does, bit for bit: Pillow's Image.resize (8-bit ImagingResample, anti-aliased when it downscales), HF's centre
+ * crop, x = f32(f64(v) * rescale_factor), y = (x - mean_c) / std_c in f32.  images_f32_out then holds HF's pixel_values, in HWC order.
+ * The resize and the crop run in two kernels, a horizontal pass into a per-slot scratch and a vertical pass that writes the patch
+ * matrix, so a processor call launches one kernel more than vit_image_preprocess (vitb200_forward_u8 without outputs: 2).
+ * The processor is read on the host when a call is enqueued; changing it between asynchronous calls is safe.  bilinear != 0 is
+ * refused while one is set (the processor fixes the resample). */
+typedef struct vitb200_image_proc
+{
+    int32_t shortest_edge;           /* > 0: resize so the short side is this and the long side int(shortest_edge * long / short) (HF's
+                                      * get_resize_output_image_size, default_to_square = False); 0: resize to height x width */
+    int32_t height, width;           /* the resize target when shortest_edge == 0 */
+    int32_t crop_height, crop_width; /* HF's centre crop after the resize: top = (h - crop_h) / 2, left = (w - crop_w) / 2; 0 = none */
+    int32_t resample;                /* Pillow's ids, as preprocessor_config.json stores them: 2 BILINEAR, 3 BICUBIC */
+    double rescale_factor;           /* x = f32(f64(v) * rescale_factor) (1.0 when the config's do_rescale is false) */
+    float mean[3], std[3];           /* y = (x - mean_c) / std_c in f32 (0 and 1 when do_normalize is false) */
+} vitb200_image_proc;
+/* Set (p != NULL) or clear (p == NULL: back to vit_image_preprocess) the engine's image processor.  Refused, naming the field, before
+ * anything changes: a 1-channel (ViTSTR) engine; resample other than 2 or 3; a negative or missing size (shortest_edge 0 with height or
+ * width <= 0, or one crop extent 0 and the other not); shortest_edge without a crop (the output shape would depend on the image); a crop
+ * larger than the resize target (HF would pad); a final size other than img_size x img_size; a non-finite or non-positive
+ * rescale_factor; a non-finite mean; a zero or non-finite std.  A call is refused when an image's taps along one axis do not fit in
+ * shared memory: a bicubic downscale by more than 453, or a bilinear one by more than 906, along one axis.
+ * A GGUF file carries a processor in the optional keys vit.image_proc.shortest_edge, .height, .width, .crop_height, .crop_width,
+ * .resample (integers), .rescale_factor (float64), .image_mean and .image_std (arrays of 3 float32); the loader sets it through the
+ * same checks.  A file without them, and every legacy-ggml file, has none. */
+int vitb200_set_image_proc(vitb200_engine *e, const vitb200_image_proc *p);
+int vitb200_get_image_proc(const vitb200_engine *e, vitb200_image_proc *out); /* 0; *out all zero when none is set */
+
 /* Text recognition with a ViTSTR model (1-channel, head_tokens >= 2; reference extensions/vitstr.cpp), image to text on the GPU:
  * the extension's vit_image_preprocess (vitstr.cpp:128-201: grayscale in double, its own bilinear resize to img^2 with no half-pixel
  * offset, (v / 255 - 0.5) * 2), the forward pass, and its greedy decode (vitstr.cpp:1020-1054: the arg-max of token rows
@@ -263,7 +295,7 @@ int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const i
                         const vitb200_features_req *req, void *tokens, void *prelogits);
 
 /* Number of kernels launched by the most recent call on this engine that enqueued work: a forward, features or recognition call,
- * including one that only pre-processes images (vitb200_forward_u8 without outputs: 1).  A call rejected by its argument checks
+ * including one that only pre-processes images (vitb200_forward_u8 without outputs: 1, or 2 with an image processor).  A call rejected by its argument checks
  * leaves the count as it was. */
 int vitb200_last_launch_count(const vitb200_engine *e);
 

@@ -5,6 +5,8 @@
     python -m convert <CLIP model.safetensors|.pth> <out.gguf> --hf-config config.json             (Hugging Face CLIP vision tower)
     python -m convert <DINOv2 model.safetensors> <out.gguf> --hf-config config.json [--img-size S]  (Hugging Face DINOv2)
     python -m convert <SigLIP model.safetensors> <out.gguf> --hf-config config.json               (Hugging Face SigLIP vision tower)
+    python -m convert <any of the above, or a converted model file> <out.gguf> ... --hf-preprocessor preprocessor_config.json
+                                                                    (the u8 entry points prepare images as this HF image processor does)
     python -m convert --quantize <in.gguf> <out.gguf> q8_0
 
 * `state_dict_to_model_file` follows reference convert-pth-to-ggml.py:105-158 step by step (header, id2label table, tensors in
@@ -143,13 +145,14 @@ def resample_pos_embed(pos: np.ndarray, prefix: int, grid: int, antialias: bool 
 def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: int = 1, heads: Optional[int] = None,
                              id2label: Optional[Dict[int, str]] = None, container: str = "legacy", keep_norm_pre: bool = False,
                              activation: str = "gelu_tanh", eps: float = 1e-6, pool: str = "token", img_size: Optional[int] = None,
-                             antialias: bool = False) -> None:
+                             antialias: bool = False, image_proc: Optional[dict] = None) -> None:
     """keep_norm_pre, activation, eps: the architecture of a CLIP-pretrained timm ViT (norm_pre, QuickGELU or erf GELU, eps 1e-5);
     GGUF only.  Without them the file is the reference converter's, which drops norm_pre.  LayerScale ('blocks.{i}.ls1.gamma' /
     'ls2.gamma') and register tokens ('reg_token', with their R rows after the class row of pos_embed) are taken when the state dict has
     them; pool 'cls_patch_mean' makes the head read [class token || patch mean] (DINOv2's classifier); pools 'map' and 'mean' (SigLIP) are
     for a state dict without 'cls_token', 'map' with the 13 'attn_pool.*' tensors.  img_size: resample the patch position grid to
-    img_size / patch (resample_pos_embed)."""
+    img_size / patch (resample_pos_embed).  image_proc: a Hugging Face preprocessor_config.json dict, written as the vit.image_proc.* keys
+    (GGUF only) after gf.image_proc_from_config has checked it against the model's input size."""
     assert ftype in (0, 1)
     layer_scale = int(any(k.endswith(".ls1.gamma") for k in sd))
     R = reg_token_count(sd)
@@ -168,12 +171,15 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
     if container != "gguf" and (keep_norm_pre or activation != "gelu_tanh" or eps != 1e-6):
         raise ValueError("a pre-norm, another activation or another eps needs --container gguf: a legacy ggml file carries the "
                          "reference's architecture only")
+    if container != "gguf" and image_proc is not None:
+        raise ValueError("an image processor needs --container gguf: a legacy ggml file carries vit.cpp's preprocessing only")
     if keep_norm_pre and not ("norm_pre.weight" in sd and "norm_pre.bias" in sd):
         raise ValueError("keep_norm_pre: the state_dict has no norm_pre.weight / norm_pre.bias")
     hidden, layers, heads, classes, patch, img, in_chans = infer_hparams(sd, heads)
     id2label = id2label or {i: f"LABEL_{i}" for i in range(classes)}   # convert-pth-to-ggml.py:95-96 fallback names
     vf = gf.VitFile(hidden, layers, heads, classes, patch, img, ftype, dict(id2label), eps=eps, pre_norm=int(keep_norm_pre),
-                    activation=activation, layer_scale=layer_scale, reg_tokens=R, pool=pool)
+                    activation=activation, layer_scale=layer_scale, reg_tokens=R, pool=pool,
+                    image_proc=None if image_proc is None else gf.image_proc_from_config(image_proc, img))
     for k, v in sd.items():
         if k.startswith("norm_pre") and not keep_norm_pre:               # convert-pth-to-ggml.py:127-130
             continue
@@ -251,12 +257,13 @@ def clip_to_timm(sd: Dict[str, np.ndarray], config: dict):
 
 
 def clip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
-                       container: str = "gguf") -> None:
+                       container: str = "gguf", image_proc: Optional[dict] = None) -> None:
     """A Hugging Face CLIP vision tower -> GGUF model file (pre-norm, the config's activation and eps)."""
     if container != "gguf":
         raise ValueError("a CLIP tower needs --container gguf: a legacy ggml file carries the reference's architecture only")
     tsd, heads, activation, eps = clip_to_timm(sd, config)
-    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", keep_norm_pre=True, activation=activation, eps=eps)
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", keep_norm_pre=True, activation=activation, eps=eps,
+                             image_proc=image_proc)
 
 
 _DINOV2_PREFIXES = ("dinov2.", "dinov2_with_registers.")
@@ -330,7 +337,7 @@ def dinov2_to_timm(sd: Dict[str, np.ndarray], config: dict):
 
 
 def dinov2_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
-                         container: str = "gguf", img_size: Optional[int] = None) -> None:
+                         container: str = "gguf", img_size: Optional[int] = None, image_proc: Optional[dict] = None) -> None:
     """A Hugging Face DINOv2 -> GGUF model file (LayerScale, registers, erf GELU or SwiGLU, the config's eps; the classifier's pool)."""
     if container != "gguf":
         raise ValueError("a DINOv2 model needs --container gguf: a legacy ggml file carries the reference's architecture only")
@@ -338,7 +345,7 @@ def dinov2_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str,
     if id2label is None and "id2label" in config and "classifier.weight" in sd:
         id2label = {int(k): str(x) for k, x in config["id2label"].items()}
     state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool, img_size=img_size,
-                             antialias=antialias)
+                             antialias=antialias, image_proc=image_proc)
 
 
 def is_hf_siglip(sd: Dict[str, np.ndarray]) -> bool:
@@ -402,7 +409,7 @@ def siglip_to_timm(sd: Dict[str, np.ndarray], config: dict):
 
 
 def siglip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
-                         container: str = "gguf") -> None:
+                         container: str = "gguf", image_proc: Optional[dict] = None) -> None:
     """A Hugging Face SigLIP vision tower -> GGUF model file (no class token, gelu_pytorch_tanh, the config's eps; pool 'map' or, with a
     classifier, 'mean')."""
     if container != "gguf":
@@ -410,7 +417,7 @@ def siglip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str,
     tsd, heads, activation, eps, pool = siglip_to_timm(sd, config)
     if id2label is None and "id2label" in config and "classifier.weight" in sd:
         id2label = {int(k): str(x) for k, x in config["id2label"].items()}
-    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool)
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool, image_proc=image_proc)
 
 
 def write_legacy(path: str, vf) -> None:
@@ -478,6 +485,16 @@ def quantize_model_file(src: str, dst: str, fmt: str = "q8_0") -> None:
     write_legacy(dst, out)
 
 
+def add_image_proc(src: str, dst: str, preprocessor_config: dict) -> None:
+    """A converted model file (GGUF, or the reference's legacy ggml with f32 / f16 tensors) -> GGUF with the vit.image_proc.* keys of a
+    Hugging Face preprocessor_config.json dict; tensors and the other keys unchanged."""
+    with open(src, "rb") as f:
+        gguf = f.read(4) == gf.GGUF_MAGIC
+    vf = gf.read_gguf(src) if gguf else gf.read(src)
+    vf.image_proc = gf.image_proc_from_config(preprocessor_config, vf.img_size)
+    gf.write_gguf(dst, vf, "keep")
+
+
 def main(argv):
     import argparse
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
@@ -496,32 +513,40 @@ def main(argv):
     ap.add_argument("--eps", type=float, default=1e-6, help="timm: the LayerNorm epsilon (GGUF only)")
     ap.add_argument("--img-size", type=int, default=None,
                     help="resample the patch position embeddings to this input size (default: the checkpoint's grid)")
+    ap.add_argument("--hf-preprocessor", default=None,
+                    help="preprocessor_config.json of a Hugging Face image processor: the u8 entry points prepare images as it does (GGUF)")
     a = ap.parse_args(argv)
     if a.quantize:
         quantize_model_file(a.src, a.dst, a.fmt)
         return
     labels = {int(k): v for k, v in json.load(open(a.labels)).items()} if a.labels else None
+    proc = json.load(open(a.hf_preprocessor)) if a.hf_preprocessor else None
+    with open(a.src, "rb") as f:
+        magic = f.read(4)
+    if proc is not None and (magic == gf.GGUF_MAGIC or magic == struct.pack("i", gf.GGML_FILE_MAGIC)):
+        add_image_proc(a.src, a.dst, proc)
+        return
     sd = load_state_dict(a.src)
     if is_hf_dinov2(sd):
         if not a.hf_config:
             raise SystemExit("a Hugging Face DINOv2 state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
-        dinov2_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", a.img_size)
+        dinov2_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", a.img_size, proc)
         return
     if is_hf_siglip(sd):
         if not a.hf_config:
             raise SystemExit("a Hugging Face SigLIP state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
         if a.img_size:
             raise SystemExit("--img-size: resampling a SigLIP tower's position embeddings is not supported")
-        siglip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf")
+        siglip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", proc)
         return
     if is_hf_clip(sd):
         if not a.hf_config:
             raise SystemExit("a Hugging Face CLIP state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")
-        clip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf")
+        clip_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype, labels, a.container or "gguf", proc)
         return
-    new_arch = a.keep_norm_pre or a.activation != "gelu_tanh" or a.eps != 1e-6
+    new_arch = a.keep_norm_pre or a.activation != "gelu_tanh" or a.eps != 1e-6 or proc is not None
     state_dict_to_model_file(sd, a.dst, a.ftype, a.heads, labels, a.container or ("gguf" if new_arch else "legacy"),
-                             a.keep_norm_pre, a.activation, a.eps, img_size=a.img_size)
+                             a.keep_norm_pre, a.activation, a.eps, img_size=a.img_size, image_proc=proc)
 
 
 if __name__ == "__main__":

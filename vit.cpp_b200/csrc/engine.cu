@@ -134,6 +134,15 @@ struct GraphKey
 
 // One of the two host-pipeline slots (vitb200_forward_async, the u8 and recognition entry points): call n uses slot n & 1, so its
 // H2D copy on the copy stream can overlap call n - 1's kernels on the compute stream
+// The image processor's layout of one u8 call (plan_proc): per-image geometry, the tap-table widths of the two passes, the most source
+// rows of one image and the scratch bytes of the horizontal pass
+struct ProcPlan
+{
+    std::vector<ProcGeom> geo;
+    int kh = 1, kv = 1, max_rows = 1;
+    size_t tmp_total = 0;
+};
+
 struct Slot
 {
     float *img = nullptr, *probs = nullptr, *logits = nullptr, *topk_val = nullptr;
@@ -145,6 +154,9 @@ struct Slot
     // descriptors) and its device twin; grown only when a batch needs more than any batch before it
     uint8_t *h_u8 = nullptr, *d_u8 = nullptr;
     size_t u8_cap = 0;
+    // the image processor's horizontal pass (vitb200_set_image_proc): [rows][img_size][3] u8 per image, grown like the staging buffer
+    uint8_t *d_proc = nullptr;
+    size_t proc_cap = 0;
     cudaEvent_t ev_h2d = nullptr, ev_done = nullptr;
 };
 
@@ -195,6 +207,10 @@ struct vitb200_engine
     cudaStream_t copy_stream = nullptr;
     Slot slot[2];
     unsigned long long submits = 0;
+    // Hugging Face's image preprocessing for the RGB u8 entry points (vitb200_set_image_proc); proc_geom is the per-call host table
+    bool has_proc = false;
+    vitb200_image_proc proc{};
+    ProcPlan proc_plan;
     // CUDA-graph cache for the kernel schedule of one forward, keyed by its arguments (launch-bound inner loop: ~90 kernels)
     struct GraphEntry { GraphKey key; int state; int launches; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -1704,6 +1720,59 @@ int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out)
     });
 }
 
+// vitb200_set_image_proc's checks for a model of C input channels and input size S, shared with the GGUF loader (which runs them before
+// it creates the engine); each refusal names the field
+static int check_image_proc(int C, int S, const vitb200_image_proc &p)
+{
+    if (C != 3) return fail("image_proc: this model takes %d-channel input; Hugging Face's image processors are for RGB models", C);
+    if (p.resample != 2 && p.resample != 3) return fail("image_proc.resample = %d: 2 (BILINEAR) or 3 (BICUBIC) only", p.resample);
+    if (p.shortest_edge < 0) return fail("image_proc.shortest_edge = %d: must not be negative", p.shortest_edge);
+    if (p.shortest_edge == 0 && (p.height <= 0 || p.width <= 0))
+        return fail("image_proc.height / width = %d x %d: must be positive when shortest_edge is 0", p.height, p.width);
+    if (p.crop_height < 0 || p.crop_width < 0 || (p.crop_height == 0) != (p.crop_width == 0))
+        return fail("image_proc.crop_height / crop_width = %d x %d: both positive, or both 0 (no crop)", p.crop_height, p.crop_width);
+    const bool crop = p.crop_height > 0;
+    if (p.shortest_edge > 0 && !crop)
+        return fail("image_proc.shortest_edge = %d without crop_height / crop_width: the output size would depend on the image", p.shortest_edge);
+    const int rh = p.shortest_edge > 0 ? p.shortest_edge : p.height, rw = p.shortest_edge > 0 ? p.shortest_edge : p.width;
+    if (crop && (p.crop_height > rh || p.crop_width > rw))
+        return fail("image_proc.crop_height / crop_width = %d x %d: larger than the resize target %d x %d (padding is not supported)", p.crop_height,
+                    p.crop_width, rh, rw);
+    const int fh = crop ? p.crop_height : p.height, fw = crop ? p.crop_width : p.width;
+    if (fh != S || fw != S)
+        return fail("image_proc: the final size %d x %d (%s) is not the model's img_size %d x %d", fh, fw, crop ? "crop_height x crop_width" : "height x width", S, S);
+    if (!std::isfinite(p.rescale_factor) || !(p.rescale_factor > 0.0)) return fail("image_proc.rescale_factor = %g: must be finite and positive", p.rescale_factor);
+    for (int c = 0; c < 3; ++c)
+    {
+        if (!std::isfinite(p.mean[c])) return fail("image_proc.mean[%d] = %g: must be finite", c, (double)p.mean[c]);
+        if (!std::isfinite(p.std[c]) || p.std[c] == 0.0f) return fail("image_proc.std[%d] = %g: must be finite and non-zero", c, (double)p.std[c]);
+    }
+    return 0;
+}
+
+static int set_image_proc(vitb200_engine *e, const vitb200_image_proc *p)
+{
+    if (!e) return fail("null argument");
+    if (p && check_image_proc(e->C, e->hp.img_size, *p)) return 1;
+    e->has_proc = p != nullptr;
+    e->proc = p ? *p : vitb200_image_proc{};
+    return 0;
+}
+
+int vitb200_set_image_proc(vitb200_engine *e, const vitb200_image_proc *p)
+{
+    return guarded(__func__, [&] { return set_image_proc(e, p); });
+}
+
+int vitb200_get_image_proc(const vitb200_engine *e, vitb200_image_proc *out)
+{
+    return guarded(__func__, [&] {
+        if (!e || !out) return fail("null argument");
+        *out = e->proc;
+        return 0;
+    });
+}
+
 void vitb200_destroy(vitb200_engine *e)
 {
     if (!e) return;
@@ -1714,6 +1783,7 @@ void vitb200_destroy(vitb200_engine *e)
     {
         if (sl.d_u8) cudaFree(sl.d_u8);
         if (sl.h_u8) cudaFreeHost(sl.h_u8);
+        if (sl.d_proc) cudaFree(sl.d_proc);
         if (sl.ev_h2d) cudaEventDestroy(sl.ev_h2d);
         if (sl.ev_done) cudaEventDestroy(sl.ev_done);
     }
@@ -2116,12 +2186,15 @@ static int check_u8_images(const uint8_t *const *images, const int *nx, const in
     return 0;
 }
 
-static int stage_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, size_t &table_off)
+// extra / extra_bytes: a second per-call table (the image processor's ProcGeom rows), copied after the PreImage table at
+// table_off + batch * sizeof(PreImage) in the same host-to-device copy
+static int stage_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, size_t &table_off,
+                    const void *extra = nullptr, size_t extra_bytes = 0)
 {
     size_t total = 0;
     for (int b = 0; b < batch; ++b) total += ((size_t)nx[b] * ny[b] * 3 + 255) / 256 * 256;
     table_off = total;
-    total += (size_t)batch * sizeof(PreImage);
+    total += (size_t)batch * sizeof(PreImage) + extra_bytes;
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t s = e->stream, cs = e->copy_stream;
     // this slot's previous call (two submissions ago) must have consumed its staging buffer before the host overwrites it
@@ -2145,15 +2218,128 @@ static int stage_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, c
         table[b].offset = off; table[b].nx = nx[b]; table[b].ny = ny[b];
         off += (n + 255) / 256 * 256;
     }
+    if (extra_bytes) memcpy(sl.h_u8 + table_off + (size_t)batch * sizeof(PreImage), extra, extra_bytes);
     CUDA_TRY(cudaMemcpyAsync(sl.d_u8, sl.h_u8, total, cudaMemcpyHostToDevice, cs));
     CUDA_TRY(cudaEventRecord(sl.ev_h2d, cs));
     CUDA_TRY(cudaStreamWaitEvent(s, sl.ev_h2d, 0));
     return 0;
 }
 
+// Pillow's precompute_coeffs along one axis of a resize in -> out, on the host: the tap-table width ksize = ceil(support) * 2 + 1 (1 when
+// the axis keeps its size), and the source range [first, end) of output index xx, in the device's operation order (pil_coeffs)
+static double pil_ksize(int64_t in, int64_t out, int resample)
+{
+    if (in == out) return 1.0;
+    const double scale = (double)in / (double)out;
+    return std::ceil((resample == 2 ? 1.0 : 2.0) * (scale < 1.0 ? 1.0 : scale)) * 2.0 + 1.0;
+}
+
+static void pil_range(int64_t in, int64_t out, int64_t xx, int resample, int64_t &first, int64_t &end)
+{
+    if (in == out) { first = xx; end = xx + 1; return; }
+    const double scale = (double)in / (double)out;
+    const double support = (resample == 2 ? 1.0 : 2.0) * (scale < 1.0 ? 1.0 : scale);
+    const double center = ((double)xx + 0.5) * scale;
+    const double lo = center - support + 0.5, hi = center + support + 0.5;
+    first = std::max<int64_t>((int64_t)lo, 0);
+    end = std::min<int64_t>((int64_t)hi, in);
+}
+
+// The geometry of the image processor's two passes for a batch of checked images, worked out on the host in 64-bit integers before
+// anything is enqueued, so that a 1 x 5000 photo (resized to 224 x 1120000) costs what its crop costs
+static int plan_proc(vitb200_engine *e, const int *nx, const int *ny, int batch)
+{
+    const vitb200_image_proc &p = e->proc;
+    const int S = e->hp.img_size;
+    const size_t smem_max = 227 * 1024; // the opt-in shared memory of one H100 CTA
+    ProcPlan &plan = e->proc_plan;
+    plan.geo.resize((size_t)batch);
+    double kh = 1.0, kv = 1.0;
+    plan.max_rows = 1;
+    plan.tmp_total = 0;
+    for (int b = 0; b < batch; ++b)
+    {
+        const int64_t w = nx[b], h = ny[b];
+        int64_t ow = p.width, oh = p.height;
+        if (p.shortest_edge > 0)
+        {
+            const int64_t sh = std::min(w, h), lg = std::max(w, h);
+            const int64_t nl = (int64_t)((double)(p.shortest_edge * lg) / (double)sh);
+            ow = w <= h ? p.shortest_edge : nl;
+            oh = w <= h ? nl : p.shortest_edge;
+        }
+        if (ow > (1 << 30) || oh > (1 << 30))
+            return fail("image %d (%dx%d): resized to %lld x %lld pixels, more than 2^30 along one side", b, nx[b], ny[b], (long long)ow, (long long)oh);
+        const int64_t ch = p.crop_height ? p.crop_height : oh, cw = p.crop_width ? p.crop_width : ow;
+        const int64_t top = (oh - ch) / 2, left = (ow - cw) / 2;
+        int64_t y0, y1, unused;
+        pil_range(h, oh, top, p.resample, y0, unused);
+        pil_range(h, oh, top + S - 1, p.resample, unused, y1);
+        const double kx = pil_ksize(w, ow, p.resample), ky = pil_ksize(h, oh, p.resample);
+        if ((kx + 2.0) * IMG_PROC_H_COLS * sizeof(int) > smem_max || (ky + 2.0) * IMG_PROC_V_ROWS * sizeof(int) > smem_max)
+            return fail("image %d (%dx%d): resizing it to %lld x %lld pixels needs more taps than fit in shared memory", b, nx[b], ny[b],
+                        (long long)ow, (long long)oh);
+        kh = std::max(kh, kx);
+        kv = std::max(kv, ky);
+        ProcGeom &g = plan.geo[(size_t)b];
+        g.tmp = plan.tmp_total;
+        g.ow = (int)ow; g.oh = (int)oh; g.left = (int)left; g.top = (int)top; g.y0 = (int)y0; g.rows = (int)(y1 - y0);
+        plan.max_rows = std::max(plan.max_rows, g.rows);
+        plan.tmp_total += ((size_t)g.rows * S * 3 + 255) / 256 * 256;
+    }
+    plan.kh = (int)kh;
+    plan.kv = (int)kv;
+    return 0;
+}
+
+// The u8 entry points' checks: the images, and with an image processor the bilinear flag and the batch's geometry (plan_proc)
+static int check_u8_call(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear)
+{
+    if (check_u8_images(images, nx, ny, batch)) return 1;
+    if (!e->has_proc) return 0;
+    if (bilinear) return fail("bilinear = %d: the engine's image processor fixes the resample (vitb200_set_image_proc)", bilinear);
+    return plan_proc(e, nx, ny, batch);
+}
+
+// The image processor's two passes (image_proc_h_kernel, image_proc_v_kernel) as plan_proc laid them out
+static int preprocess_proc(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch,
+                           float *images_f32_out)
+{
+    const vitb200_image_proc &p = e->proc;
+    const ProcPlan &plan = e->proc_plan;
+    const int S = e->hp.img_size;
+    size_t table_off = 0;
+    if (stage_u8(e, sl, images, nx, ny, batch, table_off, plan.geo.data(), plan.geo.size() * sizeof(ProcGeom))) return 1;
+    if (plan.tmp_total > sl.proc_cap)
+    {
+        const size_t cap = plan.tmp_total + plan.tmp_total / 4;
+        if (sl.d_proc) cudaFree(sl.d_proc);
+        sl.d_proc = nullptr; sl.proc_cap = 0;
+        CUDA_TRY(cudaMalloc((void **)&sl.d_proc, cap));
+        sl.proc_cap = cap;
+    }
+    const PreImage *d_imgs = reinterpret_cast<const PreImage *>(sl.d_u8 + table_off);
+    const ProcGeom *d_geo = reinterpret_cast<const ProcGeom *>(sl.d_u8 + table_off + (size_t)batch * sizeof(PreImage));
+    cudaStream_t s = e->stream;
+    float *d_f32 = images_f32_out ? sl.img : nullptr;
+    const ProcNorm nm{p.rescale_factor, {p.mean[0], p.mean[1], p.mean[2]}, {p.std[0], p.std[1], p.std[2]}};
+    const int KH = plan.kh, KV = plan.kv, max_rows = plan.max_rows;
+    if (launch(e, image_proc_h_kernel, dim3((unsigned)((S + IMG_PROC_H_COLS - 1) / IMG_PROC_H_COLS),
+                                            (unsigned)((max_rows + IMG_PROC_H_ROWS - 1) / IMG_PROC_H_ROWS), (unsigned)batch),
+               dim3(256), (size_t)(KH + 2) * IMG_PROC_H_COLS * sizeof(int), s, LAUNCH_PLAIN, sl.d_u8, d_imgs, d_geo, sl.d_proc, S,
+               (int)p.resample, KH) ||
+        launch(e, image_proc_v_kernel, dim3((unsigned)((S + IMG_PROC_V_ROWS - 1) / IMG_PROC_V_ROWS), (unsigned)batch), dim3(256),
+               (size_t)(KV + 2) * IMG_PROC_V_ROWS * sizeof(int), s, LAUNCH_PDL, (const uint8_t *)sl.d_proc, d_imgs, d_geo, d_f32, S,
+               (int)p.resample, KV, nm, e->PA, e->hp.patch_size, e->KPp))
+        return 1;
+    if (images_f32_out) CUDA_TRY(cudaMemcpyAsync(images_f32_out, d_f32, (size_t)batch * 3 * S * S * sizeof(float), cudaMemcpyDeviceToHost, s));
+    return 0;
+}
+
 static int preprocess_u8(vitb200_engine *e, Slot &sl, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                          float *images_f32_out)
 {
+    if (e->has_proc) return preprocess_proc(e, sl, images, nx, ny, batch, images_f32_out);
     size_t table_off = 0;
     if (stage_u8(e, sl, images, nx, ny, batch, table_off)) return 1;
     cudaStream_t s = e->stream;
@@ -2172,7 +2358,7 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
 {
     if (!e || !images || !nx || !ny) return fail("null argument");
     if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-    if (check_batch(e, batch) || check_k(e, k) || check_u8_images(images, nx, ny, batch)) return 1;
+    if (check_batch(e, batch) || check_k(e, k) || check_u8_call(e, images, nx, ny, batch, bilinear)) return 1;
     Slot &sl = begin_submit(e);
     if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, images_f32_out)) return 1;
     if ((probs || logits || (k > 0 && (topk_idx || topk_prob))) && classify_to_host(e, sl, nullptr, batch, probs, logits, topk_idx, topk_prob, k, nullptr))
@@ -2202,7 +2388,7 @@ int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const i
         if (check_features(e, images, batch, req, tokens, prelogits)) return 1;
         if (!nx || !ny) return fail("vitb200_features_u8: null argument");
         if (e->C != 3) return fail("vitb200_features_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
-        if (check_u8_images(images, nx, ny, batch)) return 1;
+        if (check_u8_call(e, images, nx, ny, batch, bilinear)) return 1;
         Slot &sl = begin_submit(e);
         if (preprocess_u8(e, sl, images, nx, ny, batch, bilinear, nullptr) || features_to_host(e, nullptr, batch, req, tokens, prelogits) ||
             end_submit(e, sl))
@@ -2486,7 +2672,18 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
         ts[i].n_dims = g.tensors[i].n_dims;
         for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
     }
-    return create_impl(&hp, &arch, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out, &g.labels);
+    const vitb200_image_proc proc{i32(g.ip_shortest_edge), i32(g.ip_height), i32(g.ip_width), i32(g.ip_crop_height), i32(g.ip_crop_width),
+                                  i32(g.ip_resample), g.ip_rescale_factor, {g.ip_mean[0], g.ip_mean[1], g.ip_mean[2]},
+                                  {g.ip_std[0], g.ip_std[1], g.ip_std[2]}};
+    if (g.has_image_proc)
+    {
+        // the input channels as create_impl takes them, from the patch kernel [P, P, C, D] (a file without one fails there)
+        const vitb200_tensor *pw = find_tensor(ts.data(), (int)ts.size(), "patch_embed.proj.weight");
+        if (check_image_proc(pw ? (int)dim_of(pw, 2) : 3, hp.img_size, proc))
+            return fail("invalid model file '%s' (vit.%s)", path, std::string(g_err).c_str());
+    }
+    if (create_impl(&hp, &arch, ts.data(), (int)ts.size(), device, max_batch, head_tokens, fp8, out, &g.labels)) return 1;
+    return g.has_image_proc ? set_image_proc(*out, &proc) : 0;
 }
 
 extern "C" int vitb200_create_from_file(const char *path, int device, int max_batch, vitb200_engine **out)

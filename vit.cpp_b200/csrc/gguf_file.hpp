@@ -13,6 +13,8 @@
 //     vit.reg_tokens (integer, default 0: register tokens 'reg_token' after the class token)
 //     vit.pool (string, default "token"; "cls_patch_mean": the head reads the class token || the mean of the patch tokens; "map" or
 //              "mean": SigLIP, no class token, the head reads the attention-pooling head's output or the mean of the tokens)
+//     vit.image_proc.shortest_edge, .height, .width, .crop_height, .crop_width, .resample (integers), .rescale_factor (float64),
+//     vit.image_proc.image_mean, .image_std (arrays of 3 float32): Hugging Face's image preprocessing (vitb200_image_proc), optional
 // Layout (gguf.md): header {magic "GGUF", u32 version, u64 n_tensors, u64 n_kv}, n_kv x {string key, u32 type, value},
 // n_tensors x {string name, u32 n_dims, u64 ne[n_dims], u32 type, u64 offset}, padding to the alignment, tensor data (offsets
 // relative to the start of the data section).  Strings are {u64 length, bytes}.
@@ -41,6 +43,12 @@ struct GgufModel
     int32_t activation = 0; // vit.activation: 0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh, 4 swiglu (vitb200_arch.activation)
     int64_t layer_scale = 0, reg_tokens = 0; // vit.layer_scale, vit.reg_tokens (vitb200_arch; the loader checks the ranges)
     int32_t pool = 0;       // vit.pool: 0 token, 1 cls_patch_mean, 2 map, 3 mean (vitb200_arch.pool)
+    // vit.image_proc.* (vitb200_image_proc; the loader checks the values): has_image_proc once any of the keys is present.  A missing
+    // key keeps a value the checks refuse (resample 0, rescale_factor 0, a mean or std without 3 values)
+    bool has_image_proc = false;
+    int64_t ip_shortest_edge = 0, ip_height = 0, ip_width = 0, ip_crop_height = 0, ip_crop_width = 0, ip_resample = 0;
+    double ip_rescale_factor = 0.0;
+    float ip_mean[3] = {0, 0, 0}, ip_std[3] = {0, 0, 0};
     std::map<int, std::string> labels;
     std::vector<GgufTensor> tensors;
     std::string error;
@@ -119,6 +127,15 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             uint32_t et = 0;
             uint64_t cnt = 0;
             if (!rd(&et, 4) || !rd(&cnt, 8) || et > 12 || et == 9) return fail("corrupt GGUF array");
+            float *f3 = key == "vit.image_proc.image_mean" ? m.ip_mean : key == "vit.image_proc.image_std" ? m.ip_std : nullptr;
+            if (f3)
+            {
+                if (et != 6 || cnt != 3) return fail(key + " must be an array of 3 float32");
+                if (!rd(f3, 12)) return fail("truncated GGUF array");
+                m.has_image_proc = true;
+                continue;
+            }
+            if (key.compare(0, 15, "vit.image_proc.") == 0) return fail("unknown key " + key);
             for (uint64_t j = 0; j < cnt; ++j)
             {
                 if (et == 8)
@@ -167,6 +184,17 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             else if (key == "vit.pre_norm") m.pre_norm = iv;
             else if (key == "vit.layer_scale") m.layer_scale = iv;
             else if (key == "vit.reg_tokens") m.reg_tokens = iv;
+            else if (key.compare(0, 15, "vit.image_proc.") == 0)
+            {
+                const std::string f = key.substr(15);
+                int64_t *dst = f == "shortest_edge" ? &m.ip_shortest_edge : f == "height" ? &m.ip_height : f == "width" ? &m.ip_width
+                             : f == "crop_height" ? &m.ip_crop_height : f == "crop_width" ? &m.ip_crop_width : f == "resample" ? &m.ip_resample
+                             : nullptr;
+                if (dst) *dst = iv;
+                else if (f == "rescale_factor") m.ip_rescale_factor = fv;
+                else return fail("unknown key " + key);
+                m.has_image_proc = true;
+            }
         }
     }
     if (!arch.empty() && arch != "vit") return fail("GGUF architecture is '" + arch + "', expected 'vit'");

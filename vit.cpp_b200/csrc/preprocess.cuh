@@ -109,6 +109,166 @@ __global__ void preprocess_kernel(const uint8_t *__restrict__ staging, const Pre
     }
 }
 
+// ---- Hugging Face's PIL image processors (vitb200_image_proc; CLIPImageProcessor, SiglipImageProcessor, BitImageProcessor with the
+// PIL backend): Pillow's 8-bit ImagingResample (bicubic a = -0.5 or bilinear, anti-aliased when downscaling) to the resized size, HF's
+// centre crop, x = f32(f64(v) * rescale_factor), y = (x - mean_c) / std_c in f32.  Two kernels, only over the crop window (an output
+// pixel depends on its own taps alone, so this gives Pillow's bits for the whole image cropped afterwards):
+//   image_proc_h_kernel  the horizontal pass: the crop's S columns of the source rows the vertical taps reach, rounded to u8, into a
+//                        per-slot scratch [rows][S][3];
+//   image_proc_v_kernel  the vertical pass over that scratch, rounded to u8, then rescale and normalise, written like preprocess_kernel.
+// Pillow runs the horizontal pass first and rounds in between, so the order is fixed.  It skips a pass whose axis keeps its size; here
+// such a pass is one tap of weight 1 << 22, the identity, which is what Pillow's coefficients would be too.
+// Coefficients are Pillow's precompute_coeffs + normalize_coeffs_8bpc in double, operation for operation with explicit roundings: a
+// contracted multiply-add moves a coefficient, and one coefficient moves a pixel by a level.  Each CTA computes the ones it needs into
+// shared memory, laid out [tap][row or column] so that the threads of a warp read different banks.
+constexpr int PIL_PRECISION_BITS = 22;   // Pillow's 32 - 8 - 2
+constexpr int IMG_PROC_H_COLS = 32;      // output columns per CTA of the horizontal pass (one per lane)
+constexpr int IMG_PROC_H_ROWS = 64;      // source rows per CTA of the horizontal pass (8 warps, 8 rows each)
+constexpr int IMG_PROC_V_ROWS = 8;       // output rows per CTA of the vertical pass
+
+// Per image, computed on the host in 64-bit integers: the resized size, the crop's offset in it, and the source rows the horizontal
+// pass writes (y0 .. y0 + rows - 1) at byte offset tmp of the scratch
+struct ProcGeom
+{
+    size_t tmp;
+    int ow, oh, left, top, y0, rows;
+};
+
+struct ProcNorm
+{
+    double rescale;
+    float mean[3], std_[3];
+};
+
+__device__ __forceinline__ double pil_filter(double x, int resample)
+{
+    x = fabs(x);
+    if (resample == 2) return x < 1.0 ? __dsub_rn(1.0, x) : 0.0; // bilinear_filter
+    // bicubic_filter, a = -0.5: ((a + 2) x - (a + 3)) x x + 1 and (((x - 5) x + 8) x - 4) a
+    if (x < 1.0) return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(1.5, x), 2.5), x), x), 1.0);
+    if (x < 2.0) return __dmul_rn(__dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(x, 5.0), x), 8.0), x), 4.0), -0.5);
+    return 0.0;
+}
+
+// Fixed-point taps of output index xx of a resize in -> out along one axis, into k[t * stride] (t < K); *first = the first source index,
+// *n = the tap count.  in == out: the identity tap.
+__device__ void pil_coeffs(int in, int out, int xx, int resample, int K, int *k, int stride, int *first, int *n)
+{
+    if (in == out)
+    {
+        *first = xx; *n = 1; k[0] = 1 << PIL_PRECISION_BITS;
+        return;
+    }
+    const double scale = __ddiv_rn((double)in, (double)out);
+    const double filterscale = scale < 1.0 ? 1.0 : scale;
+    const double support = __dmul_rn(resample == 2 ? 1.0 : 2.0, filterscale);
+    const double ss = __ddiv_rn(1.0, filterscale);
+    const double center = __dmul_rn(__dadd_rn((double)xx, 0.5), scale);
+    int xmin = (int)__dadd_rn(__dsub_rn(center, support), 0.5);
+    if (xmin < 0) xmin = 0;
+    int xmax = (int)__dadd_rn(__dadd_rn(center, support), 0.5);
+    if (xmax > in) xmax = in;
+    xmax -= xmin;
+    if (xmax > K) xmax = K; // cannot happen: K = ceil(support) * 2 + 1 bounds Pillow's tap count
+    double ww = 0.0;
+    for (int x = 0; x < xmax; ++x) ww = __dadd_rn(ww, pil_filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss), resample));
+    for (int x = 0; x < xmax; ++x)
+    {
+        double w = pil_filter(__dmul_rn(__dadd_rn(__dsub_rn((double)(x + xmin), center), 0.5), ss), resample);
+        if (ww != 0.0) w = __ddiv_rn(w, ww);
+        const double f = __dmul_rn(w, (double)(1 << PIL_PRECISION_BITS));
+        k[x * stride] = w < 0 ? (int)__dadd_rn(-0.5, f) : (int)__dadd_rn(0.5, f);
+    }
+    *first = xmin; *n = xmax;
+}
+
+__device__ __forceinline__ uint8_t pil_clip8(int v) { return (uint8_t)(v <= 0 ? 0 : (v >> PIL_PRECISION_BITS > 255 ? 255 : v >> PIL_PRECISION_BITS)); }
+
+// grid (ceil(S / 32), ceil(max rows / 64), batch), 256 threads; dynamic shared memory 32 * (K + 2) ints
+__global__ void image_proc_h_kernel(const uint8_t *__restrict__ staging, const PreImage *__restrict__ imgs, const ProcGeom *__restrict__ geo,
+                                    uint8_t *__restrict__ tmp, int S, int resample, int K)
+{
+    extern __shared__ int pil_k[]; // [K][32] taps, then first[32], n[32]
+    const int b = blockIdx.z;
+    const ProcGeom g = geo[b];
+    const int r0 = blockIdx.y * IMG_PROC_H_ROWS;
+    if (r0 >= g.rows) return;
+    const PreImage im = imgs[b];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int j = blockIdx.x * IMG_PROC_H_COLS + lane;
+    int *first = pil_k + K * IMG_PROC_H_COLS, *count = first + IMG_PROC_H_COLS;
+    if (warp == 0 && j < S) pil_coeffs(im.nx, g.ow, g.left + j, resample, K, pil_k + lane, IMG_PROC_H_COLS, first + lane, count + lane);
+    __syncthreads();
+    if (j >= S) return;
+    const int x0 = first[lane], n = count[lane];
+    const int r1 = min(r0 + IMG_PROC_H_ROWS, g.rows);
+    for (int r = r0 + warp; r < r1; r += 8)
+    {
+        const uint8_t *src = staging + im.offset + ((size_t)(g.y0 + r) * im.nx + x0) * 3;
+        int s0 = 1 << (PIL_PRECISION_BITS - 1), s1 = s0, s2 = s0;
+        for (int t = 0; t < n; ++t)
+        {
+            const int k = pil_k[t * IMG_PROC_H_COLS + lane];
+            s0 += (int)src[3 * t] * k; s1 += (int)src[3 * t + 1] * k; s2 += (int)src[3 * t + 2] * k;
+        }
+        uint8_t *o = tmp + g.tmp + ((size_t)r * S + j) * 3;
+        o[0] = pil_clip8(s0); o[1] = pil_clip8(s1); o[2] = pil_clip8(s2);
+    }
+}
+
+// grid (ceil(S / 8), batch), 256 threads; dynamic shared memory 8 * (K + 2) ints.  Launched programmatically: the taps are computed
+// while the horizontal pass finishes, the scratch is read after griddepcontrol.wait.  out / patches as preprocess_kernel.
+__global__ void image_proc_v_kernel(const uint8_t *__restrict__ tmp, const PreImage *__restrict__ imgs, const ProcGeom *__restrict__ geo,
+                                    float *__restrict__ out, int S, int resample, int K, ProcNorm nm, __half *__restrict__ patches, int P, int ldk)
+{
+    extern __shared__ int pil_k[]; // [K][8] taps, then first[8], n[8]
+    const int b = blockIdx.y;
+    const ProcGeom g = geo[b];
+    const PreImage im = imgs[b];
+    const int i0 = blockIdx.x * IMG_PROC_V_ROWS;
+    int *first = pil_k + K * IMG_PROC_V_ROWS, *count = first + IMG_PROC_V_ROWS;
+    if (threadIdx.x < IMG_PROC_V_ROWS && i0 + (int)threadIdx.x < S)
+        pil_coeffs(im.ny, g.oh, g.top + i0 + threadIdx.x, resample, K, pil_k + threadIdx.x, IMG_PROC_V_ROWS, first + threadIdx.x,
+                   count + threadIdx.x);
+    __syncthreads();
+    ptx::grid_dep_wait();
+    const int G = S / P;
+    for (int p = threadIdx.x; p < IMG_PROC_V_ROWS * S; p += blockDim.x)
+    {
+        const int il = p / S, j = p - il * S, i = i0 + il;
+        if (i >= S) break;
+        const int n = count[il];
+        const int y = min(max(first[il] - g.y0, 0), g.rows - n); // always first - y0; clamped so the reads stay in the scratch
+        const uint8_t *src = tmp + g.tmp + ((size_t)y * S + j) * 3;
+        int s[3] = {1 << (PIL_PRECISION_BITS - 1), 1 << (PIL_PRECISION_BITS - 1), 1 << (PIL_PRECISION_BITS - 1)};
+        for (int t = 0; t < n; ++t)
+        {
+            const int k = pil_k[t * IMG_PROC_V_ROWS + il];
+            const uint8_t *q = src + (size_t)t * S * 3;
+            s[0] += (int)q[0] * k; s[1] += (int)q[1] * k; s[2] += (int)q[2] * k;
+        }
+        float px3[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+        {
+            const float x = (float)__dmul_rn((double)pil_clip8(s[c]), nm.rescale);
+            px3[c] = __fdiv_rn(__fsub_rn(x, nm.mean[c]), nm.std_[c]);
+        }
+        if (out)
+        {
+            float *o = out + ((size_t)b * S * S + (size_t)i * S + j) * 3;
+            o[0] = px3[0]; o[1] = px3[1]; o[2] = px3[2];
+        }
+        if (patches)
+        {
+            const int py = i / P, ky = i - py * P, pxi = j / P, kx = j - pxi * P;
+            __half *row = patches + ((size_t)b * G * G + (size_t)py * G + pxi) * ldk + ky * P + kx;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) row[c * P * P] = __float2half_rn(px3[c]);
+        }
+    }
+}
+
 // ---- The ViTSTR extension's vit_image_preprocess (reference extensions/vitstr.cpp:128-201): u8 RGB -> grayscale -> bilinear resize
 // to img_size^2 -> (v / 255 - 0.5) * 2, 1 channel, no rounding to u8 in between.  Operation for operation as the extension's build
 // (gcc -O3 -mavx2 -mfma, -std=gnu++11 so contraction is on) computes it, read off its disassembly:

@@ -17,6 +17,7 @@ from typing import Optional
 import numpy as np
 
 from .ggml_file import ARCH_ACTIVATIONS, PATCH_ONLY_POOLS, POOLS  # vitb200_arch.activation / .pool -> name (GGUF vit.activation / vit.pool)
+from .ggml_file import IMAGE_PROC_FIELDS, image_proc_from_config
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
@@ -39,6 +40,12 @@ class Arch(C.Structure):
     activation) is a CLIP tower."""
     _fields_ = [("pre_norm", C.c_int32), ("activation", C.c_int32), ("layer_scale", C.c_int32), ("reg_tokens", C.c_int32),
                 ("pool", C.c_int32)]
+
+
+class ImageProc(C.Structure):
+    """vitb200_image_proc (include/vitb200.h): Hugging Face's image preprocessing for the u8 entry points."""
+    _fields_ = [(n, C.c_int32) for n in IMAGE_PROC_FIELDS[:6]] + [("rescale_factor", C.c_double), ("mean", C.c_float * 3),
+                                                                   ("std", C.c_float * 3)]
 
 
 class Taps(C.Structure):
@@ -84,6 +91,8 @@ def lib():
         L.vitb200_mlp_dim.argtypes = [vp]
         L.vitb200_create_arch.argtypes = [vp, C.POINTER(Arch), vp, i32, i32, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_get_arch.argtypes = [vp, C.POINTER(Arch)]
+        L.vitb200_set_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
+        L.vitb200_get_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
         L.vitb200_test_gemm_fp8.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
         L.vitb200_test_layernorm_fp8.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
@@ -155,6 +164,29 @@ class VitModel:
             self.n_tokens -= 1
         self._labels = None
 
+    @property
+    def image_proc(self) -> Optional[dict]:
+        """The image processor the u8 entry points use (vitb200_get_image_proc), as a dict of ggml_file.IMAGE_PROC_FIELDS; None for
+        vit.cpp's preprocessing."""
+        p = ImageProc()
+        _check(lib().vitb200_get_image_proc(self._h, C.byref(p)), "vitb200_get_image_proc")
+        if p.resample == 0:
+            return None
+        d = {n: getattr(p, n) for n in IMAGE_PROC_FIELDS[:7]}
+        d["mean"], d["std"] = list(p.mean), list(p.std)
+        return d
+
+    def set_image_proc(self, config: Optional[dict]):
+        """Give the u8 entry points Hugging Face's preprocessing (vitb200_set_image_proc): `config` is a preprocessor_config.json dict
+        (ggml_file.image_proc_from_config) or a dict like image_proc returns; None restores vit.cpp's preprocessing."""
+        if config is None:
+            _check(lib().vitb200_set_image_proc(self._h, None), "vitb200_set_image_proc")
+            return
+        d = image_proc_from_config(config, self.img_size)
+        p = ImageProc(*[int(d[n]) for n in IMAGE_PROC_FIELDS[:6]], float(d["rescale_factor"]), (C.c_float * 3)(*d["mean"]),
+                      (C.c_float * 3)(*d["std"]))
+        _check(lib().vitb200_set_image_proc(self._h, C.byref(p)), "vitb200_set_image_proc")
+
     def label(self, i: int) -> Optional[str]:
         s = lib().vitb200_label(self._h, i)
         return s.decode() if s else None
@@ -194,11 +226,13 @@ def vit_model_load(fname: str, device: int = 0, max_batch: int = 256, head_token
     return VitModel(h, device, max_batch)
 
 
-def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens: int = 1, edit=None, fp8: bool = False) -> VitModel:
+def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens: int = 1, edit=None, fp8: bool = False,
+                           image_proc: Optional[dict] = None) -> VitModel:
     """vitb200_create_arch with a caller-built tensor list -- what the vit.h-side shim does with vit_model::tensors.  `vf` is a parsed
     model file (ggml_file.VitFile: numpy-shaped f32 / f16 arrays, its eps, pre_norm and activation); `edit(entries)` may reorder /
     duplicate / reshape the list of [name, array, ggml_type, ne] entries first (tests of the loader's shape and name checks).
-    fp8 = True: the FP8 engine (vitb200_create_fp8).  A reference-architecture file gives what vitb200_create_ex gives."""
+    fp8 = True: the FP8 engine (vitb200_create_fp8).  A reference-architecture file gives what vitb200_create_ex gives.  image_proc: a
+    preprocessor_config.json dict (VitModel.set_image_proc); default: the file's own (vf.image_proc), if any."""
     entries = []
     for name, arr in vf.tensors.items():
         if name.endswith(".q8_0_raw"):
@@ -227,7 +261,11 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
     h = C.c_void_p()
     _check(lib().vitb200_create_arch(C.byref(hp), C.byref(arch), ts, len(entries), device, max_batch, head_tokens, int(fp8), C.byref(h)),
            "vitb200_create")
-    return VitModel(h, device, max_batch)
+    model = VitModel(h, device, max_batch)
+    image_proc = image_proc if image_proc is not None else getattr(vf, "image_proc", None)
+    if image_proc is not None:
+        model.set_image_proc(image_proc)
+    return model
 
 
 def vit_predict(model: VitModel, images: np.ndarray, topk: int = 5, want_logits: bool = False):
@@ -295,7 +333,8 @@ def sync_all(models):
 
 
 def vit_image_preprocess_predict(model: VitModel, images_u8, bilinear: bool = False, topk: int = 5, predict: bool = True):
-    """reference vit_image_preprocess (vit.cpp:289) + vit_predict on the GPU for a list of HxWx3 uint8 RGB arrays of any size.
+    """reference vit_image_preprocess (vit.cpp:289) + vit_predict on the GPU for a list of HxWx3 uint8 RGB arrays of any size, or the
+    model's Hugging Face image processor when it has one (model.image_proc; then image_f32 is HF's pixel_values in HWC order).
     Returns (image_f32 batch [B,S,S,3], probs, topk_idx, topk_prob, logits); the last four are None if predict is False."""
     _, B, ptrs, nx, ny = _u8_batch(images_u8)
     S = model.img_size
@@ -385,7 +424,8 @@ def vit_features(model: VitModel, images: np.ndarray, layers=None, norm: bool = 
 
 def vit_features_u8(model: VitModel, images_u8, bilinear: bool = False, layers=None, norm: bool = True, tokens: bool = True,
                     prelogits: bool = False, dtype=np.float32):
-    """vit_features of HxWx3 uint8 RGB images of any size, pre-processed on the GPU like vit_image_preprocess_predict."""
+    """vit_features of HxWx3 uint8 RGB images of any size, pre-processed on the GPU like vit_image_preprocess_predict (through the
+    model's image processor when it has one)."""
     _, B, ptrs, nx, ny = _u8_batch(images_u8)
     return _features_call(model, B, layers, norm, tokens, prelogits, dtype, lambda req, t, p: _check(
         lib().vitb200_features_u8(model.handle, ptrs, nx, ny, B, int(bilinear), req, t, p), "vit_features_u8"))

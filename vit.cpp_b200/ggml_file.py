@@ -19,7 +19,7 @@ from __future__ import annotations
 
 import struct
 from dataclasses import dataclass, field
-from typing import Dict, Tuple
+from typing import Dict, Optional, Tuple
 
 import numpy as np
 
@@ -88,11 +88,75 @@ class VitFile:
     layer_scale: int = 0         # 1: LayerScale 'blocks.{i}.ls1.gamma' / 'ls2.gamma' on the attention and MLP branches
     reg_tokens: int = 0          # register tokens 'reg_token' [1, R, D], rows 1 .. R of every image
     pool: str = "token"          # head input: one of POOLS
+    # Hugging Face image preprocessing for the u8 entry points (GGUF keys vit.image_proc.*): a dict with the IMAGE_PROC_FIELDS, or None
+    image_proc: Optional[dict] = None
 
     @property
     def n_tokens(self) -> int:
         g = self.img_size // self.patch_size
         return g * g if self.pool in PATCH_ONLY_POOLS else g * g + 1 + self.reg_tokens
+
+
+# vitb200_image_proc (include/vitb200.h), field by field; each is also the GGUF key vit.image_proc.<field> ('mean' and 'std' are stored
+# as vit.image_proc.image_mean / image_std, as preprocessor_config.json names them)
+IMAGE_PROC_FIELDS = ("shortest_edge", "height", "width", "crop_height", "crop_width", "resample", "rescale_factor", "mean", "std")
+PIL_BILINEAR, PIL_BICUBIC = 2, 3  # PIL.Image.Resampling ids, as preprocessor_config.json stores them
+
+
+def image_proc_from_config(config: dict, img_size: int) -> dict:
+    """A Hugging Face preprocessor_config.json dict (CLIPImageProcessor, SiglipImageProcessor, BitImageProcessor, or their to_dict())
+    -> the vitb200_image_proc fields of a model of input size img_size.  A dict that already holds exactly IMAGE_PROC_FIELDS is taken as
+    it is.  An integer size is a shortest edge and an integer crop_size a square, as CLIP and Bit read them.  Refused, naming the field:
+    do_resize false, a size with longest_edge or max_size, a resample other than 2 or 3, do_pad, a crop larger than the resize and a
+    final size other than img_size."""
+    if set(config) == set(IMAGE_PROC_FIELDS):
+        return {k: config[k] for k in IMAGE_PROC_FIELDS}
+    if not config.get("do_resize", True):
+        raise ValueError("preprocessor config: do_resize false is not supported (the engine needs img_size x img_size pixels)")
+    if config.get("do_pad"):
+        raise ValueError("preprocessor config: do_pad is not supported")
+    size = config.get("size")
+    if isinstance(size, int):
+        size = {"shortest_edge": size}
+    if not isinstance(size, dict):
+        raise ValueError(f"preprocessor config: size {size!r} is not supported (shortest_edge, or height and width)")
+    for k in ("longest_edge", "max_size"):
+        if size.get(k) is not None:
+            raise ValueError(f"preprocessor config: size.{k} is not supported")
+    if config.get("max_size") is not None:
+        raise ValueError("preprocessor config: max_size is not supported")
+    se = int(size.get("shortest_edge") or 0)
+    h, w = (0, 0) if se else (int(size.get("height") or 0), int(size.get("width") or 0))
+    if se <= 0 and (h <= 0 or w <= 0):
+        raise ValueError(f"preprocessor config: size {size!r} is not supported (shortest_edge, or height and width)")
+    ch = cw = 0
+    if config.get("do_center_crop"):
+        crop = config.get("crop_size")
+        if isinstance(crop, int):
+            crop = {"height": crop, "width": crop}
+        if not isinstance(crop, dict) or not crop.get("height") or not crop.get("width"):
+            raise ValueError(f"preprocessor config: crop_size {crop!r} is not supported (height and width)")
+        ch, cw = int(crop["height"]), int(crop["width"])
+        rh, rw = (se, se) if se else (h, w)
+        if ch > rh or cw > rw:
+            raise ValueError(f"preprocessor config: crop_size {ch} x {cw} is larger than the resize {rh} x {rw} (padding is not supported)")
+    elif se:
+        raise ValueError("preprocessor config: size.shortest_edge without do_center_crop: the output size would depend on the image")
+    resample = int(config.get("resample", PIL_BICUBIC))
+    if resample not in (PIL_BILINEAR, PIL_BICUBIC):
+        raise ValueError(f"preprocessor config: resample {resample} is not supported (2 BILINEAR or 3 BICUBIC)")
+    fh, fw = (ch, cw) if ch else (h, w)
+    if (fh, fw) != (img_size, img_size):
+        raise ValueError(f"preprocessor config: the final size {fh} x {fw} ({'crop_size' if ch else 'size'}) is not the model's "
+                         f"img_size {img_size} x {img_size}")
+    norm = config.get("do_normalize", True)
+    mean = [float(x) for x in config.get("image_mean", ())] if norm else [0.0] * 3
+    std = [float(x) for x in config.get("image_std", ())] if norm else [1.0] * 3
+    if len(mean) != 3 or len(std) != 3:
+        raise ValueError("preprocessor config: image_mean and image_std need 3 values each")
+    return {"shortest_edge": se, "height": h, "width": w, "crop_height": ch, "crop_width": cw, "resample": resample,
+            "rescale_factor": float(config.get("rescale_factor", 1 / 255)) if config.get("do_rescale", True) else 1.0,
+            "mean": mean, "std": std}
 
 
 def tensor_specs(hidden: int, layers: int, classes: int, patch: int, img: int, in_chans: int = 3):
@@ -303,7 +367,7 @@ def synthetic_images(batch: int, img_size: int, seed: int = 1234) -> np.ndarray:
 # True GGUF (v3) container -- the SURVEY.md 8(f) rank-3 extension read by csrc/gguf_file.hpp (key names documented there).
 GGUF_MAGIC = b"GGUF"
 GGML_TYPE_BF16 = 30  # current ggml; the reference's pinned ggml has no bf16 type
-_GGUF_U32, _GGUF_F32, _GGUF_STR, _GGUF_ARR = 4, 6, 8, 9
+_GGUF_U32, _GGUF_I32, _GGUF_F32, _GGUF_STR, _GGUF_ARR, _GGUF_F64 = 4, 5, 6, 8, 9, 12
 
 
 def f32_to_bf16_bits(x: np.ndarray) -> np.ndarray:
@@ -349,6 +413,15 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
         if vf.pool not in POOLS:
             raise ValueError(f"write_gguf: unknown pool {vf.pool!r} ({', '.join(POOLS)})")
         kv.append(gstr(b"vit.pool") + struct.pack("<I", _GGUF_STR) + gstr(vf.pool.encode()))
+    if vf.image_proc is not None:
+        ip = vf.image_proc
+        for k in IMAGE_PROC_FIELDS[:6]:  # int32: the loader refuses a negative size by name
+            kv.append(gstr(("vit.image_proc." + k).encode()) + struct.pack("<Ii", _GGUF_I32, int(ip[k])))
+        kv.append(gstr(b"vit.image_proc.rescale_factor") + struct.pack("<Id", _GGUF_F64, float(ip["rescale_factor"])))
+        for k, key in (("mean", b"vit.image_proc.image_mean"), ("std", b"vit.image_proc.image_std")):
+            if len(ip[k]) != 3:
+                raise ValueError(f"write_gguf: image_proc {k} needs 3 values, not {len(ip[k])}")
+            kv.append(gstr(key) + struct.pack("<IIQ", _GGUF_ARR, _GGUF_F32, 3) + np.asarray(ip[k], "<f4").tobytes())
     if vf.id2label:
         labels = [vf.id2label.get(i, "").encode() for i in range(max(vf.id2label) + 1)]
         kv.append(gstr(b"vit.id2label") + struct.pack("<IIQ", _GGUF_ARR, _GGUF_STR, len(labels)) + b"".join(gstr(x) for x in labels))
@@ -426,6 +499,10 @@ def read_gguf(path: str) -> VitFile:
     vf.layer_scale = int(kv.get("vit.layer_scale", 0))
     vf.reg_tokens = int(kv.get("vit.reg_tokens", 0))
     vf.pool = kv.get("vit.pool", "token")
+    if any(k.startswith("vit.image_proc.") for k in kv):
+        vf.image_proc = {k: kv.get("vit.image_proc." + k, 0) for k in IMAGE_PROC_FIELDS[:7]}
+        vf.image_proc["mean"] = list(kv.get("vit.image_proc.image_mean", []))
+        vf.image_proc["std"] = list(kv.get("vit.image_proc.image_std", []))
     align = kv.get("general.alignment", 32)
     infos = []
     for _ in range(n_tensors):
