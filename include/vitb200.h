@@ -294,6 +294,58 @@ int vitb200_features_device(vitb200_engine *e, const float *d_images, int batch,
 int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const int *nx, const int *ny, int batch, int bilinear,
                         const vitb200_features_req *req, void *tokens, void *prelogits);
 
+/* ---- text towers: CLIP and SigLIP (no reference counterpart) --------------------------------------------------------------------
+ * The text half of CLIP (HF CLIPTextModel, CLIPTextModelWithProjection, the text tower of CLIPModel) and SigLIP (SiglipTextModel, the text
+ * tower of SiglipModel): the same pre-LN blocks as the image towers, fed with token ids.  Tokenisation is the caller's job (Hugging Face
+ * tokenizers): its vocabulary files, normalisation and BPE merges are host-side string work that each model family defines its own way,
+ * and the ids are all the GPU needs.
+ * hp: hidden_size, num_hidden_layers, num_attention_heads, eps and ftype as for images; num_classes = E, the projection width (the head's
+ * rows); patch_size and img_size must be 0.  Tensors: 'token_embd.weight' [V][D] (any weight format, stored f16), 'pos_embed' [1][N][D] f32,
+ * 'blocks.*' as for images, 'norm.*' (the final LayerNorm), 'head.weight' [E][D] and 'head.bias' [E] (zeros for CLIP's projection; the
+ * identity for CLIPTextModel).  The image checks apply (head dim 64, D <= 2048, MLP 4 D, unique names, shapes); context must equal the
+ * 'pos_embed' rows and be at most 224 and V >= 1.  Anything else fails before the device is touched, naming the limit.
+ * A GGUF file is a text tower when it has the key vit.text.context_length; it then carries vit.text.causal (bool or integer),
+ * vit.text.pool ("eos", "eos_argmax" or "last"; any other string fails the load), vit.text.eos_token_id (integer) and optionally
+ * vit.text.logit_scale / vit.text.logit_bias (float32), must not carry vit.patch_size, vit.image_size, vit.pre_norm, vit.layer_scale,
+ * vit.reg_tokens, vit.pool or vit.image_proc.*, refuses unknown vit.text.* keys, and holds 12 L + 6 tensors.  vitb200_create_from_file and
+ * vitb200_create_from_file_fp8 (head_tokens 1) create a text engine from it. */
+typedef struct vitb200_text_arch
+{
+    int32_t context;      /* N tokens per sequence = 'pos_embed' rows, 1..224 */
+    int32_t causal;       /* 1 CLIP's causal mask (query t sees keys 0..t), 0 bidirectional (SigLIP) */
+    int32_t pool;         /* 0 "eos": the first position whose id == eos_token_id, row 0 if there is none;
+                           * 1 "eos_argmax": the first position of the largest id (HF CLIP configs with eos_token_id == 2);
+                           * 2 "last": row N - 1 (SigLIP) */
+    int32_t eos_token_id; /* pool 0 only */
+    int32_t activation;   /* 0..3 as vitb200_arch.activation; 4 (SwiGLU) is refused */
+    float logit_scale, logit_bias; /* HF's parameters as stored (the scale is its log), NaN when absent; metadata, no kernel reads them */
+} vitb200_text_arch;
+
+/* fp8 as vitb200_create_arch.  An engine is either a text or an image engine: every image entry point (forward, u8, features,
+ * recognition, sharded, image processor, vitb200_get_arch) fails on a text engine with a message, and the text entry points fail on an
+ * image engine.  vitb200_get_hparams, vitb200_mlp_dim, vitb200_fp8, vitb200_last_launch_count and profiling work on both. */
+int vitb200_create_text(const vitb200_hparams *hp, const vitb200_text_arch *ta, const vitb200_tensor *t, int n, int device, int max_batch,
+                        int fp8, vitb200_engine **out);
+int vitb200_get_text_arch(const vitb200_engine *e, vitb200_text_arch *out); /* non-zero on an image engine */
+/* ids: int32 [batch][N], padded by the caller to the context length (under the causal mask the padding leaves CLIP's EOS row as it is;
+ * SigLIP was trained on padded sequences).
+ * embeds (may be NULL): f32 [batch][E], the head applied to the f16 final LayerNorm of the pooled row: HF's text_embeds, or pooler_output
+ * when the head is the identity.
+ * req, tokens (may be NULL together): as vitb200_features: tokens [batch][N][D] after req->layers blocks, through the final LayerNorm or
+ * not, f32 / f16 / bf16 (layers = L - 1, norm = 0 is HF's hidden_states[-2], SDXL's conditioning).  Both outputs may be asked for in one
+ * call: the tokens are emitted after block req->layers and the remaining blocks run; blocks past req->layers run only when embeds is
+ * requested.  At least one output.
+ * vitb200_encode_text: HOST buffers, blocking; an id outside [0, V) is refused before anything is enqueued, naming the sequence and the
+ * position.  Small batches replay a cached CUDA graph.
+ * vitb200_encode_text_device: DEVICE buffers (16-byte aligned) on `stream` (NULL = the engine's), not synchronised; a sequence holding an
+ * id outside [0, V) gets NaN in every row (and so NaN outputs), its table rows are never read, and its batch mates are unaffected.
+ * Sequences are independent: a sequence's outputs depend only on its own ids.
+ * Launches: 1 + 7 L + 2 for embeds alone (token gather, the blocks, the pool kernel, the head GEMM); tokens add one kernel (or a copy, for
+ * un-normalised f32) and skip the blocks past req->layers when embeds is NULL.  Profile kinds: the gather is kind 0, the pool kernel 7. */
+int vitb200_encode_text(vitb200_engine *e, const int32_t *ids, int batch, float *embeds, const vitb200_features_req *req, void *tokens);
+int vitb200_encode_text_device(vitb200_engine *e, const int32_t *d_ids, int batch, float *d_embeds, const vitb200_features_req *req,
+                               void *d_tokens, void *stream);
+
 /* Number of kernels launched by the most recent call on this engine that enqueued work: a forward, features or recognition call,
  * including one that only pre-processes images (vitb200_forward_u8 without outputs: 1, or 2 with an image processor).  A call rejected by its argument checks
  * leaves the count as it was. */
@@ -388,6 +440,8 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
  * the sum of two f16 numbers, qkv_hi + qkv_lo (what the qkv GEMM's hi-lo epilogue leaves behind: hi = f16(x), lo = f16(x - hi)), so
  * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858). */
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+/* The same with CLIP's causal mask (vitb200_text_arch.causal): query row t attends to keys 0 .. t of its sequence. */
+int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 
 /* Stand-alone run of the attention-pooling head's attention kernel (vitb200_arch.pool = 2) through the engine's launcher: one query
  * q float32 [H*64] (the probe's, scaled by 1/8 inside) per head against the P key rows of each image; kv = f16 bits [B*P][2*H*64], every

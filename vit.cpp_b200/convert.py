@@ -7,6 +7,7 @@
     python -m convert <SigLIP model.safetensors> <out.gguf> --hf-config config.json               (Hugging Face SigLIP vision tower)
     python -m convert <any of the above, or a converted model file> <out.gguf> ... --hf-preprocessor preprocessor_config.json
                                                                     (the u8 entry points prepare images as this HF image processor does)
+    python -m convert <CLIP or SigLIP model.safetensors> <out.gguf> --hf-config config.json --text     (the text tower)
     python -m convert --quantize <in.gguf> <out.gguf> q8_0
 
 * `state_dict_to_model_file` follows reference convert-pth-to-ggml.py:105-158 step by step (header, id2label table, tensors in
@@ -23,6 +24,9 @@
 * `siglip_to_model_file` converts a Hugging Face SigLIP vision tower (SiglipVisionModel, the vision tower of SiglipModel, or
   SiglipForImageClassification) to a GGUF file without a class token, with PyTorch's tanh GELU and the attention-pooling head (pool 'map')
   or, with a classifier, the token mean (pool 'mean') (`siglip_to_timm`).
+* `text_to_model_file` converts the text tower of a Hugging Face CLIP (CLIPTextModel, CLIPTextModelWithProjection, CLIPModel) or SigLIP
+  (SiglipTextModel, SiglipModel) to a GGUF text file (vitb200_text_arch: token table, causal mask for CLIP, EOS or last-row pooling, the
+  projection as the head, logit_scale / logit_bias as metadata) (`text_to_timm`).  Tokenisation stays with the caller's HF tokenizer.
 * `quantize_model_file` restates reference quantize.cpp for q8_0 (every 2-D `*weight` tensor, quantize_row_q8_0_reference,
   ggml-quants.c): byte-identical to the reference binary's output (pinned by the CPU test-suite).
 
@@ -420,6 +424,72 @@ def siglip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str,
     state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool, image_proc=image_proc)
 
 
+# Hugging Face text activations -> the file's; HF's "gelu" is the erf form
+_HF_TEXT_ACTIVATIONS = {"quick_gelu": "quick_gelu", "gelu": "gelu_erf", "gelu_pytorch_tanh": "gelu_pytorch_tanh"}
+MAX_TEXT_CONTEXT = 224  # the split-precision attention's keys
+
+
+def text_to_timm(sd: Dict[str, np.ndarray], config: dict):
+    """The text tower (`text_model.*`) of a Hugging Face CLIP or SigLIP state dict -> (state dict in the engine's names, heads, activation,
+    eps, text arch dict for VitFile.text).  config: config.json (a CLIPConfig's or SiglipConfig's `text_config` is used when present).
+    SigLIP is recognised by its text head (`text_model.head.*`, the pooled row's projection with a bias) and pools the last row,
+    bidirectionally; CLIP runs causally and pools the EOS row ('eos_argmax' when eos_token_id == 2, as HF does, 'eos' otherwise), with
+    `text_projection` as the head (bias 0) or, for CLIPTextModel, the identity.  logit_scale / logit_bias are copied when present."""
+    tc = config.get("text_config", config)
+    v = {k[len("text_model."):]: np.asarray(a, np.float32) for k, a in sd.items() if k.startswith("text_model.")}
+    if "embeddings.token_embedding.weight" not in v:
+        raise ValueError("no text tower: the state dict has no text_model.embeddings.token_embedding.weight")
+    siglip = "head.weight" in v
+    act = tc.get("hidden_act", "gelu_pytorch_tanh" if siglip else "quick_gelu")
+    if act not in _HF_TEXT_ACTIVATIONS:
+        raise ValueError(f"hidden_act {act!r} is not supported ({', '.join(_HF_TEXT_ACTIVATIONS)})")
+    tok = v["embeddings.token_embedding.weight"]                         # (V, D)
+    D = int(tok.shape[1])
+    heads = int(tc.get("num_attention_heads", D // 64))
+    if D % heads or D // heads != 64:
+        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    pos = v["embeddings.position_embedding.weight"]                      # (N, D)
+    if pos.shape[0] > MAX_TEXT_CONTEXT:
+        raise ValueError(f"context {pos.shape[0]} is not supported (at most {MAX_TEXT_CONTEXT} tokens)")
+    layers = 1 + max(int(m.group(1)) for k in v for m in [re.match(r"encoder\.layers\.(\d+)\.", k)] if m)
+    out = {"token_embd.weight": tok, "pos_embed": pos.reshape(1, -1, D)}
+    hf_name = {"norm1": "layer_norm1", "attn.proj": "self_attn.out_proj", "norm2": "layer_norm2", "mlp.fc1": "mlp.fc1", "mlp.fc2": "mlp.fc2"}
+    for i in range(layers):
+        h, t = f"encoder.layers.{i}.", f"blocks.{i}."
+        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        for dst in ("norm1", "attn.qkv", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"):
+            for p in ("weight", "bias"):
+                if dst == "attn.qkv":  # rows [q; k; v]
+                    out[f"{t}{dst}.{p}"] = np.concatenate([v[f"{h}self_attn.{x}_proj.{p}"] for x in "qkv"], axis=0)
+                else:
+                    out[f"{t}{dst}.{p}"] = v[f"{h}{hf_name[dst]}.{p}"]
+    out["norm.weight"], out["norm.bias"] = v["final_layer_norm.weight"], v["final_layer_norm.bias"]
+    if siglip:
+        out["head.weight"], out["head.bias"] = v["head.weight"], v["head.bias"]
+    else:
+        proj = sd.get("text_projection.weight")
+        out["head.weight"] = np.asarray(proj, np.float32) if proj is not None else np.eye(D, dtype=np.float32)
+        out["head.bias"] = np.zeros(out["head.weight"].shape[0], np.float32)
+    eos = int(tc.get("eos_token_id", 2))
+    scalar = lambda k: float(np.asarray(sd[k], np.float32).reshape(-1)[0]) if k in sd else None
+    text = {"context": int(pos.shape[0]), "causal": 0 if siglip else 1, "pool": "last" if siglip else ("eos_argmax" if eos == 2 else "eos"),
+            "eos_token_id": eos, "logit_scale": scalar("logit_scale"), "logit_bias": scalar("logit_bias")}
+    return out, heads, _HF_TEXT_ACTIVATIONS[act], float(tc.get("layer_norm_eps", 1e-6 if siglip else 1e-5)), text
+
+
+def text_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1) -> None:
+    """The text tower of a Hugging Face CLIP or SigLIP checkpoint -> GGUF text file (vitb200_create_text)."""
+    tsd, heads, activation, eps, text = text_to_timm(sd, config)
+    D, layers = int(tsd["token_embd.weight"].shape[1]), sum(1 for k in tsd if k.endswith(".norm1.weight"))
+    vf = gf.VitFile(D, layers, heads, int(tsd["head.weight"].shape[0]), 0, 0, ftype, eps=eps, activation=activation, text=text)
+    for k, a in tsd.items():
+        f16 = ftype == 1 and a.ndim == 2  # the matrices; pos_embed [1, N, D] and every 1-D tensor stay f32
+        vf.tensors[k] = np.asarray(a, np.float16 if f16 else np.float32)
+        vf.tensor_ftype[k] = 1 if f16 else 0
+    gf.write_gguf(out_path, vf, "keep")
+
+
 def write_legacy(path: str, vf) -> None:
     """A VitFile (f32 / f16 / raw q8_0 tensors) -> legacy-ggml container, tensor order as stored."""
     with open(path, "wb") as f:
@@ -513,6 +583,7 @@ def main(argv):
     ap.add_argument("--eps", type=float, default=1e-6, help="timm: the LayerNorm epsilon (GGUF only)")
     ap.add_argument("--img-size", type=int, default=None,
                     help="resample the patch position embeddings to this input size (default: the checkpoint's grid)")
+    ap.add_argument("--text", action="store_true", help="convert the text tower of a Hugging Face CLIP or SigLIP checkpoint (GGUF)")
     ap.add_argument("--hf-preprocessor", default=None,
                     help="preprocessor_config.json of a Hugging Face image processor: the u8 entry points prepare images as it does (GGUF)")
     a = ap.parse_args(argv)
@@ -527,6 +598,11 @@ def main(argv):
         add_image_proc(a.src, a.dst, proc)
         return
     sd = load_state_dict(a.src)
+    if a.text:
+        if not a.hf_config:
+            raise SystemExit("--text needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads, eos_token_id)")
+        text_to_model_file(sd, json.load(open(a.hf_config)), a.dst, a.ftype)
+        return
     if is_hf_dinov2(sd):
         if not a.hf_config:
             raise SystemExit("a Hugging Face DINOv2 state dict needs --hf-config <config.json> (hidden_act, layer_norm_eps, heads)")

@@ -10,7 +10,9 @@
 //             call) reaches shared memory, and a NaN or Inf there cannot turn the P V product of this image into NaN
 //   S = QK^T  wgmma.m64n224k16, A = Q tile and B = K from shared memory, f32 accumulators in registers (one warpgroup per 64-query
 //             tile; two warpgroups, each taking every other tile): S = Ql Kh^T + Qh Kl^T + Qh Kh^T (kernels.cuh explains why)
-//   softmax   in registers: each row lives in one quad of lanes; P is packed to f16 in place, already in the A-fragment layout
+//   softmax   in registers: each row lives in one quad of lanes; P is packed to f16 in place, already in the A-fragment layout.
+//             CAUSAL (CLIP's text towers): first every score with key > row becomes -inf, so it is left out of the row maximum and gets
+//             P = f16(ex2(-inf)) = 0 -- what the keys past N get.  Key 0 is in every row, so no row is empty
 //   O = P V   wgmma.m64n64k16 with A = P from registers and B = V (MN-major) from shared memory: O = P Vl + P Vh
 #pragma once
 #include "kernels.cuh"
@@ -29,6 +31,7 @@ __host__ __device__ inline int attention_wgmma_smem_bytes()
     return 1024 + ATTW_PARTS * (4 * ATTW_QTILE_BYTES + 2 * ATTW_KV_BYTES) + 64;
 }
 
+template <bool CAUSAL>
 __global__ void __launch_bounds__(ATTW_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                        const __grid_constant__ CUtensorMap tmQl, const __grid_constant__ CUtensorMap tmKVl,
@@ -95,6 +98,19 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         ptx::wgmma_wait<0>();
         ptx::fence_regs(s);
 
+        if constexpr (CAUSAL)
+        {
+            const int r = mt * 64 + warp * 16 + (lane >> 2); // query rows r and r + 8 of this thread
+#pragma unroll
+            for (int j = 0; j < ATTW_KEYS / 8; ++j)
+            {
+                const int key = 8 * j + c0;
+                if (key > r) s[4 * j] = -INFINITY;
+                if (key + 1 > r) s[4 * j + 1] = -INFINITY;
+                if (key > r + 8) s[4 * j + 2] = -INFINITY;
+                if (key + 1 > r + 8) s[4 * j + 3] = -INFINITY;
+            }
+        }
         // ---- soft-max over the valid keys: rows r (s[4j], s[4j+1]) and r + 8 (s[4j+2], s[4j+3]) of this quad
         float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll

@@ -157,6 +157,7 @@ struct Slot
     // the image processor's horizontal pass (vitb200_set_image_proc): [rows][img_size][3] u8 per image, grown like the staging buffer
     uint8_t *d_proc = nullptr;
     size_t proc_cap = 0;
+    int32_t *ids = nullptr; // text engines: the token ids of the call [max_batch][N]
     cudaEvent_t ev_h2d = nullptr, ev_done = nullptr;
 };
 
@@ -189,6 +190,13 @@ struct vitb200_engine
     std::vector<void *> allocs;
     // weights
     float *cls = nullptr, *pos = nullptr, *norm_w = nullptr, *norm_b = nullptr; // cls: [1 + reg_tokens][D], cls_token then reg_token
+    // text towers (vitb200_create_text): the token table tok [V][D] f16 replaces the patch embedding; TOKS stages the host call's token
+    // rows ([max_batch][N][D] f32 at most), which are written mid-schedule, while H16 is still in use
+    bool text = false;
+    vitb200_text_arch text_arch{};
+    __half *tok = nullptr;
+    int V = 0;
+    uint8_t *TOKS = nullptr;
     Linear patch, head;
     std::vector<Layer> layers;
     // activations (static arena, sized for max_batch)
@@ -807,8 +815,9 @@ int make_attention_maps(vitb200_engine *e)
 int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int H = e->hp.num_attention_heads;
-    return launch(e, attention_wgmma_kernel, dim3(B * H), dim3(ATTW_THREADS), (size_t)attention_wgmma_smem_bytes(), s, LAUNCH_PDL, e->tmQ, e->tmKV,
-                  e->tmQl, e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, e->max_batch, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
+    const auto kern = e->text && e->text_arch.causal ? attention_wgmma_kernel<true> : attention_wgmma_kernel<false>;
+    return launch(e, kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)attention_wgmma_smem_bytes(), s, LAUNCH_PDL, e->tmQ, e->tmKV, e->tmQl,
+                  e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, e->max_batch, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
 }
 
 // The mma.sync kernels hold K and V of one (image, head) problem in shared memory: N tokens padded to whole key chunks, 64 f16 each.
@@ -901,9 +910,8 @@ int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
     return 0;
 }
 
-// The encoder part of the fixed kernel schedule: embeddings (vit.cpp:772-797), then blocks 0 .. layers-1 (vit.cpp:802-901); afterwards
-// the residual stream X holds the encoder's output at that depth.
-int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cudaStream_t s, const vitb200_taps *taps)
+// The embedding stage of the image schedule (vit.cpp:772-797): afterwards the residual stream X holds the input of block 0
+int run_embed(vitb200_engine *e, const float *d_images, int B, cudaStream_t s, const vitb200_taps *taps)
 {
     const int D = e->hp.hidden_size, N = e->N, T = B * N;
     __half *PA = e->PA;
@@ -932,8 +940,14 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (launch_layernorm_inplace(e, e->X, e->npre_w, e->npre_b, T, s)) return 1;
     }
     if (taps && tap_f32(taps->embed, e->X, (size_t)T * D, s)) return 1;
+    return 0;
+}
 
-    for (int il = 0; il < layers; ++il)
+// Blocks first .. last-1 (vit.cpp:802-901) on the residual stream X of B images or sequences, in place
+int run_blocks(vitb200_engine *e, int B, int first, int last, cudaStream_t s, const vitb200_taps *taps)
+{
+    const int D = e->hp.hidden_size, N = e->N, T = B * N;
+    for (int il = first; il < last; ++il)
     {
         const Layer &L = e->layers[il];
         const bool tap = taps && taps->layer == il;
@@ -994,6 +1008,13 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
         if (tap && tap_f32(taps->x2, e->X, (size_t)T * D, s)) return 1;
     }
     return 0;
+}
+
+// The encoder part of the fixed kernel schedule: embeddings, then blocks 0 .. layers-1; afterwards the residual stream X holds the
+// encoder's output at that depth.
+int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cudaStream_t s, const vitb200_taps *taps)
+{
+    return run_embed(e, d_images, B, s, taps) || run_blocks(e, B, 0, layers, s, taps);
 }
 
 int check_batch(const vitb200_engine *e, int batch)
@@ -1098,31 +1119,37 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
 // Encoder features (vitb200_features*): the encoder up to block req->layers, then the requested rows of the residual stream -- all T
 // token rows into d_tokens, the head_tokens pooled rows of every image into d_prelogits -- normalised with the final LayerNorm or not,
 // as f32 / f16 / bf16.  Device destinations; either may be NULL.  An un-normalised f32 output is a copy, every other one a kernel.
+// The requested rows of the residual stream X into dst, as req asks for them: rows_per_group of every group of N rows, normalised with the
+// final LayerNorm or not, as f32 / f16 / bf16.  An un-normalised f32 output is a copy, every other one a kernel.  dst NULL: nothing.
+int emit_rows(vitb200_engine *e, const vitb200_features_req *req, void *dst, int rows, int rows_per_group, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size, N = e->N;
+    if (!dst) return 0;
+    if (!req->norm && req->dtype == 0)
+    {
+        // [B][rows_per_group][D] out of [B][N][D]: one 2-D copy (the token rows are a single plain copy)
+        const size_t w = (size_t)rows_per_group * D * sizeof(float);
+        CUDA_TRY(cudaMemcpy2DAsync(dst, w, e->X, (size_t)N * D * sizeof(float), w, (size_t)rows / rows_per_group, cudaMemcpyDeviceToDevice, s));
+        return 0;
+    }
+    ProfScope ps(e, PK_LN, 0.0, s);
+    const size_t gs = (size_t)N * D;
+    switch (req->dtype * 2 + (req->norm ? 1 : 0))
+    {
+    case 1: return launch_layernorm_rows<float, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (float *)dst, rows, s, rows_per_group, gs);
+    case 2: return launch_layernorm_rows<__half, false>(e, e->X, (size_t)D, nullptr, nullptr, (__half *)dst, rows, s, rows_per_group, gs);
+    case 3: return launch_layernorm_rows<__half, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__half *)dst, rows, s, rows_per_group, gs);
+    case 4: return launch_layernorm_rows<__nv_bfloat16, false>(e, e->X, (size_t)D, nullptr, nullptr, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
+    case 5: return launch_layernorm_rows<__nv_bfloat16, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
+    }
+    return fail("features: dtype %d unknown", req->dtype);
+}
+
 int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_features_req *req, void *d_tokens, void *d_prelogits, cudaStream_t s)
 {
     const int D = e->hp.hidden_size, N = e->N, TH = e->head_tokens;
     if (run_encoder(e, d_images, B, req->layers, s, nullptr)) return 1;
-    auto emit = [&](void *dst, int rows, int rows_per_group) -> int {
-        if (!dst) return 0;
-        if (!req->norm && req->dtype == 0)
-        {
-            // [B][rows_per_group][D] out of [B][N][D]: one 2-D copy (the token rows are a single plain copy)
-            const size_t w = (size_t)rows_per_group * D * sizeof(float);
-            CUDA_TRY(cudaMemcpy2DAsync(dst, w, e->X, (size_t)N * D * sizeof(float), w, (size_t)rows / rows_per_group, cudaMemcpyDeviceToDevice, s));
-            return 0;
-        }
-        ProfScope ps(e, PK_LN, 0.0, s);
-        const size_t gs = (size_t)N * D;
-        switch (req->dtype * 2 + (req->norm ? 1 : 0))
-        {
-        case 1: return launch_layernorm_rows<float, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (float *)dst, rows, s, rows_per_group, gs);
-        case 2: return launch_layernorm_rows<__half, false>(e, e->X, (size_t)D, nullptr, nullptr, (__half *)dst, rows, s, rows_per_group, gs);
-        case 3: return launch_layernorm_rows<__half, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__half *)dst, rows, s, rows_per_group, gs);
-        case 4: return launch_layernorm_rows<__nv_bfloat16, false>(e, e->X, (size_t)D, nullptr, nullptr, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
-        case 5: return launch_layernorm_rows<__nv_bfloat16, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
-        }
-        return fail("features: dtype %d unknown", req->dtype);
-    };
+    auto emit = [&](void *dst, int rows, int rows_per_group) { return emit_rows(e, req, dst, rows, rows_per_group, s); };
     if (d_prelogits && e->arch.pool == 2)
     {
         // SigLIP's attention-pooling head on the final LayerNorm of the rows at this depth (norm = 1, check_features), before the
@@ -1222,10 +1249,78 @@ int run_features_graphed(vitb200_engine *e, const float *d_images, int B, const 
     return run_graphed(e, key, s, [&] { return run_features(e, d_images, B, req, d_tokens, d_prelogits, s); });
 }
 
+// The text schedule (vitb200_encode_text*): the token rows, blocks 0 .. L-1 with the token rows emitted after block req->layers (the blocks
+// past it only when embeds are wanted), then each sequence's pooled row through the final LayerNorm and the head.  Device destinations;
+// either may be NULL (req is read only with d_tokens).
+int run_text(vitb200_engine *e, const int32_t *d_ids, int B, float *d_embeds, const vitb200_features_req *req, void *d_tokens, cudaStream_t s)
+{
+    const int D = e->hp.hidden_size, N = e->N, L = e->hp.num_hidden_layers, E = e->hp.num_classes;
+    {
+        ProfScope ps(e, PK_PATCH, 0.0, s);
+        if (launch(e, token_embed_kernel, dim3((unsigned)N, (unsigned)B), dim3(TOKEN_EMBED_THREADS), 0, s, LAUNCH_PLAIN, d_ids, e->tok, e->pos,
+                   e->X, N, D, e->V))
+            return 1;
+    }
+    const int at = d_tokens ? req->layers : L;
+    if (run_blocks(e, B, 0, at, s, nullptr) || (d_tokens && emit_rows(e, req, d_tokens, B * N, N, s))) return 1;
+    if (!d_embeds) return 0;
+    if (run_blocks(e, B, at, L, s, nullptr)) return 1;
+    {
+        ProfScope ps(e, PK_LN, 0.0, s);
+        const auto kern = D <= 4 * 128 ? text_pool_kernel<4> : D <= 8 * 128 ? text_pool_kernel<8> : text_pool_kernel<LN_ROWS_MAX_V>;
+        if (launch(e, kern, dim3((unsigned)((B + TEXT_POOL_WARPS - 1) / TEXT_POOL_WARPS)), dim3(TEXT_POOL_WARPS * 32), 0, s, LAUNCH_PDL, e->X, d_ids,
+                   B, N, e->text_arch.pool, e->text_arch.eos_token_id, e->norm_w, e->norm_b, e->CLS16, D, e->hp.eps))
+            return 1;
+    }
+    // rows of pitch Cp (E padded to 4) unless the caller's dense rows coincide, as the image head's logits
+    float *lg = e->Cp == E ? d_embeds : e->d_logits;
+    GemmParams p{};
+    p.M = B; p.N = e->Cp; p.K = D; p.bias = e->head.b; p.out = lg; p.ldo = e->Cp;
+    {
+        ProfScope ps(e, PK_HEAD, 2.0 * B * E * D, s);
+        if (launch_gemm(e, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
+    }
+    if (lg != d_embeds)
+        CUDA_TRY(cudaMemcpy2DAsync(d_embeds, (size_t)E * 4, lg, (size_t)e->Cp * 4, (size_t)E * 4, (size_t)B, cudaMemcpyDeviceToDevice, s));
+    return 0;
+}
+
+int run_text_graphed(vitb200_engine *e, const int32_t *d_ids, int B, float *d_embeds, const vitb200_features_req *req, void *d_tokens, cudaStream_t s)
+{
+    const GraphKey key{d_ids, B, nullptr, d_embeds, nullptr, nullptr, 0, d_tokens ? req->layers : -1, d_tokens ? req->norm : 0,
+                       d_tokens ? req->dtype : 0, d_tokens, nullptr};
+    return run_graphed(e, key, s, [&] { return run_text(e, d_ids, B, d_embeds, req, d_tokens, s); });
+}
+
+// The refusal of an image entry point on a text engine
+int image_only(const vitb200_engine *e, const char *fn)
+{
+    if (e && e->text) return fail("%s: this is a text engine (vitb200_create_text); it takes token ids through vitb200_encode_text", fn);
+    return 0;
+}
+
+// Argument checks of the two vitb200_encode_text entry points, before anything is enqueued
+int check_text(const vitb200_engine *e, const void *ids, int batch, const void *embeds, const vitb200_features_req *req, const void *tokens)
+{
+    if (!e || !ids) return fail("vitb200_encode_text: null argument");
+    if (!e->text) return fail("vitb200_encode_text: this is an image engine; the text entry points need a text tower (vitb200_create_text)");
+    if (!embeds && !tokens) return fail("vitb200_encode_text: both outputs are NULL");
+    if (tokens)
+    {
+        if (!req) return fail("vitb200_encode_text: tokens need a vitb200_features_req");
+        if (req->layers < 0 || req->layers > e->hp.num_hidden_layers)
+            return fail("vitb200_encode_text: layers %d out of range (0..%d)", req->layers, e->hp.num_hidden_layers);
+        if (req->norm != 0 && req->norm != 1) return fail("vitb200_encode_text: norm must be 0 or 1 (got %d)", req->norm);
+        if (req->dtype < 0 || req->dtype > 2) return fail("vitb200_encode_text: dtype %d unknown (0 f32, 1 f16, 2 bf16)", req->dtype);
+    }
+    return check_batch(e, batch);
+}
+
 // Argument checks of the three vitb200_features entry points, before anything is enqueued
 int check_features(const vitb200_engine *e, const void *images, int batch, const vitb200_features_req *req, const void *tokens, const void *prelogits)
 {
     if (!e || !images || !req) return fail("vitb200_features: null argument");
+    if (image_only(e, "vitb200_features")) return 1;
     if (req->layers < 0 || req->layers > e->hp.num_hidden_layers)
         return fail("vitb200_features: layers %d out of range (0..%d)", req->layers, e->hp.num_hidden_layers);
     if (req->norm != 0 && req->norm != 1) return fail("vitb200_features: norm must be 0 or 1 (got %d)", req->norm);
@@ -1316,6 +1411,31 @@ int upload_probe_query(vitb200_engine *e, const vitb200_tensor *t, int n, int D)
     if (dev_alloc(e, &e->pool_q, (size_t)D)) return 1;
     CUDA_TRY(cudaMemcpy(e->pool_q, q.data(), (size_t)D * sizeof(float), cudaMemcpyHostToDevice));
     return 0;
+}
+
+// The weights of every block ('blocks.{i}.*': LayerNorms, qkv, proj, fc1, fc2 and, with layer_scale, the LayerScale gammas) and the final
+// LayerNorm ('norm.*'), as e->hp, e->F and e->fp8 describe them; swiglu: fc1 is SwiGLU's [2 F][D]
+int upload_blocks(vitb200_engine *e, const vitb200_tensor *t, int n, bool swiglu, bool layer_scale)
+{
+    const int D = e->hp.hidden_size, F = e->F;
+    const bool fp8 = e->fp8;
+    e->layers.resize(e->hp.num_hidden_layers);
+    for (int i = 0; i < e->hp.num_hidden_layers; ++i)
+    {
+        Layer &L = e->layers[i];
+        const std::string p = "blocks." + std::to_string(i) + ".";
+        if (upload_f32(e, t, n, p + "norm1.weight", D, 1, 1, 1, &L.n1w) || upload_f32(e, t, n, p + "norm1.bias", D, 1, 1, 1, &L.n1b) ||
+            upload_f32(e, t, n, p + "norm2.weight", D, 1, 1, 1, &L.n2w) || upload_f32(e, t, n, p + "norm2.bias", D, 1, 1, 1, &L.n2b))
+            return 1;
+        if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv, 0, fp8) ||
+            upload_linear(e, t, n, p + "attn.proj.weight", p + "attn.proj.bias", D, D, D, &L.proj) ||
+            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", swiglu ? 2 * F : F, D, D, &L.fc1, 0, fp8, swiglu) ||
+            upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, F, F, &L.fc2))
+            return 1;
+        if (layer_scale && (upload_f32(e, t, n, p + "ls1.gamma", D, 1, 1, 1, &L.ls1) || upload_f32(e, t, n, p + "ls2.gamma", D, 1, 1, 1, &L.ls2)))
+            return 1;
+    }
+    return upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b);
 }
 
 // Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
@@ -1457,23 +1577,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (upload_linear(e, t, n, "patch_embed.proj.weight", "patch_embed.proj.bias", D, e->KP, e->KPp, &e->patch, P)) return 1;
     if (ar.pre_norm && (upload_f32(e, t, n, "norm_pre.weight", D, 1, 1, 1, &e->npre_w) || upload_f32(e, t, n, "norm_pre.bias", D, 1, 1, 1, &e->npre_b)))
         return 1;
-    e->layers.resize(hp->num_hidden_layers);
-    for (int i = 0; i < hp->num_hidden_layers; ++i)
-    {
-        Layer &L = e->layers[i];
-        const std::string p = "blocks." + std::to_string(i) + ".";
-        if (upload_f32(e, t, n, p + "norm1.weight", D, 1, 1, 1, &L.n1w) || upload_f32(e, t, n, p + "norm1.bias", D, 1, 1, 1, &L.n1b) ||
-            upload_f32(e, t, n, p + "norm2.weight", D, 1, 1, 1, &L.n2w) || upload_f32(e, t, n, p + "norm2.bias", D, 1, 1, 1, &L.n2b))
-            return 1;
-        if (upload_linear(e, t, n, p + "attn.qkv.weight", p + "attn.qkv.bias", 3 * D, D, D, &L.qkv, 0, fp8) ||
-            upload_linear(e, t, n, p + "attn.proj.weight", p + "attn.proj.bias", D, D, D, &L.proj) ||
-            upload_linear(e, t, n, p + "mlp.fc1.weight", p + "mlp.fc1.bias", ar.activation == 4 ? 2 * F : F, D, D, &L.fc1, 0, fp8, ar.activation == 4) ||
-            upload_linear(e, t, n, p + "mlp.fc2.weight", p + "mlp.fc2.bias", D, F, F, &L.fc2))
-            return 1;
-        if (ar.layer_scale && (upload_f32(e, t, n, p + "ls1.gamma", D, 1, 1, 1, &L.ls1) || upload_f32(e, t, n, p + "ls2.gamma", D, 1, 1, 1, &L.ls2)))
-            return 1;
-    }
-    if (upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b)) return 1;
+    if (upload_blocks(e, t, n, ar.activation == 4, ar.layer_scale != 0)) return 1;
     if (upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, e->KH, e->KH, &e->head)) return 1;
     if (ar.pool == 2 &&
         (upload_linear(e, t, n, "attn_pool.kv.weight", "attn_pool.kv.bias", 2 * D, D, D, &e->pool_kv) ||
@@ -1532,6 +1636,103 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e))) return 1;
     if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
     if (labels) e->labels = *labels;
+    *out = owner.release();
+    return 0;
+}
+
+template <typename T>
+int upload(vitb200_engine *e, T **d, const void *src, size_t count);
+
+// Builds a text engine (vitb200_create_text); *out receives it only when everything succeeded.  The blocks, the final LayerNorm and the
+// head are the image engine's; the token table and the position rows replace the patch embedding, and N = context <= 224, so the qkv GEMM
+// always writes hi + lo for the split-precision attention.
+int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, const vitb200_tensor *t, int n, int device, int max_batch, bool fp8,
+                     vitb200_engine **out)
+{
+    if (!hp || !ta || !t || !out) return fail("vitb200_create_text: null argument");
+    *out = nullptr;
+    if (hp->hidden_size < 64 || hp->hidden_size > 8192 || hp->num_hidden_layers < 1 || hp->num_hidden_layers > 4096 ||
+        hp->num_attention_heads < 1 || hp->num_attention_heads > 128 || hp->num_classes < 1 || hp->num_classes > (1 << 20) || n < 1)
+        return fail("invalid hyper-parameters (hidden %d, layers %d, heads %d, projection %d)", hp->hidden_size, hp->num_hidden_layers,
+                    hp->num_attention_heads, hp->num_classes);
+    if (hp->patch_size != 0 || hp->img_size != 0)
+        return fail("vitb200_create_text: patch_size and img_size must be 0 for a text tower (got %d and %d)", hp->patch_size, hp->img_size);
+    const vitb200_text_arch a = *ta;
+    if (a.context < 1 || a.context > ATTW_KEYS)
+        return fail("vitb200_text_arch.context = %d out of range (1..%d tokens: the keys of the split-precision attention)", a.context, ATTW_KEYS);
+    if (a.causal != 0 && a.causal != 1) return fail("vitb200_text_arch.causal = %d out of range (0 bidirectional, 1 causal)", a.causal);
+    if (a.pool < 0 || a.pool > 2) return fail("vitb200_text_arch.pool = %d out of range (0 eos, 1 eos_argmax, 2 last)", a.pool);
+    if (a.activation < 0 || a.activation > 3)
+        return fail("vitb200_text_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh; swiglu is "
+                    "not a text tower's MLP)", a.activation);
+    const int D = hp->hidden_size;
+    if (D % hp->num_attention_heads != 0 || D / hp->num_attention_heads != 64)
+        return fail("head dim %d not supported (64 only)", D / hp->num_attention_heads);
+    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
+    const vitb200_tensor *te = find_tensor(t, n, "token_embd.weight"), *pe = find_tensor(t, n, "pos_embed");
+    if (!te) return fail("missing tensor 'token_embd.weight'");
+    const int64_t V = dim_of(te, 1);
+    if (dim_of(te, 0) != D || V < 1 || V > (1 << 30) || dim_of(te, 2) != 1 || dim_of(te, 3) != 1)
+        return fail("tensor 'token_embd.weight' must be [V][%d] with 1 <= V <= 2^30, got [%lld, %lld, %lld, %lld] (ggml order)", D,
+                    (long long)dim_of(te, 0), (long long)dim_of(te, 1), (long long)dim_of(te, 2), (long long)dim_of(te, 3));
+    if (pe && dim_of(pe, 1) != a.context)
+        return fail("vitb200_text_arch.context = %d, but 'pos_embed' has %lld rows", a.context, (long long)dim_of(pe, 1));
+    cudaDeviceProp prop;
+    if (open_device(device, prop)) return 1;
+    if (max_batch < 1) return fail("max_batch must be >= 1");
+    if (check_unique_names(t, n)) return 1;
+
+    EnginePtr owner(new vitb200_engine());
+    vitb200_engine *e = owner.get();
+    e->hp = *hp;
+    if (e->hp.eps <= 0.f) e->hp.eps = 1e-6f;
+    e->text = true;
+    e->text_arch = a;
+    e->arch.activation = a.activation; // the fc1 epilogue (fc1_epilogue)
+    e->device = device;
+    e->max_batch = max_batch;
+    e->fp8 = fp8;
+    e->num_sms = prop.multiProcessorCount;
+    e->N = a.context;
+    e->F = 4 * D;
+    e->C = 0;
+    e->KH = D;
+    e->V = (int)V;
+    e->Cp = (hp->num_classes + 3) / 4 * 4;
+    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
+    {
+        // the token table in f16, whatever its file format (as upload_linear converts a weight)
+        std::vector<double> v;
+        if (host_values(te, "token_embd.weight", v)) return 1;
+        std::vector<uint16_t> h(v.size());
+        for (size_t i = 0; i < v.size(); ++i) h[i] = host_f32_to_f16((float)v[i]);
+        if (upload(e, &e->tok, h.data(), h.size())) return 1;
+    }
+    if (upload_f32(e, t, n, "pos_embed", D, e->N, 1, 1, &e->pos) || upload_blocks(e, t, n, false, false) ||
+        upload_linear(e, t, n, "head.weight", "head.bias", hp->num_classes, D, D, &e->head))
+        return 1;
+
+    const size_t B = (size_t)max_batch, T = B * e->N;
+    if (dev_alloc(e, &e->X, T * D) || dev_alloc(e, &e->A16, T * D) || dev_alloc(e, &e->QKV16, T * 3 * D) || dev_alloc(e, &e->QKV16L, T * 3 * D) ||
+        dev_alloc(e, &e->H16, T * e->F) || dev_alloc(e, &e->CLS16, B * D) || dev_alloc(e, &e->d_logits, B * e->Cp) ||
+        dev_alloc(e, &e->TOKS, T * D * sizeof(float)))
+        return 1;
+    for (Slot &sl : e->slot)
+    {
+        if (dev_alloc(e, &sl.ids, T) || dev_alloc(e, &sl.logits, B * hp->num_classes)) return 1;
+        if (cudaEventCreateWithFlags(&sl.ev_h2d, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming) != cudaSuccess)
+            return fail("cudaEventCreate failed");
+    }
+    if (cudaStreamCreateWithFlags(&e->copy_stream, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed");
+    auto a_map = [&](CUtensorMap *m, const void *ptr, cuuint64_t rows, cuuint64_t cols, bool e4m3 = false) {
+        return e4m3 ? make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, ptr, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_A_BOX_ROWS})
+                    : make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_A_BOX_ROWS});
+    };
+    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, (cuuint64_t)e->F) || a_map(&e->tmA_C, e->CLS16, B, D) || make_attention_maps(e))
+        return 1;
+    if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
+    if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
     *out = owner.release();
     return 0;
 }
@@ -1711,10 +1912,27 @@ int vitb200_create_arch(const vitb200_hparams *hp, const vitb200_arch *arch, con
     return guarded(__func__, [&] { return create_impl(hp, arch, t, n, device, max_batch, head_tokens, fp8 != 0, out); });
 }
 
+int vitb200_create_text(const vitb200_hparams *hp, const vitb200_text_arch *ta, const vitb200_tensor *t, int n, int device, int max_batch,
+                        int fp8, vitb200_engine **out)
+{
+    return guarded(__func__, [&] { return create_text_impl(hp, ta, t, n, device, max_batch, fp8 != 0, out); });
+}
+
+int vitb200_get_text_arch(const vitb200_engine *e, vitb200_text_arch *out)
+{
+    return guarded(__func__, [&] {
+        if (!e || !out) return fail("null argument");
+        if (!e->text) return fail("vitb200_get_text_arch: this is an image engine");
+        *out = e->text_arch;
+        return 0;
+    });
+}
+
 int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out)
 {
     return guarded(__func__, [&] {
         if (!e || !out) return fail("null argument");
+        if (image_only(e, __func__)) return 1;
         *out = e->arch;
         return 0;
     });
@@ -1753,6 +1971,7 @@ static int check_image_proc(int C, int S, const vitb200_image_proc &p)
 static int set_image_proc(vitb200_engine *e, const vitb200_image_proc *p)
 {
     if (!e) return fail("null argument");
+    if (image_only(e, "vitb200_set_image_proc")) return 1;
     if (p && check_image_proc(e->C, e->hp.img_size, *p)) return 1;
     e->has_proc = p != nullptr;
     e->proc = p ? *p : vitb200_image_proc{};
@@ -1768,6 +1987,7 @@ int vitb200_get_image_proc(const vitb200_engine *e, vitb200_image_proc *out)
 {
     return guarded(__func__, [&] {
         if (!e || !out) return fail("null argument");
+        if (image_only(e, __func__)) return 1;
         *out = e->proc;
         return 0;
     });
@@ -1850,13 +2070,16 @@ int vitb200_profile_read(vitb200_engine *e, int kind, double *ms_total, int *lau
     });
 }
 
-static int test_attention_impl(int device, int kernel, int B, int N, int H, const uint16_t *qkv, const uint16_t *qkv_lo, float *out)
+// causal: the wgmma kernel with CLIP's causal mask, as a causal text engine launches it
+static int test_attention_impl(int device, int kernel, int B, int N, int H, const uint16_t *qkv, const uint16_t *qkv_lo, float *out,
+                               bool causal = false)
 {
     if (!qkv || !out || B < 1 || N < 1 || H < 1) return fail("bad argument");
     EnginePtr owner;
     if (scratch_engine(device, owner)) return 1;
     vitb200_engine *e = owner.get();
     e->N = N; e->hp.hidden_size = H * 64; e->hp.num_attention_heads = H; e->max_batch = B;
+    e->text = causal; e->text_arch.causal = causal ? 1 : 0;
     const int D = H * 64;
     const uint64_t T = (uint64_t)B * N;
     // the kernels read the HEAD-MAJOR layout the qkv GEMM writes ([3 H][T][64]); the caller hands over the reference's [T][3 D]
@@ -1893,6 +2116,14 @@ int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t 
     return guarded(__func__, [&] {
         if (!qkv_lo) return fail("bad argument");
         return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out);
+    });
+}
+
+int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
+{
+    return guarded(__func__, [&] {
+        if (!qkv_lo) return fail("bad argument");
+        return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out, true);
     });
 }
 
@@ -1977,6 +2208,7 @@ int vitb200_forward_device(vitb200_engine *e, const float *d_images, int batch, 
 {
     return guarded(__func__, [&]() -> int {
         if (!e || !d_images) return fail("null argument");
+        if (image_only(e, __func__)) return 1;
         CUDA_TRY(cudaSetDevice(e->device));
         if (check_batch(e, batch) || check_k(e, k)) return 1;
         e->launches = 0;
@@ -2037,6 +2269,7 @@ static int forward_enqueue(vitb200_engine *e, const float *images, int batch, fl
                            float *topk_prob, int k, const vitb200_taps *taps)
 {
     if (!e || !images) return fail("null argument");
+    if (image_only(e, "vitb200_forward")) return 1;
     if (check_batch(e, batch) || check_k(e, k)) return 1; // before anything is enqueued
     CUDA_TRY(cudaSetDevice(e->device));
     Slot &sl = begin_submit(e);
@@ -2357,6 +2590,7 @@ static int forward_u8_enqueue(vitb200_engine *e, const uint8_t *const *images, c
                               float *images_f32_out, float *probs, float *logits, int32_t *topk_idx, float *topk_prob, int k)
 {
     if (!e || !images || !nx || !ny) return fail("null argument");
+    if (image_only(e, "vitb200_forward_u8")) return 1;
     if (e->C != 3) return fail("vitb200_forward_u8 implements vit_image_preprocess (RGB, vit.cpp:289-305); this model takes %d-channel input", e->C);
     if (check_batch(e, batch) || check_k(e, k) || check_u8_call(e, images, nx, ny, batch, bilinear)) return 1;
     Slot &sl = begin_submit(e);
@@ -2405,6 +2639,7 @@ static int recognize_enqueue(vitb200_engine *e, const uint8_t *const *images, co
                              int32_t *chars, int32_t *lengths, double *scores, float *probs)
 {
     if (!e || !images || !nx || !ny) return fail("vitb200_recognize_u8: null argument");
+    if (image_only(e, "vitb200_recognize_u8")) return 1;
     if (e->C != 1)
         return fail("vitb200_recognize_u8 implements the ViTSTR grayscale preprocess (1-channel, vitstr.cpp:128-201); this model takes "
                     "%d-channel input", e->C);
@@ -2453,6 +2688,44 @@ int vitb200_recognize_u8(vitb200_engine *e, const uint8_t *const *images, const 
     return guarded(__func__, [&] {
         if (recognize_enqueue(e, images, nx, ny, batch, images_f32_out, chars, lengths, scores, probs)) return 1;
         return vitb200_sync(e);
+    });
+}
+
+int vitb200_encode_text(vitb200_engine *e, const int32_t *ids, int batch, float *embeds, const vitb200_features_req *req, void *tokens)
+{
+    return guarded(__func__, [&]() -> int {
+        if (check_text(e, ids, batch, embeds, req, tokens)) return 1;
+        const int N = e->N, D = e->hp.hidden_size;
+        for (int b = 0; b < batch; ++b)
+            for (int t = 0; t < N; ++t)
+                if (ids[(size_t)b * N + t] < 0 || ids[(size_t)b * N + t] >= e->V)
+                    return fail("vitb200_encode_text: sequence %d, position %d: id %d out of range (0..%d)", b, t, ids[(size_t)b * N + t], e->V - 1);
+        CUDA_TRY(cudaSetDevice(e->device));
+        Slot &sl = begin_submit(e);
+        cudaStream_t s = e->stream, cs = e->copy_stream;
+        // the ids into this call's slot once its previous call has consumed them; the token rows are staged in TOKS (written mid-schedule)
+        if (e->submits >= 2) CUDA_TRY(cudaStreamWaitEvent(cs, sl.ev_done, 0));
+        CUDA_TRY(cudaMemcpyAsync(sl.ids, ids, (size_t)batch * N * sizeof(int32_t), cudaMemcpyHostToDevice, cs));
+        CUDA_TRY(cudaEventRecord(sl.ev_h2d, cs));
+        CUDA_TRY(cudaStreamWaitEvent(s, sl.ev_h2d, 0));
+        if (run_text_graphed(e, sl.ids, batch, embeds ? sl.logits : nullptr, req, tokens ? e->TOKS : nullptr, s)) return 1;
+        if (embeds) CUDA_TRY(cudaMemcpyAsync(embeds, sl.logits, (size_t)batch * e->hp.num_classes * sizeof(float), cudaMemcpyDeviceToHost, s));
+        if (tokens)
+            CUDA_TRY(cudaMemcpyAsync(tokens, e->TOKS, (size_t)batch * N * D * features_elem_bytes(req), cudaMemcpyDeviceToHost, s));
+        if (end_submit(e, sl)) return 1;
+        return vitb200_sync(e);
+    });
+}
+
+int vitb200_encode_text_device(vitb200_engine *e, const int32_t *d_ids, int batch, float *d_embeds, const vitb200_features_req *req,
+                               void *d_tokens, void *stream)
+{
+    return guarded(__func__, [&]() -> int {
+        if (check_text(e, d_ids, batch, d_embeds, req, d_tokens)) return 1;
+        if (((uintptr_t)d_embeds | (uintptr_t)d_tokens) % 16 != 0) return fail("vitb200_encode_text_device: output buffers must be 16-byte aligned");
+        CUDA_TRY(cudaSetDevice(e->device));
+        e->launches = 0;
+        return run_text_graphed(e, d_ids, batch, d_embeds, req, d_tokens, stream ? (cudaStream_t)stream : e->stream);
     });
 }
 
@@ -2653,6 +2926,29 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
     hp.num_attention_heads = i32(g.num_attention_heads); hp.num_classes = i32(g.num_classes);
     hp.patch_size = i32(g.patch_size); hp.img_size = i32(g.img_size); hp.ftype = i32(g.ftype); hp.eps = g.eps;
     if (hp.num_hidden_layers < 1 || hp.num_hidden_layers > 4096) return fail("invalid model file '%s' (num_hidden_layers %d)", path, hp.num_hidden_layers);
+    auto tensor_list = [&](std::vector<vitb200_tensor> &ts) {
+        ts.resize(g.tensors.size());
+        for (size_t i = 0; i < g.tensors.size(); ++i)
+        {
+            ts[i].name = g.tensors[i].name.c_str();
+            ts[i].data = buf.data() + g.tensors[i].offset;
+            ts[i].type = g.tensors[i].type;
+            ts[i].n_dims = g.tensors[i].n_dims;
+            for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
+        }
+    };
+    if (g.text)
+    {
+        // a CLIP or SigLIP text tower: token_embd, pos_embed, the blocks, norm and head
+        if (head_tokens != 1) return fail("'%s' is a text tower: head_tokens must be 1 (got %d)", path, head_tokens);
+        if (g.text_causal != 0 && g.text_causal != 1) return fail("invalid model file '%s' (vit.text.causal %lld)", path, (long long)g.text_causal);
+        const vitb200_text_arch ta{i32(g.text_context), (int32_t)g.text_causal, g.text_pool, i32(g.text_eos), g.activation, g.logit_scale, g.logit_bias};
+        const int expected = 12 * hp.num_hidden_layers + 6;
+        if ((int)g.tensors.size() != expected) return fail("model file has %d tensors, but %d tensors were expected", (int)g.tensors.size(), expected);
+        std::vector<vitb200_tensor> ts;
+        tensor_list(ts);
+        return create_text_impl(&hp, &ta, ts.data(), (int)ts.size(), device, max_batch, fp8, out);
+    }
     if (g.pre_norm != 0 && g.pre_norm != 1) return fail("invalid model file '%s' (vit.pre_norm %lld)", path, (long long)g.pre_norm);
     if (g.layer_scale != 0 && g.layer_scale != 1) return fail("invalid model file '%s' (vit.layer_scale %lld)", path, (long long)g.layer_scale);
     if (g.reg_tokens < 0 || g.reg_tokens > VB_MAX_REG_TOKENS)
@@ -2663,15 +2959,8 @@ static int create_from_file(const char *path, int device, int max_batch, int hea
     const int expected = 4 + 12 * hp.num_hidden_layers + 4 + 2 * arch.pre_norm + 2 * hp.num_hidden_layers * arch.layer_scale + (arch.reg_tokens > 0) -
                          (arch.pool >= 2) + (arch.pool == 2 ? kPoolTensorCount : 0);
     if ((int)g.tensors.size() != expected) return fail("model file has %d tensors, but %d tensors were expected", (int)g.tensors.size(), expected);
-    std::vector<vitb200_tensor> ts(g.tensors.size());
-    for (size_t i = 0; i < g.tensors.size(); ++i)
-    {
-        ts[i].name = g.tensors[i].name.c_str();
-        ts[i].data = buf.data() + g.tensors[i].offset;
-        ts[i].type = g.tensors[i].type;
-        ts[i].n_dims = g.tensors[i].n_dims;
-        for (int j = 0; j < 4; ++j) ts[i].ne[j] = g.tensors[i].ne[j];
-    }
+    std::vector<vitb200_tensor> ts;
+    tensor_list(ts);
     const vitb200_image_proc proc{i32(g.ip_shortest_edge), i32(g.ip_height), i32(g.ip_width), i32(g.ip_crop_height), i32(g.ip_crop_width),
                                   i32(g.ip_resample), g.ip_rescale_factor, {g.ip_mean[0], g.ip_mean[1], g.ip_mean[2]},
                                   {g.ip_std[0], g.ip_std[1], g.ip_std[2]}};

@@ -15,6 +15,10 @@
 //              "mean": SigLIP, no class token, the head reads the attention-pooling head's output or the mean of the tokens)
 //     vit.image_proc.shortest_edge, .height, .width, .crop_height, .crop_width, .resample (integers), .rescale_factor (float64),
 //     vit.image_proc.image_mean, .image_std (arrays of 3 float32): Hugging Face's image preprocessing (vitb200_image_proc), optional
+//     vit.text.context_length (integer): the file is a CLIP or SigLIP text tower (vitb200_text_arch), with vit.text.causal (bool or
+//              integer), vit.text.pool ("eos", "eos_argmax" or "last"), vit.text.eos_token_id (integer) and optionally
+//              vit.text.logit_scale / vit.text.logit_bias (float32); it carries no image key (patch_size, image_size, pre_norm, layer_scale,
+//              reg_tokens, pool, image_proc.*), and no other vit.text.* key
 // Layout (gguf.md): header {magic "GGUF", u32 version, u64 n_tensors, u64 n_kv}, n_kv x {string key, u32 type, value},
 // n_tensors x {string name, u32 n_dims, u64 ne[n_dims], u32 type, u64 offset}, padding to the alignment, tensor data (offsets
 // relative to the start of the data section).  Strings are {u64 length, bytes}.
@@ -49,6 +53,13 @@ struct GgufModel
     int64_t ip_shortest_edge = 0, ip_height = 0, ip_width = 0, ip_crop_height = 0, ip_crop_width = 0, ip_resample = 0;
     double ip_rescale_factor = 0.0;
     float ip_mean[3] = {0, 0, 0}, ip_std[3] = {0, 0, 0};
+    // vit.text.* (vitb200_text_arch; the loader checks the values): text once vit.text.context_length is present.  image_key: the first
+    // image-only key seen, which a text file must not have
+    bool text = false;
+    int64_t text_context = 0, text_causal = 0, text_eos = 0;
+    int32_t text_pool = 0;
+    float logit_scale = __builtin_nanf(""), logit_bias = __builtin_nanf("");
+    std::string image_key;
     std::map<int, std::string> labels;
     std::vector<GgufTensor> tensors;
     std::string error;
@@ -104,6 +115,14 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             std::string v;
             if (!rd_str(v)) return fail("truncated GGUF string value");
             if (key == "general.architecture") arch = v;
+            else if (key == "vit.text.pool")
+            {
+                if (v == "eos") m.text_pool = 0;
+                else if (v == "eos_argmax") m.text_pool = 1;
+                else if (v == "last") m.text_pool = 2;
+                else return fail("unknown vit.text.pool '" + v + "' (eos, eos_argmax or last)");
+            }
+            else if (key.compare(0, 9, "vit.text.") == 0) return fail("unknown key " + key + " (or not a string)");
             else if (key == "vit.activation")
             {
                 if (v == "gelu_tanh") m.activation = 0;
@@ -115,6 +134,7 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             }
             else if (key == "vit.pool")
             {
+                if (m.image_key.empty()) m.image_key = key;
                 if (v == "token") m.pool = 0;
                 else if (v == "cls_patch_mean") m.pool = 1;
                 else if (v == "map") m.pool = 2;
@@ -133,9 +153,10 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
                 if (et != 6 || cnt != 3) return fail(key + " must be an array of 3 float32");
                 if (!rd(f3, 12)) return fail("truncated GGUF array");
                 m.has_image_proc = true;
+                if (m.image_key.empty()) m.image_key = key;
                 continue;
             }
-            if (key.compare(0, 15, "vit.image_proc.") == 0) return fail("unknown key " + key);
+            if (key.compare(0, 15, "vit.image_proc.") == 0 || key.compare(0, 9, "vit.text.") == 0) return fail("unknown key " + key);
             for (uint64_t j = 0; j < cnt; ++j)
             {
                 if (et == 8)
@@ -172,6 +193,9 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             case 12: memcpy(&fv, raw, 8); iv = (int64_t)fv; break;
             }
             if (vt != 6 && vt != 12) fv = (double)iv;
+            const bool image_only = key == "vit.patch_size" || key == "vit.image_size" || key == "vit.img_size" || key == "vit.pre_norm" ||
+                                    key == "vit.layer_scale" || key == "vit.reg_tokens" || key.compare(0, 15, "vit.image_proc.") == 0;
+            if (image_only && m.image_key.empty()) m.image_key = key;
             if (key == "general.alignment") alignment = (uint64_t)iv;
             else if (key == "general.file_type") m.ftype = iv;
             else if (key == "vit.hidden_size") m.hidden_size = iv;
@@ -184,6 +208,16 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
             else if (key == "vit.pre_norm") m.pre_norm = iv;
             else if (key == "vit.layer_scale") m.layer_scale = iv;
             else if (key == "vit.reg_tokens") m.reg_tokens = iv;
+            else if (key.compare(0, 9, "vit.text.") == 0)
+            {
+                const std::string f = key.substr(9);
+                if (f == "context_length") { m.text_context = iv; m.text = true; }
+                else if (f == "causal") m.text_causal = iv;
+                else if (f == "eos_token_id") m.text_eos = iv;
+                else if ((f == "logit_scale" || f == "logit_bias") && vt == 6) (f == "logit_scale" ? m.logit_scale : m.logit_bias) = (float)fv;
+                else if (f == "logit_scale" || f == "logit_bias") return fail(key + " must be float32");
+                else return fail("unknown key " + key);
+            }
             else if (key.compare(0, 15, "vit.image_proc.") == 0)
             {
                 const std::string f = key.substr(15);
@@ -199,7 +233,9 @@ inline bool parse_gguf(const char *buf, size_t size, GgufModel &m)
     }
     if (!arch.empty() && arch != "vit") return fail("GGUF architecture is '" + arch + "', expected 'vit'");
     if (alignment < 8 || alignment % 8 != 0 || alignment > (1u << 20)) return fail("bad general.alignment");
-    if (m.hidden_size <= 0 || m.num_hidden_layers <= 0 || m.num_attention_heads <= 0 || m.num_classes <= 0 || m.patch_size <= 0 || m.img_size <= 0)
+    if (m.text && !m.image_key.empty()) return fail("a text tower (vit.text.context_length) must not carry the image key " + m.image_key);
+    if (m.hidden_size <= 0 || m.num_hidden_layers <= 0 || m.num_attention_heads <= 0 || m.num_classes <= 0 ||
+        (!m.text && (m.patch_size <= 0 || m.img_size <= 0)))
         return fail("GGUF file lacks the vit.* hyper-parameter keys");
 
     m.tensors.resize((size_t)n_tensors);

@@ -5,6 +5,8 @@
 //   cls_patch_mean_kernel    DINOv2's classifier input: LN(token 0) || the mean of LN(patch rows), one CTA per image; without a class
 //                            token (SigLIP) the mean alone
 //   attention_pool_kernel    SigLIP's attention-pooling head: one learned query attending over an image's token rows, per head
+//   token_embed_kernel       text towers: token rows = the token table's row of each id + pos_embed, replacing the patch embedding
+//   text_pool_kernel         text towers: the pooled row of each sequence (CLIP's EOS row, SigLIP's last row) through the final LayerNorm
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
 //                            and un-normalised forms write the encoder features (vitb200_features), its e4m3 form the FP8 A operand
 //   layernorm_inplace_kernel the same arithmetic in place on f32 rows (the pre-norm of CLIP towers)
@@ -403,6 +405,81 @@ cls_patch_mean_kernel(const float *__restrict__ x, int ntok, int first_patch, co
 #pragma unroll
         for (int k = 1; k < POOL_WARPS; ++k) s = __fadd_rn(s, part[k * D + c]);
         yi[cls * D + c] = to_out<OutT>(__fdiv_rn(s, count));
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Text towers (vitb200_create_text): the token rows of sequence b are x[b N + t][:] = f32(tok[ids[b][t]][:]) + pos[t][:], tok the f16
+// token table [V][D].  A sequence holding an id outside [0, V) gets NaN in every one of its rows and the table is not read for it, so
+// no batch mate changes.  One CTA per (position, sequence): it first checks the sequence's N ids, then writes its row 4 columns per
+// thread.  D % 4 == 0.
+constexpr int TOKEN_EMBED_THREADS = 128;
+
+__global__ void __launch_bounds__(TOKEN_EMBED_THREADS)
+token_embed_kernel(const int32_t *__restrict__ ids, const __half *__restrict__ tok, const float *__restrict__ pos, float *__restrict__ x,
+                   int N, int D, int V)
+{
+    const int t = blockIdx.x, b = blockIdx.y;
+    const int32_t *seq = ids + (size_t)b * N;
+    int bad = 0;
+    for (int i = threadIdx.x; i < N; i += TOKEN_EMBED_THREADS) bad |= seq[i] < 0 || seq[i] >= V;
+    bad = __syncthreads_or(bad);
+    const int id = seq[t];
+    float4 *xr = reinterpret_cast<float4 *>(x + ((size_t)b * N + t) * D);
+    const float4 *pr = reinterpret_cast<const float4 *>(pos + (size_t)t * D);
+    const uint2 *tr = reinterpret_cast<const uint2 *>(tok + (size_t)(bad ? 0 : id) * D);
+    for (int c = threadIdx.x; c < D / 4; c += TOKEN_EMBED_THREADS)
+    {
+        if (bad) { xr[c] = make_float4(NAN, NAN, NAN, NAN); continue; }
+        const uint2 u = __ldg(tr + c);
+        const float4 p = __ldg(pr + c);
+        const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&u.x)), e = __half22float2(*reinterpret_cast<const __half2 *>(&u.y));
+        xr[c] = make_float4(__fadd_rn(a.x, p.x), __fadd_rn(a.y, p.y), __fadd_rn(e.x, p.z), __fadd_rn(e.y, p.w));
+    }
+}
+
+// Text towers: one warp per sequence picks the pooled row of its N ids and writes it through the final LayerNorm (the arithmetic of
+// layernorm_row_regs) as the head's f16 A operand y [B][D].  pool 0: the first position whose id is eos, row 0 when there is none;
+// 1: the first position of the largest id; 2: row N - 1 (vitb200_text_arch.pool).  Ties go to the first position, as torch's argmax.
+constexpr int TEXT_POOL_WARPS = 4;
+
+template <int MAXV>
+__global__ void __launch_bounds__(TEXT_POOL_WARPS * 32)
+text_pool_kernel(const float *__restrict__ x, const int32_t *__restrict__ ids, int B, int N, int pool, int eos, const float *__restrict__ w,
+                 const float *__restrict__ b, __half *__restrict__ y, int D, float eps)
+{
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
+    const int seq = blockIdx.x * TEXT_POOL_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (seq >= B) return;
+    const int32_t *s = ids + (size_t)seq * N;
+    // (key, position) of this lane's best candidate; a smaller key wins, then the smaller position
+    constexpr long long kNone = 0x7fffffffffffffffll;
+    long long best = kNone;
+    for (int t = lane; t < N; t += 32)
+    {
+        const long long pos = t;
+        if (pool == 0 && s[t] == eos) best = min(best, pos);
+        else if (pool == 1) best = min(best, ((0x7fffffffll - max(s[t], 0)) << 32) | pos); // the largest id first
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+    const int row = pool == 2 ? N - 1 : best == kNone ? 0 : (int)(best & 0xffffffffll);
+    float4 o[MAXV];
+    layernorm_row_regs<MAXV, true>(x + ((size_t)seq * N + row) * D, w, b, D, eps, lane, o);
+    __half *yr = y + (size_t)seq * D;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j)
+    {
+        const int i = lane + 32 * j;
+        if (i < (D >> 2))
+        {
+            const __half2 h0 = __floats2half2_rn(o[j].x, o[j].y), h1 = __floats2half2_rn(o[j].z, o[j].w);
+            uint2 u;
+            u.x = *reinterpret_cast<const uint32_t *>(&h0);
+            u.y = *reinterpret_cast<const uint32_t *>(&h1);
+            reinterpret_cast<uint2 *>(yr)[i] = u;
+        }
     }
 }
 

@@ -17,7 +17,7 @@ from typing import Optional
 import numpy as np
 
 from .ggml_file import ARCH_ACTIVATIONS, PATCH_ONLY_POOLS, POOLS  # vitb200_arch.activation / .pool -> name (GGUF vit.activation / vit.pool)
-from .ggml_file import IMAGE_PROC_FIELDS, image_proc_from_config
+from .ggml_file import IMAGE_PROC_FIELDS, TEXT_POOLS, image_proc_from_config
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvitb200.so")
@@ -46,6 +46,13 @@ class ImageProc(C.Structure):
     """vitb200_image_proc (include/vitb200.h): Hugging Face's image preprocessing for the u8 entry points."""
     _fields_ = [(n, C.c_int32) for n in IMAGE_PROC_FIELDS[:6]] + [("rescale_factor", C.c_double), ("mean", C.c_float * 3),
                                                                    ("std", C.c_float * 3)]
+
+
+class TextArch(C.Structure):
+    """vitb200_text_arch (include/vitb200.h): a CLIP or SigLIP text tower.  pool is an index into ggml_file.TEXT_POOLS, activation one
+    into ggml_file.ARCH_ACTIVATIONS; logit_scale / logit_bias are NaN when absent."""
+    _fields_ = [(n, C.c_int32) for n in ("context", "causal", "pool", "eos_token_id", "activation")] + [
+        ("logit_scale", C.c_float), ("logit_bias", C.c_float)]
 
 
 class Taps(C.Structure):
@@ -91,6 +98,11 @@ def lib():
         L.vitb200_mlp_dim.argtypes = [vp]
         L.vitb200_create_arch.argtypes = [vp, C.POINTER(Arch), vp, i32, i32, i32, i32, i32, C.POINTER(vp)]
         L.vitb200_get_arch.argtypes = [vp, C.POINTER(Arch)]
+        L.vitb200_create_text.argtypes = [vp, C.POINTER(TextArch), vp, i32, i32, i32, i32, C.POINTER(vp)]
+        L.vitb200_get_text_arch.argtypes = [vp, C.POINTER(TextArch)]
+        L.vitb200_encode_text.argtypes = [vp, vp, i32, vp, C.POINTER(FeaturesReq), vp]
+        L.vitb200_encode_text_device.argtypes = [vp, vp, i32, vp, C.POINTER(FeaturesReq), vp, vp]
+        L.vitb200_test_attention_hilo_causal.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_set_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
         L.vitb200_get_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
@@ -148,21 +160,31 @@ class VitModel:
         _check(lib().vitb200_get_hparams(self._h, C.byref(hp)), "vitb200_get_hparams")
         self.hparams = hp
         self.hidden_size, self.num_classes, self.img_size = hp.hidden_size, hp.num_classes, hp.img_size
-        self.n_tokens = (hp.img_size // hp.patch_size) ** 2 + 1
-        self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713)
+        self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713); 0 for a text tower
         self.head_tokens = lib().vitb200_head_tokens(self._h)  # classifier rows per image (1, or 25 for ViTSTR)
         self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
+        self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or SwiGLU's F
+        self._labels = None
+        ta = TextArch()
+        # a text tower (vitb200_create_text): text_arch as a dict of ggml_file.TEXT_FIELDS plus its activation; None for an image tower
+        self.text_arch = None
+        if self.in_chans == 0:
+            _check(lib().vitb200_get_text_arch(self._h, C.byref(ta)), "vitb200_get_text_arch")
+            nan = lambda x: None if x != x else float(x)
+            self.text_arch = {"context": ta.context, "causal": ta.causal, "pool": TEXT_POOLS[ta.pool], "eos_token_id": ta.eos_token_id,
+                              "activation": ARCH_ACTIVATIONS[ta.activation], "logit_scale": nan(ta.logit_scale), "logit_bias": nan(ta.logit_bias)}
+            self.n_tokens, self.embed_dim = ta.context, hp.num_classes
+            return
+        self.n_tokens = (hp.img_size // hp.patch_size) ** 2 + 1
         a = Arch()
         _check(lib().vitb200_get_arch(self._h, C.byref(a)), "vitb200_get_arch")
         # the architecture (vitb200_arch): {"pre_norm": bool, "activation": one of ARCH_ACTIVATIONS}; the reference's is (False, "gelu_tanh")
         self.arch = {"pre_norm": bool(a.pre_norm), "activation": ARCH_ACTIVATIONS[a.activation]}
-        self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or SwiGLU's F
         # DINOv2 (vitb200_arch): LayerScale on, register tokens (rows 1 .. reg_tokens of every image), the head's input (one of POOLS)
         self.layer_scale, self.reg_tokens, self.pool = bool(a.layer_scale), int(a.reg_tokens), POOLS[a.pool]
         self.n_tokens += self.reg_tokens
         if self.pool in PATCH_ONLY_POOLS:  # SigLIP: the token rows are the patch rows only
             self.n_tokens -= 1
-        self._labels = None
 
     @property
     def image_proc(self) -> Optional[dict]:
@@ -256,9 +278,17 @@ def vit_model_from_tensors(vf, device: int = 0, max_batch: int = 8, head_tokens:
             t.ne[i] = ne[i] if i < len(ne) else 1
     hp = Hparams(vf.hidden_size, vf.num_hidden_layers, vf.num_attention_heads, vf.num_classes, vf.patch_size, vf.img_size, vf.ftype, vf.eps)
     act = ARCH_ACTIVATIONS.index(vf.activation) if vf.activation in ARCH_ACTIVATIONS else -1  # an unknown name is refused by the engine
+    h = C.c_void_p()
+    if vf.text is not None:  # a text tower: vitb200_create_text
+        t = vf.text
+        nan = lambda x: float("nan") if x is None else float(x)
+        ta = TextArch(int(t["context"]), int(t["causal"]), TEXT_POOLS.index(t["pool"]) if t["pool"] in TEXT_POOLS else -1,
+                      int(t["eos_token_id"]), act, nan(t.get("logit_scale")), nan(t.get("logit_bias")))
+        _check(lib().vitb200_create_text(C.byref(hp), C.byref(ta), ts, len(entries), device, max_batch, int(fp8), C.byref(h)),
+               "vitb200_create_text")
+        return VitModel(h, device, max_batch)
     pool = POOLS.index(vf.pool) if vf.pool in POOLS else -1  # likewise
     arch = Arch(int(vf.pre_norm), act, int(vf.layer_scale), int(vf.reg_tokens), pool)
-    h = C.c_void_p()
     _check(lib().vitb200_create_arch(C.byref(hp), C.byref(arch), ts, len(entries), device, max_batch, head_tokens, int(fp8), C.byref(h)),
            "vitb200_create")
     model = VitModel(h, device, max_batch)
@@ -431,6 +461,44 @@ def vit_features_u8(model: VitModel, images_u8, bilinear: bool = False, layers=N
         lib().vitb200_features_u8(model.handle, ptrs, nx, ny, B, int(bilinear), req, t, p), "vit_features_u8"))
 
 
+def _text_call(model: VitModel, B: int, layers, norm: bool, tokens: bool, embeds: bool, dtype, call):
+    key = dtype if isinstance(dtype, str) else np.dtype(dtype)
+    if key not in _FEATURE_DTYPES:
+        raise ValueError(f"dtype must be float32, float16 or {BFLOAT16!r}, not {dtype!r}")
+    code, np_type = _FEATURE_DTYPES[key]
+    req = FeaturesReq(model.hparams.num_hidden_layers if layers is None else int(layers), int(bool(norm)), code)
+    tok = np.empty((B, model.n_tokens, model.hidden_size), np_type) if tokens else None
+    emb = np.empty((B, model.embed_dim), np.float32) if embeds else None
+    call(emb.ctypes.data if emb is not None else None, C.byref(req), tok.ctypes.data if tok is not None else None)
+    return emb, tok
+
+
+def vit_encode_text(model: VitModel, ids, layers=None, norm: bool = True, tokens: bool = False, embeds: bool = True, dtype=np.float32):
+    """A text tower on token ids (vitb200_encode_text): ids int [B, N] (or [N]) from the model's Hugging Face tokenizer, padded to the
+    context length N.  Returns (embeds float32 [B, E], tokens [B, N, D]), None for an output not asked for: embeds are HF's text_embeds
+    (pooler_output for CLIPTextModel); tokens the residual stream after `layers` blocks (None = all), through the final LayerNorm when
+    `norm` (layers = L - 1, norm = False: hidden_states[-2]), as float32, float16 or BFLOAT16 (uint16 bit patterns).  An id outside the
+    vocabulary is refused."""
+    x = np.ascontiguousarray(ids, np.int32)
+    if x.ndim == 1:
+        x = x[None]
+    if x.ndim != 2 or x.shape[1] != model.n_tokens:
+        raise ValueError(f"ids must be [batch, {model.n_tokens}] (padded to the context length), not {list(x.shape)}")
+    return _text_call(model, x.shape[0], layers, norm, tokens, embeds, dtype, lambda e, req, t: _check(
+        lib().vitb200_encode_text(model.handle, x.ctypes.data, x.shape[0], e, req, t), "vit_encode_text"))
+
+
+def zero_shot_logits(image_embeds, text_embeds, logit_scale: float, logit_bias: Optional[float] = None) -> np.ndarray:
+    """Hugging Face's logits_per_image on the host: both embeddings L2-normalised, exp(logit_scale) * img @ txt.T, + logit_bias for
+    SigLIP.  image_embeds [I, E], text_embeds [T, E] -> [I, T] (float64)."""
+    img = np.asarray(image_embeds, np.float64)
+    txt = np.asarray(text_embeds, np.float64)
+    img = img / np.linalg.norm(img, axis=-1, keepdims=True)
+    txt = txt / np.linalg.norm(txt, axis=-1, keepdims=True)
+    logits = np.exp(logit_scale) * img @ txt.T
+    return logits if logit_bias is None else logits + logit_bias
+
+
 TAP_SHAPES = {
     "embed": lambda B, N, D: (B, N, D), "ln1": lambda B, N, D: (B, N, D), "qkv": lambda B, N, D: (B, N, 3 * D),
     "attn": lambda B, N, D: (B, N, D), "x1": lambda B, N, D: (B, N, D), "ln2": lambda B, N, D: (B, N, D),
@@ -492,6 +560,15 @@ def test_attention_hilo(qkv32: np.ndarray, B: int, N: int, H: int, device: int =
     out = np.empty((B * N, H * 64), np.float32)
     _check(lib().vitb200_test_attention_hilo(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
            "vitb200_test_attention_hilo")
+    return out
+
+
+def test_attention_hilo_causal(qkv32: np.ndarray, B: int, N: int, H: int, device: int = 0) -> np.ndarray:
+    """test_attention_hilo with CLIP's causal mask (vitb200_test_attention_hilo_causal): query t attends to keys 0 .. t."""
+    hi, lo = split_hi_lo(np.asarray(qkv32, np.float32).reshape(B * N, 3 * H * 64))
+    out = np.empty((B * N, H * 64), np.float32)
+    _check(lib().vitb200_test_attention_hilo_causal(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
+           "vitb200_test_attention_hilo_causal")
     return out
 
 

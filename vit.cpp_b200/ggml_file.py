@@ -36,6 +36,11 @@ ARCH_ACTIVATIONS = ACTIVATIONS + ("swiglu",)
 POOLS = ("token", "cls_patch_mean", "map", "mean")
 # pools whose token rows are the patch rows only
 PATCH_ONLY_POOLS = ("map", "mean")
+# text towers' pooled row, in the order of vitb200_text_arch.pool: the first EOS id (row 0 without one), the first largest id (HF CLIP
+# configs with eos_token_id 2), the last row (SigLIP)
+TEXT_POOLS = ("eos", "eos_argmax", "last")
+# vitb200_text_arch's fields besides the activation (GGUF keys vit.text.<field>, context as vit.text.context_length)
+TEXT_FIELDS = ("context", "causal", "pool", "eos_token_id", "logit_scale", "logit_bias")
 
 CONFIGS = {
     # name: (hidden, layers, heads, patch, img)
@@ -90,9 +95,14 @@ class VitFile:
     pool: str = "token"          # head input: one of POOLS
     # Hugging Face image preprocessing for the u8 entry points (GGUF keys vit.image_proc.*): a dict with the IMAGE_PROC_FIELDS, or None
     image_proc: Optional[dict] = None
+    # a CLIP or SigLIP text tower (GGUF keys vit.text.*): a dict with the TEXT_FIELDS (pool one of TEXT_POOLS, logit_scale / logit_bias a
+    # float or None), or None for an image tower.  Its patch_size and img_size are 0
+    text: Optional[dict] = None
 
     @property
     def n_tokens(self) -> int:
+        if self.text is not None:
+            return int(self.text["context"])
         g = self.img_size // self.patch_size
         return g * g if self.pool in PATCH_ONLY_POOLS else g * g + 1 + self.reg_tokens
 
@@ -393,10 +403,23 @@ def write_gguf(path: str, vf: VitFile, weight_type: str = "keep", alignment: int
     kv.append(gstr(b"general.architecture") + struct.pack("<I", _GGUF_STR) + gstr(b"vit"))
     kv_u32("general.alignment", alignment)
     kv_u32("general.file_type", vf.ftype)
+    text = vf.text
+    if text is not None and (vf.pre_norm or vf.layer_scale or vf.reg_tokens or vf.pool != "token" or vf.image_proc is not None):
+        raise ValueError("write_gguf: a text tower has no pre-norm, LayerScale, registers, image pool or image processor")
     for k, v in (("vit.hidden_size", vf.hidden_size), ("vit.num_hidden_layers", vf.num_hidden_layers),
-                 ("vit.num_attention_heads", vf.num_attention_heads), ("vit.num_classes", vf.num_classes),
-                 ("vit.patch_size", vf.patch_size), ("vit.image_size", vf.img_size)):
+                 ("vit.num_attention_heads", vf.num_attention_heads), ("vit.num_classes", vf.num_classes)) + (
+                 () if text is not None else (("vit.patch_size", vf.patch_size), ("vit.image_size", vf.img_size))):
         kv_u32(k, v)
+    if text is not None:
+        if text["pool"] not in TEXT_POOLS:
+            raise ValueError(f"write_gguf: unknown text pool {text['pool']!r} ({', '.join(TEXT_POOLS)})")
+        kv_u32("vit.text.context_length", int(text["context"]))
+        kv_u32("vit.text.causal", int(text["causal"]))
+        kv.append(gstr(b"vit.text.pool") + struct.pack("<I", _GGUF_STR) + gstr(text["pool"].encode()))
+        kv.append(gstr(b"vit.text.eos_token_id") + struct.pack("<Ii", _GGUF_I32, int(text["eos_token_id"])))
+        for k in ("logit_scale", "logit_bias"):
+            if text.get(k) is not None:
+                kv.append(gstr(("vit.text." + k).encode()) + struct.pack("<If", _GGUF_F32, float(text[k])))
     kv.append(gstr(b"vit.layer_norm_eps") + struct.pack("<If", _GGUF_F32, vf.eps))
     # the architecture keys only when they differ from the reference's values, so that a reference-architecture file is unchanged
     if vf.pre_norm:
@@ -491,7 +514,11 @@ def read_gguf(path: str) -> VitFile:
         else:
             kv[key] = rd(scalar[vt])
     vf = VitFile(kv["vit.hidden_size"], kv["vit.num_hidden_layers"], kv["vit.num_attention_heads"], kv["vit.num_classes"],
-                 kv["vit.patch_size"], kv.get("vit.image_size", kv.get("vit.img_size")), kv.get("general.file_type", 1))
+                 kv.get("vit.patch_size", 0), kv.get("vit.image_size", kv.get("vit.img_size", 0)), kv.get("general.file_type", 1))
+    if "vit.text.context_length" in kv:
+        vf.text = {"context": kv["vit.text.context_length"], "causal": int(kv.get("vit.text.causal", 0)),
+                   "pool": kv.get("vit.text.pool", "eos"), "eos_token_id": kv.get("vit.text.eos_token_id", 0),
+                   "logit_scale": kv.get("vit.text.logit_scale"), "logit_bias": kv.get("vit.text.logit_bias")}
     vf.id2label = dict(enumerate(kv.get("vit.id2label", [])))
     vf.eps = kv.get("vit.layer_norm_eps", 1e-6)
     vf.pre_norm = int(kv.get("vit.pre_norm", 0))
