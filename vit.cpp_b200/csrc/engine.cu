@@ -715,19 +715,26 @@ constexpr int VB_MAX_REG_TOKENS = 16;
 // Token rows in front of an image's patch rows: the class token and the registers, or none with SigLIP's pools (vitb200_arch.pool 2, 3)
 int prefix_rows(const vitb200_arch &a) { return a.pool >= 2 ? 0 : 1 + a.reg_tokens; }
 
-template <typename OutT, bool NORM>
-int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
-                          cudaStream_t s, int rows_per_group, size_t group_stride, float *y_scale = nullptr)
+// Launches kernel(std::integral_constant<int, MAXV>), a kernel holding rows in registers, MAXV = 4, 8 or LN_ROWS_MAX_V as D needs
+template <class Kernel, typename... Args>
+int launch_rows_kernel(vitb200_engine *e, Kernel kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args &&...args)
 {
     const int D = e->hp.hidden_size;
     if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
+    const auto kern = D <= 4 * 128 ? kernel(std::integral_constant<int, 4>())
+                    : D <= 8 * 128 ? kernel(std::integral_constant<int, 8>()) : kernel(std::integral_constant<int, LN_ROWS_MAX_V>());
+    return launch(e, kern, grid, block, smem, s, LAUNCH_PDL, std::forward<Args>(args)...);
+}
+
+template <bool NORM, typename OutT>
+int launch_layernorm_rows(vitb200_engine *e, const float *x, size_t x_row_stride, const float *w, const float *b, OutT *y, int rows,
+                          cudaStream_t s, int rows_per_group, size_t group_stride, float *y_scale = nullptr)
+{
     if (rows_per_group <= 0) rows_per_group = rows > 0 ? rows : 1; // one group: plain consecutive rows
     const int threads = 256, rows_per_block = threads / 32;
     const int blocks = (rows + rows_per_block - 1) / rows_per_block;
-    const auto kern = D <= 4 * 128 ? layernorm_f16_kernel<4, OutT, NORM>
-                    : D <= 8 * 128 ? layernorm_f16_kernel<8, OutT, NORM> : layernorm_f16_kernel<LN_ROWS_MAX_V, OutT, NORM>;
-    return launch(e, kern, dim3(blocks), dim3(threads), 0, s, LAUNCH_PDL, x, x_row_stride, rows_per_group, group_stride, w, b, y, rows, D,
-                  e->hp.eps, y_scale);
+    return launch_rows_kernel(e, [](auto V) { return layernorm_f16_kernel<V(), OutT, NORM>; }, dim3(blocks), dim3(threads), 0, s, x, x_row_stride,
+                              rows_per_group, group_stride, w, b, y, rows, e->hp.hidden_size, e->hp.eps, y_scale);
 }
 
 // OutT = __half: the f16 A operand; __nv_fp8_e4m3: the FP8 engine's e4m3 A operand and its row scales y_scale
@@ -749,30 +756,25 @@ int launch_layernorm(vitb200_engine *e, const float *x, size_t x_row_stride, con
                                  layernorm_tma_kernel<5, OutT>, layernorm_tma_kernel<6, OutT>, layernorm_tma_kernel<7, OutT>, layernorm_tma_kernel<8, OutT>};
         return launch(e, kernels[D / 128 - 1], dim3(grid), dim3(LN_TMA_THREADS), (size_t)smem, s, LAUNCH_PDL, x, w, b, y, rows, e->hp.eps, y_scale);
     }
-    return launch_layernorm_rows<OutT, true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride, y_scale);
+    return launch_layernorm_rows<true>(e, x, x_row_stride, w, b, y, rows, s, rows_per_group, group_stride, y_scale);
 }
 
 // The pre-norm: the row-per-warp LayerNorm in place on `rows` consecutive f32 rows of x
 int launch_layernorm_inplace(vitb200_engine *e, float *x, const float *w, const float *b, int rows, cudaStream_t s)
 {
-    const int D = e->hp.hidden_size;
-    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     const int threads = 256, blocks = (rows + threads / 32 - 1) / (threads / 32);
-    const auto kern = D <= 4 * 128 ? layernorm_inplace_kernel<4> : D <= 8 * 128 ? layernorm_inplace_kernel<8> : layernorm_inplace_kernel<LN_ROWS_MAX_V>;
-    return launch(e, kern, dim3(blocks), dim3(threads), 0, s, LAUNCH_PDL, x, w, b, rows, D, e->hp.eps);
+    return launch_rows_kernel(e, [](auto V) { return layernorm_inplace_kernel<V()>; }, dim3(blocks), dim3(threads), 0, s, x, w, b, rows,
+                              e->hp.hidden_size, e->hp.eps);
 }
 
 // DINOv2's classifier input (vitb200_arch.pool = 1): per image, [LN(token 0) || mean of LN(patch rows)] into y [B][2 D] (NORM = false:
 // the rows as they are), rows 1 .. reg_tokens left out.  SigLIP's (pool = 3, no class token): the mean of LN(every row) into y [B][D]
-template <typename OutT, bool NORM>
+template <bool NORM, typename OutT>
 int launch_pool(vitb200_engine *e, OutT *y, int B, cudaStream_t s)
 {
     const int D = e->hp.hidden_size;
-    if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
-    const auto kern = D <= 4 * 128 ? cls_patch_mean_kernel<4, OutT, NORM>
-                    : D <= 8 * 128 ? cls_patch_mean_kernel<8, OutT, NORM> : cls_patch_mean_kernel<LN_ROWS_MAX_V, OutT, NORM>;
-    return launch(e, kern, dim3(B), dim3(POOL_WARPS * 32), (size_t)POOL_WARPS * D * sizeof(float), s, LAUNCH_PDL, e->X, e->N,
-                  prefix_rows(e->arch), e->norm_w, e->norm_b, y, D, e->hp.eps);
+    return launch_rows_kernel(e, [](auto V) { return cls_patch_mean_kernel<V(), OutT, NORM>; }, dim3(B), dim3(POOL_WARPS * 32),
+                              (size_t)POOL_WARPS * D * sizeof(float), s, e->X, e->N, prefix_rows(e->arch), e->norm_w, e->norm_b, y, D, e->hp.eps);
 }
 
 // The fc1 epilogue of the model's MLP activation (vitb200_arch.activation)
@@ -1065,7 +1067,7 @@ int run_map_head(vitb200_engine *e, int B, cudaStream_t s)
     }
     {
         ProfScope ps(e, PK_LN, 0.0, s);
-        if (launch_layernorm_rows<__half, true>(e, e->POOL32, (size_t)D, e->pool_nw, e->pool_nb, e->A16, B, s, 0, 0)) return 1;
+        if (launch_layernorm_rows<true>(e, e->POOL32, (size_t)D, e->pool_nw, e->pool_nb, e->A16, B, s, 0, 0)) return 1;
     }
     GemmParams f1{};
     f1.M = B; f1.N = 4 * D; f1.K = D; f1.bias = e->pool_fc1.b; f1.out = e->H16; f1.ldo = 4 * D;
@@ -1094,9 +1096,9 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     {
         if (run_map_head(e, B, s)) return 1;
         ProfScope ps(e, PK_POOL, 0.0, s);
-        if (launch_layernorm_rows<__half, false>(e, e->POOL32, (size_t)D, nullptr, nullptr, e->CLS16, B, s, 0, 0)) return 1;
+        if (launch_layernorm_rows<false>(e, e->POOL32, (size_t)D, nullptr, nullptr, e->CLS16, B, s, 0, 0)) return 1;
     }
-    else if (e->arch.pool ? launch_pool<__half, true>(e, e->CLS16, B, s)
+    else if (e->arch.pool ? launch_pool<true>(e, e->CLS16, B, s)
                           : launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->CLS16, R, s, TH, (size_t)N * D))
         return 1;
     if (taps && tap_f16(taps->final_ln, e->CLS16, (size_t)R * e->KH, s)) return 1;
@@ -1116,6 +1118,17 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     return 0;
 }
 
+// run((OutT *)dst, std::integral_constant<bool, NORM>) for a features output: dtype 0 f32, 1 f16, 2 bf16, normalised or not
+template <class Run>
+int with_features_type(int dtype, bool norm, void *dst, Run run)
+{
+    auto typed = [&](auto *y) { return norm ? run(y, std::true_type()) : run(y, std::false_type()); };
+    if (dtype == 0) return typed((float *)dst);
+    if (dtype == 1) return typed((__half *)dst);
+    if (dtype == 2) return typed((__nv_bfloat16 *)dst);
+    return fail("features: dtype %d unknown", dtype);
+}
+
 // Encoder features (vitb200_features*): the encoder up to block req->layers, then the requested rows of the residual stream -- all T
 // token rows into d_tokens, the head_tokens pooled rows of every image into d_prelogits -- normalised with the final LayerNorm or not,
 // as f32 / f16 / bf16.  Device destinations; either may be NULL.  An un-normalised f32 output is a copy, every other one a kernel.
@@ -1125,24 +1138,18 @@ int emit_rows(vitb200_engine *e, const vitb200_features_req *req, void *dst, int
 {
     const int D = e->hp.hidden_size, N = e->N;
     if (!dst) return 0;
-    if (!req->norm && req->dtype == 0)
-    {
+    return with_features_type(req->dtype, req->norm, dst, [&](auto *y, auto norm) -> int {
+        if constexpr (norm() || !std::is_same<decltype(y), float *>::value)
+        {
+            ProfScope ps(e, PK_LN, 0.0, s);
+            return launch_layernorm_rows<norm()>(e, e->X, (size_t)D, norm() ? e->norm_w : nullptr, norm() ? e->norm_b : nullptr, y, rows, s,
+                                                 rows_per_group, (size_t)N * D);
+        }
         // [B][rows_per_group][D] out of [B][N][D]: one 2-D copy (the token rows are a single plain copy)
         const size_t w = (size_t)rows_per_group * D * sizeof(float);
         CUDA_TRY(cudaMemcpy2DAsync(dst, w, e->X, (size_t)N * D * sizeof(float), w, (size_t)rows / rows_per_group, cudaMemcpyDeviceToDevice, s));
         return 0;
-    }
-    ProfScope ps(e, PK_LN, 0.0, s);
-    const size_t gs = (size_t)N * D;
-    switch (req->dtype * 2 + (req->norm ? 1 : 0))
-    {
-    case 1: return launch_layernorm_rows<float, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (float *)dst, rows, s, rows_per_group, gs);
-    case 2: return launch_layernorm_rows<__half, false>(e, e->X, (size_t)D, nullptr, nullptr, (__half *)dst, rows, s, rows_per_group, gs);
-    case 3: return launch_layernorm_rows<__half, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__half *)dst, rows, s, rows_per_group, gs);
-    case 4: return launch_layernorm_rows<__nv_bfloat16, false>(e, e->X, (size_t)D, nullptr, nullptr, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
-    case 5: return launch_layernorm_rows<__nv_bfloat16, true>(e, e->X, (size_t)D, e->norm_w, e->norm_b, (__nv_bfloat16 *)dst, rows, s, rows_per_group, gs);
-    }
-    return fail("features: dtype %d unknown", req->dtype);
+    });
 }
 
 int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_features_req *req, void *d_tokens, void *d_prelogits, cudaStream_t s)
@@ -1157,10 +1164,13 @@ int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_
         if (run_map_head(e, B, s)) return 1;
         {
             ProfScope ps(e, PK_POOL, 0.0, s);
-            const size_t D_ = (size_t)D;
-            if (req->dtype == 0) CUDA_TRY(cudaMemcpyAsync(d_prelogits, e->POOL32, (size_t)B * D_ * sizeof(float), cudaMemcpyDeviceToDevice, s));
-            else if (req->dtype == 1 ? launch_layernorm_rows<__half, false>(e, e->POOL32, D_, nullptr, nullptr, (__half *)d_prelogits, B, s, 0, 0)
-                                     : launch_layernorm_rows<__nv_bfloat16, false>(e, e->POOL32, D_, nullptr, nullptr, (__nv_bfloat16 *)d_prelogits, B, s, 0, 0))
+            if (with_features_type(req->dtype, false, d_prelogits, [&](auto *y, auto) -> int {
+                    if constexpr (std::is_same<decltype(y), float *>::value)
+                        CUDA_TRY(cudaMemcpyAsync(d_prelogits, e->POOL32, (size_t)B * D * sizeof(float), cudaMemcpyDeviceToDevice, s));
+                    else
+                        return launch_layernorm_rows<false>(e, e->POOL32, (size_t)D, nullptr, nullptr, y, B, s, 0, 0);
+                    return 0;
+                }))
                 return 1;
         }
         return emit(d_tokens, B * N, N);
@@ -1170,16 +1180,7 @@ int run_features(vitb200_engine *e, const float *d_images, int B, const vitb200_
     {
         // DINOv2: [token 0 || mean of the patch rows] per image, through the final LayerNorm or not; SigLIP (pool = 3): the mean alone
         ProfScope ps(e, PK_LN, 0.0, s);
-        switch (req->dtype * 2 + (req->norm ? 1 : 0))
-        {
-        case 0: return launch_pool<float, false>(e, (float *)d_prelogits, B, s);
-        case 1: return launch_pool<float, true>(e, (float *)d_prelogits, B, s);
-        case 2: return launch_pool<__half, false>(e, (__half *)d_prelogits, B, s);
-        case 3: return launch_pool<__half, true>(e, (__half *)d_prelogits, B, s);
-        case 4: return launch_pool<__nv_bfloat16, false>(e, (__nv_bfloat16 *)d_prelogits, B, s);
-        case 5: return launch_pool<__nv_bfloat16, true>(e, (__nv_bfloat16 *)d_prelogits, B, s);
-        }
-        return fail("features: dtype %d unknown", req->dtype);
+        return with_features_type(req->dtype, req->norm, d_prelogits, [&](auto *y, auto norm) { return launch_pool<norm()>(e, y, B, s); });
     }
     return emit(d_prelogits, B * TH, TH);
 }
@@ -1267,9 +1268,9 @@ int run_text(vitb200_engine *e, const int32_t *d_ids, int B, float *d_embeds, co
     if (run_blocks(e, B, at, L, s, nullptr)) return 1;
     {
         ProfScope ps(e, PK_LN, 0.0, s);
-        const auto kern = D <= 4 * 128 ? text_pool_kernel<4> : D <= 8 * 128 ? text_pool_kernel<8> : text_pool_kernel<LN_ROWS_MAX_V>;
-        if (launch(e, kern, dim3((unsigned)((B + TEXT_POOL_WARPS - 1) / TEXT_POOL_WARPS)), dim3(TEXT_POOL_WARPS * 32), 0, s, LAUNCH_PDL, e->X, d_ids,
-                   B, N, e->text_arch.pool, e->text_arch.eos_token_id, e->norm_w, e->norm_b, e->CLS16, D, e->hp.eps))
+        if (launch_rows_kernel(e, [](auto V) { return text_pool_kernel<V()>; }, dim3((unsigned)((B + TEXT_POOL_WARPS - 1) / TEXT_POOL_WARPS)),
+                               dim3(TEXT_POOL_WARPS * 32), 0, s, e->X, d_ids, B, N, e->text_arch.pool, e->text_arch.eos_token_id, e->norm_w, e->norm_b,
+                               e->CLS16, D, e->hp.eps))
             return 1;
     }
     // rows of pitch Cp (E padded to 4) unless the caller's dense rows coincide, as the image head's logits
@@ -2763,7 +2764,7 @@ int vitb200_test_gemm_layer_scale(int device, int M, int N, int K, const uint16_
 int vitb200_test_layernorm(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, float *y)
 {
     return guarded(__func__, [&] {
-        if (!x || !w || !b || !y || rows < 1 || D < 4 || D % 4 != 0 || D > 2048) return fail("bad argument");
+        if (!x || !w || !b || !y || rows < 1 || D < 4 || D % 4 != 0 || D > LN_MAX_HIDDEN) return fail("bad argument");
         EnginePtr owner;
         __half *dy = nullptr;
         if (test_layernorm_impl(device, rows, D, x, w, b, eps, &dy, nullptr, owner)) return 1;
@@ -2797,7 +2798,7 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
 int vitb200_test_layernorm_fp8(int device, int rows, int D, const float *x, const float *w, const float *b, float eps, uint8_t *q, float *sa)
 {
     return guarded(__func__, [&]() -> int {
-        if (!x || !w || !b || !q || !sa || rows < 1 || D < 4 || D % 16 != 0 || D > 2048) return fail("bad argument");
+        if (!x || !w || !b || !q || !sa || rows < 1 || D < 4 || D % 16 != 0 || D > LN_MAX_HIDDEN) return fail("bad argument");
         EnginePtr owner;
         __nv_fp8_e4m3 *dq = nullptr;
         float *ds = nullptr;

@@ -113,6 +113,87 @@ __global__ void cls_rows_kernel(float *__restrict__ x, const float *__restrict__
 }
 
 // ------------------------------------------------------------------------------------------------
+// The LayerNorm arithmetic, written once for every LayerNorm kernel below: f32 mean and biased variance (the reference sums in
+// double; the difference is ~1e-7 relative), y = ((x - mean) * scale) * w + b as three separately rounded f32 ops like the reference's
+// NORM, MUL, ADD nodes, and the FP8 engine's per-row e4m3 quantisation of y.  A warp holds a row, float4 j of lane l being float4
+// l + 32 j of the row.
+
+// Butterfly reductions over the 32 lanes: every lane gets the result
+__device__ __forceinline__ float warp_sum(float v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+__device__ __forceinline__ float warp_max(float v)
+{
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+    return v;
+}
+
+// A lane's part of the row sum
+__device__ __forceinline__ float sum4(float4 v) { return (v.x + v.y) + (v.z + v.w); }
+
+// Centres the lane's float4 of the row (those with index < nvec) on the row mean, given the lane's part of the row sum, and returns
+// scale = 1 / sqrt(biased variance + eps)
+template <int MAXV>
+__device__ __forceinline__ float ln_center(float4 (&v)[MAXV], float sum, int lane, int nvec, int D, float eps)
+{
+    const float mean = warp_sum(sum) / (float)D;
+    float sq = 0.f;
+#pragma unroll
+    for (int j = 0; j < MAXV; ++j)
+    {
+        if (lane + 32 * j < nvec)
+        {
+            v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
+            sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
+        }
+    }
+    return 1.0f / sqrtf(warp_sum(sq) / (float)D + eps);
+}
+
+// The affine of a centred float4: (v * scale) * w + b, each op rounded
+__device__ __forceinline__ float4 ln_affine(float4 v, float scale, float4 w, float4 b)
+{
+    return make_float4(__fadd_rn(__fmul_rn(__fmul_rn(v.x, scale), w.x), b.x), __fadd_rn(__fmul_rn(__fmul_rn(v.y, scale), w.y), b.y),
+                       __fadd_rn(__fmul_rn(__fmul_rn(v.z, scale), w.z), b.z), __fadd_rn(__fmul_rn(__fmul_rn(v.w, scale), w.w), b.w));
+}
+
+// e4m3 rows: amax = max |y| over the row (abs_max4: a lane's part, then warp_max), the row's scale amax / 448 and
+// y = e4m3_rn_satfinite(y (448 / amax)); an all-zero row gets scale 1.  (The scale and the multiplier are two functions: one function
+// computing both changes the code the compiler generates for its callers.)
+__device__ __forceinline__ float abs_max4(float4 v) { return fmaxf(fmaxf(fabsf(v.x), fabsf(v.y)), fmaxf(fabsf(v.z), fabsf(v.w))); }
+__device__ __forceinline__ float e4m3_row_scale(float amax) { return amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f; }
+__device__ __forceinline__ float e4m3_multiplier(float amax) { return amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f; }
+
+__device__ __forceinline__ uint32_t e4m3x4(float4 v, float inv)
+{
+    return ptx::cvt_e4m3x4(__fmul_rn(v.x, inv), __fmul_rn(v.y, inv), __fmul_rn(v.z, inv), __fmul_rn(v.w, inv));
+}
+
+// Four f32 values rounded to nearest even f16 or bf16 (OutT), packed in order
+template <typename OutT>
+__device__ __forceinline__ uint2 pack4(float4 v)
+{
+    uint2 u;
+    if constexpr (std::is_same<OutT, __half>::value)
+    {
+        const __half2 h0 = __floats2half2_rn(v.x, v.y), h1 = __floats2half2_rn(v.z, v.w);
+        u.x = *reinterpret_cast<const uint32_t *>(&h0);
+        u.y = *reinterpret_cast<const uint32_t *>(&h1);
+    }
+    else
+    {
+        const __nv_bfloat162 h0 = __floats2bfloat162_rn(v.x, v.y), h1 = __floats2bfloat162_rn(v.z, v.w);
+        u.x = *reinterpret_cast<const uint32_t *>(&h0);
+        u.y = *reinterpret_cast<const uint32_t *>(&h1);
+    }
+    return u;
+}
+
 // Four f32 results -> OutT, stored at float4 index i of a row.  16-bit outputs pair up neighbouring lanes (lanes 2k and 2k+1 hold
 // consecutive float4 indices) so that the even lane issues one 16-byte store for both; `vec16` requires an even float4 count per row.
 // Every lane of the warp must call this (shuffles), `live` says whether its own index is inside the row.
@@ -125,19 +206,7 @@ __device__ __forceinline__ void store4(OutT *__restrict__ yr, int i, bool live, 
     }
     else
     {
-        uint2 u;
-        if constexpr (std::is_same<OutT, __half>::value)
-        {
-            const __half2 h0 = __floats2half2_rn(o0, o1), h1 = __floats2half2_rn(o2, o3);
-            u.x = *reinterpret_cast<const uint32_t *>(&h0);
-            u.y = *reinterpret_cast<const uint32_t *>(&h1);
-        }
-        else
-        {
-            const __nv_bfloat162 h0 = __floats2bfloat162_rn(o0, o1), h1 = __floats2bfloat162_rn(o2, o3);
-            u.x = *reinterpret_cast<const uint32_t *>(&h0);
-            u.y = *reinterpret_cast<const uint32_t *>(&h1);
-        }
+        const uint2 u = pack4<OutT>(make_float4(o0, o1, o2, o3));
         if (vec16)
         {
             const uint32_t nx = __shfl_xor_sync(0xffffffffu, u.x, 1), ny = __shfl_xor_sync(0xffffffffu, u.y, 1);
@@ -148,13 +217,10 @@ __device__ __forceinline__ void store4(OutT *__restrict__ yr, int i, bool live, 
     }
 }
 
-// One warp per row.  mean / biased variance in f32 (the reference sums in double; the difference is
-// ~1e-7 relative), then y = ((x-mean)*scale)*w + b as three separately rounded f32 ops like the
-// reference's NORM, MUL, ADD nodes, then RNE to f16 (the GEMM's src1 conversion, ggml.c:9493-9506).
-// OutT = float stores those f32 values before that rounding, __nv_bfloat16 rounds them to nearest even bf16 instead.
+// One warp per row: the LayerNorm above, then RNE to f16 (the GEMM's src1 conversion, ggml.c:9493-9506).
+// OutT = float stores the f32 values before that rounding, __nv_bfloat16 rounds them to nearest even bf16 instead.
 // NORM = false skips the normalisation: the selected rows of x are converted and stored as they are (w and b are not read).
-// OutT = __nv_fp8_e4m3 (FP8 engine, NORM only) quantises each row of those f32 values with its own scale: amax = max |y| over the row,
-// y_scale[row] = amax / 448 and y = e4m3_rn_satfinite(y (448 / amax)); an all-zero row gets scale 1.
+// OutT = __nv_fp8_e4m3 (FP8 engine, NORM only) quantises each row with its own scale, y_scale[row].
 // The body is a device function so that the in-place form below can run it with y == x: a warp holds its whole row in registers
 // before it writes any of it, and no two warps share a row.
 template <int MAXV, typename OutT, bool NORM>
@@ -183,31 +249,11 @@ __device__ __forceinline__ void layernorm_row_warp(const float *x, size_t x_row_
         if (i < nvec)
         {
             v[j] = xr[i];
-            sum += (v[j].x + v[j].y) + (v[j].z + v[j].w);
+            sum += sum4(v[j]);
         }
     }
     float scale = 1.f;
-    if constexpr (NORM)
-    {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-        const float mean = sum / (float)D;
-        float sq = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXV; ++j)
-        {
-            const int i = lane + 32 * j;
-            if (i < nvec)
-            {
-                v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
-                sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
-            }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-        const float var = sq / (float)D;
-        scale = 1.0f / sqrtf(var + eps);
-    }
+    if constexpr (NORM) scale = ln_center(v, sum, lane, nvec, D, eps);
     const float4 *w4 = reinterpret_cast<const float4 *>(w);
     const float4 *b4 = reinterpret_cast<const float4 *>(b);
     const bool vec16 = (nvec & 1) == 0;
@@ -217,42 +263,30 @@ __device__ __forceinline__ void layernorm_row_warp(const float *x, size_t x_row_
     for (int j = 0; j < MAXV; ++j)
     {
         const int i = lane + 32 * j;
-        float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f;
+        float o0 = 0.f, o1 = 0.f, o2 = 0.f, o3 = 0.f; // four floats, not a float4: that reorders the f16 / bf16 packing
         if (i < nvec)
         {
-            if constexpr (NORM)
-            {
-                const float4 ww = __ldg(w4 + i), bb = __ldg(b4 + i);
-                o0 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww.x), bb.x);
-                o1 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww.y), bb.y);
-                o2 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww.z), bb.z);
-                o3 = __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww.w), bb.w);
-            }
-            else
-            {
-                o0 = v[j].x; o1 = v[j].y; o2 = v[j].z; o3 = v[j].w;
-            }
+            float4 o = v[j];
+            if constexpr (NORM) o = ln_affine(v[j], scale, __ldg(w4 + i), __ldg(b4 + i));
+            o0 = o.x; o1 = o.y; o2 = o.z; o3 = o.w;
         }
         if constexpr (kE4M3)
         {
             v[j] = make_float4(o0, o1, o2, o3);
-            amax = fmaxf(amax, fmaxf(fmaxf(fabsf(o0), fabsf(o1)), fmaxf(fabsf(o2), fabsf(o3))));
+            amax = fmaxf(amax, abs_max4(v[j]));
         }
         else store4(yr, i, i < nvec, vec16, o0, o1, o2, o3);
     }
     if constexpr (kE4M3)
     {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-        const float inv = amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f;
-        if (lane == 0) y_scale[row] = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+        amax = warp_max(amax);
+        const float inv = e4m3_multiplier(amax);
+        if (lane == 0) y_scale[row] = e4m3_row_scale(amax);
 #pragma unroll
         for (int j = 0; j < MAXV; ++j)
         {
             const int i = lane + 32 * j;
-            if (i < nvec)
-                reinterpret_cast<uint32_t *>(yr)[i] =
-                    ptx::cvt_e4m3x4(__fmul_rn(v[j].x, inv), __fmul_rn(v[j].y, inv), __fmul_rn(v[j].z, inv), __fmul_rn(v[j].w, inv));
+            if (i < nvec) reinterpret_cast<uint32_t *>(yr)[i] = e4m3x4(v[j], inv);
         }
     }
 }
@@ -279,7 +313,7 @@ __global__ void layernorm_inplace_kernel(float *x, const float *__restrict__ w, 
 
 // ------------------------------------------------------------------------------------------------
 // DINOv2's classifier input (vitb200_arch.pool = 1): per image, y[0 .. D) = LN(token 0) and y[D .. 2 D) = the mean over the patch rows
-// first_patch .. ntok-1 of LN(row) (the register rows between them are left out), LN = the row-per-warp LayerNorm's arithmetic above
+// first_patch .. ntok-1 of LN(row) (the register rows between them are left out), LN = layernorm_row_regs
 // (NORM = false: the rows as they are).  first_patch = 0 (no class token, vitb200_arch.pool = 3): y[0 .. D) = the mean over all ntok rows,
 // rows of D.  One CTA of 8 warps per image: warp w normalises patch rows w, w + 8, ... and keeps its column
 // sums in registers in that order; the eight partial sums then meet in shared memory and are added warp 0 first, 7 last, and divided
@@ -296,8 +330,7 @@ __device__ __forceinline__ OutT to_out(float v)
     else return v;
 }
 
-// One row of D floats into a warp's registers, normalised as layernorm_row_warp normalises it (NORM = false: as it is): lane l holds
-// float4 l + 32 j of the row in o[j]
+// One row of D floats into a warp's registers, normalised (NORM = false: as it is): lane l holds float4 l + 32 j of the row in o[j]
 template <int MAXV, bool NORM>
 __device__ __forceinline__ void layernorm_row_regs(const float *__restrict__ xrow, const float *__restrict__ w, const float *__restrict__ b,
                                                    int D, float eps, int lane, float4 (&o)[MAXV])
@@ -313,42 +346,19 @@ __device__ __forceinline__ void layernorm_row_regs(const float *__restrict__ xro
         if (i < nvec)
         {
             o[j] = xr[i];
-            sum += (o[j].x + o[j].y) + (o[j].z + o[j].w);
+            sum += sum4(o[j]);
         }
     }
     if constexpr (NORM)
     {
-#pragma unroll
-        for (int s = 16; s > 0; s >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, s);
-        const float mean = sum / (float)D;
-        float sq = 0.f;
-#pragma unroll
-        for (int j = 0; j < MAXV; ++j)
-        {
-            const int i = lane + 32 * j;
-            if (i < nvec)
-            {
-                o[j].x -= mean; o[j].y -= mean; o[j].z -= mean; o[j].w -= mean;
-                sq += (o[j].x * o[j].x + o[j].y * o[j].y) + (o[j].z * o[j].z + o[j].w * o[j].w);
-            }
-        }
-#pragma unroll
-        for (int s = 16; s > 0; s >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, s);
-        const float scale = 1.0f / sqrtf(sq / (float)D + eps);
+        const float scale = ln_center(o, sum, lane, nvec, D, eps);
         const float4 *w4 = reinterpret_cast<const float4 *>(w);
         const float4 *b4 = reinterpret_cast<const float4 *>(b);
 #pragma unroll
         for (int j = 0; j < MAXV; ++j)
         {
             const int i = lane + 32 * j;
-            if (i < nvec)
-            {
-                const float4 ww = __ldg(w4 + i), bb = __ldg(b4 + i);
-                o[j].x = __fadd_rn(__fmul_rn(__fmul_rn(o[j].x, scale), ww.x), bb.x);
-                o[j].y = __fadd_rn(__fmul_rn(__fmul_rn(o[j].y, scale), ww.y), bb.y);
-                o[j].z = __fadd_rn(__fmul_rn(__fmul_rn(o[j].z, scale), ww.z), bb.z);
-                o[j].w = __fadd_rn(__fmul_rn(__fmul_rn(o[j].w, scale), ww.w), bb.w);
-            }
+            if (i < nvec) o[j] = ln_affine(o[j], scale, __ldg(w4 + i), __ldg(b4 + i));
         }
     }
 }
@@ -438,8 +448,8 @@ token_embed_kernel(const int32_t *__restrict__ ids, const __half *__restrict__ t
     }
 }
 
-// Text towers: one warp per sequence picks the pooled row of its N ids and writes it through the final LayerNorm (the arithmetic of
-// layernorm_row_regs) as the head's f16 A operand y [B][D].  pool 0: the first position whose id is eos, row 0 when there is none;
+// Text towers: one warp per sequence picks the pooled row of its N ids and writes it through the final LayerNorm (layernorm_row_regs)
+// as the head's f16 A operand y [B][D].  pool 0: the first position whose id is eos, row 0 when there is none;
 // 1: the first position of the largest id; 2: row N - 1 (vitb200_text_arch.pool).  Ties go to the first position, as torch's argmax.
 constexpr int TEXT_POOL_WARPS = 4;
 
@@ -472,14 +482,7 @@ text_pool_kernel(const float *__restrict__ x, const int32_t *__restrict__ ids, i
     for (int j = 0; j < MAXV; ++j)
     {
         const int i = lane + 32 * j;
-        if (i < (D >> 2))
-        {
-            const __half2 h0 = __floats2half2_rn(o[j].x, o[j].y), h1 = __floats2half2_rn(o[j].z, o[j].w);
-            uint2 u;
-            u.x = *reinterpret_cast<const uint32_t *>(&h0);
-            u.y = *reinterpret_cast<const uint32_t *>(&h1);
-            reinterpret_cast<uint2 *>(yr)[i] = u;
-        }
+        if (i < (D >> 2)) reinterpret_cast<uint2 *>(yr)[i] = pack4<__half>(o[j]);
     }
 }
 
@@ -579,11 +582,10 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
 // ------------------------------------------------------------------------------------------------
 // The same LayerNorm for the block LayerNorms (all T rows consecutive, D % 128 == 0, D <= 1024) as a PERSISTENT kernel on bulk copies:
 // CTAs (2 per SM) walk 8-row blocks of X (8 D floats = one contiguous run) last block first; warp 8 streams them into a 3-deep
-// shared-memory ring with cp.async.bulk + mbarrier, warps 0-7 each normalise one row out of shared memory (identical arithmetic to the
-// kernel above, w / b kept in registers for the whole launch) into a double-buffered staging block that leaves as ONE contiguous
-// bulk store of 8 f16 rows.  Purpose: the row-per-warp kernel above reaches 5.9 TB/s alone but 4.8 TB/s inside the step (6 304 short
-// blocks ramping up and draining between two persistent GEMMs).  OutT = __nv_fp8_e4m3: the FP8 engine's per-row quantisation, as
-// layernorm_f16_kernel does it; the row scales go straight to y_scale.
+// shared-memory ring with cp.async.bulk + mbarrier, warps 0-7 each normalise one row out of shared memory (w / b kept in registers for
+// the whole launch) into a double-buffered staging block that leaves as ONE contiguous bulk store of 8 f16 rows.  Purpose: the
+// row-per-warp kernel above reaches 5.9 TB/s alone but 4.8 TB/s inside the step (6 304 short blocks ramping up and draining between two
+// persistent GEMMs).  OutT = __nv_fp8_e4m3: the FP8 engine's per-row quantisation; the row scales go straight to y_scale.
 constexpr int LN_TMA_ROWS = 8, LN_TMA_STAGES = 3, LN_TMA_THREADS = 288;
 __host__ __device__ inline int layernorm_tma_smem_bytes(int D) { return 128 + LN_TMA_STAGES * LN_TMA_ROWS * D * 4 + 2 * LN_TMA_ROWS * D * 2 + 64; }
 
@@ -652,23 +654,11 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
             if (warp < nr)
             {
 #pragma unroll
-                for (int j = 0; j < NV; ++j) { v[j] = xr[lane + 32 * j]; sum += (v[j].x + v[j].y) + (v[j].z + v[j].w); }
+                for (int j = 0; j < NV; ++j) { v[j] = xr[lane + 32 * j]; sum += sum4(v[j]); }
             }
             __syncwarp();
             if (lane == 0) ptx::mbar_arrive(empty_bar(st)); // this row is in registers: the slot may be refilled once all eight have left it
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-            const float mean = sum / (float)D;
-            float sq = 0.f;
-#pragma unroll
-            for (int j = 0; j < NV; ++j)
-            {
-                v[j].x -= mean; v[j].y -= mean; v[j].z -= mean; v[j].w -= mean;
-                sq += (v[j].x * v[j].x + v[j].y * v[j].y) + (v[j].z * v[j].z + v[j].w * v[j].w);
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-            const float scale = 1.0f / sqrtf(sq / (float)D + eps);
+            const float scale = ln_center(v, sum, lane, NV * 32, D, eps);
             // the staging block of two iterations ago must have left shared memory before it is overwritten
             const uint32_t ob = s_out + (uint32_t)(it & 1) * OUT_BYTES;
             if (threadIdx.x == 0) ptx::tma_store_wait_read<1>();
@@ -681,35 +671,22 @@ layernorm_tma_kernel(const float *__restrict__ x, const float *__restrict__ w, c
 #pragma unroll
                     for (int j = 0; j < NV; ++j)
                     {
-                        v[j].x = __fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww[j].x), bb[j].x);
-                        v[j].y = __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww[j].y), bb[j].y);
-                        v[j].z = __fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww[j].z), bb[j].z);
-                        v[j].w = __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww[j].w), bb[j].w);
-                        amax = fmaxf(amax, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
+                        v[j] = ln_affine(v[j], scale, ww[j], bb[j]);
+                        amax = fmaxf(amax, abs_max4(v[j]));
                     }
-#pragma unroll
-                    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
-                    const float inv = amax > 0.f ? __fdiv_rn(448.f, amax) : 1.f;
-                    if (lane == 0) y_scale[row0 + warp] = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
+                    amax = warp_max(amax);
+                    const float inv = e4m3_multiplier(amax);
+                    if (lane == 0) y_scale[row0 + warp] = e4m3_row_scale(amax);
                     uint32_t *yr = reinterpret_cast<uint32_t *>(smem + (ob - base) + (size_t)warp * D);
 #pragma unroll
-                    for (int j = 0; j < NV; ++j)
-                        yr[lane + 32 * j] = ptx::cvt_e4m3x4(__fmul_rn(v[j].x, inv), __fmul_rn(v[j].y, inv), __fmul_rn(v[j].z, inv), __fmul_rn(v[j].w, inv));
+                    for (int j = 0; j < NV; ++j) yr[lane + 32 * j] = e4m3x4(v[j], inv);
                 }
             }
             else if (warp < nr)
             {
                 uint2 *yr = reinterpret_cast<uint2 *>(smem + (ob - base) + (size_t)warp * D * 2);
 #pragma unroll
-                for (int j = 0; j < NV; ++j)
-                {
-                    const __half2 h0 = __floats2half2_rn(__fadd_rn(__fmul_rn(__fmul_rn(v[j].x, scale), ww[j].x), bb[j].x), __fadd_rn(__fmul_rn(__fmul_rn(v[j].y, scale), ww[j].y), bb[j].y));
-                    const __half2 h1 = __floats2half2_rn(__fadd_rn(__fmul_rn(__fmul_rn(v[j].z, scale), ww[j].z), bb[j].z), __fadd_rn(__fmul_rn(__fmul_rn(v[j].w, scale), ww[j].w), bb[j].w));
-                    uint2 u;
-                    u.x = *reinterpret_cast<const uint32_t *>(&h0);
-                    u.y = *reinterpret_cast<const uint32_t *>(&h1);
-                    yr[lane + 32 * j] = u;
-                }
+                for (int j = 0; j < NV; ++j) yr[lane + 32 * j] = pack4<OutT>(ln_affine(v[j], scale, ww[j], bb[j]));
             }
             ptx::fence_proxy_async_smem();
             ptx::named_bar_sync(1, 32 * LN_TMA_ROWS);
