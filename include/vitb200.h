@@ -58,9 +58,11 @@ typedef struct vitb200_tensor
  * max_batch bounds the batch accepted by vitb200_forward*.  Replaces, per model, what the reference re-does per
  * image in vit_predict (graph build x2, ggml_allocr, thread pool; vit.cpp:1009-1036).
  * Accepted shapes (every create function; anything else fails here, with a message naming the limit, not in the first forward):
- *   head dim 64 (hidden_size = 64 * num_attention_heads), hidden_size <= 2048 (the widest LayerNorm row a warp holds);
+ *   head dim 64 or 80 (hidden_size = 64 or 80 * num_attention_heads), hidden_size <= 2048 (the widest LayerNorm row a warp holds);
+ *   head dim 80 (ViT-H/14) without the attention-pooling head (vitb200_arch.pool = 2, whose kernel is 64 columns wide);
  *   patch_size 8, 14, 16 or 32 for 3-channel input, 8 or 16 for 1-channel input, dividing img_size;
- *   at most 896 tokens, (img_size / patch_size)^2 + 1 (K and V of one attention head in 227 KB of shared memory). */
+ *   at most 896 tokens at head dim 64 and 640 at head dim 80, (img_size / patch_size)^2 + 1 (K and V of one attention head in 227 KB of
+ *   shared memory). */
 int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                    vitb200_engine **out);
 
@@ -442,6 +444,12 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 /* The same with CLIP's causal mask (vitb200_text_arch.causal): query row t attends to keys 0 .. t of its sequence. */
 int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+/* Stand-alone run of the attention kernel of head dim hd (64 or 80) over a row-major QKV buffer: qkv_hi = f16 bits [B*N][3*H*hd],
+ * out = float32 [B*N][H*hd].  hd 80 runs the head-dim-80 kernel (kernel 0 = the engine's choice, or 4; 1 <= N <= 640, the
+ * engine's limit): on split-precision operands qkv_hi + qkv_lo when qkv_lo is given (N <= 224, as the engine runs it there), on the
+ * f16 values of qkv_hi when qkv_lo is NULL (as the engine runs it above 224 tokens).  hd 64 runs vitb200_test_attention's kernels, with
+ * the lo halves when qkv_lo is given (kernel 0 or 2). */
+int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 
 /* Stand-alone run of the attention-pooling head's attention kernel (vitb200_arch.pool = 2) through the engine's launcher: one query
  * q float32 [H*64] (the probe's, scaled by 1/8 inside) per head against the P key rows of each image; kv = f16 bits [B*P][2*H*64], every

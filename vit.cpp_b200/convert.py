@@ -231,8 +231,8 @@ def clip_to_timm(sd: Dict[str, np.ndarray], config: dict):
     pw = v["embeddings.patch_embedding.weight"]                          # (D, C, P, P), no bias
     D = int(pw.shape[0])
     heads = int(vc.get("num_attention_heads", D // 64))
-    if D % heads or D // heads != 64:
-        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    if D % heads or D // heads not in (64, 80):  # 80: the ViT-H/14 towers (LAION-2B, DFN5B, MetaCLIP)
+        raise ValueError(f"head dim {D / heads:g} is not supported (64 or 80)")
     layers = 1 + max(int(m.group(1)) for k in v for m in [re.match(r"encoder\.layers\.(\d+)\.", k)] if m)
     out = {
         "cls_token": v["embeddings.class_embedding"].reshape(1, 1, D),

@@ -795,8 +795,9 @@ int resid_epilogue(const vitb200_engine *e) { return e->arch.layer_scale ? EPI_B
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
 // token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision; ATT_MMA16 = the mma.sync kernel with 16 warps,
-// 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.
-enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3 };
+// 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.  Head dim 80 has one kernel,
+// ATT_MMA80 = attention_hd80_kernel (split precision up to 224 tokens, f16 operands beyond), which ATT_AUTO picks for it.
+enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3, ATT_MMA80 = 4 };
 constexpr int ATT_MAX_KEYS_16 = 640;
 
 // q / k / v tensor maps (hi and lo halves) of the wgmma attention over planes of max_batch * N token rows
@@ -828,6 +829,36 @@ constexpr int attention_smem_bytes(int N) { return 2 * ((N + ATT_KC - 1) / ATT_K
 constexpr int ATT_MAX_TOKENS = kSmemOptinMax / (2 * 128) / ATT_KC * ATT_KC;
 static_assert(attention_smem_bytes(ATT_MAX_TOKENS) <= kSmemOptinMax && attention_smem_bytes(ATT_MAX_TOKENS + 1) > kSmemOptinMax);
 
+// attention_hd80_kernel holds K and V (and, split, their lo halves) of one problem in rows of ATT80_ROW_BYTES, N padded to whole key
+// chunks.  Its f16 form bounds the token count of a head-dim-80 model; the split form runs up to ATTW_KEYS tokens.
+constexpr int attention_hd80_smem_bytes(int N, bool split) { return (split ? 4 : 2) * ((N + ATT_KC - 1) / ATT_KC * ATT_KC) * ATT80_ROW_BYTES; }
+constexpr int ATT80_MAX_TOKENS = kSmemOptinMax / (2 * ATT80_ROW_BYTES) / ATT_KC * ATT_KC;
+static_assert(attention_hd80_smem_bytes(ATT80_MAX_TOKENS, false) <= kSmemOptinMax &&
+              attention_hd80_smem_bytes(ATT80_MAX_TOKENS + 1, false) > kSmemOptinMax);
+static_assert(attention_hd80_smem_bytes(ATTW_KEYS, true) <= kSmemOptinMax);
+
+int head_dim(const vitb200_engine *e) { return e->hp.hidden_size / e->hp.num_attention_heads; }
+
+// the most tokens an image engine of head dim hd accepts
+constexpr int max_tokens(int hd) { return hd == ATT80_HD ? ATT80_MAX_TOKENS : ATT_MAX_TOKENS; }
+
+// head dim 80: split precision exactly when the qkv GEMM writes lo halves (N <= ATTW_KEYS), 8 warps; f16 operands with 16 warps
+int launch_attention_hd80(vitb200_engine *e, int B, cudaStream_t s)
+{
+    const int N = e->N, D = e->hp.hidden_size, H = e->hp.num_attention_heads;
+    const int Npad = (N + ATT_KC - 1) / ATT_KC * ATT_KC;
+    const bool split = e->QKV16L != nullptr;
+    if (split && N > ATTW_KEYS) return fail("split-precision head-dim-80 attention needs N <= %d (got %d)", ATTW_KEYS, N);
+    const int smem = attention_hd80_smem_bytes(N, split);
+    if (smem > kSmemOptinMax) return fail("attention: %d tokens do not fit in shared memory (max %d at head dim 80)", N, ATT80_MAX_TOKENS);
+    const float scale = 1.0f / sqrtf((float)ATT80_HD);
+    if (split)
+        return launch(e, attention_hd80_kernel<8, true>, dim3(B * H), dim3(8 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16, e->QKV16L, e->A16, N,
+                      D, H, Npad, scale);
+    return launch(e, attention_hd80_kernel<16, false>, dim3(B * H), dim3(16 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16,
+                  static_cast<const __half *>(nullptr), e->A16, N, D, H, Npad, scale);
+}
+
 template <int NW>
 int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
 {
@@ -841,6 +872,12 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
 
 int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO)
 {
+    if (head_dim(e) == ATT80_HD)
+    {
+        if (kernel != ATT_AUTO && kernel != ATT_MMA80) return fail("attention kernel %d does not run head dim 80", kernel);
+        return launch_attention_hd80(e, B, s);
+    }
+    if (kernel == ATT_MMA80) return fail("attention kernel %d runs head dim 80 only", kernel);
     if (kernel == ATT_AUTO) kernel = e->N <= ATTW_KEYS ? ATT_WGMMA : (e->N <= ATT_MAX_KEYS_16 ? ATT_MMA16 : ATT_MMA8);
     if (kernel == ATT_WGMMA) return launch_attention_wgmma(e, B, s);
     if (e->QKV16L) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
@@ -898,11 +935,13 @@ int tap_e4m3(float *dst, const uint8_t *q, const float *scale, size_t rows, size
     return 0;
 }
 
-// debug tap of the q | k | v activations in the reference's [tokens][3 D] order (the device buffers are head-major: [3 H][rows][64])
+// debug tap of the q | k | v activations in the reference's [tokens][3 D] order (the device buffers are head-major, [3 H][rows][64], at
+// head dim 64, and already in that order at head dim 80)
 int tap_qkv(vitb200_engine *e, float *dst, int T, cudaStream_t s)
 {
     if (!dst) return 0;
     const int D = e->hp.hidden_size, H = e->hp.num_attention_heads;
+    if (head_dim(e) != 64) return tap_f16(dst, e->QKV16, (size_t)T * 3 * D, s, e->QKV16L);
     const size_t plane_rows = (size_t)e->max_batch * e->N, n = (size_t)3 * H * plane_rows * 64;
     std::vector<float> tmp(n);
     if (tap_f16(tmp.data(), e->QKV16, n, s, e->QKV16L)) return 1;
@@ -968,14 +1007,16 @@ int run_blocks(vitb200_engine *e, int B, int first, int last, cudaStream_t s, co
         }
         {
             GemmParams p{};
-            p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D; p.headmajor = 1; p.plane_rows = (size_t)e->max_batch * N;
+            // head dim 64: the head-major planes the attention's TMA maps read; head dim 80: row-major [T][3 D]
+            p.M = T; p.N = 3 * D; p.K = D; p.bias = L.qkv.b; p.out = e->QKV16; p.out2 = e->QKV16L; p.ldo = 3 * D;
+            p.headmajor = head_dim(e) == 64; p.plane_rows = (size_t)e->max_batch * N;
             p.a_scale = e->SA; p.w_scale = L.qkv.w_scale;
             ProfScope ps(e, PK_QKV, 2.0 * p.M * p.N * p.K, s);
             if (launch_gemm(e, e->QKV16L ? EPI_BIAS_F16_HILO : EPI_BIAS_F16, e->fp8 ? e->tmA8 : e->tmA_D, L.qkv.tm, p, s, e->fp8)) return 1; // vit.cpp:820-821
         }
         if (tap && tap_qkv(e, taps->qkv, T, s)) return 1;
         {
-            ProfScope ps(e, PK_ATTN, 4.0 * B * e->hp.num_attention_heads * (double)N * N * 64, s);
+            ProfScope ps(e, PK_ATTN, 4.0 * B * e->hp.num_attention_heads * (double)N * N * head_dim(e), s);
             if (launch_attention(e, B, s)) return 1; // vit.cpp:826-866
         }
         if (tap && tap_f16(taps->attn, e->A16, (size_t)T * D, s)) return 1;
@@ -1528,15 +1569,19 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         return fail("tensor 'patch_embed.proj.weight' is missing or is not a 1- or 3-channel %dx%d kernel", hp->patch_size, hp->patch_size);
     const int in_chans = (int)(nelem(pw) / per_c);
     // shapes no kernel is built for: rejected here, where the caller can act on it, rather than by every forward call
-    if (hp->hidden_size % hp->num_attention_heads != 0 || hp->hidden_size / hp->num_attention_heads != 64)
-        return fail("head dim %d not supported (64 only)", hp->hidden_size / hp->num_attention_heads);
+    const int hd = hp->hidden_size / hp->num_attention_heads;
+    if (hp->hidden_size % hp->num_attention_heads != 0 || (hd != 64 && hd != ATT80_HD))
+        return fail("head dim %d not supported (64 or 80)", hd);
+    if (hd == ATT80_HD && ar.pool == 2)
+        return fail("vitb200_arch.pool = 2 (map) not supported at head dim 80 (the attention-pooling head's kernel is 64 columns wide)");
     if (hp->img_size % hp->patch_size != 0) return fail("img_size %d not a multiple of patch_size %d", hp->img_size, hp->patch_size);
     if (!patchify_supports(hp->patch_size, in_chans))
         return fail("patch size %d not supported for %d-channel input (%s)", hp->patch_size, in_chans, patchify_sizes(in_chans));
     if (hp->hidden_size > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", hp->hidden_size, LN_MAX_HIDDEN);
     const int n_tokens = (hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size) + prefix_rows(ar);
-    if (n_tokens > ATT_MAX_TOKENS)
-        return fail("%d tokens not supported (max %d: K and V of one attention head must fit in shared memory)", n_tokens, ATT_MAX_TOKENS);
+    if (n_tokens > max_tokens(hd))
+        return fail("%d tokens not supported (max %d at head dim %d: K and V of one attention head must fit in shared memory)", n_tokens,
+                    max_tokens(hd), hd);
     cudaDeviceProp prop;
     if (open_device(device, prop)) return 1;
     if (max_batch < 1) return fail("max_batch must be >= 1");
@@ -1633,8 +1678,9 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         return 1;
     if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
     // split-precision q, k, v (reference: f32 operands, vit.cpp:848,858) wherever hi + lo K and V fit next to each other in shared
-    // memory (N <= 224), i.e. wherever the wgmma attention runs
-    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || make_attention_maps(e))) return 1;
+    // memory (N <= 224), i.e. wherever the wgmma attention runs, or the head-dim-80 kernel in its split form (which reads the row-major
+    // buffers directly: no TMA maps)
+    if (e->N <= ATTW_KEYS && (dev_alloc(e, &e->QKV16L, T * 3 * D) || (hd == 64 && make_attention_maps(e)))) return 1;
     if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
     if (labels) e->labels = *labels;
     *out = owner.release();
@@ -2125,6 +2171,34 @@ int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const ui
     return guarded(__func__, [&] {
         if (!qkv_lo) return fail("bad argument");
         return test_attention_impl(device, ATT_WGMMA, B, N, H, qkv_hi, qkv_lo, out, true);
+    });
+}
+
+int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
+{
+    return guarded(__func__, [&]() -> int {
+        if (hd == 64)
+        {
+            if (qkv_lo && ((kernel != ATT_AUTO && kernel != ATT_WGMMA) || N > ATTW_KEYS))
+                return fail("split-precision operands run in the wgmma kernel (N <= %d)", ATTW_KEYS);
+            return test_attention_impl(device, kernel, B, N, H, qkv_hi, qkv_lo, out);
+        }
+        if (hd != ATT80_HD) return fail("head dim %d not supported (64 or 80)", hd);
+        if (!qkv_hi || !out || B < 1 || N < 1 || H < 1 || H > 128) return fail("bad argument");
+        if (kernel != ATT_AUTO && kernel != ATT_MMA80) return fail("attention kernel %d does not run head dim 80", kernel);
+        if (N > ATT80_MAX_TOKENS) return fail("%d tokens not supported (max %d at head dim 80)", N, ATT80_MAX_TOKENS);
+        if (qkv_lo && N > ATTW_KEYS) return fail("split-precision head-dim-80 attention needs N <= %d (got %d)", ATTW_KEYS, N);
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        e->N = N; e->hp.hidden_size = H * hd; e->hp.num_attention_heads = H; e->max_batch = B;
+        const size_t T = (size_t)B * N, D = (size_t)H * hd;
+        // the row-major [T][3 D] buffer the qkv GEMM writes at this head dim, as given; lo halves (the split form) when passed
+        if (upload(e, &e->QKV16, qkv_hi, T * 3 * D) || (qkv_lo && upload(e, &e->QKV16L, qkv_lo, T * 3 * D)) || dev_alloc(e, &e->A16, T * D))
+            return 1;
+        CUDA_TRY(cudaMemset(e->A16, 0xFF, T * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
+        if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
+        return tap_f16(out, e->A16, T * D, e->stream);
     });
 }
 

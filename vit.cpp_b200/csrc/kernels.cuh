@@ -866,6 +866,193 @@ attention_kernel(const __half *__restrict__ qkv, size_t plane_rows, __half *__re
 }
 
 // ------------------------------------------------------------------------------------------------
+// Attention for head dim 80 (ViT-H/14), every token count up to ATT80_MAX_TOKENS.  The soft-max of attention_kernel: two passes,
+// the TRUE row maximum, e = f16(exp(f16(s * scale - max))), l = sum e in f32, O = (P V) * (1 / l).  scale = 1 / sqrtf(80) is not a
+// power of two, but f32 rounding is monotone, so f32(max(s) * scale) == max(f32(s * scale)) still holds exactly.
+// qkv: the row-major [T][3 D] buffer the qkv GEMM writes for this head dim (q | k | v, head h at columns h 80, D + h 80 and
+// 2 D + h 80), out [T][D] f16.  One CTA per (image, head); it reads only the image's own N rows.  K and V live in shared memory in
+// rows of ATT80_ROW_BYTES: 160 B of data and 16 B of padding, so the 8 row starts of an ldmatrix (stride 11 x 16 B) fall in 8
+// distinct 16-B bank groups.  Rows past N are zero.  S = Q K^T is 5 k16 steps per 8-key tile, O = P V 10 n8 tiles.
+// SPLIT (N <= 224, like the wgmma kernel for head dim 64): qkv and qkv_lo hold hi = f16(x) and lo = f16(x - hi) of every value, and
+// S = Ql Kh^T + Qh Kl^T + Qh Kh^T, O = P Vl + P Vh (hi and lo of K and V in shared memory).  Otherwise the f16 values of qkv.
+constexpr int ATT80_HD = 80;
+constexpr int ATT80_ROW_BYTES = 176;
+constexpr int ATT80_KS = ATT80_HD / 16; // k16 steps of S = Q K^T
+constexpr int ATT80_DT = ATT80_HD / 8;  // n8 tiles of O = P V
+
+template <bool SPLIT>
+__device__ __forceinline__ void att80_scores(float (&s)[ATT_KC / 8][4], const uint32_t (&qh)[ATT80_KS][4], const uint32_t (&ql)[ATT80_KS][4],
+                                             uint32_t sKh, uint32_t sKl, int kc, int lane)
+{
+#pragma unroll
+    for (int nt = 0; nt < ATT_KC / 8; ++nt) { s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f; }
+    const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+    for (int ks = 0; ks < ATT80_KS; ++ks)
+    {
+#pragma unroll
+        for (int ntp = 0; ntp < ATT_KC / 16; ++ntp)
+        {
+            const int key = kc + (2 * ntp + (mi >> 1)) * 8 + lr;
+            const uint32_t off = (uint32_t)(key * ATT80_ROW_BYTES + (ks * 2 + (mi & 1)) * 16);
+            uint32_t b0, b1, b2, b3;
+            ptx::ldmatrix_x4(sKh + off, b0, b1, b2, b3);
+            if constexpr (SPLIT)
+            {
+                uint32_t c0, c1, c2, c3;
+                ptx::ldmatrix_x4(sKl + off, c0, c1, c2, c3);
+                ptx::mma_m16n8k16_f16(s[2 * ntp], ql[ks], b0, b1);
+                ptx::mma_m16n8k16_f16(s[2 * ntp + 1], ql[ks], b2, b3);
+                ptx::mma_m16n8k16_f16(s[2 * ntp], qh[ks], c0, c1);
+                ptx::mma_m16n8k16_f16(s[2 * ntp + 1], qh[ks], c2, c3);
+            }
+            ptx::mma_m16n8k16_f16(s[2 * ntp], qh[ks], b0, b1);
+            ptx::mma_m16n8k16_f16(s[2 * ntp + 1], qh[ks], b2, b3);
+        }
+    }
+}
+
+template <int NWARPS, bool SPLIT>
+__global__ void __launch_bounds__(NWARPS * 32)
+attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__ qkv_lo, __half *__restrict__ out, int N, int D, int H, int Npad,
+                      float scale)
+{
+    extern __shared__ __align__(16) uint8_t att80_smem[];
+    // launched with programmatic dependent launch: q, k, v are read only once the qkv GEMM has completed
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
+    const int b = blockIdx.x / H, h = blockIdx.x - b * H;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    constexpr int kParts = SPLIT ? 2 : 1;
+    const size_t ld = 3 * (size_t)D;                                     // row stride of qkv
+    const size_t q_off = (size_t)b * N * ld + (size_t)h * ATT80_HD;      // q of row 0 of this (image, head); k and v D and 2 D further
+    const uint32_t part_bytes = (uint32_t)Npad * ATT80_ROW_BYTES;
+    // [part] K | [part] V, part 0 = hi (or the f16 values), part 1 = lo
+    for (int part = 0; part < kParts; ++part)
+    {
+        const __half *src = (part ? qkv_lo : qkv) + q_off;
+        uint8_t *dK = att80_smem + part * part_bytes, *dV = att80_smem + (kParts + part) * part_bytes;
+        for (int idx = tid; idx < Npad * (ATT80_HD / 8); idx += NWARPS * 32)
+        {
+            const int t = idx / (ATT80_HD / 8), c = idx - t * (ATT80_HD / 8);
+            uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
+            if (t < N)
+            {
+                kv = __ldg(reinterpret_cast<const uint4 *>(src + (size_t)t * ld + D) + c);
+                vv = __ldg(reinterpret_cast<const uint4 *>(src + (size_t)t * ld + 2 * (size_t)D) + c);
+            }
+            *reinterpret_cast<uint4 *>(dK + t * ATT80_ROW_BYTES + c * 16) = kv;
+            *reinterpret_cast<uint4 *>(dV + t * ATT80_ROW_BYTES + c * 16) = vv;
+        }
+    }
+    __syncthreads();
+    const uint32_t sKh = ptx::smem_u32(att80_smem), sKl = sKh + part_bytes;
+    const uint32_t sVh = sKh + kParts * part_bytes, sVl = sVh + part_bytes;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int n_qtiles = (N + 15) >> 4;
+    for (int qt = warp; qt < n_qtiles; qt += NWARPS)
+    {
+        const int r0 = qt * 16 + g, r1 = r0 + 8;
+        uint32_t qh[ATT80_KS][4], ql[ATT80_KS][4];
+#pragma unroll
+        for (int part = 0; part < kParts; ++part)
+        {
+            const __half *src = (part ? qkv_lo : qkv) + q_off;
+#pragma unroll
+            for (int ks = 0; ks < ATT80_KS; ++ks)
+            {
+                const int col = ks * 16 + 2 * t4;
+                uint32_t(&qa)[4] = part ? ql[ks] : qh[ks];
+                qa[0] = r0 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r0 * ld + col)) : 0u;
+                qa[1] = r1 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r1 * ld + col)) : 0u;
+                qa[2] = r0 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r0 * ld + col + 8)) : 0u;
+                qa[3] = r1 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r1 * ld + col + 8)) : 0u;
+            }
+        }
+        // ---- pass 1: true row maximum of the unscaled scores
+        float mx0 = -INFINITY, mx1 = -INFINITY;
+        for (int kc = 0; kc < Npad; kc += ATT_KC)
+        {
+            float s[ATT_KC / 8][4];
+            att80_scores<SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
+#pragma unroll
+            for (int nt = 0; nt < ATT_KC / 8; ++nt)
+            {
+                const int key = kc + nt * 8 + 2 * t4;
+                if (key < N) { mx0 = fmaxf(mx0, s[nt][0]); mx1 = fmaxf(mx1, s[nt][2]); }
+                if (key + 1 < N) { mx0 = fmaxf(mx0, s[nt][1]); mx1 = fmaxf(mx1, s[nt][3]); }
+            }
+        }
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+        mx0 = __fmul_rn(mx0, scale); // == the maximum of the scaled scores (monotone rounding)
+        mx1 = __fmul_rn(mx1, scale);
+        // ---- pass 2: P = f16 exp(f16(s*scale - max)), l = sum P, O += P V
+        float o[ATT80_DT][4];
+#pragma unroll
+        for (int dt = 0; dt < ATT80_DT; ++dt) { o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f; }
+        float l0 = 0.f, l1 = 0.f;
+        for (int kc = 0; kc < Npad; kc += ATT_KC)
+        {
+            float s[ATT_KC / 8][4];
+            att80_scores<SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
+            uint32_t pa[ATT_KC / 16][4];
+#pragma unroll
+            for (int nt = 0; nt < ATT_KC / 8; ++nt)
+            {
+                const int key = kc + nt * 8 + 2 * t4;
+                const bool v0 = key < N, v1 = key + 1 < N;
+                const __half p00 = v0 ? exp_f16_semantics(__fmul_rn(s[nt][0], scale) - mx0) : __float2half_rn(0.f);
+                const __half p01 = v1 ? exp_f16_semantics(__fmul_rn(s[nt][1], scale) - mx0) : __float2half_rn(0.f);
+                const __half p10 = v0 ? exp_f16_semantics(__fmul_rn(s[nt][2], scale) - mx1) : __float2half_rn(0.f);
+                const __half p11 = v1 ? exp_f16_semantics(__fmul_rn(s[nt][3], scale) - mx1) : __float2half_rn(0.f);
+                l0 += __half2float(p00) + __half2float(p01);
+                l1 += __half2float(p10) + __half2float(p11);
+                const __half2 h0 = __halves2half2(p00, p01), h1 = __halves2half2(p10, p11);
+                pa[nt >> 1][(nt & 1) * 2 + 0] = *reinterpret_cast<const uint32_t *>(&h0);
+                pa[nt >> 1][(nt & 1) * 2 + 1] = *reinterpret_cast<const uint32_t *>(&h1);
+            }
+            const int mi = lane >> 3, lr = lane & 7;
+#pragma unroll
+            for (int j = 0; j < ATT_KC / 16; ++j)
+            {
+#pragma unroll
+                for (int dt = 0; dt < ATT80_DT; dt += 2)
+                {
+                    const int key = kc + j * 16 + (mi & 1) * 8 + lr;
+                    const uint32_t off = (uint32_t)(key * ATT80_ROW_BYTES + (dt + (mi >> 1)) * 16);
+                    uint32_t b0, b1, b2, b3;
+                    if constexpr (SPLIT)
+                    {
+                        ptx::ldmatrix_x4_trans(sVl + off, b0, b1, b2, b3);
+                        ptx::mma_m16n8k16_f16(o[dt], pa[j], b0, b1);
+                        ptx::mma_m16n8k16_f16(o[dt + 1], pa[j], b2, b3);
+                    }
+                    ptx::ldmatrix_x4_trans(sVh + off, b0, b1, b2, b3);
+                    ptx::mma_m16n8k16_f16(o[dt], pa[j], b0, b1);
+                    ptx::mma_m16n8k16_f16(o[dt + 1], pa[j], b2, b3);
+                }
+            }
+        }
+        l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+        l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+        const float inv0 = 1.0f / l0, inv1 = 1.0f / l1; // p_i = e_i * (1/sum)  (ggml.c:10556-10558)
+        __half *o0 = out + ((size_t)b * N + r0) * D + h * ATT80_HD + 2 * t4;
+        __half *o1 = out + ((size_t)b * N + r1) * D + h * ATT80_HD + 2 * t4;
+#pragma unroll
+        for (int dt = 0; dt < ATT80_DT; ++dt)
+        {
+            if (r0 < N) *reinterpret_cast<__half2 *>(o0 + dt * 8) = __floats2half2_rn(o[dt][0] * inv0, o[dt][1] * inv0);
+            if (r1 < N) *reinterpret_cast<__half2 *>(o1 + dt * 8) = __floats2half2_rn(o[dt][2] * inv1, o[dt][3] * inv1);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // One CTA per classifier row: probs = softmax(logits) with the reference's f16-exp semantics, then top-k (value descending, index
 // ascending on ties) by k rounds of block arg-max.  logits rows have pitch ldl (>= C: the head GEMM pads the class count to a
 // multiple of 4), probs rows are dense.  The working copy of the row lives in dynamic shared memory when C floats fit (the

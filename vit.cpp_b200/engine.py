@@ -140,6 +140,7 @@ def lib():
         L.vitb200_test_attention_hilo.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_test_softmax_topk.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
         L.vitb200_test_attention_pool.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+        L.vitb200_test_attention_hd.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -534,8 +535,8 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
 
 
 # attention kernels of vitb200_test_attention (include/vitb200.h): engine's choice, mma.sync with 8 warps (any N), wgmma (N <= 224,
-# the split-precision kernel), mma.sync with 16 warps (128 < N <= 640)
-ATTN_AUTO, ATTN_MMA8, ATTN_WGMMA, ATTN_MMA16 = 0, 1, 2, 3
+# the split-precision kernel), mma.sync with 16 warps (128 < N <= 640); the head-dim-80 kernel (vitb200_test_attention_hd)
+ATTN_AUTO, ATTN_MMA8, ATTN_WGMMA, ATTN_MMA16, ATTN_MMA80 = 0, 1, 2, 3, 4
 
 
 def test_attention(qkv16: np.ndarray, B: int, N: int, H: int, kernel: int = ATTN_AUTO, device: int = 0) -> np.ndarray:
@@ -569,6 +570,18 @@ def test_attention_hilo_causal(qkv32: np.ndarray, B: int, N: int, H: int, device
     out = np.empty((B * N, H * 64), np.float32)
     _check(lib().vitb200_test_attention_hilo_causal(device, B, N, H, hi.ctypes.data, lo.ctypes.data, out.ctypes.data),
            "vitb200_test_attention_hilo_causal")
+    return out
+
+
+def test_attention_hd(qkv32: np.ndarray, B: int, N: int, H: int, hd: int, split: bool, kernel: int = ATTN_AUTO,
+                      device: int = 0) -> np.ndarray:
+    """The attention kernel of head dim hd (64 or 80) alone (vitb200_test_attention_hd): qkv32 float32 [B*N, 3*H*hd], row-major
+    q | k | v, passed as hi + lo (split_hi_lo) when `split`, else as its f16 values -> float32 [B*N, H*hd]."""
+    x = np.ascontiguousarray(qkv32, np.float32).reshape(B * N, 3 * H * hd)
+    hi, lo = split_hi_lo(x) if split else (x.astype(np.float16), None)
+    out = np.empty((B * N, H * hd), np.float32)
+    _check(lib().vitb200_test_attention_hd(device, kernel, B, N, H, hd, hi.ctypes.data, None if lo is None else lo.ctypes.data,
+                                           out.ctypes.data), "vitb200_test_attention_hd")
     return out
 
 
