@@ -16,6 +16,7 @@ from tests.emulation_hd import Emulation
 from tests.hf_oracle import save_and_convert
 from tests.test_gpu_forward import check_parity
 from tests.test_gpu_fp8 import E2E_TOL
+from tests.test_gpu_kernels import _attention_ref
 from tests.test_head80 import GEOMETRIES, build_hf
 from tests.util import pkg, gf
 
@@ -27,18 +28,6 @@ pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 HD = 80
 MAX_TOKENS = 640   # the engine's limit at head dim 80 (ATT80_MAX_TOKENS)
-
-
-def _attention_ref(qkv, B, N, H):
-    """float64 restatement of vit.cpp:826-866 at head dim 80 on the values qkv [B*N][3*H*80] (row-major q | k | v), with the reference's
-    soft-max semantics (ggml.c:10533-10558): s in f32 times f32(1 / sqrtf(80)), e = f16(exp(f16(s - max))), p = e * (1/sum e)."""
-    x = qkv.astype(np.float64).reshape(B, N, 3, H, HD)
-    q, k, v = (x[:, :, i].transpose(0, 2, 1, 3) for i in range(3))
-    s = np.einsum("bhqd,bhkd->bhqk", q, k).astype(np.float32) * (np.float32(1) / np.sqrt(np.float32(HD)))
-    z = (s - s.max(-1, keepdims=True)).astype(np.float16).astype(np.float64)
-    e = np.exp(z).astype(np.float16).astype(np.float64)
-    o = np.einsum("bhqk,bhkd->bhqd", e, v) / e.sum(-1, keepdims=True)
-    return o.transpose(0, 2, 1, 3).reshape(B * N, H * HD)
 
 
 HOOK_CASES = [(2, n, 2) for n in (1, 17, 64, 224, 225, 257, 577, MAX_TOKENS)] + [(24, 257, 16)]   # (B, N, H)
@@ -63,13 +52,13 @@ def test_hook_against_numpy(B, N, H, split):
         seen = hi.astype(np.float32) + lo.astype(np.float32)
     else:
         seen = qkv.astype(np.float16).astype(np.float32)
-    ref = _attention_ref(seen, B, N, H)
+    ref = _attention_ref(seen, B, N, H, HD)
     assert np.isfinite(out).all()
     err = np.abs(out - ref)
     tol = 2.0 ** -10 * np.abs(ref) + 2e-3 * np.abs(ref).max()
     assert (err <= tol).all(), (err.max(), np.abs(ref).max(), np.unravel_index(err.argmax(), err.shape))
     if split and N > 1:   # closer to the split-operand restatement than to the f16-operand one (one key: O = f16(v) either way)
-        ref16 = _attention_ref(qkv.astype(np.float16).astype(np.float32), B, N, H)
+        ref16 = _attention_ref(qkv.astype(np.float16), B, N, H, HD)
         assert np.abs(out - ref).mean() < 0.6 * np.abs(out - ref16).mean()
 
 

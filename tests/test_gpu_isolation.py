@@ -3,7 +3,8 @@ them to Inf), must not change a single bit of its batch mates' outputs, nor of a
 images give on a fresh engine, which batch invariance makes bit-exact.
 
 Geometries: micro (17 tokens) and tiny (197) run the wgmma attention, whose 224-row key box spans 13 micro images; large384x2 (577)
-the 16-warp and p8 (785) the 8-warp mma.sync kernel; a CLIP micro tower (pre-norm) and a DINOv2 micro model with registers and the
+the 16-warp and p8 (785) the 8-warp mma.sync kernel; h80_micro (17) and h80_h14 (257), with 80-column heads, the split-precision and
+the f16 form of the head-dim-80 kernel; a CLIP micro tower (pre-norm) and a DINOv2 micro model with registers and the
 class-plus-patch-mean pool; and a ViTSTR model through the text recognition entry point."""
 import numpy as np
 import pytest
@@ -11,12 +12,13 @@ import pytest
 from tests import clip_oracle as co
 from tests import dinov2_oracle as do
 from tests.hf_oracle import save_and_convert
+from tests.test_gpu_head80 import _model_path as head80_model_path, mg
 from tests.util import pkg, gf, model_path
 
 eng = pkg.engine
 pytestmark = pytest.mark.gpu
 
-GEOS = ["micro", "tiny", "large384x2", "p8", "clip_micro", "dinov2_micro_reg"]
+GEOS = ["micro", "tiny", "large384x2", "p8", "h80_micro", "h80_h14", "clip_micro", "dinov2_micro_reg"]
 GRAPH_TOKENS = 8192   # calls of batch * N <= this many tokens run through a cached CUDA graph (captured on an argument set's 2nd call)
 POISONS = ["nan_pixel", "f16_overflow"]
 TOPK = 5
@@ -32,6 +34,8 @@ def _path(geo, tmp_path_factory):
         elif geo == "dinov2_micro_reg":
             d = str(tmp_path_factory.mktemp("dinov2_micro_reg"))
             _paths[geo] = save_and_convert(do.build_hf("micro_reg", True), d, "dinov2", do.convert_size("micro_reg"))
+        elif geo in mg.CASES:
+            _paths[geo] = head80_model_path(geo, tmp_path_factory)
         else:
             _paths[geo] = model_path(geo, "f16")
     return _paths[geo]
@@ -111,8 +115,8 @@ def _check_poisoned_rows(out, rows, C):
 
 
 def _batch(geo):
-    """A batch that spans the wgmma kernel's 224-row box (13 micro images), or five images for the larger token counts."""
-    return {"micro": 16, "clip_micro": 16, "dinov2_micro_reg": 16}.get(geo, 5)
+    """16 images of the 17-token geometries (13 of them span the wgmma kernel's 224-row box), or five for the larger token counts."""
+    return {"micro": 16, "h80_micro": 16, "clip_micro": 16, "dinov2_micro_reg": 16}.get(geo, 5)
 
 
 @pytest.mark.parametrize("kind", POISONS)

@@ -1,4 +1,6 @@
 """GPU tests of individual kernels through the C ABI (vitb200_test_gemm) against numpy / the oracle's primitives."""
+from typing import Callable, NamedTuple
+
 import numpy as np
 import pytest
 
@@ -90,29 +92,24 @@ def test_gemm_linearity_at_full_size():
 
 
 
-def _attention_ref(qkv16, B, N, H):
-    """float64 restatement of vit.cpp:826-866 on f16 inputs with the reference soft-max semantics (ggml.c:10533-10558):
-    e = f16(exp(f16(s/8 - max))), p = e * (1/sum e); O = P V."""
-    D = H * 64
-    x = qkv16.astype(np.float64).reshape(B, N, 3, H, 64)
-    q, k, v = x[:, :, 0].transpose(0, 2, 1, 3), x[:, :, 1].transpose(0, 2, 1, 3), x[:, :, 2].transpose(0, 2, 1, 3)
-    s = np.einsum("bhqd,bhkd->bhqk", q, k).astype(np.float32) * np.float32(0.125)
+def _scale(hd):
+    """The kernels' score scale, the host's 1.0f / sqrtf(hd) in f32: exactly 0.125 at head dim 64."""
+    return np.float32(1) / np.sqrt(np.float32(hd))
+
+
+def _attention_ref(x, B, N, H, hd=64, causal=False):
+    """float64 restatement of vit.cpp:826-866 on the values the kernel sees, x [B*N][3*H*hd] (row-major q | k | v: f16 values, or
+    hi + lo), with the reference soft-max semantics (ggml.c:10533-10558): s in f32 times the f32 scale, keys past the row at -inf when
+    causal (CLIP's text mask), e = f16(exp(f16(s - max))), O = e V / sum e."""
+    x = np.asarray(x, np.float64).reshape(B, N, 3, H, hd)
+    q, k, v = (x[:, :, i].transpose(0, 2, 1, 3) for i in range(3))
+    s = np.einsum("bhqd,bhkd->bhqk", q, k).astype(np.float32) * _scale(hd)
+    if causal:
+        s = np.where(np.tril(np.ones((N, N), bool)), s, np.float32(-np.inf))
     z = (s - s.max(-1, keepdims=True)).astype(np.float16).astype(np.float64)
     e = np.exp(z).astype(np.float16).astype(np.float64)
     o = np.einsum("bhqk,bhkd->bhqd", e, v) / e.sum(-1, keepdims=True)
-    return o.transpose(0, 2, 1, 3).reshape(B * N, D)
-
-
-def _attention_ref_f32(qkv32, B, N, H):
-    """The same on f32 q, k, v (what the reference's attention mat-muls see, vit.cpp:848,858)."""
-    D = H * 64
-    x = qkv32.astype(np.float64).reshape(B, N, 3, H, 64)
-    q, k, v = x[:, :, 0].transpose(0, 2, 1, 3), x[:, :, 1].transpose(0, 2, 1, 3), x[:, :, 2].transpose(0, 2, 1, 3)
-    s = np.einsum("bhqd,bhkd->bhqk", q, k).astype(np.float32) * np.float32(0.125)
-    z = (s - s.max(-1, keepdims=True)).astype(np.float16).astype(np.float64)
-    e = np.exp(z).astype(np.float16).astype(np.float64)
-    o = np.einsum("bhqk,bhkd->bhqd", e, v) / e.sum(-1, keepdims=True)
-    return o.transpose(0, 2, 1, 3).reshape(B * N, D), s
+    return o.transpose(0, 2, 1, 3).reshape(B * N, H * hd)
 
 
 @pytest.mark.parametrize("B,N,H", [(3, 17, 2), (2, 197, 3), (1, 224, 1), (40, 197, 12), (2, 50, 1)])
@@ -127,8 +124,8 @@ def test_attention_split_precision_against_f32_operand_reference(B, N, H):
     hi, lo = eng.split_hi_lo(qkv)
     q22 = hi.astype(np.float32) + lo.astype(np.float32)   # the 22-bit values the kernel actually sees
     out = eng.test_attention_hilo(qkv, B, N, H)
-    ref, _ = _attention_ref_f32(q22, B, N, H)
-    ref16, _ = _attention_ref_f32(hi.astype(np.float32), B, N, H)
+    ref = _attention_ref(q22, B, N, H)
+    ref16 = _attention_ref(hi, B, N, H)
     assert np.isfinite(out).all()
     err = np.abs(out - ref)
     tol = 2.0 ** -10 * np.abs(ref) + 2e-3 * np.abs(ref).max()
@@ -219,114 +216,212 @@ def test_layernorm_matches_the_restatement(rows, D):
 
 
 # ---- attention kernels at their edges ------------------------------------------------------------------------------------------------
-# Token counts on both sides of every tile boundary of each kernel: the wgmma kernel's 64-query tiles and 224-key box, the mma.sync
-# kernels' 16-query warp tiles, 32-key chunks and the 16-warp kernel's 640-key limit.  "hilo" is the wgmma kernel on split-precision
-# operands (vitb200_test_attention_hilo), the way the engine runs it.
-EDGE_N = {eng.ATTN_WGMMA: [1, 63, 64, 65, 128, 129, 197, 223, 224], "hilo": [1, 63, 64, 65, 128, 129, 197, 223, 224],
-          eng.ATTN_MMA16: [129, 160, 640], eng.ATTN_MMA8: [1, 31, 32, 33, 641, 896]}
-EDGE_CASES = [(kern, n) for kern, ns in EDGE_N.items() for n in ns]
-EDGE_IDS = [f"{'hilo' if kern == 'hilo' else {1: 'mma8', 2: 'wgmma', 3: 'mma16'}[kern]}-N{n}" for kern, n in EDGE_CASES]
-EDGE_B, EDGE_H = 3, 2
+class EdgeForm(NamedTuple):
+    """One way the engine runs attention: head dim, heads per image, CLIP's causal mask (query i attends to keys 0 .. i), hi + lo
+    operands (split_hi_lo) instead of f16 values, the hook (qkv32 [B*N][3*H*hd], B, N, H) -> [B*N][H*hd], and its token counts."""
+    hd: int
+    H: int
+    causal: bool
+    split: bool
+    run: Callable
+    ns: tuple
+
+
+# Token counts on both sides of every tile boundary of each form.  The wgmma kernel (wgmma on f16 operands, hilo on hi + lo as the
+# engine runs it, causal as text towers run it): 64-query tiles and the 224-key box; causal adds 2 (the first row with a masked key) and
+# CLIP's 77.  The head-dim-64 mma.sync kernels: 16-query warp tiles, 32-key chunks and the 16-warp kernel's 640-key limit.  The
+# head-dim-80 kernel: 16-query warp tiles, 32-key chunks, sweeps of 128 (8 warps, split form, up to 224 tokens) or 256 query rows
+# (16 warps, f16 form, 225 to 640 tokens); its three heads put the head slices of a row at 0, 160 and 320 bytes.
+_WGMMA_N = (1, 63, 64, 65, 128, 129, 197, 223, 224)
+EDGE_FORMS = {
+    "wgmma": EdgeForm(64, 2, False, False, lambda x, B, N, H: eng.test_attention(x.astype(np.float16), B, N, H, eng.ATTN_WGMMA), _WGMMA_N),
+    "hilo": EdgeForm(64, 2, False, True, eng.test_attention_hilo, _WGMMA_N),
+    "mma16": EdgeForm(64, 2, False, False, lambda x, B, N, H: eng.test_attention(x.astype(np.float16), B, N, H, eng.ATTN_MMA16),
+                      (129, 160, 640)),
+    "mma8": EdgeForm(64, 2, False, False, lambda x, B, N, H: eng.test_attention(x.astype(np.float16), B, N, H, eng.ATTN_MMA8),
+                     (1, 31, 32, 33, 641, 896)),
+    "hd80split": EdgeForm(80, 3, False, True, lambda x, B, N, H: eng.test_attention_hd(x, B, N, H, 80, True),
+                          (1, 15, 16, 17, 31, 32, 33, 127, 128, 129, 197, 223, 224)),
+    "hd80f16": EdgeForm(80, 3, False, False, lambda x, B, N, H: eng.test_attention_hd(x, B, N, H, 80, False),
+                        (225, 255, 256, 257, 287, 288, 289, 577, 639, 640)),
+    "causal": EdgeForm(64, 2, True, True, eng.test_attention_hilo_causal, (1, 2, 63, 64, 65, 77, 128, 129, 193, 224)),
+}
+EDGE_CASES = [(form, n) for form, f in EDGE_FORMS.items() for n in f.ns]
+EDGE_IDS = [f"{form}-N{n}" for form, n in EDGE_CASES]
+CAUSAL_CASES = [(form, n) for form, n in EDGE_CASES if EDGE_FORMS[form].causal]
+EDGE_B = 3
 
 
 def _pack(q, k, v):
-    """q, k, v [B][N][H][64] -> the fused [B*N][3*H*64] buffer the qkv GEMM leaves behind (q heads, then k heads, then v heads)."""
-    B, N, H, _ = q.shape
-    return np.stack([q, k, v], axis=2).reshape(B * N, 3 * H * 64)
+    """q, k, v [B][N][H][hd] -> the fused [B*N][3*H*hd] buffer the qkv GEMM leaves behind (q heads, then k heads, then v heads)."""
+    B, N, H, hd = q.shape
+    return np.stack([q, k, v], axis=2).reshape(B * N, 3 * H * hd)
 
 
-def _run_attention(kern, qkv32, B, N, H):
-    """f16 kernels get f16(qkv); the hi + lo hook gets qkv as f32 and reads hi = f16(x), lo = f16(x - hi)."""
-    if kern == "hilo":
-        return eng.test_attention_hilo(qkv32, B, N, H)
-    return eng.test_attention(qkv32.astype(np.float16), B, N, H, kern)
+def _run_attention(f, qkv32, B, N):
+    return f.run(qkv32, B, N, f.H)
 
 
-def _operand(kern, x32):
-    """The value the kernel sees for an f32 operand: f16(x), or hi + lo for the split-precision hook."""
-    if kern == "hilo":
+def _operand(f, x32):
+    """The value the kernel sees for an f32 operand: f16(x), or hi + lo for the split-precision forms."""
+    if f.split:
         hi, lo = eng.split_hi_lo(x32)
         return hi.astype(np.float64) + lo.astype(np.float64)
     return x32.astype(np.float16).astype(np.float64)
 
 
-@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
-def test_attention_routes_every_row_exactly(kern, N):
-    """Keys are random +-1 rows and q_i = 8 k_pi(i) for a random permutation pi of each (image, head): the chosen score (64 after the 1/8
-    scale) beats every other by >= 20, and f16(exp(x)) is exactly 0 below -17.33, so every probability row is exactly one-hot and the
-    output row i must be v_pi(i) bit for bit.  Every K and V row of every image, head, key chunk and query tile must land where it belongs."""
-    B, H = EDGE_B, EDGE_H
+def _scores(f, q, k, masked=False):
+    """Scaled scores [B][H][i][j] of the operand values in float64 with the f32 scale; -inf past the row if masked and f is causal."""
+    s = np.einsum("bihd,bjhd->bhij", _operand(f, q), _operand(f, k)) * np.float64(_scale(f.hd))
+    if masked and f.causal:
+        s = np.where(np.tril(np.ones(s.shape[-2:], bool)), s, -np.inf)
+    return s
+
+
+# Each case builder asserts its design (score gaps, score ranges, exact operands) before anything is launched, and returns the packed
+# input with what the kernel must produce.
+def _routing_case(f, N):
+    """Keys are random +-1 rows and q_i = 8 k_pi(i): pi is a random permutation of each (image, head), or under the causal mask a
+    random key of 0 .. i.  The chosen scaled score (8 hd / sqrt(hd): 64 at hd 64, 71.6 at hd 80) beats every other key of the row by
+    >= 20, and f16(exp(x)) is exactly 0 below -17.33, so every probability row is exactly one-hot: output row i is f16(v_pi(i))."""
+    B, H, hd = EDGE_B, f.H, f.hd
     rng = np.random.default_rng(1000 + N)
-    k = rng.choice(np.array([-1.0, 1.0], np.float32), size=(B, N, H, 64))
-    perm = np.stack([np.stack([rng.permutation(N) for _ in range(H)], 1) for _ in range(B)])  # [B][N][H]
-    q = np.take_along_axis(k, perm[..., None], axis=1) * 8.0
-    v = rng.standard_normal((B, N, H, 64)).astype(np.float32)
-    s = np.einsum("bihd,bjhd->bhij", q.astype(np.float64), k.astype(np.float64)) / 8.0
-    chosen = np.take_along_axis(s, perm.transpose(0, 2, 1)[..., None], axis=-1)[..., 0]
-    assert (chosen == 64.0).all()
+    k = rng.choice(np.array([-1.0, 1.0], np.float32), size=(B, N, H, hd))
+    if f.causal:
+        pick = rng.integers(0, np.arange(1, N + 1)[:, None], size=(B, N, H))
+    else:
+        pick = np.stack([np.stack([rng.permutation(N) for _ in range(H)], 1) for _ in range(B)])  # [B][N][H]
+    q = np.take_along_axis(k, pick[..., None], axis=1) * 8.0
+    v = rng.standard_normal((B, N, H, hd)).astype(np.float32)
+    s = _scores(f, q, k, masked=True)
+    chosen = np.take_along_axis(s, pick.transpose(0, 2, 1)[..., None], axis=-1)[..., 0]
+    assert (chosen == 8.0 * hd * np.float64(_scale(hd))).all()
     if N > 1:
         runner_up = np.sort(s, axis=-1)[..., -2]
         assert (chosen - runner_up >= 20.0).all(), float((chosen - runner_up).min())
-    out = _run_attention(kern, _pack(q, k, v), B, N, H)
-    want = np.take_along_axis(_operand(kern, v), perm[..., None], axis=1).astype(np.float16).astype(np.float32)
-    got = out.reshape(B, N, H, 64)
+    want = np.take_along_axis(_operand(f, v), pick[..., None], axis=1).astype(np.float16).astype(np.float32)
+    return _pack(q, k, v), want
+
+
+def _diagonal_case(f, N):
+    """k_j = 20 (j - 112) e_0 and q_i = 8 e_0, exact in f16 (lo = 0) and in the f32 score: scaled score 20 (j - 112).  Unmasked, every
+    row's maximum is key N - 1; under the mask row i's is key i and every other key of the row scores >= 20 lower, so output row i is
+    f16(v_i).  A mask one key late gives v_(i+1), a missing mask v_(N-1)."""
+    B, H, hd = EDGE_B, f.H, f.hd
+    rng = np.random.default_rng(5000 + N)
+    q = np.zeros((B, N, H, hd), np.float32)
+    k = np.zeros((B, N, H, hd), np.float32)
+    q[..., 0] = 8.0
+    k[..., 0] = 20.0 * (np.arange(N)[:, None] - 112)
+    v = rng.standard_normal((B, N, H, hd)).astype(np.float32)
+    assert (_operand(f, q) == q).all() and (_operand(f, k) == k).all()
+    dot = np.einsum("bihd,bjhd->bhij", q.astype(np.float64), k.astype(np.float64))
+    assert (dot.astype(np.float32) == dot).all()
+    assert (_scores(f, q, k).argmax(-1) == N - 1).all()
+    s = _scores(f, q, k, masked=True)
+    assert (s.argmax(-1) == np.arange(N)).all()
+    if N > 1:
+        top2 = np.sort(s, axis=-1)[..., -2:]
+        assert (top2[..., 1] - top2[..., 0] >= 20.0).all()
+    return _pack(q, k, v), _operand(f, v).astype(np.float16).astype(np.float32)
+
+
+def _uniform_case(f, N):
+    """q = 0: every score is 0, every e is 1 and output row i is the mean of the V rows it attends to (all N, or 0 .. i under the
+    mask).  Tolerance: one f16 output ulp plus the f32 summation error over those n keys."""
+    B, H, hd = EDGE_B, f.H, f.hd
+    rng = np.random.default_rng(2000 + N)
+    q = np.zeros((B, N, H, hd), np.float32)
+    k = rng.standard_normal((B, N, H, hd)).astype(np.float32)
+    v = (1.0 + 0.5 * rng.standard_normal((B, N, H, hd))).astype(np.float32)
+    vs = _operand(f, v)
+    if f.causal:
+        n = np.arange(1, N + 1)[:, None, None]
+        ref, mean_abs = np.cumsum(vs, axis=1) / n, np.cumsum(np.abs(vs), axis=1) / n
+    else:
+        n = N
+        ref, mean_abs = vs.mean(axis=1, keepdims=True), np.abs(vs).mean(axis=1, keepdims=True)
+    tol = np.spacing(np.abs(ref).astype(np.float16)).astype(np.float64) + 2 * (n + 2) * 2.0 ** -24 * mean_abs
+    return _pack(q, k, v), ref, tol
+
+
+def _all_negative_case(f, N):
+    """Dimension 0 carries -24 after scaling and the rest lies within +-2: every scaled score in [-26, -22], asserted in float64."""
+    B, H, hd = EDGE_B, f.H, f.hd
+    rng = np.random.default_rng(3000 + N)
+    k = rng.standard_normal((B, N, H, hd)).astype(np.float32)
+    q = (0.3 * rng.standard_normal((B, N, H, hd))).astype(np.float32)
+    k[..., 0], q[..., 0] = 1.0, -24.0 / _scale(hd)
+    v = rng.standard_normal((B, N, H, hd)).astype(np.float32)
+    s = _scores(f, q, k)
+    assert s.min() >= -26.0 and s.max() <= -22.0, (s.min(), s.max())
+    qkv = _pack(q, k, v)
+    return qkv, _attention_ref(_operand(f, qkv), B, N, H, hd, f.causal)
+
+
+@pytest.mark.parametrize("form,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_routes_every_row_exactly(form, N):
+    """One-hot probability rows (_routing_case): output row i must be the chosen V row bit for bit.  Every K and V row of every image,
+    head, key chunk and query tile must land where it belongs; the head-dim-80 hook fills its output with NaN first, so a row the
+    kernel never writes fails too."""
+    f = EDGE_FORMS[form]
+    qkv, want = _routing_case(f, N)
+    got = _run_attention(f, qkv, EDGE_B, N).reshape(want.shape)
     bad = np.argwhere(got != want)
     assert bad.size == 0, (len(bad), bad[:5].tolist())
 
 
-@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
-def test_attention_uniform_rows_average_exactly_the_real_keys(kern, N):
-    """q = 0: every score is 0, every e is 1 and the output is the mean of the N real V rows.  Against float64 within one f16 output
-    ulp plus the f32 summation error; a padded or foreign key counted in the sum l scales the output by N / N_padded and fails."""
-    B, H = EDGE_B, EDGE_H
-    rng = np.random.default_rng(2000 + N)
-    q = np.zeros((B, N, H, 64), np.float32)
-    k = rng.standard_normal((B, N, H, 64)).astype(np.float32)
-    v = (1.0 + 0.5 * rng.standard_normal((B, N, H, 64))).astype(np.float32)
-    out = _run_attention(kern, _pack(q, k, v), B, N, H).reshape(B, N, H, 64)
-    vs = _operand(kern, v)
-    ref = vs.mean(axis=1, keepdims=True)
-    tol = np.spacing(np.abs(ref).astype(np.float16)).astype(np.float64) + 2 * (N + 2) * 2.0 ** -24 * np.abs(vs).mean(axis=1, keepdims=True)
+@pytest.mark.parametrize("form,N", CAUSAL_CASES, ids=[f"{form}-N{n}" for form, n in CAUSAL_CASES])
+def test_causal_attention_takes_the_diagonal_only_under_the_mask(form, N):
+    """Scores that rise with the key index (_diagonal_case): under the mask each row's largest score is its own key's, so output row i
+    must be v_i bit for bit.  An off-by-one or missing mask routes the row to a later key."""
+    f = EDGE_FORMS[form]
+    qkv, want = _diagonal_case(f, N)
+    got = _run_attention(f, qkv, EDGE_B, N).reshape(want.shape)
+    bad = np.argwhere(got != want)
+    assert bad.size == 0, (len(bad), bad[:5].tolist())
+
+
+@pytest.mark.parametrize("form,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_uniform_rows_average_exactly_the_real_keys(form, N):
+    """Equal scores (_uniform_case) against float64: a padded or foreign key counted in the sum l scales the output by N / N_padded,
+    and a key the causal mask should hide changes the mean; both fail."""
+    f = EDGE_FORMS[form]
+    qkv, ref, tol = _uniform_case(f, N)
+    out = _run_attention(f, qkv, EDGE_B, N).reshape(EDGE_B, N, f.H, f.hd)
     err = np.abs(out - ref)
     assert (err <= tol).all(), float((err / tol).max())
 
 
-@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
-def test_attention_all_negative_scores(kern, N):
-    """Every scaled score in [-6, -2] (asserted in float64): against the float64 restatement at the usual tolerance.  A zero-filled
-    padding key (score 0) that escaped the masking would become the row maximum and add e = 1 per padded key to l."""
-    B, H = EDGE_B, EDGE_H
-    rng = np.random.default_rng(3000 + N)
-    k = rng.standard_normal((B, N, H, 64)).astype(np.float32)
-    q = (0.3 * rng.standard_normal((B, N, H, 64))).astype(np.float32)
-    k[..., 0], q[..., 0] = 1.0, -32.0                    # -4 after the 1/8 scale, the rest within +-2
-    v = rng.standard_normal((B, N, H, 64)).astype(np.float32)
-    qkv = _pack(q, k, v)
-    x = _operand(kern, qkv)
-    s = np.einsum("bihd,bjhd->bhij", x.reshape(B, N, 3, H, 64)[:, :, 0], x.reshape(B, N, 3, H, 64)[:, :, 1]) / 8.0
-    assert s.min() >= -6.0 and s.max() <= -2.0, (s.min(), s.max())
-    out = _run_attention(kern, qkv, B, N, H)
-    ref = _attention_ref_f32(x.astype(np.float32), B, N, H)[0] if kern == "hilo" else _attention_ref(qkv.astype(np.float16), B, N, H)
+@pytest.mark.parametrize("form,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_all_negative_scores(form, N):
+    """Every real scaled score in [-26, -22] (_all_negative_case): against the float64 restatement at the usual tolerance.  A
+    zero-filled padding key (score 0) that escaped the masking would become the row maximum, which makes f16(exp) of every real key 0
+    (l = 0, NaN output), or, counted in l, add e = f16(exp(>= 22)) = Inf to it (output 0)."""
+    f = EDGE_FORMS[form]
+    qkv, ref = _all_negative_case(f, N)
+    out = _run_attention(f, qkv, EDGE_B, N)
     err = np.abs(out - ref)
     tol = 2.0 ** -10 * np.abs(ref) + 2e-3 * np.abs(ref).max()
     assert (err <= tol).all(), (err.max(), np.abs(ref).max())
 
 
-@pytest.mark.parametrize("kern,N", EDGE_CASES, ids=EDGE_IDS)
-def test_attention_non_finite_values_stay_in_their_image(kern, N):
-    """NaN, then +Inf, in the Q rows, then the K rows, then the V rows of one image (first, middle, last of three): every other image's
-    output is bit-identical to the same launch with that image clean."""
-    B, H = EDGE_B, EDGE_H
+@pytest.mark.parametrize("form,N", EDGE_CASES, ids=EDGE_IDS)
+def test_attention_non_finite_values_stay_in_their_image(form, N):
+    """NaN, then +Inf, in the Q rows, then the K rows, then the V rows of one image or sequence (first, middle, last of three): every
+    other one's output is bit-identical to the same launch with that one clean."""
+    f = EDGE_FORMS[form]
+    B, H = EDGE_B, f.H
     rng = np.random.default_rng(4000 + N)
-    qkv = rng.normal(0.0, 1.0, (B, N, 3, H, 64)).astype(np.float32)
-    clean = _run_attention(kern, qkv.reshape(B * N, -1), B, N, H).reshape(B, N, -1)
+    qkv = rng.normal(0.0, 1.0, (B, N, 3, H, f.hd)).astype(np.float32)
+    clean = _run_attention(f, qkv.reshape(B * N, -1), B, N).reshape(B, N, -1)
     assert np.isfinite(clean).all()
     for val in (np.nan, np.inf):
         for part in range(3):
             for img in range(B):
                 x = qkv.copy()
                 x[img, :, part] = val
-                out = _run_attention(kern, x.reshape(B * N, -1), B, N, H).reshape(B, N, -1)
+                out = _run_attention(f, x.reshape(B * N, -1), B, N).reshape(B, N, -1)
                 others = [b for b in range(B) if b != img]
                 assert np.array_equal(out[others], clean[others]), (val, "qkv"[part], img)
 
