@@ -136,7 +136,8 @@ typedef struct vitb200_arch
  * point works on such an engine; the u8 entry points keep vit.cpp's preprocessing unless an image processor is set
  * (vitb200_set_image_proc: Hugging Face's CLIP, SigLIP and DINOv2 preprocessing).  The launch count of one forward is 3 + 7 L + 3 for pools 0 and 1, plus 1 with the
  * pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm); 2 + 7 L + 3 for pool 3 (no class-row kernel); 2 + 7 L + 10 for
- * pool 2 (the head adds LN, k | v GEMM, attention, out_proj, LN, fc1, fc2 and the f16 rounding of its row).
+ * pool 2 (the head adds LN, k | v GEMM, attention, out_proj, LN, fc1, fc2 and the f16 rounding of its row); each plus 1 (the similarity
+ * kernel) while a zero-shot head is set (vitb200_set_zero_shot).
  * A GGUF file selects the architecture with the keys vit.pre_norm (bool or integer), vit.activation ("gelu_tanh", "gelu_erf",
  * "quick_gelu", "gelu_pytorch_tanh", "swiglu"; any other string fails the load), vit.layer_scale (bool or integer), vit.reg_tokens (integer) and
  * vit.pool ("token", "cls_patch_mean", "map" or "mean"; any other string fails the load), and then holds 2 more tensors with the
@@ -237,6 +238,42 @@ typedef struct vitb200_image_proc
  * same checks.  A file without them, and every legacy-ggml file, has none. */
 int vitb200_set_image_proc(vitb200_engine *e, const vitb200_image_proc *p);
 int vitb200_get_image_proc(const vitb200_engine *e, vitb200_image_proc *out); /* 0; *out all zero when none is set */
+
+/* ---- zero-shot heads: CLIP and SigLIP (no reference counterpart) --------------------------------------------------------------
+ * Zero-shot classification against text embeddings, on the GPU: Hugging Face's logits_per_image.  With a head set, each image's head
+ * output x (the f32 row of num_classes = E values, the projection width, that the logits are without a head) becomes C class scores
+ *     logit[c] = s * (x . t_c) / ||x|| + b
+ * t_c = row c of class_embeds normalised once at set time (in f64, stored f32), s = f32(exp(logit_scale)) (logit_scale as HF stores it:
+ * vitb200_text_arch.logit_scale), b = logit_bias, or 0 when it is NaN.  mode 0: probs = the soft-max over the C scores with the reference's
+ * f16-exp semantics (CLIP), exactly as vitb200_forward's soft-max; mode 1: probs = 1 / (1 + exp(-logit)) per class (SigLIP), and the top-k
+ * ranks the scores, not the probabilities (which round to 1.0f above about 17), and returns the probability of each entry.  Top-k rules
+ * are vitb200_forward's: the lowest class id first on ties, (-1, 0) past C and for a row with a NaN score.
+ * The class matrix is [C][E] f32, any rows: usually text embeddings (vitb200_encode_text), or the mean of several prompt templates per
+ * class.  The scores are f32 FFMA dot products with the image norm computed in the same kernel, each summed in a fixed order, so an
+ * image's scores depend only on that image.  A forward with a head launches one kernel more than without (the similarity kernel). */
+typedef struct vitb200_zero_shot
+{
+    const float *class_embeds; /* [n_classes][num_classes] f32, row-major; copied (normalised) by the setter */
+    int32_t n_classes;         /* C, 1 .. 2^20 */
+    float logit_scale;         /* the log of the scale, as HF stores it */
+    float logit_bias;          /* added to every score (SigLIP); NaN for none (CLIP) */
+    int32_t mode;              /* 0 soft-max (CLIP), 1 sigmoid (SigLIP) */
+} vitb200_zero_shot;
+/* Set (z != NULL) or clear (z == NULL) the engine's zero-shot head.  While one is set, every entry point that returns probs, logits or
+ * top-k returns them over the C classes: vitb200_forward, _async, _device, _debug, vitb200_forward_u8, _u8_async, and
+ * vitb200_forward_sharded, _sharded_async (which refuse engines whose output widths differ, naming the engine); logits are the scores
+ * above.  Features calls and recognition are unchanged, and with no head every call behaves as before.
+ * Refused, naming the field or the row, before anything changes: a text engine; a 1-channel engine or head_tokens > 1 (ViTSTR); C < 1 or
+ * C > 2^20; a NULL class_embeds; a non-finite value or a row of zero norm in class_embeds; a non-finite logit_scale, or one whose exp
+ * overflows f32; a logit_bias of +-Inf; a mode other than 0 or 1.
+ * The setter waits for all work enqueued on the engine's device (its buffers are replaced) and drops the engine's cached CUDA graphs (a
+ * replayed graph would run the schedule and the buffers of its capture); the next small-batch calls run eagerly and capture again.  It
+ * sizes the per-slot probs and logits, the internal scores and the soft-max scratch for C classes; no forward call allocates. */
+int vitb200_set_zero_shot(vitb200_engine *e, const vitb200_zero_shot *z);
+/* The head as set (any pointer may be NULL): *n_classes = 0 (and the rest 0) when none is set. */
+int vitb200_get_zero_shot(const vitb200_engine *e, int32_t *n_classes, float *logit_scale, float *logit_bias, int32_t *mode);
+/* Per-row width of probs and logits: C while a zero-shot head is set, else num_classes. */
+int vitb200_num_outputs(const vitb200_engine *e);
 
 /* Text recognition with a ViTSTR model (1-channel, head_tokens >= 2; reference extensions/vitstr.cpp), image to text on the GPU:
  * the extension's vit_image_preprocess (vitstr.cpp:128-201: grayscale in double, its own bilinear resize to img^2 with no half-pixel
@@ -462,6 +499,13 @@ int vitb200_test_attention_pool(int device, int B, int P, int H, const float *q,
  * as the head GEMM leaves them, with NaN in the padding columns; probs float32 [rows][C], topk_idx int32 / topk_val float32 [rows][k]
  * on the host (may be NULL when k == 0).  0 <= k <= 16; top-k entries as vitb200_forward returns them. */
 int vitb200_test_softmax_topk(int device, int rows, int C, int k, const float *logits, float *probs, int32_t *topk_idx, float *topk_val);
+
+/* Stand-alone run of the zero-shot head's kernels (vitb200_set_zero_shot), launched as the forward launches them: x float32 [rows][E] (the
+ * head's rows, copied into rows of pitch round_up(E, 4) with NaN in the padding columns), T float32 [C][E] raw class rows (normalised and
+ * checked as the setter does), logit_scale / logit_bias / mode as in vitb200_zero_shot.  Outputs on the host: logits float32 [rows][C] (the
+ * scores), probs float32 [rows][C], topk_idx int32 / topk_val float32 [rows][k] (may be NULL when k == 0); 0 <= k <= 16. */
+int vitb200_test_zero_shot(int device, int rows, int E, int C, const float *x, const float *T, float logit_scale, float logit_bias, int mode, int k,
+                           float *probs, float *logits, int32_t *topk_idx, float *topk_val);
 
 /* Host-only: the upload-time weight conversion of one quantised tensor, `n_blocks` ggml blocks of 32 weights
  * (type = ggml_type / file ftype: 2 q4_0, 3 q4_1, 6 q5_0, 7 q5_1, 8 q8_0; ggml-quants.h:11-47) -> f16 bits, exactly what

@@ -219,6 +219,14 @@ struct vitb200_engine
     bool has_proc = false;
     vitb200_image_proc proc{};
     ProcPlan proc_plan;
+    // the zero-shot head (vitb200_set_zero_shot): zs_C > 0 classes, the unit class rows ZS_T [zs_C][num_classes] f32, the internal score
+    // rows ZS_S [max_batch][zs_C] (when the caller takes no logits), s = f32(exp(logit_scale)), b = logit_bias (0 for NaN), mode 0
+    // soft-max / 1 sigmoid; the arguments as set are kept for vitb200_get_zero_shot.  out_cols / sm_cols: the floats per row of the slot
+    // probs and logits and of the soft-max scratch, grown to zs_C when a head needs more
+    int zs_C = 0, zs_mode = 0;
+    float zs_s = 0.f, zs_b = 0.f, zs_logit_scale = 0.f, zs_logit_bias = 0.f;
+    float *ZS_T = nullptr, *ZS_S = nullptr;
+    int out_cols = 0, sm_cols = 0;
     // CUDA-graph cache for the kernel schedule of one forward, keyed by its arguments (launch-bound inner loop: ~90 kernels)
     struct GraphEntry { GraphKey key; int state; int launches; cudaGraphExec_t exec; };
     std::vector<GraphEntry> graphs;
@@ -243,6 +251,16 @@ int dev_alloc(vitb200_engine *e, T **p, size_t count)
     CUDA_TRY(cudaMemset(q, 0, count * sizeof(T) + 256));
     *p = reinterpret_cast<T *>(q);
     return 0;
+}
+
+// Frees the engine-owned buffer *p (from dev_alloc, or NULL) and sets it to NULL
+template <typename T>
+void dev_free(vitb200_engine *e, T **p)
+{
+    if (!*p) return;
+    e->allocs.erase(std::remove(e->allocs.begin(), e->allocs.end(), (void *)*p), e->allocs.end());
+    cudaFree(*p);
+    *p = nullptr;
 }
 
 const vitb200_tensor *find_tensor(const vitb200_tensor *t, int n, const std::string &name)
@@ -1060,6 +1078,9 @@ int run_encoder(vitb200_engine *e, const float *d_images, int B, int layers, cud
     return run_embed(e, d_images, B, s, taps) || run_blocks(e, B, 0, layers, s, taps);
 }
 
+// per-row width of probs and logits: the zero-shot head's classes while one is set, else the model's
+int num_outputs(const vitb200_engine *e) { return e->zs_C ? e->zs_C : e->hp.num_classes; }
+
 int check_batch(const vitb200_engine *e, int batch)
 {
     if (batch < 1 || batch > e->max_batch) return fail("batch %d out of range (1..%d)", batch, e->max_batch);
@@ -1073,15 +1094,31 @@ int check_k(const vitb200_engine *e, int k)
 }
 
 // Soft-max + top-k of `rows` logits rows of pitch ldl >= C: the working row in dynamic shared memory up to kSoftmaxSmemMax, beyond it
-// in e->d_sm_scratch ([rows][C] floats)
+// in e->d_sm_scratch ([rows][C] floats).  sigmoid: the zero-shot head's mode 1 (per-class sigmoid, top-k by logit)
 int launch_softmax_topk(vitb200_engine *e, const float *lg, int ldl, int rows, int C, float *d_probs, int32_t *d_topk_idx, float *d_topk_val,
-                        int k, cudaStream_t s)
+                        int k, cudaStream_t s, bool sigmoid = false)
 {
     const size_t row_bytes = (size_t)C * sizeof(float);
     float *scratch = row_bytes > kSoftmaxSmemMax ? e->d_sm_scratch : nullptr;
     if (row_bytes > kSoftmaxSmemMax && !scratch) return fail("soft-max: %d classes need a global working row and none is allocated", C);
-    return launch(e, softmax_topk_kernel, dim3(rows), dim3(256), scratch ? 0 : row_bytes, s, LAUNCH_PLAIN, lg, ldl, d_probs, d_topk_idx,
-                  d_topk_val, C, k, scratch);
+    return launch(e, sigmoid ? softmax_topk_kernel<true> : softmax_topk_kernel<false>, dim3(rows), dim3(256), scratch ? 0 : row_bytes, s,
+                  LAUNCH_PLAIN, lg, ldl, d_probs, d_topk_idx, d_topk_val, C, k, scratch);
+}
+
+// After the head GEMM has written the R rows lg (pitch ldl, num_classes columns): the zero-shot head's scores into d_logits (dense
+// [R][zs_C]) or, when the caller takes none, into ZS_S, then its soft-max or sigmoid and top-k over the zs_C classes.  One launch more
+// than the schedule without a head (the head's scores replace the 2-D copy of the logits).
+int run_zero_shot(vitb200_engine *e, const float *lg, int ldl, int R, float *d_probs, float *d_logits, int32_t *d_topk_idx, float *d_topk_val,
+                  int k, cudaStream_t s)
+{
+    const int Z = e->zs_C;
+    float *z = d_logits ? d_logits : e->ZS_S;
+    if (launch(e, zero_shot_kernel, dim3((unsigned)((R + ZS_TILE - 1) / ZS_TILE), (unsigned)((Z + ZS_TILE - 1) / ZS_TILE)), dim3(ZS_THREADS), 0, s,
+               LAUNCH_PLAIN, lg, ldl, (const float *)e->ZS_T, z, Z, R, e->hp.num_classes, Z, e->zs_s, e->zs_b))
+        return 1;
+    if (d_probs || (k > 0 && (d_topk_idx || d_topk_val)))
+        return launch_softmax_topk(e, z, Z, R, Z, d_probs, d_topk_idx, d_topk_val, k, s, e->zs_mode == 1);
+    return 0;
 }
 
 // SigLIP's attention-pooling head (vitb200_arch.pool = 2, HF SiglipMultiheadAttentionPoolingHead) on the residual stream X of B images
@@ -1146,13 +1183,14 @@ int run_forward(vitb200_engine *e, const float *d_images, int B, float *d_probs,
     // internal logits rows have pitch Cp (num_classes padded to 4; the padded W rows are TMA zero fill, the padded bias is 0);
     // a caller's dense [rows][num_classes] buffer is written directly when the two coincide, else through a 2-D copy
     const int Cp = e->Cp;
-    float *lg = (d_logits && Cp == C) ? d_logits : e->d_logits;
+    float *lg = (d_logits && Cp == C && !e->zs_C) ? d_logits : e->d_logits;
     {
         GemmParams p{};
         p.M = R; p.N = Cp; p.K = e->KH; p.bias = e->head.b; p.out = lg; p.ldo = Cp;
         ProfScope ps(e, PK_HEAD, 2.0 * p.M * C * p.K, s);
         if (launch_gemm(e, EPI_BIAS_F32, e->tmA_C, e->head.tm, p, s)) return 1;
     }
+    if (e->zs_C) return run_zero_shot(e, lg, Cp, R, d_probs, d_logits, d_topk_idx, d_topk_val, k, s);
     if (d_logits && lg != d_logits)
         CUDA_TRY(cudaMemcpy2DAsync(d_logits, (size_t)C * 4, lg, (size_t)Cp * 4, (size_t)C * 4, (size_t)R, cudaMemcpyDeviceToDevice, s));
     if ((d_probs || (k > 0 && (d_topk_idx || d_topk_val))) && launch_softmax_topk(e, lg, Cp, R, C, d_probs, d_topk_idx, d_topk_val, k, s)) return 1;
@@ -1649,6 +1687,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         return 1;
     // soft-max working row: dynamic shared memory up to the per-CTA limit, global scratch beyond it
     if ((size_t)hp->num_classes * sizeof(float) > kSoftmaxSmemMax && dev_alloc(e, &e->d_sm_scratch, R * hp->num_classes)) return 1;
+    e->out_cols = hp->num_classes;
+    e->sm_cols = e->d_sm_scratch ? hp->num_classes : 0;
     for (Slot &sl : e->slot)
     {
         if (dev_alloc(e, &sl.img, B * img_elems) || dev_alloc(e, &sl.probs, R * hp->num_classes) || dev_alloc(e, &sl.logits, R * hp->num_classes) ||
@@ -1922,7 +1962,7 @@ int classify_to_host(vitb200_engine *e, const Slot &sl, const float *d_images, i
     const int kk = want_topk ? k : 0;
     if (taps ? run_forward(e, d_images, batch, dp, sl.logits, di, dv, kk, s, taps) : run_forward_graphed(e, d_images, batch, dp, sl.logits, di, dv, kk, s))
         return 1;
-    const size_t rows = (size_t)batch * e->head_tokens, C = e->hp.num_classes; // classifier rows returned
+    const size_t rows = (size_t)batch * e->head_tokens, C = (size_t)num_outputs(e); // classifier rows returned
     if (probs) CUDA_TRY(cudaMemcpyAsync(probs, sl.probs, rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (logits) CUDA_TRY(cudaMemcpyAsync(logits, sl.logits, rows * C * sizeof(float), cudaMemcpyDeviceToHost, s));
     if (want_topk && topk_idx) CUDA_TRY(cudaMemcpyAsync(topk_idx, sl.topk_idx, rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost, s));
@@ -2039,6 +2079,105 @@ int vitb200_get_image_proc(const vitb200_engine *e, vitb200_image_proc *out)
         return 0;
     });
 }
+
+// vitb200_set_zero_shot's checks on a head for an engine whose head rows are E wide, shared with vitb200_test_zero_shot; each refusal
+// names the field or the row.  On success T holds the unit class rows (normalised in f64, stored f32), s = f32(exp(logit_scale)) (the
+// exponential in f64) and b = logit_bias, 0 for NaN.
+static int prepare_zero_shot(const vitb200_zero_shot &z, int E, std::vector<float> &T, float &s, float &b)
+{
+    if (z.n_classes < 1 || z.n_classes > (1 << 20)) return fail("zero_shot.n_classes = %d out of range (1..%d)", z.n_classes, 1 << 20);
+    if (!z.class_embeds) return fail("zero_shot.class_embeds is NULL");
+    if (z.mode != 0 && z.mode != 1) return fail("zero_shot.mode = %d: 0 (soft-max, CLIP) or 1 (sigmoid, SigLIP)", z.mode);
+    if (!std::isfinite(z.logit_scale)) return fail("zero_shot.logit_scale = %g: must be finite", (double)z.logit_scale);
+    const float sc = (float)std::exp((double)z.logit_scale);
+    if (!std::isfinite(sc)) return fail("zero_shot.logit_scale = %g: exp(logit_scale) overflows f32", (double)z.logit_scale);
+    if (std::isinf(z.logit_bias)) return fail("zero_shot.logit_bias = %g: must be finite, or NaN for none", (double)z.logit_bias);
+    T.resize((size_t)z.n_classes * E);
+    for (int c = 0; c < z.n_classes; ++c)
+    {
+        const float *row = z.class_embeds + (size_t)c * E;
+        double ss = 0.0;
+        for (int k = 0; k < E; ++k)
+        {
+            if (!std::isfinite(row[k])) return fail("zero_shot.class_embeds[%d][%d] = %g: must be finite", c, k, (double)row[k]);
+            ss += (double)row[k] * row[k];
+        }
+        if (ss == 0.0) return fail("zero_shot.class_embeds row %d has zero norm", c);
+        const double norm = std::sqrt(ss);
+        for (int k = 0; k < E; ++k) T[(size_t)c * E + k] = (float)(row[k] / norm);
+    }
+    s = sc;
+    b = std::isnan(z.logit_bias) ? 0.f : z.logit_bias;
+    return 0;
+}
+
+static int set_zero_shot(vitb200_engine *e, const vitb200_zero_shot *z)
+{
+    if (!e) return fail("null argument");
+    if (image_only(e, "vitb200_set_zero_shot")) return 1;
+    if (e->C != 3) return fail("vitb200_set_zero_shot: this model takes %d-channel input; a zero-shot head is for RGB image towers", e->C);
+    if (e->head_tokens > 1)
+        return fail("vitb200_set_zero_shot: head_tokens is %d (ViTSTR); a zero-shot head scores one row per image", e->head_tokens);
+    std::vector<float> T;
+    float s = 0.f, b = 0.f;
+    if (z && prepare_zero_shot(*z, e->hp.num_classes, T, s, b)) return 1;
+    CUDA_TRY(cudaSetDevice(e->device));
+    // work already enqueued (on any stream: vitb200_forward_device may run on the caller's) can still read the buffers replaced below
+    CUDA_TRY(cudaDeviceSynchronize());
+    // a captured graph holds the schedule and the buffer addresses of its capture
+    for (auto &g : e->graphs)
+        if (g.exec) cudaGraphExecDestroy(g.exec);
+    e->graphs.clear();
+    e->zs_C = 0;
+    dev_free(e, &e->ZS_T);
+    dev_free(e, &e->ZS_S);
+    if (!z) return 0;
+    const size_t R = (size_t)e->max_batch * e->head_tokens, Z = (size_t)z->n_classes;
+    if (upload(e, &e->ZS_T, T.data(), T.size()) || dev_alloc(e, &e->ZS_S, R * Z)) return 1;
+    if ((int)Z > e->out_cols)
+    {
+        for (Slot &sl : e->slot)
+        {
+            dev_free(e, &sl.probs);
+            dev_free(e, &sl.logits);
+            if (dev_alloc(e, &sl.probs, R * Z) || dev_alloc(e, &sl.logits, R * Z)) return 1;
+        }
+        e->out_cols = (int)Z;
+    }
+    if (Z * sizeof(float) > kSoftmaxSmemMax && (int)Z > e->sm_cols)
+    {
+        dev_free(e, &e->d_sm_scratch);
+        if (dev_alloc(e, &e->d_sm_scratch, R * Z)) return 1;
+        e->sm_cols = (int)Z;
+    }
+    e->zs_s = s;
+    e->zs_b = b;
+    e->zs_mode = z->mode;
+    e->zs_logit_scale = z->logit_scale;
+    e->zs_logit_bias = z->logit_bias;
+    e->zs_C = (int)Z;
+    return 0;
+}
+
+int vitb200_set_zero_shot(vitb200_engine *e, const vitb200_zero_shot *z)
+{
+    return guarded(__func__, [&] { return set_zero_shot(e, z); });
+}
+
+int vitb200_get_zero_shot(const vitb200_engine *e, int32_t *n_classes, float *logit_scale, float *logit_bias, int32_t *mode)
+{
+    return guarded(__func__, [&] {
+        if (!e) return fail("null argument");
+        if (image_only(e, __func__)) return 1;
+        if (n_classes) *n_classes = e->zs_C;
+        if (logit_scale) *logit_scale = e->zs_C ? e->zs_logit_scale : 0.f;
+        if (logit_bias) *logit_bias = e->zs_C ? e->zs_logit_bias : 0.f;
+        if (mode) *mode = e->zs_C ? e->zs_mode : 0;
+        return 0;
+    });
+}
+
+int vitb200_num_outputs(const vitb200_engine *e) { return e ? num_outputs(e) : 0; }
 
 void vitb200_destroy(vitb200_engine *e)
 {
@@ -2260,6 +2399,51 @@ int vitb200_test_softmax_topk(int device, int rows, int C, int k, const float *l
     });
 }
 
+int vitb200_test_zero_shot(int device, int rows, int E, int C, const float *x, const float *T, float logit_scale, float logit_bias, int mode, int k,
+                           float *probs, float *logits, int32_t *topk_idx, float *topk_val)
+{
+    return guarded(__func__, [&]() -> int {
+        if (!x || !T || !probs || !logits || rows < 1 || E < 1 || E > (1 << 20)) return fail("bad argument");
+        if (k > 0 && (!topk_idx || !topk_val)) return fail("null argument");
+        std::vector<float> Tn;
+        float s = 0.f, b = 0.f;
+        if (prepare_zero_shot(vitb200_zero_shot{T, C, logit_scale, logit_bias, mode}, E, Tn, s, b)) return 1;
+        EnginePtr owner;
+        if (scratch_engine(device, owner)) return 1;
+        vitb200_engine *e = owner.get();
+        e->max_k = 16;
+        if (check_k(e, k)) return 1;
+        e->hp.num_classes = E;
+        e->zs_C = C; e->zs_s = s; e->zs_b = b; e->zs_mode = mode;
+        // head rows of pitch round_up(E, 4), as the head GEMM leaves them; the padding columns hold NaN, which the kernel must never read
+        const int Ep = (E + 3) / 4 * 4;
+        std::vector<float> padded((size_t)rows * Ep, std::nanf(""));
+        for (int r = 0; r < rows; ++r) memcpy(&padded[(size_t)r * Ep], x + (size_t)r * E, (size_t)E * sizeof(float));
+        float *dx = nullptr, *dp = nullptr, *dl = nullptr, *dv = nullptr;
+        int32_t *di = nullptr;
+        const size_t RC = (size_t)rows * C;
+        if (upload(e, &dx, padded.data(), padded.size()) || upload(e, &e->ZS_T, Tn.data(), Tn.size()) || dev_alloc(e, &dp, RC) ||
+            dev_alloc(e, &dl, RC) || dev_alloc(e, &di, (size_t)rows * k + 1) || dev_alloc(e, &dv, (size_t)rows * k + 1))
+            return 1;
+        // outputs poisoned with 0x7f bytes (3.4e38, index 2139062143): an entry the kernels never write cannot pass for a result
+        CUDA_TRY(cudaMemset(dp, 0x7f, RC * sizeof(float)));
+        CUDA_TRY(cudaMemset(dl, 0x7f, RC * sizeof(float)));
+        CUDA_TRY(cudaMemset(di, 0x7f, ((size_t)rows * k + 1) * sizeof(int32_t)));
+        CUDA_TRY(cudaMemset(dv, 0x7f, ((size_t)rows * k + 1) * sizeof(float)));
+        if ((size_t)C * sizeof(float) > kSoftmaxSmemMax && dev_alloc(e, &e->d_sm_scratch, RC)) return 1;
+        if (run_scratch(e, "zero-shot kernels", [&] { return run_zero_shot(e, dx, Ep, rows, dp, dl, k ? di : nullptr, k ? dv : nullptr, k, e->stream); }))
+            return 1;
+        CUDA_TRY(cudaMemcpy(probs, dp, RC * sizeof(float), cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(logits, dl, RC * sizeof(float), cudaMemcpyDeviceToHost));
+        if (k > 0)
+        {
+            CUDA_TRY(cudaMemcpy(topk_idx, di, (size_t)rows * k * sizeof(int32_t), cudaMemcpyDeviceToHost));
+            CUDA_TRY(cudaMemcpy(topk_val, dv, (size_t)rows * k * sizeof(float), cudaMemcpyDeviceToHost));
+        }
+        return 0;
+    });
+}
+
 int vitb200_test_dequant(int type, const void *blocks, int64_t n_blocks, uint16_t *out_f16)
 {
     return guarded(__func__, [&] {
@@ -2398,7 +2582,7 @@ static int forward_sharded_impl(vitb200_engine *const *engines, int n_engines, c
         }
     }
     const size_t img_elems = (size_t)e0->C * e0->hp.img_size * e0->hp.img_size;
-    const size_t C = (size_t)e0->hp.num_classes * e0->head_tokens; // output floats per image
+    const size_t C = (size_t)num_outputs(e0) * e0->head_tokens; // output floats per image
     const size_t kk = (size_t)k * e0->head_tokens;                 // top-k entries per image
     const int base = batch / n_engines, rem = batch % n_engines;
     int begin = 0;
@@ -2410,6 +2594,9 @@ static int forward_sharded_impl(vitb200_engine *const *engines, int n_engines, c
         if (engines[g]->hp.img_size != e0->hp.img_size || engines[g]->hp.num_classes != e0->hp.num_classes || engines[g]->head_tokens != e0->head_tokens ||
             engines[g]->C != e0->C)
             return fail("engine %d holds a different model", g);
+        if (num_outputs(engines[g]) != num_outputs(e0))
+            return fail("engine %d returns %d outputs per row and engine 0 returns %d (set the same zero-shot head on every engine)", g,
+                        num_outputs(engines[g]), num_outputs(e0));
         if (vitb200_forward_async(engines[g], images + (size_t)begin * img_elems, cnt, probs ? probs + (size_t)begin * C : nullptr,
                                   logits ? logits + (size_t)begin * C : nullptr, topk_idx ? topk_idx + (size_t)begin * kk : nullptr,
                                   topk_prob ? topk_prob + (size_t)begin * kk : nullptr, k))

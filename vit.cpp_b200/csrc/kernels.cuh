@@ -12,7 +12,9 @@
 //   layernorm_inplace_kernel the same arithmetic in place on f32 rows (the pre-norm of CLIP towers)
 //   attention_kernel         per (image, head): S = QK^T / sqrt(hd), softmax with the reference's f16-exp
 //                            semantics (ggml.c:10536-10558), O = P V   (vit.cpp:826-866)
-//   softmax_topk_kernel      final soft-max (vit.cpp:931) + top-k (replaces the host std::sort, vit.cpp:1047-1057)
+//   softmax_topk_kernel      final soft-max (vit.cpp:931) + top-k (replaces the host std::sort, vit.cpp:1047-1057); its sigmoid form
+//                            for SigLIP's zero-shot head
+//   zero_shot_kernel         the zero-shot head (vitb200_set_zero_shot): cosine similarity of each head row with the class matrix, scaled
 #pragma once
 #include "ptx.cuh"
 
@@ -1058,6 +1060,10 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
 // multiple of 4), probs rows are dense.  The working copy of the row lives in dynamic shared memory when C floats fit (the
 // launcher opts in up to the 227 KB limit), otherwise in `scratch` (global, [rows][C]); entries r >= C of a top-k list (k > C)
 // are (-1, 0), and so is every entry of a row whose probabilities are NaN (a NaN logit, or +Inf: Inf - Inf).
+// SIGMOID (the zero-shot head's mode 1, SigLIP): probs = 1 / (1 + exp(-x)) per class, evaluated in f64 as exp(x) / (1 + exp(x)) below 0
+// so that small probabilities keep their relative precision, and the top-k ranks the LOGITS (the probability rounds to 1.0f above about
+// 17, which would tie distinct classes) and reports the probability of each; a NaN logit is never ranked, so a NaN row gives (-1, 0).
+template <bool SIGMOID>
 __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, float *__restrict__ probs, int32_t *__restrict__ topk_idx,
                                     float *__restrict__ topk_val, int C, int k, float *__restrict__ scratch)
 {
@@ -1067,35 +1073,55 @@ __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, f
     const int img = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
     float *sp = scratch ? scratch + (size_t)img * C : sp_smem;
     const float *lg = logits + (size_t)img * ldl;
-    float mx = -INFINITY;
-    for (int i = tid; i < C; i += blockDim.x) { const float v = lg[i]; sp[i] = v; mx = fmaxf(mx, v); }
-    for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
-    if (lane == 0) red_v[warp] = mx;
-    __syncthreads();
-    mx = red_v[0];
-    for (int w = 1; w < nw; ++w) mx = fmaxf(mx, red_v[w]);
-    __syncthreads();
-    float sum = 0.f;
-    for (int i = tid; i < C; i += blockDim.x)
+    // in f64, rounded once to f32: within 2^-24 relative of the exact sigmoid of the f32 logit (expf's 2 ulp would not be)
+    auto sigmoid = [](float x) {
+        const double e = exp(-fabs((double)x));
+        return (float)((x >= 0.f ? 1.0 : e) / (1.0 + e));
+    };
+    if constexpr (SIGMOID)
     {
-        const float e = __half2float(exp_f16_semantics(sp[i] - mx));
-        sp[i] = e;
-        sum += e;
+        for (int i = tid; i < C; i += blockDim.x)
+        {
+            const float v = lg[i];
+            sp[i] = v;
+            if (probs) probs[(size_t)img * C + i] = sigmoid(v);
+        }
     }
-    for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-    if (lane == 0) red_v[warp] = sum;
-    __syncthreads();
-    sum = 0.f;
-    for (int w = 0; w < nw; ++w) sum += red_v[w];
-    const float inv = 1.0f / sum;
-    __syncthreads();
-    for (int i = tid; i < C; i += blockDim.x)
+    else
     {
-        const float pr = __fmul_rn(sp[i], inv);
-        sp[i] = pr;
-        if (probs) probs[(size_t)img * C + i] = pr;
+        float mx = -INFINITY;
+        for (int i = tid; i < C; i += blockDim.x) { const float v = lg[i]; sp[i] = v; mx = fmaxf(mx, v); }
+        for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        if (lane == 0) red_v[warp] = mx;
+        __syncthreads();
+        mx = red_v[0];
+        for (int w = 1; w < nw; ++w) mx = fmaxf(mx, red_v[w]);
+        __syncthreads();
+        float sum = 0.f;
+        for (int i = tid; i < C; i += blockDim.x)
+        {
+            const float e = __half2float(exp_f16_semantics(sp[i] - mx));
+            sp[i] = e;
+            sum += e;
+        }
+        for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        if (lane == 0) red_v[warp] = sum;
+        __syncthreads();
+        sum = 0.f;
+        for (int w = 0; w < nw; ++w) sum += red_v[w];
+        const float inv = 1.0f / sum;
+        __syncthreads();
+        for (int i = tid; i < C; i += blockDim.x)
+        {
+            const float pr = __fmul_rn(sp[i], inv);
+            sp[i] = pr;
+            if (probs) probs[(size_t)img * C + i] = pr;
+        }
     }
     __syncthreads();
+    // probabilities are >= 0 and a taken entry becomes -2; logits may be -Inf, so the sigmoid form starts below every logit and marks a
+    // taken entry NaN
+    constexpr float kNone = SIGMOID ? -INFINITY : -1.f;
     for (int r = 0; r < k; ++r)
     {
         if (r >= C) // fewer classes than requested entries
@@ -1107,7 +1133,7 @@ __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, f
             }
             continue;
         }
-        float bv = -1.f;
+        float bv = kNone;
         int bi = 0x7fffffff;
         for (int i = tid; i < C; i += blockDim.x)
         {
@@ -1126,12 +1152,80 @@ __global__ void softmax_topk_kernel(const float *__restrict__ logits, int ldl, f
         {
             for (int w = 1; w < nw; ++w)
                 if (red_v[w] > bv || (red_v[w] == bv && red_i[w] < bi)) { bv = red_v[w]; bi = red_i[w]; }
-            if (bi == 0x7fffffff) { bi = -1; bv = 0.f; } // no probability compares >= 0: a NaN row
+            if (bi == 0x7fffffff) { bi = -1; bv = 0.f; } // nothing compares >= the floor: a NaN row
+            else if constexpr (SIGMOID) bv = sigmoid(bv);
             if (topk_idx) topk_idx[(size_t)img * k + r] = bi;
             if (topk_val) topk_val[(size_t)img * k + r] = bv;
-            if (bi >= 0 && bi < C) sp[bi] = -2.f;
+            if (bi >= 0 && bi < C) sp[bi] = SIGMOID ? __int_as_float(0x7fffffff) : -2.f;
         }
         __syncthreads();
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// The zero-shot head (vitb200_set_zero_shot): out[r][c] = s * (x_r . t_c) / ||x_r|| + b for the R head rows x (pitch ldx, E columns) and
+// the C unit rows of the class matrix t [C][E] (dense); out rows have pitch ldo.  One CTA per ZS_TILE rows x ZS_TILE classes, 256 threads
+// of 4 x 4 outputs, operands staged through shared memory ZS_BK columns at a time.  Each dot product is one thread's f32 FFMA chain over
+// k = 0 .. E-1 in order, and ||x_r|| is a lane-strided sum of squares with a fixed xor tree, so a row's scores depend on that row alone:
+// not on its batch mates, its position in the grid or the batch size.  A NaN or Inf in x_r (or a zero x_r) gives a NaN row.
+constexpr int ZS_TILE = 64, ZS_BK = 16, ZS_THREADS = 256;
+__global__ void __launch_bounds__(ZS_THREADS)
+zero_shot_kernel(const float *__restrict__ x, int ldx, const float *__restrict__ t, float *__restrict__ out, int ldo, int R, int E, int C, float s,
+                 float b)
+{
+    // [k][row] and [k][class]; rows of ZS_TILE + 4 keep the 16-byte reads aligned and spread the transposing stores over the banks
+    __shared__ __align__(16) float sx[ZS_BK][ZS_TILE + 4], st[ZS_BK][ZS_TILE + 4];
+    __shared__ float nrm[ZS_TILE];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, tx = tid & 15, ty = tid >> 4;
+    const int r0 = blockIdx.x * ZS_TILE, c0 = blockIdx.y * ZS_TILE;
+    for (int i = warp; i < ZS_TILE; i += ZS_THREADS / 32)
+    {
+        float ss = 0.f;
+        if (r0 + i < R)
+            for (int k = lane; k < E; k += 32) { const float v = x[(size_t)(r0 + i) * ldx + k]; ss = fmaf(v, v, ss); }
+        for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+        if (lane == 0) nrm[i] = sqrtf(ss);
+    }
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int k0 = 0; k0 < E; k0 += ZS_BK)
+    {
+        for (int i = tid; i < ZS_TILE * ZS_BK; i += ZS_THREADS)
+        {
+            const int kk = i % ZS_BK, rr = i / ZS_BK, k = k0 + kk;
+            sx[kk][rr] = (r0 + rr < R && k < E) ? x[(size_t)(r0 + rr) * ldx + k] : 0.f;
+            st[kk][rr] = (c0 + rr < C && k < E) ? t[(size_t)(c0 + rr) * E + k] : 0.f;
+        }
+        __syncthreads();
+        // past E both operands are 0: fmaf(0, 0, acc) leaves acc as it is
+#pragma unroll
+        for (int kk = 0; kk < ZS_BK; ++kk)
+        {
+            const float4 a = *reinterpret_cast<const float4 *>(&sx[kk][ty * 4]);
+            const float4 w = *reinterpret_cast<const float4 *>(&st[kk][tx * 4]);
+            const float av[4] = {a.x, a.y, a.z, a.w}, wv[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], wv[j], acc[i][j]);
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+    {
+        const int r = r0 + ty * 4 + i;
+        if (r >= R) continue;
+        const float n = nrm[ty * 4 + i];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+        {
+            const int c = c0 + tx * 4 + j;
+            if (c < C) out[(size_t)r * ldo + c] = fmaf(s, __fdiv_rn(acc[i][j], n), b);
+        }
     }
 }
 

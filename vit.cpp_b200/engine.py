@@ -55,6 +55,15 @@ class TextArch(C.Structure):
         ("logit_scale", C.c_float), ("logit_bias", C.c_float)]
 
 
+class ZeroShot(C.Structure):
+    """vitb200_zero_shot (include/vitb200.h): a zero-shot head over class embeddings [n_classes][E]."""
+    _fields_ = [("class_embeds", C.c_void_p), ("n_classes", C.c_int32), ("logit_scale", C.c_float), ("logit_bias", C.c_float),
+                ("mode", C.c_int32)]
+
+
+ZERO_SHOT_MODES = ("softmax", "sigmoid")  # vitb200_zero_shot.mode: CLIP, SigLIP
+
+
 class Taps(C.Structure):
     _fields_ = [("layer", C.c_int32)] + [(n, C.c_void_p) for n in
                                          ("embed", "ln1", "qkv", "attn", "x1", "ln2", "h", "x2", "final_ln", "x_final")]
@@ -105,6 +114,10 @@ def lib():
         L.vitb200_test_attention_hilo_causal.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_set_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
         L.vitb200_get_image_proc.argtypes = [vp, C.POINTER(ImageProc)]
+        L.vitb200_set_zero_shot.argtypes = [vp, C.POINTER(ZeroShot)]
+        L.vitb200_get_zero_shot.argtypes = [vp, vp, vp, vp, vp]
+        L.vitb200_num_outputs.argtypes = [vp]
+        L.vitb200_test_zero_shot.argtypes = [i32, i32, i32, i32, vp, vp, C.c_float, C.c_float, i32, i32, vp, vp, vp, vp]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
         L.vitb200_test_gemm_fp8.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
         L.vitb200_test_layernorm_fp8.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
@@ -166,6 +179,7 @@ class VitModel:
         self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
         self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or SwiGLU's F
         self._labels = None
+        self._zero_shot_labels = None
         ta = TextArch()
         # a text tower (vitb200_create_text): text_arch as a dict of ggml_file.TEXT_FIELDS plus its activation; None for an image tower
         self.text_arch = None
@@ -210,12 +224,56 @@ class VitModel:
                       (C.c_float * 3)(*d["std"]))
         _check(lib().vitb200_set_image_proc(self._h, C.byref(p)), "vitb200_set_image_proc")
 
+    @property
+    def n_outputs(self) -> int:
+        """Per-row width of probs and logits (vitb200_num_outputs): the zero-shot head's class count while one is set, else num_classes."""
+        return lib().vitb200_num_outputs(self._h)
+
+    @property
+    def zero_shot(self) -> Optional[dict]:
+        """The zero-shot head as set (vitb200_get_zero_shot): {"n_classes", "logit_scale", "logit_bias" (None for none), "probs"}; None when
+        no head is set."""
+        n, sc, b, mode = C.c_int32(), C.c_float(), C.c_float(), C.c_int32()
+        _check(lib().vitb200_get_zero_shot(self._h, C.byref(n), C.byref(sc), C.byref(b), C.byref(mode)), "vitb200_get_zero_shot")
+        if n.value == 0:
+            return None
+        return {"n_classes": n.value, "logit_scale": sc.value, "logit_bias": None if b.value != b.value else b.value,
+                "probs": ZERO_SHOT_MODES[mode.value]}
+
+    def set_zero_shot(self, class_embeds, logit_scale: Optional[float] = None, logit_bias: Optional[float] = None, probs: str = "softmax",
+                      labels=None):
+        """Classify against class embeddings on the GPU (vitb200_set_zero_shot): class_embeds [C, E] (E = num_classes, the projection
+        width), usually vit_encode_text's embeds or the mean of several prompt templates per class, normalised by the engine.  Every
+        prediction call then returns HF's logits_per_image over the C classes, exp(logit_scale) * cos + logit_bias, with probs "softmax"
+        (CLIP) or "sigmoid" (SigLIP); logit_scale / logit_bias as the text tower stores them (text_arch).  labels: C class names that
+        labels() returns while the head is set.  class_embeds None clears the head."""
+        if class_embeds is None:
+            _check(lib().vitb200_set_zero_shot(self._h, None), "vitb200_set_zero_shot")
+            self._zero_shot_labels = None
+            return
+        if probs not in ZERO_SHOT_MODES:
+            raise ValueError(f"probs must be one of {ZERO_SHOT_MODES}, not {probs!r}")
+        if logit_scale is None:
+            raise ValueError("logit_scale is required with class_embeds")
+        T = np.ascontiguousarray(class_embeds, np.float32)
+        if T.ndim != 2 or T.shape[1] != self.num_classes:
+            raise ValueError(f"class_embeds must be [classes, {self.num_classes}], not {list(T.shape)}")
+        if labels is not None and len(labels) != T.shape[0]:
+            raise ValueError(f"{len(labels)} labels for {T.shape[0]} classes")
+        z = ZeroShot(T.ctypes.data, T.shape[0], float(logit_scale), float("nan") if logit_bias is None else float(logit_bias),
+                     ZERO_SHOT_MODES.index(probs))
+        _check(lib().vitb200_set_zero_shot(self._h, C.byref(z)), "vitb200_set_zero_shot")
+        self._zero_shot_labels = None if labels is None else [str(x) for x in labels]
+
     def label(self, i: int) -> Optional[str]:
         s = lib().vitb200_label(self._h, i)
         return s.decode() if s else None
 
     def labels(self) -> Optional[list]:
-        """id2label as a list indexed by class id; None unless the model file names every class."""
+        """id2label as a list indexed by class id; None unless the model file names every class.  While a zero-shot head is set: the
+        labels given to set_zero_shot (None if none were)."""
+        if self.in_chans and self.zero_shot is not None:
+            return self._zero_shot_labels
         if self._labels is None:
             self._labels = [self.label(i) for i in range(self.num_classes)]
         return None if any(s is None for s in self._labels) else self._labels
@@ -310,8 +368,8 @@ def vit_predict(model: VitModel, images: np.ndarray, topk: int = 5, want_logits:
     B = imgs.shape[0]
     assert imgs.size == B * model.img_size * model.img_size * ch, imgs.shape
     lead = (B,) if model.head_tokens == 1 else (B, model.head_tokens)
-    probs = np.empty(lead + (model.num_classes,), np.float32)
-    logits = np.empty(lead + (model.num_classes,), np.float32) if want_logits else None
+    probs = np.empty(lead + (model.n_outputs,), np.float32)
+    logits = np.empty(lead + (model.n_outputs,), np.float32) if want_logits else None
     idx = np.empty(lead + (topk,), np.int32)
     val = np.empty(lead + (topk,), np.float32)
     _check(lib().vitb200_forward(model.handle, imgs.ctypes.data, B, probs.ctypes.data,
@@ -325,8 +383,8 @@ def vit_predict_sharded(models, images: np.ndarray, topk: int = 5):
     vit_predict: a ViTSTR model (head_tokens = n) returns probs[B,n,C], topk[B,n,k]; all engines must hold the same model."""
     imgs = np.ascontiguousarray(images, dtype=np.float32)
     B = imgs.shape[0]
-    nc, ht = models[0].num_classes, models[0].head_tokens
-    if any(m.head_tokens != ht or m.num_classes != nc or m.in_chans != models[0].in_chans for m in models):
+    nc, ht = models[0].n_outputs, models[0].head_tokens
+    if any(m.head_tokens != ht or m.n_outputs != nc or m.in_chans != models[0].in_chans for m in models):
         raise VitB200Error("vit_predict_sharded: the engines hold different models")
     assert imgs.size == B * models[0].img_size * models[0].img_size * models[0].in_chans, imgs.shape
     lead = (B,) if ht == 1 else (B, ht)
@@ -370,8 +428,8 @@ def vit_image_preprocess_predict(model: VitModel, images_u8, bilinear: bool = Fa
     _, B, ptrs, nx, ny = _u8_batch(images_u8)
     S = model.img_size
     f32 = np.empty((B, S, S, 3), np.float32)
-    probs = np.empty((B, model.num_classes), np.float32) if predict else None
-    logits = np.empty((B, model.num_classes), np.float32) if predict else None
+    probs = np.empty((B, model.n_outputs), np.float32) if predict else None
+    logits = np.empty((B, model.n_outputs), np.float32) if predict else None
     idx = np.empty((B, topk), np.int32) if predict else None
     val = np.empty((B, topk), np.float32) if predict else None
     _check(lib().vitb200_forward_u8(model.handle, ptrs, nx, ny, B, int(bilinear), f32.ctypes.data,
@@ -491,7 +549,8 @@ def vit_encode_text(model: VitModel, ids, layers=None, norm: bool = True, tokens
 
 def zero_shot_logits(image_embeds, text_embeds, logit_scale: float, logit_bias: Optional[float] = None) -> np.ndarray:
     """Hugging Face's logits_per_image on the host: both embeddings L2-normalised, exp(logit_scale) * img @ txt.T, + logit_bias for
-    SigLIP.  image_embeds [I, E], text_embeds [T, E] -> [I, T] (float64)."""
+    SigLIP.  image_embeds [I, E], text_embeds [T, E] -> [I, T] (float64).  The float64 check of VitModel.set_zero_shot, which computes
+    the same scores on the GPU."""
     img = np.asarray(image_embeds, np.float64)
     txt = np.asarray(text_embeds, np.float64)
     img = img / np.linalg.norm(img, axis=-1, keepdims=True)
@@ -516,8 +575,8 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
         imgs = imgs[None]
     B = imgs.shape[0]
     lead = (B,) if model.head_tokens == 1 else (B, model.head_tokens)
-    probs = np.empty(lead + (model.num_classes,), np.float32)
-    logits = np.empty(lead + (model.num_classes,), np.float32)
+    probs = np.empty(lead + (model.n_outputs,), np.float32)
+    logits = np.empty(lead + (model.n_outputs,), np.float32)
     tp = Taps()
     tp.layer = tap_layer
     out = {}
@@ -606,6 +665,25 @@ def test_softmax_topk(logits: np.ndarray, k: int, device: int = 0):
     _check(lib().vitb200_test_softmax_topk(device, rows, C, k, x.ctypes.data, probs.ctypes.data, idx.ctypes.data if k else None,
                                            val.ctypes.data if k else None), "vitb200_test_softmax_topk")
     return probs, idx, val
+
+
+def test_zero_shot(x, class_embeds, logit_scale: float, logit_bias: Optional[float] = None, probs: str = "softmax", k: int = 0,
+                   device: int = 0):
+    """The zero-shot head's kernels alone (vitb200_test_zero_shot): head rows x float32 [rows][E], raw class rows [C][E] -> (probs
+    float32 [rows][C], scores float32 [rows][C], topk_idx int32 [rows][k], topk_val float32 [rows][k])."""
+    X = np.ascontiguousarray(x, np.float32)
+    T = np.ascontiguousarray(class_embeds, np.float32)
+    rows, E = X.shape
+    n = T.shape[0]
+    pr = np.empty((rows, n), np.float32)
+    lg = np.empty((rows, n), np.float32)
+    idx = np.empty((rows, k), np.int32)
+    val = np.empty((rows, k), np.float32)
+    _check(lib().vitb200_test_zero_shot(device, rows, E, n, X.ctypes.data, T.ctypes.data, float(logit_scale),
+                                        float("nan") if logit_bias is None else float(logit_bias), ZERO_SHOT_MODES.index(probs), k,
+                                        pr.ctypes.data, lg.ctypes.data, idx.ctypes.data if k else None, val.ctypes.data if k else None),
+           "vitb200_test_zero_shot")
+    return pr, lg, idx, val
 
 
 def test_dequant(ggml_type: int, blocks: np.ndarray) -> np.ndarray:
