@@ -59,9 +59,12 @@ typedef struct vitb200_tensor
  * image in vit_predict (graph build x2, ggml_allocr, thread pool; vit.cpp:1009-1036).
  * Accepted shapes (every create function; anything else fails here, with a message naming the limit, not in the first forward):
  *   head dim 64 or 80 (hidden_size = 64 or 80 * num_attention_heads), hidden_size <= 2048 (the widest LayerNorm row a warp holds);
- *   head dim 80 (ViT-H/14) without the attention-pooling head (vitb200_arch.pool = 2, whose kernel is 64 columns wide);
- *   patch_size 8, 14, 16 or 32 for 3-channel input, 8 or 16 for 1-channel input, dividing img_size;
- *   at most 896 tokens at head dim 64 and 640 at head dim 80, (img_size / patch_size)^2 + 1 (K and V of one attention head in 227 KB of
+ *   head dim 72 (SigLIP So400m) with the SigLIP pools 2 and 3 only (vitb200_create_arch) and in SigLIP text towers;
+ *   head dim 80 (ViT-H/14) without the attention-pooling head (vitb200_arch.pool = 2, whose kernel is 64 or 72 columns wide);
+ *   patch_size 8, 14, 16 or 32 for 3-channel input, 8 or 16 for 1-channel input, dividing img_size (with pools 2 and 3 it need not: the
+ *   grid is then G = floor(img_size / patch_size), as HF's valid-padding conv takes it; with patch size 8, 16 or 32, whose patch
+ *   embedding reads pixel rows in 16-byte loads, such an img_size must then be a multiple of 4);
+ *   at most 896 tokens at head dim 64, 800 at head dim 72 and 640 at head dim 80, G^2 + 1 (K and V of one attention head in 227 KB of
  *   shared memory). */
 int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                    vitb200_engine **out);
@@ -122,17 +125,23 @@ typedef struct vitb200_arch
                           * 2 'map': the attention-pooling head (HF SiglipMultiheadAttentionPoolingHead, timm AttentionPoolLatent): one learned
                           *   probe 'attn_pool.latent' [1, 1, D], q = latent Wq^T + bq ('attn_pool.q.*', computed once at load in f64, kept
                           *   in f32), attends per head over k | v = LN(rows) Wkv^T + bkv ('attn_pool.kv.*' [2 D, D], rows k then v; LN = the
-                          *   final LayerNorm) with softmax(q k / 8) in f32; h = out_proj ('attn_pool.proj.*'); pooled = h + fc2(act(fc1(
-                          *   LN_head(h)))) ('attn_pool.norm.*', 'attn_pool.mlp.fc1.*' [4 D, D], 'attn_pool.mlp.fc2.*'), f32.  The head reads
+                          *   final LayerNorm) with softmax(q k / sqrt(hd)) in f32 (1 / 8 at head dim 64, f32(1 / sqrtf(72)) at 72); h =
+                          *   out_proj ('attn_pool.proj.*'); pooled = h + fc2(act(fc1(LN_head(h)))) ('attn_pool.norm.*', 'attn_pool.mlp.fc1.*'
+                          *   [F, D], 'attn_pool.mlp.fc2.*' [D, F], F the blocks' MLP width), f32.  The head reads
                           *   f16(pooled): HF's pooler_output.  f16 operands and f32 accumulation in the f16 and FP8 engines alike.
-                          * 3 'mean': the head reads the mean over all P rows of LN(row): SiglipForImageClassification's classifier input. */
+                          * 3 'mean': the head reads the mean over all P rows of LN(row): SiglipForImageClassification's classifier input.
+                          * With pools 2 and 3 the MLP width F is read from block 0's 'mlp.fc1.weight' [F][D] (So400m: 4304) with SwiGLU's checks,
+                          * img_size need not be a multiple of patch_size (So400m at 384 px: a 27 x 27 grid, P = 729; at patch size 8, 16 or 32
+                          * it must then be a multiple of 4), and images still arrive
+                          * img_size x img_size: the pixels past G patch_size in each direction are read by no patch. */
 } vitb200_arch;
 /* vitb200_create_ex (fp8 = 0) or vitb200_create_fp8 (fp8 = 1) for a model of architecture `arch` (NULL = all zero, the reference).
  * Fields out of range, activation = 3 with pool 0 or 1, activation = 4 with pool 2 or 3, activation = 4 with an odd fc1 row count, an
  * F that is not a multiple of 8 or outside 8..8 D, or a block whose fc1 or fc2 disagrees with F, pre_norm = 1 without both norm_pre tensors, layer_scale = 1 without every
  * ls1 / ls2 gamma, reg_tokens > 0 without 'reg_token', pool > 0 with head_tokens > 1, pool 2 or 3 with a 'cls_token' tensor, with
  * reg_tokens > 0 or with a 'pos_embed' of other than P rows, pool 2 without one of its 13 'attn_pool.*' tensors, and a head whose K is
- * not D (pools 0, 2, 3) or 2 D (pool 1) fail here before the device is touched; so does N > 896 tokens, registers included.  Every entry
+ * not D (pools 0, 2, 3) or 2 D (pool 1) fail here before the device is touched, and so do an 'attn_pool.mlp.fc1' / 'fc2' whose width is not
+ * the blocks' F and N above the head dim's token limit (896, 800 at 72, 640 at 80), registers included.  Every entry
  * point works on such an engine; the u8 entry points keep vit.cpp's preprocessing unless an image processor is set
  * (vitb200_set_image_proc: Hugging Face's CLIP, SigLIP and DINOv2 preprocessing).  The launch count of one forward is 3 + 7 L + 3 for pools 0 and 1, plus 1 with the
  * pre-norm (the pool of pool = 1 replaces the head rows' LayerNorm); 2 + 7 L + 3 for pool 3 (no class-row kernel); 2 + 7 L + 10 for
@@ -149,7 +158,8 @@ int vitb200_get_arch(const vitb200_engine *e, vitb200_arch *out);
 int vitb200_fp8(const vitb200_engine *e);         /* 1 for an FP8 engine, else 0 */
 int vitb200_in_chans(const vitb200_engine *e);    /* 3, or 1 for a ViTSTR model */
 int vitb200_head_tokens(const vitb200_engine *e); /* classifier rows per image */
-int vitb200_mlp_dim(const vitb200_engine *e);     /* the MLP's hidden width: F with activation 4 (SwiGLU), else 4 D */
+int vitb200_mlp_dim(const vitb200_engine *e);     /* the MLP's hidden width: F with activation 4 (SwiGLU), pools 2 and 3 and SigLIP text
+                                                   * towers, else 4 D */
 
 void vitb200_destroy(vitb200_engine *e);
 
@@ -341,7 +351,8 @@ int vitb200_features_u8(vitb200_engine *e, const uint8_t *const *images, const i
  * hp: hidden_size, num_hidden_layers, num_attention_heads, eps and ftype as for images; num_classes = E, the projection width (the head's
  * rows); patch_size and img_size must be 0.  Tensors: 'token_embd.weight' [V][D] (any weight format, stored f16), 'pos_embed' [1][N][D] f32,
  * 'blocks.*' as for images, 'norm.*' (the final LayerNorm), 'head.weight' [E][D] and 'head.bias' [E] (zeros for CLIP's projection; the
- * identity for CLIPTextModel).  The image checks apply (head dim 64, D <= 2048, MLP 4 D, unique names, shapes); context must equal the
+ * identity for CLIPTextModel).  The image checks apply (head dim 64, D <= 2048, MLP 4 D, unique names, shapes), except that a bidirectional
+ * (SigLIP, causal = 0) tower may have head dim 72 (So400m) and reads its MLP width F from the weights as pools 2 and 3 do; context must equal the
  * 'pos_embed' rows and be at most 224 and V >= 1.  Anything else fails before the device is touched, naming the limit.
  * A GGUF file is a text tower when it has the key vit.text.context_length; it then carries vit.text.causal (bool or integer),
  * vit.text.pool ("eos", "eos_argmax" or "last"; any other string fails the load), vit.text.eos_token_id (integer) and optionally
@@ -416,7 +427,7 @@ typedef struct vitb200_taps
     float *attn;     /* [batch][N][D]  */
     float *x1;       /* [batch][N][D]  */
     float *ln2;      /* [batch][N][D]  */
-    float *h;        /* [batch][N][F]  the MLP's hidden activations, F = vitb200_mlp_dim (4 D but with SwiGLU) */
+    float *h;        /* [batch][N][F]  the MLP's hidden activations, F = vitb200_mlp_dim */
     float *x2;       /* [batch][N][D]  */
     float *final_ln; /* [batch][D]     the head's f16 input ([batch][2 D] with vitb200_arch.pool = 1; the pooled row with pool 2, 3) */
     float *x_final;  /* [batch][N][D]  */
@@ -487,12 +498,18 @@ int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const ui
  * f16 values of qkv_hi when qkv_lo is NULL (as the engine runs it above 224 tokens).  hd 64 runs vitb200_test_attention's kernels, with
  * the lo halves when qkv_lo is given (kernel 0 or 2). */
 int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+/* The same for head dim 72 (SigLIP So400m), which vitb200_test_attention_hd refuses: qkv_hi = f16 bits [B*N][3*H*72], out = float32
+ * [B*N][H*72], 1 <= N <= 800; split precision with qkv_lo (N <= 224), the f16 values of qkv_hi without it. */
+int vitb200_test_attention_hd72(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 
 /* Stand-alone run of the attention-pooling head's attention kernel (vitb200_arch.pool = 2) through the engine's launcher: one query
  * q float32 [H*64] (the probe's, scaled by 1/8 inside) per head against the P key rows of each image; kv = f16 bits [B*P][2*H*64], every
  * row k then v (what the k | v GEMM computes), out = float32 [B][H*64] = the f16 result sum_j softmax_j(q_h k_j / 8) v_j, widened.
  * 1 <= P <= 896. */
 int vitb200_test_attention_pool(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out);
+/* The same at head dim 72: q float32 [H*72] (scaled by f32(1 / sqrtf(72)) inside), kv = f16 bits [B*P][2*H*72], every row k then v, as
+ * the engine's k | v GEMM leaves it for this head dim, out = float32 [B][H*72].  1 <= P <= 800. */
+int vitb200_test_attention_pool_hd72(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out);
 
 /* Stand-alone run of the classifier's soft-max + top-k kernel, launched as the forward launches it (the working row in shared memory
  * up to 227 KB of classes, in global scratch beyond): logits float32 [rows][C] (dense) are copied into rows of pitch round_up(C, 4),

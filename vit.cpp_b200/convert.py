@@ -166,10 +166,12 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
         raise ValueError("LayerScale, register tokens or another pool need --container gguf: a legacy ggml file carries the reference's "
                          "architecture only")
     if img_size is not None:
+        # pools 'map' and 'mean' (SigLIP) take the floor grid of a size the patch does not divide, as HF's valid conv does
         P = int(sd["patch_embed.proj.weight"].shape[2])
-        if img_size % P:
+        if img_size % P and pool not in ("map", "mean"):
             raise ValueError(f"img_size {img_size} is not a multiple of the patch size {P}")
-        sd = dict(sd, pos_embed=resample_pos_embed(sd["pos_embed"], 1 + R, img_size // P, antialias))
+        prefix = 1 + R if "cls_token" in sd else 0
+        sd = dict(sd, pos_embed=resample_pos_embed(sd["pos_embed"], prefix, img_size // P, antialias))
     if activation not in gf.ARCH_ACTIVATIONS:
         raise ValueError(f"activation {activation!r} unknown ({', '.join(gf.ARCH_ACTIVATIONS)})")
     if container != "gguf" and (keep_norm_pre or activation != "gelu_tanh" or eps != 1e-6):
@@ -180,6 +182,7 @@ def state_dict_to_model_file(sd: Dict[str, np.ndarray], out_path: str, ftype: in
     if keep_norm_pre and not ("norm_pre.weight" in sd and "norm_pre.bias" in sd):
         raise ValueError("keep_norm_pre: the state_dict has no norm_pre.weight / norm_pre.bias")
     hidden, layers, heads, classes, patch, img, in_chans = infer_hparams(sd, heads)
+    img = img if img_size is None else img_size
     id2label = id2label or {i: f"LABEL_{i}" for i in range(classes)}   # convert-pth-to-ggml.py:95-96 fallback names
     vf = gf.VitFile(hidden, layers, heads, classes, patch, img, ftype, dict(id2label), eps=eps, pre_norm=int(keep_norm_pre),
                     activation=activation, layer_scale=layer_scale, reg_tokens=R, pool=pool,
@@ -374,11 +377,18 @@ def siglip_to_timm(sd: Dict[str, np.ndarray], config: dict):
     pw = v["embeddings.patch_embedding.weight"]                          # (D, C, P, P)
     D = int(pw.shape[0])
     heads = int(vc.get("num_attention_heads", D // 64))
-    if D % heads or D // heads != 64:
-        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
-    inter = int(vc.get("intermediate_size", 4 * D))
-    if inter != 4 * D:
-        raise ValueError(f"intermediate_size {inter} is not supported (4 x hidden = {4 * D} only)")
+    if D % heads or D // heads not in (64, 72):
+        raise ValueError(f"head dim {D / heads:g} is not supported (64, or 72 as So400m)")
+    # the MLP width from the weights (So400m: 4304, not 4 D); a config that states another is refused
+    F = int(v["encoder.layers.0.mlp.fc1.weight"].shape[0])
+    inter = int(vc.get("intermediate_size", F))
+    if inter != F:
+        raise ValueError(f"intermediate_size {inter} is not supported: the weights' mlp.fc1 has {F} rows")
+    # the input size: a patch that does not divide it drops the last pixel rows and columns (So400m at 384 px, 14-px patches: 27 x 27)
+    P = int(pw.shape[2])
+    n_pos = int(v["embeddings.position_embedding.weight"].shape[0])
+    if "image_size" in vc and n_pos != (int(vc["image_size"]) // P) ** 2:
+        raise ValueError(f"image_size {vc['image_size']}: {n_pos} position rows, not ({vc['image_size']} // {P})^2")
     classifier = "classifier.weight" in sd
     if not classifier and not vc.get("vision_use_head", True):
         raise ValueError("vision_use_head = false is not supported without a classifier: the tower's pooled output is its attention-pooling "
@@ -389,8 +399,8 @@ def siglip_to_timm(sd: Dict[str, np.ndarray], config: dict):
     hf_name = {"norm1": "layer_norm1", "attn.proj": "self_attn.out_proj", "norm2": "layer_norm2", "mlp.fc1": "mlp.fc1", "mlp.fc2": "mlp.fc2"}
     for i in range(layers):
         h, t = f"encoder.layers.{i}.", f"blocks.{i}."
-        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
-            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        if v[h + "mlp.fc1.weight"].shape[0] != F:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} in block {i} is not supported (block 0's is {F})")
         for dst in ("norm1", "attn.qkv", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"):  # timm's state_dict order
             for p in ("weight", "bias"):
                 if dst == "attn.qkv":  # rows [q; k; v]
@@ -415,13 +425,16 @@ def siglip_to_timm(sd: Dict[str, np.ndarray], config: dict):
 def siglip_to_model_file(sd: Dict[str, np.ndarray], config: dict, out_path: str, ftype: int = 1, id2label: Optional[Dict[int, str]] = None,
                          container: str = "gguf", image_proc: Optional[dict] = None) -> None:
     """A Hugging Face SigLIP vision tower -> GGUF model file (no class token, gelu_pytorch_tanh, the config's eps; pool 'map' or, with a
-    classifier, 'mean')."""
+    classifier, 'mean').  img_size is the config's image_size (So400m-384: 384 with a 27 x 27 grid of 14-px patches), or the grid's
+    pixels without one."""
     if container != "gguf":
         raise ValueError("a SigLIP tower needs --container gguf: a legacy ggml file carries the reference's architecture only")
     tsd, heads, activation, eps, pool = siglip_to_timm(sd, config)
     if id2label is None and "id2label" in config and "classifier.weight" in sd:
         id2label = {int(k): str(x) for k, x in config["id2label"].items()}
-    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool, image_proc=image_proc)
+    img = config.get("vision_config", config).get("image_size")
+    state_dict_to_model_file(tsd, out_path, ftype, heads, id2label, "gguf", activation=activation, eps=eps, pool=pool,
+                             img_size=None if img is None else int(img), image_proc=image_proc)
 
 
 # Hugging Face text activations -> the file's; HF's "gelu" is the erf form
@@ -446,8 +459,10 @@ def text_to_timm(sd: Dict[str, np.ndarray], config: dict):
     tok = v["embeddings.token_embedding.weight"]                         # (V, D)
     D = int(tok.shape[1])
     heads = int(tc.get("num_attention_heads", D // 64))
-    if D % heads or D // heads != 64:
-        raise ValueError(f"head dim {D / heads:g} is not supported (64 only)")
+    if D % heads or D // heads not in ((64, 72) if siglip else (64,)):
+        raise ValueError(f"head dim {D / heads:g} is not supported (64; 72 in SigLIP towers)")
+    # CLIP's MLP is 4 D; SigLIP's width is read from the weights (So400m: 4304)
+    F = int(v["encoder.layers.0.mlp.fc1.weight"].shape[0]) if siglip else 4 * D
     pos = v["embeddings.position_embedding.weight"]                      # (N, D)
     if pos.shape[0] > MAX_TEXT_CONTEXT:
         raise ValueError(f"context {pos.shape[0]} is not supported (at most {MAX_TEXT_CONTEXT} tokens)")
@@ -456,8 +471,9 @@ def text_to_timm(sd: Dict[str, np.ndarray], config: dict):
     hf_name = {"norm1": "layer_norm1", "attn.proj": "self_attn.out_proj", "norm2": "layer_norm2", "mlp.fc1": "mlp.fc1", "mlp.fc2": "mlp.fc2"}
     for i in range(layers):
         h, t = f"encoder.layers.{i}.", f"blocks.{i}."
-        if v[h + "mlp.fc1.weight"].shape[0] != 4 * D:
-            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (4 x hidden = {4 * D} only)")
+        if v[h + "mlp.fc1.weight"].shape[0] != F:
+            raise ValueError(f"intermediate size {v[h + 'mlp.fc1.weight'].shape[0]} is not supported (" +
+                             (f"block 0's is {F})" if siglip else f"4 x hidden = {4 * D} only)"))
         for dst in ("norm1", "attn.qkv", "attn.proj", "norm2", "mlp.fc1", "mlp.fc2"):
             for p in ("weight", "bias"):
                 if dst == "attn.qkv":  # rows [q; k; v]

@@ -705,6 +705,10 @@ PatchifyKernel patchify_kernel(int P, int C)
     return nullptr;
 }
 inline bool patchify_supports(int P, int C) { return patchify_kernel(P, C) != nullptr; }
+// Whether the patchify kernel of patch size P reads pixel rows in 16-byte loads (patchify16_warp_kernel, and patchify_f16_kernel's
+// float4 path, taken when P % 4 == 0): the row starts (b S + y) S C floats must then be 16-byte aligned, i.e. img_size % 4 == 0.  A
+// patch that divides img_size guarantees it; the floor grid of pools 2 and 3 does not.
+inline bool patchify_reads_16b(int P) { return P % 4 == 0; }
 inline const char *patchify_sizes(int C) { return C == 1 ? "8, 16" : "8, 14, 16, 32"; }
 
 int launch_patchify(vitb200_engine *e, const float *img, __half *A, int B, cudaStream_t s)
@@ -814,7 +818,8 @@ int resid_epilogue(const vitb200_engine *e) { return e->arch.layer_scale ? EPI_B
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
 // token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision; ATT_MMA16 = the mma.sync kernel with 16 warps,
 // 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.  Head dim 80 has one kernel,
-// ATT_MMA80 = attention_hd80_kernel (split precision up to 224 tokens, f16 operands beyond), which ATT_AUTO picks for it.
+// ATT_MMA80 = attention_rowmajor_kernel<80> (split precision up to 224 tokens, f16 operands beyond), which ATT_AUTO picks for it.
+// Head dim 72 runs attention_rowmajor_kernel<72> alike, through ATT_AUTO only.
 enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3, ATT_MMA80 = 4 };
 constexpr int ATT_MAX_KEYS_16 = 640;
 
@@ -847,33 +852,41 @@ constexpr int attention_smem_bytes(int N) { return 2 * ((N + ATT_KC - 1) / ATT_K
 constexpr int ATT_MAX_TOKENS = kSmemOptinMax / (2 * 128) / ATT_KC * ATT_KC;
 static_assert(attention_smem_bytes(ATT_MAX_TOKENS) <= kSmemOptinMax && attention_smem_bytes(ATT_MAX_TOKENS + 1) > kSmemOptinMax);
 
-// attention_hd80_kernel holds K and V (and, split, their lo halves) of one problem in rows of ATT80_ROW_BYTES, N padded to whole key
-// chunks.  Its f16 form bounds the token count of a head-dim-80 model; the split form runs up to ATTW_KEYS tokens.
-constexpr int attention_hd80_smem_bytes(int N, bool split) { return (split ? 4 : 2) * ((N + ATT_KC - 1) / ATT_KC * ATT_KC) * ATT80_ROW_BYTES; }
+// attention_rowmajor_kernel holds K and V (and, split, their lo halves) of one problem in rows of att_row_bytes(hd), N padded to whole
+// key chunks.  Its f16 form bounds the token count of a head-dim-80 or -72 model; the split form runs up to ATTW_KEYS tokens.
+constexpr int attention_rm_smem_bytes(int hd, int N, bool split) { return (split ? 4 : 2) * ((N + ATT_KC - 1) / ATT_KC * ATT_KC) * att_row_bytes(hd); }
+constexpr int attention_hd80_smem_bytes(int N, bool split) { return attention_rm_smem_bytes(ATT80_HD, N, split); }
 constexpr int ATT80_MAX_TOKENS = kSmemOptinMax / (2 * ATT80_ROW_BYTES) / ATT_KC * ATT_KC;
 static_assert(attention_hd80_smem_bytes(ATT80_MAX_TOKENS, false) <= kSmemOptinMax &&
               attention_hd80_smem_bytes(ATT80_MAX_TOKENS + 1, false) > kSmemOptinMax);
 static_assert(attention_hd80_smem_bytes(ATTW_KEYS, true) <= kSmemOptinMax);
+// head dim 72: 2 x 144 B per padded key in the f16 form, 800 tokens (So400m at 384 px: 729 tokens, padded to 736, 211 968 B)
+constexpr int ATT72_MAX_TOKENS = kSmemOptinMax / (2 * att_row_bytes(ATT72_HD)) / ATT_KC * ATT_KC;
+static_assert(ATT72_MAX_TOKENS == 800 && attention_rm_smem_bytes(ATT72_HD, ATT72_MAX_TOKENS, false) <= kSmemOptinMax &&
+              attention_rm_smem_bytes(ATT72_HD, ATT72_MAX_TOKENS + 1, false) > kSmemOptinMax);
+static_assert(attention_rm_smem_bytes(ATT72_HD, ATTW_KEYS, true) <= kSmemOptinMax);
 
 int head_dim(const vitb200_engine *e) { return e->hp.hidden_size / e->hp.num_attention_heads; }
 
 // the most tokens an image engine of head dim hd accepts
-constexpr int max_tokens(int hd) { return hd == ATT80_HD ? ATT80_MAX_TOKENS : ATT_MAX_TOKENS; }
+constexpr int max_tokens(int hd) { return hd == ATT80_HD ? ATT80_MAX_TOKENS : hd == ATT72_HD ? ATT72_MAX_TOKENS : ATT_MAX_TOKENS; }
 
-// head dim 80: split precision exactly when the qkv GEMM writes lo halves (N <= ATTW_KEYS), 8 warps; f16 operands with 16 warps
-int launch_attention_hd80(vitb200_engine *e, int B, cudaStream_t s)
+// head dims 80 and 72: split precision exactly when the qkv GEMM writes lo halves (N <= ATTW_KEYS), 8 warps; f16 operands with 16 warps
+template <int HD>
+int launch_attention_rowmajor(vitb200_engine *e, int B, cudaStream_t s)
 {
     const int N = e->N, D = e->hp.hidden_size, H = e->hp.num_attention_heads;
     const int Npad = (N + ATT_KC - 1) / ATT_KC * ATT_KC;
     const bool split = e->QKV16L != nullptr;
-    if (split && N > ATTW_KEYS) return fail("split-precision head-dim-80 attention needs N <= %d (got %d)", ATTW_KEYS, N);
-    const int smem = attention_hd80_smem_bytes(N, split);
-    if (smem > kSmemOptinMax) return fail("attention: %d tokens do not fit in shared memory (max %d at head dim 80)", N, ATT80_MAX_TOKENS);
-    const float scale = 1.0f / sqrtf((float)ATT80_HD);
+    if (split && N > ATTW_KEYS) return fail("split-precision head-dim-%d attention needs N <= %d (got %d)", HD, ATTW_KEYS, N);
+    const int smem = attention_rm_smem_bytes(HD, N, split);
+    if (smem > kSmemOptinMax)
+        return fail("attention: %d tokens do not fit in shared memory (max %d at head dim %d)", N, max_tokens(HD), HD);
+    const float scale = 1.0f / sqrtf((float)HD);
     if (split)
-        return launch(e, attention_hd80_kernel<8, true>, dim3(B * H), dim3(8 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16, e->QKV16L, e->A16, N,
-                      D, H, Npad, scale);
-    return launch(e, attention_hd80_kernel<16, false>, dim3(B * H), dim3(16 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16,
+        return launch(e, attention_rowmajor_kernel<HD, 8, true>, dim3(B * H), dim3(8 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16, e->QKV16L,
+                      e->A16, N, D, H, Npad, scale);
+    return launch(e, attention_rowmajor_kernel<HD, 16, false>, dim3(B * H), dim3(16 * 32), (size_t)smem, s, LAUNCH_PDL, e->QKV16,
                   static_cast<const __half *>(nullptr), e->A16, N, D, H, Npad, scale);
 }
 
@@ -893,7 +906,12 @@ int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_
     if (head_dim(e) == ATT80_HD)
     {
         if (kernel != ATT_AUTO && kernel != ATT_MMA80) return fail("attention kernel %d does not run head dim 80", kernel);
-        return launch_attention_hd80(e, B, s);
+        return launch_attention_rowmajor<ATT80_HD>(e, B, s);
+    }
+    if (head_dim(e) == ATT72_HD)
+    {
+        if (kernel != ATT_AUTO) return fail("attention kernel %d does not run head dim 72", kernel);
+        return launch_attention_rowmajor<ATT72_HD>(e, B, s);
     }
     if (kernel == ATT_MMA80) return fail("attention kernel %d runs head dim 80 only", kernel);
     if (kernel == ATT_AUTO) kernel = e->N <= ATTW_KEYS ? ATT_WGMMA : (e->N <= ATT_MAX_KEYS_16 ? ATT_MMA16 : ATT_MMA8);
@@ -903,13 +921,13 @@ int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_
     return launch_attention_t<8>(e, B, s);
 }
 
-// The attention-pooling head's attention (attention_pool_kernel): the probe query q [D] f32 against the k | v head-major planes kv
-// ([2 H][max_batch * N][64] f16) of B images, N = P key rows each -> out [B][D] f16
+// The attention-pooling head's attention (attention_pool_kernel): the probe query q [D] f32 against the k | v of B images, N = P key rows
+// each -> out [B][D] f16.  kv: head-major planes [2 H][max_batch * N][64] f16 at head dim 64, row-major [B * N][2 D] at head dim 72.
 int launch_attention_pool(vitb200_engine *e, const float *q, const __half *kv, __half *out, int B, cudaStream_t s)
 {
     const int P = e->N, H = e->hp.num_attention_heads;
-    return launch(e, attention_pool_kernel, dim3(B * H), dim3(APOOL_THREADS), (size_t)P * sizeof(float), s, LAUNCH_PLAIN, kv,
-                  (size_t)e->max_batch * P, q, out, P, H);
+    return launch(e, head_dim(e) == ATT72_HD ? attention_pool_kernel<ATT72_HD> : attention_pool_kernel<64>, dim3(B * H), dim3(APOOL_THREADS),
+                  (size_t)P * sizeof(float), s, LAUNCH_PLAIN, kv, (size_t)e->max_batch * P, q, out, P, H);
 }
 
 // D2H helpers for the debug taps
@@ -1132,9 +1150,10 @@ int run_map_head(vitb200_engine *e, int B, cudaStream_t s)
         if (launch_layernorm(e, e->X, (size_t)D, e->norm_w, e->norm_b, e->A16, T, s)) return 1; // post_layernorm, every token row
     }
     {
-        // k | v of every row into the head-major planes 0 .. 2 H - 1 of QKV16, as the qkv GEMM lays out k and v
+        // k | v of every row into QKV16 as the qkv GEMM lays out k and v: the head-major planes 0 .. 2 H - 1 at head dim 64, row-major
+        // [T][2 D] at head dim 72
         GemmParams kv{};
-        kv.M = T; kv.N = 2 * D; kv.K = D; kv.bias = e->pool_kv.b; kv.out = e->QKV16; kv.ldo = 2 * D; kv.headmajor = 1;
+        kv.M = T; kv.N = 2 * D; kv.K = D; kv.bias = e->pool_kv.b; kv.out = e->QKV16; kv.ldo = 2 * D; kv.headmajor = head_dim(e) == 64;
         kv.plane_rows = (size_t)e->max_batch * e->N;
         GemmParams o{};
         o.M = B; o.N = D; o.K = D; o.bias = e->pool_proj.b; o.out = e->POOL32; o.ldo = D;
@@ -1147,11 +1166,12 @@ int run_map_head(vitb200_engine *e, int B, cudaStream_t s)
         ProfScope ps(e, PK_LN, 0.0, s);
         if (launch_layernorm_rows<true>(e, e->POOL32, (size_t)D, e->pool_nw, e->pool_nb, e->A16, B, s, 0, 0)) return 1;
     }
+    // the head's MLP has the blocks' width F (4 D but for So400m-shaped towers)
     GemmParams f1{};
-    f1.M = B; f1.N = 4 * D; f1.K = D; f1.bias = e->pool_fc1.b; f1.out = e->H16; f1.ldo = 4 * D;
+    f1.M = B; f1.N = e->F; f1.K = D; f1.bias = e->pool_fc1.b; f1.out = e->H16; f1.ldo = e->F;
     GemmParams f2{};
-    f2.M = B; f2.N = D; f2.K = 4 * D; f2.bias = e->pool_fc2.b; f2.out = e->POOL32; f2.ldo = D; f2.resid = e->POOL32;
-    ProfScope ps(e, PK_POOL, 2.0 * B * 8.0 * D * D, s);
+    f2.M = B; f2.N = D; f2.K = e->F; f2.bias = e->pool_fc2.b; f2.out = e->POOL32; f2.ldo = D; f2.resid = e->POOL32;
+    ProfScope ps(e, PK_POOL, 2.0 * B * 2.0 * e->F * D, s);
     return launch_gemm(e, fc1_epilogue(e), e->tmA_D, e->pool_fc1.tm, f1, s) || launch_gemm(e, EPI_BIAS_RESID_F32, e->tmA_H, e->pool_fc2.tm, f2, s);
 }
 
@@ -1518,6 +1538,29 @@ int upload_blocks(vitb200_engine *e, const vitb200_tensor *t, int n, bool swiglu
     return upload_f32(e, t, n, "norm.weight", D, 1, 1, 1, &e->norm_w) || upload_f32(e, t, n, "norm.bias", D, 1, 1, 1, &e->norm_b);
 }
 
+// The MLP's hidden width F from block 0's fc1 ([2 F][D] with SwiGLU's gate, [F][D] otherwise): F % 8 == 0 and 8 <= F <= 8 D, and every
+// block's fc1 and fc2 ([D][F]) must agree with it.  `what` names the setting that reads F from the weights in the messages.
+int mlp_width(const vitb200_tensor *t, int n, int D, int layers, bool swiglu, const char *what, int &F)
+{
+    const vitb200_tensor *w1 = find_tensor(t, n, "blocks.0.mlp.fc1.weight");
+    if (!w1) return fail("missing tensor 'blocks.0.mlp.fc1.weight'");
+    const int64_t rows = dim_of(w1, 1), f = swiglu ? rows / 2 : rows;
+    if (swiglu && rows % 2) return fail("%s needs an even row count 2 F in 'blocks.0.mlp.fc1.weight', got %lld", what, (long long)rows);
+    if (f % 8) return fail("%s: F = %lld is not a multiple of 8", what, (long long)f);
+    if (f < 8 || f > 8 * (int64_t)D) return fail("%s: F = %lld out of range (8..%d = 8 D)", what, (long long)f, 8 * D);
+    F = (int)f;
+    for (int i = 0; i < layers; ++i)
+    {
+        const std::string p = "blocks." + std::to_string(i) + ".mlp.";
+        const vitb200_tensor *a = find_tensor(t, n, p + "fc1.weight"), *b = find_tensor(t, n, p + "fc2.weight");
+        if ((a && dim_of(a, 1) != (swiglu ? 2 : 1) * f) || (b && dim_of(b, 0) != f))
+            return fail("%s: block %d's mlp.fc1 [%lld][%lld] or mlp.fc2 [%lld][%lld] disagrees with F = %d (fc1 [%sF][D], fc2 [D][F])", what, i,
+                        a ? (long long)dim_of(a, 1) : 0ll, a ? (long long)dim_of(a, 0) : 0ll, b ? (long long)dim_of(b, 1) : 0ll,
+                        b ? (long long)dim_of(b, 0) : 0ll, F, swiglu ? "2 " : "");
+    }
+    return 0;
+}
+
 // Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
 int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
                 bool fp8, vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
@@ -1551,6 +1594,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
             return fail("vitb200_arch.pool = %d out of range for a model with a class token: pools 2 (map) and 3 (mean) read patch rows only, "
                         "and the tensor 'cls_token' is present", ar.pool);
         if (ar.reg_tokens > 0) return fail("vitb200_arch.pool = %d needs reg_tokens = 0 (got %d): its token rows are the patch rows only", ar.pool, ar.reg_tokens);
+        // the floor grid G = img_size / patch_size: a size the patch does not divide drops the last pixel rows and columns (HF's valid conv)
         const int64_t np = (int64_t)(hp->img_size / hp->patch_size) * (hp->img_size / hp->patch_size);
         const vitb200_tensor *pe = find_tensor(t, n, "pos_embed");
         if (pe && dim_of(pe, 1) != np)
@@ -1569,27 +1613,23 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         }
     if (ar.reg_tokens > 0 && !find_tensor(t, n, "reg_token"))
         return fail("vitb200_arch.reg_tokens = %d needs the tensor 'reg_token'", ar.reg_tokens);
-    // the MLP's hidden width: 4 D, or SwiGLU's F, from block 0's fc1 [2 F][D]; every block's fc1 and fc2 [D][F] must agree with it
+    // the MLP's hidden width: 4 D, or F from the weights for SwiGLU and the SigLIP towers (So400m: 4304), checked by mlp_width
     int F = 4 * hp->hidden_size;
     if (ar.activation == 4)
     {
-        const vitb200_tensor *w1 = find_tensor(t, n, "blocks.0.mlp.fc1.weight");
-        if (!w1) return fail("missing tensor 'blocks.0.mlp.fc1.weight'");
-        const int64_t rows = dim_of(w1, 1), f = rows / 2;
-        if (rows % 2) return fail("vitb200_arch.activation = 4 (swiglu) needs an even row count 2 F in 'blocks.0.mlp.fc1.weight', got %lld", (long long)rows);
-        if (f % 8) return fail("vitb200_arch.activation = 4 (swiglu): F = %lld is not a multiple of 8", (long long)f);
-        if (f < 8 || f > 8 * (int64_t)hp->hidden_size)
-            return fail("vitb200_arch.activation = 4 (swiglu): F = %lld out of range (8..%d = 8 D)", (long long)f, 8 * hp->hidden_size);
-        F = (int)f;
-        for (int i = 0; i < hp->num_hidden_layers; ++i)
-        {
-            const std::string p = "blocks." + std::to_string(i) + ".mlp.";
-            const vitb200_tensor *a = find_tensor(t, n, p + "fc1.weight"), *b = find_tensor(t, n, p + "fc2.weight");
-            if ((a && dim_of(a, 1) != 2 * f) || (b && dim_of(b, 0) != f))
-                return fail("vitb200_arch.activation = 4 (swiglu): block %d's mlp.fc1 [%lld][%lld] or mlp.fc2 [%lld][%lld] disagrees with F = %d "
-                            "(fc1 [2 F][D], fc2 [D][F])", i, a ? (long long)dim_of(a, 1) : 0ll, a ? (long long)dim_of(a, 0) : 0ll,
-                            b ? (long long)dim_of(b, 1) : 0ll, b ? (long long)dim_of(b, 0) : 0ll, F);
-        }
+        if (mlp_width(t, n, hp->hidden_size, hp->num_hidden_layers, true, "vitb200_arch.activation = 4 (swiglu)", F)) return 1;
+    }
+    else if (ar.pool >= 2)
+    {
+        const std::string what = "vitb200_arch.pool = " + std::to_string(ar.pool);
+        if (mlp_width(t, n, hp->hidden_size, hp->num_hidden_layers, false, what.c_str(), F)) return 1;
+        // the attention-pooling head's MLP has the blocks' width
+        const vitb200_tensor *a = find_tensor(t, n, "attn_pool.mlp.fc1.weight"), *b = find_tensor(t, n, "attn_pool.mlp.fc2.weight");
+        if ((a && dim_of(a, 1) != F) || (b && dim_of(b, 0) != F))
+            return fail("%s: the attention-pooling head's %s [%lld][%lld] disagrees with the blocks' F = %d (fc1 [F][D], fc2 [D][F])", what.c_str(),
+                        a && dim_of(a, 1) != F ? "'attn_pool.mlp.fc1.weight'" : "'attn_pool.mlp.fc2.weight'",
+                        a && dim_of(a, 1) != F ? (long long)dim_of(a, 1) : (long long)dim_of(b, 1),
+                        a && dim_of(a, 1) != F ? (long long)dim_of(a, 0) : (long long)dim_of(b, 0), F);
     }
     if (ar.pool && head_tokens != 1) return fail("vitb200_arch.pool = %d needs head_tokens = 1 (got %d)", ar.pool, head_tokens);
     {
@@ -1608,11 +1648,15 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
     const int in_chans = (int)(nelem(pw) / per_c);
     // shapes no kernel is built for: rejected here, where the caller can act on it, rather than by every forward call
     const int hd = hp->hidden_size / hp->num_attention_heads;
-    if (hp->hidden_size % hp->num_attention_heads != 0 || (hd != 64 && hd != ATT80_HD))
-        return fail("head dim %d not supported (64 or 80)", hd);
+    if (hp->hidden_size % hp->num_attention_heads != 0 || (hd != 64 && hd != ATT80_HD && (hd != ATT72_HD || ar.pool < 2)))
+        return fail("head dim %d not supported (64 or 80; 72 with pools 2 map and 3 mean, the SigLIP towers)", hd);
     if (hd == ATT80_HD && ar.pool == 2)
-        return fail("vitb200_arch.pool = 2 (map) not supported at head dim 80 (the attention-pooling head's kernel is 64 columns wide)");
-    if (hp->img_size % hp->patch_size != 0) return fail("img_size %d not a multiple of patch_size %d", hp->img_size, hp->patch_size);
+        return fail("vitb200_arch.pool = 2 (map) not supported at head dim 80 (the attention-pooling head's kernel is 64 or 72 columns wide)");
+    if (hp->img_size % hp->patch_size != 0 && ar.pool < 2)
+        return fail("img_size %d not a multiple of patch_size %d (only the SigLIP pools 2 and 3 take the floor grid)", hp->img_size, hp->patch_size);
+    if (hp->img_size % hp->patch_size != 0 && patchify_reads_16b(hp->patch_size) && hp->img_size % 4 != 0)
+        return fail("img_size %d not supported with patch_size %d: a floor grid needs img_size %% 4 == 0 at this patch size (16-byte loads of "
+                    "each pixel row)", hp->img_size, hp->patch_size);
     if (!patchify_supports(hp->patch_size, in_chans))
         return fail("patch size %d not supported for %d-channel input (%s)", hp->patch_size, in_chans, patchify_sizes(in_chans));
     if (hp->hidden_size > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", hp->hidden_size, LN_MAX_HIDDEN);
@@ -1667,8 +1711,8 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         (upload_linear(e, t, n, "attn_pool.kv.weight", "attn_pool.kv.bias", 2 * D, D, D, &e->pool_kv) ||
          upload_linear(e, t, n, "attn_pool.proj.weight", "attn_pool.proj.bias", D, D, D, &e->pool_proj) ||
          upload_f32(e, t, n, "attn_pool.norm.weight", D, 1, 1, 1, &e->pool_nw) || upload_f32(e, t, n, "attn_pool.norm.bias", D, 1, 1, 1, &e->pool_nb) ||
-         upload_linear(e, t, n, "attn_pool.mlp.fc1.weight", "attn_pool.mlp.fc1.bias", 4 * D, D, D, &e->pool_fc1) ||
-         upload_linear(e, t, n, "attn_pool.mlp.fc2.weight", "attn_pool.mlp.fc2.bias", D, 4 * D, 4 * D, &e->pool_fc2) ||
+         upload_linear(e, t, n, "attn_pool.mlp.fc1.weight", "attn_pool.mlp.fc1.bias", F, D, D, &e->pool_fc1) ||
+         upload_linear(e, t, n, "attn_pool.mlp.fc2.weight", "attn_pool.mlp.fc2.bias", D, F, F, &e->pool_fc2) ||
          upload_probe_query(e, t, n, D) || dev_alloc(e, &e->POOL32, (size_t)max_batch * D)))
         return 1;
 
@@ -1753,8 +1797,10 @@ int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, con
         return fail("vitb200_text_arch.activation = %d out of range (0 gelu_tanh, 1 gelu_erf, 2 quick_gelu, 3 gelu_pytorch_tanh; swiglu is "
                     "not a text tower's MLP)", a.activation);
     const int D = hp->hidden_size;
-    if (D % hp->num_attention_heads != 0 || D / hp->num_attention_heads != 64)
-        return fail("head dim %d not supported (64 only)", D / hp->num_attention_heads);
+    // head dim 72 (SigLIP So400m) runs the row-major attention kernel, which has no causal mask
+    const int hd = D / hp->num_attention_heads;
+    if (D % hp->num_attention_heads != 0 || (hd != 64 && (hd != ATT72_HD || a.causal)))
+        return fail("head dim %d not supported (64; 72 with causal = 0, the SigLIP text towers)", hd);
     if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     const vitb200_tensor *te = find_tensor(t, n, "token_embd.weight"), *pe = find_tensor(t, n, "pos_embed");
     if (!te) return fail("missing tensor 'token_embd.weight'");
@@ -1764,6 +1810,9 @@ int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, con
                     (long long)dim_of(te, 0), (long long)dim_of(te, 1), (long long)dim_of(te, 2), (long long)dim_of(te, 3));
     if (pe && dim_of(pe, 1) != a.context)
         return fail("vitb200_text_arch.context = %d, but 'pos_embed' has %lld rows", a.context, (long long)dim_of(pe, 1));
+    // the MLP's width: F from the weights for the SigLIP (bidirectional) towers, 4 D for CLIP's
+    int F = 4 * D;
+    if (!a.causal && mlp_width(t, n, D, hp->num_hidden_layers, false, "vitb200_text_arch.causal = 0", F)) return 1;
     cudaDeviceProp prop;
     if (open_device(device, prop)) return 1;
     if (max_batch < 1) return fail("max_batch must be >= 1");
@@ -1781,7 +1830,7 @@ int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, con
     e->fp8 = fp8;
     e->num_sms = prop.multiProcessorCount;
     e->N = a.context;
-    e->F = 4 * D;
+    e->F = F;
     e->C = 0;
     e->KH = D;
     e->V = (int)V;
@@ -1816,7 +1865,8 @@ int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, con
         return e4m3 ? make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, ptr, {cols, rows}, {cols}, {2 * GEMM_BK, GEMM_A_BOX_ROWS})
                     : make_tmap(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, ptr, {cols, rows}, {2 * cols}, {GEMM_BK, GEMM_A_BOX_ROWS});
     };
-    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, (cuuint64_t)e->F) || a_map(&e->tmA_C, e->CLS16, B, D) || make_attention_maps(e))
+    if (a_map(&e->tmA_D, e->A16, T, D) || a_map(&e->tmA_H, e->H16, T, (cuuint64_t)e->F) || a_map(&e->tmA_C, e->CLS16, B, D) ||
+        (hd == 64 && make_attention_maps(e)))
         return 1;
     if (fp8 && (dev_alloc(e, &e->A8, T * D) || dev_alloc(e, &e->SA, T) || a_map(&e->tmA8, e->A8, T, D, true))) return 1;
     if (cudaDeviceSynchronize() != cudaSuccess) return fail("device sync after upload failed");
@@ -2313,6 +2363,26 @@ int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const ui
     });
 }
 
+// The row-major attention kernel at head dim hd (80 or 72) on the caller's [T][3 D] hi (and lo) buffers
+int test_attention_rowmajor(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
+{
+    if (!qkv_hi || !out || B < 1 || N < 1 || H < 1 || H > 128) return fail("bad argument");
+    if (kernel != ATT_AUTO && (hd != ATT80_HD || kernel != ATT_MMA80)) return fail("attention kernel %d does not run head dim %d", kernel, hd);
+    if (N > max_tokens(hd)) return fail("%d tokens not supported (max %d at head dim %d)", N, max_tokens(hd), hd);
+    if (qkv_lo && N > ATTW_KEYS) return fail("split-precision head-dim-%d attention needs N <= %d (got %d)", hd, ATTW_KEYS, N);
+    EnginePtr owner;
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
+    e->N = N; e->hp.hidden_size = H * hd; e->hp.num_attention_heads = H; e->max_batch = B;
+    const size_t T = (size_t)B * N, D = (size_t)H * hd;
+    // the row-major [T][3 D] buffer the qkv GEMM writes at this head dim, as given; lo halves (the split form) when passed
+    if (upload(e, &e->QKV16, qkv_hi, T * 3 * D) || (qkv_lo && upload(e, &e->QKV16L, qkv_lo, T * 3 * D)) || dev_alloc(e, &e->A16, T * D))
+        return 1;
+    CUDA_TRY(cudaMemset(e->A16, 0xFF, T * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
+    if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
+    return tap_f16(out, e->A16, T * D, e->stream);
+}
+
 int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
 {
     return guarded(__func__, [&]() -> int {
@@ -2323,44 +2393,44 @@ int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int h
             return test_attention_impl(device, kernel, B, N, H, qkv_hi, qkv_lo, out);
         }
         if (hd != ATT80_HD) return fail("head dim %d not supported (64 or 80)", hd);
-        if (!qkv_hi || !out || B < 1 || N < 1 || H < 1 || H > 128) return fail("bad argument");
-        if (kernel != ATT_AUTO && kernel != ATT_MMA80) return fail("attention kernel %d does not run head dim 80", kernel);
-        if (N > ATT80_MAX_TOKENS) return fail("%d tokens not supported (max %d at head dim 80)", N, ATT80_MAX_TOKENS);
-        if (qkv_lo && N > ATTW_KEYS) return fail("split-precision head-dim-80 attention needs N <= %d (got %d)", ATTW_KEYS, N);
-        EnginePtr owner;
-        if (scratch_engine(device, owner)) return 1;
-        vitb200_engine *e = owner.get();
-        e->N = N; e->hp.hidden_size = H * hd; e->hp.num_attention_heads = H; e->max_batch = B;
-        const size_t T = (size_t)B * N, D = (size_t)H * hd;
-        // the row-major [T][3 D] buffer the qkv GEMM writes at this head dim, as given; lo halves (the split form) when passed
-        if (upload(e, &e->QKV16, qkv_hi, T * 3 * D) || (qkv_lo && upload(e, &e->QKV16L, qkv_lo, T * 3 * D)) || dev_alloc(e, &e->A16, T * D))
-            return 1;
-        CUDA_TRY(cudaMemset(e->A16, 0xFF, T * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
-        if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
-        return tap_f16(out, e->A16, T * D, e->stream);
+        return test_attention_rowmajor(device, kernel, B, N, H, hd, qkv_hi, qkv_lo, out);
     });
+}
+
+int vitb200_test_attention_hd72(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out)
+{
+    return guarded(__func__, [&]() -> int { return test_attention_rowmajor(device, ATT_AUTO, B, N, H, ATT72_HD, qkv_hi, qkv_lo, out); });
+}
+
+// The attention-pool kernel at head dim hd on the caller's q [D] and k | v rows [B * P][2 D] (head-major planes built from them at 64)
+int test_attention_pool(int device, int B, int P, int H, int hd, const float *q, const uint16_t *kv, float *out)
+{
+    if (!q || !kv || !out || B < 1 || P < 1 || P > max_tokens(hd) || H < 1 || H > 128) return fail("bad argument");
+    EnginePtr owner;
+    if (scratch_engine(device, owner)) return 1;
+    vitb200_engine *e = owner.get();
+    e->N = P; e->max_batch = B; e->hp.num_attention_heads = H; e->hp.hidden_size = H * hd;
+    const size_t T = (size_t)B * P, D = (size_t)H * hd;
+    std::vector<uint16_t> hm(kv, kv + T * 2 * D);
+    // head dim 64: the head-major planes the k | v GEMM writes ([2 H][T][64]) from the caller's [T][2 D] rows
+    for (size_t r = 0; hd == 64 && r < T; ++r)
+        for (int pl = 0; pl < 2 * H; ++pl) memcpy(&hm[((size_t)pl * T + r) * 64], kv + r * 2 * D + (size_t)pl * 64, 128);
+    float *dq = nullptr;
+    __half *dkv = nullptr, *dout = nullptr;
+    if (upload(e, &dq, q, D) || upload(e, &dkv, hm.data(), hm.size()) || dev_alloc(e, &dout, (size_t)B * D)) return 1;
+    CUDA_TRY(cudaMemset(dout, 0xFF, (size_t)B * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
+    if (run_scratch(e, "attention-pool kernel", [&] { return launch_attention_pool(e, dq, dkv, dout, B, e->stream); })) return 1;
+    return tap_f16(out, dout, (size_t)B * D, e->stream);
 }
 
 int vitb200_test_attention_pool(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out)
 {
-    return guarded(__func__, [&]() -> int {
-        if (!q || !kv || !out || B < 1 || P < 1 || P > ATT_MAX_TOKENS || H < 1 || H > 128) return fail("bad argument");
-        EnginePtr owner;
-        if (scratch_engine(device, owner)) return 1;
-        vitb200_engine *e = owner.get();
-        e->N = P; e->max_batch = B; e->hp.num_attention_heads = H; e->hp.hidden_size = H * 64;
-        const size_t T = (size_t)B * P, D = (size_t)H * 64;
-        // the head-major planes the k | v GEMM writes ([2 H][T][64]) from the caller's [T][2 D] rows
-        std::vector<uint16_t> hm(T * 2 * D);
-        for (size_t r = 0; r < T; ++r)
-            for (int pl = 0; pl < 2 * H; ++pl) memcpy(&hm[((size_t)pl * T + r) * 64], kv + r * 2 * D + (size_t)pl * 64, 128);
-        float *dq = nullptr;
-        __half *dkv = nullptr, *dout = nullptr;
-        if (upload(e, &dq, q, D) || upload(e, &dkv, hm.data(), hm.size()) || dev_alloc(e, &dout, (size_t)B * D)) return 1;
-        CUDA_TRY(cudaMemset(dout, 0xFF, (size_t)B * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
-        if (run_scratch(e, "attention-pool kernel", [&] { return launch_attention_pool(e, dq, dkv, dout, B, e->stream); })) return 1;
-        return tap_f16(out, dout, (size_t)B * D, e->stream);
-    });
+    return guarded(__func__, [&]() -> int { return test_attention_pool(device, B, P, H, 64, q, kv, out); });
+}
+
+int vitb200_test_attention_pool_hd72(int device, int B, int P, int H, const float *q, const uint16_t *kv, float *out)
+{
+    return guarded(__func__, [&]() -> int { return test_attention_pool(device, B, P, H, ATT72_HD, q, kv, out); });
 }
 
 int vitb200_test_softmax_topk(int device, int rows, int C, int k, const float *logits, float *probs, int32_t *topk_idx, float *topk_val)

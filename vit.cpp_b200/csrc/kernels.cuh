@@ -5,6 +5,7 @@
 //   cls_patch_mean_kernel    DINOv2's classifier input: LN(token 0) || the mean of LN(patch rows), one CTA per image; without a class
 //                            token (SigLIP) the mean alone
 //   attention_pool_kernel    SigLIP's attention-pooling head: one learned query attending over an image's token rows, per head
+//                            (head dims 64 and 72)
 //   token_embed_kernel       text towers: token rows = the token table's row of each id + pos_embed, replacing the patch embedding
 //   text_pool_kernel         text towers: the pooled row of each sequence (CLIP's EOS row, SigLIP's last row) through the final LayerNorm
 //   layernorm_f16_kernel     ggml_norm * w + b (ggml.c:8959-9008, vit.cpp:808-812) emitting the f16 A operand; its f32 / bf16
@@ -489,29 +490,52 @@ text_pool_kernel(const float *__restrict__ x, const int32_t *__restrict__ ids, i
 }
 
 // ------------------------------------------------------------------------------------------------
-// SigLIP's attention-pooling head (vitb200_arch.pool = 2), its attention: per (image, head), one query q_h (f32 [64], the learned probe
-// projected once at load) against the image's P key rows, o = sum_j softmax_j(q_h . k_j / 8) v_j, f32 throughout, max subtracted.  k and
-// v are the head-major planes the k | v GEMM writes ([2 H planes][plane_rows][64] f16: planes 0 .. H-1 keys, H .. 2H-1 values); only
-// rows 0 .. P-1 of the image are read, so nothing of another image reaches a sum.  o -> f16 at column 64 h of out [B][D] (merged heads).
-// HBM-bound (2 x 128 B per key, no reuse): 16-byte loads, eight lanes per key row, APOOL_CHUNK keys per CTA pass.  The score of key j is
+// SigLIP's attention-pooling head (vitb200_arch.pool = 2), its attention: per (image, head), one query q_h (f32 [HD], the learned probe
+// projected once at load) against the image's P key rows, o = sum_j softmax_j(q_h . k_j / sqrt(HD)) v_j, f32 throughout, max subtracted.
+// HD = 64: k and v are the head-major planes the k | v GEMM writes ([2 H planes][plane_rows][64] f16: planes 0 .. H-1 keys, H .. 2H-1
+// values), and the scale is the exact 1 / 8.  HD = 72 (So400m): the row-major [rows][2 D] buffer the k | v GEMM writes for that head dim,
+// head h's k at column 72 h and its v at D + 72 h (plane_rows is not read), scale f32(1 / sqrtf(72)).  Only rows 0 .. P-1 of the image
+// are read, so nothing of another image reaches a sum.  o -> f16 at column HD h of out [B][D] (merged heads).
+// HBM-bound (2 x 2 HD B per key, no reuse): 16-byte loads, eight lanes per key row, APOOL_CHUNK keys per CTA pass.  Lane seg of a key
+// row holds its columns 8 seg .. 8 seg + 7; at HD = 72 lane 0 also holds the ninth segment, columns 64 .. 71.  The score of key j is
 // its lanes' products summed in a fixed butterfly, the output column sums are added chunk row by chunk row in a fixed order, so an image
 // gives the same bits alone as in any batch.  Dynamic shared memory: P scores.
 constexpr int APOOL_THREADS = 256;
 constexpr int APOOL_CHUNK = APOOL_THREADS / 8; // key rows per pass
 
+template <int HD>
 __global__ void __launch_bounds__(APOOL_THREADS)
 attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const float *__restrict__ q, __half *__restrict__ out, int P, int H)
 {
+    static_assert(HD == 64 || HD == 72, "head dims 64 (head-major k | v) and 72 (row-major)");
+    constexpr bool kTail = HD == 72; // lane 0 of each key row takes the ninth 16-B segment
     extern __shared__ float s_score[]; // [P]
     __shared__ float s_red[APOOL_THREADS / 32];
-    __shared__ float s_part[APOOL_CHUNK][64 + 1];
+    __shared__ float s_part[APOOL_CHUNK][HD + 1];
     const int img = blockIdx.x / H, h = blockIdx.x - img * H, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int seg = tid & 7, r0 = tid >> 3; // 16-byte segment (8 columns) of a row; first key row of this thread
-    const uint4 *kp = reinterpret_cast<const uint4 *>(kv + ((size_t)h * plane_rows + (size_t)img * P) * 64);
-    const uint4 *vp = reinterpret_cast<const uint4 *>(kv + ((size_t)(H + h) * plane_rows + (size_t)img * P) * 64);
-    float qr[8];
+    // a key row's stride in 16-B segments, and segment 0 of this head's k and v in key row 0 of the image
+    const size_t ld16 = kTail ? (size_t)H * HD / 4 : 8;
+    const uint4 *kp, *vp;
+    if constexpr (kTail)
+    {
+        kp = reinterpret_cast<const uint4 *>(kv + (size_t)img * P * 2 * H * HD + (size_t)h * HD);
+        vp = kp + (size_t)H * HD / 8;
+    }
+    else
+    {
+        kp = reinterpret_cast<const uint4 *>(kv + ((size_t)h * plane_rows + (size_t)img * P) * 64);
+        vp = reinterpret_cast<const uint4 *>(kv + ((size_t)(H + h) * plane_rows + (size_t)img * P) * 64);
+    }
+    const float qscale = kTail ? 1.0f / sqrtf((float)HD) : 0.125f; // 1 / sqrt(64), exact
+    float qr[8], qt[8];
 #pragma unroll
-    for (int i = 0; i < 8; ++i) qr[i] = __ldg(q + 64 * h + 8 * seg + i) * 0.125f; // 1 / sqrt(64), exact
+    for (int i = 0; i < 8; ++i) qr[i] = __ldg(q + HD * h + 8 * seg + i) * qscale;
+    if constexpr (kTail)
+    {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) qt[i] = __ldg(q + HD * h + 64 + i) * qscale;
+    }
     // scores, and the running maximum of the keys this thread saw
     // (the whole warp takes every pass, so that its shuffles see all 32 lanes; rows past P are neither read nor scored)
     float mx = -INFINITY;
@@ -519,7 +543,7 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
     {
         const int j = j0 + r0;
         const bool live = j < P;
-        const uint4 u = live ? __ldg(kp + (size_t)j * 8 + seg) : make_uint4(0u, 0u, 0u, 0u);
+        const uint4 u = live ? __ldg(kp + (size_t)j * ld16 + seg) : make_uint4(0u, 0u, 0u, 0u);
         const __half2 *k2 = reinterpret_cast<const __half2 *>(&u);
         float d = 0.f;
 #pragma unroll
@@ -528,6 +552,21 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
             const float2 f = __half22float2(k2[i]);
             d = fmaf(qr[2 * i], f.x, d);
             d = fmaf(qr[2 * i + 1], f.y, d);
+        }
+        if constexpr (kTail)
+        {
+            if (live && seg == 0)
+            {
+                const uint4 ut = __ldg(kp + (size_t)j * ld16 + 8);
+                const __half2 *t2 = reinterpret_cast<const __half2 *>(&ut);
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                {
+                    const float2 f = __half22float2(t2[i]);
+                    d = fmaf(qt[2 * i], f.x, d);
+                    d = fmaf(qt[2 * i + 1], f.y, d);
+                }
+            }
         }
         d += __shfl_xor_sync(0xffffffffu, d, 1);
         d += __shfl_xor_sync(0xffffffffu, d, 2);
@@ -546,11 +585,11 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
 #pragma unroll
     for (int w = 1; w < APOOL_THREADS / 32; ++w) mx = fmaxf(mx, s_red[w]);
     // o = sum_j e_j v_j / sum_j e_j, e_j = exp(s_j - max): this thread's 8 columns over key rows r0, r0 + CHUNK, ...
-    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, esum = 0.f;
+    float acc[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, acc_t[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, esum = 0.f;
     for (int j = r0; j < P; j += APOOL_CHUNK)
     {
         const float e = expf(s_score[j] - mx);
-        const uint4 u = __ldg(vp + (size_t)j * 8 + seg);
+        const uint4 u = __ldg(vp + (size_t)j * ld16 + seg);
         const __half2 *v2 = reinterpret_cast<const __half2 *>(&u);
 #pragma unroll
         for (int i = 0; i < 4; ++i)
@@ -559,10 +598,33 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
             acc[2 * i] = fmaf(e, f.x, acc[2 * i]);
             acc[2 * i + 1] = fmaf(e, f.y, acc[2 * i + 1]);
         }
+        if constexpr (kTail)
+        {
+            if (seg == 0)
+            {
+                const uint4 ut = __ldg(vp + (size_t)j * ld16 + 8);
+                const __half2 *t2 = reinterpret_cast<const __half2 *>(&ut);
+#pragma unroll
+                for (int i = 0; i < 4; ++i)
+                {
+                    const float2 f = __half22float2(t2[i]);
+                    acc_t[2 * i] = fmaf(e, f.x, acc_t[2 * i]);
+                    acc_t[2 * i + 1] = fmaf(e, f.y, acc_t[2 * i + 1]);
+                }
+            }
+        }
         esum += e;
     }
 #pragma unroll
     for (int i = 0; i < 8; ++i) s_part[r0][8 * seg + i] = acc[i];
+    if constexpr (kTail)
+    {
+        if (seg == 0)
+        {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) s_part[r0][64 + i] = acc_t[i];
+        }
+    }
     __syncthreads(); // every s_red[w] has been read: it takes the exp sums next
     // the exp sum: each key row's e was added by its 8 segment lanes alike, so lanes with seg == 0 hold the sums
     float es = seg == 0 ? esum : 0.f;
@@ -570,14 +632,14 @@ attention_pool_kernel(const __half *__restrict__ kv, size_t plane_rows, const fl
     for (int o = 16; o > 0; o >>= 1) es += __shfl_xor_sync(0xffffffffu, es, o);
     if (lane == 0) s_red[warp] = es;
     __syncthreads();
-    if (tid < 64)
+    if (tid < HD)
     {
         float den = s_red[0];
 #pragma unroll
         for (int w = 1; w < APOOL_THREADS / 32; ++w) den += s_red[w];
         float o = s_part[0][tid];
         for (int r = 1; r < APOOL_CHUNK; ++r) o += s_part[r][tid];
-        out[(size_t)img * H * 64 + 64 * h + tid] = __float2half_rn(__fdiv_rn(o, den));
+        out[(size_t)img * H * HD + HD * h + tid] = __float2half_rn(__fdiv_rn(o, den));
     }
 }
 
@@ -868,35 +930,39 @@ attention_kernel(const __half *__restrict__ qkv, size_t plane_rows, __half *__re
 }
 
 // ------------------------------------------------------------------------------------------------
-// Attention for head dim 80 (ViT-H/14), every token count up to ATT80_MAX_TOKENS.  The soft-max of attention_kernel: two passes,
-// the TRUE row maximum, e = f16(exp(f16(s * scale - max))), l = sum e in f32, O = (P V) * (1 / l).  scale = 1 / sqrtf(80) is not a
-// power of two, but f32 rounding is monotone, so f32(max(s) * scale) == max(f32(s * scale)) still holds exactly.
-// qkv: the row-major [T][3 D] buffer the qkv GEMM writes for this head dim (q | k | v, head h at columns h 80, D + h 80 and
-// 2 D + h 80), out [T][D] f16.  One CTA per (image, head); it reads only the image's own N rows.  K and V live in shared memory in
-// rows of ATT80_ROW_BYTES: 160 B of data and 16 B of padding, so the 8 row starts of an ldmatrix (stride 11 x 16 B) fall in 8
-// distinct 16-B bank groups.  Rows past N are zero.  S = Q K^T is 5 k16 steps per 8-key tile, O = P V 10 n8 tiles.
+// Attention for the row-major head dims HD = 80 (ViT-H/14) and 72 (SigLIP So400m), every token count up to the engine's limit for HD
+// (ATT80_MAX_TOKENS, ATT72_MAX_TOKENS).  The soft-max of attention_kernel: two passes, the TRUE row maximum,
+// e = f16(exp(f16(s * scale - max))), l = sum e in f32, O = (P V) * (1 / l).  scale = 1 / sqrtf(HD) is not a power of two, but f32
+// rounding is monotone, so f32(max(s) * scale) == max(f32(s * scale)) still holds exactly.
+// qkv: the row-major [T][3 D] buffer the qkv GEMM writes for these head dims (q | k | v, head h at columns h HD, D + h HD and
+// 2 D + h HD), out [T][D] f16.  One CTA per (image, head); it reads only the image's own N rows.  K and V live in shared memory in
+// rows of att_row_bytes(HD) whose length in 16-B units is odd, so the 8 row starts of an ldmatrix fall in 8 distinct 16-B bank
+// groups: 80 columns take 160 B of data and 16 B of padding (stride 11 x 16 B), 72 columns 144 B and none (stride 9 x 16 B).  Rows
+// past N are zero.  S = Q K^T is HD / 16 k16 steps per 8-key tile and, at 72, one k8 step for columns 64..71; O = P V is HD / 8 n8
+// tiles, in pairs from ldmatrix_x4_trans and, at 72, a last one from ldmatrix_x2_trans.
 // SPLIT (N <= 224, like the wgmma kernel for head dim 64): qkv and qkv_lo hold hi = f16(x) and lo = f16(x - hi) of every value, and
 // S = Ql Kh^T + Qh Kl^T + Qh Kh^T, O = P Vl + P Vh (hi and lo of K and V in shared memory).  Otherwise the f16 values of qkv.
-constexpr int ATT80_HD = 80;
-constexpr int ATT80_ROW_BYTES = 176;
-constexpr int ATT80_KS = ATT80_HD / 16; // k16 steps of S = Q K^T
-constexpr int ATT80_DT = ATT80_HD / 8;  // n8 tiles of O = P V
+constexpr int ATT80_HD = 80, ATT72_HD = 72;
+__host__ __device__ constexpr int att_row_bytes(int hd) { return (hd / 8) % 2 ? 2 * hd : 2 * hd + 16; }
+constexpr int ATT80_ROW_BYTES = att_row_bytes(ATT80_HD);
+static_assert(ATT80_ROW_BYTES == 176 && att_row_bytes(ATT72_HD) == 144);
 
-template <bool SPLIT>
-__device__ __forceinline__ void att80_scores(float (&s)[ATT_KC / 8][4], const uint32_t (&qh)[ATT80_KS][4], const uint32_t (&ql)[ATT80_KS][4],
-                                             uint32_t sKh, uint32_t sKl, int kc, int lane)
+template <int HD, bool SPLIT>
+__device__ __forceinline__ void att_rm_scores(float (&s)[ATT_KC / 8][4], const uint32_t (&qh)[(HD + 15) / 16][4],
+                                              const uint32_t (&ql)[(HD + 15) / 16][4], uint32_t sKh, uint32_t sKl, int kc, int lane)
 {
+    constexpr int KS = HD / 16, ROW = att_row_bytes(HD);
 #pragma unroll
     for (int nt = 0; nt < ATT_KC / 8; ++nt) { s[nt][0] = s[nt][1] = s[nt][2] = s[nt][3] = 0.f; }
     const int mi = lane >> 3, lr = lane & 7;
 #pragma unroll
-    for (int ks = 0; ks < ATT80_KS; ++ks)
+    for (int ks = 0; ks < KS; ++ks)
     {
 #pragma unroll
         for (int ntp = 0; ntp < ATT_KC / 16; ++ntp)
         {
             const int key = kc + (2 * ntp + (mi >> 1)) * 8 + lr;
-            const uint32_t off = (uint32_t)(key * ATT80_ROW_BYTES + (ks * 2 + (mi & 1)) * 16);
+            const uint32_t off = (uint32_t)(key * ROW + (ks * 2 + (mi & 1)) * 16);
             uint32_t b0, b1, b2, b3;
             ptx::ldmatrix_x4(sKh + off, b0, b1, b2, b3);
             if constexpr (SPLIT)
@@ -912,14 +978,40 @@ __device__ __forceinline__ void att80_scores(float (&s)[ATT_KC / 8][4], const ui
             ptx::mma_m16n8k16_f16(s[2 * ntp + 1], qh[ks], b2, b3);
         }
     }
+    if constexpr (HD % 16 == 8)
+    {
+        // columns HD - 8 .. HD - 1, one k8 step per 8-key tile: lanes 0-7 give the rows of key tile 2 ntp, lanes 8-15 of tile 2 ntp + 1
+#pragma unroll
+        for (int ntp = 0; ntp < ATT_KC / 16; ++ntp)
+        {
+            const uint32_t off = (uint32_t)((kc + (2 * ntp + (mi & 1)) * 8 + lr) * ROW + KS * 32);
+            uint32_t b0, b1;
+            ptx::ldmatrix_x2(sKh + off, b0, b1);
+            if constexpr (SPLIT)
+            {
+                uint32_t c0, c1;
+                ptx::ldmatrix_x2(sKl + off, c0, c1);
+                ptx::mma_m16n8k8_f16(s[2 * ntp], ql[KS][0], ql[KS][1], b0);
+                ptx::mma_m16n8k8_f16(s[2 * ntp + 1], ql[KS][0], ql[KS][1], b1);
+                ptx::mma_m16n8k8_f16(s[2 * ntp], qh[KS][0], qh[KS][1], c0);
+                ptx::mma_m16n8k8_f16(s[2 * ntp + 1], qh[KS][0], qh[KS][1], c1);
+            }
+            ptx::mma_m16n8k8_f16(s[2 * ntp], qh[KS][0], qh[KS][1], b0);
+            ptx::mma_m16n8k8_f16(s[2 * ntp + 1], qh[KS][0], qh[KS][1], b1);
+        }
+    }
 }
 
-template <int NWARPS, bool SPLIT>
+template <int HD, int NWARPS, bool SPLIT>
 __global__ void __launch_bounds__(NWARPS * 32)
-attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__ qkv_lo, __half *__restrict__ out, int N, int D, int H, int Npad,
-                      float scale)
+attention_rowmajor_kernel(const __half *__restrict__ qkv, const __half *__restrict__ qkv_lo, __half *__restrict__ out, int N, int D, int H,
+                          int Npad, float scale)
 {
-    extern __shared__ __align__(16) uint8_t att80_smem[];
+    static_assert(HD % 8 == 0 && HD > 64 && HD <= 128, "row-major head dims: whole 16-B segments, more than the 64 of attention_kernel");
+    constexpr int ROW = att_row_bytes(HD);
+    constexpr int KQ = (HD + 15) / 16; // q fragments per row: HD / 16 k16 steps, and a k8 step for the last 8 columns when HD % 16 == 8
+    constexpr int DT = HD / 8;         // n8 tiles of O = P V
+    extern __shared__ __align__(16) uint8_t att_rm_smem[];
     // launched with programmatic dependent launch: q, k, v are read only once the qkv GEMM has completed
     ptx::grid_dep_launch();
     ptx::grid_dep_wait();
@@ -927,48 +1019,51 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     constexpr int kParts = SPLIT ? 2 : 1;
     const size_t ld = 3 * (size_t)D;                                     // row stride of qkv
-    const size_t q_off = (size_t)b * N * ld + (size_t)h * ATT80_HD;      // q of row 0 of this (image, head); k and v D and 2 D further
-    const uint32_t part_bytes = (uint32_t)Npad * ATT80_ROW_BYTES;
+    const size_t q_off = (size_t)b * N * ld + (size_t)h * HD;            // q of row 0 of this (image, head); k and v D and 2 D further
+    const uint32_t part_bytes = (uint32_t)Npad * ROW;
     // [part] K | [part] V, part 0 = hi (or the f16 values), part 1 = lo
     for (int part = 0; part < kParts; ++part)
     {
         const __half *src = (part ? qkv_lo : qkv) + q_off;
-        uint8_t *dK = att80_smem + part * part_bytes, *dV = att80_smem + (kParts + part) * part_bytes;
-        for (int idx = tid; idx < Npad * (ATT80_HD / 8); idx += NWARPS * 32)
+        uint8_t *dK = att_rm_smem + part * part_bytes, *dV = att_rm_smem + (kParts + part) * part_bytes;
+        for (int idx = tid; idx < Npad * (HD / 8); idx += NWARPS * 32)
         {
-            const int t = idx / (ATT80_HD / 8), c = idx - t * (ATT80_HD / 8);
+            const int t = idx / (HD / 8), c = idx - t * (HD / 8);
             uint4 kv = make_uint4(0, 0, 0, 0), vv = make_uint4(0, 0, 0, 0);
             if (t < N)
             {
                 kv = __ldg(reinterpret_cast<const uint4 *>(src + (size_t)t * ld + D) + c);
                 vv = __ldg(reinterpret_cast<const uint4 *>(src + (size_t)t * ld + 2 * (size_t)D) + c);
             }
-            *reinterpret_cast<uint4 *>(dK + t * ATT80_ROW_BYTES + c * 16) = kv;
-            *reinterpret_cast<uint4 *>(dV + t * ATT80_ROW_BYTES + c * 16) = vv;
+            *reinterpret_cast<uint4 *>(dK + t * ROW + c * 16) = kv;
+            *reinterpret_cast<uint4 *>(dV + t * ROW + c * 16) = vv;
         }
     }
     __syncthreads();
-    const uint32_t sKh = ptx::smem_u32(att80_smem), sKl = sKh + part_bytes;
+    const uint32_t sKh = ptx::smem_u32(att_rm_smem), sKl = sKh + part_bytes;
     const uint32_t sVh = sKh + kParts * part_bytes, sVl = sVh + part_bytes;
     const int g = lane >> 2, t4 = lane & 3;
     const int n_qtiles = (N + 15) >> 4;
     for (int qt = warp; qt < n_qtiles; qt += NWARPS)
     {
         const int r0 = qt * 16 + g, r1 = r0 + 8;
-        uint32_t qh[ATT80_KS][4], ql[ATT80_KS][4];
+        uint32_t qh[KQ][4], ql[KQ][4];
 #pragma unroll
         for (int part = 0; part < kParts; ++part)
         {
             const __half *src = (part ? qkv_lo : qkv) + q_off;
 #pragma unroll
-            for (int ks = 0; ks < ATT80_KS; ++ks)
+            for (int ks = 0; ks < KQ; ++ks)
             {
                 const int col = ks * 16 + 2 * t4;
                 uint32_t(&qa)[4] = part ? ql[ks] : qh[ks];
                 qa[0] = r0 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r0 * ld + col)) : 0u;
                 qa[1] = r1 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r1 * ld + col)) : 0u;
-                qa[2] = r0 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r0 * ld + col + 8)) : 0u;
-                qa[3] = r1 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r1 * ld + col + 8)) : 0u;
+                if (ks * 16 + 16 <= HD) // the k8 step reads a[0] and a[1] only
+                {
+                    qa[2] = r0 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r0 * ld + col + 8)) : 0u;
+                    qa[3] = r1 < N ? __ldg(reinterpret_cast<const uint32_t *>(src + (size_t)r1 * ld + col + 8)) : 0u;
+                }
             }
         }
         // ---- pass 1: true row maximum of the unscaled scores
@@ -976,7 +1071,7 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
         for (int kc = 0; kc < Npad; kc += ATT_KC)
         {
             float s[ATT_KC / 8][4];
-            att80_scores<SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
+            att_rm_scores<HD, SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
 #pragma unroll
             for (int nt = 0; nt < ATT_KC / 8; ++nt)
             {
@@ -992,14 +1087,14 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
         mx0 = __fmul_rn(mx0, scale); // == the maximum of the scaled scores (monotone rounding)
         mx1 = __fmul_rn(mx1, scale);
         // ---- pass 2: P = f16 exp(f16(s*scale - max)), l = sum P, O += P V
-        float o[ATT80_DT][4];
+        float o[DT][4];
 #pragma unroll
-        for (int dt = 0; dt < ATT80_DT; ++dt) { o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f; }
+        for (int dt = 0; dt < DT; ++dt) { o[dt][0] = o[dt][1] = o[dt][2] = o[dt][3] = 0.f; }
         float l0 = 0.f, l1 = 0.f;
         for (int kc = 0; kc < Npad; kc += ATT_KC)
         {
             float s[ATT_KC / 8][4];
-            att80_scores<SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
+            att_rm_scores<HD, SPLIT>(s, qh, ql, sKh, sKl, kc, lane);
             uint32_t pa[ATT_KC / 16][4];
 #pragma unroll
             for (int nt = 0; nt < ATT_KC / 8; ++nt)
@@ -1021,10 +1116,10 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
             for (int j = 0; j < ATT_KC / 16; ++j)
             {
 #pragma unroll
-                for (int dt = 0; dt < ATT80_DT; dt += 2)
+                for (int dt = 0; dt + 1 < DT; dt += 2)
                 {
                     const int key = kc + j * 16 + (mi & 1) * 8 + lr;
-                    const uint32_t off = (uint32_t)(key * ATT80_ROW_BYTES + (dt + (mi >> 1)) * 16);
+                    const uint32_t off = (uint32_t)(key * ROW + (dt + (mi >> 1)) * 16);
                     uint32_t b0, b1, b2, b3;
                     if constexpr (SPLIT)
                     {
@@ -1036,6 +1131,20 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
                     ptx::mma_m16n8k16_f16(o[dt], pa[j], b0, b1);
                     ptx::mma_m16n8k16_f16(o[dt + 1], pa[j], b2, b3);
                 }
+                if constexpr (DT % 2)
+                {
+                    // the last n8 tile: its 16 keys as two 8x8 matrices (lanes 0-7 and 8-15 give the row addresses)
+                    const int key = kc + j * 16 + (mi & 1) * 8 + lr;
+                    const uint32_t off = (uint32_t)(key * ROW + (DT - 1) * 16);
+                    uint32_t b0, b1;
+                    if constexpr (SPLIT)
+                    {
+                        ptx::ldmatrix_x2_trans(sVl + off, b0, b1);
+                        ptx::mma_m16n8k16_f16(o[DT - 1], pa[j], b0, b1);
+                    }
+                    ptx::ldmatrix_x2_trans(sVh + off, b0, b1);
+                    ptx::mma_m16n8k16_f16(o[DT - 1], pa[j], b0, b1);
+                }
             }
         }
         l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
@@ -1043,10 +1152,10 @@ attention_hd80_kernel(const __half *__restrict__ qkv, const __half *__restrict__
         l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
         l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
         const float inv0 = 1.0f / l0, inv1 = 1.0f / l1; // p_i = e_i * (1/sum)  (ggml.c:10556-10558)
-        __half *o0 = out + ((size_t)b * N + r0) * D + h * ATT80_HD + 2 * t4;
-        __half *o1 = out + ((size_t)b * N + r1) * D + h * ATT80_HD + 2 * t4;
+        __half *o0 = out + ((size_t)b * N + r0) * D + h * HD + 2 * t4;
+        __half *o1 = out + ((size_t)b * N + r1) * D + h * HD + 2 * t4;
 #pragma unroll
-        for (int dt = 0; dt < ATT80_DT; ++dt)
+        for (int dt = 0; dt < DT; ++dt)
         {
             if (r0 < N) *reinterpret_cast<__half2 *>(o0 + dt * 8) = __floats2half2_rn(o[dt][0] * inv0, o[dt][1] * inv0);
             if (r1 < N) *reinterpret_cast<__half2 *>(o1 + dt * 8) = __floats2half2_rn(o[dt][2] * inv1, o[dt][3] * inv1);

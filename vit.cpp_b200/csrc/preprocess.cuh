@@ -100,9 +100,12 @@ __global__ void preprocess_kernel(const uint8_t *__restrict__ staging, const Pre
         float *o = out + ((size_t)b * S * S + idx) * 3;
         o[0] = px3[0]; o[1] = px3[1]; o[2] = px3[2];
     }
-    if (patches)
+    // a size the patch does not divide (SigLIP's floor grid): pixels at or past G P belong to no patch, and a row for them would be the
+    // next image's
+    const int G = S / P;
+    if (patches && i < G * P && j < G * P)
     {
-        const int G = S / P, py = i / P, ky = i - py * P, pxi = j / P, kx = j - pxi * P;
+        const int py = i / P, ky = i - py * P, pxi = j / P, kx = j - pxi * P;
         __half *row = patches + ((size_t)b * G * G + (size_t)py * G + pxi) * ldk + ky * P + kx;
 #pragma unroll
         for (int k = 0; k < 3; ++k) row[k * P * P] = __float2half_rn(px3[k]);
@@ -259,7 +262,7 @@ __global__ void image_proc_v_kernel(const uint8_t *__restrict__ tmp, const PreIm
             float *o = out + ((size_t)b * S * S + (size_t)i * S + j) * 3;
             o[0] = px3[0]; o[1] = px3[1]; o[2] = px3[2];
         }
-        if (patches)
+        if (patches && i < G * P && j < G * P) // pixels past the floor grid belong to no patch (preprocess_kernel)
         {
             const int py = i / P, ky = i - py * P, pxi = j / P, kx = j - pxi * P;
             __half *row = patches + ((size_t)b * G * G + (size_t)py * G + pxi) * ldk + ky * P + kx;

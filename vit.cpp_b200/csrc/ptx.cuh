@@ -312,6 +312,23 @@ __device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t &r0, u
                  : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
                  : "r"(addr));
 }
+// two 8x8 matrices: lanes 0-7 give the row addresses of the first, lanes 8-15 of the second
+__device__ __forceinline__ void ldmatrix_x2(uint32_t addr, uint32_t &r0, uint32_t &r1)
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
+}
+// the same, transposed
+__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t addr, uint32_t &r0, uint32_t &r1)
+{
+    asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr));
+}
+// D(16x8,f32) += A(16x8,f16) * B(8x8,f16)
+__device__ __forceinline__ void mma_m16n8k8_f16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t b0)
+{
+    asm volatile("mma.sync.aligned.m16n8k8.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5}, {%6}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a0), "r"(a1), "r"(b0));
+}
 // D(16x8,f32) += A(16x16,f16) * B(16x8,f16)
 __device__ __forceinline__ void mma_m16n8k16_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1)
 {

@@ -154,6 +154,8 @@ def lib():
         L.vitb200_test_softmax_topk.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp]
         L.vitb200_test_attention_pool.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_test_attention_hd.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp]
+        L.vitb200_test_attention_hd72.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+        L.vitb200_test_attention_pool_hd72.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         _lib = L
     return _lib
 
@@ -177,7 +179,7 @@ class VitModel:
         self.in_chans = lib().vitb200_in_chans(self._h)        # 3, or 1 for a ViTSTR model (vitstr.cpp:713); 0 for a text tower
         self.head_tokens = lib().vitb200_head_tokens(self._h)  # classifier rows per image (1, or 25 for ViTSTR)
         self.fp8 = bool(lib().vitb200_fp8(self._h))            # qkv and fc1 on the e4m3 tensor cores (vitb200_create_fp8)
-        self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or SwiGLU's F
+        self.mlp_dim = lib().vitb200_mlp_dim(self._h)          # the MLP's hidden width: 4 D, or F read from the weights
         self._labels = None
         self._zero_shot_labels = None
         ta = TextArch()
@@ -641,6 +643,28 @@ def test_attention_hd(qkv32: np.ndarray, B: int, N: int, H: int, hd: int, split:
     out = np.empty((B * N, H * hd), np.float32)
     _check(lib().vitb200_test_attention_hd(device, kernel, B, N, H, hd, hi.ctypes.data, None if lo is None else lo.ctypes.data,
                                            out.ctypes.data), "vitb200_test_attention_hd")
+    return out
+
+
+def test_attention_hd72(qkv32: np.ndarray, B: int, N: int, H: int, split: bool, device: int = 0) -> np.ndarray:
+    """The head-dim-72 attention kernel alone (vitb200_test_attention_hd72), as test_attention_hd takes its operands: qkv32 float32
+    [B*N, 3*H*72], row-major q | k | v, split into hi + lo when `split` (N <= 224), else its f16 values -> float32 [B*N, H*72]."""
+    x = np.ascontiguousarray(qkv32, np.float32).reshape(B * N, 3 * H * 72)
+    hi, lo = split_hi_lo(x) if split else (x.astype(np.float16), None)
+    out = np.empty((B * N, H * 72), np.float32)
+    _check(lib().vitb200_test_attention_hd72(device, B, N, H, hi.ctypes.data, None if lo is None else lo.ctypes.data, out.ctypes.data),
+           "vitb200_test_attention_hd72")
+    return out
+
+
+def test_attention_pool_hd72(q: np.ndarray, kv16: np.ndarray, B: int, P: int, H: int, device: int = 0) -> np.ndarray:
+    """test_attention_pool at head dim 72 (vitb200_test_attention_pool_hd72): q float32 [H*72], kv16 float16 [B*P, 2*H*72] (every row
+    k then v) -> float32 [B, H*72], the f16 results of sum_j softmax_j(q_h k_j / sqrt(72)) v_j."""
+    qq = np.ascontiguousarray(q, np.float32).reshape(H * 72)
+    kv = np.ascontiguousarray(kv16, np.float16).reshape(B * P, 2 * H * 72)
+    out = np.empty((B, H * 72), np.float32)
+    _check(lib().vitb200_test_attention_pool_hd72(device, B, P, H, qq.ctypes.data, kv.ctypes.data, out.ctypes.data),
+           "vitb200_test_attention_pool_hd72")
     return out
 
 
