@@ -65,7 +65,9 @@ typedef struct vitb200_tensor
  *   grid is then G = floor(img_size / patch_size), as HF's valid-padding conv takes it; with patch size 8, 16 or 32, whose patch
  *   embedding reads pixel rows in 16-byte loads, such an img_size must then be a multiple of 4);
  *   at most 896 tokens at head dim 64, 800 at head dim 72 and 640 at head dim 80, G^2 + 1 (K and V of one attention head in 227 KB of
- *   shared memory). */
+ *   shared memory);
+ *   FP8 engines (vitb200_create_fp8, fp8 = 1 of vitb200_create_arch and vitb200_create_text): hidden_size a multiple of 16 (the e4m3
+ *   activation rows are read in 16-byte strides), so head dim 72 with an even head count. */
 int vitb200_create(const vitb200_hparams *hp, const vitb200_tensor *tensors, int n_tensors, int device, int max_batch,
                    vitb200_engine **out);
 
@@ -464,6 +466,15 @@ int vitb200_test_quantize_fp8(const uint16_t *w_f16, int64_t n, uint8_t *q, floa
  * as vitb200_test_gemm takes it, out [M][N / 2]) of x = acc * (a_scale[m] * w_scale) + bias[n].  K % 16 == 0. */
 int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const uint8_t *A, const float *a_scale, const uint8_t *W,
                           float w_scale, const float *bias, float *out);
+
+/* Stand-alone run of the qkv and pool k | v GEMMs as the engine runs them at head dim 64: the output in head-major planes, every 64
+ * output columns one plane of plane_rows rows, uint16 f16 bits hi [N / 64][plane_rows][64] (and lo, the same shape, for epilogue 6).
+ * epilogue: 0 bias->f16, 6 split precision (hi = f16(x), lo = f16(x - hi)); lo is given exactly with 6.  e4m3 = 0: A [M][K] and
+ * W [N][K] f16 bits, a_scale NULL, K % 8 == 0; e4m3 = 1: e4m3 bytes with a_scale float32 [M] and w_scale as vitb200_test_gemm_fp8 takes
+ * them, K % 16 == 0.  N % 64 == 0, plane_rows >= M.  Both outputs are filled with 0xFFFF first: rows M .. plane_rows - 1 of every plane
+ * must keep it.  Shapes and epilogues outside these are refused before the device is touched. */
+int vitb200_test_gemm_planes(int device, int M, int N, int K, int epilogue, int64_t plane_rows, int e4m3, const void *A, const float *a_scale,
+                             const void *W, float w_scale, const float *bias, uint16_t *hi, uint16_t *lo);
 
 /* The FP8 engine's LayerNorm 1 / 2 alone, the kernel chosen as vitb200_test_layernorm chooses it: x float32 [rows][D] -> q e4m3 bytes
  * [rows][D] and the row scales sa float32 [rows].  D % 16 == 0. */

@@ -3,6 +3,7 @@ torch's e4m3, and the accuracy cost of the FP8 recipe measured on its numpy emul
 reference's golden logits."""
 import ctypes as C
 import os
+import re
 
 import numpy as np
 import pytest
@@ -58,6 +59,46 @@ def test_null_and_bad_arguments_are_rejected():
     assert L.vitb200_test_layernorm_fp8(0, 4, 64, None, f.ctypes.data, f.ctypes.data, 1e-6, a.ctypes.data, f.ctypes.data) != 0
     assert L.vitb200_test_layernorm_fp8(0, 4, 64, f.ctypes.data, f.ctypes.data, f.ctypes.data, 1e-6, None, f.ctypes.data) != 0
     assert L.vitb200_test_layernorm_fp8(0, 4, 60, f.ctypes.data, f.ctypes.data, f.ctypes.data, 1e-6, a.ctypes.data, f.ctypes.data) != 0
+
+
+FP8_WIDTH = "FP8 engine: hidden size 72 not supported \\(a multiple of 16: the e4m3 activation rows of D bytes are read in 16-byte strides"
+
+
+def test_fp8_image_towers_need_hidden_sizes_of_16_byte_rows(tmp_path):
+    """A SigLIP-pooled image tower with one 72-column head (D = 72): the f16 engine takes it; the FP8 engine's e4m3 rows would be 72 bytes,
+    which its TMA maps cannot stride, so it is refused before the device is touched, naming the limit."""
+    path = str(tmp_path / "m.bin")
+    gf.write_synthetic(path, (72, 1, 1, 16, 64), 1)
+    vf = gf.read(path)
+    vf.pool = "mean"  # head dim 72 runs with the SigLIP pools only: patch rows, no class token
+    del vf.tensors["cls_token"]
+    vf.tensors["pos_embed"] = np.ascontiguousarray(np.asarray(vf.tensors["pos_embed"]).reshape(-1, 72)[1:][None])
+    with pytest.raises(eng.VitB200Error, match=FP8_WIDTH):
+        eng.vit_model_from_tensors(vf, 0, 2, fp8=True)
+    if torch.cuda.is_available():
+        eng.vit_model_from_tensors(vf, 0, 2).close()
+    else:
+        with pytest.raises(eng.VitB200Error, match="no CUDA device"):
+            eng.vit_model_from_tensors(vf, 0, 2)
+
+
+def test_fp8_text_towers_need_hidden_sizes_of_16_byte_rows():
+    """A SigLIP text tower with one 72-column head is refused in its FP8 form before the device is touched; with two heads (D = 144) the
+    width passes and the load goes on to the next check (here: the blocks this stub lacks)."""
+    L = eng.lib()
+    for D, heads in ((72, 1), (144, 2)):
+        tok = np.zeros((8, D), np.float16)
+        ts = (eng.Tensor * 1)()
+        ts[0].name, ts[0].data, ts[0].type, ts[0].n_dims = b"token_embd.weight", tok.ctypes.data, 1, 2
+        ts[0].ne[0], ts[0].ne[1], ts[0].ne[2], ts[0].ne[3] = D, 8, 1, 1
+        hp = eng.Hparams(D, 1, heads, 96, 0, 0, 1, 1e-6)
+        ta = eng.TextArch(16, 0, 2, 2, gf.ARCH_ACTIVATIONS.index("gelu_pytorch_tanh"), float("nan"), float("nan"))
+        h = C.c_void_p()
+        assert L.vitb200_create_text(C.byref(hp), C.byref(ta), ts, 1, 0, 2, 1, C.byref(h)) != 0 and not h.value
+        if D == 72:
+            assert re.search(FP8_WIDTH, _last_error()), _last_error()
+        else:
+            assert "FP8 engine" not in _last_error() and "hidden size" not in _last_error(), _last_error()
 
 
 def _torch_e4m3(w16, scale_inv):

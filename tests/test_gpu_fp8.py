@@ -82,10 +82,11 @@ def _check_exact(M, N, K, epi, seed):
 
 @pytest.mark.parametrize("epi", [eng.EPI_BIAS_F16, eng.EPI_BIAS_GELU_F16, eng.EPI_BIAS_F16_HILO, eng.EPI_BIAS_GELU_ERF_F16,
                                  eng.EPI_BIAS_QUICK_GELU_F16, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16, eng.EPI_SWIGLU])
-@pytest.mark.parametrize("K", [64, 192, 768, 1024, 3072])
+@pytest.mark.parametrize("K", [64, 192, 768, 1024, 3072, 144, 160, 208, 240, 400, 1040])
 def test_gemm_exact_ragged_m(epi, K):
-    """M ends inside a tile's second 64-row half; K = 64 is a partial k-block (zero-filled), 3072 runs the 6-slot ring.  SwiGLU: F = 192,
-    3 column tiles, the last pair's second tile past N."""
+    """M ends inside a tile's second 64-row half; K = 64 is a partial k-block (zero-filled), 3072 runs the 6-slot ring.  K = 144, 160,
+    208, 240, 400 and 1040 end in a k-block of 128 that holds 16, 32, 80, 112, 16 and 16 columns of K (the rest zero-filled): D = 80 H
+    with H = 2, 3, 5, 13, and the So400m micro towers' 144.  SwiGLU: F = 192, 3 column tiles, the last pair's second tile past N."""
     _check_exact(197 * 7, 384, K, epi, seed=K + epi)
 
 
@@ -93,9 +94,11 @@ def test_gemm_exact_ragged_m(epi, K):
 @pytest.mark.parametrize("K,epi", [(192, eng.EPI_BIAS_F16), (768, eng.EPI_BIAS_F16_HILO), (3072, eng.EPI_BIAS_GELU_F16),
                                    (192, eng.EPI_BIAS_GELU_ERF_F16), (3072, eng.EPI_BIAS_GELU_ERF_F16), (320, eng.EPI_BIAS_QUICK_GELU_F16),
                                    (2048, eng.EPI_BIAS_QUICK_GELU_F16), (192, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16),
-                                   (3072, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (192, eng.EPI_SWIGLU), (3072, eng.EPI_SWIGLU)])
+                                   (3072, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (192, eng.EPI_SWIGLU), (3072, eng.EPI_SWIGLU),
+                                   (400, eng.EPI_BIAS_F16_HILO), (208, eng.EPI_BIAS_F16), (240, eng.EPI_BIAS_GELU_F16)])
 def test_gemm_exact_tile_counts_around_the_grid(per_cluster, extra, K, epi):
-    """As in test_gpu_gemm_schedule.py; SwiGLU with F = 128, one pair per row band."""
+    """As in test_gpu_gemm_schedule.py; SwiGLU with F = 128, one pair per row band.  K = 400, 208 and 240: 4, 2 and 2 k-blocks, the last
+    one partly zero-filled."""
     pairs = per_cluster * (_sms() // 2) + extra
     _check_exact(pairs * BM, 2 * BN, K, epi, seed=pairs + K)
 
@@ -115,6 +118,12 @@ def test_gemm_exact_vit_b_shapes(N, K, epi):
     """qkv and fc1 of ViT-B/16 at batch 256 (tanh GELU with the f16 table, erf, QuickGELU, PyTorch's tanh GELU); ViT-g's SwiGLU fc1
     (F = 4096) at batch 64 with 4 registers (261 tokens)."""
     _check_exact(64 * 261 if epi == eng.EPI_SWIGLU else 256 * 197, N, K, epi, seed=N + K)
+
+
+@pytest.mark.parametrize("M,N,K,epi", [(M, N, K, epi) for M, N, K, epi in gs.TOWER_LAYERS if epi != eng.EPI_BIAS_RESID_F32])
+def test_gemm_exact_tower_layer_shapes(M, N, K, epi):
+    """The FP8 engine's qkv and fc1 of SigLIP So400m (3 x 729 tokens; fc1's last column tile 80 columns wide) and ViT-H/14 (3 x 257)."""
+    _check_exact(M, N, K, epi, seed=M + N + K + epi)
 
 
 # ---- GEMM, random operands -----------------------------------------------------------------------------------------------------

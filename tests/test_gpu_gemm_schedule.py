@@ -197,17 +197,29 @@ def test_fewer_tiles_than_sms(epi):
 
 _GRID_NEW = [(K, e) for e in NEW for K in (192, 320, 2048, 3072)]
 
+# (N, K, epilogue) with K % 64 != 0: the last k-block of every tile is partly past K, and TMA zero-fills that part of both operands.  The
+# reductions the engine runs: D at head dims 72 and 80 with an odd head count (72, 80, 240, ...), the So400m micro towers (144), MLP
+# widths read from the weights as fc2's K (344, 464, 2736, So400m's 4304), down to a single partial k-block (8, 24, 56); 2736 and 4304
+# run the 6-stage ring.  Every epilogue family at least once.
+K_TAILS = [(384, 8, eng.EPI_BIAS_F16), (384, 24, eng.EPI_BIAS_RESID_F32), (384, 56, eng.EPI_BIAS_F32), (384, 72, eng.EPI_BIAS_F16_HILO),
+           (384, 80, eng.EPI_BIAS_GELU_F16), (384, 144, eng.EPI_BIAS_GELU_ERF_F16), (384, 240, eng.EPI_BIAS_QUICK_GELU_F16),
+           (384, 344, eng.EPI_BIAS_SCALE_RESID_F32), (384, 464, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (2 * 2736, 72, eng.EPI_SWIGLU),
+           (384, 2736, eng.EPI_BIAS_F16), (384, 2736, eng.EPI_BIAS_SCALE_RESID_F32), (2 * 2736, 2736, eng.EPI_SWIGLU),
+           (384, 4304, eng.EPI_BIAS_RESID_F32), (384, 4304, eng.EPI_BIAS_F16_HILO), (384, 4304, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16)]
+
 
 @pytest.mark.parametrize("per_cluster,extra", [(4, 0), (4, 1), (4, -1), (3, 0), (3, 1)])
 @pytest.mark.parametrize("K,epi", [(192, eng.EPI_BIAS_F16), (64, eng.EPI_BIAS_RESID_F32), (320, eng.EPI_BIAS_F16_HILO),
-                                   (2048, eng.EPI_BIAS_F16_HILO)] + _GRID_NEW)
+                                   (2048, eng.EPI_BIAS_F16_HILO), (80, eng.EPI_BIAS_F16_HILO), (344, eng.EPI_BIAS_F16),
+                                   (4304, eng.EPI_BIAS_RESID_F32)] + _GRID_NEW)
 def test_tile_counts_around_the_grid(per_cluster, extra, K, epi):
     """per_cluster x SMs / 2 tile pairs (+ extra).  The engine launches as many clusters as fit at once, which is SMs / 2 on an H100
     SXM; where fewer fit, these counts are still uneven shares of the grid, only not the exact boundaries named here.  With SMs / 2
     clusters: equal shares, one cluster with one more, one with one fewer; an odd share gives the first warpgroup one tile more than
     the second.  K = 64, 192, 320 are 1, 3 and 5 k-blocks against the 5-slot ring, so tiles start at every slot and phase; K = 2048
-    (32 k-blocks) and 3072 run the 6-slot ring with the smaller staging buffer (and LayerScale's gamma staged per pass).  SwiGLU
-    with F = 128: one pair per row band, as for the other epilogues."""
+    (32 k-blocks) and 3072 run the 6-slot ring with the smaller staging buffer (and LayerScale's gamma staged per pass).  K = 80, 344
+    and 4304 (2, 6 and 68 k-blocks) end each tile's reduction in a k-block TMA zero-fills past K, on both rings.  SwiGLU with F = 128:
+    one pair per row band, as for the other epilogues."""
     pairs = per_cluster * (_sms() // 2) + extra
     _check(pairs * BM, 2 * BN, K, epi, seed=pairs + K)
 
@@ -217,10 +229,11 @@ def test_tile_counts_around_the_grid(per_cluster, extra, K, epi):
                                      (384, 448, eng.EPI_BIAS_GELU_ERF_F16), (384, 2048, eng.EPI_BIAS_QUICK_GELU_F16),
                                      (384, 448, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16), (128, 448, eng.EPI_BIAS_SCALE_RESID_F32),
                                      (384, 3072, eng.EPI_BIAS_SCALE_RESID_F32), (2 * 2736, 448, eng.EPI_SWIGLU),
-                                     (2 * 2736, 2048, eng.EPI_SWIGLU)])
+                                     (2 * 2736, 2048, eng.EPI_SWIGLU)] + K_TAILS)
 def test_odd_column_tile_count(N, K, epi):
     """An odd number of column tiles: the second CTA of the last pair computes a tile past N, stores nothing, and still releases its
-    share of the ring it shares with the first.  SwiGLU with F = 2736: 43 column tiles."""
+    share of the ring it shares with the first.  SwiGLU with F = 2736: 43 column tiles.  K_TAILS: reductions whose last k-block is
+    partly zero-filled."""
     _check(197 * 7, N, K, epi, seed=N + K + epi)
 
 
@@ -258,3 +271,20 @@ def test_full_size(N, K, epi):
     LayerScale proj and fc2; ViT-g's SwiGLU fc1 (F = 4096) at batch 64."""
     M = {eng.EPI_BIAS_SCALE_RESID_F32: 256 * 261, eng.EPI_SWIGLU: 64 * 261}.get(epi, 256 * 197)
     _check(M, N, K, epi, seed=N * 7 + K + epi)
+
+
+# (M, N, K, epilogue): the block GEMMs of the towers with widths that are not multiples of 128, for 3 images
+TOWER_LAYERS = [
+    (729 * 3, 3456, 1152, eng.EPI_BIAS_F16_HILO),                # SigLIP So400m at 384 px: qkv (27 column tiles)
+    (729 * 3, 4304, 1152, eng.EPI_BIAS_GELU_PYTORCH_TANH_F16),   # fc1: the last column tile holds 80 columns
+    (729 * 3, 1152, 4304, eng.EPI_BIAS_RESID_F32),               # fc2: K = 4304, a 16-column last k-block on the 6-stage ring
+    (257 * 3, 3840, 1280, eng.EPI_BIAS_F16_HILO),                # ViT-H/14 at 224 px: qkv (30 column tiles)
+    (257 * 3, 5120, 1280, eng.EPI_BIAS_GELU_ERF_F16),            # fc1, erf GELU
+    (257 * 3, 1280, 5120, eng.EPI_BIAS_RESID_F32),               # fc2
+]
+
+
+@pytest.mark.parametrize("M,N,K,epi", TOWER_LAYERS)
+def test_tower_layer_shapes(M, N, K, epi):
+    """So400m and ViT-H/14 layers once each; M = 3 x 729 and 3 x 257 end 11 and 3 rows into their last row tile."""
+    _check(M, N, K, epi, seed=M + N + K + epi)

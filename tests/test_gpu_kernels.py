@@ -30,6 +30,8 @@ CASES = [
     (300, 576, 192, eng.EPI_BIAS_RESID_F32), (197 * 3, 768, 768, eng.EPI_BIAS_RESID_F32), (197 * 3, 3072, 768, eng.EPI_BIAS_GELU_F16),
     (197 * 2, 768, 3072, eng.EPI_BIAS_RESID_F32), (197 * 2, 2304, 768, eng.EPI_BIAS_F16), (256, 1000, 768, eng.EPI_BIAS_F32),
     (7, 1000, 192, eng.EPI_BIAS_F32), (640, 128, 640, eng.EPI_BIAS_RESID_F32),
+    (129, 384, 8, eng.EPI_BIAS_F32), (300, 576, 72, eng.EPI_BIAS_F16), (300, 576, 80, eng.EPI_BIAS_GELU_F16),
+    (197 * 2, 1152, 4304, eng.EPI_BIAS_RESID_F32),
 ]
 
 

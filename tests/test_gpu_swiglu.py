@@ -16,8 +16,9 @@ from tests.test_gpu_fp8 import E2E_TOL
 eng = pkg.engine
 pytestmark = pytest.mark.gpu
 
-# (F, K): the MLP widths of D = 128 (a partial last group of 64), 384, 1024 (partial), 1536 (ViT-g), and K = 3072 for the 6-stage ring
-HOOK_CASES = [(344, 128), (1024, 384), (2736, 1024), (4096, 1536), (4096, 3072)]
+# (F, K): the MLP widths of D = 128 (a partial last group of 64), 384, 1024 (partial), 1536 (ViT-g), and K = 3072 for the 6-stage ring;
+# K = 80 and 240 (D = 80 H, H odd) end in a partly zero-filled k-block
+HOOK_CASES = [(344, 128), (1024, 384), (2736, 1024), (4096, 1536), (4096, 3072), (344, 80), (1024, 240)]
 TAIL = 16  # x1 columns driven to x1 << 0 by their bias
 
 
@@ -55,7 +56,7 @@ def test_swiglu_epilogue(F, K):
     assert (out[:, :TAIL] == 0).all() and np.isfinite(out).all()
 
 
-@pytest.mark.parametrize("F,K", [(344, 128), (2736, 1024), (4096, 3072)])
+@pytest.mark.parametrize("F,K", [(344, 128), (2736, 1024), (4096, 3072), (344, 80), (2736, 1040)])
 def test_swiglu_epilogue_e4m3(F, K):
     """The e4m3 form: A rows quantised as the FP8 LayerNorm does (quantize_rows), W as the FP8 upload does (quantize_tensor, HF's order);
     x = acc (sa sw) + bias.  The accumulation bound is test_gpu_fp8's, 2^-9 of sum_k |a w| (Hopper's e4m3 MMA sums)."""

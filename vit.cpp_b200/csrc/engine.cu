@@ -1561,6 +1561,14 @@ int mlp_width(const vitb200_tensor *t, int n, int D, int layers, bool swiglu, co
     return 0;
 }
 
+// The FP8 engine's e4m3 rows: LayerNorms 1 and 2 write D bytes per token, which the qkv and fc1 GEMMs read through TMA with a
+// 16-byte row stride
+int fail_fp8_width(int D)
+{
+    return fail("FP8 engine: hidden size %d not supported (a multiple of 16: the e4m3 activation rows of D bytes are read in 16-byte "
+                "strides; head dim 72 needs an even head count)", D);
+}
+
 // Builds an engine; *out receives it only when everything succeeded.  labels: the class names of a model file.
 int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb200_tensor *t, int n, int device, int max_batch, int head_tokens,
                 bool fp8, vitb200_engine **out, const std::map<int, std::string> *labels = nullptr)
@@ -1652,6 +1660,7 @@ int create_impl(const vitb200_hparams *hp, const vitb200_arch *arch, const vitb2
         return fail("head dim %d not supported (64 or 80; 72 with pools 2 map and 3 mean, the SigLIP towers)", hd);
     if (hd == ATT80_HD && ar.pool == 2)
         return fail("vitb200_arch.pool = 2 (map) not supported at head dim 80 (the attention-pooling head's kernel is 64 or 72 columns wide)");
+    if (fp8 && hp->hidden_size % 16 != 0) return fail_fp8_width(hp->hidden_size);
     if (hp->img_size % hp->patch_size != 0 && ar.pool < 2)
         return fail("img_size %d not a multiple of patch_size %d (only the SigLIP pools 2 and 3 take the floor grid)", hp->img_size, hp->patch_size);
     if (hp->img_size % hp->patch_size != 0 && patchify_reads_16b(hp->patch_size) && hp->img_size % 4 != 0)
@@ -1801,6 +1810,7 @@ int create_text_impl(const vitb200_hparams *hp, const vitb200_text_arch *ta, con
     const int hd = D / hp->num_attention_heads;
     if (D % hp->num_attention_heads != 0 || (hd != 64 && (hd != ATT72_HD || a.causal)))
         return fail("head dim %d not supported (64; 72 with causal = 0, the SigLIP text towers)", hd);
+    if (fp8 && D % 16 != 0) return fail_fp8_width(D);
     if (D > LN_MAX_HIDDEN) return fail("hidden size %d not supported (max %d)", D, LN_MAX_HIDDEN);
     const vitb200_tensor *te = find_tensor(t, n, "token_embd.weight"), *pe = find_tensor(t, n, "pos_embed");
     if (!te) return fail("missing tensor 'token_embd.weight'");
@@ -1938,9 +1948,12 @@ int test_layernorm_impl(int device, int rows, int D, const float *x, const float
 
 // The GEMM test hooks' one body: the GEMM alone on a scratch engine, as the engine launches it, with A [M][K] and W [N][K] f16 bits or
 // (GEMM_OP_E4M3) e4m3 bytes.  SwiGLU takes W and bias in HF's order, interleaves them as the engine uploads them and stores [M][N / 2].
+// plane_rows > 0: the f16 output is head-major, [N / 64][plane_rows][64] as the qkv and pool k | v GEMMs write it, both buffers filled
+// with 0xFFFF first (rows M .. plane_rows - 1 of every plane keep it), and hi_bits / lo_bits receive the raw planes instead of `out`.
 template <int OP, typename T>
 int test_gemm_run(int device, int M, int N, int K, int epilogue, const T *A, const T *W, const float *bias, const float *a_scale,
-                  float w_scale, const float *gamma, const float *resid, float *out)
+                  float w_scale, const float *gamma, const float *resid, float *out, size_t plane_rows = 0, uint16_t *hi_bits = nullptr,
+                  uint16_t *lo_bits = nullptr)
 {
     const GemmEpiDesc d = gemm_epi(epilogue);
     if (d.swiglu && (N < 16 || N % 16 != 0)) return fail("SwiGLU: N = 2 F with F a multiple of 8 (got N = %d)", N);
@@ -1951,13 +1964,18 @@ int test_gemm_run(int device, int M, int N, int K, int epilogue, const T *A, con
     std::vector<T> wi;
     std::vector<float> bi;
     if (d.swiglu) { wi = swiglu_interleave(W, F, (size_t)K); bi = swiglu_interleave(bias, F, 1); W = wi.data(); bias = bi.data(); }
-    const size_t MN = (size_t)M * No;
+    const size_t MN = plane_rows ? plane_rows * No : (size_t)M * No;
     T *dA = nullptr, *dW = nullptr;
     __half *hi = nullptr, *lo = nullptr;
     float *dB = nullptr, *dS = nullptr, *dG = nullptr, *o32 = nullptr;
     if (upload(e, &dA, A, (size_t)M * K) || upload(e, &dW, W, (size_t)Nw * K) || upload(e, &dB, bias, Nw)) return 1;
     if ((a_scale && upload(e, &dS, a_scale, M)) || (gamma && upload(e, &dG, gamma, N))) return 1;
     if (d.f16 && (dev_alloc(e, &hi, MN) || (d.hilo && dev_alloc(e, &lo, MN)))) return 1;
+    if (plane_rows)
+    {
+        CUDA_TRY(cudaMemset(hi, 0xFF, MN * sizeof(__half)));
+        if (lo) CUDA_TRY(cudaMemset(lo, 0xFF, MN * sizeof(__half)));
+    }
     // the residual epilogues work in place on the f32 stream, like the engine uses them (X += ...)
     if (!d.f16 && (d.resid ? upload(e, &o32, resid, MN) : dev_alloc(e, &o32, MN))) return 1;
     constexpr bool e4m3 = OP == GEMM_OP_E4M3;
@@ -1969,8 +1987,14 @@ int test_gemm_run(int device, int M, int N, int K, int epilogue, const T *A, con
         return 1;
     GemmParams p{};
     p.M = M; p.N = Nw; p.K = K; p.bias = dB; p.out = d.f16 ? (void *)hi : (void *)o32; p.out2 = lo; p.ldo = No; p.resid = o32; p.gamma = dG;
-    p.a_scale = dS; p.w_scale = w_scale; p.F = F;
+    p.a_scale = dS; p.w_scale = w_scale; p.F = F; p.headmajor = plane_rows > 0; p.plane_rows = plane_rows;
     if (run_scratch(e, e4m3 ? "e4m3 GEMM kernel" : "GEMM kernel", [&] { return launch_gemm(e, epilogue, tA, tB, p, e->stream, e4m3); })) return 1;
+    if (plane_rows)
+    {
+        CUDA_TRY(cudaMemcpy(hi_bits, hi, MN * sizeof(__half), cudaMemcpyDeviceToHost));
+        if (lo) CUDA_TRY(cudaMemcpy(lo_bits, lo, MN * sizeof(__half), cudaMemcpyDeviceToHost));
+        return 0;
+    }
     // split-precision result: hi + lo (exact in f32: the two parts do not overlap); the other f16 epilogues' hi alone, so that a -0 stays -0
     return d.f16 ? tap_f16(out, hi, MN, e->stream, lo) : tap_f32(out, o32, MN, e->stream);
 }
@@ -3122,6 +3146,29 @@ int vitb200_test_gemm_fp8(int device, int M, int N, int K, int epilogue, const u
         if (!gemm_epi(epilogue).e4m3)
             return fail("e4m3 GEMM epilogue %d not supported (%s)", epilogue, gemm_epi_list([](int epi) { return gemm_epi(epi).e4m3; }).c_str());
         return test_gemm_run<GEMM_OP_E4M3>(device, M, N, K, epilogue, A, W, bias, a_scale, w_scale, nullptr, nullptr, out);
+    });
+}
+
+// The qkv and pool k | v GEMMs as the engine runs them at head dim 64: the output in head-major planes, f16 or e4m3 operands
+int vitb200_test_gemm_planes(int device, int M, int N, int K, int epilogue, int64_t plane_rows, int e4m3, const void *A, const float *a_scale,
+                             const void *W, float w_scale, const float *bias, uint16_t *hi, uint16_t *lo)
+{
+    return guarded(__func__, [&]() -> int {
+        if (!A || !W || !bias || !hi) return fail("null argument");
+        if (epilogue != EPI_BIAS_F16 && epilogue != EPI_BIAS_F16_HILO)
+            return fail("head-major GEMM epilogue %d not supported (%d, %d: the qkv and k | v GEMMs)", epilogue, EPI_BIAS_F16, EPI_BIAS_F16_HILO);
+        if ((epilogue == EPI_BIAS_F16_HILO) != (lo != nullptr)) return fail("lo goes with epilogue %d, and only with it", EPI_BIAS_F16_HILO);
+        if (e4m3 != 0 && e4m3 != 1) return fail("e4m3 = %d out of range (0 f16 operands, 1 e4m3)", e4m3);
+        if (e4m3 != (a_scale != nullptr)) return fail("a_scale goes with e4m3 operands, and only with them");
+        const int kmul = e4m3 ? 16 : 8; // 16-byte operand rows
+        if (M < 1 || K < kmul || K % kmul != 0 || N < 64 || N % 64 != 0)
+            return fail("bad shape (M >= 1, N a multiple of 64, K a multiple of %d; got M = %d, N = %d, K = %d)", kmul, M, N, K);
+        if (plane_rows < M || plane_rows > INT32_MAX) return fail("plane_rows = %lld out of range (M = %d .. 2^31 - 1)", (long long)plane_rows, M);
+        if (e4m3)
+            return test_gemm_run<GEMM_OP_E4M3>(device, M, N, K, epilogue, (const uint8_t *)A, (const uint8_t *)W, bias, a_scale, w_scale,
+                                               nullptr, nullptr, nullptr, (size_t)plane_rows, hi, lo);
+        return test_gemm_run<GEMM_OP_F16>(device, M, N, K, epilogue, (const uint16_t *)A, (const uint16_t *)W, bias, nullptr, 0.f, nullptr,
+                                          nullptr, nullptr, (size_t)plane_rows, hi, lo);
     });
 }
 

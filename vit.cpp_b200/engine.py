@@ -120,6 +120,7 @@ def lib():
         L.vitb200_test_zero_shot.argtypes = [i32, i32, i32, i32, vp, vp, C.c_float, C.c_float, i32, i32, vp, vp, vp, vp]
         L.vitb200_test_quantize_fp8.argtypes = [vp, C.c_int64, vp, vp]
         L.vitb200_test_gemm_fp8.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
+        L.vitb200_test_gemm_planes.argtypes = [i32, i32, i32, i32, i32, C.c_int64, i32, vp, vp, vp, C.c_float, vp, vp, vp]
         L.vitb200_test_layernorm_fp8.argtypes = [i32, i32, i32, vp, vp, vp, C.c_float, vp, vp]
         L.vitb200_destroy.argtypes = [vp]
         L.vitb200_destroy.restype = None
@@ -812,6 +813,24 @@ def test_gemm_fp8(M: int, N: int, K: int, epilogue: int, A8: np.ndarray, a_scale
     _check(lib().vitb200_test_gemm_fp8(device, M, N, K, epilogue, A.ctypes.data, sa.ctypes.data, W.ctypes.data, float(w_scale),
                                        b.ctypes.data, out.ctypes.data), "vitb200_test_gemm_fp8")
     return out
+
+
+def test_gemm_planes(M: int, N: int, K: int, epilogue: int, A: np.ndarray, W: np.ndarray, bias: np.ndarray, plane_rows: int,
+                     a_scale: Optional[np.ndarray] = None, w_scale: float = 1.0, device: int = 0):
+    """The qkv / k | v GEMM with head-major output (vitb200_test_gemm_planes): A [M][K] and W [N][K] float16, or e4m3 bytes (uint8) when
+    a_scale is given -> (hi, lo) uint16 f16 bits [N // 64][plane_rows][64], lo None for EPI_BIAS_F16.  Rows past M hold 0xFFFF."""
+    e4m3 = a_scale is not None
+    dt = np.uint8 if e4m3 else np.float16
+    A, W = np.ascontiguousarray(A, dt), np.ascontiguousarray(W, dt)
+    b = np.ascontiguousarray(bias, np.float32)
+    sa = np.ascontiguousarray(a_scale, np.float32) if e4m3 else None
+    planes = (max(N, 0) // 64, max(plane_rows, 0), 64)
+    hi = np.empty(planes, np.uint16)
+    lo = np.empty(planes, np.uint16) if epilogue == EPI_BIAS_F16_HILO else None
+    _check(lib().vitb200_test_gemm_planes(device, M, N, K, epilogue, plane_rows, int(e4m3), A.ctypes.data, sa.ctypes.data if e4m3 else None,
+                                          W.ctypes.data, float(w_scale), b.ctypes.data, hi.ctypes.data,
+                                          lo.ctypes.data if lo is not None else None), "vitb200_test_gemm_planes")
+    return hi, lo
 
 
 def test_layernorm_fp8(x, w, b, eps: float = 1e-6, device: int = 0):
