@@ -499,7 +499,9 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
 
 /* The wgmma attention kernel (N <= 224) on split-precision operands, the way the engine runs it: every q, k, v value is
  * the sum of two f16 numbers, qkv_hi + qkv_lo (what the qkv GEMM's hi-lo epilogue leaves behind: hi = f16(x), lo = f16(x - hi)), so
- * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858). */
+ * the f16 tensor cores reproduce the reference's f32-operand attention mat-muls (vit.cpp:848,858).  Both halves are taken as given:
+ * lo need not be the residue of hi, so a test can place an operand in one half alone.  The same holds for the split form of
+ * vitb200_test_attention_hd and vitb200_test_attention_hd72 below. */
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 /* The same with CLIP's causal mask (vitb200_text_arch.causal): query row t attends to keys 0 .. t of its sequence. */
 int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);

@@ -220,7 +220,8 @@ def test_layernorm_matches_the_restatement(rows, D):
 # ---- attention kernels at their edges ------------------------------------------------------------------------------------------------
 class EdgeForm(NamedTuple):
     """One way the engine runs attention: head dim, heads per image, CLIP's causal mask (query i attends to keys 0 .. i), hi + lo
-    operands (split_hi_lo) instead of f16 values, the hook (qkv32 [B*N][3*H*hd], B, N, H) -> [B*N][H*hd], and its token counts."""
+    operands (split_hi_lo) instead of f16 values, the hook (qkv32 [B*N][3*H*hd], B, N, H) -> [B*N][H*hd], and its token counts.
+    The forms of tests/attention_parts.py hand their hook the f16 halves instead: (hi, lo, B, N, H)."""
     hd: int
     H: int
     causal: bool
@@ -364,7 +365,7 @@ def _all_negative_case(f, N):
 @pytest.mark.parametrize("form,N", EDGE_CASES, ids=EDGE_IDS)
 def test_attention_routes_every_row_exactly(form, N):
     """One-hot probability rows (_routing_case): output row i must be the chosen V row bit for bit.  Every K and V row of every image,
-    head, key chunk and query tile must land where it belongs; the head-dim-80 hook fills its output with NaN first, so a row the
+    head, key chunk and query tile must land where it belongs; every attention hook fills its output with NaN first, so a row the
     kernel never writes fails too."""
     f = EDGE_FORMS[form]
     qkv, want = _routing_case(f, N)

@@ -15,6 +15,12 @@ M = N = K = 128
 D, ROWS = 128, 8
 B, NT, H = 1, 16, 1
 
+
+def _attention_parts(hd, causal=False):
+    z = np.zeros((B * NT, 3 * H * hd), np.float16)
+    return eng.test_attention_parts(z, z, B, NT, H, hd, causal)
+
+
 HOOKS = {
     "gemm": lambda: eng.test_gemm(M, N, K, eng.EPI_BIAS_F16, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16), np.zeros(N, np.float32)),
     "gemm_layer_scale": lambda: eng.test_gemm_layer_scale(M, N, K, np.zeros((M, K), np.float16), np.zeros((N, K), np.float16),
@@ -28,6 +34,10 @@ HOOKS = {
     "layernorm_fp8": lambda: eng.test_layernorm_fp8(np.zeros((ROWS, D), np.float32), np.ones(D, np.float32), np.zeros(D, np.float32)),
     "attention": lambda: eng.test_attention(np.zeros((B * NT, 3 * H * 64), np.float16), B, NT, H),
     "attention_hilo": lambda: eng.test_attention_hilo(np.zeros((B * NT, 3 * H * 64), np.float32), B, NT, H),
+    "attention_parts": lambda: _attention_parts(64),
+    "attention_parts_causal": lambda: _attention_parts(64, causal=True),
+    "attention_parts_hd80": lambda: _attention_parts(80),
+    "attention_parts_hd72": lambda: _attention_parts(72),
     "softmax_topk": lambda: eng.test_softmax_topk(np.zeros((ROWS, 10), np.float32), 5),
     "attention_pool": lambda: eng.test_attention_pool(np.zeros(H * 64, np.float32), np.zeros((B * NT, 2 * H * 64), np.float16), B, NT, H),
 }

@@ -2351,6 +2351,7 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
     };
     to_head_major(qkv);
     if (upload(e, &e->QKV16, hm.data(), hm.size()) || dev_alloc(e, &e->A16, (size_t)T * D)) return 1;
+    CUDA_TRY(cudaMemset(e->A16, 0xFF, T * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
     if (kernel < ATT_AUTO || kernel > ATT_MMA16) return fail("attention kernel %d unknown", kernel);
     if (kernel == ATT_WGMMA && N > ATTW_KEYS) return fail("wgmma attention needs N <= %d", ATTW_KEYS);
     if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16);

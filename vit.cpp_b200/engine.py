@@ -658,6 +658,33 @@ def test_attention_hd72(qkv32: np.ndarray, B: int, N: int, H: int, split: bool, 
     return out
 
 
+def test_attention_parts(hi: np.ndarray, lo: np.ndarray, B: int, N: int, H: int, hd: int, causal: bool = False,
+                         device: int = 0) -> np.ndarray:
+    """The split-precision attention kernel of head dim hd (64, 80 or 72; N <= 224) on hi and lo halves passed as given: hi, lo
+    float16 [B*N, 3*H*hd], row-major q | k | v -> float32 [B*N, H*hd].  Nothing requires lo to be the rounding residue of hi, so an
+    operand can live in one half alone and each of S = Ql Kh^T + Qh Kl^T + Qh Kh^T and O = P Vl + P Vh be exercised by itself.
+    causal (CLIP's mask) runs at head dim 64 only, where the causal kernel is."""
+    if causal and hd != 64:
+        raise ValueError(f"the causal mask runs at head dim 64 only, not {hd}")
+    h = np.ascontiguousarray(hi, np.float16).reshape(B * N, 3 * H * hd)
+    l = np.ascontiguousarray(lo, np.float16).reshape(B * N, 3 * H * hd)
+    out = np.empty((B * N, H * hd), np.float32)
+    L = lib()
+    if hd == 64:
+        name = "vitb200_test_attention_hilo_causal" if causal else "vitb200_test_attention_hilo"
+        rc = getattr(L, name)(device, B, N, H, h.ctypes.data, l.ctypes.data, out.ctypes.data)
+    elif hd == 80:
+        name = "vitb200_test_attention_hd"
+        rc = L.vitb200_test_attention_hd(device, ATTN_AUTO, B, N, H, hd, h.ctypes.data, l.ctypes.data, out.ctypes.data)
+    elif hd == 72:
+        name = "vitb200_test_attention_hd72"
+        rc = L.vitb200_test_attention_hd72(device, B, N, H, h.ctypes.data, l.ctypes.data, out.ctypes.data)
+    else:
+        raise ValueError(f"split-precision attention runs head dims 64, 80 and 72, not {hd}")
+    _check(rc, name)
+    return out
+
+
 def test_attention_pool_hd72(q: np.ndarray, kv16: np.ndarray, B: int, P: int, H: int, device: int = 0) -> np.ndarray:
     """test_attention_pool at head dim 72 (vitb200_test_attention_pool_hd72): q float32 [H*72], kv16 float16 [B*P, 2*H*72] (every row
     k then v) -> float32 [B, H*72], the f16 results of sum_j softmax_j(q_h k_j / sqrt(72)) v_j."""
