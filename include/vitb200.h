@@ -492,9 +492,10 @@ int vitb200_test_gemm_q8(int device, int M, int N, int K, const float *x, const 
 
 /* Stand-alone run of one attention kernel (head dim 64) over a fused QKV buffer: qkv = f16 bits [B*N][3*H*64] (what the qkv
  * GEMM leaves behind, reference vit.cpp:826-846), out = float32 [B*N][H*64] (the merged heads before proj, vit.cpp:860-866).
- * kernel: 0 = the engine's choice for N, 1 = two-pass mma.sync with 8 warps (any N), 2 = wgmma with TMA-staged operands (N <= 224),
- * 3 = two-pass mma.sync with 16 warps (128 < N <= 640).  The wgmma kernel always runs on split-precision operands; here their lo
- * halves are zero, so it computes with the f16 values of qkv as given. */
+ * kernel: 0 = the engine's choice for N, 1 = two-pass mma.sync with 8 warps (any N), 2 = wgmma with TMA-staged operands (N <= 224:
+ * the persistent kernel up to 200 tokens, one CTA per (image, head) beyond, as the engine picks them), 3 = two-pass mma.sync with 16
+ * warps (128 < N <= 640), 5 = the one-CTA-per-(image, head) wgmma kernel at any N <= 224.  The wgmma kernels always run on
+ * split-precision operands; here their lo halves are zero, so they compute with the f16 values of qkv as given. */
 int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out);
 
 /* The wgmma attention kernel (N <= 224) on split-precision operands, the way the engine runs it: every q, k, v value is
@@ -505,11 +506,17 @@ int vitb200_test_attention(int device, int kernel, int B, int N, int H, const ui
 int vitb200_test_attention_hilo(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 /* The same with CLIP's causal mask (vitb200_text_arch.causal): query row t attends to keys 0 .. t of its sequence. */
 int vitb200_test_attention_hilo_causal(int device, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
+/* vitb200_test_attention_hilo through kernel 2 or 5 of vitb200_test_attention with the kernel's phase probe on: per CTA and per problem
+ * it takes (the first 64), 9 %globaltimer stamps in ns -- the K V load issued, then for each of the two computing warpgroups: waiting
+ * for its first q tile's operands, operands landed, S done, P V done (0 where a warpgroup had no tile).  rec receives
+ * grid x 64 x 9 stamps and must hold B*H x 64 x 9; *grid receives the grid size.  For tools/attention_phases.py. */
+int vitb200_test_attention_phases(int device, int kernel, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo,
+                                  unsigned long long *rec, int *grid);
 /* Stand-alone run of the attention kernel of head dim hd (64 or 80) over a row-major QKV buffer: qkv_hi = f16 bits [B*N][3*H*hd],
  * out = float32 [B*N][H*hd].  hd 80 runs the head-dim-80 kernel (kernel 0 = the engine's choice, or 4; 1 <= N <= 640, the
  * engine's limit): on split-precision operands qkv_hi + qkv_lo when qkv_lo is given (N <= 224, as the engine runs it there), on the
  * f16 values of qkv_hi when qkv_lo is NULL (as the engine runs it above 224 tokens).  hd 64 runs vitb200_test_attention's kernels, with
- * the lo halves when qkv_lo is given (kernel 0 or 2). */
+ * the lo halves when qkv_lo is given (kernel 0, 2 or 5). */
 int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int hd, const uint16_t *qkv_hi, const uint16_t *qkv_lo, float *out);
 /* The same for head dim 72 (SigLIP So400m), which vitb200_test_attention_hd refuses: qkv_hi = f16 bits [B*N][3*H*72], out = float32
  * [B*N][H*72], 1 <= N <= 800; split precision with qkv_lo (N <= 224), the f16 values of qkv_hi without it. */

@@ -31,7 +31,21 @@ __host__ __device__ inline int attention_wgmma_smem_bytes()
     return 1024 + ATTW_PARTS * (4 * ATTW_QTILE_BYTES + 2 * ATTW_KV_BYTES) + 64;
 }
 
-template <bool CAUSAL>
+// Phase probe of the two non-causal wgmma kernels (vitb200_test_attention_phases, tools/attention_phases.py).  With PROBE, thread 0 of
+// the loading thread and of each computing warpgroup stores %globaltimer into record (CTA, i-th problem of that CTA), fields:
+//   0 = the problem's K V load issued;  per computing warpgroup c (1 + 4 c ...): + 0 it starts waiting for the problem's operands in
+//   shared memory (q, k and v in the per-head kernel; k and v in the persistent one, whose q goes straight to registers), + 1 they have
+//   landed, + 2 S of its first tile done, + 3 that tile's P V done.
+// The engine launches PROBE = false, which compiles none of it.
+constexpr int ATT_PROBE_FIELDS = 9;
+constexpr int ATT_PROBE_PROBLEMS = 64; // records per CTA; later problems are not recorded
+__device__ unsigned long long *g_attn_probe;
+__device__ __forceinline__ void probe_stamp(int cta, int i, int field)
+{
+    if (i < ATT_PROBE_PROBLEMS) g_attn_probe[((size_t)cta * ATT_PROBE_PROBLEMS + i) * ATT_PROBE_FIELDS + field] = ptx::globaltimer();
+}
+
+template <bool CAUSAL, bool PROBE = false>
 __global__ void __launch_bounds__(ATTW_THREADS, 1)
 attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV,
                        const __grid_constant__ CUtensorMap tmQl, const __grid_constant__ CUtensorMap tmKVl,
@@ -63,6 +77,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
     ptx::grid_dep_wait();
     if (threadIdx.x == 0)
     {
+        if constexpr (PROBE) probe_stamp(blockIdx.x, 0, 0);
         ptx::mbar_arrive_expect_tx(bar, (uint32_t)(kParts * (n_mt * ATTW_QTILE_BYTES + 2 * ATTW_KV_BYTES)));
         for (int part = 0; part < kParts; ++part)
         {
@@ -73,7 +88,11 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             ptx::tma_load_3d(sV(part), mkv, bar, 0, 0, q_slice + 2 * plane_slices);
         }
     }
+    if constexpr (PROBE)
+        if ((threadIdx.x & 127) == 0) probe_stamp(blockIdx.x, 0, 1 + 4 * (threadIdx.x >> 7));
     ptx::mbar_wait(bar, 0);
+    if constexpr (PROBE)
+        if ((threadIdx.x & 127) == 0) probe_stamp(blockIdx.x, 0, 2 + 4 * (threadIdx.x >> 7));
 
     const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127, warp = tid >> 5, lane = tid & 31;
     const int c0 = 2 * (lane & 3); // key / dim columns 8 j + c0 (+ 1) of this thread
@@ -97,6 +116,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         ptx::fence_regs(s);
+        if constexpr (PROBE)
+            if (tid == 0 && mt == wg) probe_stamp(blockIdx.x, 0, 3 + 4 * wg);
 
         if constexpr (CAUSAL)
         {
@@ -166,6 +187,8 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
         ptx::wgmma_commit();
         ptx::wgmma_wait<0>();
         ptx::fence_regs(o);
+        if constexpr (PROBE)
+            if (tid == 0 && mt == wg) probe_stamp(blockIdx.x, 0, 4 + 4 * wg);
 
         const float inv0 = 1.0f / l0, inv1 = 1.0f / l1; // p_i = e_i * (1/sum)  (ggml.c:10556-10558)
         const int r0 = mt * 64 + warp * 16 + (lane >> 2), r1 = r0 + 8;
@@ -177,6 +200,229 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_con
             if (r0 < N) *reinterpret_cast<__half2 *>(o0 + dt * 8) = __floats2half2_rn(o[4 * dt] * inv0, o[4 * dt + 1] * inv0);
             if (r1 < N) *reinterpret_cast<__half2 *>(o1 + dt * 8) = __floats2half2_rn(o[4 * dt + 2] * inv1, o[4 * dt + 3] * inv1);
         }
+    }
+}
+
+// attention_wgmma_persistent_kernel -- the same attention (non-causal), N <= ATTP_KEYS tokens, on one persistent CTA per SM that loads
+// the next (image, head) problem's operands while its tensor cores work on this one.  The per-problem kernel above waits for all of
+// q, k and v and only then computes, so with one CTA per SM its loads and its MMAs never overlap.
+//
+//   producer  warpgroup 0, one thread: K and V (hi and lo) of problem i + 1 into one of two buffers while problem i runs out of the
+//             other.  The boxes are ATTP_ROWS rows of the same maps-of-N-row-slices as above: rows past N are TMA zero fill
+//   consumer  warpgroups 1 and 2 take the 64-row q tiles of each problem alternately (tile t: warpgroup 1 + t % 2).  q never enters
+//             shared memory: each thread loads its m16n8k16 A fragments (hi and lo) straight from global memory into registers, for
+//             the register-A form of wgmma, rows past N as zeros.  The loads for a warpgroup's next tile are issued as soon as S of
+//             this tile is done, so they land under the soft-max and P V.  S = Ql Kh^T + Qh Kl^T + Qh Kh^T with wgmma.m64n200k16,
+//             then the soft-max and O = P Vl + P Vh of the kernel above: keys N .. 223, which that kernel also covers, have P = 0 and
+//             zero k and v, so both compute the same bits.  A buffer is released when both consumers' last P V reading it has retired
+// Barriers: full / empty per K V buffer (a problem's phase).
+constexpr int ATTP_KEYS = 200;                       // S columns (wgmma N): N <= ATTP_KEYS
+constexpr int ATTP_ROWS = 208;                       // K and V rows per box: whole k16 steps of P V (and the S columns, rounded up)
+constexpr int ATTP_THREADS = 384;                    // producer warpgroup + two consumer warpgroups
+constexpr int ATTP_KV_BYTES = ATTP_ROWS * 128;       // 208 rows x 64 dims f16 (26 KB, 1024-B multiple)
+constexpr int ATTP_BUF_BYTES = ATTW_PARTS * 2 * ATTP_KV_BYTES; // K hi | K lo | V hi | V lo of one problem
+constexpr int ATTP_BARS = 4;                         // full[2], empty[2]
+
+__host__ __device__ constexpr int attention_persistent_smem_bytes()
+{
+    return 1024 + 2 * ATTP_BUF_BYTES + 8 * ATTP_BARS; // 1024: slack to align the SWIZZLE_128B boxes
+}
+
+template <bool PROBE = false>
+__global__ void __launch_bounds__(ATTP_THREADS, 1)
+attention_wgmma_persistent_kernel(const __grid_constant__ CUtensorMap tmKV, const __grid_constant__ CUtensorMap tmKVl,
+                                  const __half *__restrict__ qkv, const __half *__restrict__ qkv_lo, __half *__restrict__ out, int N,
+                                  int D, int H, int nb, int problems, float scale)
+// qkv / qkv_lo: the head-major hi / lo buffers [3 H][nb][N][64], nb = images per plane (the buffers' max_batch); tmKV / tmKVl: their
+// maps {64, N, 3 H nb} with ATTP_ROWS-row boxes (slice p nb + b holds the N rows of image b in plane p).  problems = B H, problem
+// p = (image p / H, head p % H); CTA c takes problems c, c + gridDim.x, ...
+{
+    extern __shared__ uint8_t attp_smem_raw[];
+    const uint32_t base = (ptx::smem_u32(attp_smem_raw) + 1023u) & ~1023u;
+    // [buffer][K hi, K lo, V hi, V lo] | barriers
+    auto sKV = [&](int buf, int kv, int part) { return base + (uint32_t)buf * ATTP_BUF_BYTES + (uint32_t)(2 * kv + part) * ATTP_KV_BYTES; };
+    const uint32_t bars = base + 2 * ATTP_BUF_BYTES;
+    auto full_bar = [&](int buf) { return bars + 8u * buf; };
+    auto empty_bar = [&](int buf) { return bars + 16u + 8u * buf; };
+
+    const int n_mt = (N + 63) >> 6;
+    const int plane_slices = H * nb; // k and v planes lie H and 2 H planes past the q plane
+    if (threadIdx.x == 0)
+    {
+        ptx::prefetch_tensormap(&tmKV);
+        ptx::prefetch_tensormap(&tmKVl);
+        for (int buf = 0; buf < 2; ++buf)
+        {
+            ptx::mbar_init(full_bar(buf), 1);
+            ptx::mbar_init(empty_bar(buf), 256); // every thread of both consumers
+        }
+        ptx::fence_barrier_init();
+    }
+    __syncthreads();
+    // launched with programmatic dependent launch: q, k, v are read only once the qkv GEMM has completed
+    ptx::grid_dep_launch();
+    ptx::grid_dep_wait();
+
+    const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+    if (wg == 0)
+    {
+        ptx::setmaxnreg_dec<40>();
+        if (tid == 0)
+        {
+            // K and V: problem i into buffer i % 2 once the consumers have released its problem i - 2 (a fresh barrier passes parity 1)
+            int i = 0;
+            for (int p = blockIdx.x; p < problems; p += gridDim.x, ++i)
+            {
+                const int buf = i & 1, b = p / H, h = p - b * H;
+                ptx::mbar_wait(empty_bar(buf), ((i >> 1) & 1) ^ 1);
+                if constexpr (PROBE) probe_stamp(blockIdx.x, i, 0);
+                ptx::mbar_arrive_expect_tx(full_bar(buf), (uint32_t)ATTP_BUF_BYTES);
+                for (int part = 0; part < ATTW_PARTS; ++part)
+                {
+                    const CUtensorMap *m = part ? &tmKVl : &tmKV;
+                    ptx::tma_load_3d(sKV(buf, 0, part), m, full_bar(buf), 0, 0, h * nb + b + plane_slices);
+                    ptx::tma_load_3d(sKV(buf, 1, part), m, full_bar(buf), 0, 0, h * nb + b + 2 * plane_slices);
+                }
+            }
+            // both buffers released: every load has landed and been read before the CTA exits
+            for (int k = 0; k < 2; ++k, ++i) ptx::mbar_wait(empty_bar(i & 1), ((i >> 1) & 1) ^ 1);
+        }
+        return;
+    }
+
+    ptx::setmaxnreg_inc<232>();
+    const int c = wg - 1, warp = tid >> 5, lane = tid & 31;
+    const int c0 = 2 * (lane & 3); // key / dim columns 8 j + c0 (+ 1) of this thread
+    // q tile mt of problem p -> A fragments {row r k c0, row r+8 k c0, row r k 8+c0, row r+8 k 8+c0} per k16 step, for both halves;
+    // rows r, r + 8 of the tile are this thread's (as in S), rows past N are zero
+    uint32_t qa[ATTW_PARTS][4][4];
+    auto load_q = [&](int p, int mt) {
+        const int b = p / H, h = p - b * H, r = mt * 64 + warp * 16 + (lane >> 2);
+        const size_t slice = ((size_t)h * nb + b) * N * 64;
+#pragma unroll
+        for (int part = 0; part < ATTW_PARTS; ++part)
+        {
+            const __half *q = (part ? qkv_lo : qkv) + slice + c0;
+            const uint32_t *q0 = reinterpret_cast<const uint32_t *>(q + (size_t)r * 64), *q1 = reinterpret_cast<const uint32_t *>(q + (size_t)(r + 8) * 64);
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+            {
+                qa[part][k][0] = r < N ? __ldg(q0 + 8 * k) : 0u;
+                qa[part][k][2] = r < N ? __ldg(q0 + 8 * k + 4) : 0u;
+                qa[part][k][1] = r + 8 < N ? __ldg(q1 + 8 * k) : 0u;
+                qa[part][k][3] = r + 8 < N ? __ldg(q1 + 8 * k + 4) : 0u;
+            }
+        }
+    };
+    if (c < n_mt && (int)blockIdx.x < problems) load_q(blockIdx.x, c);
+    int i = 0;
+    for (int p = blockIdx.x; p < problems; p += gridDim.x, ++i)
+    {
+        const int buf = i & 1, b = p / H, h = p - b * H;
+        if constexpr (PROBE)
+            if (tid == 0) probe_stamp(blockIdx.x, i, 1 + 4 * c);
+        ptx::mbar_wait(full_bar(buf), (i >> 1) & 1);
+        if constexpr (PROBE)
+            if (tid == 0) probe_stamp(blockIdx.x, i, 2 + 4 * c);
+        for (int mt = c; mt < n_mt; mt += 2)
+        {
+            // ---- S = Q K^T (f32, registers), the products in the order of attention_wgmma_kernel
+            float s[ATTP_KEYS / 2];
+#pragma unroll
+            for (int j = 0; j < ATTP_KEYS / 2; ++j) s[j] = 0.f;
+            ptx::fence_regs(s);
+            ptx::wgmma_fence();
+            const uint64_t kh = ptx::wgmma_desc_kmajor_sw128(sKV(buf, 0, 0)), kl = ptx::wgmma_desc_kmajor_sw128(sKV(buf, 0, 1));
+#pragma unroll
+            for (int k = 0; k < 4; ++k) // 64 dims = 4 x K 16 (+32 B each)
+            {
+                ptx::wgmma_m64n200k16_f16_rs(s, qa[1][k], kh + 2 * k, k != 0);
+                ptx::wgmma_m64n200k16_f16_rs(s, qa[0][k], kl + 2 * k, 1);
+                ptx::wgmma_m64n200k16_f16_rs(s, qa[0][k], kh + 2 * k, 1);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(s);
+            if constexpr (PROBE)
+                if (tid == 0 && mt == c) probe_stamp(blockIdx.x, i, 3 + 4 * c);
+            // this warpgroup's next q tile: the next one of this problem, else its first of the CTA's next problem
+            if (mt + 2 < n_mt) load_q(p, mt + 2);
+            else if (p + (int)gridDim.x < problems) load_q(p + gridDim.x, c);
+
+            // ---- soft-max over the valid keys: rows r (s[4j], s[4j+1]) and r + 8 (s[4j+2], s[4j+3]) of this quad
+            float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+            for (int j = 0; j < ATTP_KEYS / 8; ++j)
+            {
+                const int key = 8 * j + c0;
+                if (key < N) { mx0 = fmaxf(mx0, s[4 * j]); mx1 = fmaxf(mx1, s[4 * j + 2]); }
+                if (key + 1 < N) { mx0 = fmaxf(mx0, s[4 * j + 1]); mx1 = fmaxf(mx1, s[4 * j + 3]); }
+            }
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+            mx0 *= scale;
+            mx1 *= scale;
+            float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+            for (int j = 0; j < ATTP_KEYS / 8; ++j)
+            {
+                const int key = 8 * j + c0;
+                const bool v0 = key < N, v1 = key + 1 < N;
+                // exp_f16_semantics, two keys at a time: each pair's f32 -> f16 roundings are one packed cvt.rn.f16x2.f32 (the scalar
+                // conversions run at a quarter of the ALU rate and bound the soft-max); the f16 -> f32 widening is exact
+                const float2 x0 = __half22float2(__floats2half2_rn(__fmul_rn(s[4 * j], scale) - mx0, __fmul_rn(s[4 * j + 1], scale) - mx0));
+                const float2 x1 = __half22float2(__floats2half2_rn(__fmul_rn(s[4 * j + 2], scale) - mx1, __fmul_rn(s[4 * j + 3], scale) - mx1));
+                const __half2 h0 = __floats2half2_rn(v0 ? ptx::ex2_approx(x0.x * 1.4426950408889634f) : 0.f,
+                                                     v1 ? ptx::ex2_approx(x0.y * 1.4426950408889634f) : 0.f);
+                const __half2 h1 = __floats2half2_rn(v0 ? ptx::ex2_approx(x1.x * 1.4426950408889634f) : 0.f,
+                                                     v1 ? ptx::ex2_approx(x1.y * 1.4426950408889634f) : 0.f);
+                const float2 e0 = __half22float2(h0), e1 = __half22float2(h1);
+                l0 += e0.x + e0.y;
+                l1 += e1.x + e1.y;
+                s[4 * j] = __uint_as_float(*reinterpret_cast<const uint32_t *>(&h0)); // P packed in place: row r pair, row r + 8 pair
+                s[4 * j + 2] = __uint_as_float(*reinterpret_cast<const uint32_t *>(&h1));
+            }
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+
+            // ---- O = P V over ATTP_ROWS keys: the last k16 step's keys 200 .. 207 have P = 0 (no S column)
+            auto pa = [&](int j) { return j < ATTP_KEYS / 2 ? __float_as_uint(s[j]) : 0u; };
+            float o[32];
+#pragma unroll
+            for (int j = 0; j < 32; ++j) o[j] = 0.f;
+            ptx::fence_regs(o);
+            ptx::fence_regs(s);
+            ptx::wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < ATTP_ROWS / 16; ++kk)
+            {
+                const uint32_t a0 = pa(8 * kk), a1 = pa(8 * kk + 2), a2 = pa(8 * kk + 4), a3 = pa(8 * kk + 6);
+                const uint64_t vh = ptx::wgmma_desc_mnmajor_sw128(sKV(buf, 1, 0) + (uint32_t)kk * 2048u);
+                ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, ptx::wgmma_desc_mnmajor_sw128(sKV(buf, 1, 1) + (uint32_t)kk * 2048u), kk != 0);
+                ptx::wgmma_m64n64k16_f16_rs_tb(o, a0, a1, a2, a3, vh, 1);
+            }
+            ptx::wgmma_commit();
+            ptx::wgmma_wait<0>();
+            ptx::fence_regs(o);
+            if constexpr (PROBE)
+                if (tid == 0 && mt == c) probe_stamp(blockIdx.x, i, 4 + 4 * c);
+
+            const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+            const int r0 = mt * 64 + warp * 16 + (lane >> 2), r1 = r0 + 8;
+            __half *o0 = out + ((size_t)b * N + r0) * D + h * 64 + c0;
+            __half *o1 = out + ((size_t)b * N + r1) * D + h * 64 + c0;
+#pragma unroll
+            for (int dt = 0; dt < 8; ++dt)
+            {
+                if (r0 < N) *reinterpret_cast<__half2 *>(o0 + dt * 8) = __floats2half2_rn(o[4 * dt] * inv0, o[4 * dt + 1] * inv0);
+                if (r1 < N) *reinterpret_cast<__half2 *>(o1 + dt * 8) = __floats2half2_rn(o[4 * dt + 2] * inv1, o[4 * dt + 3] * inv1);
+            }
+        }
+        ptx::mbar_arrive(empty_bar(buf)); // this consumer's reads of the buffer have retired (wgmma.wait_group 0)
     }
 }
 

@@ -207,6 +207,7 @@ struct vitb200_engine
     __half *QKV16L = nullptr;
     CUtensorMap tmA_D, tmA_H, tmA_P, tmA_C;
     CUtensorMap tmQ, tmKV, tmQl, tmKVl; // attention operand maps (N <= 224: attention_wgmma_kernel)
+    CUtensorMap tmKVp, tmKVpl;          // k and v maps of attention_wgmma_persistent_kernel (N <= ATTP_KEYS): ATTP_ROWS-row boxes
     int max_k = 16;
     int launches = 0;
     std::map<int, std::string> labels;
@@ -816,11 +817,13 @@ int fc1_epilogue(const vitb200_engine *e)
 int resid_epilogue(const vitb200_engine *e) { return e->arch.layer_scale ? EPI_BIAS_SCALE_RESID_F32 : EPI_BIAS_RESID_F32; }
 
 // Attention kernels (the `kernel` argument of vitb200_test_attention): ATT_MMA8 = the two-pass mma.sync kernel with 8 warps per CTA, any
-// token count; ATT_WGMMA = attention_wgmma_kernel, N <= 224, split precision; ATT_MMA16 = the mma.sync kernel with 16 warps,
-// 128 < N <= 640.  The engine uses the wgmma kernel up to 224 tokens, 16 warps up to 640 and 8 beyond.  Head dim 80 has one kernel,
-// ATT_MMA80 = attention_rowmajor_kernel<80> (split precision up to 224 tokens, f16 operands beyond), which ATT_AUTO picks for it.
-// Head dim 72 runs attention_rowmajor_kernel<72> alike, through ATT_AUTO only.
-enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3, ATT_MMA80 = 4 };
+// token count; ATT_WGMMA = the split-precision wgmma kernel the engine picks for N <= 224: attention_wgmma_persistent_kernel up to
+// ATTP_KEYS tokens (not causal), attention_wgmma_kernel beyond; ATT_WGMMA_HEAD = attention_wgmma_kernel (one CTA per problem) at any
+// N <= 224; ATT_MMA16 = the mma.sync kernel with 16 warps, 128 < N <= 640.  The engine uses the wgmma kernels up to 224 tokens, 16
+// warps up to 640 and 8 beyond.  Head dim 80 has one kernel, ATT_MMA80 = attention_rowmajor_kernel<80> (split precision up to 224
+// tokens, f16 operands beyond), which ATT_AUTO picks for it.  Head dim 72 runs attention_rowmajor_kernel<72> alike, through ATT_AUTO
+// only.
+enum { ATT_AUTO = 0, ATT_MMA8 = 1, ATT_WGMMA = 2, ATT_MMA16 = 3, ATT_MMA80 = 4, ATT_WGMMA_HEAD = 5 };
 constexpr int ATT_MAX_KEYS_16 = 640;
 
 // q / k / v tensor maps (hi and lo halves) of the wgmma attention over planes of max_batch * N token rows
@@ -835,13 +838,23 @@ int make_attention_maps(vitb200_engine *e)
     };
     if (map(&e->tmQ, e->QKV16, 64) || map(&e->tmKV, e->QKV16, ATTW_KEYS) || map(&e->tmQl, e->QKV16L, 64) || map(&e->tmKVl, e->QKV16L, ATTW_KEYS))
         return 1;
+    if (map(&e->tmKVp, e->QKV16, ATTP_ROWS) || map(&e->tmKVpl, e->QKV16L, ATTP_ROWS)) return 1;
     return 0;
 }
 
-int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s)
+static_assert(attention_persistent_smem_bytes() <= kSmemOptinMax, "two K V buffers fit one SM's shared memory");
+
+// per_head: attention_wgmma_kernel even where the persistent kernel would run (the test hooks compare the two); probe: the kernels'
+// phase probe into g_attn_probe (vitb200_test_attention_phases, not causal)
+int launch_attention_wgmma(vitb200_engine *e, int B, cudaStream_t s, bool per_head = false, bool probe = false)
 {
     const int H = e->hp.num_attention_heads;
-    const auto kern = e->text && e->text_arch.causal ? attention_wgmma_kernel<true> : attention_wgmma_kernel<false>;
+    const bool causal = e->text && e->text_arch.causal;
+    if (!per_head && !causal && e->N <= ATTP_KEYS)
+        return launch(e, probe ? attention_wgmma_persistent_kernel<true> : attention_wgmma_persistent_kernel<false>,
+                      dim3(std::min(B * H, e->num_sms)), dim3(ATTP_THREADS), (size_t)attention_persistent_smem_bytes(), s, LAUNCH_PDL, e->tmKVp, e->tmKVpl,
+                      static_cast<const __half *>(e->QKV16), static_cast<const __half *>(e->QKV16L), e->A16, e->N, e->hp.hidden_size, H, e->max_batch, B * H, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
+    const auto kern = causal ? attention_wgmma_kernel<true> : probe ? attention_wgmma_kernel<false, true> : attention_wgmma_kernel<false>;
     return launch(e, kern, dim3(B * H), dim3(ATTW_THREADS), (size_t)attention_wgmma_smem_bytes(), s, LAUNCH_PDL, e->tmQ, e->tmKV, e->tmQl,
                   e->tmKVl, e->A16, e->N, e->hp.hidden_size, H, e->max_batch, 1.0f / sqrtf((float)(e->hp.hidden_size / H)));
 }
@@ -901,7 +914,7 @@ int launch_attention_t(vitb200_engine *e, int B, cudaStream_t s)
                   N, D, H, Npad, 1.0f / sqrtf((float)(D / H)));
 }
 
-int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO)
+int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_AUTO, bool probe = false)
 {
     if (head_dim(e) == ATT80_HD)
     {
@@ -915,7 +928,8 @@ int launch_attention(vitb200_engine *e, int B, cudaStream_t s, int kernel = ATT_
     }
     if (kernel == ATT_MMA80) return fail("attention kernel %d runs head dim 80 only", kernel);
     if (kernel == ATT_AUTO) kernel = e->N <= ATTW_KEYS ? ATT_WGMMA : (e->N <= ATT_MAX_KEYS_16 ? ATT_MMA16 : ATT_MMA8);
-    if (kernel == ATT_WGMMA) return launch_attention_wgmma(e, B, s);
+    if (kernel == ATT_WGMMA || kernel == ATT_WGMMA_HEAD) return launch_attention_wgmma(e, B, s, kernel == ATT_WGMMA_HEAD, probe);
+    if (probe) return fail("the phase probe runs in the wgmma kernels only");
     if (e->QKV16L) return fail("split-precision attention runs in the wgmma kernel (N <= %d)", ATTW_KEYS);
     if (kernel == ATT_MMA16) return launch_attention_t<16>(e, B, s);
     return launch_attention_t<8>(e, B, s);
@@ -2330,9 +2344,10 @@ int vitb200_profile_read(vitb200_engine *e, int kind, double *ms_total, int *lau
     });
 }
 
-// causal: the wgmma kernel with CLIP's causal mask, as a causal text engine launches it
+// causal: the wgmma kernel with CLIP's causal mask, as a causal text engine launches it.  probe: launch the wgmma kernel's phase probe
+// and copy its records (grid x ATT_PROBE_PROBLEMS x ATT_PROBE_FIELDS) there, the grid size to *grid
 static int test_attention_impl(int device, int kernel, int B, int N, int H, const uint16_t *qkv, const uint16_t *qkv_lo, float *out,
-                               bool causal = false)
+                               bool causal = false, unsigned long long *probe = nullptr, int *grid = nullptr)
 {
     if (!qkv || !out || B < 1 || N < 1 || H < 1) return fail("bad argument");
     EnginePtr owner;
@@ -2352,10 +2367,11 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
     to_head_major(qkv);
     if (upload(e, &e->QKV16, hm.data(), hm.size()) || dev_alloc(e, &e->A16, (size_t)T * D)) return 1;
     CUDA_TRY(cudaMemset(e->A16, 0xFF, T * D * sizeof(__half))); // an output the kernel never writes reads back as NaN
-    if (kernel < ATT_AUTO || kernel > ATT_MMA16) return fail("attention kernel %d unknown", kernel);
-    if (kernel == ATT_WGMMA && N > ATTW_KEYS) return fail("wgmma attention needs N <= %d", ATTW_KEYS);
+    const bool wgmma = kernel == ATT_WGMMA || kernel == ATT_WGMMA_HEAD;
+    if (kernel < ATT_AUTO || kernel > ATT_WGMMA_HEAD || kernel == ATT_MMA80) return fail("attention kernel %d unknown", kernel);
+    if (wgmma && N > ATTW_KEYS) return fail("wgmma attention needs N <= %d", ATTW_KEYS);
     if (kernel == ATT_MMA16 && (N <= 128 || N > ATT_MAX_KEYS_16)) return fail("16-warp attention needs 128 < N <= %d", ATT_MAX_KEYS_16);
-    if (kernel == ATT_WGMMA || (kernel == ATT_AUTO && N <= ATTW_KEYS))
+    if (wgmma || (kernel == ATT_AUTO && N <= ATTW_KEYS))
     {
         // the wgmma kernel always runs on split-precision operands: without lo halves it reads zero lo planes (dev_alloc zero-fills
         // them), whose products add exact zeros
@@ -2363,8 +2379,33 @@ static int test_attention_impl(int device, int kernel, int B, int N, int H, cons
         if (qkv_lo ? upload(e, &e->QKV16L, hm.data(), hm.size()) : dev_alloc(e, &e->QKV16L, hm.size())) return 1;
         if (make_attention_maps(e)) return 1;
     }
-    if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel); })) return 1;
+    unsigned long long *d_probe = nullptr;
+    const int n_cta = kernel == ATT_WGMMA && N <= ATTP_KEYS ? std::min(B * H, e->num_sms) : B * H;
+    const size_t n_probe = (size_t)n_cta * ATT_PROBE_PROBLEMS * ATT_PROBE_FIELDS;
+    if (probe)
+    {
+        if (dev_alloc(e, &d_probe, n_probe)) return 1;
+        CUDA_TRY(cudaMemcpyToSymbol(g_attn_probe, &d_probe, sizeof(d_probe)));
+    }
+    if (run_scratch(e, "attention kernel", [&] { return launch_attention(e, B, e->stream, kernel, probe != nullptr); })) return 1;
+    if (probe)
+    {
+        CUDA_TRY(cudaStreamSynchronize(e->stream));
+        CUDA_TRY(cudaMemcpy(probe, d_probe, n_probe * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+        *grid = n_cta;
+    }
     return tap_f16(out, e->A16, (size_t)T * D, e->stream);
+}
+
+int vitb200_test_attention_phases(int device, int kernel, int B, int N, int H, const uint16_t *qkv_hi, const uint16_t *qkv_lo,
+                                  unsigned long long *rec, int *grid)
+{
+    return guarded(__func__, [&] {
+        if (!qkv_lo || !rec || !grid) return fail("bad argument");
+        if (kernel != ATT_WGMMA && kernel != ATT_WGMMA_HEAD) return fail("the phase probe runs in the wgmma kernels (2 or 5), not %d", kernel);
+        std::vector<float> out((size_t)B * N * H * 64);
+        return test_attention_impl(device, kernel, B, N, H, qkv_hi, qkv_lo, out.data(), false, rec, grid);
+    });
 }
 
 int vitb200_test_attention(int device, int kernel, int B, int N, int H, const uint16_t *qkv, float *out)
@@ -2413,7 +2454,7 @@ int vitb200_test_attention_hd(int device, int kernel, int B, int N, int H, int h
     return guarded(__func__, [&]() -> int {
         if (hd == 64)
         {
-            if (qkv_lo && ((kernel != ATT_AUTO && kernel != ATT_WGMMA) || N > ATTW_KEYS))
+            if (qkv_lo && ((kernel != ATT_AUTO && kernel != ATT_WGMMA && kernel != ATT_WGMMA_HEAD) || N > ATTW_KEYS))
                 return fail("split-precision operands run in the wgmma kernel (N <= %d)", ATTW_KEYS);
             return test_attention_impl(device, kernel, B, N, H, qkv_hi, qkv_lo, out);
         }

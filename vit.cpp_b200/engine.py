@@ -156,6 +156,7 @@ def lib():
         L.vitb200_test_attention_pool.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_test_attention_hd.argtypes = [i32, i32, i32, i32, i32, i32, vp, vp, vp]
         L.vitb200_test_attention_hd72.argtypes = [i32, i32, i32, i32, vp, vp, vp]
+        L.vitb200_test_attention_phases.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp]
         L.vitb200_test_attention_pool_hd72.argtypes = [i32, i32, i32, i32, vp, vp, vp]
         _lib = L
     return _lib
@@ -597,8 +598,9 @@ def vit_predict_debug(model: VitModel, images: np.ndarray, tap_layer: int, taps=
 
 
 # attention kernels of vitb200_test_attention (include/vitb200.h): engine's choice, mma.sync with 8 warps (any N), wgmma (N <= 224,
-# the split-precision kernel), mma.sync with 16 warps (128 < N <= 640); the head-dim-80 kernel (vitb200_test_attention_hd)
-ATTN_AUTO, ATTN_MMA8, ATTN_WGMMA, ATTN_MMA16, ATTN_MMA80 = 0, 1, 2, 3, 4
+# the split-precision kernel the engine picks for N: persistent up to 200 tokens, one CTA per (image, head) beyond), mma.sync with 16
+# warps (128 < N <= 640); the head-dim-80 kernel (vitb200_test_attention_hd); the one-CTA-per-(image, head) wgmma kernel at any N <= 224
+ATTN_AUTO, ATTN_MMA8, ATTN_WGMMA, ATTN_MMA16, ATTN_MMA80, ATTN_WGMMA_HEAD = 0, 1, 2, 3, 4, 5
 
 
 def test_attention(qkv16: np.ndarray, B: int, N: int, H: int, kernel: int = ATTN_AUTO, device: int = 0) -> np.ndarray:
@@ -645,6 +647,22 @@ def test_attention_hd(qkv32: np.ndarray, B: int, N: int, H: int, hd: int, split:
     _check(lib().vitb200_test_attention_hd(device, kernel, B, N, H, hd, hi.ctypes.data, None if lo is None else lo.ctypes.data,
                                            out.ctypes.data), "vitb200_test_attention_hd")
     return out
+
+
+# the phase probe's records: per CTA, ATTN_PROBE_PROBLEMS problems of ATTN_PROBE_FIELDS stamps (csrc/attention_wgmma.cuh)
+ATTN_PROBE_PROBLEMS, ATTN_PROBE_FIELDS = 64, 9
+
+
+def test_attention_phases(qkv32: np.ndarray, B: int, N: int, H: int, kernel: int = ATTN_WGMMA, device: int = 0) -> np.ndarray:
+    """The split-precision wgmma kernel `kernel` (ATTN_WGMMA or ATTN_WGMMA_HEAD) with its phase probe on (vitb200_test_attention_phases):
+    qkv32 float32 [B*N, 3*H*64] passed as hi + lo -> uint64 %globaltimer stamps [grid, ATTN_PROBE_PROBLEMS, ATTN_PROBE_FIELDS] in ns,
+    0 where nothing was recorded."""
+    hi, lo = split_hi_lo(np.asarray(qkv32, np.float32).reshape(B * N, 3 * H * 64))
+    rec = np.zeros(B * H * ATTN_PROBE_PROBLEMS * ATTN_PROBE_FIELDS, np.uint64)
+    grid = C.c_int(0)
+    _check(lib().vitb200_test_attention_phases(device, kernel, B, N, H, hi.ctypes.data, lo.ctypes.data, rec.ctypes.data, C.byref(grid)),
+           "vitb200_test_attention_phases")
+    return rec[:grid.value * ATTN_PROBE_PROBLEMS * ATTN_PROBE_FIELDS].reshape(grid.value, ATTN_PROBE_PROBLEMS, ATTN_PROBE_FIELDS)
 
 
 def test_attention_hd72(qkv32: np.ndarray, B: int, N: int, H: int, split: bool, device: int = 0) -> np.ndarray:
